@@ -191,30 +191,32 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet"
 
 
 def measured_tensor_peak():
     """fp8 (e4m3) dense peak for the tensor roofline: MEASURED_PEAKS.json holds the cuBLAS bf16 burst figure; the 8-bit kinds
-    run at twice the 16-bit rate on this part (nominal 4.5 vs 2.25 PFLOP/s), so 2 x the measured bf16 number is used."""
+    run at twice the 16-bit rate on this part (H100 SXM data sheet: 1979 vs 989 TFLOP/s dense), so 2 x the measured bf16 number is used."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
             return 2.0 * float(json.load(open(p))["bf16_tflops"]), "2 x measured cuBLAS bf16 burst (fp8 runs at twice the bf16 rate)"
         except Exception:
             pass
-    return 2.0 * 1590.0, "2 x fallback bf16"
+    return 2.0 * 989.0, "2 x H100 SXM data-sheet bf16"
 
 
-def ncu_traffic(name="k1_traffic.json"):
-    """dram bytes per launch of a kernel from the committed ncu capture (profiles/), or None."""
-    p = os.path.join(ROOT, "profiles", name)
-    if os.path.exists(p):
-        try:
-            return json.load(open(p))
-        except Exception:
-            return None
-    return None
+def dump_outputs(d: str, out: dict) -> None:
+    """Writes what the timed path returned for its last step, one DIR/<name>.npy per array: the match indices and inlier flags of
+    every pair and each field of its pose result (float64 for floating-point fields, float32 for integers and flags, which it holds
+    exactly).  Two builds run with the same arguments see the same inputs, so their dumps compare array for array."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {k: out[k] for k in ("m12_pt", "m12_ls", "inlier_pt", "inlier_ls")}
+    res = out["results"]
+    arrays.update({"results_" + f: res[f] for f in res.dtype.names if f != "reserved"})
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(d, name + ".npy"), a.astype(np.float64 if a.dtype.kind == "f" else np.float32))
 
 
 def cpu_leg(sample: int, budget_s: float = 25.0, min_reps: int = 5, max_reps: int = 20, first_pair: int = 0):
@@ -390,6 +392,8 @@ def run_ours(args):
     value = world * B * args.steps / (ms * 1e-3)
     out = db.download()
     good = int(out["results"]["good"].sum())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
 
     # ---------------- per-kernel times and the roofline of the dominant kernel, rank 0 ----------------
     st = db.stage_times(iters=max(5, min(args.steps, 20)))
@@ -439,26 +443,23 @@ def run_ours(args):
         k["share_of_step"] = k["ms"] / step_ms if step_ms > 0 else 0.0
     dom_name = max(kernels, key=lambda n: kernels[n]["ms"])
     dom = kernels[dom_name]
-    traffic = ncu_traffic("k_traffic.json") or {}
     if dom["bound"] == "tensor":
         achieved = tc_flops / (dom["ms"] * 1e-3) / 1e12
         roofline = {"kernel": dom_name, "bound": "tensor", "achieved": achieved, "peak": tpeak, "unit": "TFLOP/s",
                     "frac": achieved / tpeak, "peak_kind": tpeak_kind,
-                    "traffic": (traffic.get(dom_name) or {}).get("dram_bytes_per_launch"),
                     "algorithmic_flops_per_launch": tc_flops, "ms_per_launch": dom["ms"],
                     "note": "2 x 256 flop per 256-bit pair distance (the +-1 contraction); the kernel is bound by its top-2 epilogue "
-                            "on the ALU pipe (3 packed min/max per two distances and direction), not by the tensor pipe: see `pipes`"}
+                            "on the ALU pipe (packed min/max per two distances and direction), not by the tensor pipe"}
     else:
         alg = dom.get("algorithmic_bytes", k2_bytes)
         achieved = alg / (dom["ms"] * 1e-3) / 1e9
         roofline = {"kernel": dom_name, "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                    "peak_kind": f"of {peak_kind}", "traffic": (traffic.get(dom_name) or {}).get("dram_bytes_per_launch"),
+                    "peak_kind": f"of {peak_kind}",
                     "algorithmic_bytes_per_launch": alg, "ms_per_launch": dom["ms"],
                     "note": "one persistent CTA per pair: ~16 dependent evaluate -> reduce -> 6x6 solve rounds; latency-bound, far from "
                             "the HBM roofline by construction (features are read once into shared memory)"}
     roofline["share_of_step"] = dom["share_of_step"]
     roofline["kernels"] = kernels
-    roofline["pipes"] = traffic.get("pipes")
     roofline["tensor"] = {"kernel": "tc_hamming_kernel", "achieved": tc_flops / (st["ms_distance"] * 1e-3) / 1e12, "peak": tpeak,
                           "unit": "TFLOP/s", "frac": tc_flops / (st["ms_distance"] * 1e-3) / 1e12 / tpeak, "peak_kind": tpeak_kind,
                           "pair_distances_per_s": pair_dists / (st["ms_distance"] * 1e-3)} if st["tensor_core_form"] else None
@@ -543,7 +544,7 @@ def run_ours(args):
         "config": {"workload": WORKLOADS[ACTIVE][3], "pairs_per_gpu": B, "solver": "streamed" if st["streamed_solver"] else "K2 (fp64)", "global_pairs_per_step": world * B,
                    "parallelism": f"independent pairs sharded over {world} GPU(s), no collective",
                    "l2": f"inputs larger than L2: {(h2d + kt['n_tiles'] * 0) / 1e6:.0f} MB of inputs + "
-                         f"{B * 140000 / 1e6:.0f} MB of tile partials per pass vs 126 MB L2",
+                         f"{B * 140000 / 1e6:.0f} MB of tile partials per pass vs 50 MB L2",
                    "overlap": 1.0, "outlier_frac": 0.10, "solved_ok": good, "e2e_equals_resident": bool(same),
                    "numa_bound": numa},
         "clocks": clk.summary(),
@@ -625,7 +626,7 @@ def run_ours(args):
 
 def c5_sweeps(eng, B, iters=20):
     """BASELINE config C5: high-density 1920x1080 synthetic, 8000 pts + 2000 lines per problem, `iters` GN evaluations with
-    the packed matched lists of B >= 1024 problems resident in HBM (393 MB per sweep, far beyond the 126 MB L2) so that every
+    the packed matched lists of B >= 1024 problems resident in HBM (393 MB per sweep, far beyond the 50 MB L2) so that every
     evaluation streams from HBM.  Returns (seconds per sweep, roofline object, mean error, clocks)."""
     mb, Ts, cam = synth.make_matched_batch("hd", B)
     cfg = T.kitti_config()
@@ -636,9 +637,8 @@ def c5_sweeps(eng, B, iters=20):
     alg = 32 * n + 64 * m                                              # SURVEY 8(d): 32 N_p + 64 N_l per evaluation
     peak, kind = measured_peak()
     per = ms / iters * 1e-3
-    tr = ncu_traffic("gn_traffic.json")
     roof = {"kernel": "gn_eval_stream_kernel", "bound": "hbm", "achieved": alg / per / 1e9, "peak": peak, "unit": "GB/s",
-            "frac": alg / per / 1e9 / peak, "peak_kind": f"{kind}, burst (kernel timed alone, {iters} back-to-back sweeps, each = the streaming kernel + the per-problem reduce launch)", "traffic": tr["dram_bytes_per_launch"] if tr and tr.get("problems") == B else None,
+            "frac": alg / per / 1e9 / peak, "peak_kind": f"{kind}, burst (kernel timed alone, {iters} back-to-back sweeps, each = the streaming kernel + the per-problem reduce launch)",
             "algorithmic_bytes_per_launch": alg, "problems_resident": B, "ms_per_sweep": ms / iters}
     return per, roof, float(np.mean(e)), clk.summary()
 
@@ -677,7 +677,6 @@ def c5_pipeline(eng, B, steps=3, distinct=128):
     alg = int((evals * per_eval).sum())                       # bytes the sweeps of one step have to stream
     sweep_bytes = int(per_eval.sum())                         # one sweep over every problem
     peak, kind = measured_peak()
-    tr = ncu_traffic("c5_traffic.json") or {}
     solve_s = st["ms_optimize_pose"] * 1e-3
     gn_s = (st["ms_gn_stage1"] + st["ms_gn_stage2"]) * 1e-3
     return {"workload": "C5: 1920x1080, 8000 pts + 2000 lines per frame, match + optimizePose (KITTI solver parameters), "
@@ -692,16 +691,11 @@ def c5_pipeline(eng, B, steps=3, distinct=128):
                          "bound": "hbm", "achieved": alg / gn_s / 1e9, "peak": peak, "unit": "GB/s",
                          "frac": alg / gn_s / 1e9 / peak, "peak_kind": f"of {kind}",
                          "algorithmic_bytes_per_step": alg, "bytes_per_sweep": sweep_bytes,
-                         "l2": f"{sweep_bytes / 1e6:.0f} MB per sweep vs 126 MB L2",
-                         "traffic": tr.get("dram_bytes_per_launch"),
-                         "traffic_of": "one stage-2 launch over the first half of the batch (ncu --set full, profiles/c5_traffic.json); "
-                                       f"its algorithmic bytes: {int((res['iters_stage2'][:B // 2].astype(np.int64) * per_eval[:B // 2]).sum())}",
+                         "l2": f"{sweep_bytes / 1e6:.0f} MB per sweep vs 50 MB L2",
                          "ms_gn_loops": gn_s * 1e3,
                          "ms_optimize_pose": st["ms_optimize_pose"], "ms_outliers": st["ms_outliers"],
                          "frac_of_optimize_pose": alg / solve_s / 1e9 / peak,
                          "frac_including_list_building": alg / ((st["ms_lists"] + st["ms_optimize_pose"]) * 1e-3) / 1e9 / peak,
-                         "traffic_note": "DRAM traffic below the algorithmic bytes = L2 reuse: the records of one 256-pair chunk (98 MB) stay "
-                                         "in the 126 MB L2 from one iteration to the next",
                          "note": "bytes = evaluations that actually ran x record bytes (32 B / point, 64 B / line); time = the two "
                                  "gn_loop_stream_kernel launches (CUDA events around each).  frac_of_optimize_pose divides the same bytes "
                                  "by everything after matched_pt / matched_ls exist (GN loops, gate + removeOutliers, finalisation); "
@@ -735,7 +729,7 @@ def run_c5(args):
             "n_gpus": 1, "steps": iters, "warmup": 2, "ms_per_step": per * 1e3, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32 per feature, f64 reduction", "data": "synthetic",
             "config": {"workload": "C5: 1920x1080, 8000 pts + 2000 lines, 20 GN evaluations streamed from HBM",
-                       "problems_resident": B, "l2": f"{roof['algorithmic_bytes_per_launch'] * 1e-6:.0f} MB streamed per sweep vs 126 MB L2"},
+                       "problems_resident": B, "l2": f"{roof['algorithmic_bytes_per_launch'] * 1e-6:.0f} MB streamed per sweep vs 50 MB L2"},
             "clocks": clocks, "gpu_launches": 2 * iters, "roofline": dict(roof, mean_err=mean_err)}
     print(json.dumps(line), flush=True)
     eng.close()
@@ -973,9 +967,14 @@ def main():
                     help="c2: the headline solves/s bench (default); c1 / c3: the same pipeline on the points-only and the "
                          "EuRoC-shape robust configurations; c5: HBM-roofline run of the streamed GN evaluation "
                          "(1920x1080, 8000 points + 2000 lines, >= 1024 problems resident, 20 evaluations)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (match indices, inlier flags, pose results) as "
+                         "DIR/<name>.npy; c1 / c2 / c3 workloads")
     ap.add_argument("--kernels-only", action="store_true",
                     help="profiling aid: upload, launch K1 and K2 over the whole batch twice, exit (for ncu)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.workload not in ("c1", "c2", "c3") or args.kernels_only):
+        ap.error("--dump-outputs applies to the timed path of the c1 / c2 / c3 workloads")
     global ACTIVE
     if args.workload in WORKLOADS:
         ACTIVE = args.workload

@@ -1,5 +1,5 @@
 /*
- * plstvo.h — C-ABI of the B200-native PL-StVO frame-to-frame pose engine.
+ * plstvo.h — C-ABI of the H100-native PL-StVO frame-to-frame pose engine.
  *
  * Plain C, plain pointers and sizes; no Eigen / OpenCV / torch types cross this
  * boundary.  Every entry point names the reference interface it replaces
@@ -36,7 +36,7 @@ extern "C" {
 #define PLSTVO_E_INVALID      (-1)  /* bad argument (null pointer, negative size, stride != 32) */
 #define PLSTVO_E_TOO_LARGE    (-2)  /* more than PLSTVO_MAX_FEATURES rows */
 #define PLSTVO_E_CUDA         (-3)  /* CUDA runtime failure; see plstvo_last_error() */
-#define PLSTVO_E_NO_DEVICE    (-4)  /* no sm_100 device: the library never falls back to a CPU path */
+#define PLSTVO_E_NO_DEVICE    (-4)  /* no sm_90 device: the library never falls back to a CPU path */
 #define PLSTVO_E_SIZE         (-5)  /* size mismatch (the reference's std::runtime_error cases) */
 
 /* ---- camera: PinholeStereoCamera getters used by the path
@@ -351,7 +351,7 @@ int64_t plstvo_launch_count(const PlContext* ctx);
  * launch.  n_tiles / n_pairs (optional) = CTAs per launch. */
 int     plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, double* ms_match,
                                   double* ms_solve, int32_t* n_tiles, int32_t* n_pairs);
-/* The same per stage: ms[0] = operand expansion, ms[1] = distance + top-2 kernel (tcgen05 form) or the integer K1
+/* The same per stage: ms[0] = operand expansion, ms[1] = distance + top-2 kernel (tensor-core form) or the integer K1
  * (PLSTVO_K1=popc: ms[0] = ms[2] = 0), ms[2] = index resolution, ms[3] = building matched_pt / matched_ls when that is a
  * kernel of its own (the streamed solver; 0 when K2 does it internally), ms[4] = optimizePose (K2, or the streamed solver's
  * GN-loop / outlier / finalize kernels + K2 for the problems it hands back); of ms[4], streamed solver only (0 for K2):

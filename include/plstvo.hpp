@@ -23,7 +23,7 @@ class Context {
 public:
     explicit Context(int device = -1) {
         const int rc = plstvo_create(device, &ctx_);
-        if (rc != 0) throw Error(rc, "plstvo_create failed: no sm_100 CUDA device (there is no CPU fallback)");
+        if (rc != 0) throw Error(rc, "plstvo_create failed: no sm_90 CUDA device (there is no CPU fallback)");
     }
     ~Context() { plstvo_destroy(ctx_); }
     Context(const Context&) = delete;

@@ -9,6 +9,7 @@ import ctypes as C
 import hashlib
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -20,11 +21,23 @@ _SRC = [os.path.join(_HERE, "plstvo_oracle.c"), os.path.join(_HERE, "plstvo_orac
 
 
 def _build(out: str, march: str) -> None:
-    """Same flags as oracle/Makefile (= the reference's CMakeLists.txt:18 flags)."""
+    """Same flags as oracle/Makefile (= the reference's CMakeLists.txt:18 flags).  Compiles to a private name and renames, so
+    that processes building the same library at once never load a half-written file."""
     os.makedirs(os.path.dirname(out), exist_ok=True)
+    tmp = f"{out}.{os.getpid()}.tmp"
     cmd = ["gcc", "-O3", f"-march={march}", f"-mtune={'native' if march == 'native' else 'generic'}",
-           "-std=gnu11", "-fPIC", "-ffp-contract=off", "-shared", "-o", out, _SRC[0], "-lm", "-lpthread"]
+           "-std=gnu11", "-fPIC", "-ffp-contract=off", "-shared", "-o", tmp, _SRC[0], "-lm", "-lpthread"]
     subprocess.run(cmd, check=True, capture_output=True)
+    os.replace(tmp, out)
+
+
+def _scratch_dir() -> str:
+    """Per-user directory outside the source tree for libraries compiled at run time (the tree may be read-only)."""
+    d = os.path.join(tempfile.gettempdir(), f"plstvo-oracle-{os.getuid()}")
+    os.makedirs(d, mode=0o700, exist_ok=True)
+    if os.stat(d).st_uid != os.getuid():
+        raise RuntimeError(f"{d} belongs to another user; set TMPDIR to a private directory")
+    return d
 
 
 def _stale(lib: str) -> bool:
@@ -32,14 +45,20 @@ def _stale(lib: str) -> bool:
 
 
 def lib_path(native: bool = False) -> str:
-    """Portable build (x86-64-v3: AVX2 + POPCNT) travels with the repo; the native build used for the CPU
-    baseline is compiled on the machine that times it (-march=native, the reference's own flag)."""
+    """Portable build (x86-64-v3: AVX2 + POPCNT) sits in the tree, where build() puts it (or in the per-user scratch
+    directory when the tree cannot take it); the native build used for the CPU baseline is compiled on the machine that
+    times it (-march=native, the reference's own flag), into the scratch directory."""
     override = os.environ.get("PLSTVO_ORACLE_LIB")   # e.g. an -fsanitize=address,undefined build (tools/oracle_asan.sh)
     if override:
         return override
     if not native:
         lib = os.path.join(_HERE, "libplstvo_oracle.so")
         if _stale(lib):
+            if not os.access(_HERE, os.W_OK):
+                h = hashlib.sha1(b"".join(open(src, "rb").read() for src in _SRC)).hexdigest()[:16]
+                lib = os.path.join(_scratch_dir(), "portable", h, "libplstvo_oracle.so")
+                if os.path.exists(lib):
+                    return lib
             _build(lib, "x86-64-v3")
         return lib
     try:
@@ -47,9 +66,12 @@ def lib_path(native: bool = False) -> str:
             flags = next((l for l in f if l.startswith("flags")), "")
     except OSError:
         flags = ""
-    tag = hashlib.sha1(flags.encode()).hexdigest()[:10]
-    lib = os.path.join(_HERE, "_native", tag, "libplstvo_oracle.so")
-    if _stale(lib):
+    h = hashlib.sha1(flags.encode())
+    for src in _SRC:   # the scratch directory is shared by every checkout of this user: key the build on its sources too
+        with open(src, "rb") as f:
+            h.update(f.read())
+    lib = os.path.join(_scratch_dir(), "native", h.hexdigest()[:16], "libplstvo_oracle.so")
+    if not os.path.exists(lib):
         _build(lib, "native")
     return lib
 

@@ -175,3 +175,61 @@ class Ref:
                                         priors.ctypes.data if priors is not None else None, res.ctypes.data,
                                         inl_pt.ctypes.data_as(T.c_uint8_p), inl_ls.ctypes.data_as(T.c_uint8_p))
         return rc, res, inl_pt[:-1], inl_ls[:-1]
+
+
+class Recorded:
+    """The Ref surface served from stored answers: what the reference's code returned for each call a test made, recorded once
+    where the reference sources are present (record=Ref()) and replayed everywhere else, so the comparisons keep running
+    against the reference's own results.  Calls are matched by test, position in the test and method name; inputs are
+    seeded, so the same test makes the same calls.  The store is one compressed archive: a JSON index plus a byte blob."""
+
+    def __init__(self, path: str, record: "Ref | None" = None):
+        import json
+        self.path, self.live = path, record
+        self.test, self.n = None, 0
+        self.index, self.blob = {}, bytearray()
+        if record is None:
+            z = np.load(path)
+            self.index = json.loads(bytes(z["index"]).decode())
+            self.blob = bytes(z["blob"])
+
+    def begin(self, test: str) -> None:
+        self.test, self.n = test, 0
+
+    def save(self) -> None:
+        import json
+        np.savez_compressed(self.path, index=np.frombuffer(json.dumps(self.index).encode(), np.uint8),
+                            blob=np.frombuffer(bytes(self.blob), np.uint8))
+
+    def _put(self, v):
+        if isinstance(v, (bool, int, float)):
+            return {"py": type(v).__name__, "v": v}
+        a = np.ascontiguousarray(v)
+        e = {"dtype": np.lib.format.dtype_to_descr(a.dtype), "shape": list(a.shape), "off": len(self.blob), "n": a.nbytes}
+        self.blob += a.tobytes()
+        return e
+
+    def _get(self, e):
+        if "py" in e:
+            return {"bool": bool, "int": int, "float": float}[e["py"]](e["v"])
+        dt = np.lib.format.descr_to_dtype(e["dtype"] if isinstance(e["dtype"], str) else [tuple(f) for f in e["dtype"]])
+        return np.frombuffer(self.blob, dt, count=int(np.prod(e["shape"], dtype=np.int64)), offset=e["off"]).reshape(e["shape"]).copy()
+
+    def __getattr__(self, name):
+        if name.startswith("_"):
+            raise AttributeError(name)
+
+        def call(*args, **kw):
+            key = f"{self.test}#{self.n}"
+            self.n += 1
+            if self.live is not None:
+                r = getattr(self.live, name)(*args, **kw)
+                vals = list(r) if isinstance(r, tuple) else [r]
+                self.index[key] = {"method": name, "tuple": isinstance(r, tuple), "vals": [self._put(v) for v in vals]}
+                return r
+            e = self.index.get(key)
+            assert e is not None and e["method"] == name, f"{key}: {name} was not recorded at this point of the test"
+            vals = [self._get(v) for v in e["vals"]]
+            return tuple(vals) if e["tuple"] else vals[0]
+
+        return call

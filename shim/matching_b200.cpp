@@ -13,7 +13,7 @@ namespace StVO {
 PlContext* b200_context() {                        // one context per process and GPU; safe to share between threads:
     static PlContext* ctx = [] {                   // every entry point serialises on the context's own lock and streams
         PlContext* c = nullptr;
-        if (plstvo_create(-1, &c) != 0) throw std::runtime_error("[b200] no sm_100 device");
+        if (plstvo_create(-1, &c) != 0) throw std::runtime_error("[b200] no sm_90 device");
         return c;
     }();
     return ctx;

@@ -1,7 +1,6 @@
-"""Builds the CUDA library in-tree: stvo_pl_b200/lib/libplstvo_b200.so (sm_100a only).
+"""Builds the CUDA library in-tree: stvo_pl_b200/lib/libplstvo_b200.so (sm_90a only).
 
-nvcc cross-compiles without a GPU; the built .so travels to the GPU box with the repo snapshot
-(it is git-ignored, not gpurun-ignored).
+nvcc cross-compiles without a GPU; the built .so is git-ignored.
 """
 from __future__ import annotations
 
@@ -16,7 +15,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libplstvo_b200.so")
 SOURCES = ["match.cu", "match_tc.cu", "match_grid.cu", "lift.cu", "solve.cu", "gn_stream.cu", "capi.cu"]
 HEADERS = ["common.cuh", "match_finalize.cuh", "match_tc.cuh", "gn_stream.cuh", os.path.join("..", "..", "include", "plstvo.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "--use_fast_math=false"]
 
 

@@ -722,7 +722,7 @@ int plstvo_create(int device, PlContext** out) {
     if (device >= n) return PLSTVO_E_NO_DEVICE;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return PLSTVO_E_NO_DEVICE;
-    if (prop.major != 10) return PLSTVO_E_NO_DEVICE;   // the kernels are built for sm_100a only
+    if (prop.major != 9) return PLSTVO_E_NO_DEVICE;   // the kernels are built for sm_90a only
     if (cudaSetDevice(device) != cudaSuccess) return PLSTVO_E_NO_DEVICE;
     PlContext* ctx = new PlContext();
     ctx->device = device;

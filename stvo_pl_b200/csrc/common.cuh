@@ -1,4 +1,4 @@
-// common.cuh — internal declarations shared by the sm_100a kernels and the C-ABI host code.
+// common.cuh — internal declarations shared by the sm_90a kernels and the C-ABI host code.
 // Nothing here is part of the public boundary (include/plstvo.h is).
 #pragma once
 

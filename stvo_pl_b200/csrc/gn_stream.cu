@@ -246,20 +246,14 @@ cudaError_t launch_gn_eval_stream(const PlCamera& cam, const PlConfig& cfg, cons
                                   int sm_count, double* H, double* g, double* e, cudaStream_t stream) {
     if (B <= 0) return cudaSuccess;
     const size_t smem = (size_t)GS_STAGES * GS_STAGE_BYTES;
-    static const bool packed = getenv("PLSTVO_GS_SCALAR") == nullptr;   // A/B knob: scalar-FFMA accumulators (default: packed FFMA2)
-    static size_t configured[2][64] = {};
-    cudaError_t err = packed ? ensure_dynamic_smem(reinterpret_cast<const void*>(gn_eval_stream_kernel<GsAccPacked>), smem, configured[0])
-                             : ensure_dynamic_smem(reinterpret_cast<const void*>(gn_eval_stream_kernel<GsAccScalar>), smem, configured[1]);
+    static size_t configured[64] = {};
+    cudaError_t err = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_eval_stream_kernel<GsAccScalar>), smem, configured);
     if (err != cudaSuccess) return err;
     const int n_items = B * bpp;
     const int grid = n_items < 2 * sm_count ? n_items : 2 * sm_count;
     const GsLists L{pt_off, ls_off};
-    if (packed)
-        gn_eval_stream_kernel<GsAccPacked><<<grid, GS_THREADS, smem, stream>>>(cam, (float)cfg.homog_th, L, pt, ls, DT, partial, bpp,
-                                                                               n_items);
-    else
-        gn_eval_stream_kernel<GsAccScalar><<<grid, GS_THREADS, smem, stream>>>(cam, (float)cfg.homog_th, L, pt, ls, DT, partial, bpp,
-                                                                               n_items);
+    gn_eval_stream_kernel<GsAccScalar><<<grid, GS_THREADS, smem, stream>>>(cam, (float)cfg.homog_th, L, pt, ls, DT, partial, bpp,
+                                                                           n_items);
     err = cudaGetLastError();
     if (err != cudaSuccess) return err;
     gn_eval_reduce_kernel<<<B, 32, 0, stream>>>(partial, bpp * GS_CWARPS, H, g, e);

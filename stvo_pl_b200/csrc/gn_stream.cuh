@@ -67,54 +67,6 @@ struct GsAccScalar {
     }
 };
 
-// The same sums with Blackwell's packed fp32 pipe (fma.rn.f32x2 -> FFMA2, one operand broadcast): 12 FFMA2 + 3 FMUL2 + 5
-// scalar ops per feature instead of 36.  Pairs: (00,01)(02,03)(04,05) (12,13)(14,15) (22,23)(24,25) (34,35) (44,45)
-// (g0,g1)(g2,g3)(g4,g5); scalars: 11, 33, 55, e, count.
-typedef unsigned long long gs_u64;
-__device__ __forceinline__ gs_u64 gs_pk(float lo, float hi) { gs_u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void gs_upk(gs_u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ gs_u64 gs_fma2(gs_u64 a, gs_u64 b, gs_u64 c) { gs_u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ gs_u64 gs_mul2(gs_u64 a, gs_u64 b) { gs_u64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-struct GsAccPacked {
-    gs_u64 p[12];
-    float s[5];
-    __device__ __forceinline__ void clear() {
-#pragma unroll
-        for (int i = 0; i < 12; i++) p[i] = 0ull;
-#pragma unroll
-        for (int i = 0; i < 5; i++) s[i] = 0.f;
-    }
-    __device__ __forceinline__ void add(const float* J, float r, float w, float one) {
-        const gs_u64 J01 = gs_pk(J[0], J[1]), J23 = gs_pk(J[2], J[3]), J45 = gs_pk(J[4], J[5]), ww = gs_pk(w, w), rr = gs_pk(r, r);
-        const gs_u64 W01 = gs_mul2(J01, ww), W23 = gs_mul2(J23, ww), W45 = gs_mul2(J45, ww);
-        float w0, w1, w2, w3, w4, w5;
-        gs_upk(W01, w0, w1); gs_upk(W23, w2, w3); gs_upk(W45, w4, w5);
-        const gs_u64 b0 = gs_pk(w0, w0), b1 = gs_pk(w1, w1), b2 = gs_pk(w2, w2), b3 = gs_pk(w3, w3), b4 = gs_pk(w4, w4);
-        p[0] = gs_fma2(b0, J01, p[0]); p[1] = gs_fma2(b0, J23, p[1]); p[2] = gs_fma2(b0, J45, p[2]);
-        p[3] = gs_fma2(b1, J23, p[3]); p[4] = gs_fma2(b1, J45, p[4]);
-        p[5] = gs_fma2(b2, J23, p[5]); p[6] = gs_fma2(b2, J45, p[6]);
-        p[7] = gs_fma2(b3, J45, p[7]);
-        p[8] = gs_fma2(b4, J45, p[8]);
-        p[9] = gs_fma2(W01, rr, p[9]); p[10] = gs_fma2(W23, rr, p[10]); p[11] = gs_fma2(W45, rr, p[11]);
-        s[0] = fmaf(w1, J[1], s[0]); s[1] = fmaf(w3, J[3], s[1]); s[2] = fmaf(w5, J[5], s[2]);
-        s[3] = fmaf(r * w, r, s[3]);
-        s[4] += one;
-    }
-    __device__ __forceinline__ void unpack(float* o) const {
-        gs_upk(p[0], o[0], o[1]); gs_upk(p[1], o[2], o[3]); gs_upk(p[2], o[4], o[5]);
-        o[6] = s[0];
-        gs_upk(p[3], o[7], o[8]); gs_upk(p[4], o[9], o[10]);
-        gs_upk(p[5], o[11], o[12]); gs_upk(p[6], o[13], o[14]);
-        o[15] = s[1];
-        gs_upk(p[7], o[16], o[17]);
-        gs_upk(p[8], o[18], o[19]);
-        o[20] = s[2];
-        gs_upk(p[9], o[21], o[22]); gs_upk(p[10], o[23], o[24]); gs_upk(p[11], o[25], o[26]);
-        o[27] = s[3];
-        o[28] = s[4];
-    }
-};
-
 __device__ __forceinline__ float gs_overlap_l(float ls, float le) {   // :601-610 on the two parameters
     const float lo = fminf(ls, le), hi = fmaxf(ls, le);
     float ov = fminf(hi, 1.f) - fmaxf(lo, 0.f);                       // covered part of [0, 1]
@@ -177,10 +129,6 @@ __device__ __forceinline__ GsProj gs_project(const GsPose& P, float xn, float yn
     return q;
 }
 
-// (Measured and dropped: the same per-point arithmetic with TWO points, or the two end points of a segment, in the halves of packed
-// f32x2 registers — fewer instructions, but FFMA2 occupies the FMA pipe for two cycles and the pack / unpack moves come on top: the
-// sweep kernel fell from 0.82 to 0.71 of the HBM roofline.  Packed registers pay only where the operands are already pairs: the
-// accumulation of J J^T above.)
 // point block (:563-606); `use` = a live record flagged inlier
 template <class Acc>
 __device__ __forceinline__ void gs_point(const GsPose& P, const float4 a, const float4 b, bool use, Acc& acc) {

@@ -1,4 +1,4 @@
-// match.cu — K1: brute-force 256-bit Hamming 2-NN over descriptor tiles (sm_100a).
+// match.cu — K1: brute-force 256-bit Hamming 2-NN over descriptor tiles (sm_90a).
 //
 // Replaces the arithmetic of StVO::matchNNR / StVO::match (src/matching.cpp:41-91), i.e. OpenCV's
 // cv::BFMatcher(NORM_HAMMING)::knnMatch(desc1, desc2, ., 2) called once per direction.  One pass over the

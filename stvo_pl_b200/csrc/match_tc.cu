@@ -1,24 +1,22 @@
-// match_tc.cu — K1 on the 5th-generation tensor cores: all-pairs 256-bit Hamming 2-NN as a +-1 contraction.
+// match_tc.cu — K1 on the Hopper tensor cores (wgmma): all-pairs 256-bit Hamming 2-NN as a +-1 contraction.
 //
 // Replaces the arithmetic of StVO::matchNNR / StVO::match (src/matching.cpp:41-91), i.e. OpenCV's
 // cv::BFMatcher(NORM_HAMMING)::knnMatch(desc1, desc2, ., 2) per direction.  With descriptor bits mapped to +-1,
 //     a . b = (#equal bits) - (#different bits) = 256 - 2 d(a, b)          (exact, |a . b| <= 256)
 // so the N1 x N2 distance matrix of one matching problem is a 256-deep GEMM.  Three kernels:
 //   tc_expand_kernel   32-byte descriptor rows -> 256 e4m3 bytes (+1.0 = 0x38, -1.0 = 0xB8), written directly in the
-//                      128-byte-swizzled K-major operand layout tcgen05.mma reads (tiles of 128 rows = 32 KB contiguous),
+//                      128-byte-swizzled K-major operand layout wgmma reads (tiles of 128 rows = 32 KB contiguous),
 //                      so the tiles move with plain bulk copies (UBLKCP) and need no tensor map;
-//   tc_hamming_kernel  persistent, warp-specialised: producer warp (bulk copies + mbarriers), one MMA-issuing thread
-//                      (tcgen05.mma kind::f8f6f4, 128 x 128 x 32 per instruction, f16 accumulators in TMEM: every partial
-//                      sum is an integer of magnitude <= 256, exact in f16), eight epilogue warps reading TMEM with
-//                      tcgen05.ld ... .pack::16b: two columns per register, so the top-2 update of BOTH directions
-//                      costs 3 packed min/max per two distances and direction:
-//                        row direction   (query -> trains): thread = query row, fold over the columns in registers;
+//   tc_hamming_kernel  persistent, warp-specialised: one producer warp (bulk copies + mbarriers), two consumer
+//                      warpgroups issuing wgmma m64n256k32 (e4m3 operands, f16 accumulators in registers, two columns
+//                      per register), so the top-2 update of BOTH directions costs a few packed min/max per two distances:
+//                        row direction   (query -> trains): fold over the columns in registers, then over four lanes;
 //                        column direction (train -> queries): element-wise running top-2 over the row tiles in
 //                                         registers, one cross-lane reduction per work item (not per tile).
 //                      Keys carry no indices in the hot loop: only (best, second) VALUES and a small candidate tag
-//                      (which 16-column group / which lane the best came from);
+//                      (which chunk group / lane / warp the best came from);
 //   tc_resolve_kernel  merges the per-block partials, converts to distances and recovers the best neighbour's index by
-//                      re-evaluating the <= 16 tagged candidates with XOR + POPC (exact; ties resolved to the lowest index
+//                      re-evaluating the few tagged candidates with XOR + POPC (exact; ties resolved to the lowest index
 //                      as OpenCV does), emitting the same packed keys (dist << 16 | index) K1's popcount form emits, so
 //                      everything downstream (ratio test, mutual filter, K2) is unchanged.
 // Integer-exact end to end: the bit-exact parity tests of the matcher are the acceptance test.
@@ -71,39 +69,36 @@ cudaError_t launch_tc_expand(const TcSide* sides, int n_sides, int max_tiles, cu
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// PTX helpers (tcgen05 / TMEM)
+// PTX helpers (wgmma)
 // ---------------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void tc_mma_f8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 256] (f16, 64 registers) (+)= A[64 x 32] . B[256 x 32]^T, both e4m3 and K-major in shared memory.
+// Register d[2i + h] of lane l in warp w of the warpgroup holds row 16 w + l / 4 + 8 h, columns 8 i + 2 (l % 4) + {0, 1}
+// (low half = even column).
+__device__ __forceinline__ void wg_mma_f8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, int acc) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n256k32.f16.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+        "}\n"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(acc)
         : "memory");
 }
-// 32 lanes x 32 columns of f16 accumulators -> 16 registers, two adjacent columns per register (low half = even column)
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.pack::16b.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
+// keeps the compiler from moving reads or writes of the accumulators across the wgmma fence / wait
+__device__ __forceinline__ void wg_fence_regs(uint32_t (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// packed f16x2 arithmetic on raw 32-bit registers.  max(max(a, b), c) is fused by ptxas into one 3-input VHMNMX.
+// packed f16x2 arithmetic on raw 32-bit registers
 __device__ __forceinline__ uint32_t hmax2u(uint32_t a, uint32_t b) {
     uint32_t d;
     asm("max.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
@@ -129,16 +124,6 @@ __device__ __forceinline__ uint32_t hfma2u(uint32_t a, uint32_t b, uint32_t c) {
     asm("fma.rn.f16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
     return d;
 }
-__device__ __forceinline__ uint32_t hfma2relu(uint32_t a, uint32_t b, uint32_t c) {   // max(0, a * b + c)
-    uint32_t d;
-    asm("fma.rn.relu.f16x2 %0, %1, %2, %3;" : "=r"(d) : "r"(a), "r"(b), "r"(c));
-    return d;
-}
-__device__ __forceinline__ uint32_t hadd2u(uint32_t a, uint32_t b) {
-    uint32_t d;
-    asm("add.rn.f16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-    return d;
-}
 __device__ __forceinline__ uint32_t swap16(uint32_t a) { return __byte_perm(a, a, 0x1032); }
 __device__ __forceinline__ uint32_t sel32(uint32_t mask, uint32_t a, uint32_t b) { return (mask & a) | (~mask & b); }   // one LOP3
 __device__ __forceinline__ uint32_t h2u_lo(uint32_t p) {   // low half (an integer-valued f16 >= 0) -> uint32
@@ -152,67 +137,46 @@ __device__ __forceinline__ uint32_t h2u_hi(uint32_t p) {
     return d;
 }
 
-// "no value" sentinel: -1024 (finite, so that the FMA-pipe form of the update stays exact: |x - y| <= 1280 < 2048)
+// "no value" sentinel: -1024 (below every dot product, |a . b| <= 256)
 constexpr uint32_t NEG2 = 0xE400E400u;
-constexpr uint32_t H2_NEG1 = 0xBC00BC00u, H2_NEGHALF = 0xB800B800u, H2_128 = 0x58005800u, H2_511 = 0x5FFC5FFCu;
+constexpr uint32_t H2_NEGHALF = 0xB800B800u, H2_128 = 0x58005800u, H2_511 = 0x5FFC5FFCu;
 // (best, second) dot values packed (lo, hi) -> distances d = (256 - v) / 2 (exact), "none" (sentinel) -> 511
 __device__ __forceinline__ uint32_t dots_to_dist(uint32_t pv) { return hmin2u(hfma2u(pv, H2_NEGHALF, H2_128), H2_511); }
 
-// running top-2 update with one new packed value; ALU-pipe form (3 min/max) and FMA-pipe form (5 HFMA2 / HADD2):
-//   t = relu(v - k1); k1 += t; m = v - t (= min(k1, v)); k2 += relu(m - k2)        (all values integers, exact in f16)
-__device__ __forceinline__ void top2_alu(uint32_t& k1, uint32_t& k2, uint32_t v) {
-    const uint32_t t = hmin2u(k1, v);
-    k1 = hmax2u(k1, v);
-    k2 = hmax2u(k2, t);
-}
-__device__ __forceinline__ void top2_fma(uint32_t& k1, uint32_t& k2, uint32_t v) {
-    const uint32_t t = hfma2relu(k1, H2_NEG1, v);
-    const uint32_t m = hfma2u(t, H2_NEG1, v);
-    k1 = hadd2u(k1, t);
-    k2 = hadd2u(k2, hfma2relu(k2, H2_NEG1, m));
-}
-// two new values at once: 5 ops (3 HMNMX2 + 2 VHMNMX)
+// running top-2 update with two new values at once: 5 packed min / max
 __device__ __forceinline__ void top2_pair(uint32_t& k1, uint32_t& k2, uint32_t a, uint32_t b) {
     const uint32_t hi = hmax2u(a, b), lo = hmin2u(a, b);
     const uint32_t t = hmin2u(k1, hi);
     k2 = hmax2u(hmax2u(k2, lo), t);
     k1 = hmax2u(hmax2u(k1, a), b);
 }
-
-// shared-memory operand descriptor: K-major, 128-byte swizzle, 8-row groups 1024 B apart (SBO), version 1
-__device__ __forceinline__ uint64_t tc_desc(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)0x40004040u << 32);
+// merges another (best, second) pair into (k1, k2), element-wise
+__device__ __forceinline__ void top2_merge(uint32_t& k1, uint32_t& k2, uint32_t o1, uint32_t o2) {
+    k2 = hmax2u(hmax2u(hmin2u(k1, o1), k2), o2);
+    k1 = hmax2u(k1, o1);
 }
-// instruction descriptor: D = f16, A = B = e4m3, both K-major, M = 128, N = 256
-constexpr uint32_t TC_IDESC = (uint32_t)((256 >> 3) << 17) | (uint32_t)((TC_ROWS >> 4) << 24);
+
+// shared-memory operand descriptor: K-major, 128-byte swizzle, 8-row groups 1024 B apart (SBO)
+__device__ __forceinline__ uint64_t tc_desc(uint32_t saddr) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // the matcher
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int TC_OFF_X = 0;
 constexpr int TC_OFF_Y = TC_XSTAGES * TC_TILE_BYTES;                      // [slab 0..1][256 rows]: 64 KB
-constexpr int TC_OFF_SCR = TC_OFF_Y + 2 * TC_TILE_BYTES;                  // per epilogue warp: 16 x 33 words
-constexpr int TC_SCR_WARP = 16 * 33 * 4;
-constexpr int TC_OFF_MRG = TC_OFF_SCR + TC_EW * TC_SCR_WARP;              // [groups][4 quarters][columns per group] uint2: 8 KB
-constexpr int TC_OFF_BAR = TC_OFF_MRG + 4 * 256 * 8;
+constexpr int TC_OFF_MRG = TC_OFF_Y + 2 * TC_TILE_BYTES;                  // [8 consumer warps][256 columns] uint32: 8 KB
+constexpr int TC_OFF_BAR = TC_OFF_MRG + TC_CWARPS * TC_CW * 4;
 constexpr int TC_IRING = 4;                                               // work items announced ahead
-constexpr int TC_NBARS = 2 * TC_XSTAGES + 2 + 2 * TC_ASTAGES + 2 * TC_IRING;
+constexpr int TC_NBARS = 2 * TC_XSTAGES + 2 + 2 * TC_IRING;
 constexpr int TC_OFF_RING = TC_OFF_BAR + TC_NBARS * 8;
-constexpr int TC_OFF_SLOT = TC_OFF_RING + TC_IRING * 4;
-constexpr int TC_SMEM_USED = TC_OFF_SLOT + 16;
+constexpr int TC_SMEM_USED = TC_OFF_RING + TC_IRING * 4;
 static_assert(TC_SMEM_USED + 1024 <= 227 * 1024, "tc_hamming_kernel: shared memory");
 
 size_t tc_smem_bytes() { return (size_t)TC_SMEM_USED + 1024; }
 
-template <int NF>   // NF: column-state registers per 16-register chunk updated on the FMA pipe (0 .. 16)
-#ifndef TC_MAXNREG
-#define TC_MAXNREG 0
-#endif
-#if TC_MAXNREG > 0
-__global__ void __maxnreg__(TC_MAXNREG)
-#else
 __global__ void __launch_bounds__(TC_THREADS, 1)
-#endif
 tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restrict__ items_a, int n_a,
                   const TcItem* __restrict__ items_b, int n_b, int* __restrict__ sched, __half* __restrict__ debug_tile) {
     extern __shared__ uint8_t smem_raw[];
@@ -224,12 +188,9 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
     uint64_t* x_empty = bars + TC_XSTAGES;
     uint64_t* y_full = bars + 2 * TC_XSTAGES;
     uint64_t* y_empty = y_full + 1;
-    uint64_t* t_full = y_empty + 1;
-    uint64_t* t_empty = t_full + TC_ASTAGES;
-    uint64_t* i_full = t_empty + TC_ASTAGES;
+    uint64_t* i_full = y_empty + 1;
     uint64_t* i_empty = i_full + TC_IRING;
     volatile int* iring = reinterpret_cast<volatile int*>(sm + TC_OFF_RING);
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + TC_OFF_SLOT);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int n_items = n_a + n_b;
@@ -237,36 +198,23 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
     if (tid == 0) {
         for (int i = 0; i < TC_XSTAGES; ++i) {
             mbar_init(&x_full[i], 1);
-            mbar_init(&x_empty[i], 1);
+            mbar_init(&x_empty[i], TC_CWARPS);
         }
         mbar_init(y_full, 1);
-        mbar_init(y_empty, 1);
-        for (int i = 0; i < TC_ASTAGES; ++i) {
-            mbar_init(&t_full[i], 1);
-            mbar_init(&t_empty[i], TC_EW);
-        }
+        mbar_init(y_empty, TC_CWARPS);
         for (int i = 0; i < TC_IRING; ++i) {
             mbar_init(&i_full[i], 1);
-            mbar_init(&i_empty[i], TC_EW + 1);   // the MMA thread + the epilogue warps
+            mbar_init(&i_empty[i], TC_CWARPS);
         }
         fence_mbar_init();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "n"(TC_ASTAGES * 256)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // work items are handed out by an atomic counter (long ones first: list a, then list b) and announced to the other
-    // roles through a small ring in shared memory; -1 ends the kernel
+    // work items are handed out by an atomic counter (long ones first: list a, then list b) and announced to the
+    // consumers through a small ring in shared memory; -1 ends the kernel
     auto item_at = [&](int it) -> TcItem { return it < n_a ? items_a[it] : items_b[it - n_a]; };
 
-    if (warp == 0) {
+    if (warp == TC_CWARPS) {
         // ===== producer: work distribution + bulk copies of operand tiles =====
         if (lane == 0) {
             uint32_t xs = 0, xph = 0;
@@ -297,47 +245,21 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: one thread =====
-        if (lane == 0) {
-            uint32_t xs = 0, xph = 0, as = 0, aph = 0;
-            for (uint32_t k = 0;; ++k) {
-                const uint32_t slot = k % TC_IRING;
-                mbar_wait(&i_full[slot], (k / TC_IRING) & 1);
-                const int it = iring[slot];
-                mbar_arrive(&i_empty[slot]);
-                if (it < 0) break;
-                const TcItem item = item_at(it);
-                const TcProblem pr = problems[item.problem];
-                const int nxt = (pr.n1 + TC_ROWS - 1) / TC_ROWS;
-                mbar_wait(y_full, k & 1);
-                for (int t = 0; t < nxt; ++t) {
-                    mbar_wait(&t_empty[as], aph ^ 1);
-                    mbar_wait(&x_full[xs], xph);
-                    tc_fence_after();
-                    const uint32_t xa = sbase + TC_OFF_X + xs * TC_TILE_BYTES, ya = sbase + TC_OFF_Y;
-                    const uint32_t d = tmem_base + as * 256;
-#pragma unroll
-                    for (int kk = 0; kk < 8; ++kk)
-                        tc_mma_f8(d, tc_desc(xa + (kk >> 2) * 16384 + (kk & 3) * 32),
-                                  tc_desc(ya + (kk >> 2) * 32768 + (kk & 3) * 32), TC_IDESC, kk > 0);
-                    tc_commit(&x_empty[xs]);
-                    tc_commit(&t_full[as]);
-                    if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
-                    if (++as == TC_ASTAGES) { as = 0; aph ^= 1; }
-                }
-                tc_commit(y_empty);
-            }
-        }
     } else {
-        // ===== epilogue: TC_EW warps.  quarter q = TMEM lanes 32q..32q+31 (hardware: warp id % 4), group gq = which TC_CW columns
-        // of the 256-column accumulator (TC_EW = 8: two groups of 128, two warps per scheduler; TC_EW = 16: four groups of 64, four
-        // warps per scheduler: the min / max chains of one warp issue into the dependency stalls of the others)
-        constexpr int CW = TC_CW, NCH = CW / 32, NREG = CW / 2;
-        const int ew = warp - 2, q = warp & 3, gq = ew >> 2;
-        uint32_t* scr = reinterpret_cast<uint32_t*>(sm + TC_OFF_SCR + ew * TC_SCR_WARP);
-        uint2* mrg = reinterpret_cast<uint2*>(sm + TC_OFF_MRG) + gq * 4 * CW;
-        uint32_t as = 0, aph = 0;
+        // ===== consumers: two warpgroups; warpgroup g multiplies query rows 64 g .. 64 g + 63 of every query tile with the
+        // item's 256 trains (wgmma m64n256k32, f16 accumulators in registers: every partial sum is an integer of magnitude
+        // <= 256, exact in f16), then folds the tile into
+        //   row direction    (query -> trains): each thread holds 64 columns of two rows; top-2 in registers, then over the
+        //                                      four lanes of a row by shuffle;
+        //   column direction (train -> queries): element-wise running top-2 over the rows in registers, reduced over lanes,
+        //                                      warps and warpgroups once per work item (not per tile).
+        // Keys carry no indices in the hot loop: only (best, second) VALUES and a small candidate tag.
+        const int wg = warp >> 2, w = warp & 3, q4 = lane & 3, rl = lane >> 2;
+        uint32_t* mrg = reinterpret_cast<uint32_t*>(sm + TC_OFF_MRG);
+        uint32_t d[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) d[i] = 0u;
+        uint32_t xs = 0, xph = 0;
         for (uint32_t k = 0;; ++k) {
             const uint32_t slot = k % TC_IRING;
             mbar_wait(&i_full[slot], (k / TC_IRING) & 1);
@@ -348,155 +270,125 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
             const TcItem item = item_at(it);
             const TcProblem pr = problems[item.problem];
             const int nxt = (pr.n1 + TC_ROWS - 1) / TC_ROWS;
-            const int blk = item.yblk * (256 / CW) + gq;      // CW-column block index of this group
-            const int ycol0 = blk * CW;
-            const int nvalid = min(CW, pr.n2 - ycol0);        // <= 0: nothing for this group
-            uint32_t c1[NREG], c2[NREG];
+            const int ycol0 = item.yblk * TC_CW;
+            const int nvalid = min(TC_CW, pr.n2 - ycol0);
+            uint32_t c1[32], c2[32];
 #pragma unroll
-            for (int i = 0; i < NREG; ++i) c1[i] = c2[i] = NEG2;
+            for (int i = 0; i < 32; ++i) c1[i] = c2[i] = NEG2;
+            mbar_wait(y_full, k & 1);
 
             for (int t = 0; t < nxt; ++t) {
-                mbar_wait(&t_full[as], aph);
-                tc_fence_after();
-                const int x = t * TC_ROWS + q * 32 + lane;
-                const bool xvalid = x < pr.n1;
-                // two independent row chains: A = registers 0..7 (16-column group 2c), B = registers 8..15 (group 2c + 1)
-                uint32_t ra1 = NEG2, ra2 = NEG2, rb1 = NEG2, rb2 = NEG2, ta = 0, tb = 0;
-                const uint32_t tad = tmem_base + ((uint32_t)(q * 32) << 16) + as * 256 + gq * CW;
-                auto fold = [&](const uint32_t (&v)[16], const int c) {
-                    const uint32_t olda = ra1, oldb = rb1;
+                mbar_wait(&x_full[xs], xph);
+                const uint32_t xa = sbase + TC_OFF_X + xs * TC_TILE_BYTES + wg * 8192, ya = sbase + TC_OFF_Y;
+                wg_fence_regs(d);
+                wg_fence();
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        top2_pair(ra1, ra2, v[2 * i], v[2 * i + 1]);
-                        top2_pair(rb1, rb2, v[8 + 2 * i], v[8 + 2 * i + 1]);
-                    }
-                    ta = sel32(hne2mask(ra1, olda), (uint32_t)((2 * c) * 0x00010001u), ta);
-                    tb = sel32(hne2mask(rb1, oldb), (uint32_t)((2 * c + 1) * 0x00010001u), tb);
+                for (int kk = 0; kk < 8; ++kk)
+                    wg_mma_f8(d, tc_desc(xa + (kk >> 2) * 16384 + (kk & 3) * 32), tc_desc(ya + (kk >> 2) * 32768 + (kk & 3) * 32),
+                              kk > 0);
+                wg_commit();
+                wg_wait0();
+                wg_fence_regs(d);
+                __syncwarp();
+                if (lane == 0) {
+                    mbar_arrive(&x_empty[xs]);
+                    if (t == nxt - 1) mbar_arrive(y_empty);
+                }
+                if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
+
+                const int x0 = t * TC_ROWS + wg * 64 + w * 16 + rl;   // rows x0 (registers 2i) and x0 + 8 (registers 2i + 1)
+                if (debug_tile && it == 0 && t == 0) {
 #pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                        if (i < NF) top2_fma(c1[c * 16 + i], c2[c * 16 + i], v[i]);
-                        else top2_alu(c1[c * 16 + i], c2[c * 16 + i], v[i]);
-                    }
-                };
-                if (nvalid == CW && (t + 1) * TC_ROWS <= pr.n1 && debug_tile == nullptr) {
-                    // full tile of a full block (the common case): no per-chunk branches, the next chunk's TMEM load is in
-                    // flight while this one is folded
-                    uint32_t va[16], vb[16];
-                    tc_ld32(tad, va);
+                    for (int i = 0; i < 64; ++i)
+                        *reinterpret_cast<uint32_t*>(debug_tile + (size_t)(x0 - t * TC_ROWS + 8 * (i & 1)) * 256 + 8 * (i >> 1) +
+                                                     2 * q4) = d[i];
+                }
+                if (nvalid < TC_CW || t * TC_ROWS + wg * 64 + 64 > pr.n1) {
+                    // a partial tile or block: rows past the end (zero operand rows) and columns past the end contribute nothing
+                    const bool v0 = x0 < pr.n1, v1 = x0 + 8 < pr.n1;
 #pragma unroll
-                    for (int c = 0; c < NCH; c += 2) {
-                        tc_wait_ld();
-                        tc_ld32(tad + (c + 1) * 32, vb);
-                        fold(va, c);
-                        tc_wait_ld();
-                        if (c + 2 < NCH) tc_ld32(tad + (c + 2) * 32, va);
-                        fold(vb, c + 1);
-                    }
-                } else {
-#pragma unroll
-                    for (int c = 0; c < NCH; ++c) {
-                        if (c * 32 >= nvalid) continue;           // warp-uniform: no valid column in this chunk
-                        uint32_t v[16];
-                        tc_ld32(tad + c * 32, v);
-                        tc_wait_ld();
-                        if (debug_tile && it == 0 && t == 0) {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i)
-                                *reinterpret_cast<uint32_t*>(debug_tile + (size_t)(q * 32 + lane) * 256 + gq * CW + c * 32 + 2 * i) = v[i];
-                        }
-                        if (c * 32 + 32 > nvalid) {               // the one boundary chunk of a partial block
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                const int col = c * 32 + 2 * i;
-                                if (col >= nvalid) v[i] = NEG2;
-                                else if (col + 1 >= nvalid) v[i] = (v[i] & 0xFFFFu) | (NEG2 & 0xFFFF0000u);
-                            }
-                        }
-                        if (xvalid) fold(v, c);                   // rows past the end (zero operand rows) contribute nothing
+                    for (int i = 0; i < 32; ++i) {
+                        const int col = 8 * i + 2 * q4;
+                        const uint32_t cm = col >= nvalid ? 0xFFFFFFFFu : (col + 1 >= nvalid ? 0xFFFF0000u : 0u);
+                        d[2 * i] = v0 ? sel32(cm, NEG2, d[2 * i]) : NEG2;
+                        d[2 * i + 1] = v1 ? sel32(cm, NEG2, d[2 * i + 1]) : NEG2;
                     }
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&t_empty[as]);
-                if (++as == TC_ASTAGES) { as = 0; aph ^= 1; }
-                if (xvalid && nvalid > 0) {
-                    // chains, then the even- and odd-column streams; everything packed, the result sits in the low halves
-                    const uint32_t m1 = hmax2u(ra1, rb1), m2 = hmax2u(hmax2u(hmin2u(ra1, rb1), ra2), rb2);
-                    const uint32_t tg = sel32(hgt2mask(rb1, ra1), tb, ta);
+                // row direction: one chain per row; the tag records which group of four 8-column chunks raised the best
+                uint32_t a1 = NEG2, a2 = NEG2, b1 = NEG2, b2 = NEG2, ta = 0, tb = 0;
+#pragma unroll
+                for (int g = 0; g < 8; ++g) {
+                    const uint32_t olda = a1, oldb = b1;
+                    top2_pair(a1, a2, d[8 * g + 0], d[8 * g + 2]);
+                    top2_pair(b1, b2, d[8 * g + 1], d[8 * g + 3]);
+                    top2_pair(a1, a2, d[8 * g + 4], d[8 * g + 6]);
+                    top2_pair(b1, b2, d[8 * g + 5], d[8 * g + 7]);
+                    ta = sel32(hne2mask(a1, olda), (uint32_t)g * 0x00010001u, ta);
+                    tb = sel32(hne2mask(b1, oldb), (uint32_t)g * 0x00010001u, tb);
+                }
+                // column direction: rows x0 and x0 + 8 into the running state
+#pragma unroll
+                for (int i = 0; i < 32; ++i) top2_pair(c1[i], c2[i], d[2 * i], d[2 * i + 1]);
+                // even- and odd-column streams, then the four lanes of the row; the result sits in the low halves.
+                // tag = parity | chunk group << 1 | lane % 4 << 4
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint32_t m1 = h ? b1 : a1, m2 = h ? b2 : a2, tg = h ? tb : ta;
                     const uint32_t s1 = swap16(m1), s2 = swap16(m2), st = swap16(tg);
-                    const uint32_t f1 = hmax2u(m1, s1), f2 = hmax2u(hmax2u(hmin2u(m1, s1), m2), s2);
-                    const uint32_t tag = sel32(hgt2mask(s1, m1), (st << 1) | 1u, tg << 1) & 0xFu;   // group << 1 | parity
-                    const uint32_t dd = dots_to_dist(__byte_perm(f1, f2, 0x5410));
-                    pr.rowp[(size_t)blk * pr.n1 + x] = h2u_lo(dd) | (h2u_hi(dd) << 9) | (tag << 18);
+                    uint32_t f1 = m1, f2 = m2;
+                    top2_merge(f1, f2, s1, s2);
+                    uint32_t tag = (sel32(hgt2mask(s1, m1), (st << 1) | 1u, tg << 1) & 0xFu) | ((uint32_t)q4 << 4);
+#pragma unroll
+                    for (int m = 1; m <= 2; m <<= 1) {
+                        const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, f1, m), o2 = __shfl_xor_sync(0xFFFFFFFFu, f2, m),
+                                       ot = __shfl_xor_sync(0xFFFFFFFFu, tag, m);
+                        tag = (hgt2mask(o1, f1) & 1u) ? ot : tag;
+                        top2_merge(f1, f2, o1, o2);
+                    }
+                    const int x = x0 + 8 * h;
+                    if (q4 == 0 && x < pr.n1) {
+                        const uint32_t dd = dots_to_dist(__byte_perm(f1, f2, 0x5410));
+                        pr.rowp[(size_t)item.yblk * pr.n1 + x] = h2u_lo(dd) | (h2u_hi(dd) << 9) | (tag << 18);
+                    }
                 }
             }
 
-            // ---- column direction: reduce the element-wise state over the 128 threads of the group ----
-            // per warp: transpose 16 registers at a time through shared memory; lane L folds register (L & 15) over
-            // source lanes 16 (L >> 4) .. +15, the two halves meet by shuffle; then the four quarters merge per column.
+            // ---- column direction: reduce the element-wise state over the eight lanes of a column (shuffles), then over the
+            // eight consumer warps (shared memory); the tag is the warp the best came from ----
 #pragma unroll
-            for (int p = 0; p < NCH; ++p) {
-                const int j = lane & 15, hl = lane >> 4;
+            for (int i = 0; i < 32; ++i) {
+                uint32_t m1 = c1[i], m2 = c2[i];
 #pragma unroll
-                for (int i = 0; i < 16; ++i) scr[i * 33 + lane] = c1[p * 16 + i];
-                __syncwarp();
-                uint32_t m1 = NEG2, m2 = NEG2, id = 0;
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) {
-                    const uint32_t v = scr[j * 33 + hl * 16 + kk];
-                    const uint32_t tmin = hmin2u(m1, v);
-                    const uint32_t nm = hmax2u(m1, v);
-                    m2 = hmax2u(m2, tmin);
-                    id = sel32(hne2mask(nm, m1), (uint32_t)((hl * 16 + kk) * 0x00010001u), id);
-                    m1 = nm;
-                }
-                __syncwarp();
-#pragma unroll
-                for (int i = 0; i < 16; ++i) scr[i * 33 + lane] = c2[p * 16 + i];
-                __syncwarp();
-#pragma unroll
-                for (int kk = 0; kk < 16; ++kk) m2 = hmax2u(m2, scr[j * 33 + hl * 16 + kk]);
-                __syncwarp();
-                // halves: lanes L and L ^ 16 hold the same register over the other 16 source lanes
-                const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, m1, 16), o2 = __shfl_xor_sync(0xFFFFFFFFu, m2, 16),
-                               oid = __shfl_xor_sync(0xFFFFFFFFu, id, 16);
-                const uint32_t n2v = hmax2u(hmax2u(hmin2u(m1, o1), m2), o2);
-                const uint32_t n1v = hmax2u(m1, o1);
-                const uint32_t nid = sel32(hgt2mask(o1, m1), oid, id);
-                if (hl == 0) {
-                    const int col = (p * 16 + j) * 2;
-                    mrg[q * CW + col] = make_uint2((n1v & 0xFFFFu) | (n2v << 16), nid & 0xFFFFu);
-                    mrg[q * CW + col + 1] = make_uint2((n1v >> 16) | (n2v & 0xFFFF0000u), nid >> 16);
+                for (int m = 4; m <= 16; m <<= 1)
+                    top2_merge(m1, m2, __shfl_xor_sync(0xFFFFFFFFu, m1, m), __shfl_xor_sync(0xFFFFFFFFu, m2, m));
+                if (rl == 0) {
+                    const int col = 8 * i + 2 * q4;
+                    mrg[warp * TC_CW + col] = (m1 & 0xFFFFu) | (m2 << 16);
+                    mrg[warp * TC_CW + col + 1] = (m1 >> 16) | (m2 & 0xFFFF0000u);
                 }
             }
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + gq) : "memory");
-            if (lane < CW / 4) {   // the group's four warps share its CW columns
-                const int col = (ew & 3) * (CW / 4) + lane;
+            asm volatile("bar.sync 1, %0;" ::"n"(TC_CWARPS * 32) : "memory");
+            {
+                const int col = tid;   // one column per consumer thread
                 uint32_t b1 = NEG2, b2 = NEG2, bt = 0;   // only the low halves are meaningful
 #pragma unroll
-                for (int qq = 0; qq < 4; ++qq) {
-                    const uint2 e = mrg[qq * CW + col];
-                    const uint32_t a1 = e.x & 0xFFFFu, a2 = e.x >> 16;
-                    b2 = hmax2u(hmax2u(hmin2u(b1, a1), b2), a2);
-                    bt = sel32(hgt2mask(a1, b1), (uint32_t)qq * 32u + e.y, bt);
-                    b1 = hmax2u(b1, a1);
+                for (int s = 0; s < TC_CWARPS; ++s) {
+                    const uint32_t e = mrg[s * TC_CW + col];
+                    const uint32_t a1 = e & 0xFFFFu, a2 = e >> 16;
+                    bt = (hgt2mask(a1, b1) & 1u) ? (uint32_t)s : bt;
+                    top2_merge(b1, b2, a1, a2);
                 }
                 if (col < nvalid) {
                     const uint32_t dd = dots_to_dist(__byte_perm(b1, b2, 0x5410));
-                    pr.colp[ycol0 + col] = h2u_lo(dd) | (h2u_hi(dd) << 9) | ((bt & 0x7Fu) << 18);
+                    pr.colp[ycol0 + col] = h2u_lo(dd) | (h2u_hi(dd) << 9) | (bt << 18);
                 }
             }
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + gq) : "memory");
+            asm volatile("bar.sync 1, %0;" ::"n"(TC_CWARPS * 32) : "memory");
         }
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TC_ASTAGES * 256)
-                     : "memory");
-    }
     // the last CTA out re-arms the scheduler words for the next launch on this stream
+    __syncthreads();
     if (tid == 0) {
         __threadfence();
         if (atomicAdd(sched + 1, 1) == (int)gridDim.x - 1) {
@@ -507,42 +399,24 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
     }
 }
 
-static int tc_nf() {   // tuning knob: how many of the 16 column registers per chunk use the FMA-pipe update
-    static const int nf = [] {
-        const char* v = getenv("PLSTVO_TC_NF");
-        return v ? atoi(v) : 0;
-    }();
-    return nf;
-}
-
 cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, int n_a, const TcItem* items_b, int n_b,
                               int* sched, int grid, __half* debug_tile, cudaStream_t stream) {
     const int n_items = n_a + n_b;
     if (n_items <= 0) return cudaSuccess;
-    typedef void (*Fn)(const TcProblem*, const TcItem*, int, const TcItem*, int, int*, __half*);
-    Fn fn;
-    switch (tc_nf()) {
-        case 4: fn = tc_hamming_kernel<4>; break;
-        case 6: fn = tc_hamming_kernel<6>; break;
-        case 8: fn = tc_hamming_kernel<8>; break;
-        case 10: fn = tc_hamming_kernel<10>; break;
-        case 12: fn = tc_hamming_kernel<12>; break;
-        default: fn = tc_hamming_kernel<0>; break;
-    }
-    static size_t configured[8][64] = {};
+    static size_t configured[64] = {};
     const size_t smem = tc_smem_bytes();
-    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(fn), smem, configured[(tc_nf() / 2) & 7]);
+    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(tc_hamming_kernel), smem, configured);
     if (e != cudaSuccess) return e;
     if (grid > n_items) grid = n_items;
     if (getenv("PLSTVO_TC_DIAG")) {
         cudaFuncAttributes fa;
         int occ = -1;
-        cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(fn));
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, TC_THREADS, smem);
+        cudaFuncGetAttributes(&fa, reinterpret_cast<const void*>(tc_hamming_kernel));
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, tc_hamming_kernel, TC_THREADS, smem);
         fprintf(stderr, "[tc diag] regs %d, maxThreadsPerBlock %d, static smem %zu, local %zu, dynamic smem %zu, occupancy %d\n",
                 fa.numRegs, fa.maxThreadsPerBlock, fa.sharedSizeBytes, fa.localSizeBytes, smem, occ);
     }
-    fn<<<grid, TC_THREADS, smem, stream>>>(problems, items_a, n_a, items_b, n_b, sched, debug_tile);
+    tc_hamming_kernel<<<grid, TC_THREADS, smem, stream>>>(problems, items_a, n_a, items_b, n_b, sched, debug_tile);
     return cudaGetLastError();
 }
 
@@ -562,7 +436,7 @@ __global__ void __launch_bounds__(256) tc_resolve_kernel(const MatchProblem* __r
     const int nyh = (mp.n2 + TC_CW - 1) / TC_CW, nxt = (mp.n1 + TC_ROWS - 1) / TC_ROWS;   // row partials: one per TC_CW-train block
     const int slice = blockIdx.y, nslices = gridDim.y;
     // partial word: best distance (9 bits) | second distance << 9 (511 = none) | candidate tag << 18
-    // queries: top-2 trains over the 128-train blocks (lowest block wins a tie: its indices are lower)
+    // queries: top-2 trains over the 256-train blocks (lowest block wins a tie: its indices are lower)
     for (int x = slice * blockDim.x + threadIdx.x; x < mp.n1; x += nslices * blockDim.x) {
         uint32_t b1 = 511, b2 = 511, btag = 0;
         int bh = 0;
@@ -582,10 +456,10 @@ __global__ void __launch_bounds__(256) tc_resolve_kernel(const MatchProblem* __r
                 const uint4 a0 = __ldg(reinterpret_cast<const uint4*>(mp.d1 + (size_t)x * 32)),
                             a1 = __ldg(reinterpret_cast<const uint4*>(mp.d1 + (size_t)x * 32) + 1);
                 idx = -1;
-                if (d1 != d2) {   // unique best: it is one of the 8 tagged trains (16-column group, one parity)
-                    const int base = bh * TC_CW + (int)((btag >> 1) & 7u) * 16 + (int)(btag & 1u);
-                    for (int i = 0; i < 8 && idx < 0; ++i) {
-                        const int j = base + 2 * i;
+                if (d1 != d2) {   // unique best: it is one of the 4 tagged trains (one lane's columns of a chunk group, one parity)
+                    const int base = bh * TC_CW + (int)((btag >> 1) & 7u) * 32 + (int)((btag >> 4) & 3u) * 2 + (int)(btag & 1u);
+                    for (int i = 0; i < 4 && idx < 0; ++i) {
+                        const int j = base + 8 * i;
                         if (j < mp.n2 && hamming256(a0, a1, mp.d2 + (size_t)j * 32) == d1) idx = j;
                     }
                 }
@@ -615,12 +489,13 @@ __global__ void __launch_bounds__(256) tc_resolve_kernel(const MatchProblem* __r
                     // unique best: WHICH query it is does not matter to the mutual filter (match_finalize.cuh: a query whose
                     // nearest train is y at distance d1 is that query) — no candidate is re-evaluated
                     idx = (int)KEY_IDX_UNRESOLVED;
-                } else if (d1 != d2) {   // (frames beyond 65024 rows) one of the queries the tagged epilogue thread saw (row = tag mod 128)
-                    const int t = (int)((e >> 18) & 127u);
-                    for (int i = 0; i < nxt && idx < 0; ++i) {
-                        const int j = t + i * TC_ROWS;
-                        if (j < mp.n1 && hamming256(a0, a1, mp.d1 + (size_t)j * 32) == d1) idx = j;
-                    }
+                } else if (d1 != d2) {   // (frames beyond 65024 rows) one of the 16 rows per tile the tagged consumer warp holds
+                    const int wt = (int)((e >> 18) & 7u), r0 = (wt >> 2) * 64 + (wt & 3) * 16;
+                    for (int i = 0; i < nxt && idx < 0; ++i)
+                        for (int r = 0; r < 16 && idx < 0; ++r) {
+                            const int j = r0 + r + i * TC_ROWS;
+                            if (j < mp.n1 && hamming256(a0, a1, mp.d1 + (size_t)j * 32) == d1) idx = j;
+                        }
                 }
                 if (idx < 0) {
                     for (int j = 0; j < mp.n1 && idx < 0; ++j)

@@ -6,20 +6,12 @@
 
 namespace plstvo {
 
-constexpr int TC_ROWS = 128;                    // descriptor rows per operand tile (UMMA M and N)
+constexpr int TC_ROWS = 128;                    // descriptor rows per operand tile (two wgmma M blocks of 64; N = 2 tiles)
 constexpr int TC_TILE_BYTES = TC_ROWS * 256;    // 128 rows x 256 e4m3 bytes, swizzled K-major layout
-#ifndef TC_EPILOGUE_WARPS
-#define TC_EPILOGUE_WARPS 8
-#endif
-// epilogue warps: 8 (two per scheduler, 128 accumulator columns each) or 16 (four per scheduler, 64 columns each: 96 registers per
-// thread).  Measured on 512 C2 pairs: 8 warps 0.627 ms; 16 warps 0.664 ms, 0.625 ms with half of the column updates on the FMA pipe
-// (PLSTVO_TC_NF=8) — no gain, so 8 stays the default and -DTC_EPILOGUE_WARPS=16 remains a build option.
-constexpr int TC_EW = TC_EPILOGUE_WARPS;
-constexpr int TC_CW = 1024 / TC_EW;             // accumulator columns per epilogue warp = trains per row-partial block
-constexpr int TC_XSTAGES = TC_EW == 16 ? 3 : 4; // query tiles in flight (shared memory ring; 16 warps need the room for their scratch)
-constexpr int TC_ASTAGES = 2;                   // accumulator stages in TMEM (256 columns each)
-constexpr int TC_THREADS = 64 + 32 * TC_EW;     // producer warp + MMA warp + the epilogue warps
-static_assert(TC_EW == 8 || TC_EW == 16, "epilogue warps");
+constexpr int TC_CW = 256;                      // trains per work item = per row-partial block (wgmma N)
+constexpr int TC_CWARPS = 8;                    // consumer warps: two warpgroups, 64 query rows of each tile apiece
+constexpr int TC_XSTAGES = 4;                   // query tiles in flight (shared memory ring)
+constexpr int TC_THREADS = 32 * TC_CWARPS + 32; // the consumer warpgroups + one producer warp
 
 // one descriptor matrix to expand (queries or trains of one matching problem)
 struct TcSide {
@@ -33,8 +25,8 @@ struct TcProblem {
     const uint8_t* xe;    // expanded queries  (desc1): ceil(n1 / 128) tiles
     const uint8_t* ye;    // expanded trains   (desc2): ceil(n2 / 128) tiles
     int32_t n1, n2;
-    uint32_t* rowp;       // [ceil(n2 / TC_CW)][n1]: best distance | second << 9 (511 = none) | tag << 18 (16-column group, parity)
-    uint32_t* colp;       // [n2]:                 best | second << 9 | tag << 18 (query row mod 128)
+    uint32_t* rowp;       // [ceil(n2 / TC_CW)][n1]: best distance | second << 9 (511 = none) | tag << 18 (parity, chunk group, lane)
+    uint32_t* colp;       // [n2]:                 best | second << 9 | tag << 18 (consumer warp)
 };
 
 // one work item of the persistent kernel: all query tiles of a problem against 256 trains

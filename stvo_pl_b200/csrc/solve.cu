@@ -12,7 +12,7 @@
 //      and a binary search on the V-shaped deviation sequence; isGoodSolution (:292-305) with a parallel-order
 //      Jacobi eigen-solver; pose finalisation (:372-391).
 // Features are read from HBM exactly once per solve; every GN evaluation runs out of shared memory.
-// All arithmetic is double precision like the reference (B200 has a full-rate FP64 pipe).  Summation order,
+// All arithmetic is double precision like the reference (the H100 FP64 pipe runs at half the FP32 rate).  Summation order,
 // reciprocal-multiplies and the 6x6 algorithms differ from the reference at rounding level (1e-16 relative),
 // far inside the 1e-5 rad / 1e-4 m bar; the reduction order is fixed, so results are run-to-run deterministic.
 #include <math.h>
@@ -1992,7 +1992,7 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
             } else {                           // ---- consumers ----
 #pragma unroll
                 for (int i = 0; i < 12; i++) P.r[i] = sPose[i];
-                GsAccPacked acc;
+                GsAccScalar acc;
                 acc.clear();
                 double run = 0.0;              // lane L: this warp's fp64 total of accumulator L so far
                 for (int t = 0; t < n_tiles; ++t) {

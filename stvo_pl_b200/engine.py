@@ -1,5 +1,5 @@
 """ctypes binding of the CUDA library (stvo_pl_b200/lib/libplstvo_b200.so) through its C-ABI
-(include/plstvo.h).  There is no CPU fallback: a missing extension or a missing sm_100 device raises.
+(include/plstvo.h).  There is no CPU fallback: a missing extension or a missing sm_90 device raises.
 """
 from __future__ import annotations
 
@@ -227,7 +227,7 @@ class Engine:
         ctx = C.c_void_p()
         rc = self.lib.plstvo_create(device, C.byref(ctx))
         if rc != 0:
-            raise PlstvoError(rc, "plstvo_create failed: no sm_100 CUDA device visible (no CPU fallback exists)")
+            raise PlstvoError(rc, "plstvo_create failed: no sm_90 CUDA device visible (no CPU fallback exists)")
         self.ctx = ctx
         self.pinned = PinnedPool(self.lib)
 

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run on the GPU box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

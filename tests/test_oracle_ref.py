@@ -4,26 +4,43 @@ oracle/_ref/libplstvo_ref.so holds optimizeFunctions, optimizeFunctionsRobust, g
 removeOutliers, isGoodSolution, optimizePose (src/stereoFrameHandler.cpp:292-480, 549-962, 988-1067), lineSegmentOverlap
 (src/stereoFrame.cpp:510-616), projection / backProjection (src/pinholeStereoCamera.cpp:221-237), the SE(3) helpers and
 the MAD statistics (src/auxiliar.cpp:29-44, 58-62, 113-197, 353-355, 387-430, 444-460, 556-583) compiled from the text of
-/root/reference by line range (oracle/make_ref.py) against stand-in Eigen headers.  Every comparison below is
+the reference by line range (oracle/make_ref.py) against stand-in Eigen headers.  Every comparison below is
 oracle (our restatement, oracle/plstvo_oracle.c) == that library on the same inputs.
+
+Where that library cannot be built (the reference sources are not present), the library's answers to the same calls are
+replayed from tests/golden/ref_calls.npz.  Re-record them where the reference is present with
+PLSTVO_RECORD_REF=1 python -m pytest tests/test_oracle_ref.py.
 
 What the library does NOT contain is Eigen itself: its 6x6 decompositions are the stand-in's, so the first group of tests
 holds those against LAPACK (numpy.linalg) instead.
 """
+import os
+
 import numpy as np
 import pytest
 
 import ref_numpy as R
+from conftest import GOLDEN
+from oracle import ref as ref_mod
 from stvo_pl_b200 import synth, types as T
 
-ref_mod = pytest.importorskip("oracle.ref")
-if not ref_mod.available():
-    pytest.skip("oracle/_ref not built and /root/reference absent", allow_module_level=True)
+REF_CALLS = os.path.join(GOLDEN, "ref_calls.npz")
 
 
 @pytest.fixture(scope="module")
-def ref():
-    return ref_mod.Ref()
+def ref_store():
+    if os.environ.get("PLSTVO_RECORD_REF"):
+        store = ref_mod.Recorded(REF_CALLS, record=ref_mod.Ref())
+        yield store
+        store.save()
+    else:
+        yield ref_mod.Recorded(REF_CALLS)
+
+
+@pytest.fixture
+def ref(ref_store, request):
+    ref_store.begin(request.node.name)
+    return ref_store
 
 
 def _rng(seed):
