@@ -556,7 +556,7 @@ int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t 
             // launches on the two compute streams may overlap: each has its own pair of scheduler words
             int* sched = ws.d_sched.as<int>() + (s == ctx->s_alt ? 8 : 0);
             CK(ctx, launch_tc_hamming(ws.d_tcprob.as<TcProblem>(), ws.d_tcitems[0].as<TcItem>() + a0, a1 - a0,
-                                      ws.d_tcitems[1].as<TcItem>() + b0, b1 - b0, sched, ctx->sm_count, nullptr, s));
+                                      ws.d_tcitems[1].as<TcItem>() + b0, b1 - b0, sched, ctx->sm_count, s));
             if (marks) CK(ctx, cudaEventRecord(marks[1], s));
             CK(ctx, launch_tc_resolve(ws.d_problems.as<MatchProblem>() + (size_t)2 * p0, ws.d_tcprob.as<TcProblem>() + (size_t)2 * p0,
                                       2 * (p1 - p0), 4, s));

@@ -7,9 +7,10 @@
 //   tc_expand_kernel   32-byte descriptor rows -> 256 e4m3 bytes (+1.0 = 0x38, -1.0 = 0xB8), written directly in the
 //                      128-byte-swizzled K-major operand layout wgmma reads (tiles of 128 rows = 32 KB contiguous),
 //                      so the tiles move with plain bulk copies (UBLKCP) and need no tensor map;
-//   tc_hamming_kernel  persistent, warp-specialised: one producer warp (bulk copies + mbarriers), two consumer
-//                      warpgroups issuing wgmma m64n256k32 (e4m3 operands, f16 accumulators in registers, two columns
-//                      per register), so the top-2 update of BOTH directions costs a few packed min/max per two distances:
+//   tc_hamming_kernel  persistent, warp-specialised: one producer thread (bulk copies + mbarriers), two consumer
+//                      warpgroups issuing wgmma m64n128k32 (e4m3 operands, f16 accumulators in registers, two columns
+//                      per register) on the two 128-train halves of a block, each half folded while the other is on the
+//                      tensor pipe, so the top-2 update of BOTH directions costs a few packed min/max per two distances:
 //                        row direction   (query -> trains): fold over the columns in registers, then over four lanes;
 //                        column direction (train -> queries): element-wise running top-2 over the row tiles in
 //                                         registers, one cross-lane reduction per work item (not per tile).
@@ -24,6 +25,7 @@
 
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "match_finalize.cuh"
@@ -76,26 +78,28 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 256] (f16, 64 registers) (+)= A[64 x 32] . B[256 x 32]^T, both e4m3 and K-major in shared memory.
-// Register d[2i + h] of lane l in warp w of the warpgroup holds row 16 w + l / 4 + 8 h, columns 8 i + 2 (l % 4) + {0, 1}
-// (low half = even column).
-__device__ __forceinline__ void wg_mma_f8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc, int acc) {
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (f16, 32 registers) (+)= A[64 x 32] . B[128 x 32]^T, both e4m3 and K-major in shared memory.
+// Register d[2i + r] of lane l in warp w of the warpgroup holds row 16 w + l / 4 + 8 r, columns 8 i + 2 (l % 4) + {0, 1}
+// (low half = even column), i = 0..15.
+__device__ __forceinline__ void wg_mma_f8(uint32_t (&d)[32], uint64_t adesc, uint64_t bdesc, int acc) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %66, 0;\n"
-        "wgmma.mma_async.sync.aligned.m64n256k32.f16.e4m3.e4m3 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f16.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n"
         "}\n"
-        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
         : "l"(adesc), "l"(bdesc), "r"(acc)
         : "memory");
 }
-// keeps the compiler from moving reads or writes of the accumulators across the wgmma fence / wait
-__device__ __forceinline__ void wg_fence_regs(uint32_t (&d)[64]) {
+// keeps the compiler from moving reads or writes of one accumulator set across the wgmma fence / wait.  Per set, never
+// across both: the other set is in flight meanwhile, and touching its registers makes ptxas serialise the wgmma.
+__device__ __forceinline__ void wg_fence_regs(uint32_t (&d)[32]) {
 #pragma unroll
-    for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(d[i])::"memory");
 }
 
 // packed f16x2 arithmetic on raw 32-bit registers
@@ -161,11 +165,24 @@ __device__ __forceinline__ uint64_t tc_desc(uint32_t saddr) {
     return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 
+// issues one 128-train half of a query tile into accumulator set d as one commit group: 8 K-steps (two 128-byte slabs x
+// four k32).  xa: the warpgroup's 64 query rows of the stage (slab 0); yb: the half's train tile in slab 0 of the train block
+__device__ __forceinline__ void wg_issue_half(uint32_t (&d)[32], uint32_t xa, uint32_t yb) {
+    wg_fence_regs(d);
+    wg_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+        wg_mma_f8(d, tc_desc(xa + (kk >> 2) * 16384 + (kk & 3) * 32), tc_desc(yb + (kk >> 2) * 32768 + (kk & 3) * 32), kk > 0);
+    wg_commit();
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // the matcher
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int TC_OFF_X = 0;
 constexpr int TC_OFF_Y = TC_XSTAGES * TC_TILE_BYTES;                      // [slab 0..1][256 rows]: 64 KB
+constexpr int TC_HN = TC_CW / 2;                                          // wgmma N: trains per accumulator set
+constexpr int TC_HALF_BYTES = TC_HN * 128;                                // train half 1 within a slab of the train block
 constexpr int TC_OFF_MRG = TC_OFF_Y + 2 * TC_TILE_BYTES;                  // [8 consumer warps][256 columns] uint32: 8 KB
 constexpr int TC_OFF_BAR = TC_OFF_MRG + TC_CWARPS * TC_CW * 4;
 constexpr int TC_IRING = 4;                                               // work items announced ahead
@@ -176,9 +193,22 @@ static_assert(TC_SMEM_USED + 1024 <= 227 * 1024, "tc_hamming_kernel: shared memo
 
 size_t tc_smem_bytes() { return (size_t)TC_SMEM_USED + 1024; }
 
+// Register budget: the CTA launches with 168 registers per thread (384 threads, 1 CTA / SM), too few for both accumulator
+// sets, the column state and the row chains of a consumer thread.  The producer warpgroup, one thread of which issues
+// the copies, hands most of its share to the consumers (setmaxnreg); each of the four SM sub-partitions then holds two
+// consumer warps and one producer warp: (2 x 232 + 40) x 32 <= 16384 registers.
+constexpr int TC_LAUNCH_REGS = 168, TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
+static_assert(TC_LAUNCH_REGS * TC_THREADS <= 65536 &&
+                  TC_CWARPS * TC_CONSUMER_REGS + (TC_THREADS / 32 - TC_CWARPS) * TC_PRODUCER_REGS <= TC_LAUNCH_REGS * TC_THREADS / 32,
+              "tc_hamming_kernel: register budget");
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restrict__ items_a, int n_a,
-                  const TcItem* __restrict__ items_b, int n_b, int* __restrict__ sched, __half* __restrict__ debug_tile) {
+                  const TcItem* __restrict__ items_b, int n_b, int* __restrict__ sched) {
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t sbase = (raw + 1023u) & ~1023u;
@@ -214,9 +244,10 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
     // consumers through a small ring in shared memory; -1 ends the kernel
     auto item_at = [&](int it) -> TcItem { return it < n_a ? items_a[it] : items_b[it - n_a]; };
 
-    if (warp == TC_CWARPS) {
+    if (warp >= TC_CWARPS) {
         // ===== producer: work distribution + bulk copies of operand tiles =====
-        if (lane == 0) {
+        setmaxnreg_dec<TC_PRODUCER_REGS>();
+        if (warp == TC_CWARPS && lane == 0) {
             uint32_t xs = 0, xph = 0;
             for (uint32_t k = 0;; ++k) {
                 const uint32_t slot = k % TC_IRING;
@@ -247,18 +278,21 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
         }
     } else {
         // ===== consumers: two warpgroups; warpgroup g multiplies query rows 64 g .. 64 g + 63 of every query tile with the
-        // item's 256 trains (wgmma m64n256k32, f16 accumulators in registers: every partial sum is an integer of magnitude
-        // <= 256, exact in f16), then folds the tile into
+        // item's 256 trains (f16 accumulators in registers: every partial sum is an integer of magnitude <= 256, exact in
+        // f16), then folds the tile into
         //   row direction    (query -> trains): each thread holds 64 columns of two rows; top-2 in registers, then over the
         //                                      four lanes of a row by shuffle;
         //   column direction (train -> queries): element-wise running top-2 over the rows in registers, reduced over lanes,
         //                                      warps and warpgroups once per work item (not per tile).
         // Keys carry no indices in the hot loop: only (best, second) VALUES and a small candidate tag.
+        // The 256 trains are two halves of 128 (wgmma m64n128k32), one accumulator set each, software-pipelined so that
+        // each half of a tile is folded while the MMA of the next half (t, 1) or (t + 1, 0) is on the tensor pipe.
+        setmaxnreg_inc<TC_CONSUMER_REGS>();
         const int wg = warp >> 2, w = warp & 3, q4 = lane & 3, rl = lane >> 2;
         uint32_t* mrg = reinterpret_cast<uint32_t*>(sm + TC_OFF_MRG);
-        uint32_t d[64];
+        uint32_t acc[2][32];
 #pragma unroll
-        for (int i = 0; i < 64; ++i) d[i] = 0u;
+        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i] = 0u;
         uint32_t xs = 0, xph = 0;
         for (uint32_t k = 0;; ++k) {
             const uint32_t slot = k % TC_IRING;
@@ -276,82 +310,110 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
 #pragma unroll
             for (int i = 0; i < 32; ++i) c1[i] = c2[i] = NEG2;
             mbar_wait(y_full, k & 1);
-
-            for (int t = 0; t < nxt; ++t) {
-                mbar_wait(&x_full[xs], xph);
-                const uint32_t xa = sbase + TC_OFF_X + xs * TC_TILE_BYTES + wg * 8192, ya = sbase + TC_OFF_Y;
-                wg_fence_regs(d);
-                wg_fence();
-#pragma unroll
-                for (int kk = 0; kk < 8; ++kk)
-                    wg_mma_f8(d, tc_desc(xa + (kk >> 2) * 16384 + (kk & 3) * 32), tc_desc(ya + (kk >> 2) * 32768 + (kk & 3) * 32),
-                              kk > 0);
-                wg_commit();
-                wg_wait0();
-                wg_fence_regs(d);
-                __syncwarp();
-                if (lane == 0) {
-                    mbar_arrive(&x_empty[xs]);
-                    if (t == nxt - 1) mbar_arrive(y_empty);
-                }
-                if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
-
+            const uint32_t xw = sbase + TC_OFF_X + wg * 8192, ya = sbase + TC_OFF_Y;   // + stage, + half of the trains
+            // row direction: one chain per row, carried from half 0 to half 1 of a tile; the tag records which group of
+            // four 8-column chunks (0..7 over both halves) raised the best
+            uint32_t a1, a2, b1, b2, ta, tb;
+            // masks and folds the retired accumulator set h of tile t; after half 1 the row chains are merged and stored
+            auto fold = [&](auto hc, int t) {
+                constexpr int h = decltype(hc)::value;
+                uint32_t (&d)[32] = acc[h];
                 const int x0 = t * TC_ROWS + wg * 64 + w * 16 + rl;   // rows x0 (registers 2i) and x0 + 8 (registers 2i + 1)
-                if (debug_tile && it == 0 && t == 0) {
-#pragma unroll
-                    for (int i = 0; i < 64; ++i)
-                        *reinterpret_cast<uint32_t*>(debug_tile + (size_t)(x0 - t * TC_ROWS + 8 * (i & 1)) * 256 + 8 * (i >> 1) +
-                                                     2 * q4) = d[i];
-                }
-                if (nvalid < TC_CW || t * TC_ROWS + wg * 64 + 64 > pr.n1) {
+                if (nvalid < TC_HN * (h + 1) || t * TC_ROWS + wg * 64 + 64 > pr.n1) {
                     // a partial tile or block: rows past the end (zero operand rows) and columns past the end contribute nothing
                     const bool v0 = x0 < pr.n1, v1 = x0 + 8 < pr.n1;
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int col = 8 * i + 2 * q4;
+                    for (int i = 0; i < 16; ++i) {
+                        const int col = TC_HN * h + 8 * i + 2 * q4;
                         const uint32_t cm = col >= nvalid ? 0xFFFFFFFFu : (col + 1 >= nvalid ? 0xFFFF0000u : 0u);
                         d[2 * i] = v0 ? sel32(cm, NEG2, d[2 * i]) : NEG2;
                         d[2 * i + 1] = v1 ? sel32(cm, NEG2, d[2 * i + 1]) : NEG2;
                     }
                 }
-                // row direction: one chain per row; the tag records which group of four 8-column chunks raised the best
-                uint32_t a1 = NEG2, a2 = NEG2, b1 = NEG2, b2 = NEG2, ta = 0, tb = 0;
+                if (h == 0) {
+                    a1 = a2 = b1 = b2 = NEG2;
+                    ta = tb = 0;
+                }
 #pragma unroll
-                for (int g = 0; g < 8; ++g) {
+                for (int g = 0; g < 4; ++g) {
                     const uint32_t olda = a1, oldb = b1;
                     top2_pair(a1, a2, d[8 * g + 0], d[8 * g + 2]);
                     top2_pair(b1, b2, d[8 * g + 1], d[8 * g + 3]);
                     top2_pair(a1, a2, d[8 * g + 4], d[8 * g + 6]);
                     top2_pair(b1, b2, d[8 * g + 5], d[8 * g + 7]);
-                    ta = sel32(hne2mask(a1, olda), (uint32_t)g * 0x00010001u, ta);
-                    tb = sel32(hne2mask(b1, oldb), (uint32_t)g * 0x00010001u, tb);
+                    ta = sel32(hne2mask(a1, olda), (uint32_t)(4 * h + g) * 0x00010001u, ta);
+                    tb = sel32(hne2mask(b1, oldb), (uint32_t)(4 * h + g) * 0x00010001u, tb);
                 }
-                // column direction: rows x0 and x0 + 8 into the running state
+                // column direction: rows x0 and x0 + 8 into the running state of this half's columns
 #pragma unroll
-                for (int i = 0; i < 32; ++i) top2_pair(c1[i], c2[i], d[2 * i], d[2 * i + 1]);
-                // even- and odd-column streams, then the four lanes of the row; the result sits in the low halves.
-                // tag = parity | chunk group << 1 | lane % 4 << 4
+                for (int i = 0; i < 16; ++i) top2_pair(c1[16 * h + i], c2[16 * h + i], d[2 * i], d[2 * i + 1]);
+                if constexpr (h == 1) {
+                    // even- and odd-column streams, then the four lanes of the row; the result sits in the low halves.
+                    // tag = parity | chunk group << 1 | lane % 4 << 4
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t m1 = h ? b1 : a1, m2 = h ? b2 : a2, tg = h ? tb : ta;
-                    const uint32_t s1 = swap16(m1), s2 = swap16(m2), st = swap16(tg);
-                    uint32_t f1 = m1, f2 = m2;
-                    top2_merge(f1, f2, s1, s2);
-                    uint32_t tag = (sel32(hgt2mask(s1, m1), (st << 1) | 1u, tg << 1) & 0xFu) | ((uint32_t)q4 << 4);
+                    for (int r = 0; r < 2; ++r) {
+                        const uint32_t m1 = r ? b1 : a1, m2 = r ? b2 : a2, tg = r ? tb : ta;
+                        const uint32_t s1 = swap16(m1), s2 = swap16(m2), st = swap16(tg);
+                        uint32_t f1 = m1, f2 = m2;
+                        top2_merge(f1, f2, s1, s2);
+                        uint32_t tag = (sel32(hgt2mask(s1, m1), (st << 1) | 1u, tg << 1) & 0xFu) | ((uint32_t)q4 << 4);
 #pragma unroll
-                    for (int m = 1; m <= 2; m <<= 1) {
-                        const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, f1, m), o2 = __shfl_xor_sync(0xFFFFFFFFu, f2, m),
-                                       ot = __shfl_xor_sync(0xFFFFFFFFu, tag, m);
-                        tag = (hgt2mask(o1, f1) & 1u) ? ot : tag;
-                        top2_merge(f1, f2, o1, o2);
-                    }
-                    const int x = x0 + 8 * h;
-                    if (q4 == 0 && x < pr.n1) {
-                        const uint32_t dd = dots_to_dist(__byte_perm(f1, f2, 0x5410));
-                        pr.rowp[(size_t)item.yblk * pr.n1 + x] = h2u_lo(dd) | (h2u_hi(dd) << 9) | (tag << 18);
+                        for (int m = 1; m <= 2; m <<= 1) {
+                            const uint32_t o1 = __shfl_xor_sync(0xFFFFFFFFu, f1, m), o2 = __shfl_xor_sync(0xFFFFFFFFu, f2, m),
+                                           ot = __shfl_xor_sync(0xFFFFFFFFu, tag, m);
+                            tag = (hgt2mask(o1, f1) & 1u) ? ot : tag;
+                            top2_merge(f1, f2, o1, o2);
+                        }
+                        const int x = x0 + 8 * r;
+                        if (q4 == 0 && x < pr.n1) {
+                            const uint32_t dd = dots_to_dist(__byte_perm(f1, f2, 0x5410));
+                            pr.rowp[(size_t)item.yblk * pr.n1 + x] = h2u_lo(dd) | (h2u_hi(dd) << 9) | (tag << 18);
+                        }
                     }
                 }
+            };
+            constexpr std::integral_constant<int, 0> H0{};
+            constexpr std::integral_constant<int, 1> H1{};
+
+            // Each fold runs under the MMA of the other half: (t, 1) is issued before (t, 0) is folded, (t + 1, 0) before
+            // (t, 1) is.  Two orderings are load-bearing:
+            //  * every commit group is retired inside the iteration that issued it: a group still in flight at the loop's
+            //    back edge or exit has no single retiring wait on all paths, and ptxas then treats every accumulator read
+            //    as a read of an in-flight register and serialises all the wgmma;
+            //  * the fold of set 0 precedes the issue of (t + 1, 0) into the same registers, and the wait for (t, 1)
+            //    follows that issue.  ptxas would otherwise hoist the wait above the fold, which no register ties to it.
+            mbar_wait(&x_full[xs], xph);
+            wg_issue_half(acc[0], xw + xs * TC_TILE_BYTES, ya);   // (0, 0)
+            wg_wait<0>();
+            wg_fence_regs(acc[0]);
+            for (int t = 0; t + 1 < nxt; ++t) {
+                const uint32_t nxs = xs + 1 == TC_XSTAGES ? 0 : xs + 1, nxph = nxs == 0 ? xph ^ 1 : xph;
+                wg_issue_half(acc[1], xw + xs * TC_TILE_BYTES, ya + TC_HALF_BYTES);   // (t, 1)
+                fold(H0, t);
+                mbar_wait(&x_full[nxs], nxph);
+                wg_issue_half(acc[0], xw + nxs * TC_TILE_BYTES, ya);   // (t + 1, 0)
+                wg_wait<1>();   // retires (t, 1)
+                wg_fence_regs(acc[1]);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&x_empty[xs]);   // both halves of tile t have read the stage
+                fold(H1, t);
+                wg_wait<0>();   // retires (t + 1, 0)
+                wg_fence_regs(acc[0]);
+                xs = nxs;
+                xph = nxph;
             }
+            // the last tile: nothing more to issue after its second half
+            wg_issue_half(acc[1], xw + xs * TC_TILE_BYTES, ya + TC_HALF_BYTES);
+            fold(H0, nxt - 1);
+            wg_wait<0>();
+            wg_fence_regs(acc[1]);
+            __syncwarp();
+            if (lane == 0) {   // the stage and the trains are free
+                mbar_arrive(&x_empty[xs]);
+                mbar_arrive(y_empty);
+            }
+            fold(H1, nxt - 1);
+            if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
 
             // ---- column direction: reduce the element-wise state over the eight lanes of a column (shuffles), then over the
             // eight consumer warps (shared memory); the tag is the warp the best came from ----
@@ -400,7 +462,7 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
 }
 
 cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, int n_a, const TcItem* items_b, int n_b,
-                              int* sched, int grid, __half* debug_tile, cudaStream_t stream) {
+                              int* sched, int grid, cudaStream_t stream) {
     const int n_items = n_a + n_b;
     if (n_items <= 0) return cudaSuccess;
     static size_t configured[64] = {};
@@ -416,7 +478,7 @@ cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, 
         fprintf(stderr, "[tc diag] regs %d, maxThreadsPerBlock %d, static smem %zu, local %zu, dynamic smem %zu, occupancy %d\n",
                 fa.numRegs, fa.maxThreadsPerBlock, fa.sharedSizeBytes, fa.localSizeBytes, smem, occ);
     }
-    tc_hamming_kernel<<<grid, TC_THREADS, smem, stream>>>(problems, items_a, n_a, items_b, n_b, sched, debug_tile);
+    tc_hamming_kernel<<<grid, TC_THREADS, smem, stream>>>(problems, items_a, n_a, items_b, n_b, sched);
     return cudaGetLastError();
 }
 

@@ -8,10 +8,10 @@ namespace plstvo {
 
 constexpr int TC_ROWS = 128;                    // descriptor rows per operand tile (two wgmma M blocks of 64; N = 2 tiles)
 constexpr int TC_TILE_BYTES = TC_ROWS * 256;    // 128 rows x 256 e4m3 bytes, swizzled K-major layout
-constexpr int TC_CW = 256;                      // trains per work item = per row-partial block (wgmma N)
+constexpr int TC_CW = 256;                      // trains per work item = per row-partial block (two wgmma N of 128)
 constexpr int TC_CWARPS = 8;                    // consumer warps: two warpgroups, 64 query rows of each tile apiece
 constexpr int TC_XSTAGES = 4;                   // query tiles in flight (shared memory ring)
-constexpr int TC_THREADS = 32 * TC_CWARPS + 32; // the consumer warpgroups + one producer warp
+constexpr int TC_THREADS = 32 * TC_CWARPS + 128; // the consumer warpgroups + one producer warpgroup (one thread of it works)
 
 // one descriptor matrix to expand (queries or trains of one matching problem)
 struct TcSide {
@@ -39,7 +39,7 @@ size_t tc_smem_bytes();
 cudaError_t launch_tc_expand(const TcSide* sides, int n_sides, int max_tiles, cudaStream_t stream);
 // items_a then items_b form the work list (long items first); sched: two zeroed ints per concurrently running launch
 cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, int n_a, const TcItem* items_b, int n_b,
-                              int* sched, int grid, __half* debug_tile, cudaStream_t stream);
+                              int* sched, int grid, cudaStream_t stream);
 // writes MatchProblem::rowpart[0][n1] / colpart[0][n2] (ntb = nqb = 1) in K1's packed-key format
 cudaError_t launch_tc_resolve(const MatchProblem* mps, const TcProblem* tps, int n_problems, int slices, cudaStream_t stream);
 
