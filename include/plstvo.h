@@ -370,6 +370,18 @@ int  plstvo_gn_eval_stream(PlContext* ctx, const PlCamera* cam, const PlConfig* 
  * |x - pivot[p]| rounded to float (mode 1: the MAD form of src/auxiliar.cpp:399-402). */
 int  plstvo_debug_select(PlContext* ctx, int n_lists, const int32_t* off, const double* values, const int32_t* k,
                          const double* pivot, int mode, double* out);
+/* test hook: the intermediate words of the tensor-core matcher for the problems of a plstvo_match_batch call (same B, d1 /
+ * off1, d2 / off2, nnr), after the same expand, distance + top-2 and resolve kernels.  Per problem p, in problem order:
+ *   rowp   [sum_p ceil(n2_p / 256) * n1_p]: the distance kernel's row words, [256-train block][n1] per problem: best distance
+ *          over the block | second distance << 9 (511 = none) | candidate tag << 18 (parity | chunk group << 1 | lane << 4);
+ *   colp   [sum_p n2_p]: column words, best | second << 9 | tag << 18 (the consumer warp, = (row % 128) / 16, of the best);
+ *   rowkey [sum_p n1_p][2], colkey [sum_p n2_p][2]: the resolved keys (dist << 16 | index, dist2 << 16 | 0xFFFE), or
+ *          0xFFFFFFFF as the second key when the other side has fewer than 2 rows.
+ * A problem with an empty side has no words; its slots are left unchanged.  Fails with PLSTVO_E_INVALID under PLSTVO_K1=popc
+ * (the integer matcher has no such words). */
+int  plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
+                              const int32_t* off2, float nnr, uint32_t* rowp, uint32_t* colp, uint32_t* rowkey,
+                              uint32_t* colkey);
 /* test hook for the on-chip 6x6 routines of the solver (ColPivHouseholderQR solve + log|det|, inverse, symmetric
  * eigenvalues) on n caller-supplied matrices: H [n][36] row-major, g [n][6] -> x [n][6], lad [n], inv [n][36], eig [n][6] */
 int  plstvo_debug_algebra(PlContext* ctx, int n, const double* H, const double* g, double* x, double* lad,

@@ -802,14 +802,11 @@ void plstvo_host_free(void* p) {
 int64_t plstvo_launch_count(const PlContext* ctx) { return ctx ? ctx->launches : 0; }
 
 // ---- matching.h surface -------------------------------------------------------------------------------
-int plstvo_match_batch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
-                       const int32_t* off2, float nnr, int best_lr_matches, int32_t* m12, int32_t* counts) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (B < 0 || (B > 0 && (!off1 || !off2 || !m12))) return fail(ctx, PLSTVO_E_INVALID, "bad arguments");
-    if (B == 0) return 0;
-    CK(ctx, cudaSetDevice(ctx->device));
-    // express the problems as a points-only frame batch
+// Plans the B problems of a plstvo_match_batch call as a points-only frame batch on ctx->ws, uploads them and enqueues K1
+// (expand, distance + top-2, resolve; or the integer form) on ctx->s_main.  The caller holds the lock, has validated B > 0
+// and selected the device; on success ws.problems[2 p] is problem p, its partial keys pending on ctx->s_main.
+static int match_batch_launch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
+                              const int32_t* off2, float nnr, int best_lr_matches) {
     std::vector<int32_t> zeros((size_t)B + 1, 0);
     PlFrameBatch a{}, b{};
     a.B = b.B = B;
@@ -825,7 +822,7 @@ int plstvo_match_batch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* 
     Workspace& ws = ctx->ws;
     rc = ws_prepare(ctx, ws, nullptr, &cfg, &a, &b, false, false);
     if (rc) return rc;
-    ws.planned = false;                          // this entry point patches the plan below: never reuse it
+    ws.planned = false;                          // the plan is patched below: never reuse it
     for (auto& pr : ws.problems) pr.nnr = nnr;   // the caller's float, not the config's double
     CK(ctx, cudaMemcpyAsync(ws.d_problems.p, ws.problems.data(), ws.problems.size() * sizeof(MatchProblem),
                             cudaMemcpyHostToDevice, ctx->s_h2d));
@@ -834,8 +831,19 @@ int plstvo_match_batch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* 
     cudaEvent_t up = next_event(ctx);
     CK(ctx, cudaEventRecord(up, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(ctx->s_main, up, 0));
-    rc = ws_launch_match(ctx, ws, 0, B, ctx->s_main);
+    return ws_launch_match(ctx, ws, 0, B, ctx->s_main);
+}
+
+int plstvo_match_batch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
+                       const int32_t* off2, float nnr, int best_lr_matches, int32_t* m12, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (B < 0 || (B > 0 && (!off1 || !off2 || !m12))) return fail(ctx, PLSTVO_E_INVALID, "bad arguments");
+    if (B == 0) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    int rc = match_batch_launch(ctx, B, d1, off1, d2, off2, nnr, best_lr_matches);
     if (rc) return rc;
+    Workspace& ws = ctx->ws;
     // finalize only the point problems (even indices): compact view
     CK(ctx, ctx->scratch.ensure((size_t)B * (sizeof(MatchProblem) + 4)));
     std::vector<MatchProblem> pts((size_t)B);
@@ -872,6 +880,40 @@ int plstvo_match(PlContext* ctx, const uint8_t* d1, int n1, const uint8_t* d2, i
 int plstvo_match_nnr(PlContext* ctx, const uint8_t* d1, int n1, const uint8_t* d2, int n2, int stride_bytes,
                      float nnr, int32_t* m12) {
     return plstvo_match(ctx, d1, n1, d2, n2, stride_bytes, nnr, 0, m12);
+}
+
+int plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
+                             const int32_t* off2, float nnr, uint32_t* rowp, uint32_t* colp, uint32_t* rowkey,
+                             uint32_t* colkey) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (B < 0 || (B > 0 && (!off1 || !off2 || !rowp || !colp || !rowkey || !colkey)))
+        return fail(ctx, PLSTVO_E_INVALID, "bad arguments");
+    if (!k1_use_tc())
+        return fail(ctx, PLSTVO_E_INVALID, "PLSTVO_K1=popc selects the integer matcher, which has no tensor-core partial words");
+    if (B == 0) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    int rc = match_batch_launch(ctx, B, d1, off1, d2, off2, nnr, 1);
+    if (rc) return rc;
+    const Workspace& ws = ctx->ws;
+    cudaStream_t s = ctx->s_main;
+    size_t row0 = 0;   // first row word of problem p in the caller's rowp
+    for (int p = 0; p < B; ++p) {
+        const MatchProblem& pr = ws.problems[(size_t)2 * p];
+        const TcProblem& tp = ws.tc_problems[(size_t)2 * p];
+        const size_t nrow = (size_t)((pr.n2 + TC_CW - 1) / TC_CW) * pr.n1;
+        if (pr.enabled) {   // a problem with an empty side has no words: its slots are left as they are
+            CK(ctx, cudaMemcpyAsync(rowp + row0, tp.rowp, nrow * 4, cudaMemcpyDeviceToHost, s));
+            CK(ctx, cudaMemcpyAsync(colp + off2[p], tp.colp, (size_t)pr.n2 * 4, cudaMemcpyDeviceToHost, s));
+            CK(ctx, cudaMemcpyAsync(rowkey + 2 * (size_t)off1[p], pr.rowpart, (size_t)pr.n1 * sizeof(uint2),
+                                    cudaMemcpyDeviceToHost, s));
+            CK(ctx, cudaMemcpyAsync(colkey + 2 * (size_t)off2[p], pr.colpart, (size_t)pr.n2 * sizeof(uint2),
+                                    cudaMemcpyDeviceToHost, s));
+        }
+        row0 += nrow;
+    }
+    CK(ctx, cudaStreamSynchronize(s));
+    return 0;
 }
 
 // ---- matchGrid (stereo step) -------------------------------------------------------------------------------------

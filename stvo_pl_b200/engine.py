@@ -30,6 +30,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                            "(there is no CPU fallback).")
     L = C.CDLL(path)
     vp, i32p, u8p, dp, fp = C.c_void_p, T.c_int32_p, T.c_uint8_p, T.c_double_p, T.c_float_p
+    u32p = C.POINTER(C.c_uint32)
     cam, cfg = C.POINTER(T.PlCamera), C.POINTER(T.PlConfig)
     fb, mb = C.POINTER(T.PlFrameBatch), C.POINTER(T.PlMatchedBatch)
     sig = {
@@ -85,6 +86,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_popc_rate": (C.c_int, [vp, dp]),
         "plstvo_debug_algebra": (C.c_int, [vp, C.c_int, dp, dp, dp, dp, dp, dp]),
         "plstvo_debug_select": (C.c_int, [vp, C.c_int, i32p, dp, i32p, dp, C.c_int, dp]),
+        "plstvo_debug_tc_partials": (C.c_int, [vp, C.c_int, u8p, i32p, u8p, i32p, C.c_float, u32p, u32p, u32p, u32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -102,7 +104,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_optimize_pose", "plstvo_track_batch", "plstvo_track_batch_async", "plstvo_wait", "plstvo_batch_upload", "plstvo_batch_run",
     "plstvo_batch_run_timed", "plstvo_batch_download", "plstvo_batch_free", "plstvo_synchronize",
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
-    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select"]
+    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -526,6 +528,22 @@ class Engine:
                                               _p(pv, T.c_double_p) if pv is not None else None, 0 if pv is None else 1,
                                               _p(out, T.c_double_p)))
         return out
+
+    def debug_tc_partials(self, d1, off1, d2, off2, nnr):
+        """Tensor-core matcher's intermediate words (test hook) for a match_batch problem set: rowp (per problem
+        [ceil(n2 / 256)][n1], flattened), colp [sum n2], rowkey [sum n1, 2], colkey [sum n2, 2], all uint32."""
+        d1, d2 = np.ascontiguousarray(d1, np.uint8).reshape(-1, 32), np.ascontiguousarray(d2, np.uint8).reshape(-1, 32)
+        off1, off2 = np.ascontiguousarray(off1, np.int32), np.ascontiguousarray(off2, np.int32)
+        B = len(off1) - 1
+        n1, n2 = np.diff(off1).astype(np.int64), np.diff(off2).astype(np.int64)
+        u32p = C.POINTER(C.c_uint32)
+        rowp = np.zeros(int(((n2 + 255) // 256 * n1).sum()), np.uint32)
+        colp = np.zeros(len(d2), np.uint32)
+        rowkey, colkey = np.zeros((len(d1), 2), np.uint32), np.zeros((len(d2), 2), np.uint32)
+        self._ck(self.lib.plstvo_debug_tc_partials(self.ctx, B, _p(d1, T.c_uint8_p), _p(off1, T.c_int32_p), _p(d2, T.c_uint8_p),
+                                                   _p(off2, T.c_int32_p), C.c_float(nnr), _p(rowp, u32p), _p(colp, u32p),
+                                                   _p(rowkey, u32p), _p(colkey, u32p)))
+        return rowp, colp, rowkey, colkey
 
     def debug_algebra(self, H, g):
         """On-chip 6x6 routines (test hook): returns x = H^-1 g (col-pivot QR), log|det H|, inv(H), eigvals(H)."""

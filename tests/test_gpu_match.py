@@ -6,6 +6,7 @@ import os
 import numpy as np
 import pytest
 
+import ref_match
 from conftest import GOLDEN
 from stvo_pl_b200 import synth, types as T
 
@@ -43,7 +44,7 @@ def test_match_vs_oracle(engine, oracle, n1, n2, mode):
     else:
         prev, curr, _, _ = synth.make_batch("kitti", 1, n_pt=max(n1, n2), n_ls=0)
         d1, d2 = prev.pdesc[:n1], curr.pdesc[:n2]
-    for nnr in (0.75, 0.9):
+    for nnr in (0.75, 0.9, 1.0, 1.5):   # nnr > 1 accepts ties d1 == d2: the lowest index must win
         for best_lr in (True, False):
             n_ref, ref = oracle.match(d1, d2, nnr, best_lr)
             n, m = engine.match(d1, d2, nnr, best_lr)
@@ -83,6 +84,78 @@ def test_match_batch_ragged(engine, oracle):
         np.testing.assert_array_equal(m12[off1[p]:off1[p + 1]], ref)
         assert counts[p] == n_ref
     assert total == counts.sum() and counts[-1] > 1000
+
+
+def _tie_rows(rng, n, patterns, flip):
+    """n rows drawn from a few byte patterns; flip: each with 1 or 2 bits flipped, so that its best is tied among the
+    pattern's copies at a distance above 0, where a ratio test with nnr > 1 accepts it"""
+    rows = patterns[rng.integers(0, len(patterns), n)]
+    return ref_match.flip_bits(rng, rows, 2) if flip else rows
+
+
+def test_match_batch_accepted_ties(engine, oracle):
+    """nnr 1.5, queries near a few byte patterns and trains copies of them: most rows and columns have tied bests that pass
+    the ratio test, so the resolve step's lowest-index scan feeds the mutual filter's index form."""
+    rng = np.random.default_rng(23)
+    pats = (rng.integers(0, 2, (6, 32), dtype=np.uint8) * 255).astype(np.uint8)
+    sizes = [(300, 280), (1, 7), (257, 513), (640, 129), (2, 2)]
+    d1 = _tie_rows(rng, sum(s[0] for s in sizes), pats, True)
+    d2 = _tie_rows(rng, sum(s[1] for s in sizes), pats, False)
+    off1 = np.concatenate([[0], np.cumsum([s[0] for s in sizes])]).astype(np.int32)
+    off2 = np.concatenate([[0], np.cumsum([s[1] for s in sizes])]).astype(np.int32)
+    for best_lr in (True, False):
+        total, m12, counts = engine.match_batch(d1, off1, d2, off2, 1.5, best_lr)
+        for p in range(len(sizes)):
+            n_ref, ref = oracle.match(d1[off1[p]:off1[p + 1]], d2[off2[p]:off2[p + 1]], 1.5, best_lr)
+            np.testing.assert_array_equal(m12[off1[p]:off1[p + 1]], ref)
+            assert counts[p] == n_ref
+        assert total == counts.sum() and total > 0
+
+
+def test_track_batch_accepted_ties(engine, oracle):
+    """The same accepted ties through the per-pair solver's own finalize (K2): match indices equal the oracle's."""
+    rng = np.random.default_rng(31)
+    prev, curr, _, cam = synth.make_batch("kitti", 2, n_pt=600, n_ls=150)
+    pats = (rng.integers(0, 2, (6, 32), dtype=np.uint8) * 255).astype(np.uint8)
+    for f in (prev, curr):
+        f.pdesc = np.ascontiguousarray(_tie_rows(rng, len(f.pdesc), pats, f is prev))
+        f.ldesc = np.ascontiguousarray(_tie_rows(rng, len(f.ldesc), pats, f is prev))
+    cfg = T.kitti_config()
+    cfg.min_ratio_12_p = cfg.min_ratio_12_l = 1.5
+    gpu = engine.track_batch(cam, cfg, prev, curr)
+    ref = oracle.track_batch(cam, cfg, prev, curr)
+    np.testing.assert_array_equal(gpu["m12_pt"], ref["m12_pt"])
+    np.testing.assert_array_equal(gpu["m12_ls"], ref["m12_ls"])
+    assert (gpu["m12_pt"] >= 0).sum() > 0
+
+
+def test_selected_matcher_form(engine):
+    """PLSTVO_K1=popc selects the integer matcher (and PLSTVO_K1_VARIANT its queries per thread); anything else the tensor-core
+    form.  Asserted on the plan a resident batch reports, so that a run under either switch proves which matcher it tested."""
+    from stvo_pl_b200.engine import PlstvoError
+    popc = os.environ.get("PLSTVO_K1") == "popc"
+    prev, curr, _, cam = synth.make_batch("kitti", 2, n_pt=600, n_ls=150)
+    cfg = T.kitti_config()
+    db = engine.upload(cam, cfg, prev, curr)
+    try:
+        st = db.stage_times(iters=1)
+    finally:
+        db.free()
+    assert st["tensor_core_form"] is (not popc)
+    n1 = np.concatenate([np.diff(prev.pt_off), np.diff(prev.ls_off)])
+    n2 = np.concatenate([np.diff(curr.pt_off), np.diff(curr.ls_off)])
+    if popc:
+        # integer form: one tile per (query block, train block); a batch this small is split into train blocks of 256
+        qpt = 256 * (4 if os.environ.get("PLSTVO_K1_VARIANT", "")[:1] == "4" else 2)
+        assert st["n_items"] == int(((n1 + qpt - 1) // qpt * ((n2 + 255) // 256)).sum())
+        d = np.zeros((4, 32), np.uint8)
+        with pytest.raises(PlstvoError) as ei:
+            engine.debug_tc_partials(d, [0, 4], d, [0, 4], 0.9)
+        assert ei.value.code == -1
+    else:
+        assert st["n_items"] == int(((n2 + 255) // 256).sum())   # work items: 256-train blocks
+        rowp, colp, rowkey, colkey = engine.debug_tc_partials(prev.pdesc[:5], [0, 5], curr.pdesc[:3], [0, 3], 0.9)
+        assert len(rowp) == 5 and len(colp) == 3 and rowkey.shape == (5, 2) and colkey.shape == (3, 2)
 
 
 def test_match_full_size_properties(engine):
