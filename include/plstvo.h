@@ -287,6 +287,34 @@ int plstvo_track_stereo_sequence_async(PlContext* ctx, const PlCamera* cam, cons
                                        const PlStereoConfig* scfg, const PlStereoFeatures* frames, const PlPrior* priors,
                                        PlPoseResult* results, int32_t* n_stereo);
 
+/* ---- ORB description: what cv::ORB does after key-point selection (the pdesc_l / pdesc_r above) ---- */
+typedef struct PlOrbConfig {       /* cv::ORB parameters; src/config.cpp:95-102 defaults */
+    int32_t n_levels;              /* pyramid levels (1..32) */
+    double  scale_factor;          /* level l is cvRound(W / s^l) x cvRound(H / s^l) */
+    int32_t edge_threshold;        /* key points with cvRound(pt) closer than this to the border are dropped */
+    int32_t patch_size;            /* 31 only */
+    int32_t wta_k;                 /* 2 only */
+} PlOrbConfig;
+void plstvo_default_orb_config(PlOrbConfig* c);   /* 4 levels, 1.2, 19, 31, 2 */
+/* Angles and 256-bit rBRIEF descriptors of given key points on n_img grey images of one size (images: [n_img][height][width]
+ * uint8, row-major), bit-identical to OpenCV 4.13's ORB.  Image i's key points are rows kp_off[i] .. kp_off[i + 1] of
+ * kp_xy ([n][2] float x, y in image coordinates, cv::KeyPoint::pt), kp_octave ([n]) and kp_angle ([n] degrees).
+ *   kp_angle == NULL: the angle is computed (intensity centroid at cvRound(pt / scale^octave) on the octave's level), as
+ *                     detectAndCompute does for its own key points;
+ *   kp_angle != NULL: the angles are used as given, as ORB::compute does.
+ * Key points with cvRound(pt) closer than edge_threshold to the image border are dropped (KeyPointsFilter::runByImageBorder);
+ * image i's survivors, in input order, are rows kp_off[i] .. kp_off[i] + counts[i] of out_angle ([n]), out_desc ([n][32],
+ * the layout PlStereoFeatures::pdesc_l / pdesc_r take) and src_idx ([n], index within the image's key points); later rows are
+ * left unchanged.  Returns the number of survivors.  PLSTVO_E_INVALID: patch_size != 31, wta_k != 2, n_levels outside
+ * 1..32, scale_factor <= 1 with more than one level, a level of zero size, or an octave outside [0, n_levels);
+ * PLSTVO_E_TOO_LARGE: more than PLSTVO_MAX_FEATURES key points in one image. */
+int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                             const int32_t* kp_off, const float* kp_xy, const int32_t* kp_octave, const float* kp_angle,
+                             float* out_angle, uint8_t* out_desc, int32_t* src_idx, int32_t* counts);
+/* Device time of the last plstvo_orb_compute_batch on this context, ms: [0] pyramid and blur, [1] border filter,
+ * [2] angles and descriptors. */
+int plstvo_orb_kernel_times(PlContext* ctx, float* ms3);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

@@ -108,6 +108,30 @@ inline int matchStereoPoints(Context& c, const PlCamera& cam, const PlStereoMatc
     if (disp) disp->assign(d.begin(), d.begin() + k);
     return k;
 }
+// ORB description after key-point selection (cv::ORB::compute; angle == nullptr: detectAndCompute's computed angles) for one
+// grey image (row-major, width * height bytes).  kp.pt / kp.octave are read; kp is replaced by the survivors of the border
+// filter, in input order, with their 32-byte descriptors, and angle (if given) likewise; returns the survivor count.
+inline int computeORB(Context& c, const PlOrbConfig& cfg, const uint8_t* image, int width, int height, KeyPoints& kp,
+                      std::vector<float>* angle = nullptr) {
+    const int n = (int)(kp.pt.size() / 2);
+    const int32_t off[2] = {0, n};
+    std::vector<float> ang_out((size_t)n);
+    std::vector<uint8_t> desc(32 * (size_t)n);
+    std::vector<int32_t> src((size_t)n);
+    const float* ang_in = (angle && (int)angle->size() == n) ? angle->data() : nullptr;
+    const int k = c.check(plstvo_orb_compute_batch(c.get(), &cfg, 1, width, height, image, off, kp.pt.data(), kp.octave.data(),
+                                                   ang_in, ang_out.data(), desc.data(), src.data(), nullptr));
+    KeyPoints out;
+    for (int i = 0; i < k; ++i) {
+        out.pt.push_back(kp.pt[2 * (size_t)src[i]]);
+        out.pt.push_back(kp.pt[2 * (size_t)src[i] + 1]);
+        out.octave.push_back(kp.octave[src[i]]);
+    }
+    out.desc.assign(desc.begin(), desc.begin() + 32 * (size_t)k);
+    kp = std::move(out);
+    if (angle) angle->assign(ang_out.begin(), ang_out.begin() + k);
+    return k;
+}
 inline int matchStereoLines(Context& c, const PlCamera& cam, const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
                             const KeyLines& l, const KeyLines& r, StereoFrame& out) {
     const int n = l.size();

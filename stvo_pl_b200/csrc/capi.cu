@@ -106,6 +106,9 @@ struct PlContext {
     DevBuf arena_grid, arena_lift_pt, arena_lift_ls, arena_stereo;
     DevBuf arena_track_stereo[3];   // [0]: blocking calls, [1 + slot]: plstvo_track_stereo_*_async
     DevBuf gs_in[13], gs_rec_pt, gs_rec_ls;   // resident inputs / packed records of the streamed evaluator
+    DevBuf arena_orb;      // plstvo_orb_compute_batch: images, level buffers, key points, outputs
+    bool orb_tables = false;
+    cudaEvent_t orb_ev[4] = {nullptr, nullptr, nullptr, nullptr};
     // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
     void* h_staging[3] = {nullptr, nullptr, nullptr};
     size_t h_staging_bytes[3] = {0, 0, 0};
@@ -753,6 +756,9 @@ void plstvo_destroy(PlContext* ctx) {
     for (auto& b : ctx->arena_track_stereo) b.release();
     for (auto& b : ctx->gs_in) b.release();
     ctx->gs_rec_pt.release(); ctx->gs_rec_ls.release();
+    ctx->arena_orb.release();
+    for (cudaEvent_t e : ctx->orb_ev)
+        if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->events) cudaEventDestroy(e);
     for (void* h : ctx->h_staging)
         if (h) cudaFreeHost(h);
@@ -2155,6 +2161,158 @@ int plstvo_gn_eval_stream(PlContext* ctx, const PlCamera* cam, const PlConfig* c
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
     if (ms_total) *ms_total = ms;
+    return 0;
+}
+
+
+/* ---- ORB description (orb.cu) ---- */
+void plstvo_default_orb_config(PlOrbConfig* c) {
+    if (!c) return;
+    c->n_levels = 4; c->scale_factor = 1.2; c->edge_threshold = 19; c->patch_size = 31; c->wta_k = 2;
+}
+
+namespace {
+// INTER_LINEAR_EXACT taps of one axis (cv::resize's bit-exact linear interpolation): [0, dst) source offsets, then
+// [dst, 2 dst) the 8-bit weight of the second tap; 0 where the source position is left or right of the source (edge pixel)
+void orb_linear_exact_table(int src, int dst, int32_t* t) {
+    const double scale = 1.0 / ((double)dst / (double)src);
+    for (int d = 0; d < dst; ++d) {
+        const double f = scale * ((double)d + 0.5) - 0.5;
+        const int i = (int)floor(f);
+        if (i >= 0 && src > 1 && i < src - 1) {
+            t[d] = i;
+            t[dst + d] = (int32_t)lrint((f - (double)i) * 256.0);
+        } else {
+            t[d] = (i >= 0 && src > 1) ? src - 1 : 0;
+            t[dst + d] = 0;
+        }
+    }
+}
+}  // namespace
+
+int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                             const int32_t* kp_off, const float* kp_xy, const int32_t* kp_octave, const float* kp_angle,
+                             float* out_angle, uint8_t* out_desc, int32_t* src_idx, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0) return fail(ctx, PLSTVO_E_INVALID, "null config or negative size");
+    if (cfg->patch_size != 31) return fail(ctx, PLSTVO_E_INVALID, "patch_size must be 31");
+    if (cfg->wta_k != 2) return fail(ctx, PLSTVO_E_INVALID, "wta_k must be 2");
+    if (cfg->n_levels < 1 || cfg->n_levels > ORB_MAX_LEVELS) return fail(ctx, PLSTVO_E_INVALID, "n_levels must be 1..32");
+    if (cfg->edge_threshold < 0) return fail(ctx, PLSTVO_E_INVALID, "negative edge_threshold");
+    if (cfg->n_levels > 1 && !(cfg->scale_factor > 1.0 && cfg->scale_factor < 1e6))
+        return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1");
+    if (n_img == 0) return 0;
+    if (!images || !kp_off || kp_off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null images / offsets or kp_off[0] != 0");
+    for (int i = 0; i < n_img; ++i) {
+        const int n = kp_off[i + 1] - kp_off[i];
+        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kp_off is not non-decreasing");
+        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
+    }
+    const size_t N = (size_t)kp_off[n_img];
+    if (N && (!kp_xy || !kp_octave || !out_angle || !out_desc || !src_idx))
+        return fail(ctx, PLSTVO_E_INVALID, "null key point or output array");
+    for (size_t k = 0; k < N; ++k)
+        if (kp_octave[k] < 0 || kp_octave[k] >= cfg->n_levels) return fail(ctx, PLSTVO_E_INVALID, "octave outside [0, n_levels)");
+    OrbDevLevels L{};
+    L.n = cfg->n_levels;
+    for (int l = 0; l < L.n; ++l) {
+        const float scale = (float)pow(cfg->scale_factor, (double)l);
+        L.inv[l] = 1.f / scale;
+        L.w[l] = (int)lrintf((float)width * L.inv[l]);
+        L.h[l] = (int)lrintf((float)height * L.inv[l]);
+        if (L.w[l] < 1 || L.h[l] < 1) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+        L.raw_off[l] = l ? L.raw_stride : 0;
+        if (l) L.raw_stride += (size_t)L.w[l] * L.h[l];
+        L.blur_off[l] = L.blur_stride;
+        L.blur_stride += (size_t)L.w[l] * L.h[l];
+    }
+    {   // getGaussianKernel(7, 2, CV_32F)
+        double e[7], sum = 0;
+        for (int i = 0; i < 7; ++i) {
+            e[i] = exp(-((double)(i - 3) * (i - 3)) / (2.0 * 2.0 * 2.0));
+            sum += e[i];
+        }
+        for (int i = 0; i < 7; ++i) L.taps[i] = (float)(e[i] * (1.0 / sum));
+    }
+    std::vector<int32_t> tabs;
+    std::vector<size_t> tab_off(2 * (size_t)L.n, 0);
+    for (int l = 1; l < L.n; ++l) {
+        tab_off[2 * l] = tabs.size();
+        tabs.resize(tabs.size() + 2 * (size_t)L.w[l]);
+        orb_linear_exact_table(L.w[l - 1], L.w[l], tabs.data() + tab_off[2 * l]);
+        tab_off[2 * l + 1] = tabs.size();
+        tabs.resize(tabs.size() + 2 * (size_t)L.h[l]);
+        orb_linear_exact_table(L.h[l - 1], L.h[l], tabs.data() + tab_off[2 * l + 1]);
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->orb_tables) {
+        CK(ctx, orb_upload_tables());
+        for (auto& e : ctx->orb_ev) CK(ctx, cudaEventCreate(&e));
+        ctx->orb_tables = true;
+    }
+    const size_t img_bytes = (size_t)n_img * width * height;
+    LiftArena a;
+    const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
+    const size_t o_blur = a.take((size_t)n_img * L.blur_stride), o_tab = a.take(tabs.size() * 4 + 4);
+    const size_t o_off = a.take((size_t)(n_img + 1) * 4), o_xy = a.take(N * 8), o_oct = a.take(N * 4), o_ang = a.take(N * 4);
+    const size_t o_oang = a.take(N * 4), o_desc = a.take(N * 32), o_src = a.take(N * 4), o_cnt = a.take((size_t)n_img * 4);
+    DevBuf& arena = ctx->arena_orb;
+    CK(ctx, arena.ensure(a.off));
+    uint8_t* base = arena.as<uint8_t>();
+    cudaStream_t s = ctx->s_main;
+    auto up = [&](size_t o, const void* src, size_t bytes) -> cudaError_t {
+        return (src && bytes) ? cudaMemcpyAsync(base + o, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+    };
+    auto down = [&](void* dst, size_t o, size_t bytes) -> cudaError_t {
+        return (dst && bytes) ? cudaMemcpyAsync(dst, base + o, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    };
+    auto I = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
+    auto F = [&](size_t o) { return reinterpret_cast<float*>(base + o); };
+    CK(ctx, up(o_img, images, img_bytes));
+    CK(ctx, up(o_tab, tabs.data(), tabs.size() * 4));
+    CK(ctx, up(o_off, kp_off, (size_t)(n_img + 1) * 4));
+    CK(ctx, up(o_xy, kp_xy, N * 8));
+    CK(ctx, up(o_oct, kp_octave, N * 4));
+    CK(ctx, up(o_ang, kp_angle, N * 4));
+    std::vector<const int32_t*> rs_tab(2 * (size_t)L.n, nullptr);
+    for (int l = 1; l < L.n; ++l) {
+        rs_tab[2 * l] = I(o_tab) + tab_off[2 * l];
+        rs_tab[2 * l + 1] = I(o_tab) + tab_off[2 * l + 1];
+    }
+    int launches = 0;
+    CK(ctx, launch_orb(L, n_img, width, height, cfg->edge_threshold, base + o_img, base + o_raw, base + o_blur, rs_tab.data(),
+                       I(o_off), (int)N, F(o_xy), I(o_oct), kp_angle ? F(o_ang) : nullptr, I(o_src), I(o_cnt), F(o_oang),
+                       base + o_desc, s, ctx->orb_ev, &launches));
+    ctx->launches += launches;
+    std::vector<int32_t> cnt((size_t)n_img), src_dev(N);
+    CK(ctx, down(cnt.data(), o_cnt, (size_t)n_img * 4));
+    CK(ctx, down(src_dev.data(), o_src, N * 4));
+    std::vector<float> ang_dev(N);
+    std::vector<uint8_t> desc_dev(N * 32);
+    CK(ctx, down(ang_dev.data(), o_oang, N * 4));
+    CK(ctx, down(desc_dev.data(), o_desc, N * 32));
+    CK(ctx, cudaStreamSynchronize(s));
+    long total = 0;
+    for (int i = 0; i < n_img; ++i) {   // survivors only: rows past counts[i] stay as the caller left them
+        const size_t r0 = (size_t)kp_off[i], n = (size_t)cnt[i];
+        if (n) {
+            memcpy(out_angle + r0, ang_dev.data() + r0, n * 4);
+            memcpy(out_desc + 32 * r0, desc_dev.data() + 32 * r0, n * 32);
+            memcpy(src_idx + r0, src_dev.data() + r0, n * 4);
+        }
+        if (counts) counts[i] = cnt[i];
+        total += cnt[i];
+    }
+    return (int)total;
+}
+
+int plstvo_orb_kernel_times(PlContext* ctx, float* ms3) {
+    if (!ctx || !ms3) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->orb_tables) return fail(ctx, PLSTVO_E_INVALID, "no ORB call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 3; ++k) CK(ctx, cudaEventElapsedTime(&ms3[k], ctx->orb_ev[k], ctx->orb_ev[k + 1]));
     return 0;
 }
 

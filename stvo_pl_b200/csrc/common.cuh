@@ -197,6 +197,23 @@ cudaError_t launch_lift_lines(const PlCamera& cam, const PlStereoConfig& sc, int
                               double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts,
                               cudaStream_t s, const int32_t* out_off = nullptr);
 
+// orb.cu: ORB description (pyramid, blur, border filter, angle, rBRIEF) of a batch of images of one size
+constexpr int ORB_MAX_LEVELS = 32;
+struct OrbDevLevels {
+    int n;                                   // levels
+    int w[ORB_MAX_LEVELS], h[ORB_MAX_LEVELS];
+    size_t raw_off[ORB_MAX_LEVELS];          // levels >= 1 in the resized-level buffer (level 0 is the input image)
+    size_t blur_off[ORB_MAX_LEVELS];         // every level in the blurred-level buffer
+    size_t raw_stride, blur_stride;          // bytes per image in either buffer
+    float inv[ORB_MAX_LEVELS];               // 1.f / (float)pow(scale, l)
+    float taps[7];                           // getGaussianKernel(7, 2, CV_32F)
+};
+cudaError_t orb_upload_tables();             // pattern and disc tables into the current device's constant memory
+cudaError_t launch_orb(const OrbDevLevels& L, int n_img, int W, int H, int edge, const uint8_t* images, uint8_t* raw_pyr,
+                       uint8_t* blur_pyr, const int32_t* const* rs_tab, const int32_t* kp_off, int n_rows, const float* kp_xy,
+                       const int32_t* kp_oct, const float* kp_angle, int32_t* src_idx, int32_t* counts, float* out_angle,
+                       uint8_t* out_desc, cudaStream_t s, cudaEvent_t* ev, int* launches);
+
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);
 int gn_stream_partials_per_slice();   // fp64 partial records one slice writes (one per consumer warp)   // 16 KB tiles of one problem (512 points or 256 lines each)

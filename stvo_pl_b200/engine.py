@@ -87,6 +87,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_debug_algebra": (C.c_int, [vp, C.c_int, dp, dp, dp, dp, dp, dp]),
         "plstvo_debug_select": (C.c_int, [vp, C.c_int, i32p, dp, i32p, dp, C.c_int, dp]),
         "plstvo_debug_tc_partials": (C.c_int, [vp, C.c_int, u8p, i32p, u8p, i32p, C.c_float, u32p, u32p, u32p, u32p]),
+        "plstvo_default_orb_config": (None, [C.POINTER(T.PlOrbConfig)]),
+        "plstvo_orb_compute_batch": (C.c_int, [vp, C.POINTER(T.PlOrbConfig), C.c_int, C.c_int, C.c_int, u8p, i32p, fp, i32p, fp,
+                                               fp, u8p, i32p, i32p]),
+        "plstvo_orb_kernel_times": (C.c_int, [vp, fp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -104,7 +108,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_optimize_pose", "plstvo_track_batch", "plstvo_track_batch_async", "plstvo_wait", "plstvo_batch_upload", "plstvo_batch_run",
     "plstvo_batch_run_timed", "plstvo_batch_download", "plstvo_batch_free", "plstvo_synchronize",
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
-    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials"]
+    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
+    "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -321,6 +326,32 @@ class Engine:
             _p(out["sigma2"], T.c_double_p), _p(out["level"], T.c_int32_p), _p(out["desc"], T.c_uint8_p),
             _p(out["src_idx"], T.c_int32_p), _p(out["counts"], T.c_int32_p)))
         return total, out
+
+    def orb_compute_batch(self, cfg: T.PlOrbConfig, images, kp_off, kp_xy, kp_octave, kp_angle=None):
+        """ORB angles and descriptors of given key points on images uint8[n, H, W] (OpenCV's ORB after key-point selection;
+        kp_angle None: angles computed, as detectAndCompute does; else used as given, as ORB::compute does).  Image i's
+        survivors of the border filter are rows kp_off[i] .. kp_off[i] + counts[i] of every output, in input order; later rows
+        keep their initial value (angle 0, desc 0, src_idx -1)."""
+        images = np.ascontiguousarray(images, np.uint8)
+        n_img, H, W = images.shape
+        kp_off = np.ascontiguousarray(kp_off, np.int32)
+        kp_xy = np.ascontiguousarray(kp_xy, np.float32).reshape(-1, 2)
+        kp_octave = np.ascontiguousarray(kp_octave, np.int32)
+        kp_angle = None if kp_angle is None else np.ascontiguousarray(kp_angle, np.float32)
+        n = len(kp_xy)
+        out = dict(angle=np.zeros(n, np.float32), desc=np.zeros((n, 32), np.uint8), src_idx=np.full(n, -1, np.int32),
+                   counts=np.zeros(n_img, np.int32))
+        total = self._ck(self.lib.plstvo_orb_compute_batch(
+            self.ctx, C.byref(cfg), n_img, W, H, _p(images, T.c_uint8_p), _p(kp_off, T.c_int32_p), _p(kp_xy, T.c_float_p),
+            _p(kp_octave, T.c_int32_p), _p(kp_angle, T.c_float_p), _p(out["angle"], T.c_float_p), _p(out["desc"], T.c_uint8_p),
+            _p(out["src_idx"], T.c_int32_p), _p(out["counts"], T.c_int32_p)))
+        return total, out
+
+    def orb_kernel_times(self):
+        """Device ms of the last orb_compute_batch: pyramid + blur, border filter, angles + descriptors."""
+        ms = np.zeros(3, np.float32)
+        self._ck(self.lib.plstvo_orb_kernel_times(self.ctx, _p(ms, T.c_float_p)))
+        return ms
 
     def stereo_lift_lines(self, cam, scfg: T.PlStereoConfig, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, m12):
         """Stereo matches -> LineFeature records (src/stereoFrame.cpp:348-397), batched over frames."""

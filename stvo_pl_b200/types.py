@@ -68,6 +68,16 @@ def default_stereo_config() -> "PlStereoConfig":
     return PlStereoConfig(1.0, 1.0, 0.7, 0.1, 0.75, 1.2, 1.2)   # src/config.cpp:58-69, :96, :106
 
 
+class PlOrbConfig(C.Structure):
+    """cv::ORB parameters of plstvo_orb_compute_batch (src/config.cpp:95-102); patch_size 31 and wta_k 2 only."""
+    _fields_ = [("n_levels", C.c_int32), ("scale_factor", C.c_double), ("edge_threshold", C.c_int32),
+                ("patch_size", C.c_int32), ("wta_k", C.c_int32)]
+
+
+def default_orb_config(n_levels: int = 4, scale_factor: float = 1.2) -> "PlOrbConfig":
+    return PlOrbConfig(n_levels, scale_factor, 19, 31, 2)   # config_kitti.yaml: 1 level
+
+
 class PlStereoMatchConfig(C.Structure):
     """Grid / matcher values of matchStereoPoints / matchStereoLines (include/stereoFrame.h:51-52, src/config.cpp:51, :60, :63, :91)."""
     _fields_ = [("grid_rows", C.c_int32), ("grid_cols", C.c_int32), ("matching_s_ws", C.c_int32), ("best_lr_matches", C.c_int32),
