@@ -379,8 +379,8 @@ int64_t plstvo_launch_count(const PlContext* ctx);
  * launch.  n_tiles / n_pairs (optional) = CTAs per launch. */
 int     plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, double* ms_match,
                                   double* ms_solve, int32_t* n_tiles, int32_t* n_pairs);
-/* The same per stage: ms[0] = operand expansion, ms[1] = distance + top-2 kernel (tensor-core form) or the integer K1
- * (PLSTVO_K1=popc: ms[0] = ms[2] = 0), ms[2] = index resolution, ms[3] = building matched_pt / matched_ls when that is a
+/* The same per stage: ms[0] = the interval before the matcher (operands are expanded inside it: about 0), ms[1] = operand
+ * expansion + distance + top-2 kernel (tensor-core form) or the integer K1 (PLSTVO_K1=popc: ms[0] = ms[2] = 0), ms[2] = index resolution, ms[3] = building matched_pt / matched_ls when that is a
  * kernel of its own (the streamed solver; 0 when K2 does it internally), ms[4] = optimizePose (K2, or the streamed solver's
  * GN-loop / outlier / finalize kernels + K2 for the problems it hands back); of ms[4], streamed solver only (0 for K2):
  * ms[5] = the GN loop launch of stage 1, ms[6] = the gate + removeOutliers launch, ms[7] = the GN loop launch of stage 2.
@@ -399,7 +399,7 @@ int  plstvo_gn_eval_stream(PlContext* ctx, const PlCamera* cam, const PlConfig* 
 int  plstvo_debug_select(PlContext* ctx, int n_lists, const int32_t* off, const double* values, const int32_t* k,
                          const double* pivot, int mode, double* out);
 /* test hook: the intermediate words of the tensor-core matcher for the problems of a plstvo_match_batch call (same B, d1 /
- * off1, d2 / off2, nnr), after the same expand, distance + top-2 and resolve kernels.  Per problem p, in problem order:
+ * off1, d2 / off2, nnr), after the same distance + top-2 and resolve kernels.  Per problem p, in problem order:
  *   rowp   [sum_p ceil(n2_p / 256) * n1_p]: the distance kernel's row words, [256-train block][n1] per problem: best distance
  *          over the block | second distance << 9 (511 = none) | candidate tag << 18 (parity | chunk group << 1 | lane << 4);
  *   colp   [sum_p n2_p]: column words, best | second << 9 | tag << 18 (the consumer warp, = (row % 128) / 16, of the best);

@@ -62,14 +62,12 @@ struct Workspace {
     DevBuf d_priors, d_results, d_m12p, d_m12l, d_inlp, d_inll;
     DevBuf d_rowpart, d_colpart, d_problems, d_tiles, d_feat;
     DevBuf d_phase;   // debug phase timers (PLSTVO_PHASE_DEBUG)
-    // tensor-core form of K1 (match_tc.cu): expanded operands, per-block value partials, work items
+    // tensor-core form of K1 (match_tc.cu): per-block value partials, work items
     bool use_tc = true;
     std::vector<TcProblem> tc_problems;   // [2B], parallel to `problems`
-    std::vector<TcSide> tc_sides;         // [4B]: queries, trains of every problem
     std::vector<TcItem> tc_items[2];      // work items of the point problems (long) and of the line problems (short)
     std::vector<int32_t> item_start[2];   // [B+1] first work item of each pair in either list
-    int tc_max_tiles = 0;
-    DevBuf d_tcprob, d_tcsides, d_tcitems[2], d_exp, d_rowp, d_colp, d_sched;
+    DevBuf d_tcprob, d_tcitems[2], d_rowp, d_colp, d_sched;
     DevBuf d_stream;       // arena of the streamed solver (frames too large for K2's shared memory)
     bool use_stream = false;
     size_t feat_stride = 0;
@@ -77,8 +75,8 @@ struct Workspace {
         DevBuf* all[] = {&d_poff1, &d_poff2, &d_loff1, &d_loff2, &d_pdesc1, &d_pdesc2, &d_ldesc1, &d_ldesc2,
                          &d_ptP, &d_pts2, &d_ptpl, &d_lssP, &d_lseP, &d_lsspl, &d_lsepl, &d_lss2, &d_lslev,
                          &d_lsle, &d_priors, &d_results, &d_m12p, &d_m12l, &d_inlp, &d_inll, &d_rowpart,
-                         &d_colpart, &d_problems, &d_tiles, &d_feat, &d_phase, &d_tcprob, &d_tcsides, &d_tcitems[0],
-                         &d_tcitems[1], &d_exp, &d_rowp, &d_colp, &d_sched, &d_stream};
+                         &d_colpart, &d_problems, &d_tiles, &d_feat, &d_phase, &d_tcprob, &d_tcitems[0],
+                         &d_tcitems[1], &d_rowp, &d_colp, &d_sched, &d_stream};
         for (DevBuf* b : all) b->release();
     }
 };
@@ -336,14 +334,12 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     ws.max_tsplit = 32;
     ws.cap_pt = ws.cap_ls = 0;
     ws.max_n2 = 0;
-    size_t row_elems = 0, col_elems = 0, exp_tiles = 0, rowp_elems = 0, colp_elems = 0;
+    size_t row_elems = 0, col_elems = 0, rowp_elems = 0, colp_elems = 0;
     ws.tc_problems.assign(ws.use_tc ? (size_t)2 * B : 0, TcProblem{});
-    ws.tc_sides.assign(ws.use_tc ? (size_t)4 * B : 0, TcSide{});
     for (int k = 0; k < 2; ++k) {
         ws.tc_items[k].clear();
         ws.item_start[k].assign((size_t)B + 1, 0);
     }
-    ws.tc_max_tiles = 0;
     const float nnr_p = (float)cfg->min_ratio_12_p, nnr_l = (float)cfg->min_ratio_12_l;   // double -> float at the call
     for (int p = 0; p < B; ++p) {
         ws.tile_start[p] = (int32_t)ws.tiles.size();
@@ -361,21 +357,15 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
             plan_problem(pr, n1, n2, type ? cfg->has_lines != 0 : cfg->has_points != 0, type ? nnr_l : nnr_p,
                          cfg->best_lr_matches != 0, hint, ws.use_tc);
             if (ws.use_tc) {
-                // operands and partials as element / tile indices first, fixed up after allocation
-                const int t1 = pr.enabled ? (n1 + TC_ROWS - 1) / TC_ROWS : 0, t2 = pr.enabled ? (n2 + TC_ROWS - 1) / TC_ROWS : 0;
+                // partials as element indices first, fixed up after allocation
+                const int t2 = pr.enabled ? (n2 + TC_ROWS - 1) / TC_ROWS : 0;
                 TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
                 tp.n1 = n1;
                 tp.n2 = n2;
-                tp.xe = reinterpret_cast<const uint8_t*>(exp_tiles);
-                tp.ye = reinterpret_cast<const uint8_t*>(exp_tiles + t1);
                 tp.rowp = reinterpret_cast<uint32_t*>(rowp_elems);
                 tp.colp = reinterpret_cast<uint32_t*>(colp_elems);
-                ws.tc_sides[(size_t)4 * p + 2 * type] = TcSide{nullptr, pr.enabled ? n1 : 0, nullptr};
-                ws.tc_sides[(size_t)4 * p + 2 * type + 1] = TcSide{nullptr, pr.enabled ? n2 : 0, nullptr};
-                exp_tiles += (size_t)t1 + t2;
                 rowp_elems += (size_t)(pr.enabled ? (n2 + TC_CW - 1) / TC_CW : 0) * n1;
                 colp_elems += (size_t)(pr.enabled ? n2 : 0);
-                ws.tc_max_tiles = std::max(ws.tc_max_tiles, std::max(t1, t2));
                 for (int yb = 0; yb < (t2 + 1) / 2; ++yb) ws.tc_items[type].push_back(TcItem{2 * p + type, yb});
             }
             // offsets into the partial buffers are stored as element indices first, fixed up after allocation
@@ -420,11 +410,9 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     CK(ctx, ws.d_problems.ensure(ws.problems.size() * sizeof(MatchProblem)));
     CK(ctx, ws.d_tiles.ensure(ws.tiles.size() * sizeof(MatchTile)));
     if (ws.use_tc) {
-        CK(ctx, ws.d_exp.ensure(exp_tiles * TC_TILE_BYTES + 1024));
         CK(ctx, ws.d_rowp.ensure(rowp_elems * sizeof(uint32_t)));
         CK(ctx, ws.d_colp.ensure(colp_elems * sizeof(uint32_t)));
         CK(ctx, ws.d_tcprob.ensure(ws.tc_problems.size() * sizeof(TcProblem)));
-        CK(ctx, ws.d_tcsides.ensure(ws.tc_sides.size() * sizeof(TcSide)));
         for (int k = 0; k < 2; ++k) CK(ctx, ws.d_tcitems[k].ensure(ws.tc_items[k].size() * sizeof(TcItem)));
         if (!ws.d_sched.p) {   // scheduler words of the persistent matcher: one pair per compute stream, self re-arming
             CK(ctx, ws.d_sched.ensure(64));
@@ -474,25 +462,17 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
                 pr.m12 = ws.d_m12l.as<int32_t>() + ws.l_off1[p];
             }
             if (ws.use_tc) {
+                // the matcher expands the rows of the workspace's own 32-byte-row arenas (16-byte aligned loads)
                 TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
-                uint8_t* ebase = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws.d_exp.p) + 1023) & ~(uintptr_t)1023);
-                uint8_t* xe = ebase + reinterpret_cast<size_t>(tp.xe) * TC_TILE_BYTES;
-                uint8_t* ye = ebase + reinterpret_cast<size_t>(tp.ye) * TC_TILE_BYTES;
-                tp.xe = xe;
-                tp.ye = ye;
+                tp.d1 = pr.d1;
+                tp.d2 = pr.d2;
                 tp.rowp = ws.d_rowp.as<uint32_t>() + reinterpret_cast<size_t>(tp.rowp);
                 tp.colp = ws.d_colp.as<uint32_t>() + reinterpret_cast<size_t>(tp.colp);
-                ws.tc_sides[(size_t)4 * p + 2 * type].src = pr.d1;
-                ws.tc_sides[(size_t)4 * p + 2 * type].dst = xe;
-                ws.tc_sides[(size_t)4 * p + 2 * type + 1].src = pr.d2;
-                ws.tc_sides[(size_t)4 * p + 2 * type + 1].dst = ye;
             }
         }
     cudaStream_t s = ctx->s_h2d;
     if (ws.use_tc && !ws.tc_problems.empty()) {
         CK(ctx, cudaMemcpyAsync(ws.d_tcprob.p, ws.tc_problems.data(), ws.tc_problems.size() * sizeof(TcProblem),
-                                cudaMemcpyHostToDevice, s));
-        CK(ctx, cudaMemcpyAsync(ws.d_tcsides.p, ws.tc_sides.data(), ws.tc_sides.size() * sizeof(TcSide),
                                 cudaMemcpyHostToDevice, s));
         for (int k = 0; k < 2; ++k)
             if (!ws.tc_items[k].empty())
@@ -554,8 +534,7 @@ int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t 
     if (ws.use_tc) {
         const int a0 = ws.item_start[0][p0], a1 = ws.item_start[0][p1], b0 = ws.item_start[1][p0], b1 = ws.item_start[1][p1];
         if (a1 > a0 || b1 > b0) {
-            CK(ctx, launch_tc_expand(ws.d_tcsides.as<TcSide>() + (size_t)4 * p0, 4 * (p1 - p0), ws.tc_max_tiles, s));
-            if (marks) CK(ctx, cudaEventRecord(marks[0], s));
+            if (marks) CK(ctx, cudaEventRecord(marks[0], s));   // operands are expanded inside the matcher: empty stage
             // launches on the two compute streams may overlap: each has its own pair of scheduler words
             int* sched = ws.d_sched.as<int>() + (s == ctx->s_alt ? 8 : 0);
             CK(ctx, launch_tc_hamming(ws.d_tcprob.as<TcProblem>(), ws.d_tcitems[0].as<TcItem>() + a0, a1 - a0,
@@ -563,7 +542,7 @@ int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t 
             if (marks) CK(ctx, cudaEventRecord(marks[1], s));
             CK(ctx, launch_tc_resolve(ws.d_problems.as<MatchProblem>() + (size_t)2 * p0, ws.d_tcprob.as<TcProblem>() + (size_t)2 * p0,
                                       2 * (p1 - p0), 4, s));
-            ctx->launches += 3;
+            ctx->launches += 2;
         }
         return 0;
     }
@@ -809,7 +788,7 @@ int64_t plstvo_launch_count(const PlContext* ctx) { return ctx ? ctx->launches :
 
 // ---- matching.h surface -------------------------------------------------------------------------------
 // Plans the B problems of a plstvo_match_batch call as a points-only frame batch on ctx->ws, uploads them and enqueues K1
-// (expand, distance + top-2, resolve; or the integer form) on ctx->s_main.  The caller holds the lock, has validated B > 0
+// (distance + top-2, resolve; or the integer form) on ctx->s_main.  The caller holds the lock, has validated B > 0
 // and selected the device; on success ws.problems[2 p] is problem p, its partial keys pending on ctx->s_main.
 static int match_batch_launch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
                               const int32_t* off2, float nnr, int best_lr_matches) {
@@ -1947,8 +1926,8 @@ int plstvo_batch_stage_times(PlContext* ctx, PlDeviceBatch* db, int iters, doubl
     LOCK(ctx);
     CK(ctx, cudaSetDevice(ctx->device));
     Workspace& ws = db->ws;
-    // events: 0 start, 1 expand done, 2 distance done, 3 match done, 4 lists done, 5 GN stage 1 done, 6 outlier pass done,
-    // 7 GN stage 2 done, 8 end
+    // events: 0 start, 1 before the matcher (operands are expanded inside it: 0 -> 1 is empty), 2 distance done, 3 match done,
+    // 4 lists done, 5 GN stage 1 done, 6 outlier pass done, 7 GN stage 2 done, 8 end
     cudaEvent_t ev[9];
     for (auto& e : ev) CK(ctx, cudaEventCreate(&e));
     double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};

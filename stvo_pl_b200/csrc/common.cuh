@@ -252,7 +252,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                  : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+__device__ __forceinline__ void mbar_wait(uint32_t bar /* shared address */, uint32_t parity) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
@@ -261,10 +261,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         "@p bra DONE_%=;\n"
         "bra WAIT_%=;\n"
         "DONE_%=:\n"
-        "}\n" ::"r"(smem_u32(bar)),
+        "}\n" ::"r"(bar),
         "r"(parity)
         : "memory");
 }
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 // global -> shared bulk copy completing on an mbarrier; addresses and size must be multiples of 16 B
 __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
     asm volatile(

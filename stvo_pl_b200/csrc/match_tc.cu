@@ -3,12 +3,11 @@
 // Replaces the arithmetic of StVO::matchNNR / StVO::match (src/matching.cpp:41-91), i.e. OpenCV's
 // cv::BFMatcher(NORM_HAMMING)::knnMatch(desc1, desc2, ., 2) per direction.  With descriptor bits mapped to +-1,
 //     a . b = (#equal bits) - (#different bits) = 256 - 2 d(a, b)          (exact, |a . b| <= 256)
-// so the N1 x N2 distance matrix of one matching problem is a 256-deep GEMM.  Three kernels:
-//   tc_expand_kernel   32-byte descriptor rows -> 256 e4m3 bytes (+1.0 = 0x38, -1.0 = 0xB8), written directly in the
-//                      128-byte-swizzled K-major operand layout wgmma reads (tiles of 128 rows = 32 KB contiguous),
-//                      so the tiles move with plain bulk copies (UBLKCP) and need no tensor map;
-//   tc_hamming_kernel  persistent, warp-specialised: one producer thread (bulk copies + mbarriers), two consumer
-//                      warpgroups issuing wgmma m64n128k32 (e4m3 operands, f16 accumulators in registers, two columns
+// so the N1 x N2 distance matrix of one matching problem is a 256-deep GEMM.  Two kernels:
+//   tc_hamming_kernel  persistent, warp-specialised: a producer warpgroup loads the raw 32-byte descriptor rows from
+//                      global memory and expands them in shared memory to 256 e4m3 bytes each (+1.0 = 0x38, -1.0 = 0xB8)
+//                      in the 128-byte-swizzled K-major operand layout wgmma reads; two consumer
+//                      warpgroups issue wgmma m64n128k32 (e4m3 operands, f16 accumulators in registers, two columns
 //                      per register) on the two 128-train halves of a block, each half folded while the other is on the
 //                      tensor pipe, so the top-2 update of BOTH directions costs a few packed min/max per two distances:
 //                        row direction   (query -> trains): fold over the columns in registers, then over four lanes;
@@ -37,45 +36,53 @@ namespace plstvo {
 // expand: bits -> e4m3 +-1 bytes in the swizzled operand layout
 // tile (128 rows) = [slab 0..1][row group 0..15][row 0..7][16-byte chunk position 0..7]; slab = 128 K-bytes;
 // logical chunk c of row r sits at position c ^ (r & 7)  (the 128B swizzle: address bits [4,7) ^= bits [7,10))
+// The train block of a work item is two such tiles per slab: [slab 0..1][256 rows], the same formula with r = 0..255.
+//
+// Which descriptor bit lands on which K index is free, as long as queries and trains use the same order: a . b sums
+// over K.  The order taken makes the expansion two instructions per output word: 32-bit word i of the row (bits
+// 32 i .. 32 i + 31) fills the 32 K-bytes of logical chunks 2 i and 2 i + 1, and byte k of 4-byte group j of those
+// holds bit 8 k + j of the word.  Shifting the word left by 7 - j puts bit 8 k + j at bit 7 of byte k, the e4m3 sign.
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) tc_expand_kernel(const TcSide* __restrict__ sides) {
-    const TcSide s = sides[blockIdx.y];
-    const int tile = blockIdx.x;
-    if (tile * TC_ROWS >= s.n) return;
-    __shared__ uint32_t lut[16];
-    if (threadIdx.x < 16) {
-        uint32_t w = 0;
-        for (int b = 0; b < 4; ++b) w |= ((threadIdx.x >> b) & 1 ? 0x38u : 0xB8u) << (8 * b);
-        lut[threadIdx.x] = w;
-    }
-    __syncthreads();
-    uint8_t* dst_tile = s.dst + (size_t)tile * TC_TILE_BYTES;
-#pragma unroll
-    for (int it = 0; it < 8; ++it) {
-        const int u = it * 256 + threadIdx.x;
-        const int c = u & 7, slab = (u >> 3) & 1, r = u >> 4;
-        const int row = tile * TC_ROWS + r;
-        uint4 out = make_uint4(0, 0, 0, 0);   // rows past the end: zeros (their results are masked, never used)
-        if (row < s.n) {
-            const uint32_t hw = *reinterpret_cast<const uint16_t*>(s.src + (size_t)row * 32 + slab * 16 + c * 2);
-            out = make_uint4(lut[hw & 15], lut[(hw >> 4) & 15], lut[(hw >> 8) & 15], lut[hw >> 12]);
-        }
-        *reinterpret_cast<uint4*>(dst_tile + slab * 16384 + (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) * 16)) = out;
-    }
+__device__ __forceinline__ uint4 ldg_nc16(const uint8_t* p) {
+    uint4 v;
+    asm volatile("ld.global.nc.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+    return v;
 }
-
-cudaError_t launch_tc_expand(const TcSide* sides, int n_sides, int max_tiles, cudaStream_t stream) {
-    if (n_sides <= 0 || max_tiles <= 0) return cudaSuccess;
-    tc_expand_kernel<<<dim3(max_tiles, n_sides), 256, 0, stream>>>(sides);
-    return cudaGetLastError();
+__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+// one descriptor row (lo: bytes 0..15, hi: bytes 16..31) into operand row r of the block at shared address `base`
+// (1024-byte aligned, slab stride SLAB).  A row past the end of its matrix arrives as all-ones with one = 0 and is
+// written as zeros.  The row address carries r & 7 in the chunk bits, so each chunk's swizzled address is one XOR.
+template <int SLAB>
+__device__ __forceinline__ void expand_row(uint32_t base, int r, const uint4& lo, const uint4& hi, uint32_t one) {
+    // r is opaque here: the addresses of a producer thread's rows are loop-invariant, and hoisting them out of the
+    // item loop would overflow the producer's 40 registers
+    asm volatile("" : "+r"(r));
+    const uint32_t row = base + (r >> 3) * 1024 + (r & 7) * 144;   // 128 (r & 7) + 16 (r & 7)
+    const uint32_t w[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        uint32_t o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = (~(w[i] << (7 - j)) & 0x80808080u) | one;   // set: 0x38 (+1), clear: 0xB8 (-1)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const uint32_t c = (2 * i + h) & 7;
+            sts128((row ^ (c << 4)) + (i >> 2) * SLAB, o[4 * h], o[4 * h + 1], o[4 * h + 2], o[4 * h + 3]);
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // PTX helpers (wgmma)
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+__device__ __forceinline__ void mbar_arrive(uint32_t bar /* shared address */) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) { mbar_arrive(smem_u32(bar)); }
+// orders this thread's generic-proxy shared-memory stores before later async-proxy (wgmma) reads of them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
@@ -194,9 +201,9 @@ static_assert(TC_SMEM_USED + 1024 <= 227 * 1024, "tc_hamming_kernel: shared memo
 size_t tc_smem_bytes() { return (size_t)TC_SMEM_USED + 1024; }
 
 // Register budget: the CTA launches with 168 registers per thread (384 threads, 1 CTA / SM), too few for both accumulator
-// sets, the column state and the row chains of a consumer thread.  The producer warpgroup, one thread of which issues
-// the copies, hands most of its share to the consumers (setmaxnreg); each of the four SM sub-partitions then holds two
-// consumer warps and one producer warp: (2 x 232 + 40) x 32 <= 16384 registers.
+// sets, the column state and the row chains of a consumer thread.  The producer warpgroup, which needs few registers to
+// expand one row at a time, hands most of its share to the consumers (setmaxnreg); each of the four SM sub-partitions then
+// holds two consumer warps and one producer warp: (2 x 232 + 40) x 32 <= 16384 registers.
 constexpr int TC_LAUNCH_REGS = 168, TC_PRODUCER_REGS = 40, TC_CONSUMER_REGS = 232;
 static_assert(TC_LAUNCH_REGS * TC_THREADS <= 65536 &&
                   TC_CWARPS * TC_CONSUMER_REGS + (TC_THREADS / 32 - TC_CWARPS) * TC_PRODUCER_REGS <= TC_LAUNCH_REGS * TC_THREADS / 32,
@@ -227,10 +234,10 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
 
     if (tid == 0) {
         for (int i = 0; i < TC_XSTAGES; ++i) {
-            mbar_init(&x_full[i], 1);
+            mbar_init(&x_full[i], TC_PTHREADS);
             mbar_init(&x_empty[i], TC_CWARPS);
         }
-        mbar_init(y_full, 1);
+        mbar_init(y_full, TC_PTHREADS);
         mbar_init(y_empty, TC_CWARPS);
         for (int i = 0; i < TC_IRING; ++i) {
             mbar_init(&i_full[i], 1);
@@ -245,36 +252,68 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
     auto item_at = [&](int it) -> TcItem { return it < n_a ? items_a[it] : items_b[it - n_a]; };
 
     if (warp >= TC_CWARPS) {
-        // ===== producer: work distribution + bulk copies of operand tiles =====
+        // ===== producer: work distribution + operand expansion =====
+        // Thread 0 takes the items and announces them; every producer thread reads them from the ring.  (A slot is
+        // reused four items later, when all producer threads have long read it: the item before that needed every
+        // producer thread's query rows.)  Each producer thread expands two rows of the train block and one row of every
+        // query tile, and arrives on the full barrier after its stores.
         setmaxnreg_dec<TC_PRODUCER_REGS>();
-        if (warp == TC_CWARPS && lane == 0) {
-            uint32_t xs = 0, xph = 0;
-            for (uint32_t k = 0;; ++k) {
-                const uint32_t slot = k % TC_IRING;
-                mbar_wait(&i_empty[slot], ((k / TC_IRING) & 1) ^ 1);
+        const int ptid = tid - TC_CWARPS * 32;
+        // barriers as shared addresses off the aligned base (fewer live registers than the generic pointers)
+        const uint32_t bar_x_full = sbase + TC_OFF_BAR, bar_x_empty = bar_x_full + 8 * TC_XSTAGES,
+                       bar_y_full = bar_x_full + 16 * TC_XSTAGES, bar_y_empty = bar_y_full + 8,
+                       bar_i_full = bar_y_full + 16, bar_i_empty = bar_i_full + 8 * TC_IRING;
+        // The producer has 40 registers.  Rows are opaque (asm) so that a thread's row addresses are not hoisted out of the
+        // item loop, and the query side of the problem is re-read after the train block rather than held across it; n <=
+        // 65535 rows, so row offsets fit 32 bits.  The read-only (.nc) row loads carry no ordering, so ptxas issues them
+        // ahead of the stage wait where registers allow: the ring hides their latency.
+        auto row_ptr = [&](const uint8_t* d, int row) {
+            asm volatile("" : "+r"(row));
+            return d + (uint32_t)row * 32u;
+        };
+        // a row past the end of its matrix reads as all-ones and is expanded to zeros
+        auto expand = [&](auto slab, uint32_t base, int r, const uint8_t* d, int row, int n) {
+            const bool v = row < n;
+            const uint4 ones = make_uint4(~0u, ~0u, ~0u, ~0u);
+            const uint4 lo = v ? ldg_nc16(row_ptr(d, row)) : ones, hi = v ? ldg_nc16(row_ptr(d, row) + 16) : ones;
+            expand_row<decltype(slab)::value>(base, r, lo, hi, v ? 0x38383838u : 0u);
+        };
+        constexpr std::integral_constant<int, TC_TILE_BYTES / 2> XSLAB{};
+        constexpr std::integral_constant<int, TC_TILE_BYTES> YSLAB{};
+        uint32_t xs = 0, xph = 0;
+        auto query_tile = [&](const TcProblem& pr, int t) {
+            mbar_wait(bar_x_empty + 8 * xs, xph ^ 1);
+            expand(XSLAB, sbase + TC_OFF_X + xs * TC_TILE_BYTES, ptid, pr.d1, t * TC_ROWS + ptid, pr.n1);
+            fence_proxy_async_smem();
+            mbar_arrive(bar_x_full + 8 * xs);
+            if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
+        };
+        for (uint32_t k = 0;; ++k) {
+            const uint32_t slot = k % TC_IRING;
+            if (ptid == 0) {
+                mbar_wait(bar_i_empty + 8 * slot, ((k / TC_IRING) & 1) ^ 1);
                 int it = atomicAdd(sched, 1);
                 if (it >= n_items) it = -1;
                 iring[slot] = it;
-                mbar_arrive(&i_full[slot]);
-                if (it < 0) break;
-                const TcItem item = item_at(it);
-                const TcProblem pr = problems[item.problem];
-                const int nyt = (pr.n2 + TC_ROWS - 1) / TC_ROWS, nxt = (pr.n1 + TC_ROWS - 1) / TC_ROWS;
-                const int ytiles = min(2, nyt - 2 * item.yblk);
-                mbar_wait(y_empty, (k & 1) ^ 1);
-                mbar_arrive_expect_tx(y_full, (uint32_t)ytiles * TC_TILE_BYTES);
-                for (int h = 0; h < ytiles; ++h)
-                    for (int sl = 0; sl < 2; ++sl)
-                        bulk_g2s(sm + TC_OFF_Y + sl * 32768 + h * 16384,
-                                 pr.ye + (size_t)(2 * item.yblk + h) * TC_TILE_BYTES + sl * 16384, 16384, y_full);
-                for (int t = 0; t < nxt; ++t) {
-                    mbar_wait(&x_empty[xs], xph ^ 1);
-                    mbar_arrive_expect_tx(&x_full[xs], TC_TILE_BYTES);
-                    bulk_g2s(sm + TC_OFF_X + xs * TC_TILE_BYTES, pr.xe + (size_t)t * TC_TILE_BYTES, TC_TILE_BYTES,
-                             &x_full[xs]);
-                    if (++xs == TC_XSTAGES) { xs = 0; xph ^= 1; }
-                }
+                mbar_arrive(bar_i_full + 8 * slot);
             }
+            mbar_wait(bar_i_full + 8 * slot, (k / TC_IRING) & 1);
+            const int it = iring[slot];
+            if (it < 0) break;
+            const TcItem item = item_at(it);
+            const TcProblem pr = problems[item.problem];
+            mbar_wait(bar_y_empty, (k & 1) ^ 1);
+            expand(YSLAB, sbase + TC_OFF_Y, ptid, pr.d2, item.yblk * TC_CW + ptid, pr.n2);
+            fence_proxy_async_smem();   // (also keeps the next row's loads from being hoisted into this expansion)
+            expand(YSLAB, sbase + TC_OFF_Y, ptid + TC_ROWS, pr.d2, item.yblk * TC_CW + TC_ROWS + ptid, pr.n2);
+            fence_proxy_async_smem();
+            mbar_arrive(bar_y_full);
+            // the query side, re-read through an opaque index: one register across the train block, not a 64-bit pointer
+            int pi = item.problem;
+            asm volatile("" : "+r"(pi));
+            const TcProblem& pq = problems[pi];
+            const int nxt = (pq.n1 + TC_ROWS - 1) / TC_ROWS;
+            for (int t = 0; t < nxt; ++t) query_tile(pq, t);
         }
     } else {
         // ===== consumers: two warpgroups; warpgroup g multiplies query rows 64 g .. 64 g + 63 of every query tile with the

@@ -11,19 +11,13 @@ constexpr int TC_TILE_BYTES = TC_ROWS * 256;    // 128 rows x 256 e4m3 bytes, sw
 constexpr int TC_CW = 256;                      // trains per work item = per row-partial block (two wgmma N of 128)
 constexpr int TC_CWARPS = 8;                    // consumer warps: two warpgroups, 64 query rows of each tile apiece
 constexpr int TC_XSTAGES = 4;                   // query tiles in flight (shared memory ring)
-constexpr int TC_THREADS = 32 * TC_CWARPS + 128; // the consumer warpgroups + one producer warpgroup (one thread of it works)
-
-// one descriptor matrix to expand (queries or trains of one matching problem)
-struct TcSide {
-    const uint8_t* src;   // [n][32] descriptor rows
-    int32_t n;
-    uint8_t* dst;         // ceil(n / 128) tiles of TC_TILE_BYTES
-};
+constexpr int TC_PTHREADS = 128;                // the producer warpgroup: work distribution and operand expansion
+constexpr int TC_THREADS = 32 * TC_CWARPS + TC_PTHREADS;
 
 // one matching problem = StVO::match(desc1, desc2): queries stream through the M side, trains sit on the N side
 struct TcProblem {
-    const uint8_t* xe;    // expanded queries  (desc1): ceil(n1 / 128) tiles
-    const uint8_t* ye;    // expanded trains   (desc2): ceil(n2 / 128) tiles
+    const uint8_t* d1;    // [n1][32] query descriptor rows (desc1), 16-byte aligned; expanded in the matcher
+    const uint8_t* d2;    // [n2][32] train descriptor rows (desc2), 16-byte aligned
     int32_t n1, n2;
     uint32_t* rowp;       // [ceil(n2 / TC_CW)][n1]: best distance | second << 9 (511 = none) | tag << 18 (parity, chunk group, lane)
     uint32_t* colp;       // [n2]:                 best | second << 9 | tag << 18 (consumer warp)
@@ -36,7 +30,6 @@ struct TcItem {
 };
 
 size_t tc_smem_bytes();
-cudaError_t launch_tc_expand(const TcSide* sides, int n_sides, int max_tiles, cudaStream_t stream);
 // items_a then items_b form the work list (long items first); sched: two zeroed ints per concurrently running launch
 cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, int n_a, const TcItem* items_b, int n_b,
                               int* sched, int grid, cudaStream_t stream);
