@@ -315,6 +315,30 @@ int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, 
  * [2] angles and descriptors. */
 int plstvo_orb_kernel_times(PlContext* ctx, float* ms3);
 
+/* ---- ORB detection + description: cv::ORB::detectAndCompute with an empty mask ---- */
+typedef struct PlOrbDetectConfig {
+    PlOrbConfig orb;               /* pyramid, edge threshold, patch, WTA_K (scale_factor is rounded to float, as ORB::create takes it) */
+    int32_t n_features;            /* nfeatures (>= 0), spread over the levels as ORB spreads it */
+    int32_t score_type;            /* 1: FAST_SCORE, 0: HARRIS_SCORE */
+    int32_t fast_threshold;        /* used where fast_th == NULL; clamped to [0, 255] */
+} PlOrbDetectConfig;
+void plstvo_default_orb_detect_config(PlOrbDetectConfig* c);   /* 1200, 1.2, 4, 19, FAST, 31, 2, 20 */
+/* Key points, angles and descriptors of n_img grey images of one size (images: [n_img][height][width] uint8), bit-identical
+ * to OpenCV 4.13's ORB::detectAndCompute(image, noArray()) per image.  fast_th: [n_img] FAST thresholds, or NULL for
+ * cfg->fast_threshold everywhere.  Image i's key points are rows kp_off[i] .. kp_off[i + 1] of kp_xy ([n][2], pt), kp_octave,
+ * kp_angle (degrees), kp_response (FAST score or Harris response) and desc ([n][32], the layout PlStereoFeatures takes);
+ * within an image they are ordered by level, then y, then x on the level (the set and every field equal OpenCV's; OpenCV's
+ * order is that of nth_element).  Any of kp_xy .. desc may be NULL to skip that output.  Returns the number of key points.
+ * PLSTVO_E_TOO_LARGE: more than capacity key points in all, or more than PLSTVO_MAX_FEATURES in one image; kp_off
+ * ([n_img + 1]) is still written in full, so the caller can size its buffers and call again.  PLSTVO_E_INVALID: the
+ * PlOrbConfig checks of plstvo_orb_compute_batch, n_features < 0, or score_type other than 0 or 1. */
+int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                                        const uint8_t* images, const int32_t* fast_th, int capacity, int32_t* kp_off,
+                                        float* kp_xy, int32_t* kp_octave, float* kp_angle, float* kp_response, uint8_t* desc);
+/* Device time of the last plstvo_orb_detect_and_compute_batch on this context, ms: [0] pyramid and blur, [1] FAST and
+ * non-max suppression, [2] selection (retainBest, Harris), [3] angles and descriptors. */
+int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

@@ -132,6 +132,38 @@ inline int computeORB(Context& c, const PlOrbConfig& cfg, const uint8_t* image, 
     if (angle) angle->assign(ang_out.begin(), ang_out.begin() + k);
     return k;
 }
+// ORB::detectAndCompute on one grey image (row-major, width * height bytes), as StereoFrame::detectPointFeatures calls it
+// (src/stereoFrame.cpp:104-118): fast_th != 0 replaces cfg.fast_threshold (the reference adapts it frame by frame, :109-111).
+// kp is replaced by the key points, ordered by level, then y, then x on the level, with their descriptors; angle and response
+// (if given) likewise.  Returns the key point count.
+inline int detectAndComputeORB(Context& c, const PlOrbDetectConfig& cfg, const uint8_t* image, int width, int height,
+                               KeyPoints& kp, int fast_th = 0, std::vector<float>* angle = nullptr,
+                               std::vector<float>* response = nullptr) {
+    const int32_t th = fast_th != 0 ? fast_th : cfg.fast_threshold;
+    int cap = 2 * std::max(cfg.n_features, 0) + 64;
+    std::vector<float> ang, resp;
+    for (;;) {
+        int32_t off[2] = {0, 0};
+        kp.pt.resize(2 * (size_t)cap);
+        kp.octave.resize((size_t)cap);
+        kp.desc.resize(32 * (size_t)cap);
+        ang.resize((size_t)cap);
+        resp.resize((size_t)cap);
+        const int rc = plstvo_orb_detect_and_compute_batch(c.get(), &cfg, 1, width, height, image, &th, cap, off, kp.pt.data(),
+                                                           kp.octave.data(), ang.data(), resp.data(), kp.desc.data());
+        if (rc == PLSTVO_E_TOO_LARGE && off[1] > cap && off[1] <= PLSTVO_MAX_FEATURES) {   // ties past the budget
+            cap = off[1];
+            continue;
+        }
+        const int n = c.check(rc);
+        kp.pt.resize(2 * (size_t)n);
+        kp.octave.resize((size_t)n);
+        kp.desc.resize(32 * (size_t)n);
+        if (angle) angle->assign(ang.begin(), ang.begin() + n);
+        if (response) response->assign(resp.begin(), resp.begin() + n);
+        return n;
+    }
+}
 inline int matchStereoLines(Context& c, const PlCamera& cam, const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
                             const KeyLines& l, const KeyLines& r, StereoFrame& out) {
     const int n = l.size();

@@ -107,6 +107,9 @@ struct PlContext {
     DevBuf arena_orb;      // plstvo_orb_compute_batch: images, level buffers, key points, outputs
     bool orb_tables = false;
     cudaEvent_t orb_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    DevBuf arena_orb_kp;   // plstvo_orb_detect_and_compute_batch: per-key-point arrays, sized once the selection is counted
+    bool orb_computed = false, orb_detected = false;
+    cudaEvent_t orb_det_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
     // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
     void* h_staging[3] = {nullptr, nullptr, nullptr};
     size_t h_staging_bytes[3] = {0, 0, 0};
@@ -736,7 +739,10 @@ void plstvo_destroy(PlContext* ctx) {
     for (auto& b : ctx->gs_in) b.release();
     ctx->gs_rec_pt.release(); ctx->gs_rec_ls.release();
     ctx->arena_orb.release();
+    ctx->arena_orb_kp.release();
     for (cudaEvent_t e : ctx->orb_ev)
+        if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->orb_det_ev)
         if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->events) cudaEventDestroy(e);
     for (void* h : ctx->h_staging)
@@ -2167,40 +2173,28 @@ void orb_linear_exact_table(int src, int dst, int32_t* t) {
         }
     }
 }
-}  // namespace
 
-int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, int width, int height, const uint8_t* images,
-                             const int32_t* kp_off, const float* kp_xy, const int32_t* kp_octave, const float* kp_angle,
-                             float* out_angle, uint8_t* out_desc, int32_t* src_idx, int32_t* counts) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!cfg || n_img < 0 || width < 0 || height < 0) return fail(ctx, PLSTVO_E_INVALID, "null config or negative size");
+int orb_check_config(PlContext* ctx, const PlOrbConfig* cfg) {
     if (cfg->patch_size != 31) return fail(ctx, PLSTVO_E_INVALID, "patch_size must be 31");
     if (cfg->wta_k != 2) return fail(ctx, PLSTVO_E_INVALID, "wta_k must be 2");
     if (cfg->n_levels < 1 || cfg->n_levels > ORB_MAX_LEVELS) return fail(ctx, PLSTVO_E_INVALID, "n_levels must be 1..32");
     if (cfg->edge_threshold < 0) return fail(ctx, PLSTVO_E_INVALID, "negative edge_threshold");
     if (cfg->n_levels > 1 && !(cfg->scale_factor > 1.0 && cfg->scale_factor < 1e6))
         return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1");
-    if (n_img == 0) return 0;
-    if (!images || !kp_off || kp_off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null images / offsets or kp_off[0] != 0");
-    for (int i = 0; i < n_img; ++i) {
-        const int n = kp_off[i + 1] - kp_off[i];
-        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kp_off is not non-decreasing");
-        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
-    }
-    const size_t N = (size_t)kp_off[n_img];
-    if (N && (!kp_xy || !kp_octave || !out_angle || !out_desc || !src_idx))
-        return fail(ctx, PLSTVO_E_INVALID, "null key point or output array");
-    for (size_t k = 0; k < N; ++k)
-        if (kp_octave[k] < 0 || kp_octave[k] >= cfg->n_levels) return fail(ctx, PLSTVO_E_INVALID, "octave outside [0, n_levels)");
-    OrbDevLevels L{};
+    return 0;
+}
+
+// level sizes and offsets, blur taps and resize tables of the pyramid; false: a level of zero size
+bool orb_levels(const PlOrbConfig* cfg, int width, int height, OrbDevLevels& L, std::vector<int32_t>& tabs,
+                std::vector<size_t>& tab_off) {
+    L = OrbDevLevels{};
     L.n = cfg->n_levels;
     for (int l = 0; l < L.n; ++l) {
         const float scale = (float)pow(cfg->scale_factor, (double)l);
         L.inv[l] = 1.f / scale;
         L.w[l] = (int)lrintf((float)width * L.inv[l]);
         L.h[l] = (int)lrintf((float)height * L.inv[l]);
-        if (L.w[l] < 1 || L.h[l] < 1) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+        if (L.w[l] < 1 || L.h[l] < 1) return false;
         L.raw_off[l] = l ? L.raw_stride : 0;
         if (l) L.raw_stride += (size_t)L.w[l] * L.h[l];
         L.blur_off[l] = L.blur_stride;
@@ -2214,8 +2208,8 @@ int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, 
         }
         for (int i = 0; i < 7; ++i) L.taps[i] = (float)(e[i] * (1.0 / sum));
     }
-    std::vector<int32_t> tabs;
-    std::vector<size_t> tab_off(2 * (size_t)L.n, 0);
+    tabs.clear();
+    tab_off.assign(2 * (size_t)L.n, 0);
     for (int l = 1; l < L.n; ++l) {
         tab_off[2 * l] = tabs.size();
         tabs.resize(tabs.size() + 2 * (size_t)L.w[l]);
@@ -2224,12 +2218,46 @@ int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, 
         tabs.resize(tabs.size() + 2 * (size_t)L.h[l]);
         orb_linear_exact_table(L.h[l - 1], L.h[l], tabs.data() + tab_off[2 * l + 1]);
     }
-    CK(ctx, cudaSetDevice(ctx->device));
-    if (!ctx->orb_tables) {
-        CK(ctx, orb_upload_tables());
-        for (auto& e : ctx->orb_ev) CK(ctx, cudaEventCreate(&e));
-        ctx->orb_tables = true;
+    return true;
+}
+
+cudaError_t orb_init(PlContext* ctx) {   // constant tables and timing events, once per context
+    if (ctx->orb_tables) return cudaSuccess;
+    cudaError_t e = orb_upload_tables();
+    for (auto& ev : ctx->orb_ev)
+        if (e == cudaSuccess) e = cudaEventCreate(&ev);
+    for (auto& ev : ctx->orb_det_ev)
+        if (e == cudaSuccess) e = cudaEventCreate(&ev);
+    if (e == cudaSuccess) ctx->orb_tables = true;
+    return e;
+}
+}  // namespace
+
+int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                             const int32_t* kp_off, const float* kp_xy, const int32_t* kp_octave, const float* kp_angle,
+                             float* out_angle, uint8_t* out_desc, int32_t* src_idx, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0) return fail(ctx, PLSTVO_E_INVALID, "null config or negative size");
+    if (const int rc = orb_check_config(ctx, cfg)) return rc;
+    if (n_img == 0) return 0;
+    if (!images || !kp_off || kp_off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null images / offsets or kp_off[0] != 0");
+    for (int i = 0; i < n_img; ++i) {
+        const int n = kp_off[i + 1] - kp_off[i];
+        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kp_off is not non-decreasing");
+        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
     }
+    const size_t N = (size_t)kp_off[n_img];
+    if (N && (!kp_xy || !kp_octave || !out_angle || !out_desc || !src_idx))
+        return fail(ctx, PLSTVO_E_INVALID, "null key point or output array");
+    for (size_t k = 0; k < N; ++k)
+        if (kp_octave[k] < 0 || kp_octave[k] >= cfg->n_levels) return fail(ctx, PLSTVO_E_INVALID, "octave outside [0, n_levels)");
+    OrbDevLevels L{};
+    std::vector<int32_t> tabs;
+    std::vector<size_t> tab_off;
+    if (!orb_levels(cfg, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, orb_init(ctx));
     const size_t img_bytes = (size_t)n_img * width * height;
     LiftArena a;
     const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
@@ -2263,6 +2291,7 @@ int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, 
     CK(ctx, launch_orb(L, n_img, width, height, cfg->edge_threshold, base + o_img, base + o_raw, base + o_blur, rs_tab.data(),
                        I(o_off), (int)N, F(o_xy), I(o_oct), kp_angle ? F(o_ang) : nullptr, I(o_src), I(o_cnt), F(o_oang),
                        base + o_desc, s, ctx->orb_ev, &launches));
+    ctx->orb_computed = true;
     ctx->launches += launches;
     std::vector<int32_t> cnt((size_t)n_img), src_dev(N);
     CK(ctx, down(cnt.data(), o_cnt, (size_t)n_img * 4));
@@ -2289,9 +2318,180 @@ int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, 
 int plstvo_orb_kernel_times(PlContext* ctx, float* ms3) {
     if (!ctx || !ms3) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ctx->orb_tables) return fail(ctx, PLSTVO_E_INVALID, "no ORB call on this context yet");
+    if (!ctx->orb_computed) return fail(ctx, PLSTVO_E_INVALID, "no ORB call on this context yet");
     CK(ctx, cudaSetDevice(ctx->device));
     for (int k = 0; k < 3; ++k) CK(ctx, cudaEventElapsedTime(&ms3[k], ctx->orb_ev[k], ctx->orb_ev[k + 1]));
+    return 0;
+}
+
+/* ---- ORB key-point selection + description (orb.cu) ---- */
+void plstvo_default_orb_detect_config(PlOrbDetectConfig* c) {
+    if (!c) return;
+    plstvo_default_orb_config(&c->orb);
+    c->n_features = 1200; c->score_type = 1; c->fast_threshold = 20;
+}
+
+int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                                        const uint8_t* images, const int32_t* fast_th, int capacity, int32_t* kp_off,
+                                        float* kp_xy, int32_t* kp_octave, float* kp_angle, float* kp_response, uint8_t* desc) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0 || capacity < 0)
+        return fail(ctx, PLSTVO_E_INVALID, "null config, negative size or negative capacity");
+    if (const int rc = orb_check_config(ctx, &cfg->orb)) return rc;
+    if (cfg->n_features < 0) return fail(ctx, PLSTVO_E_INVALID, "negative n_features");
+    if (cfg->score_type != 0 && cfg->score_type != 1) return fail(ctx, PLSTVO_E_INVALID, "score_type must be 0 (Harris) or 1 (FAST)");
+    if (!kp_off) return fail(ctx, PLSTVO_E_INVALID, "null kp_off");
+    kp_off[0] = 0;
+    if (n_img == 0) return 0;
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    PlOrbConfig oc = cfg->orb;
+    oc.scale_factor = (double)(float)oc.scale_factor;   // ORB::create takes a float scale factor
+    if (oc.n_levels > 1 && !(oc.scale_factor > 1.0)) return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1 in float");
+    OrbDevLevels L{};
+    std::vector<int32_t> tabs;
+    std::vector<size_t> tab_off;
+    if (!orb_levels(&oc, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    const int nl = L.n;
+    const bool harris = cfg->score_type == 0;
+    OrbDetectLevels D{};
+    {   // the per-level budget, in float as ORB computes it
+        const float factor = (float)(1.0 / oc.scale_factor);
+        float nd = (float)cfg->n_features * (1.f - factor) / (1.f - (float)pow((double)factor, (double)nl));
+        int sum = 0;
+        for (int l = 0; l < nl; ++l) {
+            int n = 0;
+            if (l < nl - 1) {
+                n = (int)lrintf(nd);
+                sum += n;
+                nd *= factor;
+            } else {
+                n = std::max(cfg->n_features - sum, 0);
+            }
+            D.keep1[l] = harris ? 2 * n : n;
+            D.keep2[l] = n;
+            D.row0[l + 1] = D.row0[l] + L.h[l];
+            D.layer_scale[l] = (float)pow(oc.scale_factor, (double)l);
+        }
+        D.edge = cfg->orb.edge_threshold;
+        const float hs = 1.f / (28 * 255.f);   // 1 / ((1 << 2) * blockSize * 255), blockSize 7
+        D.harris_scale4 = hs * hs * hs * hs;
+    }
+    const int R = D.row0[nl];
+    std::vector<int32_t> th((size_t)n_img);
+    for (int i = 0; i < n_img; ++i) th[i] = std::min(std::max(fast_th ? fast_th[i] : cfg->fast_threshold, 0), 255);
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, orb_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height, NL = (size_t)n_img * nl;
+    LiftArena a;
+    const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
+    const size_t o_blur = a.take((size_t)n_img * L.blur_stride), o_tab = a.take(tabs.size() * 4 + 4);
+    const size_t o_score = a.take((size_t)n_img * L.blur_stride), o_hist = a.take(NL * 256 * 4), o_cut = a.take(NL * 4);
+    const size_t o_rcnt = a.take((size_t)n_img * R * 4), o_rbase = a.take((size_t)n_img * (R + 1) * 4);
+    const size_t o_icnt = a.take((size_t)n_img * 4), o_soff = a.take((size_t)(n_img + 1) * 4), o_th = a.take((size_t)n_img * 4);
+    const size_t o_lkeep = a.take(NL * 4), o_ckey = a.take(NL * 4), o_hoff = a.take((size_t)(n_img + 1) * 4);
+    const size_t o_hcnt = a.take((size_t)n_img * 4);
+    DevBuf& arena = ctx->arena_orb;
+    CK(ctx, arena.ensure(a.off));
+    uint8_t* base = arena.as<uint8_t>();
+    cudaStream_t s = ctx->s_main;
+    auto I = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
+    CK(ctx, cudaMemcpyAsync(base + o_img, images, img_bytes, cudaMemcpyHostToDevice, s));
+    if (!tabs.empty()) CK(ctx, cudaMemcpyAsync(base + o_tab, tabs.data(), tabs.size() * 4, cudaMemcpyHostToDevice, s));
+    CK(ctx, cudaMemcpyAsync(base + o_th, th.data(), (size_t)n_img * 4, cudaMemcpyHostToDevice, s));
+    std::vector<const int32_t*> rs_tab(2 * (size_t)nl, nullptr);
+    for (int l = 1; l < nl; ++l) {
+        rs_tab[2 * l] = I(o_tab) + tab_off[2 * l];
+        rs_tab[2 * l + 1] = I(o_tab) + tab_off[2 * l + 1];
+    }
+    cudaEvent_t* ev = ctx->orb_det_ev;   // [0] start, [1] pyramid + blur, [2] FAST + NMS, [3] selection, [4] angle + descriptor
+    int launches = 0;
+    CK(ctx, cudaEventRecord(ev[0], s));
+    launch_orb_pyramid(L, n_img, base + o_img, base + o_raw, base + o_blur, rs_tab.data(), s, &launches);
+    CK(ctx, cudaEventRecord(ev[1], s));
+    launch_orb_fast_select(L, D, n_img, base + o_img, base + o_raw, I(o_th), base + o_score,
+                           reinterpret_cast<uint32_t*>(base + o_hist), I(o_cut), I(o_rcnt), I(o_rbase), I(o_icnt), I(o_soff), s,
+                           ev[2], &launches);
+    CK(ctx, cudaGetLastError());
+    std::vector<int32_t> off((size_t)n_img + 1);
+    CK(ctx, cudaMemcpyAsync(off.data(), I(o_soff), off.size() * 4, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    ctx->launches += launches;
+    launches = 0;
+    ctx->orb_detected = true;
+    // too many key points: kp_off in full (the caller sizes its buffers from it), nothing else written
+    auto too_large = [&]() -> int {
+        CK(ctx, cudaEventRecord(ev[3], s));
+        CK(ctx, cudaEventRecord(ev[4], s));
+        memcpy(kp_off, off.data(), off.size() * 4);
+        for (int i = 0; i < n_img; ++i)
+            if (off[i + 1] - off[i] > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
+        if (off[n_img] > capacity) return fail(ctx, PLSTVO_E_TOO_LARGE, "more key points than capacity");
+        return 0;
+    };
+    auto exceeds = [&]() {
+        if (off[n_img] > capacity) return true;
+        for (int i = 0; i < n_img; ++i)
+            if (off[i + 1] - off[i] > PLSTVO_MAX_FEATURES) return true;
+        return false;
+    };
+    if (!harris && exceeds()) return too_large();
+    const size_t N1 = (size_t)off[n_img];
+    LiftArena b;
+    const size_t o_lxy = b.take(N1 * 8), o_xy = b.take(N1 * 8), o_oct = b.take(N1 * 4), o_resp = b.take(N1 * 4);
+    const size_t o_rank = b.take(N1 * 4), o_hresp = b.take(harris ? N1 * 4 : 0), o_fxy = b.take(harris ? N1 * 8 : 0);
+    const size_t o_foct = b.take(harris ? N1 * 4 : 0), o_fresp = b.take(harris ? N1 * 4 : 0);
+    const size_t o_frank = b.take(harris ? N1 * 4 : 0), o_ang = b.take(N1 * 4), o_desc = b.take(N1 * 32);
+    DevBuf& kp_arena = ctx->arena_orb_kp;
+    CK(ctx, kp_arena.ensure(b.off));
+    uint8_t* kb = kp_arena.as<uint8_t>();
+    auto KI = [&](size_t o) { return reinterpret_cast<int32_t*>(kb + o); };
+    auto KF = [&](size_t o) { return reinterpret_cast<float*>(kb + o); };
+    launch_orb_fast_write(L, D, n_img, base + o_score, I(o_cut), I(o_rbase), I(o_soff), reinterpret_cast<int2*>(kb + o_lxy),
+                          KF(o_xy), KI(o_oct), KF(o_resp), KI(o_rank), s, &launches);
+    const int32_t *d_off = I(o_soff), *d_cnt = I(o_icnt), *d_oct = KI(o_oct), *d_rank = KI(o_rank);
+    const float *d_xy = KF(o_xy), *d_resp = KF(o_resp);
+    if (harris) {
+        uint32_t* ckey = reinterpret_cast<uint32_t*>(base + o_ckey);
+        launch_orb_harris_select(L, D, n_img, (int)N1, base + o_img, base + o_raw, I(o_rbase), I(o_soff),
+                                 reinterpret_cast<int2*>(kb + o_lxy), KI(o_oct), KF(o_hresp), ckey, I(o_lkeep), I(o_hoff),
+                                 I(o_hcnt), s, &launches);
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(off.data(), I(o_hoff), off.size() * 4, cudaMemcpyDeviceToHost, s));
+        CK(ctx, cudaStreamSynchronize(s));
+        ctx->launches += launches;
+        launches = 0;
+        if (exceeds()) return too_large();
+        launch_orb_harris_write(L, D, n_img, I(o_soff), KF(o_xy), KI(o_oct), KF(o_hresp), ckey, I(o_hoff), KF(o_fxy), KI(o_foct),
+                                KF(o_fresp), KI(o_frank), s, &launches);
+        d_off = I(o_hoff); d_cnt = I(o_hcnt); d_oct = KI(o_foct); d_rank = KI(o_frank); d_xy = KF(o_fxy); d_resp = KF(o_fresp);
+    }
+    CK(ctx, cudaEventRecord(ev[3], s));
+    const size_t N = (size_t)off[n_img];
+    launch_orb_describe(L, n_img, base + o_img, base + o_raw, base + o_blur, d_off, (int)N, d_xy, d_oct, nullptr, d_rank, d_cnt,
+                        KF(o_ang), kb + o_desc, s, &launches);
+    CK(ctx, cudaEventRecord(ev[4], s));
+    CK(ctx, cudaGetLastError());
+    ctx->launches += launches;
+    auto down = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
+        return (dst && bytes) ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    };
+    CK(ctx, down(kp_xy, d_xy, N * 8));
+    CK(ctx, down(kp_octave, d_oct, N * 4));
+    CK(ctx, down(kp_angle, KF(o_ang), N * 4));
+    CK(ctx, down(kp_response, d_resp, N * 4));
+    CK(ctx, down(desc, kb + o_desc, N * 32));
+    CK(ctx, cudaStreamSynchronize(s));
+    memcpy(kp_off, off.data(), off.size() * 4);
+    return (int)N;
+}
+
+int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4) {
+    if (!ctx || !ms4) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->orb_detected) return fail(ctx, PLSTVO_E_INVALID, "no ORB detect call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 4; ++k) CK(ctx, cudaEventElapsedTime(&ms4[k], ctx->orb_det_ev[k], ctx->orb_det_ev[k + 1]));
     return 0;
 }
 

@@ -213,6 +213,44 @@ cudaError_t launch_orb(const OrbDevLevels& L, int n_img, int W, int H, int edge,
                        uint8_t* blur_pyr, const int32_t* const* rs_tab, const int32_t* kp_off, int n_rows, const float* kp_xy,
                        const int32_t* kp_oct, const float* kp_angle, int32_t* src_idx, int32_t* counts, float* out_angle,
                        uint8_t* out_desc, cudaStream_t s, cudaEvent_t* ev, int* launches);
+// the two halves of launch_orb that key-point selection sits between
+void launch_orb_pyramid(const OrbDevLevels& L, int n_img, const uint8_t* images, uint8_t* raw_pyr, uint8_t* blur_pyr,
+                        const int32_t* const* rs_tab, cudaStream_t s, int* launches);
+void launch_orb_describe(const OrbDevLevels& L, int n_img, const uint8_t* images, const uint8_t* raw_pyr,
+                         const uint8_t* blur_pyr, const int32_t* kp_off, int n_rows, const float* kp_xy, const int32_t* kp_oct,
+                         const float* kp_angle, const int32_t* src_idx, const int32_t* counts, float* out_angle,
+                         uint8_t* out_desc, cudaStream_t s, int* launches);
+
+// ORB key-point selection (cv::ORB's computeKeyPoints with an empty mask).  Rows: the levels of one image stacked, level l's
+// row y is row row0[l] + y; key points come out per image in (level, y, x) order.
+struct OrbDetectLevels {
+    int keep1[ORB_MAX_LEVELS];        // retainBest count on the FAST score: n_l (FAST_SCORE) or 2 n_l (HARRIS_SCORE)
+    int keep2[ORB_MAX_LEVELS];        // retainBest count on the Harris response: n_l
+    int row0[ORB_MAX_LEVELS + 1];     // prefix of the level heights; row0[n] = rows per image
+    float layer_scale[ORB_MAX_LEVELS];// (float)pow(scale, l): pt = level coordinate * layer_scale
+    int edge;                         // runByImageBorder on the level
+    float harris_scale4;              // (1 / (4 * 7 * 255))^4, multiplied in float as OpenCV does
+};
+// FAST + NMS + border filter into the score maps (blur_pyr's geometry) with a 256-bin histogram per (image, level), the
+// per-(image, level) FAST cut, row counts, per-image row scan and image offsets (sel_off [n_img + 1], sel_cnt [n_img]).
+void launch_orb_fast_select(const OrbDevLevels& L, const OrbDetectLevels& D, int n_img, const uint8_t* images,
+                            const uint8_t* raw_pyr, const int32_t* fast_th, uint8_t* score, uint32_t* hist, int32_t* cut,
+                            int32_t* row_cnt, int32_t* row_base, int32_t* img_cnt, int32_t* sel_off, cudaStream_t s,
+                            cudaEvent_t ev_fast_done, int* launches);
+// writes the FAST-selected key points densely at sel_off[img] + rank: level coordinates, pt, octave, FAST response, rank
+void launch_orb_fast_write(const OrbDevLevels& L, const OrbDetectLevels& D, int n_img, const uint8_t* score, const int32_t* cut,
+                           const int32_t* row_base, const int32_t* sel_off, int2* lxy, float* xy, int32_t* oct, float* resp,
+                           int32_t* rank, cudaStream_t s, int* launches);
+// HARRIS_SCORE: responses of the FAST-selected candidates, the n_l-th largest per (image, level), and the survivors densely
+// at out_off[img] + rank (out_off [n_img + 1], out_cnt [n_img])
+void launch_orb_harris_select(const OrbDevLevels& L, const OrbDetectLevels& D, int n_img, int n_cand, const uint8_t* images,
+                              const uint8_t* raw_pyr, const int32_t* row_base, const int32_t* sel_off, const int2* lxy,
+                              const int32_t* oct, float* hresp, uint32_t* cut_key, int32_t* lvl_keep, int32_t* out_off,
+                              int32_t* out_cnt, cudaStream_t s, int* launches);
+void launch_orb_harris_write(const OrbDevLevels& L, const OrbDetectLevels& D, int n_img, const int32_t* sel_off,
+                             const float* xy, const int32_t* oct, const float* hresp, const uint32_t* cut_key,
+                             const int32_t* out_off, float* out_xy, int32_t* out_oct, float* out_resp, int32_t* out_rank,
+                             cudaStream_t s, int* launches);
 
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);

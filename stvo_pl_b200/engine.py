@@ -91,6 +91,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_orb_compute_batch": (C.c_int, [vp, C.POINTER(T.PlOrbConfig), C.c_int, C.c_int, C.c_int, u8p, i32p, fp, i32p, fp,
                                                fp, u8p, i32p, i32p]),
         "plstvo_orb_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_default_orb_detect_config": (None, [C.POINTER(T.PlOrbDetectConfig)]),
+        "plstvo_orb_detect_and_compute_batch": (C.c_int, [vp, C.POINTER(T.PlOrbDetectConfig), C.c_int, C.c_int, C.c_int, u8p,
+                                                          i32p, C.c_int, i32p, fp, i32p, fp, fp, u8p]),
+        "plstvo_orb_detect_kernel_times": (C.c_int, [vp, fp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -109,7 +113,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_batch_run_timed", "plstvo_batch_download", "plstvo_batch_free", "plstvo_synchronize",
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
-    "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times"]
+    "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
+    "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -351,6 +356,40 @@ class Engine:
         """Device ms of the last orb_compute_batch: pyramid + blur, border filter, angles + descriptors."""
         ms = np.zeros(3, np.float32)
         self._ck(self.lib.plstvo_orb_kernel_times(self.ctx, _p(ms, T.c_float_p)))
+        return ms
+
+    def orb_detect_and_compute_batch(self, cfg: T.PlOrbDetectConfig, images, fast_th=None, capacity: Optional[int] = None):
+        """ORB::detectAndCompute on each of images uint8[n, H, W] (empty mask).  fast_th: per-image FAST thresholds, or None
+        for cfg.fast_threshold.  Returns (total, dict(off [n + 1], xy [total, 2], octave, angle, response, desc [total, 32]));
+        image i's key points are rows off[i] .. off[i + 1], ordered by level, then y, then x on the level.  Without a
+        capacity the call sizes its buffers from the feature budget and, if more key points come out (ties), calls again
+        with the exact count; with one, more than capacity raises PLSTVO_E_TOO_LARGE."""
+        images = np.ascontiguousarray(images, np.uint8)
+        n_img, H, W = images.shape
+        th = None if fast_th is None else np.ascontiguousarray(np.broadcast_to(np.asarray(fast_th, np.int32), (n_img,)))
+        cap = int(capacity) if capacity is not None else n_img * (2 * max(int(cfg.n_features), 0) + 64)
+        while True:
+            off = np.zeros(n_img + 1, np.int32)
+            out = dict(off=off, xy=np.zeros((cap, 2), np.float32), octave=np.zeros(cap, np.int32),
+                       angle=np.zeros(cap, np.float32), response=np.zeros(cap, np.float32), desc=np.zeros((cap, 32), np.uint8))
+            rc = self.lib.plstvo_orb_detect_and_compute_batch(
+                self.ctx, C.byref(cfg), n_img, W, H, _p(images, T.c_uint8_p), _p(th, T.c_int32_p), cap,
+                _p(off, T.c_int32_p), _p(out["xy"], T.c_float_p), _p(out["octave"], T.c_int32_p), _p(out["angle"], T.c_float_p),
+                _p(out["response"], T.c_float_p), _p(out["desc"], T.c_uint8_p))
+            if rc == -2 and capacity is None and off[-1] > cap and np.diff(off).max() <= 65535:
+                cap = int(off[-1])
+                continue
+            total = self._ck(rc)
+            break
+        for k in ("xy", "octave", "angle", "response", "desc"):
+            out[k] = out[k][:total]
+        return total, out
+
+    def orb_detect_kernel_times(self):
+        """Device ms of the last orb_detect_and_compute_batch: pyramid + blur, FAST + NMS, selection (with Harris),
+        angles + descriptors."""
+        ms = np.zeros(4, np.float32)
+        self._ck(self.lib.plstvo_orb_detect_kernel_times(self.ctx, _p(ms, T.c_float_p)))
         return ms
 
     def stereo_lift_lines(self, cam, scfg: T.PlStereoConfig, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, m12):

@@ -78,6 +78,20 @@ def default_orb_config(n_levels: int = 4, scale_factor: float = 1.2) -> "PlOrbCo
     return PlOrbConfig(n_levels, scale_factor, 19, 31, 2)   # config_kitti.yaml: 1 level
 
 
+class PlOrbDetectConfig(C.Structure):
+    """cv::ORB parameters of plstvo_orb_detect_and_compute_batch: score_type 1 FAST_SCORE, 0 HARRIS_SCORE."""
+    _fields_ = [("orb", PlOrbConfig), ("n_features", C.c_int32), ("score_type", C.c_int32), ("fast_threshold", C.c_int32)]
+
+
+ORB_HARRIS_SCORE, ORB_FAST_SCORE = 0, 1
+
+
+def default_orb_detect_config(n_features: int = 1200, n_levels: int = 4, scale_factor: float = 1.2,
+                              score_type: int = ORB_FAST_SCORE, fast_threshold: int = 20) -> "PlOrbDetectConfig":
+    """src/config.cpp:95-102 defaults: 1200 features, scale 1.2, 4 levels, edge 19, FAST score, patch 31, WTA_K 2, FAST 20."""
+    return PlOrbDetectConfig(default_orb_config(n_levels, scale_factor), n_features, score_type, fast_threshold)
+
+
 class PlStereoMatchConfig(C.Structure):
     """Grid / matcher values of matchStereoPoints / matchStereoLines (include/stereoFrame.h:51-52, src/config.cpp:51, :60, :63, :91)."""
     _fields_ = [("grid_rows", C.c_int32), ("grid_cols", C.c_int32), ("matching_s_ws", C.c_int32), ("best_lr_matches", C.c_int32),

@@ -46,4 +46,8 @@ t1 = eng.track_stereo_batch_async(scam, T.kitti_config(), mc, sc, pc, cc, ares, 
 t2 = eng.track_stereo_batch_async(scam, T.kitti_config(), mc, sc, pc, cc, ares, ans)
 eng.wait(t1)
 eng.wait(t2)
+orb_imgs = np.stack([synth_img % 251 for synth_img in (np.arange(160 * 120, dtype=np.int64).reshape(120, 160) * 37,
+                                                       np.arange(160 * 120, dtype=np.int64).reshape(120, 160) * 91)]).astype(np.uint8)
+for st in (T.ORB_FAST_SCORE, T.ORB_HARRIS_SCORE):
+    eng.orb_detect_and_compute_batch(T.default_orb_detect_config(300, score_type=st), orb_imgs, [10, 30])
 print("sanitized run ok", int(out["results"]["good"].sum()))
