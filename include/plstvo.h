@@ -399,17 +399,18 @@ void  plstvo_host_free(void* p);
 int64_t plstvo_launch_count(const PlContext* ctx);
 /* device time of the two kernels of one pass over the resident batch, each launched alone `iters` times
  * on the context's stream and bracketed by CUDA events on that stream: *ms_match / *ms_solve = average
- * duration of one K1 (hamming_knn2 over all tiles of the batch) / one K2 (track_solve, one CTA per pair)
- * launch.  n_tiles / n_pairs (optional) = CTAs per launch. */
+ * duration of one K1 (distance + top-2 and resolve kernels over the whole batch) / one K2 (track_solve, one CTA per
+ * pair) launch.  n_tiles (optional) = matching problems the matcher works on (feature type enabled, both sides
+ * non-empty); n_pairs (optional) = pairs. */
 int     plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, double* ms_match,
                                   double* ms_solve, int32_t* n_tiles, int32_t* n_pairs);
 /* The same per stage: ms[0] = the interval before the matcher (operands are expanded inside it: about 0), ms[1] = operand
- * expansion + distance + top-2 kernel (tensor-core form) or the integer K1 (PLSTVO_K1=popc: ms[0] = ms[2] = 0), ms[2] = index resolution, ms[3] = building matched_pt / matched_ls when that is a
+ * expansion + distance + top-2 kernel, ms[2] = index resolution, ms[3] = building matched_pt / matched_ls when that is a
  * kernel of its own (the streamed solver; 0 when K2 does it internally), ms[4] = optimizePose (K2, or the streamed solver's
  * GN-loop / outlier / finalize kernels + K2 for the problems it hands back); of ms[4], streamed solver only (0 for K2):
  * ms[5] = the GN loop launch of stage 1, ms[6] = the gate + removeOutliers launch, ms[7] = the GN loop launch of stage 2.
- * counts (optional) = {bit 0: tensor-core matcher, bit 1: streamed solver, bits 8..: problems the streamed solver handed to
- * the fp64 kernel in the last pass; work items (or tiles) of the distance kernel; matching problems; pairs}. */
+ * counts (optional) = {bit 0: tensor-core matcher (always set), bit 1: streamed solver, bits 8..: problems the streamed solver handed to
+ * the fp64 kernel in the last pass; work items of the distance kernel; matching problems; pairs}. */
 int     plstvo_batch_stage_times(PlContext* ctx, PlDeviceBatch* db, int iters, double ms[8], int32_t counts[4]);
 /* GN evaluation (optimizeFunctions, src/stereoFrameHandler.cpp:549-694) of the resident matched
  * lists at given poses, streamed from HBM: the roofline kernel of config C5.
@@ -429,8 +430,7 @@ int  plstvo_debug_select(PlContext* ctx, int n_lists, const int32_t* off, const 
  *   colp   [sum_p n2_p]: column words, best | second << 9 | tag << 18 (the consumer warp, = (row % 128) / 16, of the best);
  *   rowkey [sum_p n1_p][2], colkey [sum_p n2_p][2]: the resolved keys (dist << 16 | index, dist2 << 16 | 0xFFFE), or
  *          0xFFFFFFFF as the second key when the other side has fewer than 2 rows.
- * A problem with an empty side has no words; its slots are left unchanged.  Fails with PLSTVO_E_INVALID under PLSTVO_K1=popc
- * (the integer matcher has no such words). */
+ * A problem with an empty side has no words; its slots are left unchanged. */
 int  plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
                               const int32_t* off2, float nnr, uint32_t* rowp, uint32_t* colp, uint32_t* rowkey,
                               uint32_t* colkey);

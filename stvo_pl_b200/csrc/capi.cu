@@ -50,9 +50,7 @@ struct Workspace {
     std::vector<int32_t> p_off1, p_off2, l_off1, l_off2;
     // plan
     std::vector<MatchProblem> problems;   // [2B]: points, lines
-    std::vector<MatchTile> tiles;
-    std::vector<int32_t> tile_start;      // [B+1] first tile of each pair
-    int max_tsplit = 32, cap_pt = 0, cap_ls = 0, sort_cap = 1, max_n2 = 0;
+    int cap_pt = 0, cap_ls = 0, sort_cap = 1, max_n2 = 0;
     bool feat_in_smem = true;
     // device storage
     DevBuf d_poff1, d_poff2, d_loff1, d_loff2;
@@ -60,10 +58,9 @@ struct Workspace {
     DevBuf d_ptP, d_pts2, d_ptpl;                                      // prev P, prev sigma2, curr pl
     DevBuf d_lssP, d_lseP, d_lsspl, d_lsepl, d_lss2, d_lslev, d_lsle;  // prev ...; curr le
     DevBuf d_priors, d_results, d_m12p, d_m12l, d_inlp, d_inll;
-    DevBuf d_rowpart, d_colpart, d_problems, d_tiles, d_feat;
+    DevBuf d_rowpart, d_colpart, d_problems, d_feat;
     DevBuf d_phase;   // debug phase timers (PLSTVO_PHASE_DEBUG)
-    // tensor-core form of K1 (match_tc.cu): per-block value partials, work items
-    bool use_tc = true;
+    // K1 (match_tc.cu): per-block value partials, work items
     std::vector<TcProblem> tc_problems;   // [2B], parallel to `problems`
     std::vector<TcItem> tc_items[2];      // work items of the point problems (long) and of the line problems (short)
     std::vector<int32_t> item_start[2];   // [B+1] first work item of each pair in either list
@@ -75,7 +72,7 @@ struct Workspace {
         DevBuf* all[] = {&d_poff1, &d_poff2, &d_loff1, &d_loff2, &d_pdesc1, &d_pdesc2, &d_ldesc1, &d_ldesc2,
                          &d_ptP, &d_pts2, &d_ptpl, &d_lssP, &d_lseP, &d_lsspl, &d_lsepl, &d_lss2, &d_lslev,
                          &d_lsle, &d_priors, &d_results, &d_m12p, &d_m12l, &d_inlp, &d_inll, &d_rowpart,
-                         &d_colpart, &d_problems, &d_tiles, &d_feat, &d_phase, &d_tcprob, &d_tcitems[0],
+                         &d_colpart, &d_problems, &d_feat, &d_phase, &d_tcprob, &d_tcitems[0],
                          &d_tcitems[1], &d_rowp, &d_colp, &d_sched, &d_stream};
         for (DevBuf* b : all) b->release();
     }
@@ -220,39 +217,6 @@ StreamBufs stream_bufs_at(const StreamBufs& sb, int p0) {
 }
 
 // ---- planning -------------------------------------------------------------------------------------
-// target_ctas: how many K1 tiles we would like at least, so that small batches still fill the chip
-// PLSTVO_K1=popc selects the integer (XOR + POPC) form of K1; the default is the tensor-core form (match_tc.cu)
-bool k1_use_tc() {
-    static const bool tc = [] {
-        const char* v = getenv("PLSTVO_K1");
-        return !(v && !strcmp(v, "popc"));
-    }();
-    return tc;
-}
-
-void plan_problem(MatchProblem& pr, int n1, int n2, bool enabled, float nnr, int best_lr, int tsplit_hint, bool use_tc) {
-    pr.n1 = n1;
-    pr.n2 = n2;
-    pr.nnr = nnr;
-    pr.best_lr = best_lr;
-    pr.enabled = (enabled && n1 > 0 && n2 > 0) ? 1 : 0;   // src/stereoFrameHandler.cpp:137-138, :160-161
-    if (!pr.enabled) {
-        pr.nqb = pr.ntb = 0;
-        pr.tsplit = 32;
-        return;
-    }
-    if (use_tc) {   // tc_resolve_kernel leaves ONE merged partial per row and per column
-        pr.nqb = pr.ntb = 1;
-        pr.tsplit = 32;
-        return;
-    }
-    pr.nqb = (n1 + k1_queries_per_tile() - 1) / k1_queries_per_tile();
-    int ts = ((n2 + 31) / 32) * 32;
-    if (tsplit_hint > 0 && tsplit_hint < ts) ts = tsplit_hint;
-    pr.tsplit = ts;
-    pr.ntb = (n2 + ts - 1) / ts;
-}
-
 int validate_frames(PlContext* ctx, const PlFrameBatch* prev, const PlFrameBatch* curr, bool need_features) {
     if (!prev || !curr) return fail(ctx, PLSTVO_E_INVALID, "null frame batch");
     if (prev->B != curr->B) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold a different number of frames");
@@ -306,7 +270,6 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     }
     ws.planned = false;
     ws.B = B;
-    ws.use_tc = k1_use_tc();
     if (cam) ws.cam = *cam;
     ws.cfg = *cfg;
     ws.has_priors = has_priors;
@@ -316,75 +279,48 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     ws.l_off2.assign(curr->ls_off, curr->ls_off + B + 1);
     const size_t np1 = ws.p_off1[B], np2 = ws.p_off2[B], nl1 = ws.l_off1[B], nl2 = ws.l_off2[B];
 
-    // --- tile split: enough CTAs for a small batch, whole train sets per tile for a big one ---
-    long base_tiles = 0;
-    for (int p = 0; p < B; ++p) {
-        base_tiles += (ws.p_off1[p + 1] - ws.p_off1[p] + k1_queries_per_tile() - 1) / k1_queries_per_tile();
-        base_tiles += (ws.l_off1[p + 1] - ws.l_off1[p] + k1_queries_per_tile() - 1) / k1_queries_per_tile();
-    }
-    const long want = 3L * ctx->sm_count;   // about one full wave of resident K1 CTAs
-    int split = 1;
-    if (base_tiles > 0 && base_tiles < want) split = (int)((want + base_tiles - 1) / base_tiles);
-    // Big batches too: four train blocks per problem (tiles of 512 queries x ~n2/4 trains, at least 256).  Finer tiles shrink
-    // the tail of the last wave of CTAs (2560 tiles of 0.57 ms on 444 slots = 5.77 waves); measured on C2: K1 3.32 -> 3.12 ms,
-    // 129.0 -> 132.4 K solves/s, the blocking call 99 -> 109 K; beyond 4 the extra partials cost K2 more than K1 gains.
-    static const int forced_split = getenv("PLSTVO_K1_SPLIT") ? atoi(getenv("PLSTVO_K1_SPLIT")) : 0;   // tuning knob
-    split = forced_split > 0 ? forced_split : std::max(split, 4);
-
     ws.problems.assign((size_t)2 * B, MatchProblem{});
-    ws.tiles.clear();
-    ws.tile_start.assign((size_t)B + 1, 0);
-    ws.max_tsplit = 32;
+    ws.tc_problems.assign((size_t)2 * B, TcProblem{});
     ws.cap_pt = ws.cap_ls = 0;
     ws.max_n2 = 0;
     size_t row_elems = 0, col_elems = 0, rowp_elems = 0, colp_elems = 0;
-    ws.tc_problems.assign(ws.use_tc ? (size_t)2 * B : 0, TcProblem{});
     for (int k = 0; k < 2; ++k) {
         ws.tc_items[k].clear();
         ws.item_start[k].assign((size_t)B + 1, 0);
     }
     const float nnr_p = (float)cfg->min_ratio_12_p, nnr_l = (float)cfg->min_ratio_12_l;   // double -> float at the call
     for (int p = 0; p < B; ++p) {
-        ws.tile_start[p] = (int32_t)ws.tiles.size();
         ws.item_start[0][p] = (int32_t)ws.tc_items[0].size();
         ws.item_start[1][p] = (int32_t)ws.tc_items[1].size();
         for (int type = 0; type < 2; ++type) {
             MatchProblem& pr = ws.problems[(size_t)2 * p + type];
+            TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
             const int n1 = type ? ws.l_off1[p + 1] - ws.l_off1[p] : ws.p_off1[p + 1] - ws.p_off1[p];
             const int n2 = type ? ws.l_off2[p + 1] - ws.l_off2[p] : ws.p_off2[p + 1] - ws.p_off2[p];
-            int hint = 0;
-            if (split > 1) {
-                hint = ((n2 + split - 1) / split + 31) / 32 * 32;
-                if (hint < 256) hint = 256;
-            }
-            plan_problem(pr, n1, n2, type ? cfg->has_lines != 0 : cfg->has_points != 0, type ? nnr_l : nnr_p,
-                         cfg->best_lr_matches != 0, hint, ws.use_tc);
-            if (ws.use_tc) {
-                // partials as element indices first, fixed up after allocation
-                const int t2 = pr.enabled ? (n2 + TC_ROWS - 1) / TC_ROWS : 0;
-                TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
-                tp.n1 = n1;
-                tp.n2 = n2;
-                tp.rowp = reinterpret_cast<uint32_t*>(rowp_elems);
-                tp.colp = reinterpret_cast<uint32_t*>(colp_elems);
-                rowp_elems += (size_t)(pr.enabled ? (n2 + TC_CW - 1) / TC_CW : 0) * n1;
-                colp_elems += (size_t)(pr.enabled ? n2 : 0);
-                for (int yb = 0; yb < (t2 + 1) / 2; ++yb) ws.tc_items[type].push_back(TcItem{2 * p + type, yb});
-            }
+            const bool wanted = type ? cfg->has_lines != 0 : cfg->has_points != 0;
+            pr.n1 = tp.n1 = n1;
+            pr.n2 = tp.n2 = n2;
+            pr.nnr = type ? nnr_l : nnr_p;
+            pr.best_lr = cfg->best_lr_matches != 0;
+            pr.enabled = (wanted && n1 > 0 && n2 > 0) ? 1 : 0;   // src/stereoFrameHandler.cpp:137-138, :160-161
             // offsets into the partial buffers are stored as element indices first, fixed up after allocation
             pr.rowpart = reinterpret_cast<uint2*>(row_elems);
             pr.colpart = reinterpret_cast<uint2*>(col_elems);
-            row_elems += (size_t)pr.ntb * n1;
-            col_elems += (size_t)pr.nqb * n2;
-            for (int qb = 0; qb < pr.nqb; ++qb)
-                for (int tb = 0; tb < pr.ntb; ++tb) ws.tiles.push_back(MatchTile{2 * p + type, qb, tb});
-            if (pr.enabled) ws.max_tsplit = std::max(ws.max_tsplit, pr.tsplit);
+            tp.rowp = reinterpret_cast<uint32_t*>(rowp_elems);
+            tp.colp = reinterpret_cast<uint32_t*>(colp_elems);
+            if (pr.enabled) {
+                row_elems += (size_t)n1;
+                col_elems += (size_t)n2;
+                rowp_elems += (size_t)((n2 + TC_CW - 1) / TC_CW) * n1;
+                colp_elems += (size_t)n2;
+                const int t2 = (n2 + TC_ROWS - 1) / TC_ROWS;
+                for (int yb = 0; yb < (t2 + 1) / 2; ++yb) ws.tc_items[type].push_back(TcItem{2 * p + type, yb});
+            }
             ws.max_n2 = std::max(ws.max_n2, n2);
             if (type == 0) ws.cap_pt = std::max(ws.cap_pt, n1);
             else ws.cap_ls = std::max(ws.cap_ls, n1);
         }
     }
-    ws.tile_start[B] = (int32_t)ws.tiles.size();
     ws.item_start[0][B] = (int32_t)ws.tc_items[0].size();
     ws.item_start[1][B] = (int32_t)ws.tc_items[1].size();
     ws.cap_pt = std::max(ws.cap_pt, 1);
@@ -398,8 +334,6 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     // PLSTVO_MAX_FEATURES rows
     if (with_features && !ws.feat_in_smem && k2_smem_bytes(ws.cap_pt, ws.cap_ls, ws.sort_cap, false) > ctx->smem_optin)
         return fail(ctx, PLSTVO_E_TOO_LARGE, "frame too large for the per-pair solver's shared memory");
-    if (!ws.use_tc && k1_smem_bytes(ws.max_tsplit) > ctx->smem_optin)
-        return fail(ctx, PLSTVO_E_TOO_LARGE, "train set too large for one K1 tile");
 
     // --- device storage ---
     CK(ctx, ws.d_pdesc1.ensure(np1 * 32));
@@ -411,16 +345,13 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     CK(ctx, ws.d_rowpart.ensure(row_elems * sizeof(uint2)));
     CK(ctx, ws.d_colpart.ensure(col_elems * sizeof(uint2)));
     CK(ctx, ws.d_problems.ensure(ws.problems.size() * sizeof(MatchProblem)));
-    CK(ctx, ws.d_tiles.ensure(ws.tiles.size() * sizeof(MatchTile)));
-    if (ws.use_tc) {
-        CK(ctx, ws.d_rowp.ensure(rowp_elems * sizeof(uint32_t)));
-        CK(ctx, ws.d_colp.ensure(colp_elems * sizeof(uint32_t)));
-        CK(ctx, ws.d_tcprob.ensure(ws.tc_problems.size() * sizeof(TcProblem)));
-        for (int k = 0; k < 2; ++k) CK(ctx, ws.d_tcitems[k].ensure(ws.tc_items[k].size() * sizeof(TcItem)));
-        if (!ws.d_sched.p) {   // scheduler words of the persistent matcher: one pair per compute stream, self re-arming
-            CK(ctx, ws.d_sched.ensure(64));
-            CK(ctx, cudaMemsetAsync(ws.d_sched.p, 0, 64, ctx->s_h2d));
-        }
+    CK(ctx, ws.d_rowp.ensure(rowp_elems * sizeof(uint32_t)));
+    CK(ctx, ws.d_colp.ensure(colp_elems * sizeof(uint32_t)));
+    CK(ctx, ws.d_tcprob.ensure(ws.tc_problems.size() * sizeof(TcProblem)));
+    for (int k = 0; k < 2; ++k) CK(ctx, ws.d_tcitems[k].ensure(ws.tc_items[k].size() * sizeof(TcItem)));
+    if (!ws.d_sched.p) {   // scheduler words of the persistent matcher: one pair per compute stream, self re-arming
+        CK(ctx, ws.d_sched.ensure(64));
+        CK(ctx, cudaMemsetAsync(ws.d_sched.p, 0, 64, ctx->s_h2d));
     }
     if (with_features) {
         CK(ctx, ws.d_poff1.ensure((B + 1) * 4));
@@ -464,17 +395,15 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
                 pr.d2 = ws.d_ldesc2.as<uint8_t>() + (size_t)ws.l_off2[p] * 32;
                 pr.m12 = ws.d_m12l.as<int32_t>() + ws.l_off1[p];
             }
-            if (ws.use_tc) {
-                // the matcher expands the rows of the workspace's own 32-byte-row arenas (16-byte aligned loads)
-                TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
-                tp.d1 = pr.d1;
-                tp.d2 = pr.d2;
-                tp.rowp = ws.d_rowp.as<uint32_t>() + reinterpret_cast<size_t>(tp.rowp);
-                tp.colp = ws.d_colp.as<uint32_t>() + reinterpret_cast<size_t>(tp.colp);
-            }
+            // the matcher expands the rows of the workspace's own 32-byte-row arenas (16-byte aligned loads)
+            TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
+            tp.d1 = pr.d1;
+            tp.d2 = pr.d2;
+            tp.rowp = ws.d_rowp.as<uint32_t>() + reinterpret_cast<size_t>(tp.rowp);
+            tp.colp = ws.d_colp.as<uint32_t>() + reinterpret_cast<size_t>(tp.colp);
         }
     cudaStream_t s = ctx->s_h2d;
-    if (ws.use_tc && !ws.tc_problems.empty()) {
+    if (!ws.tc_problems.empty()) {
         CK(ctx, cudaMemcpyAsync(ws.d_tcprob.p, ws.tc_problems.data(), ws.tc_problems.size() * sizeof(TcProblem),
                                 cudaMemcpyHostToDevice, s));
         for (int k = 0; k < 2; ++k)
@@ -484,9 +413,6 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     }
     if (!ws.problems.empty())
         CK(ctx, cudaMemcpyAsync(ws.d_problems.p, ws.problems.data(), ws.problems.size() * sizeof(MatchProblem),
-                                cudaMemcpyHostToDevice, s));
-    if (!ws.tiles.empty())
-        CK(ctx, cudaMemcpyAsync(ws.d_tiles.p, ws.tiles.data(), ws.tiles.size() * sizeof(MatchTile),
                                 cudaMemcpyHostToDevice, s));
     if (with_features) {
         CK(ctx, cudaMemcpyAsync(ws.d_poff1.p, ws.p_off1.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
@@ -534,26 +460,17 @@ int ws_upload_range(PlContext* ctx, Workspace& ws, const PlFrameBatch* prev, con
 }
 
 int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t s, cudaEvent_t* marks = nullptr) {
-    if (ws.use_tc) {
-        const int a0 = ws.item_start[0][p0], a1 = ws.item_start[0][p1], b0 = ws.item_start[1][p0], b1 = ws.item_start[1][p1];
-        if (a1 > a0 || b1 > b0) {
-            if (marks) CK(ctx, cudaEventRecord(marks[0], s));   // operands are expanded inside the matcher: empty stage
-            // launches on the two compute streams may overlap: each has its own pair of scheduler words
-            int* sched = ws.d_sched.as<int>() + (s == ctx->s_alt ? 8 : 0);
-            CK(ctx, launch_tc_hamming(ws.d_tcprob.as<TcProblem>(), ws.d_tcitems[0].as<TcItem>() + a0, a1 - a0,
-                                      ws.d_tcitems[1].as<TcItem>() + b0, b1 - b0, sched, ctx->sm_count, s));
-            if (marks) CK(ctx, cudaEventRecord(marks[1], s));
-            CK(ctx, launch_tc_resolve(ws.d_problems.as<MatchProblem>() + (size_t)2 * p0, ws.d_tcprob.as<TcProblem>() + (size_t)2 * p0,
-                                      2 * (p1 - p0), 4, s));
-            ctx->launches += 2;
-        }
-        return 0;
-    }
-    const int t0 = ws.tile_start[p0], t1 = ws.tile_start[p1];
-    if (t1 > t0) {
-        CK(ctx, launch_hamming_knn2(ws.d_problems.as<MatchProblem>(), ws.d_tiles.as<MatchTile>() + t0, t1 - t0,
-                                    ws.max_tsplit, s));
-        ctx->launches++;
+    const int a0 = ws.item_start[0][p0], a1 = ws.item_start[0][p1], b0 = ws.item_start[1][p0], b1 = ws.item_start[1][p1];
+    if (a1 > a0 || b1 > b0) {
+        if (marks) CK(ctx, cudaEventRecord(marks[0], s));   // operands are expanded inside the matcher: empty stage
+        // launches on the two compute streams may overlap: each has its own pair of scheduler words
+        int* sched = ws.d_sched.as<int>() + (s == ctx->s_alt ? 8 : 0);
+        CK(ctx, launch_tc_hamming(ws.d_tcprob.as<TcProblem>(), ws.d_tcitems[0].as<TcItem>() + a0, a1 - a0,
+                                  ws.d_tcitems[1].as<TcItem>() + b0, b1 - b0, sched, ctx->sm_count, s));
+        if (marks) CK(ctx, cudaEventRecord(marks[1], s));
+        CK(ctx, launch_tc_resolve(ws.d_problems.as<MatchProblem>() + (size_t)2 * p0, ws.d_tcprob.as<TcProblem>() + (size_t)2 * p0,
+                                  2 * (p1 - p0), 4, s));
+        ctx->launches += 2;
     }
     return 0;
 }
@@ -621,28 +538,20 @@ int ws_download_range(PlContext* ctx, Workspace& ws, int p0, int p1, PlPoseResul
     return 0;
 }
 
+// Pairs per chunk of the resident pass and of a pipelined end-to-end step: the whole batch up to one pair per SM, beyond that
+// two halves (two launches per pass: measured best).
+int pass_chunk(int B, int sm_count) { return std::max(1, std::max(std::min(B, sm_count), (B + 1) / 2)); }
+
 // Pipeline chunking of the host-buffer entry point: small first chunks (the GPU starts working after a few MB have
 // crossed PCIe), then chunks of about two thirds of the SM count in pairs (K2 runs one pair per SM; the rest of the
 // chip keeps running the next chunk's distance tiles on the other compute stream).
 // With batches in flight behind one another (plstvo_track_batch_async) the previous batch's kernels already hide the copy:
 // no ramp, the resident pass's chunking (two launches per pass) is used instead.
 std::vector<int> chunk_schedule(int B, int sm_count, bool pipelined) {
-    static const int forced = getenv("PLSTVO_E2E_CHUNK") ? atoi(getenv("PLSTVO_E2E_CHUNK")) : 0;
     std::vector<int> bounds{0};
-    if (forced > 0 || pipelined) {
-        const int step = forced > 0 ? forced : std::max(1, std::max(std::min(B, sm_count), (B + 1) / 2));
+    if (pipelined) {
+        const int step = pass_chunk(B, sm_count);
         for (int p = step; p < B; p += step) bounds.push_back(p);
-        bounds.push_back(B);
-        return bounds;
-    }
-    const char* list = getenv("PLSTVO_E2E_BOUNDS");         // tuning knob: explicit chunk ends, e.g. "74,293"
-    if (list && *list) {
-        for (const char* c = list; *c;) {
-            const int v = atoi(c);
-            if (v > bounds.back() && v < B) bounds.push_back(v);
-            while (*c && *c != ',') ++c;
-            if (*c == ',') ++c;
-        }
         bounds.push_back(B);
         return bounds;
     }
@@ -660,17 +569,11 @@ std::vector<int> chunk_schedule(int B, int sm_count, bool pipelined) {
     return bounds;
 }
 
-int run_chunk(const Workspace& ws, int sm_count) {
-    static const int forced = getenv("PLSTVO_RUN_CHUNK") ? atoi(getenv("PLSTVO_RUN_CHUNK")) : 0;
-    if (forced > 0) return forced;
-    return std::max(1, std::max(std::min(ws.B, sm_count), (ws.B + 1) / 2));   // two launches per pass (measured best)
-}
-
 // resident pass: K1 / K2 over the whole batch, chunked over two streams so that the (latency-bound) per-pair
 // solver of chunk i overlaps the (throughput-bound) distance tiles of chunk i+1
 int ws_run(PlContext* ctx, Workspace& ws, bool have_level) {
     if (ws.B == 0) return 0;
-    const int chunk = run_chunk(ws, ctx->sm_count);
+    const int chunk = pass_chunk(ws.B, ctx->sm_count);
     cudaEvent_t start = next_event(ctx);
     CK(ctx, cudaEventRecord(start, ctx->s_main));
     CK(ctx, cudaStreamWaitEvent(ctx->s_alt, start, 0));
@@ -794,7 +697,7 @@ int64_t plstvo_launch_count(const PlContext* ctx) { return ctx ? ctx->launches :
 
 // ---- matching.h surface -------------------------------------------------------------------------------
 // Plans the B problems of a plstvo_match_batch call as a points-only frame batch on ctx->ws, uploads them and enqueues K1
-// (distance + top-2, resolve; or the integer form) on ctx->s_main.  The caller holds the lock, has validated B > 0
+// (distance + top-2, resolve) on ctx->s_main.  The caller holds the lock, has validated B > 0
 // and selected the device; on success ws.problems[2 p] is problem p, its partial keys pending on ctx->s_main.
 static int match_batch_launch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
                               const int32_t* off2, float nnr, int best_lr_matches) {
@@ -880,8 +783,6 @@ int plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const int
     LOCK(ctx);
     if (B < 0 || (B > 0 && (!off1 || !off2 || !rowp || !colp || !rowkey || !colkey)))
         return fail(ctx, PLSTVO_E_INVALID, "bad arguments");
-    if (!k1_use_tc())
-        return fail(ctx, PLSTVO_E_INVALID, "PLSTVO_K1=popc selects the integer matcher, which has no tensor-core partial words");
     if (B == 0) return 0;
     CK(ctx, cudaSetDevice(ctx->device));
     int rc = match_batch_launch(ctx, B, d1, off1, d2, off2, nnr, 1);
@@ -1773,7 +1674,7 @@ int plstvo_track_batch_async(PlContext* ctx, const PlCamera* cam, const PlConfig
     if (!ctx->slot_done[slot]) CK(ctx, cudaEventCreateWithFlags(&ctx->slot_done[slot], cudaEventDisableTiming));
     if (prev->B > 0) {
         rc = track_enqueue(ctx, ctx->ws_async[slot], cam, cfg, prev, curr, priors, results, m12_pt, m12_ls, inlier_pt,
-                           inlier_ls, getenv("PLSTVO_ASYNC_RAMP") == nullptr);
+                           inlier_ls, true);
         if (rc) return rc;
     }
     CK(ctx, cudaEventRecord(ctx->slot_done[slot], ctx->s_d2h));
@@ -1922,7 +1823,8 @@ int plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, doub
     }
     if (ms_match) *ms_match = tm / iters;
     if (ms_solve) *ms_solve = tsv / iters;
-    if (n_tiles) *n_tiles = (int32_t)ws.tiles.size();
+    if (n_tiles) *n_tiles = (int32_t)std::count_if(ws.problems.begin(), ws.problems.end(),
+                                                   [](const MatchProblem& pr) { return pr.enabled != 0; });
     if (n_pairs) *n_pairs = ws.B;
     return 0;
 }
@@ -1939,10 +1841,8 @@ int plstvo_batch_stage_times(PlContext* ctx, PlDeviceBatch* db, int iters, doubl
     double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     for (int i = 0; i < iters; ++i) {
         CK(ctx, cudaEventRecord(ev[0], ctx->s_main));
-        if (!ws.use_tc) CK(ctx, cudaEventRecord(ev[1], ctx->s_main));   // the integer form is one kernel: reported in slot 1
-        int rc = ws_launch_match(ctx, ws, 0, ws.B, ctx->s_main, ws.use_tc ? &ev[1] : nullptr);
+        int rc = ws_launch_match(ctx, ws, 0, ws.B, ctx->s_main, &ev[1]);
         if (rc) return rc;
-        if (!ws.use_tc) CK(ctx, cudaEventRecord(ev[2], ctx->s_main));
         CK(ctx, cudaEventRecord(ev[3], ctx->s_main));
         rc = ws_launch_solve(ctx, ws, 0, ws.B, ws.have_level, ctx->s_main, &ev[4]);
         if (rc) return rc;
@@ -1970,8 +1870,8 @@ int plstvo_batch_stage_times(PlContext* ctx, PlDeviceBatch* db, int iters, doubl
             CK(ctx, cudaMemcpy(act.data(), sb.active, (size_t)ws.B * sizeof(int32_t), cudaMemcpyDeviceToHost));
             for (int32_t a : act) delegated += a != 0;
         }
-        counts[0] = (ws.use_tc ? 1 : 0) | (ws.use_stream ? 2 : 0) | (delegated << 8);
-        counts[1] = ws.use_tc ? (int32_t)(ws.tc_items[0].size() + ws.tc_items[1].size()) : (int32_t)ws.tiles.size();
+        counts[0] = 1 | (ws.use_stream ? 2 : 0) | (delegated << 8);   // bit 0: the tensor-core matcher, the only form
+        counts[1] = (int32_t)(ws.tc_items[0].size() + ws.tc_items[1].size());
         counts[2] = (int32_t)ws.problems.size();
         counts[3] = ws.B;
     }

@@ -17,8 +17,8 @@
 //                      (which chunk group / lane / warp the best came from);
 //   tc_resolve_kernel  merges the per-block partials, converts to distances and recovers the best neighbour's index by
 //                      re-evaluating the few tagged candidates with XOR + POPC (exact; ties resolved to the lowest index
-//                      as OpenCV does), emitting the same packed keys (dist << 16 | index) K1's popcount form emits, so
-//                      everything downstream (ratio test, mutual filter, K2) is unchanged.
+//                      as OpenCV does), emitting the packed keys (dist << 16 | index) that everything
+//                      downstream (ratio test, mutual filter, K2) reads.
 // Integer-exact end to end: the bit-exact parity tests of the matcher are the acceptance test.
 #include <cuda_fp16.h>
 

@@ -33,7 +33,7 @@ size_t tc_smem_bytes();
 // items_a then items_b form the work list (long items first); sched: two zeroed ints per concurrently running launch
 cudaError_t launch_tc_hamming(const TcProblem* problems, const TcItem* items_a, int n_a, const TcItem* items_b, int n_b,
                               int* sched, int grid, cudaStream_t stream);
-// writes MatchProblem::rowpart[0][n1] / colpart[0][n2] (ntb = nqb = 1) in K1's packed-key format
+// writes MatchProblem::rowpart[n1] / colpart[n2]: one resolved key pair per row and per column (dist << 16 | index)
 cudaError_t launch_tc_resolve(const MatchProblem* mps, const TcProblem* tps, int n_problems, int slices, cudaStream_t stream);
 
 }  // namespace plstvo

@@ -1452,7 +1452,7 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
     const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nth >> 5;
     const PlConfig& cfg = prm.cfg;
     if (prm.mode == 0) {
-        // ---- A. finish the matching: merge partials, ratio test, mutual filter -> m12 (global) ----
+        // ---- A. finish the matching: ratio test, mutual filter -> m12 (global) ----
         const MatchProblem pp = prm.problems[2 * pair], pl = prm.problems[2 * pair + 1];
         match_finalize_block(pp, reinterpret_cast<uint16_t*>(sortbuf));
         __syncthreads();

@@ -130,10 +130,8 @@ def test_track_batch_accepted_ties(engine, oracle):
 
 
 def test_selected_matcher_form(engine):
-    """PLSTVO_K1=popc selects the integer matcher (and PLSTVO_K1_VARIANT its queries per thread); anything else the tensor-core
-    form.  Asserted on the plan a resident batch reports, so that a run under either switch proves which matcher it tested."""
-    from stvo_pl_b200.engine import PlstvoError
-    popc = os.environ.get("PLSTVO_K1") == "popc"
+    """The tensor-core matcher is the one that runs: asserted on the plan a resident batch reports (its form and its work items,
+    one per 256-train block) and on the shapes of the matcher's intermediate words."""
     prev, curr, _, cam = synth.make_batch("kitti", 2, n_pt=600, n_ls=150)
     cfg = T.kitti_config()
     db = engine.upload(cam, cfg, prev, curr)
@@ -141,21 +139,11 @@ def test_selected_matcher_form(engine):
         st = db.stage_times(iters=1)
     finally:
         db.free()
-    assert st["tensor_core_form"] is (not popc)
-    n1 = np.concatenate([np.diff(prev.pt_off), np.diff(prev.ls_off)])
+    assert st["tensor_core_form"] is True
     n2 = np.concatenate([np.diff(curr.pt_off), np.diff(curr.ls_off)])
-    if popc:
-        # integer form: one tile per (query block, train block); a batch this small is split into train blocks of 256
-        qpt = 256 * (4 if os.environ.get("PLSTVO_K1_VARIANT", "")[:1] == "4" else 2)
-        assert st["n_items"] == int(((n1 + qpt - 1) // qpt * ((n2 + 255) // 256)).sum())
-        d = np.zeros((4, 32), np.uint8)
-        with pytest.raises(PlstvoError) as ei:
-            engine.debug_tc_partials(d, [0, 4], d, [0, 4], 0.9)
-        assert ei.value.code == -1
-    else:
-        assert st["n_items"] == int(((n2 + 255) // 256).sum())   # work items: 256-train blocks
-        rowp, colp, rowkey, colkey = engine.debug_tc_partials(prev.pdesc[:5], [0, 5], curr.pdesc[:3], [0, 3], 0.9)
-        assert len(rowp) == 5 and len(colp) == 3 and rowkey.shape == (5, 2) and colkey.shape == (3, 2)
+    assert st["n_items"] == int(((n2 + 255) // 256).sum())   # work items: 256-train blocks
+    rowp, colp, rowkey, colkey = engine.debug_tc_partials(prev.pdesc[:5], [0, 5], curr.pdesc[:3], [0, 3], 0.9)
+    assert len(rowp) == 5 and len(colp) == 3 and rowkey.shape == (5, 2) and colkey.shape == (3, 2)
 
 
 def test_match_full_size_properties(engine):

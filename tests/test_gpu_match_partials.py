@@ -8,15 +8,12 @@ and requires them to equal the reference, and every unique-best tag to name the 
 
 The grid below runs as one batch call of about 600 work items (more than four per SM), so every CTA of the persistent kernel
 wraps its work-item ring and carries its query-stage phase and train-buffer parity across items of mixed lengths."""
-import os
-
 import numpy as np
 import pytest
 
 import ref_match as R
 
-pytestmark = [pytest.mark.gpu,
-              pytest.mark.skipif(os.environ.get("PLSTVO_K1") == "popc", reason="the integer matcher has no partial words")]
+pytestmark = pytest.mark.gpu
 
 # query tiles are 128 rows (two warpgroups of 64); 640 and 1025 rows are more tiles than the 4 query stages
 N1 = (1, 2, 63, 64, 65, 127, 128, 129, 255, 256, 257, 640, 1025)
