@@ -173,13 +173,16 @@ __device__ __forceinline__ uint64_t tc_desc(uint32_t saddr) {
 }
 
 // issues one 128-train half of a query tile into accumulator set d as one commit group: 8 K-steps (two 128-byte slabs x
-// four k32).  xa: the warpgroup's 64 query rows of the stage (slab 0); yb: the half's train tile in slab 0 of the train block
+// four k32).  xa: the warpgroup's 64 query rows of the stage (slab 0); yb: the half's train tile in slab 0 of the train block.
+// The K-steps' descriptors are the first one's plus a constant: shared addresses stay below 2^18, so the 14-bit start
+// address field (address >> 4) never carries into the next field.
 __device__ __forceinline__ void wg_issue_half(uint32_t (&d)[32], uint32_t xa, uint32_t yb) {
+    const uint64_t da = tc_desc(xa), db = tc_desc(yb);
     wg_fence_regs(d);
     wg_fence();
 #pragma unroll
     for (int kk = 0; kk < 8; ++kk)
-        wg_mma_f8(d, tc_desc(xa + (kk >> 2) * 16384 + (kk & 3) * 32), tc_desc(yb + (kk >> 2) * 32768 + (kk & 3) * 32), kk > 0);
+        wg_mma_f8(d, da + (((kk >> 2) * 16384 + (kk & 3) * 32) >> 4), db + (((kk >> 2) * 32768 + (kk & 3) * 32) >> 4), kk > 0);
     wg_commit();
 }
 
@@ -327,7 +330,9 @@ tc_hamming_kernel(const TcProblem* __restrict__ problems, const TcItem* __restri
         // The 256 trains are two halves of 128 (wgmma m64n128k32), one accumulator set each, software-pipelined so that
         // each half of a tile is folded while the MMA of the next half (t, 1) or (t + 1, 0) is on the tensor pipe.
         setmaxnreg_inc<TC_CONSUMER_REGS>();
-        const int wg = warp >> 2, w = warp & 3, q4 = lane & 3, rl = lane >> 2;
+        // the warpgroup index through a shuffle from lane 0: ptxas then knows it is warp-uniform and keeps the operand
+        // addresses and wgmma descriptors derived from it in uniform registers, off the vector ALU the fold saturates
+        const int wg = __shfl_sync(0xFFFFFFFFu, warp >> 2, 0), w = warp & 3, q4 = lane & 3, rl = lane >> 2;
         uint32_t* mrg = reinterpret_cast<uint32_t*>(sm + TC_OFF_MRG);
         uint32_t acc[2][32];
 #pragma unroll
