@@ -339,6 +339,21 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
  * non-max suppression, [2] selection (retainBest, Harris), [3] angles and descriptors. */
 int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4);
 
+/* ---- LBD line description: BinaryDescriptor::compute of given key lines ---- */
+/* BinaryDescriptor::compute (3rdparty/line_descriptor/src/binary_descriptor_custom.cpp:539-687, default Params: 9 bands of
+ * width 7, one octave) of octave-0 key lines on n_img grey images of one size (images: [n_img][height][width] uint8),
+ * bit-identical to the reference evaluated unfused.  Image i's lines are rows kl_off[i] .. kl_off[i + 1] of kl_seg ([n][4]
+ * float sPointInOctaveX, sPointInOctaveY, ePointInOctaveX, ePointInOctaveY), kl_angle ([n] KeyLine::angle, radians) and
+ * kl_npix ([n] KeyLine::numOfPixels); out_desc [n][32] (the layout PlStereoFeatures::ldesc_l / ldesc_r take).  Row i is
+ * line i's descriptor (KeyLine::class_id is not read).  An image without lines writes nothing.  Returns the number of
+ * lines.  PLSTVO_E_INVALID: a null pointer where lines exist, width or height outside 1..32767, a numOfPixels outside
+ * 1..32767, or offsets that do not start at 0 or decrease; PLSTVO_E_TOO_LARGE: more than PLSTVO_MAX_FEATURES lines in one
+ * image. */
+int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, const uint8_t* images, const int32_t* kl_off,
+                             const float* kl_seg, const float* kl_angle, const int32_t* kl_npix, uint8_t* out_desc);
+/* Device time of the last plstvo_lbd_compute_batch on this context, ms: [0] blur and Sobel, [1] descriptors. */
+int plstvo_lbd_kernel_times(PlContext* ctx, float* ms2);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

@@ -164,6 +164,23 @@ inline int detectAndComputeORB(Context& c, const PlOrbDetectConfig& cfg, const u
         return n;
     }
 }
+// LBD description of given octave-0 key lines (BinaryDescriptor::compute, default Params) on one grey image (row-major,
+// width * height bytes), as StereoFrame::detectLineFeatures calls it after LSD (src/stereoFrame.cpp:242).  kl.seg (start
+// and end point in the image) and kl.angle are read with num_pixels ([m] KeyLine::numOfPixels); kl.desc is replaced by the
+// m descriptors, row i for line i.  Returns m; throws Error(PLSTVO_E_INVALID) when the three arrays do not describe the same
+// m lines.
+inline int computeLBD(Context& c, const uint8_t* image, int width, int height, KeyLines& kl,
+                      const std::vector<int32_t>& num_pixels) {
+    const int n = (int)(kl.seg.size() / 4);
+    if (kl.seg.size() % 4 != 0 || kl.angle.size() != (size_t)n || num_pixels.size() != (size_t)n)
+        throw Error(PLSTVO_E_INVALID, "computeLBD: kl.seg must hold 4 floats per line, kl.angle and num_pixels one entry per line");
+    const int32_t off[2] = {0, n};
+    std::vector<uint8_t> desc(32 * (size_t)n);
+    const int k = c.check(plstvo_lbd_compute_batch(c.get(), 1, width, height, image, off, kl.seg.data(), kl.angle.data(),
+                                                   num_pixels.data(), desc.data()));
+    kl.desc = std::move(desc);
+    return k;
+}
 inline int matchStereoLines(Context& c, const PlCamera& cam, const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
                             const KeyLines& l, const KeyLines& r, StereoFrame& out) {
     const int n = l.size();

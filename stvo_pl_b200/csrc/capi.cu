@@ -107,6 +107,9 @@ struct PlContext {
     DevBuf arena_orb_kp;   // plstvo_orb_detect_and_compute_batch: per-key-point arrays, sized once the selection is counted
     bool orb_computed = false, orb_detected = false;
     cudaEvent_t orb_det_ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+    DevBuf arena_lbd;      // plstvo_lbd_compute_batch: images, gradients, key lines, descriptors
+    bool lbd_tables = false, lbd_computed = false;
+    cudaEvent_t lbd_ev[3] = {nullptr, nullptr, nullptr};
     // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
     void* h_staging[3] = {nullptr, nullptr, nullptr};
     size_t h_staging_bytes[3] = {0, 0, 0};
@@ -646,6 +649,9 @@ void plstvo_destroy(PlContext* ctx) {
     for (cudaEvent_t e : ctx->orb_ev)
         if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->orb_det_ev)
+        if (e) cudaEventDestroy(e);
+    ctx->arena_lbd.release();
+    for (cudaEvent_t e : ctx->lbd_ev)
         if (e) cudaEventDestroy(e);
     for (cudaEvent_t e : ctx->events) cudaEventDestroy(e);
     for (void* h : ctx->h_staging)
@@ -2221,6 +2227,94 @@ int plstvo_orb_kernel_times(PlContext* ctx, float* ms3) {
     if (!ctx->orb_computed) return fail(ctx, PLSTVO_E_INVALID, "no ORB call on this context yet");
     CK(ctx, cudaSetDevice(ctx->device));
     for (int k = 0; k < 3; ++k) CK(ctx, cudaEventElapsedTime(&ms3[k], ctx->orb_ev[k], ctx->orb_ev[k + 1]));
+    return 0;
+}
+
+/* ---- LBD description (lbd.cu) ---- */
+namespace {
+cudaError_t lbd_init(PlContext* ctx) {   // coefficient tables and timing events, once per context
+    if (ctx->lbd_tables) return cudaSuccess;
+    // BinaryDescriptor's constructor (binary_descriptor_custom.cpp:217-259) with widthOfBand_ 7, NUM_OF_BANDS 9: the
+    // centres and sigmas are integer divisions, the weights exp() in double, rounded to float where computeLBD reads them
+    float coef_l[21], coef_g[63];
+    double u = (7 * 3 - 1) / 2, sigma = (7 * 2 + 1) / 2, invsigma2 = -1 / (2 * sigma * sigma);
+    for (int i = 0; i < 21; ++i) {
+        const double dis = i - u;
+        coef_l[i] = (float)exp(dis * dis * invsigma2);
+    }
+    u = (9 * 7 - 1) / 2;
+    sigma = u;
+    invsigma2 = -1 / (2 * sigma * sigma);
+    for (int i = 0; i < 63; ++i) {
+        const double dis = i - u;
+        coef_g[i] = (float)exp(dis * dis * invsigma2);
+    }
+    cudaError_t e = lbd_upload_tables(coef_g, coef_l);
+    for (auto& ev : ctx->lbd_ev)
+        if (e == cudaSuccess) e = cudaEventCreate(&ev);
+    if (e == cudaSuccess) ctx->lbd_tables = true;
+    return e;
+}
+}  // namespace
+
+int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, const uint8_t* images, const int32_t* kl_off,
+                             const float* kl_seg, const float* kl_angle, const int32_t* kl_npix, uint8_t* out_desc) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (n_img < 0) return fail(ctx, PLSTVO_E_INVALID, "negative n_img");
+    // the reference indexes pixels and counts samples in short
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+    if (n_img == 0) return 0;
+    if (!kl_off || kl_off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null offsets or kl_off[0] != 0");
+    for (int i = 0; i < n_img; ++i) {
+        const int n = kl_off[i + 1] - kl_off[i];
+        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kl_off is not non-decreasing");
+        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+    }
+    const size_t N = (size_t)kl_off[n_img];
+    if (N == 0) return 0;
+    if (!images || !kl_seg || !kl_angle || !kl_npix || !out_desc) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
+    for (size_t k = 0; k < N; ++k)
+        if (kl_npix[k] < 1 || kl_npix[k] > 32767) return fail(ctx, PLSTVO_E_INVALID, "numOfPixels must be 1..32767");
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, lbd_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height;
+    LiftArena a;
+    const size_t o_img = a.take(img_bytes), o_grad = a.take(img_bytes * 4), o_off = a.take((size_t)(n_img + 1) * 4);
+    const size_t o_seg = a.take(N * 16), o_dir = a.take(N * 8), o_npix = a.take(N * 4), o_desc = a.take(N * 32);
+    DevBuf& arena = ctx->arena_lbd;
+    CK(ctx, arena.ensure(a.off));
+    uint8_t* base = arena.as<uint8_t>();
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, cudaMemcpyAsync(base + o_img, images, img_bytes, cudaMemcpyHostToDevice, s));
+    CK(ctx, cudaMemcpyAsync(base + o_off, kl_off, (size_t)(n_img + 1) * 4, cudaMemcpyHostToDevice, s));
+    CK(ctx, cudaMemcpyAsync(base + o_seg, kl_seg, N * 16, cudaMemcpyHostToDevice, s));
+    // dL = (cos, sin) of the float angle.  The reference's unqualified cos(float) / sin(float) bind to std::cos(float) /
+    // std::sin(float), the C library's cosf / sinf (its translation unit includes <math.h>, whose C++ form puts the float
+    // overloads into the global namespace), and GCC merges the pair into sincosf.  They are evaluated here, with the same
+    // library, because no device function rounds them the same way.
+    std::vector<float> dir(2 * N);
+    for (size_t k = 0; k < N; ++k) sincosf(kl_angle[k], &dir[2 * k + 1], &dir[2 * k]);
+    CK(ctx, cudaMemcpyAsync(base + o_dir, dir.data(), N * 8, cudaMemcpyHostToDevice, s));
+    CK(ctx, cudaMemcpyAsync(base + o_npix, kl_npix, N * 4, cudaMemcpyHostToDevice, s));
+    int launches = 0;
+    CK(ctx, launch_lbd(n_img, width, height, base + o_img, reinterpret_cast<const int32_t*>(base + o_off), (int)N,
+                       reinterpret_cast<const float*>(base + o_seg), reinterpret_cast<const float2*>(base + o_dir),
+                       reinterpret_cast<const int32_t*>(base + o_npix), reinterpret_cast<short2*>(base + o_grad),
+                       base + o_desc, s, ctx->lbd_ev, &launches));
+    ctx->lbd_computed = true;
+    ctx->launches += launches;
+    CK(ctx, cudaMemcpyAsync(out_desc, base + o_desc, N * 32, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return (int)N;
+}
+
+int plstvo_lbd_kernel_times(PlContext* ctx, float* ms2) {
+    if (!ctx || !ms2) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->lbd_computed) return fail(ctx, PLSTVO_E_INVALID, "no LBD call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 2; ++k) CK(ctx, cudaEventElapsedTime(&ms2[k], ctx->lbd_ev[k], ctx->lbd_ev[k + 1]));
     return 0;
 }
 

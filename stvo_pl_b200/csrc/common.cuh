@@ -237,6 +237,12 @@ void launch_orb_harris_write(const OrbDevLevels& L, const OrbDetectLevels& D, in
                              const int32_t* out_off, float* out_xy, int32_t* out_oct, float* out_resp, int32_t* out_rank,
                              cudaStream_t s, int* launches);
 
+// lbd.cu: LBD descriptors of given octave-0 key lines (BinaryDescriptor::compute, default Params) on a batch of images
+cudaError_t lbd_upload_tables(const float* coef_g, const float* coef_l);   // (float)gaussCoefG_ [63], (float)gaussCoefL_ [21]
+cudaError_t launch_lbd(int n_img, int W, int H, const uint8_t* images, const int32_t* kl_off, int n_lines, const float* seg,
+                       const float2* dir, const int32_t* npix, short2* grad, uint8_t* out_desc, cudaStream_t s,
+                       cudaEvent_t* ev, int* launches);   // dir: (cosf, sinf) of each angle; ev[0..2]: start, gradients, descriptors
+
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);
 int gn_stream_partials_per_slice();   // fp64 partial records one slice writes (one per consumer warp)   // 16 KB tiles of one problem (512 points or 256 lines each)

@@ -95,6 +95,8 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_orb_detect_and_compute_batch": (C.c_int, [vp, C.POINTER(T.PlOrbDetectConfig), C.c_int, C.c_int, C.c_int, u8p,
                                                           i32p, C.c_int, i32p, fp, i32p, fp, fp, u8p]),
         "plstvo_orb_detect_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_lbd_compute_batch": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, u8p, i32p, fp, fp, i32p, u8p]),
+        "plstvo_lbd_kernel_times": (C.c_int, [vp, fp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -114,7 +116,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
-    "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times"]
+    "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
+    "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -390,6 +393,28 @@ class Engine:
         angles + descriptors."""
         ms = np.zeros(4, np.float32)
         self._ck(self.lib.plstvo_orb_detect_kernel_times(self.ctx, _p(ms, T.c_float_p)))
+        return ms
+
+    def lbd_compute_batch(self, images, kl_off, kl_seg, kl_angle, kl_npix):
+        """LBD descriptors (BinaryDescriptor::compute, default Params) of octave-0 key lines on images uint8[n, H, W].  Image
+        i's lines are rows kl_off[i] .. kl_off[i + 1] of kl_seg ([m, 4] float sPointInOctaveX, sPointInOctaveY,
+        ePointInOctaveX, ePointInOctaveY), kl_angle ([m] radians) and kl_npix ([m] numOfPixels).  Returns desc uint8[m, 32],
+        row i being line i's descriptor."""
+        images = np.ascontiguousarray(images, np.uint8)
+        n_img, H, W = images.shape
+        kl_off = np.ascontiguousarray(kl_off, np.int32)
+        kl_seg = np.ascontiguousarray(kl_seg, np.float32).reshape(-1, 4)
+        kl_angle, kl_npix = np.ascontiguousarray(kl_angle, np.float32), np.ascontiguousarray(kl_npix, np.int32)
+        desc = np.zeros((len(kl_seg), 32), np.uint8)
+        self._ck(self.lib.plstvo_lbd_compute_batch(
+            self.ctx, n_img, W, H, _p(images, T.c_uint8_p), _p(kl_off, T.c_int32_p), _p(kl_seg, T.c_float_p),
+            _p(kl_angle, T.c_float_p), _p(kl_npix, T.c_int32_p), _p(desc, T.c_uint8_p)))
+        return desc
+
+    def lbd_kernel_times(self):
+        """Device ms of the last lbd_compute_batch: blur + Sobel, descriptors."""
+        ms = np.zeros(2, np.float32)
+        self._ck(self.lib.plstvo_lbd_kernel_times(self.ctx, _p(ms, T.c_float_p)))
         return ms
 
     def stereo_lift_lines(self, cam, scfg: T.PlStereoConfig, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, m12):
