@@ -354,6 +354,49 @@ int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, c
 /* Device time of the last plstvo_lbd_compute_batch on this context, ms: [0] blur and Sobel, [1] descriptors. */
 int plstvo_lbd_kernel_times(PlContext* ctx, float* ms2);
 
+/* ---- stereo images in, pose out: StereoFrame::extractStereoFeatures (src/stereoFrame.cpp:59-118, :182-243) with LSD left
+ * to the caller, then matchStereoPoints / matchStereoLines, f2fTracking and optimizePose ---- */
+typedef struct PlStereoImages {
+    int32_t        B;                                  /* frames */
+    int32_t        width, height;                      /* every image; must equal cam->width / height */
+    const uint8_t* img_l;  const uint8_t* img_r;       /* [B][height][width] grey, row-major */
+    const int32_t* fast_th;                            /* [B] or NULL; per frame, both images; 0 = ocfg->fast_threshold (:109-111) */
+    const int32_t* ll_off; const int32_t* lr_off;      /* [B+1] key lines (octave 0) of the left / right images */
+    const float*   seg_l;  const float*   seg_r;       /* [m][4] sPointInOctave{X,Y}, ePointInOctave{X,Y} (= start/end point at octave 0) */
+    const float*   angle_l; const float*  angle_r;     /* KeyLine::angle */
+    const int32_t* npix_l; const int32_t* npix_r;      /* KeyLine::numOfPixels */
+} PlStereoImages;
+/* Results and n_stereo equal, byte for byte, what the same inputs give through the three calls
+ *   1. plstvo_orb_detect_and_compute_batch on all images, frame f's threshold applied to both of its images;
+ *   2. plstvo_lbd_compute_batch on all key lines;
+ *   3. plstvo_track_stereo_batch / _sequence on the resulting PlStereoFeatures, with loct_l all 0;
+ * but images and key lines go up once and no feature data comes back: ORB's key points and descriptors and LBD's descriptors
+ * stay in HBM and feed the stereo step directly.  The host hops after the uploads are ORB's per-image key-point counts (one
+ * readback, two under HARRIS_SCORE), the stereo step's survivor counts, and the results.  The sequence form detects and
+ * describes each frame's images once.
+ * cfg->has_points == 0: ORB does not run (detectStereoPoints returns early in the reference too) and the frames have no key
+ * points.  cfg->has_lines == 0: LBD does not run, the frames have no key lines, and every line array may be NULL.
+ * fast_th[f] == 0 or fast_th == NULL means ocfg->fast_threshold (detectPointFeatures); values are clamped to [0, 255].  The
+ * adaptive threshold of the handler is sequential across frames: a batch or sequence takes the thresholds as given.
+ * Returns 0 (a sequence of one frame: 0, no results).  PLSTVO_E_INVALID: a null argument (images where a stage runs), the
+ * ORB checks of plstvo_orb_detect_and_compute_batch, or the key-line checks of plstvo_lbd_compute_batch (width / height and
+ * numOfPixels 1..32767, offsets that start at 0 and do not decrease); PLSTVO_E_SIZE: prev->B != curr->B, or an image size
+ * other than cam's (the reference takes the grid scale from the image, the library from cam); PLSTVO_E_TOO_LARGE: more than
+ * PLSTVO_MAX_FEATURES key points or key lines in one image; and the stereo step's matchGrid codes.  The call also updates
+ * what plstvo_orb_detect_kernel_times and plstvo_lbd_kernel_times report. */
+int plstvo_track_stereo_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                     const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* prev,
+                                     const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results,
+                                     int32_t* n_stereo /* [B][4], as plstvo_track_stereo_batch */);
+int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                        const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
+                                        const PlPrior* priors, PlPoseResult* results,
+                                        int32_t* n_stereo /* [B+1][2], as plstvo_track_stereo_sequence */);
+/* Device time of the last images call, ms: [0] image and key-line upload, [1] ORB (pyramid .. descriptors),
+ * [2] LBD (gradient + descriptors), [3] stereo step (both passes, all feature sets), [4] f2fTracking + optimizePose.
+ * [1] and [2] run on different streams and overlap; a stage that did not run reports 0. */
+int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

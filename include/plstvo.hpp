@@ -181,6 +181,87 @@ inline int computeLBD(Context& c, const uint8_t* image, int width, int height, K
     kl.desc = std::move(desc);
     return k;
 }
+// One stereo frame as StereoFrame::extractStereoFeatures starts it (src/stereoFrame.cpp:59-118, :182-243): the two grey images
+// (row-major, width * height bytes each) and the key lines LSD kept on each (octave 0: start / end point [m][4], KeyLine::angle,
+// KeyLine::numOfPixels).  fast_th 0: the config's FAST threshold.
+struct StereoImageFrame {
+    const uint8_t* img_l = nullptr;
+    const uint8_t* img_r = nullptr;
+    int32_t fast_th = 0;
+    std::vector<float> seg_l, seg_r, angle_l, angle_r;
+    std::vector<int32_t> npix_l, npix_r;
+};
+namespace detail {
+struct StereoImagesPack {   // frames packed into the arrays a PlStereoImages points at
+    std::vector<uint8_t> img_l, img_r;
+    std::vector<int32_t> th, ll_off{0}, lr_off{0}, npix_l, npix_r;
+    std::vector<float> seg_l, seg_r, angle_l, angle_r;
+    PlStereoImages view{};
+};
+inline void packStereoImages(const std::vector<StereoImageFrame>& frames, int width, int height, StereoImagesPack& p) {
+    const size_t px = (size_t)width * (size_t)height;
+    for (const StereoImageFrame& f : frames) {
+        const size_t nl = f.seg_l.size() / 4, nr = f.seg_r.size() / 4;
+        if (!f.img_l || !f.img_r || f.seg_l.size() % 4 || f.seg_r.size() % 4 || f.angle_l.size() != nl || f.npix_l.size() != nl ||
+            f.angle_r.size() != nr || f.npix_r.size() != nr)
+            throw Error(PLSTVO_E_INVALID, "trackStereoImages: every frame needs both images, and seg (4 floats per line), angle and "
+                                          "npix must describe the same lines on each side");
+        p.img_l.insert(p.img_l.end(), f.img_l, f.img_l + px);
+        p.img_r.insert(p.img_r.end(), f.img_r, f.img_r + px);
+        p.th.push_back(f.fast_th);
+        p.ll_off.push_back(p.ll_off.back() + (int32_t)nl);
+        p.lr_off.push_back(p.lr_off.back() + (int32_t)nr);
+        p.seg_l.insert(p.seg_l.end(), f.seg_l.begin(), f.seg_l.end());
+        p.seg_r.insert(p.seg_r.end(), f.seg_r.begin(), f.seg_r.end());
+        p.angle_l.insert(p.angle_l.end(), f.angle_l.begin(), f.angle_l.end());
+        p.angle_r.insert(p.angle_r.end(), f.angle_r.begin(), f.angle_r.end());
+        p.npix_l.insert(p.npix_l.end(), f.npix_l.begin(), f.npix_l.end());
+        p.npix_r.insert(p.npix_r.end(), f.npix_r.begin(), f.npix_r.end());
+    }
+    p.view = PlStereoImages{(int32_t)frames.size(), width, height, p.img_l.data(), p.img_r.data(), p.th.data(), p.ll_off.data(),
+                            p.lr_off.data(), p.seg_l.data(), p.seg_r.data(), p.angle_l.data(), p.angle_r.data(), p.npix_l.data(),
+                            p.npix_r.data()};
+}
+}  // namespace detail
+// Stereo images in, pose out (plstvo_track_stereo_images_batch): extractStereoFeatures with LSD left to the caller, then
+// f2fTracking + optimizePose, for prev.size() independent (prev[p], curr[p]) pairs of images of cam's size.  priors: one per
+// pair or empty (identity).  n_stereo (optional) receives [pairs][4] = stereo points, lines of prev, then of curr.
+inline std::vector<PlPoseResult> trackStereoImages(Context& c, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                                                   const PlStereoConfig& sc, const PlOrbDetectConfig& oc,
+                                                   const std::vector<StereoImageFrame>& prev, const std::vector<StereoImageFrame>& curr,
+                                                   const std::vector<PlPrior>& priors = {}, std::vector<int32_t>* n_stereo = nullptr) {
+    if (prev.size() != curr.size()) throw Error(PLSTVO_E_SIZE, "trackStereoImages: prev and curr hold different numbers of frames");
+    if (!priors.empty() && priors.size() != prev.size()) throw Error(PLSTVO_E_INVALID, "trackStereoImages: one prior per pair");
+    detail::StereoImagesPack a, b;
+    detail::packStereoImages(prev, cam.width, cam.height, a);
+    detail::packStereoImages(curr, cam.width, cam.height, b);
+    std::vector<PlPoseResult> res(std::max<size_t>(prev.size(), 1));
+    std::vector<int32_t> ns(4 * prev.size());
+    c.check(plstvo_track_stereo_images_batch(c.get(), &cam, &cfg, &mc, &sc, &oc, &a.view, &b.view,
+                                             priors.empty() ? nullptr : priors.data(), res.data(), ns.data()));
+    res.resize(prev.size());
+    if (n_stereo) *n_stereo = std::move(ns);
+    return res;
+}
+// The same for consecutive frames (plstvo_track_stereo_images_sequence): frames.size() - 1 results, pair p = (frame p, frame p + 1);
+// every frame's images are detected and described once.  n_stereo (optional): [frames][2] = stereo points, lines per frame.
+inline std::vector<PlPoseResult> trackStereoImageSequence(Context& c, const PlCamera& cam, const PlConfig& cfg,
+                                                          const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
+                                                          const PlOrbDetectConfig& oc, const std::vector<StereoImageFrame>& frames,
+                                                          const std::vector<PlPrior>& priors = {},
+                                                          std::vector<int32_t>* n_stereo = nullptr) {
+    const size_t pairs = frames.empty() ? 0 : frames.size() - 1;
+    if (!priors.empty() && priors.size() != pairs) throw Error(PLSTVO_E_INVALID, "trackStereoImageSequence: one prior per pair");
+    detail::StereoImagesPack a;
+    detail::packStereoImages(frames, cam.width, cam.height, a);
+    std::vector<PlPoseResult> res(std::max<size_t>(pairs, 1));   // the call takes a non-null results array even with no pair
+    std::vector<int32_t> ns(2 * frames.size());
+    c.check(plstvo_track_stereo_images_sequence(c.get(), &cam, &cfg, &mc, &sc, &oc, &a.view,
+                                                priors.empty() ? nullptr : priors.data(), res.data(), ns.data()));
+    res.resize(pairs);
+    if (n_stereo) *n_stereo = std::move(ns);
+    return res;
+}
 inline int matchStereoLines(Context& c, const PlCamera& cam, const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
                             const KeyLines& l, const KeyLines& r, StereoFrame& out) {
     const int n = l.size();

@@ -4,7 +4,9 @@
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
+#include <climits>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -110,6 +112,10 @@ struct PlContext {
     DevBuf arena_lbd;      // plstvo_lbd_compute_batch: images, gradients, key lines, descriptors
     bool lbd_tables = false, lbd_computed = false;
     cudaEvent_t lbd_ev[3] = {nullptr, nullptr, nullptr};
+    // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
+    cudaEvent_t img_ev[4] = {nullptr, nullptr, nullptr, nullptr}, img_join = nullptr;
+    float img_ms[5] = {0, 0, 0, 0, 0};
+    bool img_timed = false;
     // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
     void* h_staging[3] = {nullptr, nullptr, nullptr};
     size_t h_staging_bytes[3] = {0, 0, 0};
@@ -653,6 +659,9 @@ void plstvo_destroy(PlContext* ctx) {
     ctx->arena_lbd.release();
     for (cudaEvent_t e : ctx->lbd_ev)
         if (e) cudaEventDestroy(e);
+    for (cudaEvent_t e : ctx->img_ev)
+        if (e) cudaEventDestroy(e);
+    if (ctx->img_join) cudaEventDestroy(ctx->img_join);
     for (cudaEvent_t e : ctx->events) cudaEventDestroy(e);
     for (void* h : ctx->h_staging)
         if (h) cudaFreeHost(h);
@@ -1235,12 +1244,27 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
 }
 
 // ---- raw stereo features -> pose, records resident in HBM ---------------------------------------------------------
+namespace {
+// Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the
+// stream `lines_ready` was recorded on).  A set with on_device reads xy_l, xy_r, oct, d1, d2 from here instead of uploading
+// the PlStereoFeatures arrays (oct null: all octaves 0); offsets and line angles still come from the host struct.
+struct StereoDevInputs {
+    struct Set {
+        bool on_device = false;
+        const float *xy_l = nullptr, *xy_r = nullptr; const int32_t* oct = nullptr; const uint8_t *d1 = nullptr, *d2 = nullptr;
+    } set[4];
+    cudaEvent_t lines_ready = nullptr;   // waited on before the first line set's stereo step
+    cudaEvent_t* marks = nullptr;        // [3] timing events: stereo step start, its end, tracking end (all on s_main)
+};
+}  // namespace
+
 // sequence == false: B independent (prev, curr) pairs, four feature sets of B frames.
 // sequence == true : prev holds NF = B + 1 consecutive frames, pair p = (frame p, frame p + 1); two feature sets of NF frames,
 //                    every frame goes through the stereo step once and is lifted twice (as a previous and as a current frame).
 static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
-                               const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot) {
+                               const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
+                               const StereoDevInputs* dev = nullptr) {
     // slot < 0: blocking (returns with the results in host memory); slot 0 / 1: enqueue only, results valid after plstvo_wait
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
@@ -1261,26 +1285,39 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
     struct Set {
         bool lines; const int32_t *l_off, *r_off; const float *xy_l, *xy_r, *ang; const int32_t* oct; const uint8_t *d1, *d2;
         size_t N1, N2, o_loff, o_roff, o_xyl, o_xyr, o_ang, o_oct, o_d1, o_d2, o_m12, o_cnt, o_gcnt, o_ooff, o_ooff2, o_prob;
+        bool on_device;
+        const float *g_xyl, *g_xyr; const int32_t* g_oct; const uint8_t *g_d1, *g_d2;   // where the kernels read the inputs
     };
     Set sets[4] = {
         {false, prev->pl_off, prev->pr_off, prev->kp_l, prev->kp_r, nullptr, prev->poct_l, prev->pdesc_l, prev->pdesc_r},
         {true, prev->ll_off, prev->lr_off, prev->seg_l, prev->seg_r, prev->angle_l, prev->loct_l, prev->ldesc_l, prev->ldesc_r},
         {false, curr->pl_off, curr->pr_off, curr->kp_l, curr->kp_r, nullptr, curr->poct_l, curr->pdesc_l, curr->pdesc_r},
         {true, curr->ll_off, curr->lr_off, curr->seg_l, curr->seg_r, curr->angle_l, curr->loct_l, curr->ldesc_l, curr->ldesc_r}};
+    if (dev)
+        for (int k = 0; k < NSETS; ++k)
+            if (dev->set[k].on_device) {
+                const StereoDevInputs::Set& d = dev->set[k];
+                Set& st = sets[k];
+                st.xy_l = d.xy_l; st.xy_r = d.xy_r; st.oct = d.oct; st.d1 = d.d1; st.d2 = d.d2;
+            }
     LiftArena a;
     size_t maxN1 = 0, maxN2 = 0, max_items = 0;
     for (int k = 0; k < NSETS; ++k) {
         Set& st = sets[k];
+        st.on_device = dev && dev->set[k].on_device;
         int rc = lift_check_offsets(ctx, NF, st.l_off, st.r_off);
         if (rc) return rc;
         st.N1 = st.l_off[NF];
         st.N2 = st.r_off[NF];
-        if (st.N1 && (!st.xy_l || !st.oct || !st.d1 || (st.lines && !st.ang))) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+        if (st.N1 && (!st.xy_l || (!st.oct && !st.on_device) || !st.d1 || (st.lines && !st.ang)))
+            return fail(ctx, PLSTVO_E_INVALID, "null input array");
         if (st.N2 && (!st.xy_r || !st.d2)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
         const int cw = st.lines ? 4 : 2;
+        const size_t host = st.on_device ? 0 : 1;   // device-resident inputs take no arena space (but zero octaves do)
         st.o_loff = a.take((size_t)(NF + 1) * 4); st.o_roff = a.take((size_t)(NF + 1) * 4);
-        st.o_xyl = a.take(st.N1 * cw * 4); st.o_xyr = a.take(st.N2 * cw * 4); st.o_ang = a.take(st.lines ? st.N1 * 4 : 0);
-        st.o_oct = a.take(st.N1 * 4); st.o_d1 = a.take(st.N1 * 32); st.o_d2 = a.take(st.N2 * 32); st.o_m12 = a.take(st.N1 * 4);
+        st.o_xyl = a.take(host * st.N1 * cw * 4); st.o_xyr = a.take(host * st.N2 * cw * 4); st.o_ang = a.take(st.lines ? st.N1 * 4 : 0);
+        st.o_oct = a.take(st.on_device && st.oct ? 0 : st.N1 * 4); st.o_d1 = a.take(host * st.N1 * 32);
+        st.o_d2 = a.take(host * st.N2 * 32); st.o_m12 = a.take(st.N1 * 4);
         st.o_cnt = a.take((size_t)NF * 4); st.o_gcnt = a.take((size_t)NF * 4); st.o_ooff = a.take((size_t)(NF + 1) * 4);
         st.o_ooff2 = a.take((size_t)(NF + 1) * 4);
         st.o_prob = a.take((size_t)NF * sizeof(GridProblem));
@@ -1299,6 +1336,14 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
     auto I = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
     auto D = [&](size_t o) { return reinterpret_cast<double*>(base + o); };
     auto F = [&](size_t o) { return reinterpret_cast<float*>(base + o); };
+    for (int k = 0; k < NSETS; ++k) {
+        Set& st = sets[k];
+        st.g_xyl = st.on_device ? st.xy_l : F(st.o_xyl);
+        st.g_xyr = st.on_device ? st.xy_r : F(st.o_xyr);
+        st.g_oct = st.on_device && st.oct ? st.oct : I(st.o_oct);
+        st.g_d1 = st.on_device ? st.d1 : base + st.o_d1;
+        st.g_d2 = st.on_device ? st.d2 : base + st.o_d2;
+    }
     cudaStream_t s = ctx->s_main, sh = ctx->s_h2d;   // uploads of set k + 1 run under the kernels of set k
     auto up = [&](size_t o, const void* src, size_t bytes) -> cudaError_t {
         return (src && bytes) ? cudaMemcpyAsync(base + o, src, bytes, cudaMemcpyHostToDevice, sh) : cudaSuccess;
@@ -1313,6 +1358,8 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
     uint8_t* hst = static_cast<uint8_t*>(ctx->h_staging[slot + 1]);
     int32_t* cnt = reinterpret_cast<int32_t*>(hst + 4 * prob_bytes);
     int32_t* gcnt = cnt + (size_t)4 * NF;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[0], s));
+    bool joined = false;
     // ---- pass 1: cells -> matchGrid -> lifting filters (count only) per set ----
     for (int k = 0; k < NSETS; ++k) {
         Set& st = sets[k];
@@ -1325,11 +1372,11 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
             g.n1 = st.l_off[p + 1] - st.l_off[p];
             g.n2 = st.r_off[p + 1] - st.r_off[p];
             g.q_cell = I(o_qcell) + qa * cw;
-            g.d1 = base + st.o_d1 + qa * 32;
+            g.d1 = st.g_d1 + qa * 32;
             g.t_cell = st.lines ? nullptr : I(o_tcell) + tb * 2;
             g.t_line = st.lines ? D(o_tline) + tb * 4 : nullptr;
             g.t_dir = st.lines ? D(o_tdir) + tb * 2 : nullptr;
-            g.d2 = base + st.o_d2 + tb * 32;
+            g.d2 = st.g_d2 + tb * 32;
             g.m12 = I(st.o_m12) + qa;
             g.count = I(st.o_gcnt) + p;
             g.grid_items = I(o_items) + tb * per_train_cells;
@@ -1343,27 +1390,35 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
         }
         CK(ctx, up(st.o_loff, st.l_off, (size_t)(NF + 1) * 4));
         CK(ctx, up(st.o_roff, st.r_off, (size_t)(NF + 1) * 4));
-        CK(ctx, up(st.o_xyl, st.xy_l, st.N1 * cw * 4));
-        CK(ctx, up(st.o_xyr, st.xy_r, st.N2 * cw * 4));
         if (st.lines) CK(ctx, up(st.o_ang, st.ang, st.N1 * 4));
-        CK(ctx, up(st.o_oct, st.oct, st.N1 * 4));
-        CK(ctx, up(st.o_d1, st.d1, st.N1 * 32));
-        CK(ctx, up(st.o_d2, st.d2, st.N2 * 32));
+        if (!st.on_device) {
+            CK(ctx, up(st.o_xyl, st.xy_l, st.N1 * cw * 4));
+            CK(ctx, up(st.o_xyr, st.xy_r, st.N2 * cw * 4));
+            CK(ctx, up(st.o_oct, st.oct, st.N1 * 4));
+            CK(ctx, up(st.o_d1, st.d1, st.N1 * 32));
+            CK(ctx, up(st.o_d2, st.d2, st.N2 * 32));
+        } else if (!st.oct && st.N1) {
+            CK(ctx, cudaMemsetAsync(base + st.o_oct, 0, st.N1 * 4, sh));   // key lines of octave 0
+        }
         CK(ctx, up(st.o_prob, probs, (size_t)NF * sizeof(GridProblem)));
         cudaEvent_t uploaded = next_event(ctx);
         CK(ctx, cudaEventRecord(uploaded, sh));
         CK(ctx, cudaStreamWaitEvent(s, uploaded, 0));
+        if (st.lines && dev && dev->lines_ready && !joined) {   // the line descriptors come from another stream
+            CK(ctx, cudaStreamWaitEvent(s, dev->lines_ready, 0));
+            joined = true;
+        }
         if (st.lines) {
-            CK(ctx, launch_stereo_cells_lines((int)st.N1, (int)st.N2, inv_w, inv_h, F(st.o_xyl), F(st.o_xyr), I(o_qcell), D(o_tline),
+            CK(ctx, launch_stereo_cells_lines((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, I(o_qcell), D(o_tline),
                                               D(o_tdir), s));
             CK(ctx, launch_match_grid(reinterpret_cast<GridProblem*>(base + st.o_prob), NF, gprm, true, s));
-            CK(ctx, launch_lift_lines(*cam, *sc, NF, I(st.o_loff), F(st.o_xyl), F(st.o_ang), I(st.o_oct), base + st.o_d1, I(st.o_roff),
-                                      F(st.o_xyr), I(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+            CK(ctx, launch_lift_lines(*cam, *sc, NF, I(st.o_loff), st.g_xyl, F(st.o_ang), st.g_oct, st.g_d1, I(st.o_roff),
+                                      st.g_xyr, I(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                                       nullptr, nullptr, nullptr, nullptr, I(st.o_cnt), s));
         } else {
-            CK(ctx, launch_stereo_cells_points((int)st.N1, (int)st.N2, inv_w, inv_h, F(st.o_xyl), F(st.o_xyr), I(o_qcell), I(o_tcell), s));
+            CK(ctx, launch_stereo_cells_points((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, I(o_qcell), I(o_tcell), s));
             CK(ctx, launch_match_grid(reinterpret_cast<GridProblem*>(base + st.o_prob), NF, gprm, false, s));
-            CK(ctx, launch_lift_points(*cam, *sc, NF, I(st.o_loff), F(st.o_xyl), I(st.o_oct), base + st.o_d1, I(st.o_roff), F(st.o_xyr),
+            CK(ctx, launch_lift_points(*cam, *sc, NF, I(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, I(st.o_roff), st.g_xyr,
                                        I(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, I(st.o_cnt), s));
         }
         ctx->launches += 3;
@@ -1406,24 +1461,24 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
     // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
     // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
     auto lift_prev_points = [&](const Set& st) -> cudaError_t {
-        return launch_lift_points(*cam, *sc, B, I(st.o_loff), F(st.o_xyl), I(st.o_oct), base + st.o_d1, I(st.o_roff), F(st.o_xyr),
+        return launch_lift_points(*cam, *sc, B, I(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, I(st.o_roff), st.g_xyr,
                                   I(st.o_m12), nullptr, nullptr, ws.d_ptP.as<double>(), ws.d_pts2.as<double>(), nullptr,
                                   ws.d_pdesc1.as<uint8_t>(), nullptr, I(st.o_cnt), s, I(st.o_ooff));
     };
     auto lift_prev_lines = [&](const Set& st) -> cudaError_t {
-        return launch_lift_lines(*cam, *sc, B, I(st.o_loff), F(st.o_xyl), F(st.o_ang), I(st.o_oct), base + st.o_d1, I(st.o_roff),
-                                 F(st.o_xyr), I(st.o_m12), ws.d_lsspl.as<double>(), ws.d_lsepl.as<double>(), nullptr, nullptr,
+        return launch_lift_lines(*cam, *sc, B, I(st.o_loff), st.g_xyl, F(st.o_ang), st.g_oct, st.g_d1, I(st.o_roff),
+                                 st.g_xyr, I(st.o_m12), ws.d_lsspl.as<double>(), ws.d_lsepl.as<double>(), nullptr, nullptr,
                                  ws.d_lssP.as<double>(), ws.d_lseP.as<double>(), nullptr, nullptr, ws.d_lss2.as<double>(),
                                  ws.d_lslev.as<int32_t>(), ws.d_ldesc1.as<uint8_t>(), nullptr, I(st.o_cnt), s, I(st.o_ooff));
     };
     auto lift_curr_points = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
-        return launch_lift_points(*cam, *sc, B, I(st.o_loff) + first, F(st.o_xyl), I(st.o_oct), base + st.o_d1, I(st.o_roff) + first,
-                                  F(st.o_xyr), I(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
+        return launch_lift_points(*cam, *sc, B, I(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, I(st.o_roff) + first,
+                                  st.g_xyr, I(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
                                   ws.d_pdesc2.as<uint8_t>(), nullptr, I(st.o_cnt) + first, s, I(o_out));
     };
     auto lift_curr_lines = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
-        return launch_lift_lines(*cam, *sc, B, I(st.o_loff) + first, F(st.o_xyl), F(st.o_ang), I(st.o_oct), base + st.o_d1,
-                                 I(st.o_roff) + first, F(st.o_xyr), I(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+        return launch_lift_lines(*cam, *sc, B, I(st.o_loff) + first, st.g_xyl, F(st.o_ang), st.g_oct, st.g_d1,
+                                 I(st.o_roff) + first, st.g_xyr, I(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
                                  ws.d_lsle.as<double>(), nullptr, nullptr, nullptr, ws.d_ldesc2.as<uint8_t>(), nullptr,
                                  I(st.o_cnt) + first, s, I(o_out));
     };
@@ -1437,10 +1492,12 @@ static int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConf
         CK(ctx, lift_curr_lines(sets[3], 0, sets[3].o_ooff));
     }
     ctx->launches += 4;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
     rc = ws_launch_match(ctx, ws, 0, B, s);
     if (rc) return rc;
     rc = ws_launch_solve(ctx, ws, 0, B, true, s);
     if (rc) return rc;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[2], s));
     CK(ctx, cudaMemcpyAsync(results, ws.d_results.p, (size_t)B * sizeof(PlPoseResult), cudaMemcpyDeviceToHost, s));
     if (slot < 0) CK(ctx, cudaStreamSynchronize(s));
     return 0;
@@ -2255,6 +2312,96 @@ cudaError_t lbd_init(PlContext* ctx) {   // coefficient tables and timing events
     if (e == cudaSuccess) ctx->lbd_tables = true;
     return e;
 }
+
+// key lines of n_img consecutive images: kl_off [n_img + 1] and the per-line arrays
+struct LineSrc {
+    int n_img; const int32_t* off; const float* seg; const float* angle; const int32_t* npix;
+};
+
+// the key-line checks of plstvo_lbd_compute_batch on one LineSrc (the arrays only where lines exist)
+int lbd_check_lines(PlContext* ctx, const LineSrc& l) {
+    if (!l.off || l.off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null offsets or kl_off[0] != 0");
+    for (int i = 0; i < l.n_img; ++i) {
+        const int n = l.off[i + 1] - l.off[i];
+        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kl_off is not non-decreasing");
+        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+    }
+    const size_t N = (size_t)l.off[l.n_img];
+    if (N && (!l.seg || !l.angle || !l.npix)) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
+    for (size_t k = 0; k < N; ++k)
+        if (l.npix[k] < 1 || l.npix[k] > 32767) return fail(ctx, PLSTVO_E_INVALID, "numOfPixels must be 1..32767");
+    return 0;
+}
+
+struct ImgPart {   // consecutive host images of one size
+    const uint8_t* p; int n;
+};
+
+// Enqueues LBD description on stream s for checked key lines (parts, in image order; at least one line in all) of images of one
+// size: either device images (d_img, ready once img_ready has completed) or host images that go into arena_lbd (img_parts).
+// Leaves the key lines' segments (sPointInOctave, ePointInOctave as given) and descriptors in arena_lbd.
+int lbd_enqueue(PlContext* ctx, int width, int height, const std::vector<LineSrc>& parts, const uint8_t* d_img,
+                cudaEvent_t img_ready, const std::vector<ImgPart>& img_parts, cudaStream_t s, const float** d_seg,
+                const uint8_t** d_desc) {
+    int n_img = 0;
+    std::vector<int32_t> off(1, 0);
+    for (const LineSrc& l : parts) {
+        for (int i = 0; i < l.n_img; ++i) off.push_back(off.back() + l.off[i + 1] - l.off[i]);
+        n_img += l.n_img;
+    }
+    const size_t N = (size_t)off.back();
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, lbd_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height;
+    LiftArena a;
+    const size_t o_img = a.take(d_img ? 0 : img_bytes), o_grad = a.take(img_bytes * 4), o_off = a.take((size_t)(n_img + 1) * 4);
+    const size_t o_seg = a.take(N * 16), o_dir = a.take(N * 8), o_npix = a.take(N * 4), o_desc = a.take(N * 32);
+    DevBuf& arena = ctx->arena_lbd;
+    CK(ctx, arena.ensure(a.off));
+    uint8_t* base = arena.as<uint8_t>();
+    if (!d_img) {
+        size_t o = o_img;
+        for (const ImgPart& ip : img_parts) {
+            const size_t bytes = (size_t)ip.n * width * height;
+            CK(ctx, cudaMemcpyAsync(base + o, ip.p, bytes, cudaMemcpyHostToDevice, s));
+            o += bytes;
+        }
+    }
+    CK(ctx, cudaMemcpyAsync(base + o_off, off.data(), (size_t)(n_img + 1) * 4, cudaMemcpyHostToDevice, s));
+    // dL = (cos, sin) of the float angle.  The reference's unqualified cos(float) / sin(float) bind to std::cos(float) /
+    // std::sin(float), the C library's cosf / sinf (its translation unit includes <math.h>, whose C++ form puts the float
+    // overloads into the global namespace), and GCC merges the pair into sincosf.  They are evaluated here, with the same
+    // library, because no device function rounds them the same way.
+    std::vector<float> dir(2 * N);
+    size_t r = 0;
+    for (const LineSrc& l : parts) {
+        const size_t n = (size_t)l.off[l.n_img];
+        if (!n) continue;
+        CK(ctx, cudaMemcpyAsync(base + o_seg + r * 16, l.seg, n * 16, cudaMemcpyHostToDevice, s));
+        const float* kl_angle = l.angle;
+        float* d = dir.data() + 2 * r;
+        for (size_t k = 0; k < n; ++k) sincosf(kl_angle[k], &d[2 * k + 1], &d[2 * k]);
+        r += n;
+    }
+    CK(ctx, cudaMemcpyAsync(base + o_dir, dir.data(), N * 8, cudaMemcpyHostToDevice, s));
+    r = 0;
+    for (const LineSrc& l : parts) {
+        const size_t n = (size_t)l.off[l.n_img];
+        if (n) CK(ctx, cudaMemcpyAsync(base + o_npix + r * 4, l.npix, n * 4, cudaMemcpyHostToDevice, s));
+        r += n;
+    }
+    if (d_img && img_ready) CK(ctx, cudaStreamWaitEvent(s, img_ready, 0));
+    int launches = 0;
+    CK(ctx, launch_lbd(n_img, width, height, d_img ? d_img : base + o_img, reinterpret_cast<const int32_t*>(base + o_off), (int)N,
+                       reinterpret_cast<const float*>(base + o_seg), reinterpret_cast<const float2*>(base + o_dir),
+                       reinterpret_cast<const int32_t*>(base + o_npix), reinterpret_cast<short2*>(base + o_grad),
+                       base + o_desc, s, ctx->lbd_ev, &launches));
+    ctx->lbd_computed = true;
+    ctx->launches += launches;
+    *d_seg = reinterpret_cast<const float*>(base + o_seg);
+    *d_desc = base + o_desc;
+    return 0;
+}
 }  // namespace
 
 int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, const uint8_t* images, const int32_t* kl_off,
@@ -2265,46 +2412,17 @@ int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, c
     // the reference indexes pixels and counts samples in short
     if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
     if (n_img == 0) return 0;
-    if (!kl_off || kl_off[0] != 0) return fail(ctx, PLSTVO_E_INVALID, "null offsets or kl_off[0] != 0");
-    for (int i = 0; i < n_img; ++i) {
-        const int n = kl_off[i + 1] - kl_off[i];
-        if (n < 0) return fail(ctx, PLSTVO_E_INVALID, "kl_off is not non-decreasing");
-        if (n > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
-    }
+    const LineSrc lines{n_img, kl_off, kl_seg, kl_angle, kl_npix};
+    if (const int rc = lbd_check_lines(ctx, lines)) return rc;
     const size_t N = (size_t)kl_off[n_img];
     if (N == 0) return 0;
-    if (!images || !kl_seg || !kl_angle || !kl_npix || !out_desc) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
-    for (size_t k = 0; k < N; ++k)
-        if (kl_npix[k] < 1 || kl_npix[k] > 32767) return fail(ctx, PLSTVO_E_INVALID, "numOfPixels must be 1..32767");
-    CK(ctx, cudaSetDevice(ctx->device));
-    CK(ctx, lbd_init(ctx));
-    const size_t img_bytes = (size_t)n_img * width * height;
-    LiftArena a;
-    const size_t o_img = a.take(img_bytes), o_grad = a.take(img_bytes * 4), o_off = a.take((size_t)(n_img + 1) * 4);
-    const size_t o_seg = a.take(N * 16), o_dir = a.take(N * 8), o_npix = a.take(N * 4), o_desc = a.take(N * 32);
-    DevBuf& arena = ctx->arena_lbd;
-    CK(ctx, arena.ensure(a.off));
-    uint8_t* base = arena.as<uint8_t>();
+    if (!images || !out_desc) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
     cudaStream_t s = ctx->s_main;
-    CK(ctx, cudaMemcpyAsync(base + o_img, images, img_bytes, cudaMemcpyHostToDevice, s));
-    CK(ctx, cudaMemcpyAsync(base + o_off, kl_off, (size_t)(n_img + 1) * 4, cudaMemcpyHostToDevice, s));
-    CK(ctx, cudaMemcpyAsync(base + o_seg, kl_seg, N * 16, cudaMemcpyHostToDevice, s));
-    // dL = (cos, sin) of the float angle.  The reference's unqualified cos(float) / sin(float) bind to std::cos(float) /
-    // std::sin(float), the C library's cosf / sinf (its translation unit includes <math.h>, whose C++ form puts the float
-    // overloads into the global namespace), and GCC merges the pair into sincosf.  They are evaluated here, with the same
-    // library, because no device function rounds them the same way.
-    std::vector<float> dir(2 * N);
-    for (size_t k = 0; k < N; ++k) sincosf(kl_angle[k], &dir[2 * k + 1], &dir[2 * k]);
-    CK(ctx, cudaMemcpyAsync(base + o_dir, dir.data(), N * 8, cudaMemcpyHostToDevice, s));
-    CK(ctx, cudaMemcpyAsync(base + o_npix, kl_npix, N * 4, cudaMemcpyHostToDevice, s));
-    int launches = 0;
-    CK(ctx, launch_lbd(n_img, width, height, base + o_img, reinterpret_cast<const int32_t*>(base + o_off), (int)N,
-                       reinterpret_cast<const float*>(base + o_seg), reinterpret_cast<const float2*>(base + o_dir),
-                       reinterpret_cast<const int32_t*>(base + o_npix), reinterpret_cast<short2*>(base + o_grad),
-                       base + o_desc, s, ctx->lbd_ev, &launches));
-    ctx->lbd_computed = true;
-    ctx->launches += launches;
-    CK(ctx, cudaMemcpyAsync(out_desc, base + o_desc, N * 32, cudaMemcpyDeviceToHost, s));
+    const float* d_seg = nullptr;
+    const uint8_t* d_desc = nullptr;
+    if (const int rc = lbd_enqueue(ctx, width, height, {lines}, nullptr, nullptr, {ImgPart{images, n_img}}, s, &d_seg, &d_desc))
+        return rc;
+    CK(ctx, cudaMemcpyAsync(out_desc, d_desc, N * 32, cudaMemcpyDeviceToHost, s));
     CK(ctx, cudaStreamSynchronize(s));
     return (int)N;
 }
@@ -2325,20 +2443,29 @@ void plstvo_default_orb_detect_config(PlOrbDetectConfig* c) {
     c->n_features = 1200; c->score_type = 1; c->fast_threshold = 20;
 }
 
-int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
-                                        const uint8_t* images, const int32_t* fast_th, int capacity, int32_t* kp_off,
-                                        float* kp_xy, int32_t* kp_octave, float* kp_angle, float* kp_response, uint8_t* desc) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!cfg || n_img < 0 || width < 0 || height < 0 || capacity < 0)
-        return fail(ctx, PLSTVO_E_INVALID, "null config, negative size or negative capacity");
+namespace {
+int orb_detect_check(PlContext* ctx, const PlOrbDetectConfig* cfg) {
     if (const int rc = orb_check_config(ctx, &cfg->orb)) return rc;
     if (cfg->n_features < 0) return fail(ctx, PLSTVO_E_INVALID, "negative n_features");
     if (cfg->score_type != 0 && cfg->score_type != 1) return fail(ctx, PLSTVO_E_INVALID, "score_type must be 0 (Harris) or 1 (FAST)");
-    if (!kp_off) return fail(ctx, PLSTVO_E_INVALID, "null kp_off");
-    kp_off[0] = 0;
-    if (n_img == 0) return 0;
-    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    return 0;
+}
+
+// key points of an ORB detect call, left in HBM (CSR by image, arena_orb_kp) with the host copy of the offsets
+struct OrbDetected {
+    std::vector<int32_t> off;   // [n_img + 1]; also written in full when the call fails with PLSTVO_E_TOO_LARGE
+    const float *xy = nullptr, *angle = nullptr, *response = nullptr;
+    const int32_t* octave = nullptr;
+    const uint8_t* desc = nullptr;
+};
+
+// Uploads n_img (> 0) host images (parts, in order) into arena_orb and enqueues detection and description on s_main, for a
+// checked config and per-image FAST thresholds th (clamped here).  `beside` (optional) is called with the device images and an
+// event that completes once they are uploaded, after the pyramid and FAST launches are enqueued and before the first offsets
+// readback blocks this thread: work enqueued there on another stream overlaps those stages.
+int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                       const std::vector<ImgPart>& parts, const int32_t* fast_th, int capacity,
+                       const std::function<int(const uint8_t*, cudaEvent_t)>& beside, OrbDetected& out) {
     PlOrbConfig oc = cfg->orb;
     oc.scale_factor = (double)(float)oc.scale_factor;   // ORB::create takes a float scale factor
     if (oc.n_levels > 1 && !(oc.scale_factor > 1.0)) return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1 in float");
@@ -2373,7 +2500,7 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
     }
     const int R = D.row0[nl];
     std::vector<int32_t> th((size_t)n_img);
-    for (int i = 0; i < n_img; ++i) th[i] = std::min(std::max(fast_th ? fast_th[i] : cfg->fast_threshold, 0), 255);
+    for (int i = 0; i < n_img; ++i) th[i] = std::min(std::max(fast_th[i], 0), 255);
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, orb_init(ctx));
     const size_t img_bytes = (size_t)n_img * width * height, NL = (size_t)n_img * nl;
@@ -2390,7 +2517,19 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
     uint8_t* base = arena.as<uint8_t>();
     cudaStream_t s = ctx->s_main;
     auto I = [&](size_t o) { return reinterpret_cast<int32_t*>(base + o); };
-    CK(ctx, cudaMemcpyAsync(base + o_img, images, img_bytes, cudaMemcpyHostToDevice, s));
+    {
+        size_t o = o_img;
+        for (const ImgPart& ip : parts) {
+            const size_t bytes = (size_t)ip.n * width * height;
+            CK(ctx, cudaMemcpyAsync(base + o, ip.p, bytes, cudaMemcpyHostToDevice, s));
+            o += bytes;
+        }
+    }
+    cudaEvent_t uploaded = nullptr;
+    if (beside) {
+        uploaded = next_event(ctx);
+        CK(ctx, cudaEventRecord(uploaded, s));
+    }
     if (!tabs.empty()) CK(ctx, cudaMemcpyAsync(base + o_tab, tabs.data(), tabs.size() * 4, cudaMemcpyHostToDevice, s));
     CK(ctx, cudaMemcpyAsync(base + o_th, th.data(), (size_t)n_img * 4, cudaMemcpyHostToDevice, s));
     std::vector<const int32_t*> rs_tab(2 * (size_t)nl, nullptr);
@@ -2407,17 +2546,19 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
                            reinterpret_cast<uint32_t*>(base + o_hist), I(o_cut), I(o_rcnt), I(o_rbase), I(o_icnt), I(o_soff), s,
                            ev[2], &launches);
     CK(ctx, cudaGetLastError());
-    std::vector<int32_t> off((size_t)n_img + 1);
+    if (beside)
+        if (const int rc = beside(base + o_img, uploaded)) return rc;
+    std::vector<int32_t>& off = out.off;
+    off.assign((size_t)n_img + 1, 0);
     CK(ctx, cudaMemcpyAsync(off.data(), I(o_soff), off.size() * 4, cudaMemcpyDeviceToHost, s));
     CK(ctx, cudaStreamSynchronize(s));
     ctx->launches += launches;
     launches = 0;
     ctx->orb_detected = true;
-    // too many key points: kp_off in full (the caller sizes its buffers from it), nothing else written
+    // too many key points: the offsets in full (the caller sizes its buffers from them), no key points
     auto too_large = [&]() -> int {
         CK(ctx, cudaEventRecord(ev[3], s));
         CK(ctx, cudaEventRecord(ev[4], s));
-        memcpy(kp_off, off.data(), off.size() * 4);
         for (int i = 0; i < n_img; ++i)
             if (off[i + 1] - off[i] > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
         if (off[n_img] > capacity) return fail(ctx, PLSTVO_E_TOO_LARGE, "more key points than capacity");
@@ -2467,17 +2608,196 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
     CK(ctx, cudaEventRecord(ev[4], s));
     CK(ctx, cudaGetLastError());
     ctx->launches += launches;
+    out.xy = d_xy; out.octave = d_oct; out.angle = KF(o_ang); out.response = d_resp; out.desc = kb + o_desc;
+    return 0;
+}
+}  // namespace
+
+int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                                        const uint8_t* images, const int32_t* fast_th, int capacity, int32_t* kp_off,
+                                        float* kp_xy, int32_t* kp_octave, float* kp_angle, float* kp_response, uint8_t* desc) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0 || capacity < 0)
+        return fail(ctx, PLSTVO_E_INVALID, "null config, negative size or negative capacity");
+    if (const int rc = orb_detect_check(ctx, cfg)) return rc;
+    if (!kp_off) return fail(ctx, PLSTVO_E_INVALID, "null kp_off");
+    kp_off[0] = 0;
+    if (n_img == 0) return 0;
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    std::vector<int32_t> th((size_t)n_img, cfg->fast_threshold);
+    if (fast_th) std::copy(fast_th, fast_th + n_img, th.begin());
+    OrbDetected o;
+    const int rc = orb_detect_enqueue(ctx, cfg, n_img, width, height, {ImgPart{images, n_img}}, th.data(), capacity, nullptr, o);
+    if (rc == PLSTVO_E_TOO_LARGE && o.off.size() == (size_t)n_img + 1) memcpy(kp_off, o.off.data(), o.off.size() * 4);
+    if (rc) return rc;
+    const size_t N = (size_t)o.off[n_img];
+    cudaStream_t s = ctx->s_main;
     auto down = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
         return (dst && bytes) ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
     };
-    CK(ctx, down(kp_xy, d_xy, N * 8));
-    CK(ctx, down(kp_octave, d_oct, N * 4));
-    CK(ctx, down(kp_angle, KF(o_ang), N * 4));
-    CK(ctx, down(kp_response, d_resp, N * 4));
-    CK(ctx, down(desc, kb + o_desc, N * 32));
+    CK(ctx, down(kp_xy, o.xy, N * 8));
+    CK(ctx, down(kp_octave, o.octave, N * 4));
+    CK(ctx, down(kp_angle, o.angle, N * 4));
+    CK(ctx, down(kp_response, o.response, N * 4));
+    CK(ctx, down(desc, o.desc, N * 32));
     CK(ctx, cudaStreamSynchronize(s));
-    memcpy(kp_off, off.data(), off.size() * 4);
+    memcpy(kp_off, o.off.data(), o.off.size() * 4);
     return (int)N;
+}
+
+/* ---- stereo images -> pose: ORB and LBD feed the stereo step and the tracker without leaving HBM ---- */
+// The images go up once into arena_orb in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left]
+// [curr right].  Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.
+static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                            const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
+                            const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
+                            bool sequence) {
+    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
+        return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    const int NF = prev->B;
+    if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
+    if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (const int rc = orb_detect_check(ctx, oc)) return rc;
+    const int nfs = sequence ? 1 : 2;   // frame sets: the sequence, or prev and curr
+    const PlStereoImages* fs[2] = {prev, curr};
+    const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0;
+    const int W = cam->width, H = cam->height;
+    std::vector<LineSrc> lsrc;   // key lines per image block
+    if (NF > 0) {
+        for (int j = 0; j < nfs; ++j) {
+            // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
+            if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
+            if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
+        }
+        if (lns) {
+            if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+            for (int j = 0; j < nfs; ++j) {
+                lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
+                lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
+            }
+            for (const LineSrc& l : lsrc)
+                if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        }
+    }
+    if (NF == 0 || (sequence && NF == 1)) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    if (!ctx->img_join) {
+        for (auto& ev : ctx->img_ev) CK(ctx, cudaEventCreate(&ev));
+        CK(ctx, cudaEventCreateWithFlags(&ctx->img_join, cudaEventDisableTiming));
+    }
+    ctx->img_timed = false;
+    const int nblk = 2 * nfs, n_img = nblk * NF;
+    std::vector<ImgPart> iparts;
+    std::vector<int32_t> th((size_t)n_img), lbase((size_t)nblk + 1, 0);
+    for (int b = 0; b < nblk; ++b) {
+        const PlStereoImages* f = fs[b / 2];
+        iparts.push_back(ImgPart{b % 2 ? f->img_r : f->img_l, NF});
+        for (int i = 0; i < NF; ++i)   // 0 = the configured threshold, as detectPointFeatures / plstvo::detectAndComputeORB
+            th[(size_t)b * NF + i] = f->fast_th && f->fast_th[i] ? f->fast_th[i] : oc->fast_threshold;
+        lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
+    }
+    const bool run_lbd = lbase[nblk] > 0;
+    const float* d_seg = nullptr;
+    const uint8_t* d_ldesc = nullptr;
+    // LBD on the second stream; with ORB running it reads ORB's copy of the images once their upload has completed
+    auto enqueue_lbd = [&](const uint8_t* d_img, cudaEvent_t ready) -> int {
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, iparts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+        CK(ctx, cudaEventRecord(ctx->img_join, ctx->s_alt));
+        return 0;
+    };
+    CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
+    OrbDetected orb;
+    if (pts) {
+        std::function<int(const uint8_t*, cudaEvent_t)> beside;
+        if (run_lbd) beside = enqueue_lbd;
+        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, iparts, th.data(), INT_MAX, beside, orb)) return rc;
+    } else {
+        orb.off.assign((size_t)n_img + 1, 0);
+        if (run_lbd)
+            if (const int rc = enqueue_lbd(nullptr, nullptr)) return rc;
+    }
+    // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
+    std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
+    PlStereoFeatures feat[2]{};
+    StereoDevInputs dev;
+    for (int j = 0; j < nfs; ++j) {
+        const int bl = 2 * j, br = 2 * j + 1;
+        const size_t kl = orb.off[(size_t)bl * NF], kr = orb.off[(size_t)br * NF];
+        pl_off[j].resize((size_t)NF + 1);
+        pr_off[j].resize((size_t)NF + 1);
+        for (int i = 0; i <= NF; ++i) {
+            pl_off[j][i] = orb.off[(size_t)bl * NF + i] - (int32_t)kl;
+            pr_off[j][i] = orb.off[(size_t)br * NF + i] - (int32_t)kr;
+        }
+        PlStereoFeatures& F = feat[j];
+        F.B = NF;
+        F.pl_off = pl_off[j].data(); F.pr_off = pr_off[j].data();
+        F.ll_off = lns ? fs[j]->ll_off : none.data(); F.lr_off = lns ? fs[j]->lr_off : none.data();
+        F.angle_l = lns ? fs[j]->angle_l : nullptr;
+        StereoDevInputs::Set& P = dev.set[2 * j];
+        P.on_device = true;
+        if (pts) {
+            P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
+            P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
+        }
+        StereoDevInputs::Set& Ls = dev.set[2 * j + 1];
+        Ls.on_device = true;   // oct stays null: key lines of octave 0
+        if (run_lbd) {
+            Ls.xy_l = d_seg + 4 * (size_t)lbase[bl]; Ls.xy_r = d_seg + 4 * (size_t)lbase[br];
+            Ls.d1 = d_ldesc + 32 * (size_t)lbase[bl]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[br];
+        }
+    }
+    dev.lines_ready = run_lbd ? ctx->img_join : nullptr;
+    dev.marks = ctx->img_ev + 1;
+    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], sequence ? nullptr : &feat[1], priors, results,
+                                           n_stereo, sequence, -1, &dev))
+        return rc;
+    float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
+    std::fill(ms, ms + 5, 0.f);
+    // uploads end where the first stage starts: LBD waits for the images and its key lines, ORB for the images only
+    const cudaEvent_t up_end = run_lbd ? ctx->lbd_ev[0] : pts ? ctx->orb_det_ev[0] : nullptr;
+    if (up_end) CK(ctx, cudaEventElapsedTime(&ms[0], ctx->img_ev[0], up_end));
+    if (pts) CK(ctx, cudaEventElapsedTime(&ms[1], ctx->orb_det_ev[0], ctx->orb_det_ev[4]));
+    if (run_lbd) CK(ctx, cudaEventElapsedTime(&ms[2], ctx->lbd_ev[0], ctx->lbd_ev[2]));
+    CK(ctx, cudaEventElapsedTime(&ms[3], ctx->img_ev[1], ctx->img_ev[2]));
+    CK(ctx, cudaEventElapsedTime(&ms[4], ctx->img_ev[2], ctx->img_ev[3]));
+    ctx->img_timed = true;
+    return 0;
+}
+
+static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                               const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
+                               const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
+                               bool sequence) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, prev, curr, priors, results, n_stereo, sequence);
+    // LBD may still run on the second stream after an error: the next call may reuse its arena
+    const cudaError_t e = cudaStreamSynchronize(ctx->s_alt);
+    if (rc) return rc;
+    CK(ctx, e);
+    return 0;
+}
+
+int plstvo_track_stereo_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                     const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* prev,
+                                     const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, prev, curr, priors, results, n_stereo, false);
+}
+
+int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                        const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
+                                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {
+    if (!ctx || !ms5) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->img_timed) return fail(ctx, PLSTVO_E_INVALID, "no images call on this context yet");
+    memcpy(ms5, ctx->img_ms, sizeof(ctx->img_ms));
+    return 0;
 }
 
 int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4) {

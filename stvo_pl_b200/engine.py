@@ -97,6 +97,13 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_orb_detect_kernel_times": (C.c_int, [vp, fp]),
         "plstvo_lbd_compute_batch": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, u8p, i32p, fp, fp, i32p, u8p]),
         "plstvo_lbd_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_track_stereo_images_batch": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig), C.POINTER(T.PlStereoConfig),
+                                                       C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlStereoImages),
+                                                       C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_track_stereo_images_sequence": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                          C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                          C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_track_stereo_images_stage_times": (C.c_int, [vp, fp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -117,7 +124,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
-    "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times"]
+    "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_track_stereo_images_batch",
+    "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_stage_times"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -536,6 +544,42 @@ class Engine:
                                                        results.ctypes.data, _p(n_stereo, T.c_int32_p)))
         del keep
         return results, n_stereo
+
+    def track_stereo_images_batch(self, cam, cfg, mcfg, scfg, ocfg, prev: dict, curr: dict, priors=None, results=None):
+        """Stereo images and key lines of B (prev, curr) frame pairs -> poses: ORB detection, LBD description, the stereo step,
+        f2fTracking and optimizePose, feature data resident in HBM.  prev / curr: dicts with img_l / img_r uint8[B, H, W] and
+        the other PlStereoImages fields (see T.stereo_images_as_c).  Returns (results, n_stereo[B, 4])."""
+        ps, keep_p = T.stereo_images_as_c(prev)
+        cs, keep_c = T.stereo_images_as_c(curr)
+        B = ps.B
+        if results is None:
+            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((B, 4), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_images_batch(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg), C.byref(ps), C.byref(cs),
+            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep_p, keep_c
+        return results, n_stereo
+
+    def track_stereo_images_sequence(self, cam, cfg, mcfg, scfg, ocfg, frames: dict, priors=None, results=None):
+        """NF consecutive stereo frames (images and key lines) -> NF - 1 poses; every frame's images are detected and described
+        once.  Returns (results, n_stereo[NF, 2])."""
+        fs, keep = T.stereo_images_as_c(frames)
+        NF = fs.B
+        if results is None:
+            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((NF, 2), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_images_sequence(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg), C.byref(fs),
+            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep
+        return results, n_stereo
+
+    def track_stereo_images_stage_times(self):
+        """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB), stereo step, f2fTracking + optimizePose."""
+        ms = np.zeros(5, np.float32)
+        self._ck(self.lib.plstvo_track_stereo_images_stage_times(self.ctx, _p(ms, T.c_float_p)))
+        return ms
 
     # ---- stereoFrameHandler.h surface ----
     def f2f_tracking(self, cfg, prev: T.FrameBatch, curr: T.FrameBatch):

@@ -126,6 +126,30 @@ def stereo_features_as_c(d: dict):
     return s, keep
 
 
+class PlStereoImages(C.Structure):
+    """Stereo images and their key lines of B frames (PlStereoImages, include/plstvo.h)."""
+    _fields_ = [("B", C.c_int32), ("width", C.c_int32), ("height", C.c_int32), ("img_l", c_uint8_p), ("img_r", c_uint8_p),
+                ("fast_th", c_int32_p), ("ll_off", c_int32_p), ("lr_off", c_int32_p), ("seg_l", c_float_p), ("seg_r", c_float_p),
+                ("angle_l", c_float_p), ("angle_r", c_float_p), ("npix_l", c_int32_p), ("npix_r", c_int32_p)]
+
+
+STEREO_IMAGE_DTYPES = dict(img_l=np.uint8, img_r=np.uint8, fast_th=np.int32, ll_off=np.int32, lr_off=np.int32, seg_l=np.float32,
+                           seg_r=np.float32, angle_l=np.float32, angle_r=np.float32, npix_l=np.int32, npix_r=np.int32)
+
+
+def stereo_images_as_c(d: dict):
+    """dict with img_l / img_r uint8[B, H, W] and optionally fast_th [B] and the key-line arrays (keys of STEREO_IMAGE_DTYPES;
+    a missing or None entry is passed as NULL) -> (PlStereoImages, keep-alive dict)."""
+    keep = {k: None if d.get(k) is None else np.ascontiguousarray(d[k], dt) for k, dt in STEREO_IMAGE_DTYPES.items()}
+    s = PlStereoImages()
+    B, H, W = keep["img_l"].shape
+    s.B, s.width, s.height = B, W, H
+    for k, a in keep.items():
+        typ = dict(PlStereoImages._fields_)[k]
+        setattr(s, k, C.cast(None, typ) if a is None else a.ctypes.data_as(typ))
+    return s, keep
+
+
 GRID_ROWS, GRID_COLS = 48, 64     # include/stereoFrame.h:51-52
 
 
