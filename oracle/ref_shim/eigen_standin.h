@@ -69,6 +69,14 @@ public:
         for (int i = 0; i < r_ * c_; ++i) s += d_[i];
         return s;
     }
+    M cross(const M& o) const {   // 3-vectors: Eigen's coefficient formulas, (1,2), (2,0), (0,1)
+        assert(size() == 3 && o.size() == 3);
+        M t(r_, c_);
+        t.d_[0] = d_[1] * o.d_[2] - d_[2] * o.d_[1];
+        t.d_[1] = d_[2] * o.d_[0] - d_[0] * o.d_[2];
+        t.d_[2] = d_[0] * o.d_[1] - d_[1] * o.d_[0];
+        return t;
+    }
     M cwiseAbs() const {
         M t(r_, c_);
         for (int i = 0; i < r_ * c_; ++i) t.d_[i] = std::fabs(d_[i]);

@@ -89,7 +89,7 @@ __device__ void mg_sequential(const GridProblem& pr, const GridParams& prm, cons
         if (LINES) {
             vx = (double)(qc[2] - qc[0]);
             vy = (double)(qc[3] - qc[1]);
-            const double mag = sqrt(vx * vx + vy * vy);
+            const double mag = sqrt(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));   // unfused, as dot (matching.h:39-41)
             vx /= mag;
             vy /= mag;
         }
@@ -107,8 +107,8 @@ __device__ void mg_sequential(const GridProblem& pr, const GridParams& prm, cons
                     if (atomicExch(&stamp[i2], q) == q) continue;   // already in this query's candidate set
                     any = 1;
                     if (LINES) {
-                        const double dt = vx * pr.t_dir[2 * i2] + vy * pr.t_dir[2 * i2 + 1];
-                        if (fabs(dt) < prm.line_sim_th) continue;    // NaN passes (:221)
+                        const double dt = __dadd_rn(__dmul_rn(vx, pr.t_dir[2 * i2]), __dmul_rn(vy, pr.t_dir[2 * i2 + 1]));
+                        if (fabs(dt) < prm.line_sim_th) continue;    // NaN passes (:221); unfused, a fused dot flips |dt| ~ th
                     }
                     const int d = mg_distance(dq, pr.d2 + (size_t)i2 * 32);
                     if (prm.best_lr) {          // each train appears once per query: no race on dist[i2]
@@ -226,7 +226,7 @@ __global__ void __launch_bounds__(MG_THREADS) match_grid_kernel(const GridProble
         if (LINES) {   // v = normalize(ep - sp) in INTEGER cell coordinates (:207-211): NaN when both share a cell
             vx = (double)(qc[2] - qc[0]);
             vy = (double)(qc[3] - qc[1]);
-            const double mag = sqrt(vx * vx + vy * vy);
+            const double mag = sqrt(__dadd_rn(__dmul_rn(vx, vx), __dmul_rn(vy, vy)));   // unfused, as dot (matching.h:39-41)
             vx /= mag;
             vy /= mag;
         }
@@ -249,8 +249,8 @@ __global__ void __launch_bounds__(MG_THREADS) match_grid_kernel(const GridProble
                         int d = -1;                // -1: in the candidate set but dropped by the direction filter
                         bool pass = true;
                         if (LINES) {
-                            const double dt = vx * pr.t_dir[2 * i2] + vy * pr.t_dir[2 * i2 + 1];
-                            if (fabs(dt) < prm.line_sim_th) pass = false;   // NaN passes (:221)
+                            const double dt = __dadd_rn(__dmul_rn(vx, pr.t_dir[2 * i2]), __dmul_rn(vy, pr.t_dir[2 * i2 + 1]));
+                            if (fabs(dt) < prm.line_sim_th) pass = false;   // NaN passes (:221); unfused (see mg_sequential)
                         }
                         if (pass) d = mg_distance(dq, pr.d2 + (size_t)i2 * 32);
                         seg[k++] = make_int2(i2, d);
