@@ -1,0 +1,679 @@
+// capi_features.cu — the C-ABI's feature extraction on the GPU: ORB description and detection (orb.cu), LBD description
+// (lbd.cu), and pose tracking from stereo images, where both feed the stereo step and the tracker without leaving HBM.
+#include <climits>
+#include <cstring>
+#include <functional>
+
+#include "host.cuh"
+
+using namespace plstvo;
+
+extern "C" {
+
+/* ---- ORB description (orb.cu) ---- */
+void plstvo_default_orb_config(PlOrbConfig* c) {
+    if (!c) return;
+    c->n_levels = 4; c->scale_factor = 1.2; c->edge_threshold = 19; c->patch_size = 31; c->wta_k = 2;
+}
+
+namespace {
+// INTER_LINEAR_EXACT taps of one axis (cv::resize's bit-exact linear interpolation): [0, dst) source offsets, then
+// [dst, 2 dst) the 8-bit weight of the second tap; 0 where the source position is left or right of the source (edge pixel)
+void orb_linear_exact_table(int src, int dst, int32_t* t) {
+    const double scale = 1.0 / ((double)dst / (double)src);
+    for (int d = 0; d < dst; ++d) {
+        const double f = scale * ((double)d + 0.5) - 0.5;
+        const int i = (int)floor(f);
+        if (i >= 0 && src > 1 && i < src - 1) {
+            t[d] = i;
+            t[dst + d] = (int32_t)lrint((f - (double)i) * 256.0);
+        } else {
+            t[d] = (i >= 0 && src > 1) ? src - 1 : 0;
+            t[dst + d] = 0;
+        }
+    }
+}
+
+int orb_check_config(PlContext* ctx, const PlOrbConfig* cfg) {
+    if (cfg->patch_size != 31) return fail(ctx, PLSTVO_E_INVALID, "patch_size must be 31");
+    if (cfg->wta_k != 2) return fail(ctx, PLSTVO_E_INVALID, "wta_k must be 2");
+    if (cfg->n_levels < 1 || cfg->n_levels > ORB_MAX_LEVELS) return fail(ctx, PLSTVO_E_INVALID, "n_levels must be 1..32");
+    if (cfg->edge_threshold < 0) return fail(ctx, PLSTVO_E_INVALID, "negative edge_threshold");
+    if (cfg->n_levels > 1 && !(cfg->scale_factor > 1.0 && cfg->scale_factor < 1e6))
+        return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1");
+    return 0;
+}
+
+// level sizes and offsets, blur taps and resize tables of the pyramid; false: a level of zero size
+bool orb_levels(const PlOrbConfig* cfg, int width, int height, OrbDevLevels& L, std::vector<int32_t>& tabs,
+                std::vector<size_t>& tab_off) {
+    L = OrbDevLevels{};
+    L.n = cfg->n_levels;
+    for (int l = 0; l < L.n; ++l) {
+        const float scale = (float)pow(cfg->scale_factor, (double)l);
+        L.inv[l] = 1.f / scale;
+        L.w[l] = (int)lrintf((float)width * L.inv[l]);
+        L.h[l] = (int)lrintf((float)height * L.inv[l]);
+        if (L.w[l] < 1 || L.h[l] < 1) return false;
+        L.raw_off[l] = l ? L.raw_stride : 0;
+        if (l) L.raw_stride += (size_t)L.w[l] * L.h[l];
+        L.blur_off[l] = L.blur_stride;
+        L.blur_stride += (size_t)L.w[l] * L.h[l];
+    }
+    {   // getGaussianKernel(7, 2, CV_32F)
+        double e[7], sum = 0;
+        for (int i = 0; i < 7; ++i) {
+            e[i] = exp(-((double)(i - 3) * (i - 3)) / (2.0 * 2.0 * 2.0));
+            sum += e[i];
+        }
+        for (int i = 0; i < 7; ++i) L.taps[i] = (float)(e[i] * (1.0 / sum));
+    }
+    tabs.clear();
+    tab_off.assign(2 * (size_t)L.n, 0);
+    for (int l = 1; l < L.n; ++l) {
+        tab_off[2 * l] = tabs.size();
+        tabs.resize(tabs.size() + 2 * (size_t)L.w[l]);
+        orb_linear_exact_table(L.w[l - 1], L.w[l], tabs.data() + tab_off[2 * l]);
+        tab_off[2 * l + 1] = tabs.size();
+        tabs.resize(tabs.size() + 2 * (size_t)L.h[l]);
+        orb_linear_exact_table(L.h[l - 1], L.h[l], tabs.data() + tab_off[2 * l + 1]);
+    }
+    return true;
+}
+
+// the launchers' rs_tab: device pointers of the x and y resize tables of levels 1 .. n - 1 (d_tabs: orb_levels' tabs uploaded)
+std::vector<const int32_t*> orb_resize_tabs(const int32_t* d_tabs, const std::vector<size_t>& tab_off, int n) {
+    std::vector<const int32_t*> rs_tab(2 * (size_t)n, nullptr);
+    for (size_t k = 2; k < rs_tab.size(); ++k) rs_tab[k] = d_tabs + tab_off[k];
+    return rs_tab;
+}
+
+cudaError_t orb_init(PlContext* ctx) {   // constant tables and timing events, once per context
+    if (ctx->orb_tables) return cudaSuccess;
+    cudaError_t e = orb_upload_tables();
+    if (e == cudaSuccess) e = ctx->orb_ev.create();
+    if (e == cudaSuccess) e = ctx->orb_det_ev.create();
+    if (e == cudaSuccess) ctx->orb_tables = true;
+    return e;
+}
+}  // namespace
+
+int plstvo_orb_compute_batch(PlContext* ctx, const PlOrbConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                             const int32_t* kp_off, const float* kp_xy, const int32_t* kp_octave, const float* kp_angle,
+                             float* out_angle, uint8_t* out_desc, int32_t* src_idx, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0) return fail(ctx, PLSTVO_E_INVALID, "null config or negative size");
+    if (const int rc = orb_check_config(ctx, cfg)) return rc;
+    if (n_img == 0) return 0;
+    const char* bad = "null images / offsets or kp_off[0] != 0";
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, bad);
+    if (const int rc = check_offsets(ctx, n_img, {kp_off}, bad, "kp_off is not non-decreasing",
+                                     "more than 65535 key points in one image"))
+        return rc;
+    const size_t N = (size_t)kp_off[n_img];
+    if (N && (!kp_xy || !kp_octave || !out_angle || !out_desc || !src_idx))
+        return fail(ctx, PLSTVO_E_INVALID, "null key point or output array");
+    for (size_t k = 0; k < N; ++k)
+        if (kp_octave[k] < 0 || kp_octave[k] >= cfg->n_levels) return fail(ctx, PLSTVO_E_INVALID, "octave outside [0, n_levels)");
+    OrbDevLevels L{};
+    std::vector<int32_t> tabs;
+    std::vector<size_t> tab_off;
+    if (!orb_levels(cfg, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, orb_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height;
+    Arena a;
+    const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
+    const size_t o_blur = a.take((size_t)n_img * L.blur_stride), o_tab = a.take(tabs.size() * 4 + 4);
+    const size_t o_off = a.take((size_t)(n_img + 1) * 4), o_xy = a.take(N * 8), o_oct = a.take(N * 4), o_ang = a.take(N * 4);
+    const size_t o_oang = a.take(N * 4), o_desc = a.take(N * 32), o_src = a.take(N * 4), o_cnt = a.take((size_t)n_img * 4);
+    CK(ctx, a.alloc(ctx->arena_orb));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(o_img, images, img_bytes, s));
+    CK(ctx, a.up(o_tab, tabs.data(), tabs.size() * 4, s));
+    CK(ctx, a.up(o_off, kp_off, (size_t)(n_img + 1) * 4, s));
+    CK(ctx, a.up(o_xy, kp_xy, N * 8, s));
+    CK(ctx, a.up(o_oct, kp_octave, N * 4, s));
+    CK(ctx, a.up(o_ang, kp_angle, N * 4, s));
+    const std::vector<const int32_t*> rs_tab = orb_resize_tabs(a.i32(o_tab), tab_off, L.n);
+    int launches = 0;
+    CK(ctx, launch_orb(L, n_img, width, height, cfg->edge_threshold, a.u8(o_img), a.u8(o_raw), a.u8(o_blur), rs_tab.data(),
+                       a.i32(o_off), (int)N, a.f32(o_xy), a.i32(o_oct), kp_angle ? a.f32(o_ang) : nullptr, a.i32(o_src),
+                       a.i32(o_cnt), a.f32(o_oang), a.u8(o_desc), s, ctx->orb_ev.ev, &launches));
+    ctx->orb_computed = true;
+    ctx->launches += launches;
+    std::vector<int32_t> cnt((size_t)n_img), src_dev(N);
+    CK(ctx, a.down(cnt.data(), o_cnt, (size_t)n_img * 4, s));
+    CK(ctx, a.down(src_dev.data(), o_src, N * 4, s));
+    std::vector<float> ang_dev(N);
+    std::vector<uint8_t> desc_dev(N * 32);
+    CK(ctx, a.down(ang_dev.data(), o_oang, N * 4, s));
+    CK(ctx, a.down(desc_dev.data(), o_desc, N * 32, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    long total = 0;
+    for (int i = 0; i < n_img; ++i) {   // survivors only: rows past counts[i] stay as the caller left them
+        const size_t r0 = (size_t)kp_off[i], n = (size_t)cnt[i];
+        if (n) {
+            memcpy(out_angle + r0, ang_dev.data() + r0, n * 4);
+            memcpy(out_desc + 32 * r0, desc_dev.data() + 32 * r0, n * 32);
+            memcpy(src_idx + r0, src_dev.data() + r0, n * 4);
+        }
+        if (counts) counts[i] = cnt[i];
+        total += cnt[i];
+    }
+    return (int)total;
+}
+
+int plstvo_orb_kernel_times(PlContext* ctx, float* ms3) {
+    if (!ctx || !ms3) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->orb_computed) return fail(ctx, PLSTVO_E_INVALID, "no ORB call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 3; ++k) CK(ctx, cudaEventElapsedTime(&ms3[k], ctx->orb_ev[k], ctx->orb_ev[k + 1]));
+    return 0;
+}
+
+/* ---- LBD description (lbd.cu) ---- */
+namespace {
+cudaError_t lbd_init(PlContext* ctx) {   // coefficient tables and timing events, once per context
+    if (ctx->lbd_tables) return cudaSuccess;
+    // BinaryDescriptor's constructor (binary_descriptor_custom.cpp:217-259) with widthOfBand_ 7, NUM_OF_BANDS 9: the
+    // centres and sigmas are integer divisions, the weights exp() in double, rounded to float where computeLBD reads them
+    float coef_l[21], coef_g[63];
+    double u = (7 * 3 - 1) / 2, sigma = (7 * 2 + 1) / 2, invsigma2 = -1 / (2 * sigma * sigma);
+    for (int i = 0; i < 21; ++i) {
+        const double dis = i - u;
+        coef_l[i] = (float)exp(dis * dis * invsigma2);
+    }
+    u = (9 * 7 - 1) / 2;
+    sigma = u;
+    invsigma2 = -1 / (2 * sigma * sigma);
+    for (int i = 0; i < 63; ++i) {
+        const double dis = i - u;
+        coef_g[i] = (float)exp(dis * dis * invsigma2);
+    }
+    cudaError_t e = lbd_upload_tables(coef_g, coef_l);
+    if (e == cudaSuccess) e = ctx->lbd_ev.create();
+    if (e == cudaSuccess) ctx->lbd_tables = true;
+    return e;
+}
+
+// key lines of n_img consecutive images: kl_off [n_img + 1] and the per-line arrays
+struct LineSrc {
+    int n_img; const int32_t* off; const float* seg; const float* angle; const int32_t* npix;
+};
+
+// the key-line checks of plstvo_lbd_compute_batch on one LineSrc (the arrays only where lines exist)
+int lbd_check_lines(PlContext* ctx, const LineSrc& l) {
+    if (const int rc = check_offsets(ctx, l.n_img, {l.off}, "null offsets or kl_off[0] != 0", "kl_off is not non-decreasing",
+                                     "more than 65535 key lines in one image"))
+        return rc;
+    const size_t N = (size_t)l.off[l.n_img];
+    if (N && (!l.seg || !l.angle || !l.npix)) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
+    for (size_t k = 0; k < N; ++k)
+        if (l.npix[k] < 1 || l.npix[k] > 32767) return fail(ctx, PLSTVO_E_INVALID, "numOfPixels must be 1..32767");
+    return 0;
+}
+
+struct ImgPart {   // consecutive host images of one size
+    const uint8_t* p; int n;
+};
+
+// Enqueues LBD description on stream s for checked key lines (parts, in image order; at least one line in all) of images of one
+// size: either device images (d_img, ready once img_ready has completed) or host images that go into arena_lbd (img_parts).
+// Leaves the key lines' segments (sPointInOctave, ePointInOctave as given) and descriptors in arena_lbd.
+int lbd_enqueue(PlContext* ctx, int width, int height, const std::vector<LineSrc>& parts, const uint8_t* d_img,
+                cudaEvent_t img_ready, const std::vector<ImgPart>& img_parts, cudaStream_t s, const float** d_seg,
+                const uint8_t** d_desc) {
+    int n_img = 0;
+    std::vector<int32_t> off(1, 0);
+    for (const LineSrc& l : parts) {
+        for (int i = 0; i < l.n_img; ++i) off.push_back(off.back() + l.off[i + 1] - l.off[i]);
+        n_img += l.n_img;
+    }
+    const size_t N = (size_t)off.back();
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, lbd_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height;
+    Arena a;
+    const size_t o_img = a.take(d_img ? 0 : img_bytes), o_grad = a.take(img_bytes * 4), o_off = a.take((size_t)(n_img + 1) * 4);
+    const size_t o_seg = a.take(N * 16), o_dir = a.take(N * 8), o_npix = a.take(N * 4), o_desc = a.take(N * 32);
+    CK(ctx, a.alloc(ctx->arena_lbd));
+    if (!d_img) {
+        size_t o = o_img;
+        for (const ImgPart& ip : img_parts) {
+            const size_t bytes = (size_t)ip.n * width * height;
+            CK(ctx, cudaMemcpyAsync(a.u8(o), ip.p, bytes, cudaMemcpyHostToDevice, s));
+            o += bytes;
+        }
+    }
+    CK(ctx, cudaMemcpyAsync(a.u8(o_off), off.data(), (size_t)(n_img + 1) * 4, cudaMemcpyHostToDevice, s));
+    // dL = (cos, sin) of the float angle.  The reference's unqualified cos(float) / sin(float) bind to std::cos(float) /
+    // std::sin(float), the C library's cosf / sinf (its translation unit includes <math.h>, whose C++ form puts the float
+    // overloads into the global namespace), and GCC merges the pair into sincosf.  They are evaluated here, with the same
+    // library, because no device function rounds them the same way.
+    std::vector<float> dir(2 * N);
+    size_t r = 0;
+    for (const LineSrc& l : parts) {
+        const size_t n = (size_t)l.off[l.n_img];
+        if (!n) continue;
+        CK(ctx, cudaMemcpyAsync(a.u8(o_seg) + r * 16, l.seg, n * 16, cudaMemcpyHostToDevice, s));
+        const float* kl_angle = l.angle;
+        float* d = dir.data() + 2 * r;
+        for (size_t k = 0; k < n; ++k) sincosf(kl_angle[k], &d[2 * k + 1], &d[2 * k]);
+        r += n;
+    }
+    CK(ctx, cudaMemcpyAsync(a.u8(o_dir), dir.data(), N * 8, cudaMemcpyHostToDevice, s));
+    r = 0;
+    for (const LineSrc& l : parts) {
+        const size_t n = (size_t)l.off[l.n_img];
+        if (n) CK(ctx, cudaMemcpyAsync(a.u8(o_npix) + r * 4, l.npix, n * 4, cudaMemcpyHostToDevice, s));
+        r += n;
+    }
+    if (d_img && img_ready) CK(ctx, cudaStreamWaitEvent(s, img_ready, 0));
+    int launches = 0;
+    CK(ctx, launch_lbd(n_img, width, height, d_img ? d_img : a.u8(o_img), a.i32(o_off), (int)N, a.f32(o_seg),
+                       a.at<float2>(o_dir), a.i32(o_npix), a.at<short2>(o_grad), a.u8(o_desc), s, ctx->lbd_ev.ev, &launches));
+    ctx->lbd_computed = true;
+    ctx->launches += launches;
+    *d_seg = a.f32(o_seg);
+    *d_desc = a.u8(o_desc);
+    return 0;
+}
+}  // namespace
+
+int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, const uint8_t* images, const int32_t* kl_off,
+                             const float* kl_seg, const float* kl_angle, const int32_t* kl_npix, uint8_t* out_desc) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (n_img < 0) return fail(ctx, PLSTVO_E_INVALID, "negative n_img");
+    // the reference indexes pixels and counts samples in short
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+    if (n_img == 0) return 0;
+    const LineSrc lines{n_img, kl_off, kl_seg, kl_angle, kl_npix};
+    if (const int rc = lbd_check_lines(ctx, lines)) return rc;
+    const size_t N = (size_t)kl_off[n_img];
+    if (N == 0) return 0;
+    if (!images || !out_desc) return fail(ctx, PLSTVO_E_INVALID, "null image or key line array");
+    cudaStream_t s = ctx->s_main;
+    const float* d_seg = nullptr;
+    const uint8_t* d_desc = nullptr;
+    if (const int rc = lbd_enqueue(ctx, width, height, {lines}, nullptr, nullptr, {ImgPart{images, n_img}}, s, &d_seg, &d_desc))
+        return rc;
+    CK(ctx, cudaMemcpyAsync(out_desc, d_desc, N * 32, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return (int)N;
+}
+
+int plstvo_lbd_kernel_times(PlContext* ctx, float* ms2) {
+    if (!ctx || !ms2) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->lbd_computed) return fail(ctx, PLSTVO_E_INVALID, "no LBD call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 2; ++k) CK(ctx, cudaEventElapsedTime(&ms2[k], ctx->lbd_ev[k], ctx->lbd_ev[k + 1]));
+    return 0;
+}
+
+/* ---- ORB key-point selection + description (orb.cu) ---- */
+void plstvo_default_orb_detect_config(PlOrbDetectConfig* c) {
+    if (!c) return;
+    plstvo_default_orb_config(&c->orb);
+    c->n_features = 1200; c->score_type = 1; c->fast_threshold = 20;
+}
+
+namespace {
+int orb_detect_check(PlContext* ctx, const PlOrbDetectConfig* cfg) {
+    if (const int rc = orb_check_config(ctx, &cfg->orb)) return rc;
+    if (cfg->n_features < 0) return fail(ctx, PLSTVO_E_INVALID, "negative n_features");
+    if (cfg->score_type != 0 && cfg->score_type != 1) return fail(ctx, PLSTVO_E_INVALID, "score_type must be 0 (Harris) or 1 (FAST)");
+    return 0;
+}
+
+// key points of an ORB detect call, left in HBM (CSR by image, arena_orb_kp) with the host copy of the offsets
+struct OrbDetected {
+    std::vector<int32_t> off;   // [n_img + 1]; also written in full when the call fails with PLSTVO_E_TOO_LARGE
+    const float *xy = nullptr, *angle = nullptr, *response = nullptr;
+    const int32_t* octave = nullptr;
+    const uint8_t* desc = nullptr;
+};
+
+// Uploads n_img (> 0) host images (parts, in order) into arena_orb and enqueues detection and description on s_main, for a
+// checked config and per-image FAST thresholds th (clamped here).  `beside` (optional) is called with the device images and an
+// event that completes once they are uploaded, after the pyramid and FAST launches are enqueued and before the first offsets
+// readback blocks this thread: work enqueued there on another stream overlaps those stages.
+int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                       const std::vector<ImgPart>& parts, const int32_t* fast_th, int capacity,
+                       const std::function<int(const uint8_t*, cudaEvent_t)>& beside, OrbDetected& out) {
+    PlOrbConfig oc = cfg->orb;
+    oc.scale_factor = (double)(float)oc.scale_factor;   // ORB::create takes a float scale factor
+    if (oc.n_levels > 1 && !(oc.scale_factor > 1.0)) return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1 in float");
+    OrbDevLevels L{};
+    std::vector<int32_t> tabs;
+    std::vector<size_t> tab_off;
+    if (!orb_levels(&oc, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    const int nl = L.n;
+    const bool harris = cfg->score_type == 0;
+    OrbDetectLevels D{};
+    {   // the per-level budget, in float as ORB computes it
+        const float factor = (float)(1.0 / oc.scale_factor);
+        float nd = (float)cfg->n_features * (1.f - factor) / (1.f - (float)pow((double)factor, (double)nl));
+        int sum = 0;
+        for (int l = 0; l < nl; ++l) {
+            int n = 0;
+            if (l < nl - 1) {
+                n = (int)lrintf(nd);
+                sum += n;
+                nd *= factor;
+            } else {
+                n = std::max(cfg->n_features - sum, 0);
+            }
+            D.keep1[l] = harris ? 2 * n : n;
+            D.keep2[l] = n;
+            D.row0[l + 1] = D.row0[l] + L.h[l];
+            D.layer_scale[l] = (float)pow(oc.scale_factor, (double)l);
+        }
+        D.edge = cfg->orb.edge_threshold;
+        const float hs = 1.f / (28 * 255.f);   // 1 / ((1 << 2) * blockSize * 255), blockSize 7
+        D.harris_scale4 = hs * hs * hs * hs;
+    }
+    const int R = D.row0[nl];
+    std::vector<int32_t> th((size_t)n_img);
+    for (int i = 0; i < n_img; ++i) th[i] = std::min(std::max(fast_th[i], 0), 255);
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, orb_init(ctx));
+    const size_t img_bytes = (size_t)n_img * width * height, NL = (size_t)n_img * nl;
+    Arena a;
+    const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
+    const size_t o_blur = a.take((size_t)n_img * L.blur_stride), o_tab = a.take(tabs.size() * 4 + 4);
+    const size_t o_score = a.take((size_t)n_img * L.blur_stride), o_hist = a.take(NL * 256 * 4), o_cut = a.take(NL * 4);
+    const size_t o_rcnt = a.take((size_t)n_img * R * 4), o_rbase = a.take((size_t)n_img * (R + 1) * 4);
+    const size_t o_icnt = a.take((size_t)n_img * 4), o_soff = a.take((size_t)(n_img + 1) * 4), o_th = a.take((size_t)n_img * 4);
+    const size_t o_lkeep = a.take(NL * 4), o_ckey = a.take(NL * 4), o_hoff = a.take((size_t)(n_img + 1) * 4);
+    const size_t o_hcnt = a.take((size_t)n_img * 4);
+    CK(ctx, a.alloc(ctx->arena_orb));
+    cudaStream_t s = ctx->s_main;
+    {
+        size_t o = o_img;
+        for (const ImgPart& ip : parts) {
+            const size_t bytes = (size_t)ip.n * width * height;
+            CK(ctx, cudaMemcpyAsync(a.u8(o), ip.p, bytes, cudaMemcpyHostToDevice, s));
+            o += bytes;
+        }
+    }
+    cudaEvent_t uploaded = nullptr;
+    if (beside) {
+        uploaded = next_event(ctx);
+        CK(ctx, cudaEventRecord(uploaded, s));
+    }
+    CK(ctx, a.up(o_tab, tabs.data(), tabs.size() * 4, s));
+    CK(ctx, a.up(o_th, th.data(), (size_t)n_img * 4, s));
+    const std::vector<const int32_t*> rs_tab = orb_resize_tabs(a.i32(o_tab), tab_off, nl);
+    cudaEvent_t* ev = ctx->orb_det_ev.ev;   // [0] start, [1] pyramid + blur, [2] FAST + NMS, [3] selection, [4] angle + descriptor
+    int launches = 0;
+    CK(ctx, cudaEventRecord(ev[0], s));
+    launch_orb_pyramid(L, n_img, a.u8(o_img), a.u8(o_raw), a.u8(o_blur), rs_tab.data(), s, &launches);
+    CK(ctx, cudaEventRecord(ev[1], s));
+    launch_orb_fast_select(L, D, n_img, a.u8(o_img), a.u8(o_raw), a.i32(o_th), a.u8(o_score),
+                           a.at<uint32_t>(o_hist), a.i32(o_cut), a.i32(o_rcnt), a.i32(o_rbase), a.i32(o_icnt), a.i32(o_soff), s,
+                           ev[2], &launches);
+    CK(ctx, cudaGetLastError());
+    if (beside)
+        if (const int rc = beside(a.u8(o_img), uploaded)) return rc;
+    std::vector<int32_t>& off = out.off;
+    off.assign((size_t)n_img + 1, 0);
+    CK(ctx, cudaMemcpyAsync(off.data(), a.i32(o_soff), off.size() * 4, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    ctx->launches += launches;
+    launches = 0;
+    ctx->orb_detected = true;
+    // too many key points: the offsets in full (the caller sizes its buffers from them), no key points
+    auto too_large = [&]() -> int {
+        CK(ctx, cudaEventRecord(ev[3], s));
+        CK(ctx, cudaEventRecord(ev[4], s));
+        for (int i = 0; i < n_img; ++i)
+            if (off[i + 1] - off[i] > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key points in one image");
+        if (off[n_img] > capacity) return fail(ctx, PLSTVO_E_TOO_LARGE, "more key points than capacity");
+        return 0;
+    };
+    auto exceeds = [&]() {
+        if (off[n_img] > capacity) return true;
+        for (int i = 0; i < n_img; ++i)
+            if (off[i + 1] - off[i] > PLSTVO_MAX_FEATURES) return true;
+        return false;
+    };
+    if (!harris && exceeds()) return too_large();
+    const size_t N1 = (size_t)off[n_img];
+    Arena b;
+    const size_t o_lxy = b.take(N1 * 8), o_xy = b.take(N1 * 8), o_oct = b.take(N1 * 4), o_resp = b.take(N1 * 4);
+    const size_t o_rank = b.take(N1 * 4), o_hresp = b.take(harris ? N1 * 4 : 0), o_fxy = b.take(harris ? N1 * 8 : 0);
+    const size_t o_foct = b.take(harris ? N1 * 4 : 0), o_fresp = b.take(harris ? N1 * 4 : 0);
+    const size_t o_frank = b.take(harris ? N1 * 4 : 0), o_ang = b.take(N1 * 4), o_desc = b.take(N1 * 32);
+    CK(ctx, b.alloc(ctx->arena_orb_kp));
+    launch_orb_fast_write(L, D, n_img, a.u8(o_score), a.i32(o_cut), a.i32(o_rbase), a.i32(o_soff), b.at<int2>(o_lxy),
+                          b.f32(o_xy), b.i32(o_oct), b.f32(o_resp), b.i32(o_rank), s, &launches);
+    const int32_t *d_off = a.i32(o_soff), *d_cnt = a.i32(o_icnt), *d_oct = b.i32(o_oct), *d_rank = b.i32(o_rank);
+    const float *d_xy = b.f32(o_xy), *d_resp = b.f32(o_resp);
+    if (harris) {
+        uint32_t* ckey = a.at<uint32_t>(o_ckey);
+        launch_orb_harris_select(L, D, n_img, (int)N1, a.u8(o_img), a.u8(o_raw), a.i32(o_rbase), a.i32(o_soff),
+                                 b.at<int2>(o_lxy), b.i32(o_oct), b.f32(o_hresp), ckey, a.i32(o_lkeep), a.i32(o_hoff),
+                                 a.i32(o_hcnt), s, &launches);
+        CK(ctx, cudaGetLastError());
+        CK(ctx, cudaMemcpyAsync(off.data(), a.i32(o_hoff), off.size() * 4, cudaMemcpyDeviceToHost, s));
+        CK(ctx, cudaStreamSynchronize(s));
+        ctx->launches += launches;
+        launches = 0;
+        if (exceeds()) return too_large();
+        launch_orb_harris_write(L, D, n_img, a.i32(o_soff), b.f32(o_xy), b.i32(o_oct), b.f32(o_hresp), ckey, a.i32(o_hoff),
+                                b.f32(o_fxy), b.i32(o_foct), b.f32(o_fresp), b.i32(o_frank), s, &launches);
+        d_off = a.i32(o_hoff); d_cnt = a.i32(o_hcnt); d_oct = b.i32(o_foct); d_rank = b.i32(o_frank); d_xy = b.f32(o_fxy);
+        d_resp = b.f32(o_fresp);
+    }
+    CK(ctx, cudaEventRecord(ev[3], s));
+    const size_t N = (size_t)off[n_img];
+    launch_orb_describe(L, n_img, a.u8(o_img), a.u8(o_raw), a.u8(o_blur), d_off, (int)N, d_xy, d_oct, nullptr, d_rank, d_cnt,
+                        b.f32(o_ang), b.u8(o_desc), s, &launches);
+    CK(ctx, cudaEventRecord(ev[4], s));
+    CK(ctx, cudaGetLastError());
+    ctx->launches += launches;
+    out.xy = d_xy; out.octave = d_oct; out.angle = b.f32(o_ang); out.response = d_resp; out.desc = b.u8(o_desc);
+    return 0;
+}
+}  // namespace
+
+int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+                                        const uint8_t* images, const int32_t* fast_th, int capacity, int32_t* kp_off,
+                                        float* kp_xy, int32_t* kp_octave, float* kp_angle, float* kp_response, uint8_t* desc) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || width < 0 || height < 0 || capacity < 0)
+        return fail(ctx, PLSTVO_E_INVALID, "null config, negative size or negative capacity");
+    if (const int rc = orb_detect_check(ctx, cfg)) return rc;
+    if (!kp_off) return fail(ctx, PLSTVO_E_INVALID, "null kp_off");
+    kp_off[0] = 0;
+    if (n_img == 0) return 0;
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    std::vector<int32_t> th((size_t)n_img, cfg->fast_threshold);
+    if (fast_th) std::copy(fast_th, fast_th + n_img, th.begin());
+    OrbDetected o;
+    const int rc = orb_detect_enqueue(ctx, cfg, n_img, width, height, {ImgPart{images, n_img}}, th.data(), capacity, nullptr, o);
+    if (rc == PLSTVO_E_TOO_LARGE && o.off.size() == (size_t)n_img + 1) memcpy(kp_off, o.off.data(), o.off.size() * 4);
+    if (rc) return rc;
+    const size_t N = (size_t)o.off[n_img];
+    cudaStream_t s = ctx->s_main;
+    auto down = [&](void* dst, const void* src, size_t bytes) -> cudaError_t {
+        return (dst && bytes) ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    };
+    CK(ctx, down(kp_xy, o.xy, N * 8));
+    CK(ctx, down(kp_octave, o.octave, N * 4));
+    CK(ctx, down(kp_angle, o.angle, N * 4));
+    CK(ctx, down(kp_response, o.response, N * 4));
+    CK(ctx, down(desc, o.desc, N * 32));
+    CK(ctx, cudaStreamSynchronize(s));
+    memcpy(kp_off, o.off.data(), o.off.size() * 4);
+    return (int)N;
+}
+
+/* ---- stereo images -> pose: ORB and LBD feed the stereo step and the tracker without leaving HBM ---- */
+// The images go up once into arena_orb in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left]
+// [curr right].  Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.
+static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                            const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
+                            const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
+                            bool sequence) {
+    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
+        return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    const int NF = prev->B;
+    if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
+    if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (const int rc = orb_detect_check(ctx, oc)) return rc;
+    const int nfs = sequence ? 1 : 2;   // frame sets: the sequence, or prev and curr
+    const PlStereoImages* fs[2] = {prev, curr};
+    const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0;
+    const int W = cam->width, H = cam->height;
+    std::vector<LineSrc> lsrc;   // key lines per image block
+    if (NF > 0) {
+        for (int j = 0; j < nfs; ++j) {
+            // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
+            if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
+            if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
+        }
+        if (lns) {
+            if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+            for (int j = 0; j < nfs; ++j) {
+                lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
+                lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
+            }
+            for (const LineSrc& l : lsrc)
+                if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        }
+    }
+    if (NF == 0 || (sequence && NF == 1)) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, ctx->img_ev.create());
+    CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
+    ctx->img_timed = false;
+    const int nblk = 2 * nfs, n_img = nblk * NF;
+    std::vector<ImgPart> iparts;
+    std::vector<int32_t> th((size_t)n_img), lbase((size_t)nblk + 1, 0);
+    for (int b = 0; b < nblk; ++b) {
+        const PlStereoImages* f = fs[b / 2];
+        iparts.push_back(ImgPart{b % 2 ? f->img_r : f->img_l, NF});
+        for (int i = 0; i < NF; ++i)   // 0 = the configured threshold, as detectPointFeatures / plstvo::detectAndComputeORB
+            th[(size_t)b * NF + i] = f->fast_th && f->fast_th[i] ? f->fast_th[i] : oc->fast_threshold;
+        lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
+    }
+    const bool run_lbd = lbase[nblk] > 0;
+    const float* d_seg = nullptr;
+    const uint8_t* d_ldesc = nullptr;
+    // LBD on the second stream; with ORB running it reads ORB's copy of the images once their upload has completed
+    auto enqueue_lbd = [&](const uint8_t* d_img, cudaEvent_t ready) -> int {
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, iparts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+        CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
+        return 0;
+    };
+    CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
+    OrbDetected orb;
+    if (pts) {
+        std::function<int(const uint8_t*, cudaEvent_t)> beside;
+        if (run_lbd) beside = enqueue_lbd;
+        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, iparts, th.data(), INT_MAX, beside, orb)) return rc;
+    } else {
+        orb.off.assign((size_t)n_img + 1, 0);
+        if (run_lbd)
+            if (const int rc = enqueue_lbd(nullptr, nullptr)) return rc;
+    }
+    // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
+    std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
+    PlStereoFeatures feat[2]{};
+    StereoDevInputs dev;
+    for (int j = 0; j < nfs; ++j) {
+        const int bl = 2 * j, br = 2 * j + 1;
+        const size_t kl = orb.off[(size_t)bl * NF], kr = orb.off[(size_t)br * NF];
+        pl_off[j].resize((size_t)NF + 1);
+        pr_off[j].resize((size_t)NF + 1);
+        for (int i = 0; i <= NF; ++i) {
+            pl_off[j][i] = orb.off[(size_t)bl * NF + i] - (int32_t)kl;
+            pr_off[j][i] = orb.off[(size_t)br * NF + i] - (int32_t)kr;
+        }
+        PlStereoFeatures& F = feat[j];
+        F.B = NF;
+        F.pl_off = pl_off[j].data(); F.pr_off = pr_off[j].data();
+        F.ll_off = lns ? fs[j]->ll_off : none.data(); F.lr_off = lns ? fs[j]->lr_off : none.data();
+        F.angle_l = lns ? fs[j]->angle_l : nullptr;
+        StereoDevInputs::Set& P = dev.set[2 * j];
+        P.on_device = true;
+        if (pts) {
+            P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
+            P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
+        }
+        StereoDevInputs::Set& Ls = dev.set[2 * j + 1];
+        Ls.on_device = true;   // oct stays null: key lines of octave 0
+        if (run_lbd) {
+            Ls.xy_l = d_seg + 4 * (size_t)lbase[bl]; Ls.xy_r = d_seg + 4 * (size_t)lbase[br];
+            Ls.d1 = d_ldesc + 32 * (size_t)lbase[bl]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[br];
+        }
+    }
+    dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
+    dev.marks = ctx->img_ev.ev + 1;
+    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], sequence ? nullptr : &feat[1], priors, results,
+                                           n_stereo, sequence, -1, &dev))
+        return rc;
+    float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
+    std::fill(ms, ms + 5, 0.f);
+    // uploads end where the first stage starts: LBD waits for the images and its key lines, ORB for the images only
+    const cudaEvent_t up_end = run_lbd ? ctx->lbd_ev[0] : pts ? ctx->orb_det_ev[0] : nullptr;
+    if (up_end) CK(ctx, cudaEventElapsedTime(&ms[0], ctx->img_ev[0], up_end));
+    if (pts) CK(ctx, cudaEventElapsedTime(&ms[1], ctx->orb_det_ev[0], ctx->orb_det_ev[4]));
+    if (run_lbd) CK(ctx, cudaEventElapsedTime(&ms[2], ctx->lbd_ev[0], ctx->lbd_ev[2]));
+    CK(ctx, cudaEventElapsedTime(&ms[3], ctx->img_ev[1], ctx->img_ev[2]));
+    CK(ctx, cudaEventElapsedTime(&ms[4], ctx->img_ev[2], ctx->img_ev[3]));
+    ctx->img_timed = true;
+    return 0;
+}
+
+static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                               const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
+                               const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
+                               bool sequence) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, prev, curr, priors, results, n_stereo, sequence);
+    // LBD may still run on the second stream after an error: the next call may reuse its arena
+    const cudaError_t e = cudaStreamSynchronize(ctx->s_alt);
+    if (rc) return rc;
+    CK(ctx, e);
+    return 0;
+}
+
+int plstvo_track_stereo_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                     const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* prev,
+                                     const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, prev, curr, priors, results, n_stereo, false);
+}
+
+int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                        const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
+                                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {
+    if (!ctx || !ms5) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->img_timed) return fail(ctx, PLSTVO_E_INVALID, "no images call on this context yet");
+    memcpy(ms5, ctx->img_ms, sizeof(ctx->img_ms));
+    return 0;
+}
+
+int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4) {
+    if (!ctx || !ms4) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->orb_detected) return fail(ctx, PLSTVO_E_INVALID, "no ORB detect call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 4; ++k) CK(ctx, cudaEventElapsedTime(&ms4[k], ctx->orb_det_ev[k], ctx->orb_det_ev[k + 1]));
+    return 0;
+}
+
+}  // extern "C"

@@ -1,0 +1,554 @@
+// capi_stereo.cu — the C-ABI's stereo step: matchGrid, 3-D lifting, matchStereo in one device pass, and pose tracking from
+// raw stereo features (the stereo step feeding the tracker without leaving HBM).
+#include "host.cuh"
+
+using namespace plstvo;
+
+namespace {
+
+int check_stereo_offsets(PlContext* ctx, int B, const int32_t* l_off, const int32_t* r_off) {
+    return check_offsets(ctx, B, {l_off, r_off}, "bad offsets", "offsets are not non-decreasing", "more than 65535 features");
+}
+
+}  // namespace
+
+extern "C" {
+
+// ---- matchGrid (stereo step) -------------------------------------------------------------------------------------
+static int match_grid_common(PlContext* ctx, bool lines, int B, int rows, int cols, PlGridWindow w, int best_lr,
+                             double ratio, double line_sim_th, const int32_t* q_off, const int32_t* q_cell,
+                             const uint8_t* d1, const int32_t* t_off, const int32_t* t_cell, const double* t_line,
+                             const double* t_dir, const uint8_t* d2, int32_t* m12, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (B < 0 || !grid_ok(rows, cols)) return fail(ctx, PLSTVO_E_INVALID, "bad grid");
+    if (B == 0) return 0;
+    if (!m12) return fail(ctx, PLSTVO_E_INVALID, "bad offsets");
+    if (const int rc = check_stereo_offsets(ctx, B, q_off, t_off)) return rc;
+    CK(ctx, cudaSetDevice(ctx->device));
+    const int qw = lines ? 4 : 2;
+    const size_t N1 = q_off[B], N2 = t_off[B];
+    if ((N1 && (!q_cell || !d1)) || (N2 && (!d2 || (lines ? (!t_line || !t_dir) : !t_cell))))
+        return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    // one arena for inputs, outputs and scratch
+    Arena a;
+    const size_t o_d1 = a.take(N1 * 32), o_d2 = a.take(N2 * 32), o_m12 = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    const GridScratch g(a, rows, cols, B, N1, N2, N2 * grid_cells_per_train(lines, rows, cols), !lines, lines);
+    const size_t o_prob = a.take((size_t)B * sizeof(GridProblem));
+    CK(ctx, a.alloc(ctx->arena_grid));
+    std::vector<GridProblem> probs((size_t)B);
+    g.fill(probs.data(), B, lines, q_off, t_off, a.u8(o_d1), a.u8(o_d2), a.i32(o_m12), a.i32(o_cnt));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(g.qcell, q_cell, N1 * qw * 4, s));
+    CK(ctx, a.up(o_d1, d1, N1 * 32, s));
+    CK(ctx, a.up(o_d2, d2, N2 * 32, s));
+    if (lines) {
+        CK(ctx, a.up(g.tline, t_line, N2 * 32, s));
+        CK(ctx, a.up(g.tdir, t_dir, N2 * 16, s));
+    } else {
+        CK(ctx, a.up(g.tcell, t_cell, N2 * 8, s));
+    }
+    CK(ctx, a.up(o_prob, probs.data(), (size_t)B * sizeof(GridProblem), s));
+    GridParams prm{rows, cols, GRID_CAP, best_lr ? 1 : 0, w, ratio, line_sim_th};
+    CK(ctx, launch_match_grid(a.at<GridProblem>(o_prob), B, prm, lines, s));
+    ctx->launches++;
+    CK(ctx, a.down(m12, o_m12, N1 * 4, s));
+    return counts_total(ctx, s, B, a.i32(o_cnt), counts, a.i32(o_cnt));
+}
+
+int plstvo_match_grid_points(PlContext* ctx, int B, int grid_rows, int grid_cols, PlGridWindow w, int best_lr_matches,
+                             double min_ratio_12_p, const int32_t* q_off, const int32_t* q_cell, const uint8_t* d1,
+                             const int32_t* t_off, const int32_t* t_cell, const uint8_t* d2, int32_t* m12,
+                             int32_t* counts) {
+    return match_grid_common(ctx, false, B, grid_rows, grid_cols, w, best_lr_matches, min_ratio_12_p, 0.0, q_off, q_cell, d1,
+                             t_off, t_cell, nullptr, nullptr, d2, m12, counts);
+}
+
+int plstvo_match_grid_lines(PlContext* ctx, int B, int grid_rows, int grid_cols, PlGridWindow w, int best_lr_matches,
+                            double min_ratio_12_p, double line_sim_th, const int32_t* q_off, const int32_t* q_line,
+                            const uint8_t* d1, const int32_t* t_off, const double* t_line, const double* t_dir,
+                            const uint8_t* d2, int32_t* m12, int32_t* counts) {
+    return match_grid_common(ctx, true, B, grid_rows, grid_cols, w, best_lr_matches, min_ratio_12_p, line_sim_th, q_off,
+                             q_line, d1, t_off, nullptr, t_line, t_dir, d2, m12, counts);
+}
+
+// ---- 3-D lifting of the stereo matches (src/stereoFrame.cpp:149-172, :348-397) ------------------------------
+void plstvo_default_stereo_config(PlStereoConfig* c) {   // src/config.cpp:58-69, :96, :106
+    if (!c) return;
+    c->max_dist_epip = 1.0; c->min_disp = 1.0; c->ls_min_disp_ratio = 0.7; c->line_horiz_th = 0.1;
+    c->stereo_overlap_th = 0.75; c->orb_scale_factor = 1.2; c->lsd_scale = 1.2;
+}
+
+int plstvo_stereo_lift_points(PlContext* ctx, const PlCamera* cam, const PlStereoConfig* scfg, int B, const int32_t* l_off,
+                              const float* kp_l, const int32_t* octave_l, const uint8_t* desc_l, const int32_t* r_off,
+                              const float* kp_r, const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P,
+                              double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cam || !scfg || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
+    if (B == 0) return 0;
+    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
+    const size_t N1 = l_off[B], N2 = r_off[B];
+    if (N1 && (!kp_l || !octave_l || !desc_l || !m12)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    if (N2 && !kp_r) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    CK(ctx, cudaSetDevice(ctx->device));
+    Arena a;
+    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_kpl = a.take(N1 * 8);
+    const size_t o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_kpr = a.take(N2 * 8), o_m12 = a.take(N1 * 4);
+    const size_t o_pl = a.take(N1 * 16), o_disp = a.take(N1 * 8), o_P = a.take(N1 * 24), o_s2 = a.take(N1 * 8);
+    const size_t o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32), o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    CK(ctx, a.alloc(ctx->arena_lift_pt));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_kpl, kp_l, N1 * 8, s));
+    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
+    CK(ctx, a.up(o_desc, desc_l, N1 * 32, s));
+    CK(ctx, a.up(o_kpr, kp_r, N2 * 8, s));
+    CK(ctx, a.up(o_m12, m12, N1 * 4, s));
+    CK(ctx, launch_lift_points(*cam, *scfg, B, a.i32(o_loff), a.f32(o_kpl), a.i32(o_oct), a.u8(o_desc), a.i32(o_roff),
+                               a.f32(o_kpr), a.i32(o_m12), a.f64(o_pl), a.f64(o_disp), a.f64(o_P), a.f64(o_s2), a.i32(o_lvl),
+                               a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+    ctx->launches++;
+    CK(ctx, a.down(pt_pl, o_pl, N1 * 16, s));
+    CK(ctx, a.down(pt_disp, o_disp, N1 * 8, s));
+    CK(ctx, a.down(pt_P, o_P, N1 * 24, s));
+    CK(ctx, a.down(pt_sigma2, o_s2, N1 * 8, s));
+    CK(ctx, a.down(pt_level, o_lvl, N1 * 4, s));
+    CK(ctx, a.down(pdesc_out, o_dout, N1 * 32, s));
+    CK(ctx, a.down(src_idx, o_src, N1 * 4, s));
+    return counts_total(ctx, s, B, a.i32(o_cnt), counts);
+}
+
+int plstvo_stereo_lift_lines(PlContext* ctx, const PlCamera* cam, const PlStereoConfig* scfg, int B, const int32_t* l_off,
+                             const float* seg_l, const float* angle_l, const int32_t* octave_l, const uint8_t* desc_l,
+                             const int32_t* r_off, const float* seg_r, const int32_t* m12, double* ls_spl, double* ls_epl,
+                             double* ls_sdisp, double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le,
+                             double* ls_angle, double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx,
+                             int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cam || !scfg || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
+    if (B == 0) return 0;
+    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
+    const size_t N1 = l_off[B], N2 = r_off[B];
+    if (N1 && (!seg_l || !angle_l || !octave_l || !desc_l || !m12)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    if (N2 && !seg_r) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    CK(ctx, cudaSetDevice(ctx->device));
+    Arena a;
+    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_segl = a.take(N1 * 16);
+    const size_t o_ang = a.take(N1 * 4), o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_segr = a.take(N2 * 16);
+    const size_t o_m12 = a.take(N1 * 4), o_spl = a.take(N1 * 16), o_epl = a.take(N1 * 16), o_sd = a.take(N1 * 8);
+    const size_t o_ed = a.take(N1 * 8), o_sP = a.take(N1 * 24), o_eP = a.take(N1 * 24), o_le = a.take(N1 * 24);
+    const size_t o_angd = a.take(N1 * 8), o_s2 = a.take(N1 * 8), o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32);
+    const size_t o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    CK(ctx, a.alloc(ctx->arena_lift_ls));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_segl, seg_l, N1 * 16, s));
+    CK(ctx, a.up(o_ang, angle_l, N1 * 4, s));
+    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
+    CK(ctx, a.up(o_desc, desc_l, N1 * 32, s));
+    CK(ctx, a.up(o_segr, seg_r, N2 * 16, s));
+    CK(ctx, a.up(o_m12, m12, N1 * 4, s));
+    CK(ctx, launch_lift_lines(*cam, *scfg, B, a.i32(o_loff), a.f32(o_segl), a.f32(o_ang), a.i32(o_oct), a.u8(o_desc),
+                              a.i32(o_roff), a.f32(o_segr), a.i32(o_m12), a.f64(o_spl), a.f64(o_epl), a.f64(o_sd), a.f64(o_ed),
+                              a.f64(o_sP), a.f64(o_eP), a.f64(o_le), a.f64(o_angd), a.f64(o_s2), a.i32(o_lvl), a.u8(o_dout),
+                              a.i32(o_src), a.i32(o_cnt), s));
+    ctx->launches++;
+    CK(ctx, a.down(ls_spl, o_spl, N1 * 16, s));
+    CK(ctx, a.down(ls_epl, o_epl, N1 * 16, s));
+    CK(ctx, a.down(ls_sdisp, o_sd, N1 * 8, s));
+    CK(ctx, a.down(ls_edisp, o_ed, N1 * 8, s));
+    CK(ctx, a.down(ls_sP, o_sP, N1 * 24, s));
+    CK(ctx, a.down(ls_eP, o_eP, N1 * 24, s));
+    CK(ctx, a.down(ls_le, o_le, N1 * 24, s));
+    CK(ctx, a.down(ls_angle, o_angd, N1 * 8, s));
+    CK(ctx, a.down(ls_sigma2, o_s2, N1 * 8, s));
+    CK(ctx, a.down(ls_level, o_lvl, N1 * 4, s));
+    CK(ctx, a.down(ldesc_out, o_dout, N1 * 32, s));
+    CK(ctx, a.down(src_idx, o_src, N1 * 4, s));
+    return counts_total(ctx, s, B, a.i32(o_cnt), counts);
+}
+
+// ---- matchStereoPoints / matchStereoLines in one device pass (src/stereoFrame.cpp:120-173, :309-398) ----------------
+void plstvo_default_stereo_match_config(PlStereoMatchConfig* c) {   // include/stereoFrame.h:51-52, src/config.cpp:51, :60, :63, :91
+    if (!c) return;
+    c->grid_rows = 48; c->grid_cols = 64; c->matching_s_ws = 10; c->best_lr_matches = 1;
+    c->min_ratio_12_p = 0.9; c->line_sim_th = 0.75;
+}
+
+namespace {
+struct StereoOut {   // host destinations of the lifted records (points use the first seven)
+    int32_t* m12; double *a_pl, *a_disp, *a_P, *a_s2; int32_t* level; uint8_t* desc; int32_t *src, *counts;
+    double *epl, *edisp, *eP, *le, *angle;   // lines only
+};
+
+int match_stereo_common(PlContext* ctx, bool lines, const PlCamera* cam, const PlStereoMatchConfig* mc, const PlStereoConfig* sc,
+                        int B, const int32_t* l_off, const float* xy_l, const float* angle_l, const int32_t* octave_l,
+                        const uint8_t* desc_l, const int32_t* r_off, const float* xy_r, const uint8_t* desc_r,
+                        const StereoOut& out) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cam || !mc || !sc || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
+    const int rows = mc->grid_rows, cols = mc->grid_cols;
+    if (!grid_ok(rows, cols) || cam->width <= 0 || cam->height <= 0)
+        return fail(ctx, PLSTVO_E_INVALID, "bad grid or image size");
+    if (B == 0) return 0;
+    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
+    const size_t N1 = l_off[B], N2 = r_off[B];
+    if (N1 && (!xy_l || !octave_l || !desc_l || (lines && !angle_l))) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    if (N2 && (!xy_r || !desc_r)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    CK(ctx, cudaSetDevice(ctx->device));
+    const int cw = lines ? 4 : 2;                 // floats per feature (segment / key point) and ints per query cell record
+    Arena a;
+    // raw inputs
+    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_xyl = a.take(N1 * cw * 4);
+    const size_t o_xyr = a.take(N2 * cw * 4), o_ang = a.take(lines ? N1 * 4 : 0), o_oct = a.take(N1 * 4);
+    const size_t o_d1 = a.take(N1 * 32), o_d2 = a.take(N2 * 32);
+    // matchGrid
+    const size_t o_m12 = a.take(N1 * 4), o_gcnt = a.take((size_t)B * 4);
+    const GridScratch g(a, rows, cols, B, N1, N2, N2 * grid_cells_per_train(lines, rows, cols), !lines, lines);
+    const size_t o_prob = a.take((size_t)B * sizeof(GridProblem));
+    // lifted records
+    const size_t o_pl = a.take(N1 * 16), o_disp = a.take(N1 * 8), o_P = a.take(N1 * 24), o_s2 = a.take(N1 * 8);
+    const size_t o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32), o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    const size_t o_epl = a.take(lines ? N1 * 16 : 0), o_edisp = a.take(lines ? N1 * 8 : 0), o_eP = a.take(lines ? N1 * 24 : 0);
+    const size_t o_le = a.take(lines ? N1 * 24 : 0), o_angd = a.take(lines ? N1 * 8 : 0);
+    CK(ctx, a.alloc(ctx->arena_stereo));
+    std::vector<GridProblem> probs((size_t)B);
+    g.fill(probs.data(), B, lines, l_off, r_off, a.u8(o_d1), a.u8(o_d2), a.i32(o_m12), a.i32(o_gcnt));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
+    CK(ctx, a.up(o_xyl, xy_l, N1 * cw * 4, s));
+    CK(ctx, a.up(o_xyr, xy_r, N2 * cw * 4, s));
+    if (lines) CK(ctx, a.up(o_ang, angle_l, N1 * 4, s));
+    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
+    CK(ctx, a.up(o_d1, desc_l, N1 * 32, s));
+    CK(ctx, a.up(o_d2, desc_r, N2 * 32, s));
+    CK(ctx, a.up(o_prob, probs.data(), (size_t)B * sizeof(GridProblem), s));
+    // 1. grid coordinates (:47-48: inv_width = GRID_COLS / image width, inv_height = GRID_ROWS / image height)
+    const double inv_w = cols / static_cast<double>(cam->width), inv_h = rows / static_cast<double>(cam->height);
+    if (lines)
+        CK(ctx, launch_stereo_cells_lines((int)N1, (int)N2, inv_w, inv_h, a.f32(o_xyl), a.f32(o_xyr), a.i32(g.qcell),
+                                          a.f64(g.tline), a.f64(g.tdir), s));
+    else
+        CK(ctx, launch_stereo_cells_points((int)N1, (int)N2, inv_w, inv_h, a.f32(o_xyl), a.f32(o_xyr), a.i32(g.qcell),
+                                           a.i32(g.tcell), s));
+    // 2. matchGrid with the stereo window (:141-143, :340-342: matching_s_ws cells to the left, same row)
+    GridParams prm{rows, cols, GRID_CAP, mc->best_lr_matches ? 1 : 0, PlGridWindow{mc->matching_s_ws, 0, 0, 0},
+                   mc->min_ratio_12_p, mc->line_sim_th};
+    CK(ctx, launch_match_grid(a.at<GridProblem>(o_prob), B, prm, lines, s));
+    // 3. lifting, reading the match list where matchGrid left it
+    if (lines)
+        CK(ctx, launch_lift_lines(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.f32(o_ang), a.i32(o_oct), a.u8(o_d1),
+                                  a.i32(o_roff), a.f32(o_xyr), a.i32(o_m12), a.f64(o_pl), a.f64(o_epl), a.f64(o_disp),
+                                  a.f64(o_edisp), a.f64(o_P), a.f64(o_eP), a.f64(o_le), a.f64(o_angd), a.f64(o_s2),
+                                  a.i32(o_lvl), a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+    else
+        CK(ctx, launch_lift_points(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.i32(o_oct), a.u8(o_d1), a.i32(o_roff),
+                                   a.f32(o_xyr), a.i32(o_m12), a.f64(o_pl), a.f64(o_disp), a.f64(o_P), a.f64(o_s2),
+                                   a.i32(o_lvl), a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+    ctx->launches += 3;
+    CK(ctx, a.down(out.m12, o_m12, N1 * 4, s));
+    CK(ctx, a.down(out.a_pl, o_pl, N1 * 16, s));
+    CK(ctx, a.down(out.a_disp, o_disp, N1 * 8, s));
+    CK(ctx, a.down(out.a_P, o_P, N1 * 24, s));
+    CK(ctx, a.down(out.a_s2, o_s2, N1 * 8, s));
+    CK(ctx, a.down(out.level, o_lvl, N1 * 4, s));
+    CK(ctx, a.down(out.desc, o_dout, N1 * 32, s));
+    CK(ctx, a.down(out.src, o_src, N1 * 4, s));
+    if (lines) {
+        CK(ctx, a.down(out.epl, o_epl, N1 * 16, s));
+        CK(ctx, a.down(out.edisp, o_edisp, N1 * 8, s));
+        CK(ctx, a.down(out.eP, o_eP, N1 * 24, s));
+        CK(ctx, a.down(out.le, o_le, N1 * 24, s));
+        CK(ctx, a.down(out.angle, o_angd, N1 * 8, s));
+    }
+    return counts_total(ctx, s, B, a.i32(o_cnt), out.counts, a.i32(o_gcnt));
+}
+}  // namespace
+
+int plstvo_match_stereo_points(PlContext* ctx, const PlCamera* cam, const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                               int B, const int32_t* l_off, const float* kp_l, const int32_t* octave_l, const uint8_t* desc_l,
+                               const int32_t* r_off, const float* kp_r, const uint8_t* desc_r, int32_t* m12, double* pt_pl,
+                               double* pt_disp, double* pt_P, double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out,
+                               int32_t* src_idx, int32_t* counts) {
+    const StereoOut out{m12, pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts,
+                        nullptr, nullptr, nullptr, nullptr, nullptr};
+    return match_stereo_common(ctx, false, cam, mcfg, scfg, B, l_off, kp_l, nullptr, octave_l, desc_l, r_off, kp_r, desc_r, out);
+}
+
+int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                              int B, const int32_t* l_off, const float* seg_l, const float* angle_l, const int32_t* octave_l,
+                              const uint8_t* desc_l, const int32_t* r_off, const float* seg_r, const uint8_t* desc_r,
+                              int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp, double* ls_edisp, double* ls_sP,
+                              double* ls_eP, double* ls_le, double* ls_angle, double* ls_sigma2, int32_t* ls_level,
+                              uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts) {
+    const StereoOut out{m12, ls_spl, ls_sdisp, ls_sP, ls_sigma2, ls_level, ldesc_out, src_idx, counts,
+                        ls_epl, ls_edisp, ls_eP, ls_le, ls_angle};
+    return match_stereo_common(ctx, true, cam, mcfg, scfg, B, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, desc_r, out);
+}
+
+}  // extern "C"
+
+// ---- raw stereo features -> pose, records resident in HBM ---------------------------------------------------------
+// sequence == false: B independent (prev, curr) pairs, four feature sets of B frames.
+// sequence == true : prev holds NF = B + 1 consecutive frames, pair p = (frame p, frame p + 1); two feature sets of NF frames,
+//                    every frame goes through the stereo step once and is lifted twice (as a previous and as a current frame).
+int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                                const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
+                                const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
+                                const StereoDevInputs* dev) {
+    // slot < 0: blocking (returns with the results in host memory); slot 0 / 1: enqueue only, results valid after plstvo_wait
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cam || !cfg || !mc || !sc || !prev || (!sequence && !curr) || !results) return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    const int NF = prev->B;                         // frames per feature set
+    const int B = sequence ? NF - 1 : NF;           // pairs
+    if (NF < 0 || (!sequence && curr->B != NF)) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (sequence && NF == 1) return 0;              // one frame: nothing to track
+    const int rows = mc->grid_rows, cols = mc->grid_cols;
+    if (!grid_ok(rows, cols) || cam->width <= 0 || cam->height <= 0)
+        return fail(ctx, PLSTVO_E_INVALID, "bad grid or image size");
+    if (NF == 0) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    const int NSETS = sequence ? 2 : 4;
+    if (sequence) curr = prev;                      // sets 2, 3 below are unused
+    // the four feature sets: {prev, curr} x {points, lines}
+    struct Set {
+        bool lines; const int32_t *l_off, *r_off; const float *xy_l, *xy_r, *ang; const int32_t* oct; const uint8_t *d1, *d2;
+        size_t N1, N2, o_loff, o_roff, o_xyl, o_xyr, o_ang, o_oct, o_d1, o_d2, o_m12, o_cnt, o_gcnt, o_ooff, o_ooff2, o_prob;
+        bool on_device;
+        const float *g_xyl, *g_xyr; const int32_t* g_oct; const uint8_t *g_d1, *g_d2;   // where the kernels read the inputs
+    };
+    Set sets[4] = {
+        {false, prev->pl_off, prev->pr_off, prev->kp_l, prev->kp_r, nullptr, prev->poct_l, prev->pdesc_l, prev->pdesc_r},
+        {true, prev->ll_off, prev->lr_off, prev->seg_l, prev->seg_r, prev->angle_l, prev->loct_l, prev->ldesc_l, prev->ldesc_r},
+        {false, curr->pl_off, curr->pr_off, curr->kp_l, curr->kp_r, nullptr, curr->poct_l, curr->pdesc_l, curr->pdesc_r},
+        {true, curr->ll_off, curr->lr_off, curr->seg_l, curr->seg_r, curr->angle_l, curr->loct_l, curr->ldesc_l, curr->ldesc_r}};
+    if (dev)
+        for (int k = 0; k < NSETS; ++k)
+            if (dev->set[k].on_device) {
+                const StereoDevInputs::Set& d = dev->set[k];
+                Set& st = sets[k];
+                st.xy_l = d.xy_l; st.xy_r = d.xy_r; st.oct = d.oct; st.d1 = d.d1; st.d2 = d.d2;
+            }
+    Arena a;
+    size_t maxN1 = 0, maxN2 = 0, max_items = 0;
+    for (int k = 0; k < NSETS; ++k) {
+        Set& st = sets[k];
+        st.on_device = dev && dev->set[k].on_device;
+        if (const int rc = check_stereo_offsets(ctx, NF, st.l_off, st.r_off)) return rc;
+        st.N1 = st.l_off[NF];
+        st.N2 = st.r_off[NF];
+        if (st.N1 && (!st.xy_l || (!st.oct && !st.on_device) || !st.d1 || (st.lines && !st.ang)))
+            return fail(ctx, PLSTVO_E_INVALID, "null input array");
+        if (st.N2 && (!st.xy_r || !st.d2)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+        const int cw = st.lines ? 4 : 2;
+        const size_t host = st.on_device ? 0 : 1;   // device-resident inputs take no arena space (but zero octaves do)
+        st.o_loff = a.take((size_t)(NF + 1) * 4); st.o_roff = a.take((size_t)(NF + 1) * 4);
+        st.o_xyl = a.take(host * st.N1 * cw * 4); st.o_xyr = a.take(host * st.N2 * cw * 4); st.o_ang = a.take(st.lines ? st.N1 * 4 : 0);
+        st.o_oct = a.take(st.on_device && st.oct ? 0 : st.N1 * 4); st.o_d1 = a.take(host * st.N1 * 32);
+        st.o_d2 = a.take(host * st.N2 * 32); st.o_m12 = a.take(st.N1 * 4);
+        st.o_cnt = a.take((size_t)NF * 4); st.o_gcnt = a.take((size_t)NF * 4); st.o_ooff = a.take((size_t)(NF + 1) * 4);
+        st.o_ooff2 = a.take((size_t)(NF + 1) * 4);
+        st.o_prob = a.take((size_t)NF * sizeof(GridProblem));
+        maxN1 = std::max(maxN1, st.N1);
+        maxN2 = std::max(maxN2, st.N2);
+        max_items = std::max(max_items, st.N2 * grid_cells_per_train(st.lines, rows, cols));
+    }
+    // matchGrid scratch, shared by the four sets (they run one after the other on one stream)
+    const GridScratch g(a, rows, cols, NF, maxN1, maxN2, max_items, true, true);
+    CK(ctx, a.alloc(ctx->arena_track_stereo[slot + 1]));
+    for (int k = 0; k < NSETS; ++k) {
+        Set& st = sets[k];
+        st.g_xyl = st.on_device ? st.xy_l : a.f32(st.o_xyl);
+        st.g_xyr = st.on_device ? st.xy_r : a.f32(st.o_xyr);
+        st.g_oct = st.on_device && st.oct ? st.oct : a.i32(st.o_oct);
+        st.g_d1 = st.on_device ? st.d1 : a.u8(st.o_d1);
+        st.g_d2 = st.on_device ? st.d2 : a.u8(st.o_d2);
+    }
+    cudaStream_t s = ctx->s_main, sh = ctx->s_h2d;   // uploads of set k + 1 run under the kernels of set k
+    // (this slot's arena is free: a blocking call ends synchronised, an async slot is reused only after its event completed)
+    const double inv_w = cols / static_cast<double>(cam->width), inv_h = rows / static_cast<double>(cam->height);
+    const GridParams gprm{rows, cols, GRID_CAP, mc->best_lr_matches ? 1 : 0, PlGridWindow{mc->matching_s_ws, 0, 0, 0},
+                          mc->min_ratio_12_p, mc->line_sim_th};
+    // pinned staging: 4 problem tables + 2 x 4 x B counters (pageable copies would block this thread on the stream)
+    const size_t prob_bytes = ((size_t)NF * sizeof(GridProblem) + 255) / 256 * 256;
+    PinnedBuf& staging = ctx->h_staging[slot + 1];
+    CK(ctx, staging.ensure(4 * prob_bytes + (size_t)8 * NF * 4));
+    uint8_t* hst = static_cast<uint8_t*>(staging.p);
+    int32_t* cnt = reinterpret_cast<int32_t*>(hst + 4 * prob_bytes);
+    int32_t* gcnt = cnt + (size_t)4 * NF;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[0], s));
+    bool joined = false;
+    // ---- pass 1: cells -> matchGrid -> lifting filters (count only) per set ----
+    for (int k = 0; k < NSETS; ++k) {
+        Set& st = sets[k];
+        const int cw = st.lines ? 4 : 2;
+        GridProblem* probs = reinterpret_cast<GridProblem*>(hst + (size_t)k * prob_bytes);
+        g.fill(probs, NF, st.lines, st.l_off, st.r_off, st.g_d1, st.g_d2, a.i32(st.o_m12), a.i32(st.o_gcnt));
+        CK(ctx, a.up(st.o_loff, st.l_off, (size_t)(NF + 1) * 4, sh));
+        CK(ctx, a.up(st.o_roff, st.r_off, (size_t)(NF + 1) * 4, sh));
+        if (st.lines) CK(ctx, a.up(st.o_ang, st.ang, st.N1 * 4, sh));
+        if (!st.on_device) {
+            CK(ctx, a.up(st.o_xyl, st.xy_l, st.N1 * cw * 4, sh));
+            CK(ctx, a.up(st.o_xyr, st.xy_r, st.N2 * cw * 4, sh));
+            CK(ctx, a.up(st.o_oct, st.oct, st.N1 * 4, sh));
+            CK(ctx, a.up(st.o_d1, st.d1, st.N1 * 32, sh));
+            CK(ctx, a.up(st.o_d2, st.d2, st.N2 * 32, sh));
+        } else if (!st.oct && st.N1) {
+            CK(ctx, cudaMemsetAsync(a.u8(st.o_oct), 0, st.N1 * 4, sh));   // key lines of octave 0
+        }
+        CK(ctx, a.up(st.o_prob, probs, (size_t)NF * sizeof(GridProblem), sh));
+        cudaEvent_t uploaded = next_event(ctx);
+        CK(ctx, cudaEventRecord(uploaded, sh));
+        CK(ctx, cudaStreamWaitEvent(s, uploaded, 0));
+        if (st.lines && dev && dev->lines_ready && !joined) {   // the line descriptors come from another stream
+            CK(ctx, cudaStreamWaitEvent(s, dev->lines_ready, 0));
+            joined = true;
+        }
+        if (st.lines) {
+            CK(ctx, launch_stereo_cells_lines((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
+                                              a.f64(g.tline), a.f64(g.tdir), s));
+            CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, true, s));
+            CK(ctx, launch_lift_lines(*cam, *sc, NF, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
+                                      a.i32(st.o_roff), st.g_xyr, a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr,
+                                      nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.i32(st.o_cnt), s));
+        } else {
+            CK(ctx, launch_stereo_cells_points((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
+                                               a.i32(g.tcell), s));
+            CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, false, s));
+            CK(ctx, launch_lift_points(*cam, *sc, NF, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
+                                       a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                       a.i32(st.o_cnt), s));
+        }
+        ctx->launches += 3;
+        CK(ctx, cudaMemcpyAsync(cnt + (size_t)k * NF, a.u8(st.o_cnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
+        CK(ctx, cudaMemcpyAsync(gcnt + (size_t)k * NF, a.u8(st.o_gcnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
+    }
+    CK(ctx, cudaStreamSynchronize(s));     // the one host hop: survivor counts -> compact offsets and the matcher's tile plan
+    // compact offsets per set; in sequence mode the current-frame role of a set starts at its second frame
+    std::vector<int32_t> ooff[4], ooff2[2];
+    for (int k = 0; k < NSETS; ++k) {
+        if (const int rc = check_grid_counts(ctx, NF, gcnt + (size_t)k * NF)) return rc;
+        ooff[k].assign((size_t)NF + 1, 0);
+        for (int p = 0; p < NF; ++p) {
+            ooff[k][p + 1] = ooff[k][p] + cnt[(size_t)k * NF + p];
+            if (n_stereo) {
+                if (sequence) n_stereo[(size_t)p * 2 + k] = cnt[(size_t)k * NF + p];
+                else n_stereo[(size_t)p * 4 + k] = cnt[(size_t)k * NF + p];
+            }
+        }
+        CK(ctx, a.up(sets[k].o_ooff, ooff[k].data(), (size_t)(NF + 1) * 4, sh));
+        if (sequence) {
+            ooff2[k].assign((size_t)NF, 0);          // frames 1 .. NF - 1 as current frames: offsets relative to frame 1
+            for (int p = 0; p < NF; ++p) ooff2[k][p] = ooff[k][p + 1] - ooff[k][1];
+            CK(ctx, a.up(sets[k].o_ooff2, ooff2[k].data(), (size_t)NF * 4, sh));
+        }
+    }
+    // ---- the tracker's plan on the compact lists; the records are written straight into its buffers ----
+    PlFrameBatch fp{}, fc{};
+    fp.B = fc.B = B;
+    fp.pt_off = ooff[0].data(); fp.ls_off = ooff[1].data();
+    fc.pt_off = sequence ? ooff2[0].data() : ooff[2].data();
+    fc.ls_off = sequence ? ooff2[1].data() : ooff[3].data();
+    Workspace& ws = slot < 0 ? ctx->ws : ctx->ws_async[slot];
+    int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr);
+    if (rc) return rc;
+    if (priors) CK(ctx, cudaMemcpyAsync(ws.d_priors.p, priors, (size_t)B * sizeof(PlPrior), cudaMemcpyHostToDevice, ctx->s_h2d));
+    cudaEvent_t planned = next_event(ctx);
+    CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
+    CK(ctx, cudaStreamWaitEvent(s, planned, 0));
+    // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
+    // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
+    auto lift_prev_points = [&](const Set& st) -> cudaError_t {
+        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
+                                  a.i32(st.o_m12), nullptr, nullptr, ws.d_ptP.as<double>(), ws.d_pts2.as<double>(), nullptr,
+                                  ws.d_pdesc1.as<uint8_t>(), nullptr, a.i32(st.o_cnt), s, a.i32(st.o_ooff));
+    };
+    auto lift_prev_lines = [&](const Set& st) -> cudaError_t {
+        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1, a.i32(st.o_roff),
+                                 st.g_xyr, a.i32(st.o_m12), ws.d_lsspl.as<double>(), ws.d_lsepl.as<double>(), nullptr, nullptr,
+                                 ws.d_lssP.as<double>(), ws.d_lseP.as<double>(), nullptr, nullptr, ws.d_lss2.as<double>(),
+                                 ws.d_lslev.as<int32_t>(), ws.d_ldesc1.as<uint8_t>(), nullptr, a.i32(st.o_cnt), s,
+                                 a.i32(st.o_ooff));
+    };
+    auto lift_curr_points = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
+        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
+                                  st.g_xyr, a.i32(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
+                                  ws.d_pdesc2.as<uint8_t>(), nullptr, a.i32(st.o_cnt) + first, s, a.i32(o_out));
+    };
+    auto lift_curr_lines = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
+        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
+                                 a.i32(st.o_roff) + first, st.g_xyr, a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr,
+                                 nullptr, ws.d_lsle.as<double>(), nullptr, nullptr, nullptr, ws.d_ldesc2.as<uint8_t>(), nullptr,
+                                 a.i32(st.o_cnt) + first, s, a.i32(o_out));
+    };
+    CK(ctx, lift_prev_points(sets[0]));
+    CK(ctx, lift_prev_lines(sets[1]));
+    if (sequence) {
+        CK(ctx, lift_curr_points(sets[0], 1, sets[0].o_ooff2));
+        CK(ctx, lift_curr_lines(sets[1], 1, sets[1].o_ooff2));
+    } else {
+        CK(ctx, lift_curr_points(sets[2], 0, sets[2].o_ooff));
+        CK(ctx, lift_curr_lines(sets[3], 0, sets[3].o_ooff));
+    }
+    ctx->launches += 4;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
+    rc = ws_launch_match(ctx, ws, 0, B, s);
+    if (rc) return rc;
+    rc = ws_launch_solve(ctx, ws, 0, B, true, s);
+    if (rc) return rc;
+    if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[2], s));
+    CK(ctx, cudaMemcpyAsync(results, ws.d_results.p, (size_t)B * sizeof(PlPoseResult), cudaMemcpyDeviceToHost, s));
+    if (slot < 0) CK(ctx, cudaStreamSynchronize(s));
+    return 0;
+}
+
+extern "C" {
+
+// ticket bookkeeping shared with plstvo_track_batch_async: two slots, plstvo_wait(ticket) blocks until the slot's results are home
+static int stereo_async(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                        const PlStereoConfig* sc, const PlStereoFeatures* a, const PlStereoFeatures* b, const PlPrior* priors,
+                        PlPoseResult* results, int32_t* n_stereo, bool sequence) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    CK(ctx, cudaSetDevice(ctx->device));
+    const int slot = acquire_slot(ctx);
+    if (slot < 0) return slot;
+    const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, a, b, priors, results, n_stereo, sequence, slot);
+    if (rc) return rc;
+    CK(ctx, cudaEventRecord(ctx->slot_done[slot], ctx->s_main));
+    ctx->slot_busy[slot] = true;
+    return slot;
+}
+
+int plstvo_track_stereo_batch_async(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                                    const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
+                                    const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return stereo_async(ctx, cam, cfg, mc, sc, prev, curr, priors, results, n_stereo, false);
+}
+
+int plstvo_track_stereo_sequence_async(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                                       const PlStereoConfig* sc, const PlStereoFeatures* frames, const PlPrior* priors,
+                                       PlPoseResult* results, int32_t* n_stereo) {
+    return stereo_async(ctx, cam, cfg, mc, sc, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                              const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
+                              const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_stereo_common(ctx, cam, cfg, mc, sc, prev, curr, priors, results, n_stereo, false, -1);
+}
+
+int plstvo_track_stereo_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                                 const PlStereoConfig* sc, const PlStereoFeatures* frames, const PlPrior* priors,
+                                 PlPoseResult* results, int32_t* n_stereo) {
+    return track_stereo_common(ctx, cam, cfg, mc, sc, frames, nullptr, priors, results, n_stereo, true, -1);
+}
+
+}  // extern "C"

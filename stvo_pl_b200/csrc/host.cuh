@@ -1,0 +1,373 @@
+// host.cuh — host side of the C-ABI (include/plstvo.h), shared by its three translation units: capi.cu (context, matching,
+// tracking, throughput mode, instrumentation), capi_stereo.cu (matchGrid, lifting, matchStereo, tracking from stereo
+// features) and capi_features.cu (ORB, LBD, tracking from stereo images).  Not part of the public boundary.
+#pragma once
+
+#include <algorithm>
+#include <cstdio>
+#include <initializer_list>
+#include <mutex>
+#include <string>
+#include <vector>
+
+#include "common.cuh"
+#include "match_tc.cuh"
+
+namespace plstvo {
+
+// Device memory that grows on demand and is freed by its owner's destructor.
+struct DevBuf {
+    void*  p = nullptr;
+    size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+        size_t want = bytes + bytes / 4 + 256;
+        cudaError_t e = cudaMalloc(&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+    void release() {
+        if (p) cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// Pinned host memory of the size last asked for (when that grew), freed by its owner's destructor.
+struct PinnedBuf {
+    void*  p = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() {
+        if (p) cudaFreeHost(p);
+    }
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        if (p) cudaFreeHost(p);
+        p = nullptr;
+        cap = 0;
+        cudaError_t e = cudaMallocHost(&p, bytes);
+        if (e == cudaSuccess) cap = bytes;
+        return e;
+    }
+};
+
+// N CUDA events, destroyed by their owner's destructor (a context, or the scope of a timing call).
+template <int N> struct Events {
+    cudaEvent_t ev[N] = {};
+    Events() = default;
+    Events(const Events&) = delete;
+    Events& operator=(const Events&) = delete;
+    ~Events() {
+        for (cudaEvent_t e : ev)
+            if (e) cudaEventDestroy(e);
+    }
+    cudaError_t create(unsigned flags = cudaEventDefault) {   // the ones not created yet
+        for (cudaEvent_t& e : ev)
+            if (!e) {
+                cudaEvent_t t;
+                if (const cudaError_t r = cudaEventCreateWithFlags(&t, flags)) return r;
+                e = t;
+            }
+        return cudaSuccess;
+    }
+    cudaEvent_t& operator[](int k) { return ev[k]; }
+};
+
+// One DevBuf carved into slices: take() lays them out (256-byte aligned, in call order), alloc() sizes the buffer, then a
+// slice is addressed by its offset.  up / down copy nothing for a null host pointer or zero bytes.
+struct Arena {
+    size_t off = 0;
+    uint8_t* base = nullptr;
+    size_t take(size_t bytes) {
+        const size_t o = off;
+        off += (bytes + 255) / 256 * 256;
+        return o;
+    }
+    cudaError_t alloc(DevBuf& buf) {
+        const cudaError_t e = buf.ensure(off);
+        base = buf.as<uint8_t>();
+        return e;
+    }
+    template <typename T> T* at(size_t o) const { return reinterpret_cast<T*>(base + o); }
+    uint8_t* u8(size_t o) const { return base + o; }
+    int32_t* i32(size_t o) const { return at<int32_t>(o); }
+    float* f32(size_t o) const { return at<float>(o); }
+    double* f64(size_t o) const { return at<double>(o); }
+    cudaError_t up(size_t o, const void* src, size_t bytes, cudaStream_t s) const {
+        return (src && bytes) ? cudaMemcpyAsync(base + o, src, bytes, cudaMemcpyHostToDevice, s) : cudaSuccess;
+    }
+    cudaError_t down(void* dst, size_t o, size_t bytes, cudaStream_t s) const {
+        return (dst && bytes) ? cudaMemcpyAsync(dst, base + o, bytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+    }
+};
+
+// K2's list capacities and where it keeps the lists, and which solver a batch takes (capi.cu: plan_solve)
+struct SolvePlan {
+    int cap_pt = 1, cap_ls = 1, sort_cap = 1;
+    bool feat_in_smem = true;
+    bool fits = true;          // K2 can hold the lists, in shared memory or in global scratch
+    bool use_stream = false;   // the streamed solver
+    size_t feat_stride = 0;    // doubles of global list scratch per pair (0: none needed)
+};
+
+// Work plan + device storage of one batch of frame pairs (also the body of PlDeviceBatch)
+struct Workspace {
+    int B = 0;
+    PlCamera cam{};
+    PlConfig cfg{};
+    bool has_priors = false;
+    bool have_level = false;   // prev->ls_level supplied (null = level 0 everywhere)
+    bool planned = false, planned_features = false;   // plan cache (ws_prepare)
+    int sm_planned = 0;
+    // host copies of the offsets
+    std::vector<int32_t> p_off1, p_off2, l_off1, l_off2;
+    // plan
+    std::vector<MatchProblem> problems;   // [2B]: points, lines
+    int max_n2 = 0;
+    SolvePlan solver;
+    // device storage
+    DevBuf d_poff1, d_poff2, d_loff1, d_loff2;
+    DevBuf d_pdesc1, d_pdesc2, d_ldesc1, d_ldesc2;
+    DevBuf d_ptP, d_pts2, d_ptpl;                                      // prev P, prev sigma2, curr pl
+    DevBuf d_lssP, d_lseP, d_lsspl, d_lsepl, d_lss2, d_lslev, d_lsle;  // prev ...; curr le
+    DevBuf d_priors, d_results, d_m12p, d_m12l, d_inlp, d_inll;
+    DevBuf d_rowpart, d_colpart, d_problems, d_feat;
+    DevBuf d_phase;   // debug phase timers (PLSTVO_PHASE_DEBUG)
+    // K1 (match_tc.cu): per-block value partials, work items
+    std::vector<TcProblem> tc_problems;   // [2B], parallel to `problems`
+    std::vector<TcItem> tc_items[2];      // work items of the point problems (long) and of the line problems (short)
+    std::vector<int32_t> item_start[2];   // [B+1] first work item of each pair in either list
+    DevBuf d_tcprob, d_tcitems[2], d_rowp, d_colp, d_sched;
+    DevBuf d_stream;       // arena of the streamed solver (frames too large for K2's shared memory)
+};
+
+}  // namespace plstvo
+
+struct PlContext {
+    std::recursive_mutex mu;   // entry points serialise on it: one context may be shared by the caller's threads
+    int device = 0;
+    int sm_count = 0;
+    size_t smem_optin = 0;
+    cudaStream_t s_main = nullptr, s_alt = nullptr, s_h2d = nullptr, s_d2h = nullptr;
+    std::vector<cudaEvent_t> events;
+    size_t next_event = 0;
+    std::string err;
+    int64_t launches = 0;
+    plstvo::Workspace ws;          // reused by the host-buffer entry points
+    plstvo::Workspace ws_async[2]; // double-buffered workspaces of plstvo_track_batch_async
+    plstvo::Events<2> slot_done;
+    bool slot_busy[2] = {false, false};
+    int next_slot = 0;
+    plstvo::DevBuf scratch;        // misc (popc bench, L2 flush)
+    plstvo::DevBuf gn_in[8], gn_out[4];
+    // per-entry-point device arenas (context-owned: a process may hold one context per GPU)
+    plstvo::DevBuf arena_grid, arena_lift_pt, arena_lift_ls, arena_stereo;
+    plstvo::DevBuf arena_track_stereo[3];   // [0]: blocking calls, [1 + slot]: plstvo_track_stereo_*_async
+    plstvo::DevBuf gs_in[13], gs_rec_pt, gs_rec_ls;   // resident inputs / packed records of the streamed evaluator
+    plstvo::DevBuf arena_orb;      // plstvo_orb_compute_batch: images, level buffers, key points, outputs
+    bool orb_tables = false;
+    plstvo::Events<4> orb_ev;
+    plstvo::DevBuf arena_orb_kp;   // plstvo_orb_detect_and_compute_batch: per-key-point arrays, sized once the selection is counted
+    bool orb_computed = false, orb_detected = false;
+    plstvo::Events<5> orb_det_ev;
+    plstvo::DevBuf arena_lbd;      // plstvo_lbd_compute_batch: images, gradients, key lines, descriptors
+    bool lbd_tables = false, lbd_computed = false;
+    plstvo::Events<3> lbd_ev;
+    // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
+    plstvo::Events<4> img_ev;
+    plstvo::Events<1> img_join;
+    float img_ms[5] = {0, 0, 0, 0, 0};
+    bool img_timed = false;
+    // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
+    plstvo::PinnedBuf h_staging[3];
+
+    ~PlContext() {   // the owner has synchronised the device; the members free their own memory and events
+        for (cudaEvent_t e : events) cudaEventDestroy(e);
+        for (cudaStream_t s : {s_main, s_alt, s_h2d, s_d2h})
+            if (s) cudaStreamDestroy(s);
+    }
+};
+
+namespace plstvo {
+
+#define CK(ctx, call)                                                                            \
+    do {                                                                                         \
+        cudaError_t e__ = (call);                                                                \
+        if (e__ != cudaSuccess) {                                                                \
+            char buf__[512];                                                                     \
+            snprintf(buf__, sizeof(buf__), "%s:%d: %s -> %s", __FILE__, __LINE__, #call,         \
+                     cudaGetErrorString(e__));                                                   \
+            (ctx)->err = buf__;                                                                  \
+            return PLSTVO_E_CUDA;                                                                \
+        }                                                                                        \
+    } while (0)
+
+#define LOCK(ctx) std::lock_guard<std::recursive_mutex> lock__((ctx)->mu)
+
+inline int fail(PlContext* ctx, int code, const char* msg) {
+    if (ctx) ctx->err = msg;
+    return code;
+}
+
+// Cross-stream ordering events.  Each one is recorded and immediately waited on by the enqueuing host code, so a ring
+// can be recycled while earlier work is still in flight (a wait captures the record that preceded it).
+inline cudaEvent_t next_event(PlContext* ctx) {
+    constexpr size_t RING = 512;
+    if (ctx->events.size() < RING) {
+        cudaEvent_t e;
+        cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+        ctx->events.push_back(e);
+        return e;
+    }
+    return ctx->events[ctx->next_event++ % RING];
+}
+
+// CSR offsets [n + 1] of one or more row sets over the same n frames.  PLSTVO_E_INVALID with `bad` for a null array or (with
+// from_zero) a first offset other than 0; then frame by frame, PLSTVO_E_INVALID with `decreasing` for a decreasing offset in
+// any set, else PLSTVO_E_TOO_LARGE with `too_large` for more than PLSTVO_MAX_FEATURES rows in any set.
+inline int check_offsets(PlContext* ctx, int n, std::initializer_list<const int32_t*> offs, const char* bad,
+                         const char* decreasing, const char* too_large, bool from_zero = true) {
+    for (const int32_t* off : offs)
+        if (!off || (from_zero && off[0] != 0)) return fail(ctx, PLSTVO_E_INVALID, bad);
+    for (int p = 0; p < n; ++p) {
+        for (const int32_t* off : offs)
+            if (off[p + 1] - off[p] < 0) return fail(ctx, PLSTVO_E_INVALID, decreasing);
+        for (const int32_t* off : offs)
+            if (off[p + 1] - off[p] > PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, too_large);
+    }
+    return 0;
+}
+
+// matchGrid's per-frame counts: a negative one is the error code of a frame with more than GRID_CAP candidates in a window
+inline int check_grid_counts(PlContext* ctx, int n, const int32_t* gcnt) {
+    for (int p = 0; p < n; ++p)
+        if (gcnt[p] < 0) return fail(ctx, gcnt[p], "matchGrid: more than 128 candidates in one query window");
+    return 0;
+}
+
+// The end of a blocking call with per-frame counts at d_cnt (device): downloads them on s behind the call's other copies
+// (after matchGrid's, d_gcnt, when the call ran it; d_gcnt == d_cnt where they are the result), waits, fails on a negative
+// matchGrid count, else fills counts (optional) and returns the total.
+inline int counts_total(PlContext* ctx, cudaStream_t s, int n, const int32_t* d_cnt, int32_t* counts,
+                        const int32_t* d_gcnt = nullptr) {
+    std::vector<int32_t> cnt((size_t)n), gcnt(d_gcnt && d_gcnt != d_cnt ? (size_t)n : 0);
+    if (!gcnt.empty()) CK(ctx, cudaMemcpyAsync(gcnt.data(), d_gcnt, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaMemcpyAsync(cnt.data(), d_cnt, (size_t)n * 4, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    if (d_gcnt)
+        if (const int rc = check_grid_counts(ctx, n, gcnt.empty() ? cnt.data() : gcnt.data())) return rc;
+    long total = 0;
+    for (int p = 0; p < n; ++p) {
+        if (counts) counts[p] = cnt[p];
+        total += cnt[p];
+    }
+    return (int)total;
+}
+
+// The next of the two slots of the async entry points (plstvo_wait's tickets) and its completion event.  A caller that
+// skipped plstvo_wait on the batch that used the slot last gets that batch finished first.
+inline int acquire_slot(PlContext* ctx) {
+    const int slot = ctx->next_slot;
+    ctx->next_slot ^= 1;
+    if (ctx->slot_busy[slot]) {
+        CK(ctx, cudaEventSynchronize(ctx->slot_done[slot]));
+        ctx->slot_busy[slot] = false;
+    }
+    if (!ctx->slot_done[slot]) CK(ctx, cudaEventCreateWithFlags(&ctx->slot_done[slot], cudaEventDisableTiming));
+    return slot;
+}
+
+// ---- matchGrid (match_grid.cu) on arena scratch ----
+constexpr int GRID_CAP = 128;   // candidates per query window (the reference has no limit; typical: ~10)
+
+inline bool grid_ok(int rows, int cols) { return rows > 0 && cols > 0 && rows * cols <= 8192; }
+
+inline size_t grid_cells_per_train(bool lines, int rows, int cols) { return lines ? (size_t)std::max(rows, cols) + 2 : 1; }
+
+// matchGrid's scratch, carved from an arena, for frames of points and / or lines with at most maxN1 query and maxN2 train
+// rows in all (max_items: train rows times grid_cells_per_train of their kind); fill() writes the GridProblem table of B
+// frames of one kind onto it.
+struct GridScratch {
+    const Arena& a;
+    int rows, cols;
+    size_t qcell, tcell, tline, tdir, items, qpairs, qcount, tcount, tstart, tslots, seen, m21;
+    GridScratch(Arena& ar, int rows_, int cols_, int B, size_t maxN1, size_t maxN2, size_t max_items, bool points, bool lines)
+        : a(ar), rows(rows_), cols(cols_) {
+        qcell = ar.take(maxN1 * (lines ? 16 : 8));
+        tcell = ar.take(points ? maxN2 * 8 : 0);
+        tline = ar.take(lines ? maxN2 * 32 : 0);
+        tdir = ar.take(lines ? maxN2 * 16 : 0);
+        items = ar.take(max_items * 4);
+        qpairs = ar.take(maxN1 * GRID_CAP * 8);
+        qcount = ar.take(maxN1 * 4);
+        tcount = ar.take(maxN2 * 4);
+        tstart = ar.take((maxN2 + B) * 4);
+        tslots = ar.take(maxN1 * GRID_CAP * 4);
+        seen = ar.take(maxN1 * GRID_CAP);
+        m21 = ar.take(maxN2 * 4);
+    }
+    // frame p: queries q_off[p] .. of d1 (device, 32-byte rows) and m12, trains t_off[p] .. of d2, its count at count[p]
+    void fill(GridProblem* probs, int B, bool lines, const int32_t* q_off, const int32_t* t_off, const uint8_t* d1,
+              const uint8_t* d2, int32_t* m12, int32_t* count) const {
+        const size_t cells = grid_cells_per_train(lines, rows, cols);
+        for (int p = 0; p < B; ++p) {
+            GridProblem& g = probs[p];
+            const size_t qa = q_off[p], tb = t_off[p];
+            g.n1 = q_off[p + 1] - q_off[p];
+            g.n2 = t_off[p + 1] - t_off[p];
+            g.q_cell = a.i32(qcell) + qa * (lines ? 4 : 2);
+            g.d1 = d1 + qa * 32;
+            g.t_cell = lines ? nullptr : a.i32(tcell) + tb * 2;
+            g.t_line = lines ? a.f64(tline) + tb * 4 : nullptr;
+            g.t_dir = lines ? a.f64(tdir) + tb * 2 : nullptr;
+            g.d2 = d2 + tb * 32;
+            g.m12 = m12 + qa;
+            g.count = count + p;
+            g.grid_items = a.i32(items) + tb * cells;
+            g.q_pairs = a.at<int2>(qpairs) + qa * GRID_CAP;
+            g.q_count = a.i32(qcount) + qa;
+            g.t_count = a.i32(tcount) + tb;
+            g.t_start = a.i32(tstart) + tb + p;
+            g.t_slots = a.i32(tslots) + qa * GRID_CAP;
+            g.seen = a.u8(seen) + qa * GRID_CAP;
+            g.m21 = a.i32(m21) + tb;
+        }
+    }
+};
+
+// ---- capi.cu: the tracker's plan and launches, composed by the stereo paths ----
+int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfig* cfg, const PlFrameBatch* prev,
+               const PlFrameBatch* curr, bool with_features, bool has_priors);
+int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t s, cudaEvent_t* marks = nullptr);
+int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_level, cudaStream_t s,
+                    cudaEvent_t* marks = nullptr);
+
+// ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
+// Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the
+// stream `lines_ready` was recorded on).  A set with on_device reads xy_l, xy_r, oct, d1, d2 from here instead of uploading
+// the PlStereoFeatures arrays (oct null: all octaves 0); offsets and line angles still come from the host struct.
+struct StereoDevInputs {
+    struct Set {
+        bool on_device = false;
+        const float *xy_l = nullptr, *xy_r = nullptr; const int32_t* oct = nullptr; const uint8_t *d1 = nullptr, *d2 = nullptr;
+    } set[4];
+    cudaEvent_t lines_ready = nullptr;   // waited on before the first line set's stereo step
+    cudaEvent_t* marks = nullptr;        // [3] timing events: stereo step start, its end, tracking end (all on s_main)
+};
+int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                        const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
+                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
+                        const StereoDevInputs* dev = nullptr);
+
+}  // namespace plstvo

@@ -58,12 +58,16 @@ def test_golden_tool_regenerates_the_file():
 
 
 @need_ref
-def test_trig_binding_is_the_float_overload():
+def test_lbd_host_path_takes_the_float_trig_overload():
     """The reference's translation unit includes <math.h> (bitarray_custom.hpp:52), whose C++ form puts std::cos(float) /
     std::sin(float) into the global namespace: its unqualified cos(float) / sin(float) call the C library's cosf / sinf
-    (merged into sincosf).  The stand-in reproduces that, and capi.cu evaluates the line direction with the same function."""
+    (merged into sincosf).  The stand-in reproduces that, and the host source that enqueues LBD (lbd_enqueue) evaluates the
+    line direction with the same function."""
     assert lbd.trig_binding() == "float"
-    assert "sincosf(kl_angle[k]" in open(os.path.join(ROOT, "stvo_pl_b200", "csrc", "capi.cu")).read()
+    csrc = os.path.join(ROOT, "stvo_pl_b200", "csrc")
+    srcs = [open(os.path.join(csrc, f)).read() for f in sorted(os.listdir(csrc)) if f.endswith(".cu")]
+    (host,) = [s for s in srcs if "int lbd_enqueue(" in s]
+    assert "sincosf(kl_angle[k]" in host
 
 
 def test_trig_binding_case_depends_on_the_binding():
@@ -82,7 +86,7 @@ def test_trig_binding_case_depends_on_the_binding():
 
 def test_reference_coefficient_tables():
     """The reference constructor's gaussCoefL_ / gaussCoefG_ are exp() in double of integer-divided centres and sigmas, the
-    recipe capi.cu's lbd_init follows for the kernel's float tables (which the GPU goldens exercise)."""
+    recipe capi_features.cu's lbd_init follows for the kernel's float tables (which the GPU goldens exercise)."""
     if not lbd.available():
         pytest.skip("oracle/_ref/libplstvo_ref_lbd.so not built (needs the reference checkout)")
     cl, cg = lbd.coefficients()
