@@ -354,6 +354,40 @@ int plstvo_lbd_compute_batch(PlContext* ctx, int n_img, int width, int height, c
 /* Device time of the last plstvo_lbd_compute_batch on this context, ms: [0] blur and Sobel, [1] descriptors. */
 int plstvo_lbd_kernel_times(PlContext* ctx, float* ms2);
 
+/* ---- LSD line detection: StereoFrame::detectLineFeatures' LSD branch (src/stereoFrame.cpp:218-241) ---- */
+typedef struct PlLsdConfig {       /* Config::lsd*; src/config.cpp defaults */
+    int32_t refine;                /* lsd_refine: 0 (LSD_REFINE_NONE) only */
+    double  scale;                 /* lsd_scale (> 0, not 0.5): the image is blurred and resized by it before detection */
+    double  sigma_scale;           /* lsd_sigma_scale (> 0) */
+    double  quant;                 /* lsd_quant (>= 0) */
+    double  ang_th;                /* lsd_ang_th, degrees, (0, 180) */
+    int32_t n_bins;                /* lsd_n_bins, 1..4096 */
+    double  min_line_length;       /* min_line_length (>= 0), relative to min(width, height) as in Config */
+    int32_t n_features;            /* lsd_nfeatures (>= 0; 0 keeps every line) */
+} PlLsdConfig;
+void plstvo_default_lsd_config(PlLsdConfig* c);   /* 0, 1.2, 0.6, 2.0, 22.5, 1024, 0.025, 300 */
+/* Key lines of n_img grey images of one size (images: [n_img][height][width] uint8), bit-identical to the reference's
+ * LSDDetectorC::detect(img, lines, 1, 1, opts) on OpenCV 4.13's LineSegmentDetector followed by detectLineFeatures'
+ * response sort and truncation to n_features, with min_length = min_line_length * min(width, height).  Image i's lines are
+ * rows kl_off[i] .. kl_off[i + 1] of kl_seg ([n][4] float sPointInOctaveX, sPointInOctaveY, ePointInOctaveX,
+ * ePointInOctaveY), kl_angle (KeyLine::angle, radians), kl_npix (numOfPixels), kl_response and kl_length (lineLength), in
+ * the reference's order (class_id is the row within the image).  These are what plstvo_lbd_compute_batch and
+ * PlStereoImages take.  numOfPixels is LineIterator's count after clipping to the image, so it is 0 for a line whose
+ * rounded endpoints both leave the image on one side (plstvo_lbd_compute_batch rejects such a line, as it rejects any
+ * numOfPixels outside 1..32767).  Any of kl_seg .. kl_length may be NULL to skip that output.  Returns the number of lines.
+ * PLSTVO_E_TOO_LARGE: more than capacity lines in all, or more than PLSTVO_MAX_FEATURES in one image; kl_off ([n_img + 1]) is
+ * still written in full.  PLSTVO_E_INVALID: a null config, kl_off or images, more than 65535 images, width or height outside
+ * 1..32767, refine != 0,
+ * a parameter outside the ranges above, a blur wider than 31 taps, or a scaled size outside 1..32767.  The whole batch is
+ * resident at once: about 35 bytes of device memory per pixel of each scaled image (24 MB per 1241x376 image at scale 1.2);
+ * PLSTVO_E_CUDA when that cannot be allocated. */
+int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                            int capacity, int32_t* kl_off, float* kl_seg, float* kl_angle, int32_t* kl_npix,
+                            float* kl_response, float* kl_length);
+/* Device time of the last plstvo_lsd_detect_batch on this context, ms: [0] blur and resize, [1] gradient and seed order,
+ * [2] region growing, [3] the host's region angles, [4] rectangles. */
+int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5);
+
 /* ---- stereo images in, pose out: StereoFrame::extractStereoFeatures (src/stereoFrame.cpp:59-118, :182-243) with LSD left
  * to the caller, then matchStereoPoints / matchStereoLines, f2fTracking and optimizePose ---- */
 typedef struct PlStereoImages {

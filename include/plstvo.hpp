@@ -181,6 +181,40 @@ inline int computeLBD(Context& c, const uint8_t* image, int width, int height, K
     kl.desc = std::move(desc);
     return k;
 }
+// LSD key lines of one grey image (row-major, width * height bytes), as StereoFrame::detectLineFeatures detects them
+// (src/stereoFrame.cpp:218-241) with llength_th = cfg.min_line_length * min(width, height), the product
+// StereoFrameHandler computes (src/stereoFrameHandler.cpp:39).  kl.seg, kl.angle and kl.octave (all 0) are replaced by the
+// key lines in the reference's order and kl.desc is cleared; num_pixels (what computeLBD takes), response and length (if
+// given) likewise.  Returns the line count.
+inline int detectLSD(Context& c, const PlLsdConfig& cfg, const uint8_t* image, int width, int height, KeyLines& kl,
+                     std::vector<int32_t>& num_pixels, std::vector<float>* response = nullptr,
+                     std::vector<float>* length = nullptr) {
+    int cap = cfg.n_features > 0 ? cfg.n_features : 1024;
+    std::vector<float> resp, len;
+    for (;;) {
+        int32_t off[2] = {0, 0};
+        kl.seg.resize(4 * (size_t)cap);
+        kl.angle.resize((size_t)cap);
+        num_pixels.resize((size_t)cap);
+        resp.resize((size_t)cap);
+        len.resize((size_t)cap);
+        const int rc = plstvo_lsd_detect_batch(c.get(), &cfg, 1, width, height, image, cap, off, kl.seg.data(), kl.angle.data(),
+                                               num_pixels.data(), resp.data(), len.data());
+        if (rc == PLSTVO_E_TOO_LARGE && off[1] > cap && off[1] <= PLSTVO_MAX_FEATURES) {   // more lines than the first guess
+            cap = off[1];
+            continue;
+        }
+        const int n = c.check(rc);
+        kl.seg.resize(4 * (size_t)n);
+        kl.angle.resize((size_t)n);
+        kl.octave.assign((size_t)n, 0);
+        kl.desc.clear();
+        num_pixels.resize((size_t)n);
+        if (response) response->assign(resp.begin(), resp.begin() + n);
+        if (length) length->assign(len.begin(), len.begin() + n);
+        return n;
+    }
+}
 // One stereo frame as StereoFrame::extractStereoFeatures starts it (src/stereoFrame.cpp:59-118, :182-243): the two grey images
 // (row-major, width * height bytes each) and the key lines LSD kept on each (octave 0: start / end point [m][4], KeyLine::angle,
 // KeyLine::numOfPixels).  fast_th 0: the config's FAST threshold.

@@ -1,5 +1,6 @@
 // capi_features.cu — the C-ABI's feature extraction on the GPU: ORB description and detection (orb.cu), LBD description
 // (lbd.cu), and pose tracking from stereo images, where both feed the stereo step and the tracker without leaving HBM.
+#include <cfloat>
 #include <climits>
 #include <cstring>
 #include <functional>
@@ -673,6 +674,272 @@ int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4) {
     if (!ctx->orb_detected) return fail(ctx, PLSTVO_E_INVALID, "no ORB detect call on this context yet");
     CK(ctx, cudaSetDevice(ctx->device));
     for (int k = 0; k < 4; ++k) CK(ctx, cudaEventElapsedTime(&ms4[k], ctx->orb_det_ev[k], ctx->orb_det_ev[k + 1]));
+    return 0;
+}
+
+/* ---- LSD line detection (lsd.cu) ---- */
+void plstvo_default_lsd_config(PlLsdConfig* c) {
+    if (!c) return;
+    c->refine = 0; c->scale = 1.2; c->sigma_scale = 0.6; c->quant = 2.0; c->ang_th = 22.5; c->n_bins = 1024;
+    c->min_line_length = 0.025; c->n_features = 300;
+}
+
+namespace {
+constexpr double kLsdPi = 3.14159265358979323846;
+
+// cv::fastAtan2 on the host, for the trig table: x86-64's baseline has no FMA, so nothing here is fused (as in lsd.cu)
+float host_fast_atan2(float y, float x) {
+    const float deg = (float)(180 / kLsdPi);
+    const float p1 = 0.9997878412794807f * deg, p3 = -0.3258083974640975f * deg, p5 = 0.1555786518463281f * deg,
+                p7 = -0.04432655554792128f * deg;
+    const float ax = fabsf(x), ay = fabsf(y), eps = (float)2.2204460492503131e-16;
+    const bool wide = ax >= ay;
+    const float c = wide ? ay / (ax + eps) : ax / (ay + eps), c2 = c * c;
+    float a = (((p7 * c2 + p5) * c2 + p3) * c2 + p1) * c;
+    if (!wide) a = 90.f - a;
+    if (x < 0) a = 180.f - a;
+    if (y < 0) a = 360.f - a;
+    return a;
+}
+
+// Region growing moves the region angle by the float sums of cos / sin: the seed's (float)cos(double), and cosf / sinf of
+// each accepted pixel's float angle.  No device function rounds these as the C library does, and a pixel's angle depends
+// only on its gradient pair, so the four values of every pair are computed here once per context, with the same library.
+cudaError_t lsd_init(PlContext* ctx) {
+    if (ctx->lsd_trig.p) return cudaSuccess;
+    std::vector<float4> t((size_t)LSD_TRIG_SIDE * LSD_TRIG_SIDE);
+    for (int gx = -LSD_GRAD_MAX; gx <= LSD_GRAD_MAX; ++gx)
+        for (int gy = -LSD_GRAD_MAX; gy <= LSD_GRAD_MAX; ++gy) {
+            const double a = (double)host_fast_atan2((float)gx, (float)-gy) * (kLsdPi / 180.0);
+            const float af = (float)a;
+            t[(size_t)(gx + LSD_GRAD_MAX) * LSD_TRIG_SIDE + (gy + LSD_GRAD_MAX)] =
+                make_float4((float)cos(a), (float)sin(a), cosf(af), sinf(af));
+        }
+    cudaError_t e = ctx->lsd_ev.create();
+    if (e == cudaSuccess) e = ctx->lsd_trig.ensure(t.size() * sizeof(float4));
+    if (e == cudaSuccess) e = cudaMemcpy(ctx->lsd_trig.p, t.data(), t.size() * sizeof(float4), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) ctx->lsd_trig.release();
+    return e;
+}
+
+struct KeyLine {
+    float seg[4], angle, response, length;
+    int32_t npix;
+};
+
+// cv::LineIterator(img, Point(start), Point(end)).count, 8-connected.  The endpoints are rounded half to even; one in
+// [W - 0.5, W) (or the same in y) rounds outside the image, and LineIterator then clips the segment with clipLine
+// (Cohen-Sutherland on integers, intersections truncated toward zero) before counting; 0 when nothing is left.
+int line_iterator_count(int W, int H, const float* e) {
+    int64_t x1 = lrintf(e[0]), y1 = lrintf(e[1]), x2 = lrintf(e[2]), y2 = lrintf(e[3]);
+    const int64_t right = W - 1, bottom = H - 1;
+    if ((uint64_t)x1 >= (uint64_t)W || (uint64_t)x2 >= (uint64_t)W || (uint64_t)y1 >= (uint64_t)H ||
+        (uint64_t)y2 >= (uint64_t)H) {
+        int c1 = (x1 < 0) + (x1 > right) * 2 + (y1 < 0) * 4 + (y1 > bottom) * 8;
+        int c2 = (x2 < 0) + (x2 > right) * 2 + (y2 < 0) * 4 + (y2 > bottom) * 8;
+        if ((c1 & c2) == 0 && (c1 | c2) != 0) {
+            int64_t a;
+            if (c1 & 12) {
+                a = c1 < 8 ? 0 : bottom;
+                x1 += (int64_t)((double)(a - y1) * (double)(x2 - x1) / (double)(y2 - y1));
+                y1 = a;
+                c1 = (x1 < 0) + (x1 > right) * 2;
+            }
+            if (c2 & 12) {
+                a = c2 < 8 ? 0 : bottom;
+                x2 += (int64_t)((double)(a - y2) * (double)(x2 - x1) / (double)(y2 - y1));
+                y2 = a;
+                c2 = (x2 < 0) + (x2 > right) * 2;
+            }
+            if ((c1 & c2) == 0 && (c1 | c2) != 0) {
+                if (c1) {
+                    a = c1 == 1 ? 0 : right;
+                    y1 += (int64_t)((double)(a - x1) * (double)(y2 - y1) / (double)(x2 - x1));
+                    x1 = a;
+                    c1 = 0;
+                }
+                if (c2) {
+                    a = c2 == 1 ? 0 : right;
+                    y2 += (int64_t)((double)(a - x2) * (double)(y2 - y1) / (double)(x2 - x1));
+                    x2 = a;
+                    c2 = 0;
+                }
+            }
+        }
+        if (c1 | c2) return 0;
+    }
+    return (int)std::max(std::llabs(x2 - x1), std::llabs(y2 - y1)) + 1;
+}
+
+// LSDDetectorC::detectImpl's KeyLine step for one octave (3rdparty/line_descriptor/src/LSDDetector_custom.cpp:266-308)
+// and detectLineFeatures' sort-and-truncate (src/stereoFrame.cpp:232-241), on the host: a few hundred lines per image, and
+// atan2f is the C library's.  std::sort is the reference's own (libstdc++) sort, so equal responses keep its order.
+void lsd_keylines(int W, int H, const float4* raw, int n, double min_length, int n_features, std::vector<KeyLine>& out) {
+    out.clear();
+    for (int k = 0; k < n; ++k) {
+        float e[4] = {raw[k].x, raw[k].y, raw[k].z, raw[k].w};
+        for (int c = 0; c < 4; ++c) {   // checkLineExtremes
+            const int lim = (c & 1) ? H : W;
+            if (e[c] < 0) e[c] = 0;
+            if (e[c] >= lim) e[c] = (float)lim - 1.0f;
+        }
+        const double dx = (double)(e[0] - e[2]), dy = (double)(e[1] - e[3]);
+        const double length = (float)sqrt(dx * dx + dy * dy);   // (float)sqrt(pow(.., 2) + pow(.., 2)); the squares are exact
+        if (!(length > min_length)) continue;
+        KeyLine kl;
+        memcpy(kl.seg, e, sizeof e);
+        kl.length = (float)length;
+        kl.npix = line_iterator_count(W, H, e);
+        kl.angle = atan2f(e[3] - e[1], e[2] - e[0]);
+        kl.response = kl.length / (float)std::max(W, H);
+        out.push_back(kl);
+    }
+    if ((int)out.size() > n_features && n_features != 0) {
+        std::sort(out.begin(), out.end(), [](const KeyLine& a, const KeyLine& b) { return a.response > b.response; });
+        out.resize((size_t)n_features);
+    }
+}
+
+int lsd_check_config(PlContext* ctx, const PlLsdConfig* c) {
+    if (c->refine != 0) return fail(ctx, PLSTVO_E_INVALID, "lsd refine: only 0 (LSD_REFINE_NONE) is supported");
+    if (!(c->scale > 0) || !std::isfinite(c->scale) || !(c->sigma_scale > 0) || !std::isfinite(c->sigma_scale) ||
+        !(c->quant >= 0) || !std::isfinite(c->quant) || !(c->ang_th > 0 && c->ang_th < 180) || c->n_bins < 1 ||
+        c->n_bins > 4096 || !(c->min_line_length >= 0) || !std::isfinite(c->min_line_length) || c->n_features < 0)
+        return fail(ctx, PLSTVO_E_INVALID, "lsd parameter out of range");
+    // resize() takes INTER_AREA instead of INTER_LINEAR_EXACT when 1 / scale is 2 (its "area fast" case), which differs at
+    // the last row and column of odd sizes; that path is not built
+    if (fabs(1.0 / c->scale - 2.0) < DBL_EPSILON) return fail(ctx, PLSTVO_E_INVALID, "lsd scale 0.5 is not supported");
+    return 0;
+}
+}  // namespace
+
+int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                            int capacity, int32_t* kl_off, float* kl_seg, float* kl_angle, int32_t* kl_npix,
+                            float* kl_response, float* kl_length) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || capacity < 0) return fail(ctx, PLSTVO_E_INVALID, "null config, negative n_img or negative capacity");
+    if (n_img > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");   // gridDim.z of the pixel kernels
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+    if (const int rc = lsd_check_config(ctx, cfg)) return rc;
+    if (!kl_off) return fail(ctx, PLSTVO_E_INVALID, "null kl_off");
+    // flsd: blur with sigma_scale (/ scale when shrinking), half-width ceil(sigma * sqrt(2 * 3 * ln 10)), then resize
+    LsdLaunch L{};
+    L.n_img = n_img; L.W = width; L.H = height; L.scale = cfg->scale; L.n_bins = cfg->n_bins;
+    L.w = width; L.h = height;
+    if (cfg->scale != 1) {
+        const double sigma = cfg->scale < 1 ? cfg->sigma_scale / cfg->scale : cfg->sigma_scale;
+        const double kh = ceil(sigma * sqrt(2 * 3 * log(10.0)));
+        if (!(kh <= LSD_MAX_KH)) return fail(ctx, PLSTVO_E_INVALID, "lsd blur wider than 31 taps");
+        L.taps.kh = (int)kh;
+        // getGaussianKernelBitExact: exp(-x^2 / (2 sigma^2)) normalised to sum 1, rounded to 8 fractional bits
+        std::vector<double> v((size_t)L.taps.kh);
+        const double scale2 = -0.125 / (sigma * sigma);
+        double sum = 0;
+        for (int i = 0, x = -2 * L.taps.kh; i < L.taps.kh; ++i, x += 2) sum += (v[(size_t)i] = exp((double)(x * x) * scale2));
+        const double mul = 1 / (sum * 2 + 1);
+        // getGaussianKernelFixedPoint_ED: the side taps from the outside in, each rounding error carried into the next; the
+        // centre takes what is left of 256
+        double err = 0;
+        int side = 0;
+        for (int i = 0; i < L.taps.kh; ++i) {
+            const double adj = v[(size_t)i] * mul * 256.0 + err;
+            const int t = (int)lrint(adj);
+            err = adj - (double)t;
+            L.taps.t[i] = L.taps.t[2 * L.taps.kh - i] = t;
+            side += t;
+        }
+        L.taps.t[L.taps.kh] = 256 - 2 * side;
+        const double ws = rint((double)width * cfg->scale), hs = rint((double)height * cfg->scale);
+        if (!(ws >= 1 && ws <= 32767 && hs >= 1 && hs <= 32767)) return fail(ctx, PLSTVO_E_INVALID, "lsd scaled size must be 1..32767");
+        L.w = (int)ws;
+        L.h = (int)hs;
+    }
+    kl_off[0] = 0;
+    if (n_img == 0) return 0;
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    const double prec = kLsdPi * cfg->ang_th / 180, p = cfg->ang_th / 180;
+    L.prec = prec;
+    L.rho = cfg->quant / sin(prec);
+    const double log_nt = 5 * (log10((double)L.w) + log10((double)L.h)) / 2 + log10(11.0);
+    const double min_reg = -log_nt / log10(p);
+    L.min_reg = min_reg >= (double)INT_MAX ? INT_MAX : (int)(size_t)min_reg;
+    const size_t N = (size_t)L.w * L.h;
+    L.reg_cap = (int)(N / (size_t)std::max(L.min_reg, 1) + 1);
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, lsd_init(ctx));
+    cudaStream_t s = ctx->s_main;
+    const size_t in_bytes = (size_t)n_img * width * height;
+    Arena a;
+    const size_t o_img = a.take(in_bytes), o_blur = a.take(cfg->scale != 1 ? in_bytes : 0),
+                 o_scaled = a.take(cfg->scale != 1 ? (size_t)n_img * N : 0), o_scr = a.take(lsd_scratch_bytes(n_img, L.w, L.h)),
+                 o_max = a.take((size_t)n_img * 8), o_hist = a.take((size_t)n_img * L.n_bins * 4), o_ns = a.take((size_t)n_img * 4),
+                 o_reg = a.take((size_t)n_img * L.reg_cap * sizeof(LsdRegion)), o_nreg = a.take((size_t)n_img * 4);
+    CK(ctx, a.alloc(ctx->arena_lsd));
+    L.images = a.u8(o_img); L.blurred = a.u8(o_blur); L.scaled = a.u8(o_scaled); L.scratch = a.u8(o_scr);
+    L.max_bits = a.at<unsigned long long>(o_max); L.hist = a.i32(o_hist); L.n_seeds = a.i32(o_ns);
+    L.trig = ctx->lsd_trig.as<const float4>(); L.regions = a.at<LsdRegion>(o_reg); L.n_regions = a.i32(o_nreg);
+    CK(ctx, a.up(o_img, images, in_bytes, s));
+    int launches = 0;
+    cudaEvent_t* ev = ctx->lsd_ev.ev;
+    CK(ctx, launch_lsd_grow(L, s, ev, &launches));
+    ctx->lsd_ran = true;
+    std::vector<int32_t> nreg((size_t)n_img), r_off((size_t)n_img + 1, 0);
+    CK(ctx, a.down(nreg.data(), o_nreg, (size_t)n_img * 4, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    for (int i = 0; i < n_img; ++i) r_off[(size_t)i + 1] = r_off[(size_t)i] + nreg[(size_t)i];
+    const size_t R = (size_t)r_off[(size_t)n_img];
+    std::vector<LsdRegion> regs(R);
+    for (int i = 0; i < n_img; ++i)
+        CK(ctx, a.down(regs.data() + r_off[(size_t)i], o_reg + (size_t)i * L.reg_cap * sizeof(LsdRegion),
+                       (size_t)nreg[(size_t)i] * sizeof(LsdRegion), s));
+    CK(ctx, cudaStreamSynchronize(s));
+    // region2rect's dx, dy: the C library's cos / sin of the angle, as in the reference
+    std::vector<double2> dir(R);
+    for (size_t r = 0; r < R; ++r) dir[r] = make_double2(cos(regs[r].theta), sin(regs[r].theta));
+    Arena b;
+    const size_t o_roff = b.take(((size_t)n_img + 1) * 4), o_dir = b.take(R * 16), o_seg = b.take(R * 16);
+    CK(ctx, b.alloc(ctx->arena_lsd_seg));
+    CK(ctx, b.up(o_roff, r_off.data(), ((size_t)n_img + 1) * 4, s));
+    CK(ctx, b.up(o_dir, dir.data(), R * 16, s));
+    CK(ctx, cudaEventRecord(ev[4], s));
+    CK(ctx, launch_lsd_extent(L, (int)R, b.i32(o_roff), b.at<double2>(o_dir), b.at<float4>(o_seg), s, &launches));
+    CK(ctx, cudaEventRecord(ev[5], s));
+    ctx->launches += launches;
+    std::vector<float4> raw(R);
+    CK(ctx, b.down(raw.data(), o_seg, R * 16, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    // the KeyLine step and the truncation per image; kl_off in full before any capacity check
+    const double min_length = cfg->min_line_length * std::min(width, height);
+    std::vector<std::vector<KeyLine>> kls((size_t)n_img);
+    bool too_many = false;
+    for (int i = 0; i < n_img; ++i) {
+        lsd_keylines(width, height, raw.data() + r_off[(size_t)i], nreg[(size_t)i], min_length, cfg->n_features, kls[(size_t)i]);
+        const long next = (long)kl_off[i] + (long)kls[(size_t)i].size();
+        too_many |= kls[(size_t)i].size() > (size_t)PLSTVO_MAX_FEATURES || next > INT_MAX;
+        kl_off[i + 1] = (int32_t)std::min(next, (long)INT_MAX);
+    }
+    if (too_many) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+    if (kl_off[n_img] > capacity) return fail(ctx, PLSTVO_E_TOO_LARGE, "more key lines than capacity");
+    for (int i = 0; i < n_img; ++i)
+        for (size_t k = 0; k < kls[(size_t)i].size(); ++k) {
+            const KeyLine& kl = kls[(size_t)i][k];
+            const size_t r = (size_t)kl_off[i] + k;
+            if (kl_seg) memcpy(kl_seg + 4 * r, kl.seg, sizeof kl.seg);
+            if (kl_angle) kl_angle[r] = kl.angle;
+            if (kl_npix) kl_npix[r] = kl.npix;
+            if (kl_response) kl_response[r] = kl.response;
+            if (kl_length) kl_length[r] = kl.length;
+        }
+    return kl_off[n_img];
+}
+
+int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
+    if (!ctx || !ms5) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->lsd_ran) return fail(ctx, PLSTVO_E_INVALID, "no LSD call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    for (int k = 0; k < 5; ++k) CK(ctx, cudaEventElapsedTime(&ms5[k], ctx->lsd_ev[k], ctx->lsd_ev[k + 1]));
     return 0;
 }
 

@@ -237,6 +237,49 @@ void launch_orb_harris_write(const OrbDevLevels& L, const OrbDetectLevels& D, in
                              const int32_t* out_off, float* out_xy, int32_t* out_oct, float* out_resp, int32_t* out_rank,
                              cudaStream_t s, int* launches);
 
+__device__ __forceinline__ float fast_atan2(float y, float x) {   // cv::fastAtan2, unfused like OpenCV's build
+    constexpr float deg = (float)(180 / 3.14159265358979323846);
+    constexpr float p1 = 0.9997878412794807f * deg, p3 = -0.3258083974640975f * deg, p5 = 0.1555786518463281f * deg,
+                    p7 = -0.04432655554792128f * deg;
+    const float ax = fabsf(x), ay = fabsf(y), eps = (float)2.2204460492503131e-16;
+    float a, c, c2;
+    const bool wide = ax >= ay;
+    c = wide ? __fdiv_rn(ay, __fadd_rn(ax, eps)) : __fdiv_rn(ax, __fadd_rn(ay, eps));
+    c2 = __fmul_rn(c, c);
+    a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
+    if (!wide) a = __fsub_rn(90.f, a);
+    if (x < 0) a = __fsub_rn(180.f, a);
+    if (y < 0) a = __fsub_rn(360.f, a);
+    return a;
+}
+
+// lsd.cu: LSD line segments (cv::LineSegmentDetector, LSD_REFINE_NONE) on a batch of grey images of one size
+constexpr int LSD_GRAD_MAX = 510;                      // |gx|, |gy| of the 2x2 gradient
+constexpr int LSD_TRIG_SIDE = 2 * LSD_GRAD_MAX + 1;    // trig table: code = (gx + 510) * 1021 + (gy + 510)
+constexpr int LSD_MAX_KH = 15;                         // blur half-width
+struct LsdTaps { int kh; int t[2 * LSD_MAX_KH + 1]; };   // GaussianBlur's fixed-point taps (8 fractional bits)
+struct LsdRegion { double cx, cy, theta; int32_t start, count; };   // a kept region: centroid, angle, its pixels in rpix
+struct LsdLaunch {
+    int n_img, W, H, w, h;         // input size, scaled size
+    double scale, rho, prec;       // scale, gradient threshold quant / sin(prec), angle tolerance (radians)
+    int min_reg, reg_cap, n_bins;  // smallest kept region, region records per image, bins
+    LsdTaps taps;
+    const uint8_t* images;         // [n_img][H][W]
+    uint8_t *blurred, *scaled;     // [n_img][H][W], [n_img][h][w] (unused where scale == 1; scaled unused where w, h == W, H)
+    uint8_t* scratch;              // lsd_scratch_bytes(n_img, w, h)
+    unsigned long long* max_bits;  // [n_img]
+    int32_t *hist, *n_seeds;       // [n_img][n_bins], [n_img]
+    const float4* trig;            // [LSD_TRIG_SIDE^2]: (float)cos, (float)sin of the angle; cosf, sinf of (float)angle
+    LsdRegion* regions;            // [n_img][reg_cap]
+    int32_t* n_regions;            // [n_img]
+};
+size_t lsd_scratch_bytes(int n_img, int w, int h);
+// ev[0..3]: start, blur + resize, gradient + seed order, region growing
+cudaError_t launch_lsd_grow(const LsdLaunch& L, cudaStream_t s, cudaEvent_t* ev, int* launches);
+// regions r_off[i] .. r_off[i + 1] of image i (n_reg in all), dir [n_reg] (cos, sin) of their angles -> seg [n_reg]
+cudaError_t launch_lsd_extent(const LsdLaunch& L, int n_reg, const int32_t* r_off, const double2* dir, float4* seg,
+                              cudaStream_t s, int* launches);
+
 // lbd.cu: LBD descriptors of given octave-0 key lines (BinaryDescriptor::compute, default Params) on a batch of images
 cudaError_t lbd_upload_tables(const float* coef_g, const float* coef_l);   // (float)gaussCoefG_ [63], (float)gaussCoefL_ [21]
 cudaError_t launch_lbd(int n_img, int W, int H, const uint8_t* images, const int32_t* kl_off, int n_lines, const float* seg,

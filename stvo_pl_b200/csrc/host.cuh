@@ -184,6 +184,11 @@ struct PlContext {
     plstvo::DevBuf arena_lbd;      // plstvo_lbd_compute_batch: images, gradients, key lines, descriptors
     bool lbd_tables = false, lbd_computed = false;
     plstvo::Events<3> lbd_ev;
+    plstvo::DevBuf arena_lsd;      // plstvo_lsd_detect_batch: images, scaled images, per-pixel scratch, regions
+    plstvo::DevBuf arena_lsd_seg;  // its per-region arrays, sized once the regions are counted
+    plstvo::DevBuf lsd_trig;       // cos / sin table of the gradient angles (lsd.cu), built once
+    bool lsd_ran = false;
+    plstvo::Events<6> lsd_ev;
     // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
     plstvo::Events<4> img_ev;
     plstvo::Events<1> img_join;

@@ -152,22 +152,6 @@ orb_filter_kernel(int W, int H, int edge, const int32_t* __restrict__ kp_off, co
     if (tid == 0) counts[img] = s_base;
 }
 
-__device__ __forceinline__ float fast_atan2(float y, float x) {   // cv::fastAtan2, unfused like OpenCV's build
-    constexpr float deg = (float)(180 / 3.14159265358979323846);
-    constexpr float p1 = 0.9997878412794807f * deg, p3 = -0.3258083974640975f * deg, p5 = 0.1555786518463281f * deg,
-                    p7 = -0.04432655554792128f * deg;
-    const float ax = fabsf(x), ay = fabsf(y), eps = (float)2.2204460492503131e-16;
-    float a, c, c2;
-    const bool wide = ax >= ay;
-    c = wide ? __fdiv_rn(ay, __fadd_rn(ax, eps)) : __fdiv_rn(ax, __fadd_rn(ay, eps));
-    c2 = __fmul_rn(c, c);
-    a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
-    if (!wide) a = __fsub_rn(90.f, a);
-    if (x < 0) a = __fsub_rn(180.f, a);
-    if (y < 0) a = __fsub_rn(360.f, a);
-    return a;
-}
-
 __global__ void __launch_bounds__(THREADS)
 orb_describe_kernel(OrbDevLevels L, int n_img, const uint8_t* __restrict__ images, const uint8_t* __restrict__ raw_pyr,
                     const uint8_t* __restrict__ blur_pyr, const int32_t* __restrict__ kp_off, const float* __restrict__ kp_xy,

@@ -97,6 +97,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_orb_detect_kernel_times": (C.c_int, [vp, fp]),
         "plstvo_lbd_compute_batch": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, u8p, i32p, fp, fp, i32p, u8p]),
         "plstvo_lbd_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_default_lsd_config": (None, [C.POINTER(T.PlLsdConfig)]),
+        "plstvo_lsd_detect_batch": (C.c_int, [vp, C.POINTER(T.PlLsdConfig), C.c_int, C.c_int, C.c_int, u8p, C.c_int, i32p, fp, fp,
+                                              i32p, fp, fp]),
+        "plstvo_lsd_kernel_times": (C.c_int, [vp, fp]),
         "plstvo_track_stereo_images_batch": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig), C.POINTER(T.PlStereoConfig),
                                                        C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlStereoImages),
                                                        C.POINTER(T.PlStereoImages), vp, vp, i32p]),
@@ -124,7 +128,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
-    "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_track_stereo_images_batch",
+    "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
+    "plstvo_lsd_kernel_times", "plstvo_track_stereo_images_batch",
     "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_stage_times"]
 
 
@@ -423,6 +428,38 @@ class Engine:
         """Device ms of the last lbd_compute_batch: blur + Sobel, descriptors."""
         ms = np.zeros(2, np.float32)
         self._ck(self.lib.plstvo_lbd_kernel_times(self.ctx, _p(ms, T.c_float_p)))
+        return ms
+
+    def lsd_detect_batch(self, cfg: T.PlLsdConfig, images, capacity: Optional[int] = None):
+        """detectLineFeatures' LSD key lines of each of images uint8[n, H, W].  Returns (total, dict(off [n + 1], seg [total, 4]
+        sPointInOctave / ePointInOctave, angle, npix, response, length)); image i's lines are rows off[i] .. off[i + 1], in
+        the reference's order.  Without a capacity the call sizes its buffers from n_features (or calls again with the exact
+        count); with one, more than capacity raises PLSTVO_E_TOO_LARGE."""
+        images = np.ascontiguousarray(images, np.uint8)
+        n_img, H, W = images.shape
+        cap = int(capacity) if capacity is not None else n_img * (max(int(cfg.n_features), 0) or 1024)
+        while True:
+            off = np.zeros(n_img + 1, np.int32)
+            out = dict(off=off, seg=np.zeros((cap, 4), np.float32), angle=np.zeros(cap, np.float32),
+                       npix=np.zeros(cap, np.int32), response=np.zeros(cap, np.float32), length=np.zeros(cap, np.float32))
+            rc = self.lib.plstvo_lsd_detect_batch(
+                self.ctx, C.byref(cfg), n_img, W, H, _p(images, T.c_uint8_p), cap, _p(off, T.c_int32_p),
+                _p(out["seg"], T.c_float_p), _p(out["angle"], T.c_float_p), _p(out["npix"], T.c_int32_p),
+                _p(out["response"], T.c_float_p), _p(out["length"], T.c_float_p))
+            if rc == -2 and capacity is None and off[-1] > cap and np.diff(off).max() <= 65535:
+                cap = int(off[-1])
+                continue
+            total = self._ck(rc)
+            break
+        for k in ("seg", "angle", "npix", "response", "length"):
+            out[k] = out[k][:total]
+        return total, out
+
+    def lsd_kernel_times(self):
+        """Device ms of the last lsd_detect_batch: blur + resize, gradient + seed order, region growing, the host's region
+        angles (with its round trip), rectangles."""
+        ms = np.zeros(5, np.float32)
+        self._ck(self.lib.plstvo_lsd_kernel_times(self.ctx, _p(ms, T.c_float_p)))
         return ms
 
     def stereo_lift_lines(self, cam, scfg: T.PlStereoConfig, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, m12):

@@ -83,6 +83,21 @@ class PlOrbDetectConfig(C.Structure):
     _fields_ = [("orb", PlOrbConfig), ("n_features", C.c_int32), ("score_type", C.c_int32), ("fast_threshold", C.c_int32)]
 
 
+class PlLsdConfig(C.Structure):
+    """LineSegmentDetector parameters of plstvo_lsd_detect_batch (Config::lsd*), min_line_length relative to min(W, H)."""
+    _fields_ = [("refine", C.c_int32), ("scale", C.c_double), ("sigma_scale", C.c_double), ("quant", C.c_double),
+                ("ang_th", C.c_double), ("n_bins", C.c_int32), ("min_line_length", C.c_double), ("n_features", C.c_int32)]
+
+
+def default_lsd_config(n_features: int = 300, **kw) -> "PlLsdConfig":
+    """The shipped configs' LSD options: refine 0, scale 1.2, sigma_scale 0.6, quant 2.0, ang_th 22.5, n_bins 1024,
+    min_line_length 0.025; keyword arguments override any field."""
+    c = PlLsdConfig(0, 1.2, 0.6, 2.0, 22.5, 1024, 0.025, n_features)
+    for k, v in kw.items():
+        setattr(c, k, v)
+    return c
+
+
 ORB_HARRIS_SCORE, ORB_FAST_SCORE = 0, 1
 
 
