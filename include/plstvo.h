@@ -389,7 +389,8 @@ int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, i
 int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5);
 
 /* ---- stereo images in, pose out: StereoFrame::extractStereoFeatures (src/stereoFrame.cpp:59-118, :182-243) with LSD left
- * to the caller, then matchStereoPoints / matchStereoLines, f2fTracking and optimizePose ---- */
+ * to the caller, then matchStereoPoints / matchStereoLines, f2fTracking and optimizePose (plstvo_track_stereo_images_lsd_*
+ * below run LSD too) ---- */
 typedef struct PlStereoImages {
     int32_t        B;                                  /* frames */
     int32_t        width, height;                      /* every image; must equal cam->width / height */
@@ -426,9 +427,44 @@ int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, con
                                         const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
                                         const PlPrior* priors, PlPoseResult* results,
                                         int32_t* n_stereo /* [B+1][2], as plstvo_track_stereo_sequence */);
+
+/* ---- stereo images alone in, pose out: the same with LSD inside the call (StereoFrameHandler::initialize / insertStereoPair
+ * take images and nothing else, app/imagesStVO.cpp:88-97) ----
+ * The signatures of the two calls above plus lcfg.  Results and n_stereo equal, byte for byte, the two-call chain
+ *   1. plstvo_lsd_detect_batch(lcfg) on every image, in the images call's block order;
+ *   2. plstvo_track_stereo_images_batch / _sequence fed those key lines (angle, numOfPixels, octave 0);
+ * and so, through the contract above, LSD -> ORB -> LBD -> plstvo_track_stereo_*.  Each image goes up once and every stage
+ * reads that device copy.  With at least as many images in the call as the GPU has SMs, LSD's pixel stages and region growing
+ * run on a second stream beside ORB; with fewer, where LSD's one-thread-per-image region growing is the whole critical path and
+ * loses more beside ORB than ORB takes, LSD runs first and ORB then runs beside LBD.  What crosses PCIe besides the images and the results is the host hop of the
+ * lines: LSD's region counts and records come down, the double cos / sin of the region angles go up, the raw segments come
+ * down for the KeyLine step (glibc's atan2f, libstdc++'s std::sort), and the kept key lines go back up with their sincosf
+ * direction for LBD; a few KB per image.  The previous images calls' host hops apply as well.
+ * The key-line fields of every PlStereoImages (ll_off .. npix_r) must be NULL.  cfg->has_lines == 0: LSD does not run, lcfg
+ * may be NULL, and the result is that of the images call without lines; cfg->has_points == 0: ORB does not run.
+ * Returns 0 (B == 0, or a sequence of one frame: 0, nothing runs).  PLSTVO_E_INVALID: a non-NULL key-line field, a NULL lcfg
+ * with lines on, plstvo_lsd_detect_batch's config checks (refine != 0, scale 0.5, ranges, a blur wider than 31 taps, a scaled
+ * size outside 1..32767), more than 65535 images in the call (4 B for a batch, 2 B for a sequence), or a numOfPixels LSD
+ * leaves outside 1..32767 (as the chain's step 2 rejects it); PLSTVO_E_TOO_LARGE: more than PLSTVO_MAX_FEATURES key lines in
+ * one image (possible with n_features 0); and every code of the images call.  The context stays usable after any error.
+ * LSD holds the whole call's images resident: about 35 bytes per scaled pixel (24 MB per 1241x376 image at scale 1.2, so about
+ * 12 GB for a 257-frame sequence of 514 images, derived from that figure and not measured) besides the ORB and LBD arenas;
+ * PLSTVO_E_CUDA when that cannot be allocated.  The call also updates what plstvo_lsd_kernel_times, plstvo_orb_detect_kernel_times
+ * and plstvo_lbd_kernel_times report. */
+int plstvo_track_stereo_images_lsd_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                         const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                         const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
+                                         PlPoseResult* results, int32_t* n_stereo /* [B][4] */);
+int plstvo_track_stereo_images_lsd_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                            const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                            const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlStereoImages* frames,
+                                            const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo /* [B+1][2] */);
+
 /* Device time of the last images call, ms: [0] image and key-line upload, [1] ORB (pyramid .. descriptors),
  * [2] LBD (gradient + descriptors), [3] stereo step (both passes, all feature sets), [4] f2fTracking + optimizePose.
- * [1] and [2] run on different streams and overlap; a stage that did not run reports 0. */
+ * [1] and [2] run on different streams and overlap; a stage that did not run reports 0.  After
+ * plstvo_track_stereo_images_lsd_*: [0] ends when LSD starts, and [2] is the lines, from LSD's first launch to LBD's last
+ * (to LSD's last where no image has a line), the host hops in between included. */
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]);
 
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */

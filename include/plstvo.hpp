@@ -1,5 +1,6 @@
 // plstvo.hpp — header-only C++17 host layer over the C-ABI (plstvo.h): RAII context plus a StereoFrameHandler with
-// the reference's method names (include/stereoFrameHandler.h:41-54) for frames of pre-extracted features.  It has no
+// the reference's method names (include/stereoFrameHandler.h:41-54) for frames of pre-extracted features, and a
+// StereoImageHandler with the same names for stereo images alone.  It has no
 // Eigen / OpenCV dependency; the Eigen/OpenCV shim that makes it a drop-in for libstvo.so is in INTEGRATION.md.
 #pragma once
 #include <algorithm>
@@ -256,6 +257,16 @@ inline void packStereoImages(const std::vector<StereoImageFrame>& frames, int wi
                             p.lr_off.data(), p.seg_l.data(), p.seg_r.data(), p.angle_l.data(), p.angle_r.data(), p.npix_l.data(),
                             p.npix_r.data()};
 }
+// the view of images alone, for the calls that detect their own key lines: a frame that carries lines is rejected
+inline void dropLines(const std::vector<StereoImageFrame>& frames, StereoImagesPack& p, const char* who) {
+    for (const StereoImageFrame& f : frames)
+        if (!f.seg_l.empty() || !f.seg_r.empty() || !f.angle_l.empty() || !f.angle_r.empty() || !f.npix_l.empty() ||
+            !f.npix_r.empty())
+            throw Error(PLSTVO_E_INVALID, std::string(who) + ": LSD runs inside the call, so frames must carry no key lines");
+    p.view.ll_off = p.view.lr_off = nullptr;
+    p.view.seg_l = p.view.seg_r = p.view.angle_l = p.view.angle_r = nullptr;
+    p.view.npix_l = p.view.npix_r = nullptr;
+}
 }  // namespace detail
 // Stereo images in, pose out (plstvo_track_stereo_images_batch): extractStereoFeatures with LSD left to the caller, then
 // f2fTracking + optimizePose, for prev.size() independent (prev[p], curr[p]) pairs of images of cam's size.  priors: one per
@@ -292,6 +303,47 @@ inline std::vector<PlPoseResult> trackStereoImageSequence(Context& c, const PlCa
     std::vector<int32_t> ns(2 * frames.size());
     c.check(plstvo_track_stereo_images_sequence(c.get(), &cam, &cfg, &mc, &sc, &oc, &a.view,
                                                 priors.empty() ? nullptr : priors.data(), res.data(), ns.data()));
+    res.resize(pairs);
+    if (n_stereo) *n_stereo = std::move(ns);
+    return res;
+}
+// Stereo images alone in, pose out (plstvo_track_stereo_images_lsd_batch): as trackStereoImages above, with LSD under lc run
+// inside the call.  Every frame's line vectors must be empty (Error(PLSTVO_E_INVALID) otherwise).
+inline std::vector<PlPoseResult> trackStereoImages(Context& c, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                                                   const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                                                   const std::vector<StereoImageFrame>& prev, const std::vector<StereoImageFrame>& curr,
+                                                   const std::vector<PlPrior>& priors = {}, std::vector<int32_t>* n_stereo = nullptr) {
+    if (prev.size() != curr.size()) throw Error(PLSTVO_E_SIZE, "trackStereoImages: prev and curr hold different numbers of frames");
+    if (!priors.empty() && priors.size() != prev.size()) throw Error(PLSTVO_E_INVALID, "trackStereoImages: one prior per pair");
+    detail::StereoImagesPack a, b;
+    detail::packStereoImages(prev, cam.width, cam.height, a);
+    detail::packStereoImages(curr, cam.width, cam.height, b);
+    detail::dropLines(prev, a, "trackStereoImages");
+    detail::dropLines(curr, b, "trackStereoImages");
+    std::vector<PlPoseResult> res(std::max<size_t>(prev.size(), 1));
+    std::vector<int32_t> ns(4 * prev.size());
+    c.check(plstvo_track_stereo_images_lsd_batch(c.get(), &cam, &cfg, &mc, &sc, &oc, &lc, &a.view, &b.view,
+                                                 priors.empty() ? nullptr : priors.data(), res.data(), ns.data()));
+    res.resize(prev.size());
+    if (n_stereo) *n_stereo = std::move(ns);
+    return res;
+}
+// The same for consecutive frames (plstvo_track_stereo_images_lsd_sequence), as trackStereoImageSequence above.
+inline std::vector<PlPoseResult> trackStereoImageSequence(Context& c, const PlCamera& cam, const PlConfig& cfg,
+                                                          const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
+                                                          const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                                                          const std::vector<StereoImageFrame>& frames,
+                                                          const std::vector<PlPrior>& priors = {},
+                                                          std::vector<int32_t>* n_stereo = nullptr) {
+    const size_t pairs = frames.empty() ? 0 : frames.size() - 1;
+    if (!priors.empty() && priors.size() != pairs) throw Error(PLSTVO_E_INVALID, "trackStereoImageSequence: one prior per pair");
+    detail::StereoImagesPack a;
+    detail::packStereoImages(frames, cam.width, cam.height, a);
+    detail::dropLines(frames, a, "trackStereoImageSequence");
+    std::vector<PlPoseResult> res(std::max<size_t>(pairs, 1));
+    std::vector<int32_t> ns(2 * frames.size());
+    c.check(plstvo_track_stereo_images_lsd_sequence(c.get(), &cam, &cfg, &mc, &sc, &oc, &lc, &a.view,
+                                                    priors.empty() ? nullptr : priors.data(), res.data(), ns.data()));
     res.resize(pairs);
     if (n_stereo) *n_stereo = std::move(ns);
     return res;
@@ -550,6 +602,26 @@ struct KeyframeTest {
     }
 };
 
+// the prior optimizePose reads from prev_frame (src/stereoFrameHandler.cpp:317-326, :377-378)
+inline PlPrior priorOf(const StereoFrame& prev_frame) {
+    PlPrior prior;
+    std::copy(prev_frame.Tfw.begin(), prev_frame.Tfw.end(), prior.Tfw);
+    std::copy(prev_frame.Tfw_cov.begin(), prev_frame.Tfw_cov.end(), prior.Tfw_cov);
+    std::copy(prev_frame.DT.begin(), prev_frame.DT.end(), prior.DT);
+    std::copy(prev_frame.DT_cov.begin(), prev_frame.DT_cov.end(), prior.DT_cov);
+    prior.err_norm = prev_frame.err_norm;
+    return prior;
+}
+// optimizePose's results published into curr_frame (src/stereoFrameHandler.cpp:372-391)
+inline void publishPose(const PlPoseResult& r, StereoFrame& curr_frame) {
+    std::copy(r.DT, r.DT + 16, curr_frame.DT.begin());
+    std::copy(r.DT_cov, r.DT_cov + 36, curr_frame.DT_cov.begin());
+    std::copy(r.DT_cov_eig, r.DT_cov_eig + 6, curr_frame.DT_cov_eig.begin());
+    std::copy(r.Tfw, r.Tfw + 16, curr_frame.Tfw.begin());
+    std::copy(r.Tfw_cov, r.Tfw_cov + 36, curr_frame.Tfw_cov.begin());
+    curr_frame.err_norm = r.err_norm;
+}
+
 // StereoFrameHandler surface: initialize / insertStereoPair / optimizePose / updateFrame (app/imagesStVO.cpp:88-124)
 class StereoFrameHandler {
 public:
@@ -571,12 +643,7 @@ public:
     void f2fTracking() {                                 // :106-129, fused with optimizePose on the device
         std::array<int32_t, 2> po1, lo1, po2, lo2;
         const PlFrameBatch prev = prev_frame.view(po1, lo1), curr = curr_frame.view(po2, lo2);
-        PlPrior prior;
-        std::copy(prev_frame.Tfw.begin(), prev_frame.Tfw.end(), prior.Tfw);
-        std::copy(prev_frame.Tfw_cov.begin(), prev_frame.Tfw_cov.end(), prior.Tfw_cov);
-        std::copy(prev_frame.DT.begin(), prev_frame.DT.end(), prior.DT);
-        std::copy(prev_frame.DT_cov.begin(), prev_frame.DT_cov.end(), prior.DT_cov);
-        prior.err_norm = prev_frame.err_norm;
+        const PlPrior prior = priorOf(prev_frame);
         matches_pt.assign(prev_frame.n_pt(), -1);
         matches_ls.assign(prev_frame.n_ls(), -1);
         inlier_pt.assign(prev_frame.n_pt(), 0);
@@ -588,12 +655,7 @@ public:
         n_inliers = n_inliers_pt + n_inliers_ls;
     }
     void optimizePose() {                                // :307-392: publish what the device computed
-        std::copy(result_.DT, result_.DT + 16, curr_frame.DT.begin());
-        std::copy(result_.DT_cov, result_.DT_cov + 36, curr_frame.DT_cov.begin());
-        std::copy(result_.DT_cov_eig, result_.DT_cov_eig + 6, curr_frame.DT_cov_eig.begin());
-        std::copy(result_.Tfw, result_.Tfw + 16, curr_frame.Tfw.begin());
-        std::copy(result_.Tfw_cov, result_.Tfw_cov + 36, curr_frame.Tfw_cov.begin());
-        curr_frame.err_norm = result_.err_norm;
+        publishPose(result_, curr_frame);
         n_inliers_pt = result_.n_inliers_pt;
         n_inliers_ls = result_.n_inliers_ls;
         n_inliers = result_.n_inliers;
@@ -622,6 +684,99 @@ private:
     PlConfig cfg_;
     HandlerConfig hcfg_;
     PlPoseResult result_{};
+    bool has_prev_ = false;
+};
+
+// The same surface over images alone, as app/imagesStVO.cpp:88-97 drives the reference's handler: initialize(img_l, img_r, idx)
+// and insertStereoPair(img_l, img_r, idx) take two grey images of cam's size (row-major, width * height bytes each), then
+// optimizePose(), updateFrame() (with updateFastThreshold), needNewKF() and currFrameIsKF() as above.  The handler keeps
+// copies of the previous frame's images and the FAST threshold they were detected with; each insertStereoPair is one
+// plstvo_track_stereo_images_lsd_batch call with one pair: the stored images at their threshold, the new ones at the current
+// orb_fast_th, and the prior f2fTracking builds from prev_frame.  The C-ABI keeps no frame between calls, so the previous
+// frame's images are detected and described again on every call: about twice the detection work of the reference's handler,
+// which keeps the previous frame's features.  prev_frame / curr_frame hold the pose state; their feature arrays stay empty.
+class StereoImageHandler {
+public:
+    StereoImageHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                       const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                       const HandlerConfig& hcfg = HandlerConfig{})
+        : ctx_(ctx), cam_(cam), cfg_(cfg), mc_(mc), sc_(sc), oc_(oc), lc_(lc), hcfg_(hcfg) {}
+
+    void initialize(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // src/stereoFrameHandler.cpp:35-52
+        orb_fast_th = hcfg_.orb_fast_th;                 // :38
+        store(img_l, img_r, prev_l_, prev_r_);
+        prev_th_ = orb_fast_th;
+        prev_frame = StereoFrame{};
+        prev_frame.frame_idx = idx;
+        for (int i = 0; i < 36; ++i) prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+        kf = KeyframeTest{};                             // :48-51
+        has_prev_ = true;
+    }
+    void insertStereoPair(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // :54-60
+        if (!has_prev_) throw Error(PLSTVO_E_INVALID, "initialize() first");
+        store(img_l, img_r, curr_l_, curr_r_);
+        curr_th_ = orb_fast_th;
+        curr_frame = StereoFrame{};
+        curr_frame.frame_idx = idx;
+        f2fTracking();
+    }
+    void f2fTracking() {                                 // :106-129, with both frames' feature extraction, fused with optimizePose
+        const PlPrior prior = priorOf(prev_frame);
+        const PlStereoImages prev{1, cam_.width, cam_.height, prev_l_.data(), prev_r_.data(), &prev_th_},
+                             curr{1, cam_.width, cam_.height, curr_l_.data(), curr_r_.data(), &curr_th_};
+        // a frame's fast_th of 0 stands for the config's threshold; with that set to 0 too, every frame is detected with the
+        // threshold the handler chose, 0 included (updateFastThreshold returns 0 when fast_min_th <= 0), as in the reference
+        PlOrbDetectConfig oc = oc_;
+        oc.fast_threshold = 0;
+        ctx_.check(plstvo_track_stereo_images_lsd_batch(ctx_.get(), &cam_, &cfg_, &mc_, &sc_, &oc, &lc_, &prev, &curr, &prior,
+                                                        &result_, n_stereo.data()));
+        n_inliers_pt = result_.n_matched_pt;             // :126-128
+        n_inliers_ls = result_.n_matched_ls;
+        n_inliers = n_inliers_pt + n_inliers_ls;
+    }
+    void optimizePose() {                                // :307-392: publish what the device computed
+        publishPose(result_, curr_frame);
+        n_inliers_pt = result_.n_inliers_pt;
+        n_inliers_ls = result_.n_inliers_ls;
+        n_inliers = result_.n_inliers;
+    }
+    void updateFrame() {                                 // :62-102
+        orb_fast_th = updateFastThreshold(hcfg_, orb_fast_th, curr_frame, n_inliers_pt);   // :66-86
+        prev_frame = std::move(curr_frame);
+        curr_frame = StereoFrame{};
+        prev_l_.swap(curr_l_);
+        prev_r_.swap(curr_r_);
+        prev_th_ = curr_th_;
+    }
+
+    bool needNewKF() { return kf.needNewKF(hcfg_, curr_frame); }
+    void currFrameIsKF() { kf.currFrameIsKF(curr_frame); }
+    const PlPoseResult& result() const { return result_; }
+
+    StereoFrame prev_frame, curr_frame;
+    std::array<int32_t, 4> n_stereo{};                   // stereo points, lines of prev, then of curr, in the last call
+    int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
+    int orb_fast_th = 20;                                // include/stereoFrameHandler.h:62
+    KeyframeTest kf;
+
+private:
+    void store(const uint8_t* img_l, const uint8_t* img_r, std::vector<uint8_t>& l, std::vector<uint8_t>& r) const {
+        if (!img_l || !img_r) throw Error(PLSTVO_E_INVALID, "StereoImageHandler: null image");
+        const size_t px = (size_t)cam_.width * (size_t)cam_.height;
+        l.assign(img_l, img_l + px);
+        r.assign(img_r, img_r + px);
+    }
+    Context& ctx_;
+    PlCamera cam_;
+    PlConfig cfg_;
+    PlStereoMatchConfig mc_;
+    PlStereoConfig sc_;
+    PlOrbDetectConfig oc_;
+    PlLsdConfig lc_;
+    HandlerConfig hcfg_;
+    PlPoseResult result_{};
+    std::vector<uint8_t> prev_l_, prev_r_, curr_l_, curr_r_;
+    int32_t prev_th_ = 0, curr_th_ = 0;
     bool has_prev_ = false;
 };
 

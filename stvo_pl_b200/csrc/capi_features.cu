@@ -339,11 +339,12 @@ struct OrbDetected {
     const uint8_t* desc = nullptr;
 };
 
-// Uploads n_img (> 0) host images (parts, in order) into arena_orb and enqueues detection and description on s_main, for a
-// checked config and per-image FAST thresholds th (clamped here).  `beside` (optional) is called with the device images and an
-// event that completes once they are uploaded, after the pyramid and FAST launches are enqueued and before the first offsets
-// readback blocks this thread: work enqueued there on another stream overlaps those stages.
-int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height,
+// Enqueues detection and description of n_img (> 0) images on s_main, for a checked config and per-image FAST thresholds th
+// (clamped here): either device images already written on s_main (d_img) or host images (parts, in order) that go up into
+// arena_orb.  `beside` (optional) is called with the device images and an event that completes once they are on the device,
+// after the pyramid and FAST launches are enqueued and before the first offsets readback blocks this thread: work enqueued
+// there on another stream overlaps those stages.
+int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height, const uint8_t* d_img,
                        const std::vector<ImgPart>& parts, const int32_t* fast_th, int capacity,
                        const std::function<int(const uint8_t*, cudaEvent_t)>& beside, OrbDetected& out) {
     PlOrbConfig oc = cfg->orb;
@@ -385,7 +386,7 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     CK(ctx, orb_init(ctx));
     const size_t img_bytes = (size_t)n_img * width * height, NL = (size_t)n_img * nl;
     Arena a;
-    const size_t o_img = a.take(img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
+    const size_t o_img = a.take(d_img ? 0 : img_bytes), o_raw = a.take((size_t)n_img * L.raw_stride + 1);
     const size_t o_blur = a.take((size_t)n_img * L.blur_stride), o_tab = a.take(tabs.size() * 4 + 4);
     const size_t o_score = a.take((size_t)n_img * L.blur_stride), o_hist = a.take(NL * 256 * 4), o_cut = a.take(NL * 4);
     const size_t o_rcnt = a.take((size_t)n_img * R * 4), o_rbase = a.take((size_t)n_img * (R + 1) * 4);
@@ -394,7 +395,8 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     const size_t o_hcnt = a.take((size_t)n_img * 4);
     CK(ctx, a.alloc(ctx->arena_orb));
     cudaStream_t s = ctx->s_main;
-    {
+    const uint8_t* img = d_img ? d_img : a.u8(o_img);
+    if (!d_img) {
         size_t o = o_img;
         for (const ImgPart& ip : parts) {
             const size_t bytes = (size_t)ip.n * width * height;
@@ -413,14 +415,14 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     cudaEvent_t* ev = ctx->orb_det_ev.ev;   // [0] start, [1] pyramid + blur, [2] FAST + NMS, [3] selection, [4] angle + descriptor
     int launches = 0;
     CK(ctx, cudaEventRecord(ev[0], s));
-    launch_orb_pyramid(L, n_img, a.u8(o_img), a.u8(o_raw), a.u8(o_blur), rs_tab.data(), s, &launches);
+    launch_orb_pyramid(L, n_img, img, a.u8(o_raw), a.u8(o_blur), rs_tab.data(), s, &launches);
     CK(ctx, cudaEventRecord(ev[1], s));
-    launch_orb_fast_select(L, D, n_img, a.u8(o_img), a.u8(o_raw), a.i32(o_th), a.u8(o_score),
+    launch_orb_fast_select(L, D, n_img, img, a.u8(o_raw), a.i32(o_th), a.u8(o_score),
                            a.at<uint32_t>(o_hist), a.i32(o_cut), a.i32(o_rcnt), a.i32(o_rbase), a.i32(o_icnt), a.i32(o_soff), s,
                            ev[2], &launches);
     CK(ctx, cudaGetLastError());
     if (beside)
-        if (const int rc = beside(a.u8(o_img), uploaded)) return rc;
+        if (const int rc = beside(img, uploaded)) return rc;
     std::vector<int32_t>& off = out.off;
     off.assign((size_t)n_img + 1, 0);
     CK(ctx, cudaMemcpyAsync(off.data(), a.i32(o_soff), off.size() * 4, cudaMemcpyDeviceToHost, s));
@@ -457,7 +459,7 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     const float *d_xy = b.f32(o_xy), *d_resp = b.f32(o_resp);
     if (harris) {
         uint32_t* ckey = a.at<uint32_t>(o_ckey);
-        launch_orb_harris_select(L, D, n_img, (int)N1, a.u8(o_img), a.u8(o_raw), a.i32(o_rbase), a.i32(o_soff),
+        launch_orb_harris_select(L, D, n_img, (int)N1, img, a.u8(o_raw), a.i32(o_rbase), a.i32(o_soff),
                                  b.at<int2>(o_lxy), b.i32(o_oct), b.f32(o_hresp), ckey, a.i32(o_lkeep), a.i32(o_hoff),
                                  a.i32(o_hcnt), s, &launches);
         CK(ctx, cudaGetLastError());
@@ -473,7 +475,7 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     }
     CK(ctx, cudaEventRecord(ev[3], s));
     const size_t N = (size_t)off[n_img];
-    launch_orb_describe(L, n_img, a.u8(o_img), a.u8(o_raw), a.u8(o_blur), d_off, (int)N, d_xy, d_oct, nullptr, d_rank, d_cnt,
+    launch_orb_describe(L, n_img, img, a.u8(o_raw), a.u8(o_blur), d_off, (int)N, d_xy, d_oct, nullptr, d_rank, d_cnt,
                         b.f32(o_ang), b.u8(o_desc), s, &launches);
     CK(ctx, cudaEventRecord(ev[4], s));
     CK(ctx, cudaGetLastError());
@@ -498,7 +500,7 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
     std::vector<int32_t> th((size_t)n_img, cfg->fast_threshold);
     if (fast_th) std::copy(fast_th, fast_th + n_img, th.begin());
     OrbDetected o;
-    const int rc = orb_detect_enqueue(ctx, cfg, n_img, width, height, {ImgPart{images, n_img}}, th.data(), capacity, nullptr, o);
+    const int rc = orb_detect_enqueue(ctx, cfg, n_img, width, height, nullptr, {ImgPart{images, n_img}}, th.data(), capacity, nullptr, o);
     if (rc == PLSTVO_E_TOO_LARGE && o.off.size() == (size_t)n_img + 1) memcpy(kp_off, o.off.data(), o.off.size() * 4);
     if (rc) return rc;
     const size_t N = (size_t)o.off[n_img];
@@ -516,157 +518,6 @@ int plstvo_orb_detect_and_compute_batch(PlContext* ctx, const PlOrbDetectConfig*
     return (int)N;
 }
 
-/* ---- stereo images -> pose: ORB and LBD feed the stereo step and the tracker without leaving HBM ---- */
-// The images go up once into arena_orb in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left]
-// [curr right].  Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.
-static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
-                            const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
-                            const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
-                            bool sequence) {
-    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
-        return fail(ctx, PLSTVO_E_INVALID, "null argument");
-    const int NF = prev->B;
-    if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
-    if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
-    if (const int rc = orb_detect_check(ctx, oc)) return rc;
-    const int nfs = sequence ? 1 : 2;   // frame sets: the sequence, or prev and curr
-    const PlStereoImages* fs[2] = {prev, curr};
-    const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0;
-    const int W = cam->width, H = cam->height;
-    std::vector<LineSrc> lsrc;   // key lines per image block
-    if (NF > 0) {
-        for (int j = 0; j < nfs; ++j) {
-            // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
-            if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
-            if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
-        }
-        if (lns) {
-            if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
-            for (int j = 0; j < nfs; ++j) {
-                lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
-                lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
-            }
-            for (const LineSrc& l : lsrc)
-                if (const int rc = lbd_check_lines(ctx, l)) return rc;
-        }
-    }
-    if (NF == 0 || (sequence && NF == 1)) return 0;
-    CK(ctx, cudaSetDevice(ctx->device));
-    CK(ctx, ctx->img_ev.create());
-    CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
-    ctx->img_timed = false;
-    const int nblk = 2 * nfs, n_img = nblk * NF;
-    std::vector<ImgPart> iparts;
-    std::vector<int32_t> th((size_t)n_img), lbase((size_t)nblk + 1, 0);
-    for (int b = 0; b < nblk; ++b) {
-        const PlStereoImages* f = fs[b / 2];
-        iparts.push_back(ImgPart{b % 2 ? f->img_r : f->img_l, NF});
-        for (int i = 0; i < NF; ++i)   // 0 = the configured threshold, as detectPointFeatures / plstvo::detectAndComputeORB
-            th[(size_t)b * NF + i] = f->fast_th && f->fast_th[i] ? f->fast_th[i] : oc->fast_threshold;
-        lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
-    }
-    const bool run_lbd = lbase[nblk] > 0;
-    const float* d_seg = nullptr;
-    const uint8_t* d_ldesc = nullptr;
-    // LBD on the second stream; with ORB running it reads ORB's copy of the images once their upload has completed
-    auto enqueue_lbd = [&](const uint8_t* d_img, cudaEvent_t ready) -> int {
-        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, iparts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
-        CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
-        return 0;
-    };
-    CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
-    OrbDetected orb;
-    if (pts) {
-        std::function<int(const uint8_t*, cudaEvent_t)> beside;
-        if (run_lbd) beside = enqueue_lbd;
-        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, iparts, th.data(), INT_MAX, beside, orb)) return rc;
-    } else {
-        orb.off.assign((size_t)n_img + 1, 0);
-        if (run_lbd)
-            if (const int rc = enqueue_lbd(nullptr, nullptr)) return rc;
-    }
-    // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
-    std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
-    PlStereoFeatures feat[2]{};
-    StereoDevInputs dev;
-    for (int j = 0; j < nfs; ++j) {
-        const int bl = 2 * j, br = 2 * j + 1;
-        const size_t kl = orb.off[(size_t)bl * NF], kr = orb.off[(size_t)br * NF];
-        pl_off[j].resize((size_t)NF + 1);
-        pr_off[j].resize((size_t)NF + 1);
-        for (int i = 0; i <= NF; ++i) {
-            pl_off[j][i] = orb.off[(size_t)bl * NF + i] - (int32_t)kl;
-            pr_off[j][i] = orb.off[(size_t)br * NF + i] - (int32_t)kr;
-        }
-        PlStereoFeatures& F = feat[j];
-        F.B = NF;
-        F.pl_off = pl_off[j].data(); F.pr_off = pr_off[j].data();
-        F.ll_off = lns ? fs[j]->ll_off : none.data(); F.lr_off = lns ? fs[j]->lr_off : none.data();
-        F.angle_l = lns ? fs[j]->angle_l : nullptr;
-        StereoDevInputs::Set& P = dev.set[2 * j];
-        P.on_device = true;
-        if (pts) {
-            P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
-            P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
-        }
-        StereoDevInputs::Set& Ls = dev.set[2 * j + 1];
-        Ls.on_device = true;   // oct stays null: key lines of octave 0
-        if (run_lbd) {
-            Ls.xy_l = d_seg + 4 * (size_t)lbase[bl]; Ls.xy_r = d_seg + 4 * (size_t)lbase[br];
-            Ls.d1 = d_ldesc + 32 * (size_t)lbase[bl]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[br];
-        }
-    }
-    dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
-    dev.marks = ctx->img_ev.ev + 1;
-    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], sequence ? nullptr : &feat[1], priors, results,
-                                           n_stereo, sequence, -1, &dev))
-        return rc;
-    float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
-    std::fill(ms, ms + 5, 0.f);
-    // uploads end where the first stage starts: LBD waits for the images and its key lines, ORB for the images only
-    const cudaEvent_t up_end = run_lbd ? ctx->lbd_ev[0] : pts ? ctx->orb_det_ev[0] : nullptr;
-    if (up_end) CK(ctx, cudaEventElapsedTime(&ms[0], ctx->img_ev[0], up_end));
-    if (pts) CK(ctx, cudaEventElapsedTime(&ms[1], ctx->orb_det_ev[0], ctx->orb_det_ev[4]));
-    if (run_lbd) CK(ctx, cudaEventElapsedTime(&ms[2], ctx->lbd_ev[0], ctx->lbd_ev[2]));
-    CK(ctx, cudaEventElapsedTime(&ms[3], ctx->img_ev[1], ctx->img_ev[2]));
-    CK(ctx, cudaEventElapsedTime(&ms[4], ctx->img_ev[2], ctx->img_ev[3]));
-    ctx->img_timed = true;
-    return 0;
-}
-
-static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
-                               const PlStereoConfig* sc, const PlOrbDetectConfig* oc, const PlStereoImages* prev,
-                               const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo,
-                               bool sequence) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, prev, curr, priors, results, n_stereo, sequence);
-    // LBD may still run on the second stream after an error: the next call may reuse its arena
-    const cudaError_t e = cudaStreamSynchronize(ctx->s_alt);
-    if (rc) return rc;
-    CK(ctx, e);
-    return 0;
-}
-
-int plstvo_track_stereo_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
-                                     const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* prev,
-                                     const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
-    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, prev, curr, priors, results, n_stereo, false);
-}
-
-int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
-                                        const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
-                                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
-    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, frames, nullptr, priors, results, n_stereo, true);
-}
-
-int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {
-    if (!ctx || !ms5) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!ctx->img_timed) return fail(ctx, PLSTVO_E_INVALID, "no images call on this context yet");
-    memcpy(ms5, ctx->img_ms, sizeof(ctx->img_ms));
-    return 0;
-}
 
 int plstvo_orb_detect_kernel_times(PlContext* ctx, float* ms4) {
     if (!ctx || !ms4) return PLSTVO_E_INVALID;
@@ -811,20 +662,12 @@ int lsd_check_config(PlContext* ctx, const PlLsdConfig* c) {
     if (fabs(1.0 / c->scale - 2.0) < DBL_EPSILON) return fail(ctx, PLSTVO_E_INVALID, "lsd scale 0.5 is not supported");
     return 0;
 }
-}  // namespace
-
-int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, int width, int height, const uint8_t* images,
-                            int capacity, int32_t* kl_off, float* kl_seg, float* kl_angle, int32_t* kl_npix,
-                            float* kl_response, float* kl_length) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!cfg || n_img < 0 || capacity < 0) return fail(ctx, PLSTVO_E_INVALID, "null config, negative n_img or negative capacity");
-    if (n_img > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");   // gridDim.z of the pixel kernels
-    if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
-    if (const int rc = lsd_check_config(ctx, cfg)) return rc;
-    if (!kl_off) return fail(ctx, PLSTVO_E_INVALID, "null kl_off");
-    // flsd: blur with sigma_scale (/ scale when shrinking), half-width ceil(sigma * sqrt(2 * 3 * ln 10)), then resize
-    LsdLaunch L{};
+// flsd's launch parameters for n_img images of width x height under a checked config: the blur taps and the scaled size
+// (blur with sigma_scale, / scale when shrinking, half-width ceil(sigma * sqrt(2 * 3 * ln 10)), then resize), the gradient
+// threshold, the smallest kept region and the region records per image.  PLSTVO_E_INVALID: a blur wider than 31 taps or a
+// scaled size outside 1..32767.
+int lsd_plan(PlContext* ctx, const PlLsdConfig* cfg, int n_img, int width, int height, LsdLaunch& L) {
+    L = LsdLaunch{};
     L.n_img = n_img; L.W = width; L.H = height; L.scale = cfg->scale; L.n_bins = cfg->n_bins;
     L.w = width; L.h = height;
     if (cfg->scale != 1) {
@@ -855,46 +698,69 @@ int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, i
         L.w = (int)ws;
         L.h = (int)hs;
     }
-    kl_off[0] = 0;
-    if (n_img == 0) return 0;
-    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
     const double prec = kLsdPi * cfg->ang_th / 180, p = cfg->ang_th / 180;
     L.prec = prec;
     L.rho = cfg->quant / sin(prec);
     const double log_nt = 5 * (log10((double)L.w) + log10((double)L.h)) / 2 + log10(11.0);
     const double min_reg = -log_nt / log10(p);
     L.min_reg = min_reg >= (double)INT_MAX ? INT_MAX : (int)(size_t)min_reg;
-    const size_t N = (size_t)L.w * L.h;
-    L.reg_cap = (int)(N / (size_t)std::max(L.min_reg, 1) + 1);
+    L.reg_cap = (int)((size_t)L.w * L.h / (size_t)std::max(L.min_reg, 1) + 1);
+    return 0;
+}
+
+// Enqueues LSD's device half (blur and resize, gradient, seed order, region growing) on stream s for L.n_img (> 0) images of
+// one size planned by lsd_plan: either device images (d_img, ready once img_ready has completed) or host images that go into
+// arena_lsd (img_parts).  Sets L's device pointers; lsd_finish continues on the same stream.
+int lsd_enqueue(PlContext* ctx, LsdLaunch& L, const uint8_t* d_img, cudaEvent_t img_ready, const std::vector<ImgPart>& img_parts,
+                cudaStream_t s) {
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, lsd_init(ctx));
-    cudaStream_t s = ctx->s_main;
-    const size_t in_bytes = (size_t)n_img * width * height;
+    const int n_img = L.n_img;
+    const bool scaled = L.scale != 1;
+    const size_t in_bytes = (size_t)n_img * L.W * L.H, N = (size_t)L.w * L.h;
     Arena a;
-    const size_t o_img = a.take(in_bytes), o_blur = a.take(cfg->scale != 1 ? in_bytes : 0),
-                 o_scaled = a.take(cfg->scale != 1 ? (size_t)n_img * N : 0), o_scr = a.take(lsd_scratch_bytes(n_img, L.w, L.h)),
+    const size_t o_img = a.take(d_img ? 0 : in_bytes), o_blur = a.take(scaled ? in_bytes : 0),
+                 o_scaled = a.take(scaled ? (size_t)n_img * N : 0), o_scr = a.take(lsd_scratch_bytes(n_img, L.w, L.h)),
                  o_max = a.take((size_t)n_img * 8), o_hist = a.take((size_t)n_img * L.n_bins * 4), o_ns = a.take((size_t)n_img * 4),
                  o_reg = a.take((size_t)n_img * L.reg_cap * sizeof(LsdRegion)), o_nreg = a.take((size_t)n_img * 4);
     CK(ctx, a.alloc(ctx->arena_lsd));
-    L.images = a.u8(o_img); L.blurred = a.u8(o_blur); L.scaled = a.u8(o_scaled); L.scratch = a.u8(o_scr);
+    L.images = d_img ? d_img : a.u8(o_img); L.blurred = a.u8(o_blur); L.scaled = a.u8(o_scaled); L.scratch = a.u8(o_scr);
     L.max_bits = a.at<unsigned long long>(o_max); L.hist = a.i32(o_hist); L.n_seeds = a.i32(o_ns);
     L.trig = ctx->lsd_trig.as<const float4>(); L.regions = a.at<LsdRegion>(o_reg); L.n_regions = a.i32(o_nreg);
-    CK(ctx, a.up(o_img, images, in_bytes, s));
+    if (!d_img) {
+        size_t o = o_img;
+        for (const ImgPart& ip : img_parts) {
+            const size_t bytes = (size_t)ip.n * L.W * L.H;
+            CK(ctx, a.up(o, ip.p, bytes, s));
+            o += bytes;
+        }
+    } else if (img_ready) {
+        CK(ctx, cudaStreamWaitEvent(s, img_ready, 0));
+    }
     int launches = 0;
-    cudaEvent_t* ev = ctx->lsd_ev.ev;
-    CK(ctx, launch_lsd_grow(L, s, ev, &launches));
-    ctx->lsd_ran = true;
+    ctx->lsd_ran = false;   // until lsd_finish has recorded the rest of this call's events
+    CK(ctx, launch_lsd_grow(L, s, ctx->lsd_ev.ev, &launches));
+    ctx->launches += launches;
+    return 0;
+}
+
+// The host continuation of lsd_enqueue, on the same stream: the region counts and records come down, the C library's cos /
+// sin of the region angles go up (region2rect's dx, dy, as in the reference), the rectangles' raw segments come down, then
+// the KeyLine step and the truncation run per image.  kls[i]: image i's key lines in the reference's order.  Returns with s
+// synchronised.
+int lsd_finish(PlContext* ctx, const PlLsdConfig* cfg, const LsdLaunch& L, cudaStream_t s, std::vector<std::vector<KeyLine>>& kls) {
+    const int n_img = L.n_img;
     std::vector<int32_t> nreg((size_t)n_img), r_off((size_t)n_img + 1, 0);
-    CK(ctx, a.down(nreg.data(), o_nreg, (size_t)n_img * 4, s));
+    CK(ctx, cudaMemcpyAsync(nreg.data(), L.n_regions, (size_t)n_img * 4, cudaMemcpyDeviceToHost, s));
     CK(ctx, cudaStreamSynchronize(s));
     for (int i = 0; i < n_img; ++i) r_off[(size_t)i + 1] = r_off[(size_t)i] + nreg[(size_t)i];
     const size_t R = (size_t)r_off[(size_t)n_img];
     std::vector<LsdRegion> regs(R);
     for (int i = 0; i < n_img; ++i)
-        CK(ctx, a.down(regs.data() + r_off[(size_t)i], o_reg + (size_t)i * L.reg_cap * sizeof(LsdRegion),
-                       (size_t)nreg[(size_t)i] * sizeof(LsdRegion), s));
+        if (nreg[(size_t)i])
+            CK(ctx, cudaMemcpyAsync(regs.data() + r_off[(size_t)i], L.regions + (size_t)i * L.reg_cap,
+                                    (size_t)nreg[(size_t)i] * sizeof(LsdRegion), cudaMemcpyDeviceToHost, s));
     CK(ctx, cudaStreamSynchronize(s));
-    // region2rect's dx, dy: the C library's cos / sin of the angle, as in the reference
     std::vector<double2> dir(R);
     for (size_t r = 0; r < R; ++r) dir[r] = make_double2(cos(regs[r].theta), sin(regs[r].theta));
     Arena b;
@@ -902,35 +768,67 @@ int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, i
     CK(ctx, b.alloc(ctx->arena_lsd_seg));
     CK(ctx, b.up(o_roff, r_off.data(), ((size_t)n_img + 1) * 4, s));
     CK(ctx, b.up(o_dir, dir.data(), R * 16, s));
+    cudaEvent_t* ev = ctx->lsd_ev.ev;
+    int launches = 0;
     CK(ctx, cudaEventRecord(ev[4], s));
     CK(ctx, launch_lsd_extent(L, (int)R, b.i32(o_roff), b.at<double2>(o_dir), b.at<float4>(o_seg), s, &launches));
     CK(ctx, cudaEventRecord(ev[5], s));
+    ctx->lsd_ran = true;
     ctx->launches += launches;
     std::vector<float4> raw(R);
     CK(ctx, b.down(raw.data(), o_seg, R * 16, s));
     CK(ctx, cudaStreamSynchronize(s));
-    // the KeyLine step and the truncation per image; kl_off in full before any capacity check
-    const double min_length = cfg->min_line_length * std::min(width, height);
-    std::vector<std::vector<KeyLine>> kls((size_t)n_img);
+    const double min_length = cfg->min_line_length * std::min(L.W, L.H);
+    kls.assign((size_t)n_img, {});
+    for (int i = 0; i < n_img; ++i)
+        lsd_keylines(L.W, L.H, raw.data() + r_off[(size_t)i], nreg[(size_t)i], min_length, cfg->n_features, kls[(size_t)i]);
+    return 0;
+}
+
+// the key lines of images i0 .. i0 + n - 1 as rows from row 0 of each array (a null array is skipped)
+void lsd_rows(const std::vector<std::vector<KeyLine>>& kls, int i0, int n, float* seg, float* angle, int32_t* npix,
+              float* response, float* length) {
+    size_t r = 0;
+    for (int i = i0; i < i0 + n; ++i)
+        for (const KeyLine& kl : kls[(size_t)i]) {
+            if (seg) memcpy(seg + 4 * r, kl.seg, sizeof kl.seg);
+            if (angle) angle[r] = kl.angle;
+            if (npix) npix[r] = kl.npix;
+            if (response) response[r] = kl.response;
+            if (length) length[r] = kl.length;
+            ++r;
+        }
+}
+}  // namespace
+
+int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, int width, int height, const uint8_t* images,
+                            int capacity, int32_t* kl_off, float* kl_seg, float* kl_angle, int32_t* kl_npix,
+                            float* kl_response, float* kl_length) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cfg || n_img < 0 || capacity < 0) return fail(ctx, PLSTVO_E_INVALID, "null config, negative n_img or negative capacity");
+    if (n_img > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");   // gridDim.z of the pixel kernels
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+    if (const int rc = lsd_check_config(ctx, cfg)) return rc;
+    if (!kl_off) return fail(ctx, PLSTVO_E_INVALID, "null kl_off");
+    LsdLaunch L;
+    if (const int rc = lsd_plan(ctx, cfg, n_img, width, height, L)) return rc;
+    kl_off[0] = 0;
+    if (n_img == 0) return 0;
+    if (!images) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    if (const int rc = lsd_enqueue(ctx, L, nullptr, nullptr, {ImgPart{images, n_img}}, ctx->s_main)) return rc;
+    std::vector<std::vector<KeyLine>> kls;
+    if (const int rc = lsd_finish(ctx, cfg, L, ctx->s_main, kls)) return rc;
+    // kl_off in full before any capacity check
     bool too_many = false;
     for (int i = 0; i < n_img; ++i) {
-        lsd_keylines(width, height, raw.data() + r_off[(size_t)i], nreg[(size_t)i], min_length, cfg->n_features, kls[(size_t)i]);
         const long next = (long)kl_off[i] + (long)kls[(size_t)i].size();
         too_many |= kls[(size_t)i].size() > (size_t)PLSTVO_MAX_FEATURES || next > INT_MAX;
         kl_off[i + 1] = (int32_t)std::min(next, (long)INT_MAX);
     }
     if (too_many) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
     if (kl_off[n_img] > capacity) return fail(ctx, PLSTVO_E_TOO_LARGE, "more key lines than capacity");
-    for (int i = 0; i < n_img; ++i)
-        for (size_t k = 0; k < kls[(size_t)i].size(); ++k) {
-            const KeyLine& kl = kls[(size_t)i][k];
-            const size_t r = (size_t)kl_off[i] + k;
-            if (kl_seg) memcpy(kl_seg + 4 * r, kl.seg, sizeof kl.seg);
-            if (kl_angle) kl_angle[r] = kl.angle;
-            if (kl_npix) kl_npix[r] = kl.npix;
-            if (kl_response) kl_response[r] = kl.response;
-            if (kl_length) kl_length[r] = kl.length;
-        }
+    lsd_rows(kls, 0, n_img, kl_seg, kl_angle, kl_npix, kl_response, kl_length);
     return kl_off[n_img];
 }
 
@@ -940,6 +838,250 @@ int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
     if (!ctx->lsd_ran) return fail(ctx, PLSTVO_E_INVALID, "no LSD call on this context yet");
     CK(ctx, cudaSetDevice(ctx->device));
     for (int k = 0; k < 5; ++k) CK(ctx, cudaEventElapsedTime(&ms5[k], ctx->lsd_ev[k], ctx->lsd_ev[k + 1]));
+    return 0;
+}
+
+/* ---- stereo images -> pose: ORB, LSD and LBD feed the stereo step and the tracker without leaving HBM ---- */
+// The images go up once, in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left][curr right].
+// Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.  The key lines are
+// the caller's, or (detect_lines) LSD's, detected on the same device copy of the images: ORB's, or LSD's own when ORB does
+// not run.
+static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                            const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
+                            const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results,
+                            int32_t* n_stereo, bool sequence) {
+    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
+        return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    const int NF = prev->B;
+    if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
+    if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (const int rc = orb_detect_check(ctx, oc)) return rc;
+    const int nfs = sequence ? 1 : 2;   // frame sets: the sequence, or prev and curr
+    const PlStereoImages* fs[2] = {prev, curr};
+    const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0, run_lsd = detect_lines && lns;
+    const int W = cam->width, H = cam->height;
+    if (detect_lines) {
+        for (int j = 0; j < nfs; ++j) {
+            const PlStereoImages* f = fs[j];
+            if (f->ll_off || f->lr_off || f->seg_l || f->seg_r || f->angle_l || f->angle_r || f->npix_l || f->npix_r)
+                return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the call detects its own key lines");
+        }
+        if (run_lsd) {
+            if (!lc) return fail(ctx, PLSTVO_E_INVALID, "null lsd config");
+            if (const int rc = lsd_check_config(ctx, lc)) return rc;
+            if (2L * nfs * NF > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
+        }
+    }
+    const int nblk = 2 * nfs, n_img = nblk * NF;
+    std::vector<LineSrc> lsrc;   // key lines per image block
+    LsdLaunch lsd{};
+    if (NF > 0) {
+        for (int j = 0; j < nfs; ++j) {
+            // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
+            if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
+            if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
+        }
+        if (lns) {
+            if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+            if (run_lsd) {
+                if (const int rc = lsd_plan(ctx, lc, n_img, W, H, lsd)) return rc;
+            } else {
+                for (int j = 0; j < nfs; ++j) {
+                    lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
+                    lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
+                }
+                for (const LineSrc& l : lsrc)
+                    if (const int rc = lbd_check_lines(ctx, l)) return rc;
+            }
+        }
+    }
+    if (NF == 0 || (sequence && NF == 1)) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, ctx->img_ev.create());
+    CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
+    ctx->img_timed = false;
+    std::vector<ImgPart> iparts;
+    std::vector<int32_t> th((size_t)n_img), lbase((size_t)nblk + 1, 0);
+    for (int b = 0; b < nblk; ++b) {
+        const PlStereoImages* f = fs[b / 2];
+        iparts.push_back(ImgPart{b % 2 ? f->img_r : f->img_l, NF});
+        for (int i = 0; i < NF; ++i)   // 0 = the configured threshold, as detectPointFeatures / plstvo::detectAndComputeORB
+            th[(size_t)b * NF + i] = f->fast_th && f->fast_th[i] ? f->fast_th[i] : oc->fast_threshold;
+    }
+    bool run_lbd = false;
+    auto count_lines = [&]() {
+        for (int b = 0; b < nblk; ++b) lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
+        run_lbd = lbase[nblk] > 0;
+    };
+    if (!run_lsd) count_lines();
+    const float* d_seg = nullptr;
+    const uint8_t* d_ldesc = nullptr;
+    const uint8_t* d_images = nullptr;   // the device copy of the images the line stages read (null: LBD uploads its own)
+    cudaEvent_t images_ready = nullptr;
+    auto enqueue_lbd = [&]() -> int {
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_images, images_ready, iparts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+        CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
+        return 0;
+    };
+    // LSD's key lines per image block, what lsrc points at: LSD's host continuation on stream s (where its device half ran),
+    // then the key-line checks of the images call
+    std::vector<int32_t> det_off[4], det_npix[4];
+    std::vector<float> det_seg[4], det_angle[4];
+    auto lsd_lines = [&](cudaStream_t s) -> int {
+        std::vector<std::vector<KeyLine>> kls;
+        if (const int rc = lsd_finish(ctx, lc, lsd, s, kls)) return rc;
+        for (const std::vector<KeyLine>& k : kls)
+            if (k.size() > (size_t)PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+        for (int b = 0; b < nblk; ++b) {
+            det_off[b].assign(1, 0);
+            for (int i = 0; i < NF; ++i) det_off[b].push_back(det_off[b].back() + (int32_t)kls[(size_t)b * NF + i].size());
+            const size_t m = (size_t)det_off[b].back();
+            det_seg[b].resize(4 * m);
+            det_angle[b].resize(m);
+            det_npix[b].resize(m);
+            lsd_rows(kls, b * NF, NF, det_seg[b].data(), det_angle[b].data(), det_npix[b].data(), nullptr, nullptr);
+            lsrc.push_back(LineSrc{NF, det_off[b].data(), det_seg[b].data(), det_angle[b].data(), det_npix[b].data()});
+        }
+        for (const LineSrc& l : lsrc)
+            if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        count_lines();
+        return 0;
+    };
+    // With fewer images than SMs, LSD's one-warp and one-thread-per-image stages (seed order, region growing) are the whole
+    // critical path and lose more beside ORB than ORB takes (BASELINE.md), so LSD runs first on the main stream, alone, and ORB
+    // reads its device copy of the images; LBD then runs beside ORB as for the caller's key lines.  With more, ORB runs beside
+    // LSD on the second stream.
+    const bool lsd_first = run_lsd && pts && n_img < ctx->sm_count;
+    CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
+    const uint8_t* orb_images = nullptr;   // the device images ORB reads (null: ORB uploads them)
+    if (lsd_first) {
+        if (const int rc = lsd_enqueue(ctx, lsd, nullptr, nullptr, iparts, ctx->s_main)) return rc;
+        if (const int rc = lsd_lines(ctx->s_main)) return rc;
+        orb_images = lsd.images;
+    }
+    const bool lsd_beside = run_lsd && !lsd_first;
+    // the line stage that runs on the second stream beside ORB: LSD's device half, or LBD on the caller's or LSD's key lines.
+    // With ORB running it reads ORB's device images once they are there
+    auto lines_beside = [&](const uint8_t* d_img, cudaEvent_t ready) -> int {
+        d_images = d_img;
+        images_ready = ready;
+        return lsd_beside ? lsd_enqueue(ctx, lsd, d_img, ready, iparts, ctx->s_alt) : enqueue_lbd();
+    };
+    OrbDetected orb;
+    if (pts) {
+        std::function<int(const uint8_t*, cudaEvent_t)> beside;
+        if (lsd_beside || run_lbd) beside = lines_beside;
+        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, orb_images, iparts, th.data(), INT_MAX, beside, orb)) return rc;
+    } else {
+        orb.off.assign((size_t)n_img + 1, 0);
+        if (lsd_beside || run_lbd)
+            if (const int rc = lines_beside(nullptr, nullptr)) return rc;
+    }
+    if (lsd_beside) {   // LSD's host continuation (while ORB's selection and descriptors run), then LBD on the same stream
+        if (const int rc = lsd_lines(ctx->s_alt)) return rc;
+        d_images = lsd.images;   // ORB's copy, or LSD's own when ORB does not run
+        if (run_lbd)
+            if (const int rc = enqueue_lbd()) return rc;
+    }
+    // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
+    std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
+    PlStereoFeatures feat[2]{};
+    StereoDevInputs dev;
+    for (int j = 0; j < nfs; ++j) {
+        const int bl = 2 * j, br = 2 * j + 1;
+        const size_t kl = orb.off[(size_t)bl * NF], kr = orb.off[(size_t)br * NF];
+        pl_off[j].resize((size_t)NF + 1);
+        pr_off[j].resize((size_t)NF + 1);
+        for (int i = 0; i <= NF; ++i) {
+            pl_off[j][i] = orb.off[(size_t)bl * NF + i] - (int32_t)kl;
+            pr_off[j][i] = orb.off[(size_t)br * NF + i] - (int32_t)kr;
+        }
+        PlStereoFeatures& F = feat[j];
+        F.B = NF;
+        F.pl_off = pl_off[j].data(); F.pr_off = pr_off[j].data();
+        F.ll_off = lns ? lsrc[bl].off : none.data(); F.lr_off = lns ? lsrc[br].off : none.data();
+        F.angle_l = lns ? lsrc[bl].angle : nullptr;
+        StereoDevInputs::Set& P = dev.set[2 * j];
+        P.on_device = true;
+        if (pts) {
+            P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
+            P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
+        }
+        StereoDevInputs::Set& Ls = dev.set[2 * j + 1];
+        Ls.on_device = true;   // oct stays null: key lines of octave 0
+        if (run_lbd) {
+            Ls.xy_l = d_seg + 4 * (size_t)lbase[bl]; Ls.xy_r = d_seg + 4 * (size_t)lbase[br];
+            Ls.d1 = d_ldesc + 32 * (size_t)lbase[bl]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[br];
+        }
+    }
+    dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
+    dev.marks = ctx->img_ev.ev + 1;
+    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], sequence ? nullptr : &feat[1], priors, results,
+                                           n_stereo, sequence, -1, &dev))
+        return rc;
+    float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
+    std::fill(ms, ms + 5, 0.f);
+    // uploads end where the first stage starts: LSD waits for the images, LBD on the caller's lines for the images and its key
+    // lines, ORB for the images only
+    const cudaEvent_t up_end = run_lsd ? ctx->lsd_ev[0] : run_lbd ? ctx->lbd_ev[0] : pts ? ctx->orb_det_ev[0] : nullptr;
+    if (up_end) CK(ctx, cudaEventElapsedTime(&ms[0], ctx->img_ev[0], up_end));
+    if (pts) CK(ctx, cudaEventElapsedTime(&ms[1], ctx->orb_det_ev[0], ctx->orb_det_ev[4]));
+    // the lines: LSD's first launch (host hops included) to LBD's last, or LBD alone on the caller's lines
+    if (run_lsd || run_lbd)
+        CK(ctx, cudaEventElapsedTime(&ms[2], run_lsd ? ctx->lsd_ev[0] : ctx->lbd_ev[0], run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5]));
+    CK(ctx, cudaEventElapsedTime(&ms[3], ctx->img_ev[1], ctx->img_ev[2]));
+    CK(ctx, cudaEventElapsedTime(&ms[4], ctx->img_ev[2], ctx->img_ev[3]));
+    ctx->img_timed = true;
+    return 0;
+}
+
+static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
+                               const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
+                               const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
+                               PlPoseResult* results, int32_t* n_stereo, bool sequence) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, prev, curr, priors, results, n_stereo, sequence);
+    // after an error the line stages may still run on the second stream, and ORB on the first: the next call may reuse their
+    // arenas
+    const cudaError_t e = cudaStreamSynchronize(ctx->s_alt), e_main = cudaStreamSynchronize(ctx->s_main);
+    if (rc) return rc;
+    CK(ctx, e);
+    CK(ctx, e_main);
+    return 0;
+}
+
+int plstvo_track_stereo_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                     const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* prev,
+                                     const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, false, nullptr, prev, curr, priors, results, n_stereo, false);
+}
+
+int plstvo_track_stereo_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                        const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlStereoImages* frames,
+                                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, false, nullptr, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_images_lsd_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                         const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                         const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
+                                         PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, prev, curr, priors, results, n_stereo, false);
+}
+
+int plstvo_track_stereo_images_lsd_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                            const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                            const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlStereoImages* frames,
+                                            const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {
+    if (!ctx || !ms5) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->img_timed) return fail(ctx, PLSTVO_E_INVALID, "no images call on this context yet");
+    memcpy(ms5, ctx->img_ms, sizeof(ctx->img_ms));
     return 0;
 }
 

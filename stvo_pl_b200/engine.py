@@ -107,6 +107,13 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_track_stereo_images_sequence": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
                                                           C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
                                                           C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_track_stereo_images_lsd_batch": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                           C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                           C.POINTER(T.PlLsdConfig), C.POINTER(T.PlStereoImages),
+                                                           C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_track_stereo_images_lsd_sequence": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                              C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                              C.POINTER(T.PlLsdConfig), C.POINTER(T.PlStereoImages), vp, vp, i32p]),
         "plstvo_track_stereo_images_stage_times": (C.c_int, [vp, fp]),
     }
     for name, (res, args) in sig.items():
@@ -130,7 +137,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
     "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
     "plstvo_lsd_kernel_times", "plstvo_track_stereo_images_batch",
-    "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_stage_times"]
+    "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_lsd_batch", "plstvo_track_stereo_images_lsd_sequence",
+    "plstvo_track_stereo_images_stage_times"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -612,8 +620,41 @@ class Engine:
         del keep
         return results, n_stereo
 
+    def track_stereo_images_lsd_batch(self, cam, cfg, mcfg, scfg, ocfg, lcfg, prev: dict, curr: dict, priors=None, results=None):
+        """Stereo images alone of B (prev, curr) frame pairs -> poses: LSD detection inside the call, then what
+        track_stereo_images_batch does.  prev / curr: dicts with img_l / img_r uint8[B, H, W] and optionally fast_th [B], no
+        key-line arrays.  lcfg may be None where cfg.has_lines is 0.  Returns (results, n_stereo[B, 4])."""
+        ps, keep_p = T.stereo_images_as_c(prev)
+        cs, keep_c = T.stereo_images_as_c(curr)
+        B = ps.B
+        if results is None:
+            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((B, 4), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_images_lsd_batch(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
+            None if lcfg is None else C.byref(lcfg), C.byref(ps), C.byref(cs), priors.ctypes.data if priors is not None else None,
+            results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep_p, keep_c
+        return results, n_stereo
+
+    def track_stereo_images_lsd_sequence(self, cam, cfg, mcfg, scfg, ocfg, lcfg, frames: dict, priors=None, results=None):
+        """NF consecutive stereo frames (images alone) -> NF - 1 poses, LSD inside the call; every frame's images are detected
+        and described once.  Returns (results, n_stereo[NF, 2])."""
+        fs, keep = T.stereo_images_as_c(frames)
+        NF = fs.B
+        if results is None:
+            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((NF, 2), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_images_lsd_sequence(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
+            None if lcfg is None else C.byref(lcfg), C.byref(fs), priors.ctypes.data if priors is not None else None,
+            results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep
+        return results, n_stereo
+
     def track_stereo_images_stage_times(self):
-        """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB), stereo step, f2fTracking + optimizePose."""
+        """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB; after the LSD form, the lines: LSD's first launch
+        to LBD's last), stereo step, f2fTracking + optimizePose."""
         ms = np.zeros(5, np.float32)
         self._ck(self.lib.plstvo_track_stereo_images_stage_times(self.ctx, _p(ms, T.c_float_p)))
         return ms
