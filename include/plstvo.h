@@ -540,6 +540,15 @@ int     plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, 
  * counts (optional) = {bit 0: tensor-core matcher (always set), bit 1: streamed solver, bits 8..: problems the streamed solver handed to
  * the fp64 kernel in the last pass; work items of the distance kernel; matching problems; pairs}. */
 int     plstvo_batch_stage_times(PlContext* ctx, PlDeviceBatch* db, int iters, double ms[8], int32_t counts[4]);
+/* One solve pass over the resident batch (the matcher's output of the last pass is reused) with the solver kernels' cycle
+ * counters switched on; it computes what the plain pass computes.  out: [B][PLSTVO_PHASE_SLOTS] clock64 sums per pair.
+ * Slots [0, 8) are the fused kernel's phases (match-finalize, gather, GN eval, GN serial, gates/eigen, outliers, final,
+ * sort+MAD), zero for pairs it did not solve.  Slots [8 + 11 s, 19 + 11 s) are the streamed solver's GN loop of stage s
+ * (0 or 1), summed over the iterations of the pair's call: first-call record wait, evaluation, fold + store, barrier,
+ * warp-0 sum and stop tests, close-call fp64 errors, 6x6 solve, increment + pose publish, trailing barriers, end-of-call
+ * covariance, and then the iteration count; all zero where the stage did not run for the pair. */
+#define PLSTVO_PHASE_SLOTS 32
+int     plstvo_batch_phase_cycles(PlContext* ctx, PlDeviceBatch* db, int64_t* out);
 /* GN evaluation (optimizeFunctions, src/stereoFrameHandler.cpp:549-694) of the resident matched
  * lists at given poses, streamed from HBM: the roofline kernel of config C5.
  * DT: [B][16]; H: [B][36]; g: [B][6]; e: [B]. */

@@ -898,6 +898,28 @@ int plstvo_batch_run_timed(PlContext* ctx, PlDeviceBatch* db, int iters, int flu
     return 0;
 }
 
+// One solve pass over the resident batch with the solver kernels' cycle counters on; h: [B][PLSTVO_PHASE_SLOTS] on the host.
+static int ws_phase_pass(PlContext* ctx, Workspace& ws, long long* h) {
+    const size_t bytes = (size_t)ws.B * PLSTVO_PHASE_SLOTS * sizeof(long long);
+    CK(ctx, ws.d_phase.ensure(bytes));
+    CK(ctx, cudaMemsetAsync(ws.d_phase.p, 0, bytes, ctx->s_main));
+    int rc = ws_launch_solve(ctx, ws, 0, ws.B, ws.have_level, ctx->s_main);
+    if (rc) return rc;
+    CK(ctx, cudaMemcpyAsync(h, ws.d_phase.p, bytes, cudaMemcpyDeviceToHost, ctx->s_main));
+    CK(ctx, cudaStreamSynchronize(ctx->s_main));
+    ws.d_phase.release();
+    return 0;
+}
+
+int plstvo_batch_phase_cycles(PlContext* ctx, PlDeviceBatch* db, int64_t* out) {
+    if (!ctx || !db || !out) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    CK(ctx, cudaSetDevice(ctx->device));
+    if (db->ws.B <= 0) return 0;
+    static_assert(sizeof(long long) == sizeof(int64_t), "phase counters");
+    return ws_phase_pass(ctx, db->ws, reinterpret_cast<long long*>(out));
+}
+
 int plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, double* ms_match, double* ms_solve,
                               int32_t* n_tiles, int32_t* n_pairs) {
     if (!ctx || !db || iters <= 0) return PLSTVO_E_INVALID;
@@ -924,20 +946,20 @@ int plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, doub
         tm += a;
         tsv += b;
     }
-    if (getenv("PLSTVO_PHASE_DEBUG") && ws.B > 0) {   // per-phase device cycles of K2, averaged over the pairs
-        CK(ctx, ws.d_phase.ensure((size_t)ws.B * 8 * sizeof(long long)));
-        int rc2 = ws_launch_solve(ctx, ws, 0, ws.B, lev, ctx->s_main);
+    if (getenv("PLSTVO_PHASE_DEBUG") && ws.B > 0) {   // per-phase device cycles of K2 and of the GN loop kernel, averaged over the pairs
+        std::vector<long long> h((size_t)ws.B * PLSTVO_PHASE_SLOTS);
+        int rc2 = ws_phase_pass(ctx, ws, h.data());
         if (rc2) return rc2;
-        std::vector<long long> h((size_t)ws.B * 8);
-        CK(ctx, cudaMemcpyAsync(h.data(), ws.d_phase.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, ctx->s_main));
-        CK(ctx, cudaStreamSynchronize(ctx->s_main));
-        static const char* names[8] = {"match_finalize", "gather", "gn_eval", "gn_serial", "gates_eig", "outliers", "final", "sort_mad"};
-        for (int k = 0; k < 8; ++k) {
+        static const char* names[8 + 11] = {"match_finalize", "gather", "gn_eval", "gn_serial", "gates_eig", "outliers", "final",
+                                            "sort_mad", "gl_wait", "gl_eval", "gl_fold", "gl_barrier", "gl_tests", "gl_close",
+                                            "gl_solve", "gl_increment", "gl_trailing", "gl_inv6", "gl_iterations"};
+        for (int k = 0; k < 8 + 2 * 11; ++k) {
             double sum = 0;
-            for (int p = 0; p < ws.B; ++p) sum += (double)h[(size_t)p * 8 + k];
-            fprintf(stderr, "[plstvo phase] %-15s %10.0f cycles/pair\n", names[k], sum / ws.B);
+            for (int p = 0; p < ws.B; ++p) sum += (double)h[(size_t)p * PLSTVO_PHASE_SLOTS + k];
+            if (k < 8) fprintf(stderr, "[plstvo phase] %-15s %10.0f cycles/pair\n", names[k], sum / ws.B);
+            else fprintf(stderr, "[plstvo phase] %-15s stage %d %10.0f %s/pair\n", names[8 + (k - 8) % 11], 1 + (k - 8) / 11,
+                         sum / ws.B, (k - 8) % 11 == 10 ? "iterations" : "cycles");
         }
-        ws.d_phase.release();
     }
     if (ms_match) *ms_match = tm / iters;
     if (ms_solve) *ms_solve = tsv / iters;

@@ -363,6 +363,50 @@ __device__ bool warp_chol6_solve(const double* Hs, const double* gs, double* x, 
     return ok;
 }
 
+// warp_chol6_solve (without lad) with the whole system in every lane's registers: Hu = the upper triangle row-major (tri(i, j)).
+// The same fp64 operations in the same order, so x and the verdict are bit-identical; no shuffles, no shared memory.
+__device__ __forceinline__ bool chol6_solve_regs(const double* Hu, const double* gv, double* x) {
+    double A[6][6];   // lower triangle: A[i][j] = H[i][j], i >= j; column k becomes column k of L
+#pragma unroll
+    for (int j = 0; j < 6; j++)
+#pragma unroll
+        for (int i = j; i < 6; i++) A[i][j] = Hu[tri(j, i)];
+    // warp_chol6_solve's max over lanes 0..7 (lanes 6 and 7 hold 0), in its butterfly order
+    const double dmax = fmax(fmax(fmax(A[0][0], A[1][1]), fmax(A[2][2], A[3][3])), fmax(fmax(A[4][4], A[5][5]), 0.0));
+    const double thr = dmax * 1e-12;
+    bool ok = (dmax > 0.0) && (dmax == dmax) && (dmax < 1e300);
+    double rinv[6];
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        const double d = A[k][k];
+        ok = ok && (d > thr);
+        const double r = rsqrt(fmax(d, 1e-300));
+        rinv[k] = r;
+#pragma unroll
+        for (int i = k; i < 6; i++) A[i][k] = A[i][k] * r;
+#pragma unroll
+        for (int j = k + 1; j < 6; j++)
+#pragma unroll
+            for (int i = j; i < 6; i++) A[i][j] -= A[i][k] * A[j][k];
+    }
+    double y[6];
+#pragma unroll
+    for (int k = 0; k < 6; k++) {          // L y = g
+        double s = gv[k];
+#pragma unroll
+        for (int j = 0; j < k; j++) s -= A[k][j] * y[j];
+        y[k] = s * rinv[k];
+    }
+#pragma unroll
+    for (int k = 5; k >= 0; k--) {         // L^T x = y
+        double s = y[k];
+#pragma unroll
+        for (int j = k + 1; j < 6; j++) s -= A[j][k] * x[j];
+        x[k] = s * rinv[k];
+    }
+    return ok;
+}
+
 // Matrix6d::inverse() (partial-pivot LU), src/stereoFrameHandler.cpp:429, :470.  Lanes 0..5 hold the columns of A,
 // lanes 6..11 the columns of the identity; row operations are the same in every lane.  Result -> out (shared).
 __device__ void warp_inv6(const double* As /* shared row-major */, double* out /* shared row-major */) {
@@ -1088,6 +1132,14 @@ __device__ __forceinline__ void apply_increment(double* DTs, const double* inc, 
     __syncwarp();
 }
 
+// apply_increment's new pose in the calling thread's registers: R = D * inverse_se3(expmap_se3(inc)), the same operations
+__device__ __forceinline__ void increment_regs(const double* D, const double* inc, double* R) {
+    double E[16], Ei[16];
+    expmap_se3(inc, E);
+    inverse_se3(E, Ei);
+    mat4_mul(D, Ei, R);
+}
+
 // gaussNewtonOptimization (:394-431) and gaussNewtonOptimizationRobust (:433-480).
 // Pose in st.DT (in/out), covariance to st.cov, error to st.err.  Block-wide; warp 0 runs the 6x6 part.
 __device__ void gauss_newton(const Feat& f, State& st, double* sortbuf, const Cam& cam, const PlConfig& cfg,
@@ -1694,7 +1746,7 @@ __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveP
     __syncthreads();
 
     // ---- pose finalisation (:372-391), warp 0 ----
-    if (warp == 0) finalize_pose(st, prior, f, lane, prm.phase_cycles ? prm.phase_cycles + (size_t)pair * 8 : nullptr);
+    if (warp == 0) finalize_pose(st, prior, f, lane, prm.phase_cycles ? prm.phase_cycles + (size_t)pair * PLSTVO_PHASE_SLOTS : nullptr);
     __syncthreads();
     {   // result struct -> HBM, cooperatively (sizeof(PlPoseResult) is a multiple of 8)
         const uint64_t* src = reinterpret_cast<const uint64_t*>(&st.out);
@@ -1926,17 +1978,49 @@ constexpr int GL_FOLD = GL_FOLD_TILES;
 constexpr int GL_CWARPS = GL_SHAPE / 100, GL_STAGES = (GL_SHAPE / 10) % 10, GL_MINBLOCKS = GL_SHAPE % 10;
 constexpr int GL_CONSUMERS = GL_CWARPS * 32, GL_THREADS = GL_CONSUMERS + 32;
 constexpr double GL_ERR_BAND = 2.5e-7;   // relative half-width of the "could go either way" band of the error tests (~10x the noise)
-constexpr double GL_INC_BAND = 1e-3;     // the same for the increment-norm test   // tiles between fp32 -> fp64 folds of a thread's accumulators
+constexpr double GL_INC_BAND = 1e-3;     // the same for the increment-norm test
+// Cycle counters of the PHASES instantiation (thread 0's clock64, summed over one problem's call): slot GLP_FIRST + 11 s + phase
+// of the pair's [PLSTVO_PHASE_SLOTS] row for GN stage s (include/plstvo.h); slots below GLP_FIRST are K2's.
+enum GlPhase { GLP_WAIT, GLP_EVAL, GLP_FOLD, GLP_BARRIER, GLP_TESTS, GLP_CLOSE, GLP_SOLVE, GLP_INC, GLP_TRAIL, GLP_INV, GLP_ITERS, GLP_N };
+constexpr int GLP_FIRST = 8;
+constexpr int GL_STOP = 1, GL_CLOSE = 2;   // warp 0's verdict on an iteration: the call stops / the error tests are a close call
+static_assert(GLP_FIRST + 2 * GLP_N <= PLSTVO_PHASE_SLOTS, "phase slots");
+// One level of the consumers' transposed butterfly: lane L ends up with the warp's sum of accumulator L.  The level is a
+// template argument so that the loop over its OFF pairs unrolls completely and v stays in registers (with the level a loop
+// variable nvcc kept v on the stack and ran the levels as local-memory loops, most of an iteration's time).
+template <int OFF>
+__device__ __forceinline__ void fold_level(float* v, int lane) {
+    const bool up = (lane & OFF) != 0;
+#pragma unroll
+    for (int i = 0; i < OFF; i++) {
+        const float mine = up ? v[i + OFF] : v[i];
+        const float send = up ? v[i] : v[i + OFF];
+        v[i] = mine + __shfl_xor_sync(FULL_MASK, send, OFF);
+    }
+}
+
+template <bool PHASES>
 __global__ void __launch_bounds__(GL_THREADS, GL_MINBLOCKS)
 gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __restrict__ pt_off, const int32_t* __restrict__ ls_off,
                       const StreamBufs sb, int n, int max_iters, int* __restrict__ queue, double* __restrict__ feat_scratch,
-                      size_t feat_stride, int cap_pt, int cap_ls) {
+                      size_t feat_stride, int cap_pt, int cap_ls, long long* __restrict__ phase) {
     extern __shared__ __align__(128) uint8_t ring[];
     __shared__ __align__(8) uint64_t full[GL_STAGES], empty[GL_STAGES];
     __shared__ double red[GL_CWARPS + 1][32], sH[36], sg[8], sDT[16], sDTprev[16], sC[36], s_exact[4];
     __shared__ float sPose[12];
-    __shared__ int s_prob, s_stop, s_amb;
+    __shared__ int s_prob, s_flags;
+    __shared__ long long s_ph[GLP_N];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    long long t_ph = 0;
+    auto mark = [&](GlPhase ph) {          // thread 0: the cycles since its previous mark go to phase ph
+        if constexpr (PHASES) {
+            if (tid == 0) {
+                const long long t = clock64();
+                s_ph[ph] += t - t_ph;
+                t_ph = t;
+            }
+        }
+    };
     if (tid == 0) {
         for (int st = 0; st < GL_STAGES; ++st) {
             mbar_init(&full[st], 1);
@@ -1968,7 +2052,13 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
         double err_prev = c.err_prev, err = 0.0;   // warp 0's copies are the authoritative ones
         int it = 0;
         bool fail_first = false, delegated = false;
+        if constexpr (PHASES) {
+            if (tid < GLP_N) s_ph[tid] = 0;
+        }
         __syncthreads();
+        if constexpr (PHASES) {
+            if (tid == 0) t_ph = clock64();
+        }
         for (;; ++it) {
             if (warp == GL_CWARPS) {           // ---- producer ----
                 if (lane == 0 && (!resident || it == 0)) {
@@ -1997,7 +2087,11 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
                 double run = 0.0;              // lane L: this warp's fp64 total of accumulator L so far
                 for (int t = 0; t < n_tiles; ++t) {
                     const uint32_t kk = k + t, st = kk % GL_STAGES;
-                    if (!resident || it == 0) mbar_wait(&full[st], (kk / GL_STAGES) & 1);
+                    if (!resident || it == 0) {
+                        mark(GLP_EVAL);
+                        mbar_wait(&full[st], (kk / GL_STAGES) & 1);
+                        mark(GLP_WAIT);
+                    }
                     const float4* sr = reinterpret_cast<const float4*>(ring + (size_t)st * GS_STAGE_BYTES);
                     if (t < ptiles) {
                         const int cnt = min(GS_PT_TILE, np - t * GS_PT_TILE);
@@ -2023,28 +2117,78 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
                     __syncwarp();
                     if (lane == 0 && !resident) mbar_arrive(&empty[st]);
                     if ((t % GL_FOLD) == GL_FOLD - 1 || t == n_tiles - 1) {   // fp32 partials -> fp64, fixed order
+                        mark(GLP_EVAL);
                         float v[32];
                         acc.unpack(v);
 #pragma unroll
                         for (int i = GS_NACC; i < 32; i++) v[i] = 0.f;
-#pragma unroll
-                        for (int off = 16; off >= 1; off >>= 1) {
-                            const bool up = (lane & off) != 0;
-#pragma unroll
-                            for (int i = 0; i < off; i++) {
-                                const float mine = up ? v[i + off] : v[i];
-                                const float send = up ? v[i] : v[i + off];
-                                v[i] = mine + __shfl_xor_sync(FULL_MASK, send, off);
-                            }
-                        }
+                        fold_level<16>(v, lane);
+                        fold_level<8>(v, lane);
+                        fold_level<4>(v, lane);
+                        fold_level<2>(v, lane);
+                        fold_level<1>(v, lane);
                         run += (double)v[0];
                         acc.clear();
+                        mark(GLP_FOLD);
                     }
                 }
                 red[warp][lane] = run;
+                mark(GLP_FOLD);
             }
+            // ---- the loop body of :404-427 on the summed normal equations: warp 0, every lane computing the whole step ----
+            // the stop tests at (err, err_prev), the 6x6 solve and the pose update; returns GL_STOP or 0
+            auto step = [&]() -> int {
+                bool stop = false, ambiguous = false;
+                if (err > err_prev) {                                             // :405-410
+                    stop = true;
+                    fail_first = (it == 0);
+                } else if ((err < cfg.min_error) || fabs(err - err_prev) < cfg.min_error_change) {   // :412-415
+                    stop = true;
+                }
+                mark(GLP_TESTS);
+                if (!stop) {
+                    double Hu[21], gv[6], inc[6], R[16];
+#pragma unroll
+                    for (int i = 0; i < 6; i++) {
+#pragma unroll
+                        for (int j = i; j < 6; j++) Hu[tri(i, j)] = sH[i * 6 + j];
+                        gv[i] = sg[i];
+                    }
+                    if (!chol6_solve_regs(Hu, gv, inc)) {                         // :417-418
+                        double lad;
+                        warp_qr6_solve<false>(sH, sg, inc, lad);
+                    }
+                    mark(GLP_SOLVE);
+                    increment_regs(sDT, inc, R);                                  // :419
+                    __syncwarp();                      // every lane has read sDT
+                    if (lane == 0) {
+#pragma unroll
+                        for (int i = 0; i < 16; i++) {
+                            sDTprev[i] = sDT[i];
+                            sDT[i] = R[i];
+                        }
+#pragma unroll
+                        for (int i = 0; i < 12; i++) sPose[i] = gs_pose_entry(R[i], i);
+                    }
+                    const double nt = sqrt(inc[0] * inc[0] + inc[1] * inc[1] + inc[2] * inc[2]);
+                    const double nr = sqrt(inc[3] * inc[3] + inc[4] * inc[4] + inc[5] * inc[5]);
+                    if (nt < cfg.min_error_change && nr < cfg.min_error_change) stop = true;   // :421-424
+                    const double ib = GL_INC_BAND * cfg.min_error_change;
+                    // an increment whose norm sits on its threshold: the one test left to the fp64 kernel (K2 retraces the problem)
+                    ambiguous = (fabs(nt - cfg.min_error_change) <= ib && nr < cfg.min_error_change + ib) ||
+                                (fabs(nr - cfg.min_error_change) <= ib && nt < cfg.min_error_change + ib);
+                    err_prev = err;
+                }
+                if (ambiguous) {
+                    stop = true;
+                    delegated = true;
+                }
+                if (!stop && it + 1 >= max_iters) stop = true;                    // the for loop runs out
+                return stop ? GL_STOP : 0;
+            };
             __syncthreads();
-            if (warp == 0) {                   // ---- the loop body of :404-427 on the summed normal equations ----
+            mark(GLP_BARRIER);
+            if (warp == 0) {
                 double sum = 0.0;
 #pragma unroll
                 for (int w = 0; w < GL_CWARPS; w++) sum += red[w][lane];
@@ -2067,10 +2211,15 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
                 // formed again in fp64 from the fp64 lists, by the whole CTA, and the tests run on those.
                 const double band = GL_ERR_BAND * fabs(err);
                 const bool close_call = fabs((err - err_prev) + cfg.min_error_change) <= band || fabs(err - cfg.min_error) <= band;
-                if (lane == 0) s_amb = close_call ? 1 : 0;
+                // the common case publishes its verdict, the new pose and the stop flag behind ONE block barrier
+                const int fl = close_call ? GL_CLOSE : step();
+                if (lane == 0) s_flags = fl;
+                mark(GLP_INC);
             }
             __syncthreads();
-            if (s_amb) {                       // block-uniform, rare (about one problem in a hundred, once)
+            mark(GLP_TRAIL);
+            int flags = s_flags;                // rewritten by warp 0 only after the next iteration's first barrier
+            if (flags & GL_CLOSE) {            // block-uniform, rare (about one problem in a hundred, once)
                 Feat f;
                 {
                     double* fb = feat_scratch + (size_t)p * feat_stride;
@@ -2101,46 +2250,20 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
                     s_exact[tid] = t;
                 }
                 __syncthreads();
-            }
-            if (warp == 0) {
-                bool stop = false, ambiguous = false;
-                if (s_amb) {
+                mark(GLP_CLOSE);
+                if (warp == 0) {
                     err = s_exact[0] / s_exact[1];
                     if (it > 0) err_prev = s_exact[2] / s_exact[3];
+                    const int fl = step();
+                    if (lane == 0) s_flags = fl;
+                    mark(GLP_INC);
                 }
-                if (err > err_prev) {                                             // :405-410
-                    stop = true;
-                    fail_first = (it == 0);
-                } else if ((err < cfg.min_error) || fabs(err - err_prev) < cfg.min_error_change) {   // :412-415
-                    stop = true;
-                } else {
-                    double inc[6], lad;
-                    if (!warp_chol6_solve(sH, sg, inc)) warp_qr6_solve<false>(sH, sg, inc, lad);   // :417-418
-                    if (lane < 16) sDTprev[lane] = sDT[lane];
-                    __syncwarp();
-                    apply_increment(sDT, inc, lane);                              // :419
-                    if (lane < 12) sPose[lane] = gs_pose_entry(sDT[lane], lane);
-                    const double nt = sqrt(inc[0] * inc[0] + inc[1] * inc[1] + inc[2] * inc[2]);
-                    const double nr = sqrt(inc[3] * inc[3] + inc[4] * inc[4] + inc[5] * inc[5]);
-                    if (nt < cfg.min_error_change && nr < cfg.min_error_change) stop = true;   // :421-424
-                    const double ib = GL_INC_BAND * cfg.min_error_change;
-                    // an increment whose norm sits on its threshold: the one test left to the fp64 kernel (K2 retraces the problem)
-                    ambiguous = (fabs(nt - cfg.min_error_change) <= ib && nr < cfg.min_error_change + ib) ||
-                                (fabs(nr - cfg.min_error_change) <= ib && nt < cfg.min_error_change + ib);
-                    err_prev = err;
-                }
-                if (ambiguous) {
-                    stop = true;
-                    delegated = true;
-                }
-                if (!stop && it + 1 >= max_iters) stop = true;                    // the for loop runs out
-                if (lane == 0) s_stop = stop ? 1 : 0;
+                __syncthreads();
+                flags = s_flags;
+                mark(GLP_TRAIL);
             }
-            __syncthreads();
-            const int stop = s_stop;
-            __syncthreads();
             if (!resident) k += n_tiles;       // a streamed iteration used n_tiles ring slots
-            if (stop) break;
+            if (flags & GL_STOP) break;
         }
         if (resident) {                        // the records sat in the ring for the whole call: hand the stages back now
             if (warp < GL_CWARPS && lane == 0)
@@ -2149,9 +2272,17 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
         }
         if (warp == 0) {                       // :429-430 and the state the next kernels read
             if (!fail_first && !delegated) {
+                mark(GLP_TRAIL);
                 warp_inv6(sH, sC);
                 __syncwarp();
                 for (int i = lane; i < 36; i += 32) c.cov[i] = sC[i];
+                mark(GLP_INV);
+            }
+            if constexpr (PHASES) {
+                if (lane == 0) {
+                    s_ph[GLP_ITERS] = it + 1;
+                    for (int q = 0; q < GLP_N; q++) phase[(size_t)p * PLSTVO_PHASE_SLOTS + q] = s_ph[q];
+                }
             }
             if (lane < 16) sb.DT[(size_t)p * 16 + lane] = sDT[lane];
             if (lane == 0) {
@@ -2334,18 +2465,31 @@ cudaError_t launch_stream_solve(const SolveParams& prm_in, int n_pairs, const St
     if (marks) cudaEventRecord(marks[0], stream);
     const int32_t* off_p = prm.mode == 0 ? prm.prev.pt_off + prm.first_pair : prm.matched.pt_off + prm.first_pair;
     const int32_t* off_l = prm.mode == 0 ? prm.prev.ls_off + prm.first_pair : prm.matched.ls_off + prm.first_pair;
-    static size_t conf_c[64] = {};
+    static size_t conf_c[64] = {}, conf_d[64] = {};
     const size_t ring = (size_t)GL_STAGES * GS_STAGE_BYTES;
-    e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel), ring, conf_c);
+    e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<false>), ring, conf_c);
     if (e != cudaSuccess) return e;
+    if (prm.phase_cycles) {
+        e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<true>), ring, conf_d);
+        if (e != cudaSuccess) return e;
+    }
     int gn_calls = 0;
     auto gn = [&](int max_iters) -> cudaError_t {   // one GN call = one launch: persistent CTAs, one problem each at a time
-        int* q = sb.queue + (gn_calls++);
+        int* q = sb.queue + gn_calls;
         cudaError_t err = cudaMemsetAsync(q, 0, sizeof(int), stream);
         if (err != cudaSuccess) return err;
         const int grid = n_pairs < GL_MINBLOCKS * sb.sm_count ? n_pairs : GL_MINBLOCKS * sb.sm_count;
-        gn_loop_stream_kernel<<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs, max_iters, q,
-                                                                  prm.feat_scratch, (size_t)prm.feat_scratch_stride, prm.cap_pt, prm.cap_ls);
+        if (prm.phase_cycles) {
+            long long* ph = prm.phase_cycles + (size_t)prm.first_pair * PLSTVO_PHASE_SLOTS + GLP_FIRST + gn_calls * GLP_N;
+            gn_loop_stream_kernel<true><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs, max_iters, q,
+                                                                            prm.feat_scratch, (size_t)prm.feat_scratch_stride,
+                                                                            prm.cap_pt, prm.cap_ls, ph);
+        } else {
+            gn_loop_stream_kernel<false><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs, max_iters, q,
+                                                                             prm.feat_scratch, (size_t)prm.feat_scratch_stride,
+                                                                             prm.cap_pt, prm.cap_ls, nullptr);
+        }
+        ++gn_calls;
         nl += 1;
         return cudaGetLastError();
     };

@@ -13,6 +13,7 @@ from . import types as T
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PLSTVO_LIB") or os.path.join(_HERE, "lib", "libplstvo_b200.so")   # PLSTVO_LIB: A/B builds
+PHASE_SLOTS = 32   # PLSTVO_PHASE_SLOTS
 
 ERRORS = {-1: "PLSTVO_E_INVALID", -2: "PLSTVO_E_TOO_LARGE", -3: "PLSTVO_E_CUDA", -4: "PLSTVO_E_NO_DEVICE",
           -5: "PLSTVO_E_SIZE"}
@@ -82,6 +83,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_launch_count": (C.c_int64, [vp]),
         "plstvo_batch_kernel_times": (C.c_int, [vp, vp, C.c_int, dp, dp, i32p, i32p]),
         "plstvo_batch_stage_times": (C.c_int, [vp, vp, C.c_int, dp, i32p]),
+        "plstvo_batch_phase_cycles": (C.c_int, [vp, vp, C.POINTER(C.c_int64)]),
         "plstvo_gn_eval_stream": (C.c_int, [vp, cam, cfg, mb, dp, C.c_int, dp, dp, dp, C.POINTER(C.c_float)]),
         "plstvo_popc_rate": (C.c_int, [vp, dp]),
         "plstvo_debug_algebra": (C.c_int, [vp, C.c_int, dp, dp, dp, dp, dp, dp]),
@@ -132,6 +134,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_optimize_pose", "plstvo_track_batch", "plstvo_track_batch_async", "plstvo_wait", "plstvo_batch_upload", "plstvo_batch_run",
     "plstvo_batch_run_timed", "plstvo_batch_download", "plstvo_batch_free", "plstvo_synchronize",
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
+    "plstvo_batch_phase_cycles",
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
@@ -239,6 +242,12 @@ class DeviceBatch:
                     ms_outliers=float(ms[6]), ms_gn_stage2=float(ms[7]),
                     tensor_core_form=bool(cnt[0] & 1), streamed_solver=bool(cnt[0] & 2), delegated_to_fp64=int(cnt[0] >> 8), n_items=int(cnt[1]),
                     n_problems=int(cnt[2]), n_pairs=int(cnt[3]))
+
+    def phase_cycles(self):
+        """One solve pass with the solver kernels' cycle counters on: [B][PHASE_SLOTS] int64 (layout in include/plstvo.h)."""
+        out = np.zeros((self.B, PHASE_SLOTS), np.int64)
+        self.eng._ck(self.eng.lib.plstvo_batch_phase_cycles(self.eng.ctx, self.handle, out.ctypes.data_as(C.POINTER(C.c_int64))))
+        return out
 
     def download(self):
         res = np.zeros(self.B, dtype=T.POSE_RESULT_DTYPE)
