@@ -467,6 +467,65 @@ int plstvo_track_stereo_images_lsd_sequence(PlContext* ctx, const PlCamera* cam,
  * (to LSD's last where no image has a line), the host hops in between included. */
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]);
 
+/* ---- rectification: what Dataset::nextFrame runs on every frame before the handler (src/dataset.cpp:147-157), i.e.
+ * PinholeStereoCamera::rectifyImagesLR (src/pinholeStereoCamera.cpp:188-208): cv::remap(INTER_LINEAR) of each image on the
+ * CV_16SC2 maps its constructor built (:30-182) ---- */
+typedef struct PlRectifyModel {
+    double model;    /* 0: pinhole (cv::initUndistortRectifyMap), 1: equidistant (cv::fisheye::initUndistortRectifyMap) */
+    double n_dist;   /* coefficients in D: pinhole 4, 5 or 8 (k1 k2 p1 p2 [k3 [k4 k5 k6]]); fisheye 4 (k1 .. k4) */
+    double K[9];     /* camera matrix, row-major (fx, cx, fy, cy are read) */
+    double D[8];
+    double R[9];     /* rectifying rotation, row-major (cv::stereoRectify's R1 / R2, or the identity) */
+    double P[12];    /* new camera matrix, 3x4 row-major; its first three columns are used (stereoRectify's P1 / P2) */
+} PlRectifyModel;
+/* The CV_16SC2 + CV_16UC1 pair OpenCV 4.13 returns for the model: map1 [height][width][2], map2 [height][width].  Host code,
+ * no context or GPU needed; it runs once per rig.  Bit-exact with OpenCV on x86-64 as dispatched for AVX2, whose vector loop
+ * sets two things the maps show: the pinhole builder takes each row in blocks of 8 pixels (lane j at the block's start +
+ * j * the column step, the leftover columns accumulated), and in those blocks packs the integer coordinate to short with
+ * saturation where its scalar loop, the fisheye builder and the leftover columns truncate.  A coordinate * 32 outside int
+ * (and the fisheye builder's +-infinity behind the camera) becomes INT_MIN as cvRound gives it.  Exact ties of u * 32 or
+ * v * 32, which only rigs with dyadic parameters reach, may round differently where OpenCV's vector code fuses.
+ * PLSTVO_E_INVALID: a null pointer, a model other than 0 / 1, a coefficient count other than the above (no thin prism, no
+ * tilt), a singular P[:, :3] * R, or width / height outside 1..32767. */
+int plstvo_init_undistort_rectify_map(const PlRectifyModel* model, int width, int height, int16_t* map1, uint16_t* map2);
+
+/* A rig's two map pairs resident in HBM, 6 bytes per pixel per side (held once when both sides pass the same pointers, as the
+ * reference's cam_d0 branch does).  The maps may come from plstvo_init_undistort_rectify_map or from OpenCV.  Returns NULL on
+ * failure (a size outside 1..32767, a null map, or no device memory; plstvo_last_error says which).  Destroy a rectifier
+ * before its context. */
+typedef struct PlRectifier PlRectifier;
+PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, const int16_t* map1_l, const uint16_t* map2_l,
+                                     const int16_t* map1_r, const uint16_t* map2_r);
+void plstvo_rectifier_destroy(PlRectifier* rect);
+/* rectifyImagesLR on B pairs: out_l[b] = cv::remap(img_l[b], map1_l, map2_l, INTER_LINEAR, BORDER_CONSTANT, 0), and the
+ * same on the right; images [B][height][width] grey of the rectifier's size, host memory in and out.  The weights are
+ * OpenCV's INTER_LINEAR table and the sum is rounded as cv::remap rounds it, so the result equals OpenCV's byte for byte.
+ * PLSTVO_E_INVALID: a null pointer, B < 0, or a rectifier of another context.  Device memory: 2 bytes per pixel of the call
+ * (raw and rectified), kept by the context for the next call. */
+int plstvo_rectify_batch(PlContext* ctx, const PlRectifier* rect, int B, const uint8_t* img_l, const uint8_t* img_r,
+                         uint8_t* out_l, uint8_t* out_r);
+/* Device time of the last remap on this context (plstvo_rectify_batch or a raw-images call), ms. */
+int plstvo_rectify_kernel_times(PlContext* ctx, float* ms1);
+
+/* ---- raw stereo images in, pose out: Dataset::nextFrame's rectifyImagesLR, then the handler (plstvo_track_stereo_images_lsd_*)
+ * The signatures of the _lsd_ calls plus rect.  Results and n_stereo equal, byte for byte, plstvo_rectify_batch on every pair
+ * followed by plstvo_track_stereo_images_lsd_batch / _sequence on the rectified images.  rect == NULL: the _lsd_ call (the
+ * reference's copy when dist is false).  The raw images go up once into a staging slot and the remap writes the device copy
+ * that LSD, ORB and LBD read, so no rectified image crosses PCIe; stage slot [0] of plstvo_track_stereo_images_stage_times
+ * then covers the upload and the remap.  Device memory besides the _lsd_ call's: the staging copy, 1 byte per pixel of the
+ * call, and the rectifier's maps.  PLSTVO_E_SIZE: the rectifier's size differs from cam's (and so from the images');
+ * PLSTVO_E_INVALID: a rectifier of another context, and every code of the _lsd_ calls.  The context stays usable after any
+ * error.  The call also updates what plstvo_rectify_kernel_times reports when the images are read. */
+int plstvo_track_stereo_raw_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                         const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                         const PlRectifier* rect, const PlStereoImages* prev, const PlStereoImages* curr,
+                                         const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo /* [B][4] */);
+int plstvo_track_stereo_raw_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                            const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                            const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlRectifier* rect,
+                                            const PlStereoImages* frames, const PlPrior* priors, PlPoseResult* results,
+                                            int32_t* n_stereo /* [B+1][2] */);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

@@ -268,6 +268,112 @@ inline void dropLines(const std::vector<StereoImageFrame>& frames, StereoImagesP
     p.view.npix_l = p.view.npix_r = nullptr;
 }
 }  // namespace detail
+// ---- rectification: PinholeStereoCamera's maps (src/pinholeStereoCamera.cpp:30-182) and rectifyImagesLR (:196-208) ----
+// One camera's CV_16SC2 + CV_16UC1 maps: map1 [height][width][2], map2 [height][width].
+struct RectifyMaps {
+    int width = 0, height = 0;
+    std::vector<int16_t> map1;
+    std::vector<uint16_t> map2;
+};
+// cv::initUndistortRectifyMap / cv::fisheye::initUndistortRectifyMap with m1type CV_16SC2 (plstvo_init_undistort_rectify_map;
+// host code, no GPU).
+inline RectifyMaps initUndistortRectifyMap(const PlRectifyModel& model, int width, int height) {
+    RectifyMaps m;
+    m.width = width;
+    m.height = height;
+    const size_t px = width > 0 && height > 0 ? (size_t)width * (size_t)height : 1;
+    m.map1.resize(2 * px);
+    m.map2.resize(px);
+    const int rc = plstvo_init_undistort_rectify_map(&model, width, height, m.map1.data(), m.map2.data());
+    if (rc < 0) throw Error(rc, "initUndistortRectifyMap: unsupported model (coefficient count, singular P * R) or size");
+    return m;
+}
+// A rig's maps resident in HBM (plstvo_rectifier_create); one map pair for both sides where only left is given.  Destroy it
+// before its Context.
+class Rectifier {
+public:
+    Rectifier(Context& c, const RectifyMaps& left, const RectifyMaps& right) : r_(create(c, left, right)) {}
+    Rectifier(Context& c, const RectifyMaps& both) : r_(create(c, both, both)) {}
+    ~Rectifier() { plstvo_rectifier_destroy(r_); }
+    Rectifier(const Rectifier&) = delete;
+    Rectifier& operator=(const Rectifier&) = delete;
+    const PlRectifier* get() const { return r_; }
+private:
+    static PlRectifier* create(Context& c, const RectifyMaps& l, const RectifyMaps& r) {
+        if (l.width != r.width || l.height != r.height) throw Error(PLSTVO_E_SIZE, "Rectifier: the two sides' maps differ in size");
+        PlRectifier* p = plstvo_rectifier_create(c.get(), l.width, l.height, l.map1.data(), l.map2.data(), r.map1.data(),
+                                                 r.map2.data());
+        if (!p) throw Error(PLSTVO_E_INVALID, plstvo_last_error(c.get()));
+        return p;
+    }
+    PlRectifier* r_ = nullptr;
+};
+// PinholeStereoCamera::rectifyImagesLR on B pairs (plstvo_rectify_batch): out = cv::remap(img, maps, INTER_LINEAR), byte for
+// byte; [B][height][width] grey in and out.
+inline void rectifyImagesLR(Context& c, const Rectifier& r, const uint8_t* img_l, uint8_t* rec_l, const uint8_t* img_r,
+                            uint8_t* rec_r, int B = 1) {
+    c.check(plstvo_rectify_batch(c.get(), r.get(), B, img_l, img_r, rec_l, rec_r));
+}
+// The models and the rectified camera of each PinholeStereoCamera constructor branch.  stereoRectify is not built: the caller
+// passes the R1 / R2 and P1 / P2 (3x4, row-major) that cv::stereoRectify(Kl, Dl, Kr, Dr, size, R, t, ..., CALIB_ZERO_DISPARITY,
+// 0) gave, as the reference's constructor computes them.  cam: fx, fy, cx, cy from P1 and b = cam_bl, as given.
+struct StereoRectification {
+    PlRectifyModel left{}, right{};
+    PlCamera cam{};
+    bool one_map = false;   // the cam_d0 branch: the left map serves both sides
+
+    // The Kl / Dl branch (EuRoC): K = (fx, fy, cx, cy) rounded to float as Mat_<float> stores it, D in double (4, 5 or 8
+    // coefficients); equidistant: the dtype branch, cv::fisheye maps with 4 coefficients.
+    static StereoRectification pinhole(int width, int height, double b, const double Kl[4], const std::vector<double>& Dl,
+                                       const double Kr[4], const std::vector<double>& Dr, const double R1[9], const double P1[12],
+                                       const double R2[9], const double P2[12], bool equidistant = false) {
+        StereoRectification s;
+        s.left = model(equidistant, Kl, Dl, R1, P1, true);
+        s.right = model(equidistant, Kr, Dr, R2, P2, true);
+        s.cam = camera(width, height, b, P1);
+        return s;
+    }
+    // The cam_d0 branch (cam_d0 != 0): K, D (d0..d3, 0) and P in float, P's fy = fx, R = I; one map for both sides.
+    static StereoRectification camD0(int width, int height, double fx, double fy, double cx, double cy, double b, double d0,
+                                     double d1, double d2, double d3) {
+        StereoRectification s;
+        const double K[4] = {fx, fy, cx, cy};
+        const double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+        const double P[12] = {(float)fx, 0, (float)cx, 0, 0, (float)fx, (float)cy, 0, 0, 0, 1, 0};
+        const std::vector<double> D{(float)d0, (float)d1, (float)d2, (float)d3, 0.0};
+        s.left = s.right = model(false, K, D, R, P, true);
+        s.cam = camera(width, height, b, P);
+        s.one_map = true;
+        return s;
+    }
+    // the maps of both sides, uploaded once
+    Rectifier rectifier(Context& c) const {
+        const RectifyMaps l = initUndistortRectifyMap(left, cam.width, cam.height);
+        if (one_map) return Rectifier(c, l);
+        return Rectifier(c, l, initUndistortRectifyMap(right, cam.width, cam.height));
+    }
+
+private:
+    static PlRectifyModel model(bool equidistant, const double K4[4], const std::vector<double>& D, const double R[9],
+                                const double P[12], bool k_float) {
+        PlRectifyModel m{};
+        m.model = equidistant ? 1 : 0;
+        m.n_dist = (double)D.size();
+        auto kf = [k_float](double v) { return k_float ? (double)(float)v : v; };
+        const double K[9] = {kf(K4[0]), 0, kf(K4[2]), 0, kf(K4[1]), kf(K4[3]), 0, 0, 1};
+        std::copy(K, K + 9, m.K);
+        std::copy(D.begin(), D.begin() + std::min<size_t>(D.size(), 8), m.D);
+        std::copy(R, R + 9, m.R);
+        std::copy(P, P + 12, m.P);
+        return m;
+    }
+    static PlCamera camera(int width, int height, double b, const double P[12]) {
+        PlCamera c{};
+        c.fx = P[0]; c.fy = P[5]; c.cx = P[2]; c.cy = P[6]; c.b = b; c.width = width; c.height = height;
+        return c;
+    }
+};
+
 // Stereo images in, pose out (plstvo_track_stereo_images_batch): extractStereoFeatures with LSD left to the caller, then
 // f2fTracking + optimizePose, for prev.size() independent (prev[p], curr[p]) pairs of images of cam's size.  priors: one per
 // pair or empty (identity).  n_stereo (optional) receives [pairs][4] = stereo points, lines of prev, then of curr.
@@ -701,6 +807,14 @@ public:
                        const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
                        const HandlerConfig& hcfg = HandlerConfig{})
         : ctx_(ctx), cam_(cam), cfg_(cfg), mc_(mc), sc_(sc), oc_(oc), lc_(lc), hcfg_(hcfg) {}
+    // Raw images, as Dataset::nextFrame feeds the reference's handler (src/dataset.cpp:147-157): initialize / insertStereoPair
+    // take the camera's images before rectifyImagesLR, and each call rectifies them on the device under rect
+    // (plstvo_track_stereo_raw_images_batch); cam is the rectified camera (StereoRectification::cam).  rect must outlive the
+    // handler.
+    StereoImageHandler(Context& ctx, const Rectifier& rect, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                       const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                       const HandlerConfig& hcfg = HandlerConfig{})
+        : ctx_(ctx), cam_(cam), cfg_(cfg), mc_(mc), sc_(sc), oc_(oc), lc_(lc), hcfg_(hcfg), rect_(rect.get()) {}
 
     void initialize(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // src/stereoFrameHandler.cpp:35-52
         orb_fast_th = hcfg_.orb_fast_th;                 // :38
@@ -728,8 +842,9 @@ public:
         // threshold the handler chose, 0 included (updateFastThreshold returns 0 when fast_min_th <= 0), as in the reference
         PlOrbDetectConfig oc = oc_;
         oc.fast_threshold = 0;
-        ctx_.check(plstvo_track_stereo_images_lsd_batch(ctx_.get(), &cam_, &cfg_, &mc_, &sc_, &oc, &lc_, &prev, &curr, &prior,
-                                                        &result_, n_stereo.data()));
+        // without a rectifier this is plstvo_track_stereo_images_lsd_batch
+        ctx_.check(plstvo_track_stereo_raw_images_batch(ctx_.get(), &cam_, &cfg_, &mc_, &sc_, &oc, &lc_, rect_, &prev, &curr,
+                                                        &prior, &result_, n_stereo.data()));
         n_inliers_pt = result_.n_matched_pt;             // :126-128
         n_inliers_ls = result_.n_matched_ls;
         n_inliers = n_inliers_pt + n_inliers_ls;
@@ -778,6 +893,7 @@ private:
     std::vector<uint8_t> prev_l_, prev_r_, curr_l_, curr_r_;
     int32_t prev_th_ = 0, curr_th_ = 0;
     bool has_prev_ = false;
+    const PlRectifier* rect_ = nullptr;   // null: the images are already rectified
 };
 
 }  // namespace plstvo

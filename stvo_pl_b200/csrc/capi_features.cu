@@ -217,10 +217,6 @@ int lbd_check_lines(PlContext* ctx, const LineSrc& l) {
     return 0;
 }
 
-struct ImgPart {   // consecutive host images of one size
-    const uint8_t* p; int n;
-};
-
 // Enqueues LBD description on stream s for checked key lines (parts, in image order; at least one line in all) of images of one
 // size: either device images (d_img, ready once img_ready has completed) or host images that go into arena_lbd (img_parts).
 // Leaves the key lines' segments (sPointInOctave, ePointInOctave as given) and descriptors in arena_lbd.
@@ -845,13 +841,16 @@ int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
 // The images go up once, in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left][curr right].
 // Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.  The key lines are
 // the caller's, or (detect_lines) LSD's, detected on the same device copy of the images: ORB's, or LSD's own when ORB does
-// not run.
+// not run.  With a rectifier (raw images), that copy is the remap's output and every stage reads it.
 static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                             const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
-                            const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors, PlPoseResult* results,
-                            int32_t* n_stereo, bool sequence) {
+                            const PlRectifier* rect, const PlStereoImages* prev, const PlStereoImages* curr,
+                            const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence) {
     if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
         return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    if (rect && rect->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the rectifier belongs to another context");
+    if (rect && (rect->width != cam->width || rect->height != cam->height))
+        return fail(ctx, PLSTVO_E_SIZE, "rectifier size differs from the camera's");
     const int NF = prev->B;
     if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
     if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
@@ -953,9 +952,17 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     // LSD on the second stream.
     const bool lsd_first = run_lsd && pts && n_img < ctx->sm_count;
     CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
-    const uint8_t* orb_images = nullptr;   // the device images ORB reads (null: ORB uploads them)
+    // raw images: they go up into the rectifier's staging slot, and every stage reads the remap's device copy
+    const uint8_t* rectified = nullptr;
+    cudaEvent_t rectified_ready = nullptr;
+    if (rect && (pts || lns)) {
+        if (const int rc = rectify_enqueue(ctx, rect, n_img, NF, iparts, ctx->s_main, &rectified)) return rc;
+        rectified_ready = next_event(ctx);
+        CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
+    }
+    const uint8_t* orb_images = rectified;   // the device images ORB reads (null: ORB uploads them)
     if (lsd_first) {
-        if (const int rc = lsd_enqueue(ctx, lsd, nullptr, nullptr, iparts, ctx->s_main)) return rc;
+        if (const int rc = lsd_enqueue(ctx, lsd, rectified, nullptr, iparts, ctx->s_main)) return rc;
         if (const int rc = lsd_lines(ctx->s_main)) return rc;
         orb_images = lsd.images;
     }
@@ -975,7 +982,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     } else {
         orb.off.assign((size_t)n_img + 1, 0);
         if (lsd_beside || run_lbd)
-            if (const int rc = lines_beside(nullptr, nullptr)) return rc;
+            if (const int rc = lines_beside(rectified, rectified_ready)) return rc;
     }
     if (lsd_beside) {   // LSD's host continuation (while ORB's selection and descriptors run), then LBD on the same stream
         if (const int rc = lsd_lines(ctx->s_alt)) return rc;
@@ -1038,10 +1045,11 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
 static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
                                const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
-                               PlPoseResult* results, int32_t* n_stereo, bool sequence) {
+                               PlPoseResult* results, int32_t* n_stereo, bool sequence, const PlRectifier* rect = nullptr) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, prev, curr, priors, results, n_stereo, sequence);
+    const int rc =
+        track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, rect, prev, curr, priors, results, n_stereo, sequence);
     // after an error the line stages may still run on the second stream, and ORB on the first: the next call may reuse their
     // arenas
     const cudaError_t e = cudaStreamSynchronize(ctx->s_alt), e_main = cudaStreamSynchronize(ctx->s_main);
@@ -1075,6 +1083,21 @@ int plstvo_track_stereo_images_lsd_sequence(PlContext* ctx, const PlCamera* cam,
                                             const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlStereoImages* frames,
                                             const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
     return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, frames, nullptr, priors, results, n_stereo, true);
+}
+
+int plstvo_track_stereo_raw_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
+                                         const PlStereoConfig* scfg, const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                         const PlRectifier* rect, const PlStereoImages* prev, const PlStereoImages* curr,
+                                         const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, prev, curr, priors, results, n_stereo, false, rect);
+}
+
+int plstvo_track_stereo_raw_images_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                            const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                            const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlRectifier* rect,
+                                            const PlStereoImages* frames, const PlPrior* priors, PlPoseResult* results,
+                                            int32_t* n_stereo) {
+    return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, frames, nullptr, priors, results, n_stereo, true, rect);
 }
 
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {

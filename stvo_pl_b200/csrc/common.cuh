@@ -286,6 +286,11 @@ cudaError_t launch_lbd(int n_img, int W, int H, const uint8_t* images, const int
                        const float2* dir, const int32_t* npix, short2* grad, uint8_t* out_desc, cudaStream_t s,
                        cudaEvent_t* ev, int* launches);   // dir: (cosf, sinf) of each angle; ev[0..2]: start, gradients, descriptors
 
+// rectify.cu: cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of n_img grey W x H images on CV_16SC2 + CV_16UC1 maps; image z takes
+// the right maps (m1[1], m2[1]) where (z / per_block) is odd, the left ones otherwise
+cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const uint8_t* src, uint8_t* dst,
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches);
+
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);
 int gn_stream_partials_per_slice();   // fp64 partial records one slice writes (one per consumer warp)   // 16 KB tiles of one problem (512 points or 256 lines each)

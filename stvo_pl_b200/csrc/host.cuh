@@ -189,6 +189,9 @@ struct PlContext {
     plstvo::DevBuf lsd_trig;       // cos / sin table of the gradient angles (lsd.cu), built once
     bool lsd_ran = false;
     plstvo::Events<6> lsd_ev;
+    plstvo::DevBuf arena_rect;     // plstvo_rectify_batch / _raw_images_*: raw images (staging), rectified images
+    bool rect_ran = false;
+    plstvo::Events<2> rect_ev;     // the remap kernel's start and end
     // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
     plstvo::Events<4> img_ev;
     plstvo::Events<1> img_join;
@@ -202,6 +205,16 @@ struct PlContext {
         for (cudaStream_t s : {s_main, s_alt, s_h2d, s_d2h})
             if (s) cudaStreamDestroy(s);
     }
+};
+
+// A rig's two CV_16SC2 + CV_16UC1 map pairs, resident in HBM (plstvo_rectifier_create).  Where both sides were given the same
+// maps they are held once and m1[1], m2[1] alias side 0.
+struct PlRectifier {
+    PlContext* ctx = nullptr;
+    int width = 0, height = 0;
+    plstvo::DevBuf map1[2], map2[2];
+    const short2* m1[2] = {nullptr, nullptr};
+    const uint16_t* m2[2] = {nullptr, nullptr};
 };
 
 namespace plstvo {
@@ -374,5 +387,14 @@ int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg
                         const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                         const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
                         const StereoDevInputs* dev = nullptr);
+
+// ---- rectify.cu: rectifyImagesLR on the device, composed by the raw-images path ----
+struct ImgPart {   // consecutive host images of one size
+    const uint8_t* p; int n;
+};
+// Enqueues on stream s the upload of n_img raw images of rect's size (parts, in order) into arena_rect's staging slot and
+// their remap into its rectified slot (*d_out), in blocks of per_block images that alternate left, right maps.
+int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
+                    cudaStream_t s, const uint8_t** d_out);
 
 }  // namespace plstvo

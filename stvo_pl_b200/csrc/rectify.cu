@@ -1,0 +1,289 @@
+// rectify.cu — PinholeStereoCamera::rectifyImagesLR (src/pinholeStereoCamera.cpp:196-208) on the device: the rig's
+// undistort-rectify maps, built once on the host as OpenCV builds them and held in HBM, and cv::remap's INTER_LINEAR with
+// BORDER_CONSTANT 0 on a batch of grey images.
+#include <cfloat>
+#include <climits>
+#include <cmath>
+#include <cstring>
+
+#include "host.cuh"
+
+using namespace plstvo;
+
+namespace {
+
+// cv::remap's fixed point (INTER_BITS 5, INTER_REMAP_COEF_BITS 15): the weights of the four taps are ((32 - ax)(32 - ay),
+// ax (32 - ay), (32 - ax) ay, ax ay) * 32, OpenCV's INTER_LINEAR table exactly (each bilinear product is a multiple of
+// 1/1024), and the result is (sum + 2^14) >> 15, which is (sum / 32 + 2^9) >> 10.  A tap outside the image reads 0.
+__device__ __forceinline__ uint32_t remap_pixel(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
+    f &= 1023u;   // OpenCV indexes its table with map2 & (INTER_TAB_SIZE2 - 1)
+    const int ax = (int)(f & 31u), ay = (int)(f >> 5);
+    const int x = m.x, y = m.y;
+    const bool x0 = (unsigned)x < (unsigned)W, x1 = (unsigned)(x + 1) < (unsigned)W;
+    const bool y0 = (unsigned)y < (unsigned)H, y1 = (unsigned)(y + 1) < (unsigned)H;
+    const uint8_t* r0 = S + (size_t)y * W + x;
+    const int v00 = (x0 && y0) ? __ldg(r0) : 0, v01 = (x1 && y0) ? __ldg(r0 + 1) : 0;
+    const int v10 = (x0 && y1) ? __ldg(r0 + W) : 0, v11 = (x1 && y1) ? __ldg(r0 + W + 1) : 0;
+    const int sum = v00 * ((32 - ax) * (32 - ay)) + v01 * (ax * (32 - ay)) + v10 * ((32 - ax) * ay) + v11 * (ax * ay);
+    return (uint32_t)((sum + 512) >> 10);
+}
+
+// One thread writes 4 consecutive pixels of one image (flat index p0 .. p0 + 3 of W*H): one 16-byte map1 load, one 8-byte
+// map2 load, 16 byte gathers on the read-only path and one 4-byte store where the output is 4-byte aligned.  blockIdx.y is
+// the image within a slice of at most 65535 starting at z0.
+__global__ void __launch_bounds__(256) rectify_remap_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                                                            const short2* __restrict__ m1l, const uint16_t* __restrict__ m2l,
+                                                            const short2* __restrict__ m1r, const uint16_t* __restrict__ m2r,
+                                                            int W, int H, int per_block, int z0) {
+    const int z = z0 + (int)blockIdx.y;
+    const size_t N = (size_t)W * H;
+    const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (p0 >= N) return;
+    const bool right = (z / per_block) & 1;
+    const short2* m1 = right ? m1r : m1l;
+    const uint16_t* m2 = right ? m2r : m2l;
+    const uint8_t* S = src + (size_t)z * N;
+    uint8_t* D = dst + (size_t)z * N + p0;
+    if (p0 + 4 <= N) {   // the maps start 256-byte aligned, so p0 % 4 == 0 aligns both vector loads
+        const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
+        const uint2 b = __ldg(reinterpret_cast<const uint2*>(m2 + p0));
+        short2 m[4];
+        memcpy(m, &a, sizeof a);
+        const uint32_t v = remap_pixel(S, W, H, m[0], b.x & 0xffffu) | remap_pixel(S, W, H, m[1], b.x >> 16) << 8 |
+                           remap_pixel(S, W, H, m[2], b.y & 0xffffu) << 16 | remap_pixel(S, W, H, m[3], b.y >> 16) << 24;
+        if (((uintptr_t)D & 3) == 0) {
+            *reinterpret_cast<uint32_t*>(D) = v;
+        } else {
+            D[0] = (uint8_t)v; D[1] = (uint8_t)(v >> 8); D[2] = (uint8_t)(v >> 16); D[3] = (uint8_t)(v >> 24);
+        }
+    } else {
+        for (size_t p = p0; p < N; ++p) D[p - p0] = (uint8_t)remap_pixel(S, W, H, __ldg(m1 + p), __ldg(m2 + p));
+    }
+}
+
+// cvRound (saturate_cast<int>(double)) on x86-64: round half to even; cvtsd2si gives INT_MIN for a result outside int, and for NaN
+int cv_round(double v) {
+    const double r = nearbyint(v);
+    return (r >= -2147483648.0 && r <= 2147483647.0) ? (int)r : INT_MIN;
+}
+
+// The CV_16SC2 + CV_16UC1 words of one pixel.  OpenCV's vector loop (vec) packs iu >> 5 to short with saturation, its
+// scalar loop truncates.
+void store_map(double u, double v, bool vec, int16_t* m1, uint16_t* m2) {
+    const int iu = cv_round(u * 32.0), iv = cv_round(v * 32.0);
+    const int su = iu >> 5, sv = iv >> 5;
+    m1[0] = vec ? (int16_t)std::min(std::max(su, -32768), 32767) : (int16_t)su;
+    m1[1] = vec ? (int16_t)std::min(std::max(sv, -32768), 32767) : (int16_t)sv;
+    *m2 = (uint16_t)((iv & 31) * 32 + (iu & 31));
+}
+}  // namespace
+
+namespace plstvo {
+
+cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const uint8_t* src, uint8_t* dst,
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches) {
+    const size_t quads = ((size_t)W * H + 3) / 4;
+    const unsigned gx = (unsigned)((quads + 255) / 256);
+    for (int z0 = 0; z0 < n_img; z0 += 65535) {
+        const int nz = std::min(n_img - z0, 65535);
+        rectify_remap_kernel<<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block, z0);
+        ++*launches;
+    }
+    return cudaGetLastError();
+}
+
+int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
+                    cudaStream_t s, const uint8_t** d_out) {
+    const int W = rect->width, H = rect->height;
+    const size_t bytes = (size_t)n_img * W * H;
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, ctx->rect_ev.create());
+    Arena a;
+    const size_t o_raw = a.take(bytes), o_out = a.take(bytes);
+    CK(ctx, a.alloc(ctx->arena_rect));
+    size_t o = o_raw;
+    for (const ImgPart& ip : parts) {
+        const size_t b = (size_t)ip.n * W * H;
+        CK(ctx, a.up(o, ip.p, b, s));
+        o += b;
+    }
+    int launches = 0;
+    ctx->rect_ran = false;
+    CK(ctx, cudaEventRecord(ctx->rect_ev[0], s));
+    CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches));
+    CK(ctx, cudaEventRecord(ctx->rect_ev[1], s));
+    ctx->rect_ran = true;
+    ctx->launches += launches;
+    *d_out = a.u8(o_out);
+    return 0;
+}
+
+}  // namespace plstvo
+
+extern "C" {
+
+int plstvo_init_undistort_rectify_map(const PlRectifyModel* m, int width, int height, int16_t* map1, uint16_t* map2) {
+    if (!m || !map1 || !map2) return PLSTVO_E_INVALID;
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) return PLSTVO_E_INVALID;
+    const bool fisheye = m->model == 1;
+    const int nd = (int)m->n_dist;
+    if (!(m->model == 0 || fisheye) || (double)nd != m->n_dist) return PLSTVO_E_INVALID;
+    if (fisheye ? nd != 4 : !(nd == 4 || nd == 5 || nd == 8)) return PLSTVO_E_INVALID;   // no thin prism or tilt
+    // iR = (P[:, :3] R)^-1: the product summed left to right, the inverse in the cofactor form cv::invert(DECOMP_LU) takes for
+    // 3x3 (the fisheye builder inverts by SVD, which gave the same maps on every rig it was compared on)
+    const double* R = m->R;
+    const double* P = m->P;
+    double A[9];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) A[3 * i + j] = P[4 * i] * R[j] + P[4 * i + 1] * R[3 + j] + P[4 * i + 2] * R[6 + j];
+    double d = A[0] * (A[4] * A[8] - A[5] * A[7]) - A[1] * (A[3] * A[8] - A[5] * A[6]) + A[2] * (A[3] * A[7] - A[4] * A[6]);
+    if (d == 0.0 || !std::isfinite(d)) return PLSTVO_E_INVALID;
+    d = 1.0 / d;
+    const double ir[9] = {(A[4] * A[8] - A[5] * A[7]) * d, (A[2] * A[7] - A[1] * A[8]) * d, (A[1] * A[5] - A[2] * A[4]) * d,
+                          (A[5] * A[6] - A[3] * A[8]) * d, (A[0] * A[8] - A[2] * A[6]) * d, (A[2] * A[3] - A[0] * A[5]) * d,
+                          (A[3] * A[7] - A[4] * A[6]) * d, (A[1] * A[6] - A[0] * A[7]) * d, (A[0] * A[4] - A[1] * A[3]) * d};
+    const double fx = m->K[0], fy = m->K[4], u0 = m->K[2], v0 = m->K[5];   // the skew K[1] is not read, as in OpenCV
+    double k[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    for (int c = 0; c < nd; ++c) k[c] = m->D[c];
+    if (!fisheye) {
+        // cv::initUndistortRectifyMap: k1 k2 p1 p2 [k3 [k4 k5 k6]].  Its vector loop (AVX2: two 4-lane double vectors) takes
+        // blocks of 8 pixels, lane j the block's start + j*ir[0]; the columns after the last block add ir[0] per pixel.
+        const double k1 = k[0], k2 = k[1], p1 = k[2], p2 = k[3], k3 = k[4], k4 = k[5], k5 = k[6], k6 = k[7];
+        const int vec_cols = width - width % 8;
+        for (int i = 0; i < height; ++i) {
+            int16_t* m1 = map1 + (size_t)i * width * 2;
+            uint16_t* m2 = map2 + (size_t)i * width;
+            double X = i * ir[1] + ir[2], Y = i * ir[4] + ir[5], Wc = i * ir[7] + ir[8];
+            for (int j = 0; j < width;) {
+                const bool vec = j < vec_cols;
+                const int lanes = vec ? 8 : 1;
+                for (int l = 0; l < lanes; ++l, ++j) {
+                    const double _x = vec ? X + (double)l * ir[0] : X, _y = vec ? Y + (double)l * ir[3] : Y,
+                                 _w = vec ? Wc + (double)l * ir[6] : Wc;
+                    const double w = 1. / _w, x = _x * w, y = _y * w;
+                    const double x2 = x * x, y2 = y * y;
+                    const double r2 = x2 + y2, _2xy = 2 * x * y;
+                    const double kr = (1 + ((k3 * r2 + k2) * r2 + k1) * r2) / (1 + ((k6 * r2 + k5) * r2 + k4) * r2);
+                    const double xd = x * kr + p1 * _2xy + p2 * (r2 + 2 * x2);
+                    const double yd = y * kr + p1 * (r2 + 2 * y2) + p2 * _2xy;
+                    store_map(fx * xd + u0, fy * yd + v0, vec, m1 + 2 * j, m2 + j);
+                }
+                X += (double)lanes * ir[0];
+                Y += (double)lanes * ir[3];
+                Wc += (double)lanes * ir[6];
+            }
+        }
+    } else {
+        // cv::fisheye::initUndistortRectifyMap: one scalar loop, the row's X, Y, W accumulated pixel by pixel
+        for (int i = 0; i < height; ++i) {
+            int16_t* m1 = map1 + (size_t)i * width * 2;
+            uint16_t* m2 = map2 + (size_t)i * width;
+            double _x = i * ir[1] + ir[2], _y = i * ir[4] + ir[5], _w = i * ir[7] + ir[8];
+            for (int j = 0; j < width; ++j) {
+                double u, v;
+                if (_w <= 0) {
+                    u = (_x > 0) ? -INFINITY : INFINITY;
+                    v = (_y > 0) ? -INFINITY : INFINITY;
+                } else {
+                    const double x = _x / _w, y = _y / _w;
+                    const double r = sqrt(x * x + y * y);
+                    const double theta = atan(r);
+                    const double theta2 = theta * theta, theta4 = theta2 * theta2, theta6 = theta4 * theta2,
+                                 theta8 = theta4 * theta4;
+                    const double theta_d = theta * (1 + k[0] * theta2 + k[1] * theta4 + k[2] * theta6 + k[3] * theta8);
+                    const double scale = (r == 0) ? 1.0 : theta_d / r;
+                    u = fx * x * scale + u0;
+                    v = fy * y * scale + v0;
+                }
+                store_map(u, v, false, m1 + 2 * j, m2 + j);
+                _x += ir[0];
+                _y += ir[3];
+                _w += ir[6];
+            }
+        }
+    }
+    return 0;
+}
+
+PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, const int16_t* map1_l, const uint16_t* map2_l,
+                                     const int16_t* map1_r, const uint16_t* map2_r) {
+    if (!ctx) return nullptr;
+    LOCK(ctx);
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) {
+        fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+        return nullptr;
+    }
+    if (!map1_l || !map2_l || !map1_r || !map2_r) {
+        fail(ctx, PLSTVO_E_INVALID, "null map");
+        return nullptr;
+    }
+    if (cudaSetDevice(ctx->device) != cudaSuccess) {
+        fail(ctx, PLSTVO_E_CUDA, "cudaSetDevice failed");
+        return nullptr;
+    }
+    PlRectifier* r = new PlRectifier();
+    r->ctx = ctx;
+    r->width = width;
+    r->height = height;
+    const size_t N = (size_t)width * height;
+    const bool shared = map1_l == map1_r && map2_l == map2_r;
+    const int16_t* m1[2] = {map1_l, map1_r};
+    const uint16_t* m2[2] = {map2_l, map2_r};
+    for (int side = 0; side < (shared ? 1 : 2); ++side) {
+        cudaError_t e = r->map1[side].ensure(N * 4);
+        if (e == cudaSuccess) e = r->map2[side].ensure(N * 2);
+        if (e == cudaSuccess) e = cudaMemcpy(r->map1[side].p, m1[side], N * 4, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy(r->map2[side].p, m2[side], N * 2, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            ctx->err = std::string("plstvo_rectifier_create: ") + cudaGetErrorString(e);
+            delete r;
+            return nullptr;
+        }
+        r->m1[side] = r->map1[side].as<const short2>();
+        r->m2[side] = r->map2[side].as<const uint16_t>();
+    }
+    if (shared) {
+        r->m1[1] = r->m1[0];
+        r->m2[1] = r->m2[0];
+    }
+    return r;
+}
+
+void plstvo_rectifier_destroy(PlRectifier* rect) {
+    if (!rect) return;
+    {
+        LOCK(rect->ctx);   // no call of the context is using the maps once the lock is held: every call that reads them blocks
+        cudaSetDevice(rect->ctx->device);
+        rect->map1[0].release(); rect->map1[1].release(); rect->map2[0].release(); rect->map2[1].release();
+    }
+    delete rect;
+}
+
+int plstvo_rectify_batch(PlContext* ctx, const PlRectifier* rect, int B, const uint8_t* img_l, const uint8_t* img_r,
+                         uint8_t* out_l, uint8_t* out_r) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!rect || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null rectifier or negative B");
+    if (rect->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the rectifier belongs to another context");
+    if (B == 0) return 0;
+    if (!img_l || !img_r || !out_l || !out_r) return fail(ctx, PLSTVO_E_INVALID, "null image");
+    cudaStream_t s = ctx->s_main;
+    const uint8_t* d_out = nullptr;
+    if (const int rc = rectify_enqueue(ctx, rect, 2 * B, B, {ImgPart{img_l, B}, ImgPart{img_r, B}}, s, &d_out)) return rc;
+    const size_t bytes = (size_t)B * rect->width * rect->height;
+    CK(ctx, cudaMemcpyAsync(out_l, d_out, bytes, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaMemcpyAsync(out_r, d_out + bytes, bytes, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return 0;
+}
+
+int plstvo_rectify_kernel_times(PlContext* ctx, float* ms1) {
+    if (!ctx || !ms1) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ctx->rect_ran) return fail(ctx, PLSTVO_E_INVALID, "no rectify call on this context yet");
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, cudaEventElapsedTime(ms1, ctx->rect_ev[0], ctx->rect_ev[1]));
+    return 0;
+}
+
+}  // extern "C"

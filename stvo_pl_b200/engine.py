@@ -31,7 +31,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                            "(there is no CPU fallback).")
     L = C.CDLL(path)
     vp, i32p, u8p, dp, fp = C.c_void_p, T.c_int32_p, T.c_uint8_p, T.c_double_p, T.c_float_p
-    u32p = C.POINTER(C.c_uint32)
+    u32p, i16p, u16p = C.POINTER(C.c_uint32), C.POINTER(C.c_int16), C.POINTER(C.c_uint16)
     cam, cfg = C.POINTER(T.PlCamera), C.POINTER(T.PlConfig)
     fb, mb = C.POINTER(T.PlFrameBatch), C.POINTER(T.PlMatchedBatch)
     sig = {
@@ -117,6 +117,19 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                                                               C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
                                                               C.POINTER(T.PlLsdConfig), C.POINTER(T.PlStereoImages), vp, vp, i32p]),
         "plstvo_track_stereo_images_stage_times": (C.c_int, [vp, fp]),
+        "plstvo_init_undistort_rectify_map": (C.c_int, [C.POINTER(T.PlRectifyModel), C.c_int, C.c_int, i16p, u16p]),
+        "plstvo_rectifier_create": (vp, [vp, C.c_int, C.c_int, i16p, u16p, i16p, u16p]),
+        "plstvo_rectifier_destroy": (None, [vp]),
+        "plstvo_rectify_batch": (C.c_int, [vp, vp, C.c_int, u8p, u8p, u8p, u8p]),
+        "plstvo_rectify_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_track_stereo_raw_images_batch": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                           C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                           C.POINTER(T.PlLsdConfig), vp, C.POINTER(T.PlStereoImages),
+                                                           C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_track_stereo_raw_images_sequence": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                              C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                              C.POINTER(T.PlLsdConfig), vp, C.POINTER(T.PlStereoImages), vp, vp,
+                                                              i32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -141,11 +154,39 @@ EXPORTED_SYMBOLS = [
     "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
     "plstvo_lsd_kernel_times", "plstvo_track_stereo_images_batch",
     "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_lsd_batch", "plstvo_track_stereo_images_lsd_sequence",
-    "plstvo_track_stereo_images_stage_times"]
+    "plstvo_track_stereo_images_stage_times", "plstvo_init_undistort_rectify_map", "plstvo_rectifier_create",
+    "plstvo_rectifier_destroy", "plstvo_rectify_batch", "plstvo_rectify_kernel_times", "plstvo_track_stereo_raw_images_batch",
+    "plstvo_track_stereo_raw_images_sequence"]
 
 
 def _p(a: Optional[np.ndarray], typ):
     return C.cast(None, typ) if a is None else a.ctypes.data_as(typ)
+
+
+def init_undistort_rectify_map(model: int, K, D, R, P, width: int, height: int, lib: Optional[C.CDLL] = None):
+    """plstvo_init_undistort_rectify_map (host code, no GPU): (map1 int16[h, w, 2], map2 uint16[h, w]) as OpenCV 4.13 builds
+    them for CV_16SC2.  model: T.RECTIFY_PINHOLE or T.RECTIFY_FISHEYE."""
+    lib = lib or load_library()
+    m = T.rectify_model(model, K, D, R, P)
+    map1 = np.zeros((max(height, 0), max(width, 0), 2), np.int16)
+    map2 = np.zeros((max(height, 0), max(width, 0)), np.uint16)
+    rc = lib.plstvo_init_undistort_rectify_map(C.byref(m), width, height, _p(map1, C.POINTER(C.c_int16)),
+                                               _p(map2, C.POINTER(C.c_uint16)))
+    if rc < 0:
+        raise PlstvoError(rc, "plstvo_init_undistort_rectify_map rejected the model or the size")
+    return map1, map2
+
+
+class Rectifier:
+    """A PlRectifier: a rig's maps resident in HBM (Engine.rectifier_create); close() or the owning Engine frees it."""
+
+    def __init__(self, lib: C.CDLL, handle, width: int, height: int):
+        self.lib, self.handle, self.width, self.height = lib, handle, width, height
+
+    def close(self):
+        if self.handle:
+            self.lib.plstvo_rectifier_destroy(self.handle)
+            self.handle = None
 
 
 def bind_to_gpu_numa(device: int) -> Optional[int]:
@@ -275,9 +316,12 @@ class Engine:
             raise PlstvoError(rc, "plstvo_create failed: no sm_90 CUDA device visible (no CPU fallback exists)")
         self.ctx = ctx
         self.pinned = PinnedPool(self.lib)
+        self._rectifiers = []
 
     def close(self):
         if self.ctx:
+            for r in self._rectifiers:
+                r.close()
             self.pinned.close()
             self.lib.plstvo_destroy(self.ctx)
             self.ctx = None
@@ -658,6 +702,80 @@ class Engine:
             self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
             None if lcfg is None else C.byref(lcfg), C.byref(fs), priors.ctypes.data if priors is not None else None,
             results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep
+        return results, n_stereo
+
+    # ---- rectification: PinholeStereoCamera::rectifyImagesLR ----
+    def rectifier_create(self, map1_l, map2_l, map1_r=None, map2_r=None) -> Rectifier:
+        """Uploads a rig's CV_16SC2 map pairs once (map1 int16[h, w, 2], map2 uint16[h, w]); the right pair defaults to the
+        left one, which is then held once (the reference's cam_d0 branch)."""
+        m1l = np.ascontiguousarray(map1_l, np.int16)
+        m2l = np.ascontiguousarray(map2_l, np.uint16)
+        m1r = m1l if map1_r is None else np.ascontiguousarray(map1_r, np.int16)
+        m2r = m2l if map2_r is None else np.ascontiguousarray(map2_r, np.uint16)
+        H, W = m2l.shape
+        if m1l.shape != (H, W, 2) or m1r.shape != (H, W, 2) or m2r.shape != (H, W):
+            raise ValueError("map shapes differ")
+        i16p, u16p = C.POINTER(C.c_int16), C.POINTER(C.c_uint16)
+        h = self.lib.plstvo_rectifier_create(self.ctx, W, H, _p(m1l, i16p), _p(m2l, u16p), _p(m1r, i16p), _p(m2r, u16p))
+        if not h:
+            raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
+        r = Rectifier(self.lib, h, W, H)
+        self._rectifiers.append(r)
+        return r
+
+    def rectifier_destroy(self, rect: Rectifier):
+        rect.close()
+        self._rectifiers = [r for r in self._rectifiers if r is not rect]
+
+    def rectify_batch(self, rect: Rectifier, img_l, img_r):
+        """rectifyImagesLR on B pairs: (rectified left uint8[B, H, W], rectified right)."""
+        il = np.ascontiguousarray(img_l, np.uint8)
+        ir = np.ascontiguousarray(img_r, np.uint8)
+        if il.ndim == 2:
+            il, ir = il[None], ir[None]
+        if il.shape != ir.shape or il.shape[1:] != (rect.height, rect.width):
+            raise ValueError("images must be uint8[B, H, W] of the rectifier's size, both sides alike")
+        ol, orr = np.empty_like(il), np.empty_like(ir)
+        self._ck(self.lib.plstvo_rectify_batch(self.ctx, rect.handle, il.shape[0], _p(il, T.c_uint8_p), _p(ir, T.c_uint8_p),
+                                               _p(ol, T.c_uint8_p), _p(orr, T.c_uint8_p)))
+        return ol, orr
+
+    def rectify_kernel_times(self) -> float:
+        """Device ms of the last remap (rectify_batch or a raw-images call)."""
+        ms = np.zeros(1, np.float32)
+        self._ck(self.lib.plstvo_rectify_kernel_times(self.ctx, _p(ms, T.c_float_p)))
+        return float(ms[0])
+
+    def track_stereo_raw_images_batch(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], prev: dict, curr: dict,
+                                      priors=None, results=None):
+        """track_stereo_images_lsd_batch on raw (distorted) images: rect's remap runs on the device first; rect None: the
+        _lsd_ call.  Returns (results, n_stereo[B, 4])."""
+        ps, keep_p = T.stereo_images_as_c(prev)
+        cs, keep_c = T.stereo_images_as_c(curr)
+        B = ps.B
+        if results is None:
+            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((B, 4), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_raw_images_batch(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
+            None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle, C.byref(ps), C.byref(cs),
+            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep_p, keep_c
+        return results, n_stereo
+
+    def track_stereo_raw_images_sequence(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], frames: dict,
+                                         priors=None, results=None):
+        """track_stereo_images_lsd_sequence on raw images, rectified on the device.  Returns (results, n_stereo[NF, 2])."""
+        fs, keep = T.stereo_images_as_c(frames)
+        NF = fs.B
+        if results is None:
+            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((NF, 2), np.int32)
+        self._ck(self.lib.plstvo_track_stereo_raw_images_sequence(
+            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
+            None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle, C.byref(fs),
+            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
         del keep
         return results, n_stereo
 

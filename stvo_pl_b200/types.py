@@ -98,6 +98,31 @@ def default_lsd_config(n_features: int = 300, **kw) -> "PlLsdConfig":
     return c
 
 
+RECTIFY_PINHOLE, RECTIFY_FISHEYE = 0, 1
+
+
+class PlRectifyModel(C.Structure):
+    """One camera's undistort-rectify model (PlRectifyModel, include/plstvo.h): model 0 pinhole / 1 fisheye, n_dist
+    coefficients of D, K 3x3, R 3x3 and P 3x4, row-major; every field double."""
+    _fields_ = [("model", C.c_double), ("n_dist", C.c_double), ("K", C.c_double * 9), ("D", C.c_double * 8),
+                ("R", C.c_double * 9), ("P", C.c_double * 12)]
+
+
+def rectify_model(model: int, K, D, R, P) -> "PlRectifyModel":
+    """PlRectifyModel from arrays: K 3x3, D of 4 / 5 / 8 coefficients, R 3x3, P 3x3 or 3x4 (a 3x3 P gets a zero column)."""
+    D = np.asarray(D, np.float64).ravel()
+    P = np.asarray(P, np.float64)
+    if P.shape == (3, 3):
+        P = np.hstack([P, np.zeros((3, 1))])
+    m = PlRectifyModel()
+    m.model, m.n_dist = float(model), float(D.size)
+    m.K[:] = np.asarray(K, np.float64).ravel().tolist()
+    m.D[:min(D.size, 8)] = D[:8].tolist()   # a longer D keeps its count, which the library rejects
+    m.R[:] = np.asarray(R, np.float64).ravel().tolist()
+    m.P[:] = P.ravel().tolist()
+    return m
+
+
 ORB_HARRIS_SCORE, ORB_FAST_SCORE = 0, 1
 
 
