@@ -56,16 +56,8 @@ __global__ void pack_records_kernel(MatchedDev m, PlCamera cam, int B, int n_pt,
         float4* base = ls + 4 * (size_t)(l0 + t * GS_LS_TILE);
         const size_t a = (size_t)i;
         const double su = m.ls_spl[2 * a], sv = m.ls_spl[2 * a + 1], eu = m.ls_epl[2 * a], ev = m.ls_epl[2 * a + 1];
-        const double lx = eu - su, ly = ev - sv;
         double oa, ob, oc;
-        if (fabs(su - eu) < 1.0) {          // vertical (:515-544): lambda = (v - sv) / ly
-            oa = 0.0; ob = 1.0 / ly; oc = -sv / ly;
-        } else if (fabs(sv - ev) < 1.0) {   // horizontal (:545-574): lambda = (u - su) / lx
-            oa = 1.0 / lx; ob = 0.0; oc = -su / lx;
-        } else {                            // generic (:575-612): foot of the perpendicular, then (x - su) / lx
-            const double ca = sv - ev, cb = eu - su, cc = su * ev - eu * sv, lxy = 1.0 / (ca * ca + cb * cb);
-            oa = (cb * cb * lxy) / lx; ob = (-(ca * cb) * lxy) / lx; oc = (-(ca * cc) * lxy - su) / lx;
-        }
+        overlap_coeffs(su, sv, eu, ev, oa, ob, oc);
         gs_pack_line(c, m.ls_sP[3 * a], m.ls_sP[3 * a + 1], m.ls_sP[3 * a + 2], m.ls_eP[3 * a], m.ls_eP[3 * a + 1], m.ls_eP[3 * a + 2],
                      m.ls_le_obs[3 * a], m.ls_le_obs[3 * a + 1], m.ls_le_obs[3 * a + 2], oa, ob, oc, sqrt(m.ls_sigma2[a]),
                      !(m.ls_inlier && !m.ls_inlier[a]), base[r], base[cnt + r], base[2 * cnt + r], base[3 * cnt + r]);

@@ -67,11 +67,44 @@ struct GsAccScalar {
     }
 };
 
-__device__ __forceinline__ float gs_overlap_l(float ls, float le) {   // :601-610 on the two parameters
-    const float lo = fminf(ls, le), hi = fmaxf(ls, le);
-    float ov = fminf(hi, 1.f) - fmaxf(lo, 0.f);                       // covered part of [0, 1]
+// :601-610 on the two parameters.  lo / hi are std::min / std::max, NaN order included: a NaN ls makes the overlap NaN, a NaN
+// le is dropped (the reference then compares ls with itself).
+__device__ __forceinline__ float gs_overlap_l(float ls, float le) {
+    const float lo = (le < ls) ? le : ls, hi = (ls < le) ? le : ls;
+    float ov = ((hi > 1.f) ? 1.f : hi) - ((lo < 0.f) ? 0.f : lo);     // covered part of [0, 1]
     ov = (hi < 0.f || lo > 1.f) ? 0.f : ov;
     return ov;
+}
+
+// StereoFrame::lineSegmentOverlap (src/stereoFrame.cpp:510-616): for a fixed previous-frame segment (su, sv)-(eu, ev) the
+// parameter lambda of a projected endpoint (u, v) is affine in (u, v) in all three branches, lambda = oa u + ob v + oc; the
+// coefficients are computed once per matched line when the list is built.  One exception: in the vertical branch a segment
+// with ly == 0 (zero length, or |lx| < 1 and ly == 0) has lambda = (v - sv) / ly = +-inf, NaN where v == sv exactly, which no
+// finite affine form reproduces.  Its coefficients are ob = 1 / ly = +-inf, oc = -sv, and lambda = ob (v + oc)
+// (overlap_lambda / gs_lambda): v + (-sv) rounds exactly as v - sv does.
+__device__ __forceinline__ void overlap_coeffs(double su, double sv, double eu, double ev, double& oa, double& ob,
+                                               double& oc) {
+    const double lx = eu - su, ly = ev - sv;
+    if (fabs(su - eu) < 1.0) {          // vertical (:515-544): lambda = (v - sv) / ly
+        oa = 0.0; ob = 1.0 / ly; oc = isinf(ob) ? -sv : -sv / ly;
+    } else if (fabs(sv - ev) < 1.0) {   // horizontal (:545-574): lambda = (u - su) / lx
+        oa = 1.0 / lx; ob = 0.0; oc = -su / lx;
+    } else {                            // generic (:575-612): foot of the perpendicular, then (x - su) / lx
+        const double a = sv - ev, b = eu - su, c = su * ev - eu * sv;
+        const double lxy = 1.0 / (a * a + b * b);
+        oa = (b * b * lxy) / lx;
+        ob = (-(a * b) * lxy) / lx;
+        oc = (-(a * c) * lxy - su) / lx;
+    }
+}
+// lambda of the projected endpoint (u, v) from overlap_coeffs' coefficients
+__device__ __forceinline__ double overlap_lambda(double oa, double ob, double oc, double u, double v) {
+    return isinf(ob) ? ob * (v + oc) : oa * u + ob * v + oc;
+}
+// the same on a packed record: (oa, ob) = d.x, d.y, lam0 = the record's lambda term at the identity pose (gs_pack_line), which
+// holds v0 - sv where ob is infinite; (du, dv) = the endpoint's projection change
+__device__ __forceinline__ float gs_lambda(float oa, float ob, float lam0, float du, float dv) {
+    return isinf(ob) ? ob * (dv + lam0) : fmaf(oa, du, fmaf(ob, dv, lam0));
 }
 
 // The pose as the evaluator holds it: r[] = the top three rows of DT with the identity taken off the rotation, (R - I | t),
@@ -92,6 +125,7 @@ __device__ __forceinline__ float gs_pose_entry(double v, int i) { return (float)
 //   point, 32 B : {x/z, y/z, z, sqrt(sigma2)} {du0, dv0, inlier, -}                du0 = fx x/z + cx - u_obs
 //   line,  64 B : {sx/sz, sy/sz, sz, sqrt(sigma2)} {ex/ez, ey/ez, ez, inlier} {l0, l1, ds0, de0} {oa, ob, lam_s0, lam_e0}
 //                 ds0 = l . (projection of sP at identity, 1), lam_s0 = (oa, ob, oc) . (that projection, 1)
+//                 (lam_s0 = v0 + oc = v0 - sv where ob is infinite: see overlap_coeffs)
 struct GsCamD {
     double fx, fy, cx, cy;
 };
@@ -109,7 +143,10 @@ __device__ __forceinline__ void gs_pack_line(const GsCamD& c, double sx, double 
     A = make_float4((float)sxn, (float)syn, (float)sz, (float)lss);
     B = make_float4((float)exn, (float)eyn, (float)ez, inl ? 1.f : 0.f);
     C = make_float4((float)l0, (float)l1, (float)(l0 * spu + l1 * spv + l2), (float)(l0 * epu + l1 * epv + l2));
-    D = make_float4((float)oa, (float)ob, (float)(oa * spu + ob * spv + oc), (float)(oa * epu + ob * epv + oc));
+    if (isinf(ob))   // ly == 0 in the vertical branch (overlap_coeffs): the lambda terms are v0 - sv, gs_lambda scales them by ob
+        D = make_float4((float)oa, (float)ob, (float)(spv + oc), (float)(epv + oc));
+    else
+        D = make_float4((float)oa, (float)ob, (float)(oa * spu + ob * spv + oc), (float)(oa * epu + ob * epv + oc));
 }
 
 // one 3D point through the pose: camera-frame coordinates and the change of its projection against the identity pose
@@ -160,7 +197,7 @@ __device__ __forceinline__ void gs_line(const GsPose& P, const float4 a, const f
     gs_jac<true>(e.X, e.Y, e.Z, ke * c.x, ke * c.y, J);
     const float r = n * a.w;
     float w = gs_rcp(fmaf(r, r, 1.f));
-    w *= gs_overlap_l(fmaf(d.x, s.du, fmaf(d.y, s.dv, d.z)), fmaf(d.x, e.du, fmaf(d.y, e.dv, d.w)));   // :664-670
+    w *= gs_overlap_l(gs_lambda(d.x, d.y, d.z, s.du, s.dv), gs_lambda(d.x, d.y, d.w, e.du, e.dv));   // :664-670
     acc.add(J, r, use ? w : 0.f, use ? 1.f : 0.f);
 }
 

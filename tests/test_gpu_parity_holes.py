@@ -88,22 +88,29 @@ def test_degenerate_segments_through_the_streamed_evaluator(engine, oracle):
 
 
 def test_zero_length_previous_segments(engine, oracle):
-    """A zero-length previous segment divides by l(1) = 0 in the vertical branch (src/stereoFrame.cpp:515-544): the lambdas
-    are +-inf (NaN only when the projected end point has exactly the same v), the overlap comes out as 0 or 1.  The GPU
-    must take the same route: identical flags and pose, also against the reference's compiled code."""
+    """The NaN path.  A zero-length previous segment divides by l(1) = 0 in the vertical branch (src/stereoFrame.cpp:515-544):
+    lambda = (v - sv) / 0 is +-inf, and NaN where the projected end point has exactly the same v.  From the identity pose the
+    synthetic end points project exactly onto spl, so every such line's weight is NaN, so is the error, and every problem
+    fails: the oracle's verdict is good = 0.  The GPU must fail the same way: the oracle's status, verdict, iteration counts,
+    flags and (identity) pose, also against the reference's compiled code.  The same segments started from a motion-model
+    prior, where they are solved, are test_gpu_overlap_degenerate.py's."""
     cfg = T.kitti_config()
     m, Tgt, cam, *_ = _matched(oracle, "kitti", 3, cfg, n_pt=200, n_ls=120, overlap=1.0)
     deg, _, _, nz = _degenerate(m, np.random.default_rng(13), 0.1, 0.1, 0.4)
     assert nz > 60
     res, ip, il = engine.optimize_pose(cam, cfg, deg)
     rc, res_o, ip_o, il_o = oracle.optimize_pose(cam, cfg, deg)
+    assert (res_o["good"] == 0).all(), res_o["good"]
     np.testing.assert_array_equal(ip, ip_o)
     np.testing.assert_array_equal(il, il_o)
     ref = _ref_or_none()
     res_r = ref.optimize_pose(cam, cfg, deg)[1] if ref else None
     for p in range(3):
+        for k in ("status", "good", "iters_stage1", "iters_stage2"):
+            assert res[p][k] == res_o[p][k], (p, k, res[p][k], res_o[p][k])
         _same_pose(res[p], res_o[p])
         if res_r is not None:
+            assert res[p]["status"] == res_r[p]["status"]
             _same_pose(res[p], res_r[p])
 
 
