@@ -526,6 +526,50 @@ int plstvo_track_stereo_raw_images_sequence(PlContext* ctx, const PlCamera* cam,
                                             const PlStereoImages* frames, const PlPrior* priors, PlPoseResult* results,
                                             int32_t* n_stereo /* [B+1][2] */);
 
+/* ---- stereo sessions: StereoFrameHandler's prev_frame kept on the device for many independent streams
+ * (app/imagesStVO.cpp:88-124, src/stereoFrameHandler.cpp:35-102) ----
+ * A session holds, for each of n_streams independent stereo streams (cameras), the previous frame's stereo features in HBM,
+ * as the tracker reads them in the previous-frame role: per kept stereo point 64 bytes (P 24, sigma2 8, descriptor 32), per
+ * kept stereo line 124 bytes (start / end points 16 + 16, sP / eP 24 + 24, sigma2 8, level 4, descriptor 32).  The session
+ * has two such pools (the kept frames, and the next call's), each grown on demand with a quarter of slack; it keeps no
+ * images, on the host or the device.  Features carry no state from one frame to the next in the reference (matchF2FPoints /
+ * matchF2FLines flag copies, updateFrame moves curr_frame into prev_frame), so a frame's stereo features are computed once
+ * and serve as the next pair's previous frame unchanged.
+ * The configs are copied at creation and fixed for the session's life (the kept records depend on cam and scfg, the
+ * descriptors on ocfg and lcfg).  lcfg may be NULL where cfg->has_lines is 0.  rect (NULL: the images are already rectified)
+ * must belong to ctx and outlive the session.  Returns NULL on failure (a null argument, n_streams < 1, the ORB / LSD config
+ * checks of the _lsd_ calls, a bad grid, a rectifier of another context or of another size; plstvo_last_error says which).
+ * Destroy a session before its context; plstvo_stereo_session_device_bytes is its device memory (pools and call tables). */
+typedef struct PlStereoSession PlStereoSession;
+PlStereoSession* plstvo_stereo_session_create(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                              const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                              const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlRectifier* rect,
+                                              int n_streams);
+void    plstvo_stereo_session_destroy(PlStereoSession* s);
+int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* s);
+/* StereoFrameHandler::initialize(img_l, img_r) for streams ids[0 .. n) (any subset of [0, n_streams), any order, no
+ * duplicates): frames (B = n, the _lsd_ calls' frames: key-line fields NULL) are detected, go through the stereo step and
+ * replace each named stream's kept frame.  frames->fast_th[k] is stream ids[k]'s FAST threshold for its frame (0 or NULL:
+ * ocfg->fast_threshold).  n_stereo [n][2] (optional): each new frame's stereo points, lines. */
+int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* s, int n, const int32_t* ids,
+                                     const PlStereoImages* frames, int32_t* n_stereo);
+/* insertStereoPair's f2fTracking + optimizePose for streams ids[0 .. n), each of which must hold a frame: the new frame k is
+ * tracked against stream ids[k]'s kept frame and then replaces it; streams not named keep their frame untouched.  results and
+ * n_stereo ([n][4]: the kept frame's stereo points, lines, then the new frame's) equal, byte for byte, those of
+ * plstvo_track_stereo_raw_images_batch with the session's rect and configs, prev = each named stream's kept images at the
+ * threshold they were detected with, curr = frames, the same priors ([n] or NULL) and the same order (rect NULL:
+ * plstvo_track_stereo_images_lsd_batch).  Only the 2 n new images are uploaded, rectified, detected and described, and only
+ * the new frames go through the stereo step; the kept frames are gathered on the device (session_gather_kernel).
+ * Both calls return 0 or an error code, and a failed call leaves every stream's kept frame as it was and the context usable.
+ * PLSTVO_E_INVALID: a null session, a session of another context, ids null, an id outside [0, n_streams), a duplicate id,
+ * insert on a stream with no frame, more than 65535 images in the call (2 n), and every PLSTVO_E_INVALID of the _lsd_ /
+ * raw-images calls; PLSTVO_E_SIZE: frames->B != n, and that call's size codes; PLSTVO_E_TOO_LARGE: its feature limits, or
+ * more than INT_MAX kept rows; PLSTVO_E_CUDA: among others, when a pool cannot be grown.  insert updates what
+ * plstvo_track_stereo_images_stage_times and the ORB / LSD / LBD / rectify kernel-time calls report, as the images calls do
+ * (initialize too, its tracking slot then empty). */
+int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* s, int n, const int32_t* ids, const PlStereoImages* frames,
+                                 const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

@@ -1,6 +1,7 @@
 // plstvo.hpp — header-only C++17 host layer over the C-ABI (plstvo.h): RAII context plus a StereoFrameHandler with
-// the reference's method names (include/stereoFrameHandler.h:41-54) for frames of pre-extracted features, and a
-// StereoImageHandler with the same names for stereo images alone.  It has no
+// the reference's method names (include/stereoFrameHandler.h:41-54) for frames of pre-extracted features, a
+// StereoImageHandler with the same names for stereo images alone, and a StereoStreamsHandler that runs one such handler per
+// camera over a StereoSession (each stream's previous frame kept on the device).  It has no
 // Eigen / OpenCV dependency; the Eigen/OpenCV shim that makes it a drop-in for libstvo.so is in INTEGRATION.md.
 #pragma once
 #include <algorithm>
@@ -793,33 +794,97 @@ private:
     bool has_prev_ = false;
 };
 
+// A PlStereoSession (plstvo_stereo_session_create): n_streams stereo streams, each stream's previous frame kept in HBM as its
+// stereo features, so that a frame is detected and described once.  The configs are copied and fixed; rect (optional) must
+// outlive the session.  Destroy it before its Context.
+class StereoSession {
+public:
+    StereoSession(Context& c, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc, const PlStereoConfig& sc,
+                  const PlOrbDetectConfig& oc, const PlLsdConfig& lc, int n_streams, const Rectifier* rect = nullptr)
+        : c_(c), n_streams_(n_streams) {
+        s_ = plstvo_stereo_session_create(c.get(), &cam, &cfg, &mc, &sc, &oc, &lc, rect ? rect->get() : nullptr, n_streams);
+        if (!s_) throw Error(PLSTVO_E_INVALID, plstvo_last_error(c.get()));
+    }
+    ~StereoSession() { plstvo_stereo_session_destroy(s_); }
+    StereoSession(const StereoSession&) = delete;
+    StereoSession& operator=(const StereoSession&) = delete;
+    // initialize for streams ids[0 .. n): n_stereo [n][2] (optional)
+    void initialize(int n, const int32_t* ids, const PlStereoImages& frames, int32_t* n_stereo = nullptr) {
+        c_.check(plstvo_stereo_session_initialize(c_.get(), s_, n, ids, &frames, n_stereo));
+    }
+    // insertStereoPair + optimizePose for streams ids[0 .. n) against their kept frames: results [n], n_stereo [n][4] (optional)
+    void insert(int n, const int32_t* ids, const PlStereoImages& frames, const PlPrior* priors, PlPoseResult* results,
+                int32_t* n_stereo = nullptr) {
+        c_.check(plstvo_stereo_session_insert(c_.get(), s_, n, ids, &frames, priors, results, n_stereo));
+    }
+    int streams() const { return n_streams_; }
+    int64_t deviceBytes() const { return plstvo_stereo_session_device_bytes(s_); }
+    PlStereoSession* get() const { return s_; }
+private:
+    Context& c_;
+    PlStereoSession* s_ = nullptr;
+    int n_streams_ = 0;
+};
+
+namespace detail {
+// n frames of one size, copied into the contiguous arrays a PlStereoImages of images alone points at
+struct StereoImagesBatch {
+    std::vector<uint8_t> img_l, img_r;
+    std::vector<int32_t> th;
+    PlStereoImages view{};
+    void pack(int width, int height, const std::vector<const uint8_t*>& l, const std::vector<const uint8_t*>& r,
+              const std::vector<int32_t>& fast_th, const char* who) {
+        const size_t px = (size_t)width * (size_t)height, n = l.size();
+        if (r.size() != n || fast_th.size() != n) throw Error(PLSTVO_E_INVALID, std::string(who) + ": ids and images differ in number");
+        img_l.resize(n * px);
+        img_r.resize(n * px);
+        for (size_t k = 0; k < n; ++k) {
+            if (!l[k] || !r[k]) throw Error(PLSTVO_E_INVALID, std::string(who) + ": null image");
+            std::copy(l[k], l[k] + px, img_l.begin() + k * px);
+            std::copy(r[k], r[k] + px, img_r.begin() + k * px);
+        }
+        th = fast_th;
+        view = PlStereoImages{(int32_t)n, width, height, img_l.data(), img_r.data(), th.data()};
+    }
+};
+// the handler's ORB config: a frame's fast_th of 0 stands for the config's threshold; with that set to 0 too, every frame is
+// detected with the threshold the handler chose, 0 included (updateFastThreshold returns 0 when fast_min_th <= 0), as in the
+// reference
+inline PlOrbDetectConfig handlerOrbConfig(PlOrbDetectConfig oc) {
+    oc.fast_threshold = 0;
+    return oc;
+}
+}  // namespace detail
+
 // The same surface over images alone, as app/imagesStVO.cpp:88-97 drives the reference's handler: initialize(img_l, img_r, idx)
 // and insertStereoPair(img_l, img_r, idx) take two grey images of cam's size (row-major, width * height bytes each), then
-// optimizePose(), updateFrame() (with updateFastThreshold), needNewKF() and currFrameIsKF() as above.  The handler keeps
-// copies of the previous frame's images and the FAST threshold they were detected with; each insertStereoPair is one
-// plstvo_track_stereo_images_lsd_batch call with one pair: the stored images at their threshold, the new ones at the current
-// orb_fast_th, and the prior f2fTracking builds from prev_frame.  The C-ABI keeps no frame between calls, so the previous
-// frame's images are detected and described again on every call: about twice the detection work of the reference's handler,
-// which keeps the previous frame's features.  prev_frame / curr_frame hold the pose state; their feature arrays stay empty.
+// optimizePose(), updateFrame() (with updateFastThreshold), needNewKF() and currFrameIsKF() as above.  It runs on a session
+// of one stream: initialize detects the frame at orb_fast_th and keeps its stereo features on the device; each
+// insertStereoPair is one plstvo_stereo_session_insert, which detects and describes the new images only, tracks them against
+// the kept frame with the prior f2fTracking builds from prev_frame, and keeps the new frame in its place.  The results equal
+// those of plstvo_track_stereo_raw_images_batch on (previous images, new images), byte for byte.  As in the reference's loop,
+// updateFrame follows each insertStereoPair: the device already holds the new frame as the previous one.  prev_frame /
+// curr_frame hold the pose state; their feature arrays stay empty.
 class StereoImageHandler {
 public:
     StereoImageHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
                        const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
                        const HandlerConfig& hcfg = HandlerConfig{})
-        : ctx_(ctx), cam_(cam), cfg_(cfg), mc_(mc), sc_(sc), oc_(oc), lc_(lc), hcfg_(hcfg) {}
+        : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, 1) {}
     // Raw images, as Dataset::nextFrame feeds the reference's handler (src/dataset.cpp:147-157): initialize / insertStereoPair
-    // take the camera's images before rectifyImagesLR, and each call rectifies them on the device under rect
-    // (plstvo_track_stereo_raw_images_batch); cam is the rectified camera (StereoRectification::cam).  rect must outlive the
-    // handler.
+    // take the camera's images before rectifyImagesLR, and each call rectifies them on the device under rect; cam is the
+    // rectified camera (StereoRectification::cam).  rect must outlive the handler.
     StereoImageHandler(Context& ctx, const Rectifier& rect, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
                        const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
                        const HandlerConfig& hcfg = HandlerConfig{})
-        : ctx_(ctx), cam_(cam), cfg_(cfg), mc_(mc), sc_(sc), oc_(oc), lc_(lc), hcfg_(hcfg), rect_(rect.get()) {}
+        : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, 1, &rect) {}
 
     void initialize(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // src/stereoFrameHandler.cpp:35-52
         orb_fast_th = hcfg_.orb_fast_th;                 // :38
-        store(img_l, img_r, prev_l_, prev_r_);
-        prev_th_ = orb_fast_th;
+        images(img_l, img_r);
+        const int32_t id = 0;
+        session_.initialize(1, &id, frame_);
+        frame_ = PlStereoImages{};
         prev_frame = StereoFrame{};
         prev_frame.frame_idx = idx;
         for (int i = 0; i < 36; ++i) prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
@@ -828,23 +893,18 @@ public:
     }
     void insertStereoPair(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // :54-60
         if (!has_prev_) throw Error(PLSTVO_E_INVALID, "initialize() first");
-        store(img_l, img_r, curr_l_, curr_r_);
-        curr_th_ = orb_fast_th;
+        images(img_l, img_r);
         curr_frame = StereoFrame{};
         curr_frame.frame_idx = idx;
         f2fTracking();
     }
-    void f2fTracking() {                                 // :106-129, with both frames' feature extraction, fused with optimizePose
+    void f2fTracking() {                                 // :106-129, with the new frame's feature extraction, fused with optimizePose
+        if (!frame_.img_l) throw Error(PLSTVO_E_INVALID, "insertStereoPair() first");
         const PlPrior prior = priorOf(prev_frame);
-        const PlStereoImages prev{1, cam_.width, cam_.height, prev_l_.data(), prev_r_.data(), &prev_th_},
-                             curr{1, cam_.width, cam_.height, curr_l_.data(), curr_r_.data(), &curr_th_};
-        // a frame's fast_th of 0 stands for the config's threshold; with that set to 0 too, every frame is detected with the
-        // threshold the handler chose, 0 included (updateFastThreshold returns 0 when fast_min_th <= 0), as in the reference
-        PlOrbDetectConfig oc = oc_;
-        oc.fast_threshold = 0;
-        // without a rectifier this is plstvo_track_stereo_images_lsd_batch
-        ctx_.check(plstvo_track_stereo_raw_images_batch(ctx_.get(), &cam_, &cfg_, &mc_, &sc_, &oc, &lc_, rect_, &prev, &curr,
-                                                        &prior, &result_, n_stereo.data()));
+        const int32_t id = 0;
+        const PlStereoImages f = frame_;
+        frame_ = PlStereoImages{};
+        session_.insert(1, &id, f, &prior, &result_, n_stereo.data());
         n_inliers_pt = result_.n_matched_pt;             // :126-128
         n_inliers_ls = result_.n_matched_ls;
         n_inliers = n_inliers_pt + n_inliers_ls;
@@ -859,9 +919,6 @@ public:
         orb_fast_th = updateFastThreshold(hcfg_, orb_fast_th, curr_frame, n_inliers_pt);   // :66-86
         prev_frame = std::move(curr_frame);
         curr_frame = StereoFrame{};
-        prev_l_.swap(curr_l_);
-        prev_r_.swap(curr_r_);
-        prev_th_ = curr_th_;
     }
 
     bool needNewKF() { return kf.needNewKF(hcfg_, curr_frame); }
@@ -875,25 +932,118 @@ public:
     KeyframeTest kf;
 
 private:
-    void store(const uint8_t* img_l, const uint8_t* img_r, std::vector<uint8_t>& l, std::vector<uint8_t>& r) const {
+    // the caller's images for the next session call, detected at orb_fast_th (they are read during that call only)
+    void images(const uint8_t* img_l, const uint8_t* img_r) {
         if (!img_l || !img_r) throw Error(PLSTVO_E_INVALID, "StereoImageHandler: null image");
-        const size_t px = (size_t)cam_.width * (size_t)cam_.height;
-        l.assign(img_l, img_l + px);
-        r.assign(img_r, img_r + px);
+        th_ = orb_fast_th;
+        frame_ = PlStereoImages{1, cam_.width, cam_.height, img_l, img_r, &th_};
     }
-    Context& ctx_;
     PlCamera cam_;
-    PlConfig cfg_;
-    PlStereoMatchConfig mc_;
-    PlStereoConfig sc_;
-    PlOrbDetectConfig oc_;
-    PlLsdConfig lc_;
     HandlerConfig hcfg_;
+    StereoSession session_;
     PlPoseResult result_{};
-    std::vector<uint8_t> prev_l_, prev_r_, curr_l_, curr_r_;
-    int32_t prev_th_ = 0, curr_th_ = 0;
+    PlStereoImages frame_{};
+    int32_t th_ = 0;
     bool has_prev_ = false;
-    const PlRectifier* rect_ = nullptr;   // null: the images are already rectified
+};
+
+// Many StereoImageHandlers at once: one per stream (camera) of a session, each with the reference handler's state, and one
+// session call per initialize / insertStereoPairs over any subset of the streams.  Stream k behaves exactly as a
+// StereoImageHandler fed only stream k's images: the same thresholds (updateFastThreshold), priors (priorOf), poses and
+// key-frame test.  Streams need not run in lockstep; a stream not named keeps its frame and state.  Per named stream, as the
+// reference's loop: insertStereoPairs, then optimizePose, needNewKF / currFrameIsKF if wanted, and updateFrame.
+class StereoStreamsHandler {
+public:
+    struct Stream {
+        StereoFrame prev_frame, curr_frame;
+        std::array<int32_t, 4> n_stereo{};               // stereo points, lines of prev, then of curr, in the stream's last insert
+        int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
+        int orb_fast_th = 20;
+        KeyframeTest kf;
+        PlPoseResult result{};
+        bool has_prev = false;
+    };
+    StereoStreamsHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                         const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc, int n_streams,
+                         const HandlerConfig& hcfg = HandlerConfig{}, const Rectifier* rect = nullptr)
+        : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, n_streams, rect),
+          streams_((size_t)n_streams) {
+        for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
+    }
+
+    // initialize(img_l[k], img_r[k], idx[k]) of stream ids[k], in one session call (idx optional)
+    void initialize(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                    const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
+        const std::vector<int32_t> th(ids.size(), hcfg_.orb_fast_th);   // :38
+        pack_.pack(cam_.width, cam_.height, img_l, img_r, th, "StereoStreamsHandler::initialize");
+        session_.initialize((int)ids.size(), ids.data(), pack_.view);
+        for (size_t k = 0; k < ids.size(); ++k) {
+            Stream& s = streams_[(size_t)ids[k]];
+            s.orb_fast_th = hcfg_.orb_fast_th;
+            s.prev_frame = StereoFrame{};
+            s.prev_frame.frame_idx = k < idx.size() ? idx[k] : 0;
+            for (int i = 0; i < 36; ++i) s.prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+            s.curr_frame = StereoFrame{};
+            s.kf = KeyframeTest{};                       // :48-51
+            s.has_prev = true;
+        }
+    }
+    // insertStereoPair(img_l[k], img_r[k], idx[k]) of stream ids[k]: f2fTracking of every named stream in one session call
+    void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                           const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
+        std::vector<int32_t> th;
+        std::vector<PlPrior> priors;
+        for (int32_t id : ids) {
+            const Stream& s = at(id);
+            if (!s.has_prev) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: initialize() the stream first");
+            th.push_back(s.orb_fast_th);
+            priors.push_back(priorOf(s.prev_frame));
+        }
+        pack_.pack(cam_.width, cam_.height, img_l, img_r, th, "StereoStreamsHandler::insertStereoPairs");
+        std::vector<PlPoseResult> res(ids.size());
+        std::vector<int32_t> ns(4 * ids.size());
+        session_.insert((int)ids.size(), ids.data(), pack_.view, priors.data(), res.data(), ns.data());
+        for (size_t k = 0; k < ids.size(); ++k) {
+            Stream& s = streams_[(size_t)ids[k]];
+            s.curr_frame = StereoFrame{};
+            s.curr_frame.frame_idx = k < idx.size() ? idx[k] : 0;
+            s.result = res[k];
+            std::copy(ns.begin() + 4 * k, ns.begin() + 4 * k + 4, s.n_stereo.begin());
+            s.n_inliers_pt = s.result.n_matched_pt;      // :126-128
+            s.n_inliers_ls = s.result.n_matched_ls;
+            s.n_inliers = s.n_inliers_pt + s.n_inliers_ls;
+        }
+    }
+    void optimizePose(int id) {                          // :307-392
+        Stream& s = at(id);
+        publishPose(s.result, s.curr_frame);
+        s.n_inliers_pt = s.result.n_inliers_pt;
+        s.n_inliers_ls = s.result.n_inliers_ls;
+        s.n_inliers = s.result.n_inliers;
+    }
+    void updateFrame(int id) {                           // :62-102
+        Stream& s = at(id);
+        s.orb_fast_th = updateFastThreshold(hcfg_, s.orb_fast_th, s.curr_frame, s.n_inliers_pt);   // :66-86
+        s.prev_frame = std::move(s.curr_frame);
+        s.curr_frame = StereoFrame{};
+    }
+    bool needNewKF(int id) { Stream& s = at(id); return s.kf.needNewKF(hcfg_, s.curr_frame); }
+    void currFrameIsKF(int id) { Stream& s = at(id); s.kf.currFrameIsKF(s.curr_frame); }
+
+    Stream& stream(int id) { return at(id); }
+    int streams() const { return (int)streams_.size(); }
+    const StereoSession& session() const { return session_; }
+
+private:
+    Stream& at(int id) {
+        if (id < 0 || id >= (int)streams_.size()) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: stream id out of range");
+        return streams_[(size_t)id];
+    }
+    PlCamera cam_;
+    HandlerConfig hcfg_;
+    StereoSession session_;
+    std::vector<Stream> streams_;
+    detail::StereoImagesBatch pack_;
 };
 
 }  // namespace plstvo

@@ -845,17 +845,19 @@ int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
 static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                             const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
                             const PlRectifier* rect, const PlStereoImages* prev, const PlStereoImages* curr,
-                            const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence) {
-    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!sequence && !curr) || !results)
+                            const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence,
+                            PlStereoSession* session = nullptr) {
+    const bool one_set = sequence || session;   // one frame set: a sequence, or a session's new frames
+    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!one_set && !curr) || (!results && (!session || session->track)))
         return fail(ctx, PLSTVO_E_INVALID, "null argument");
     if (rect && rect->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the rectifier belongs to another context");
     if (rect && (rect->width != cam->width || rect->height != cam->height))
         return fail(ctx, PLSTVO_E_SIZE, "rectifier size differs from the camera's");
     const int NF = prev->B;
     if (NF < 0) return fail(ctx, PLSTVO_E_INVALID, "negative number of frames");
-    if (!sequence && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (!one_set && curr->B != NF) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
     if (const int rc = orb_detect_check(ctx, oc)) return rc;
-    const int nfs = sequence ? 1 : 2;   // frame sets: the sequence, or prev and curr
+    const int nfs = one_set ? 1 : 2;   // frame sets: the sequence or the session's new frames, or prev and curr
     const PlStereoImages* fs[2] = {prev, curr};
     const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0, run_lsd = detect_lines && lns;
     const int W = cam->width, H = cam->height;
@@ -1023,8 +1025,8 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     }
     dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
     dev.marks = ctx->img_ev.ev + 1;
-    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], sequence ? nullptr : &feat[1], priors, results,
-                                           n_stereo, sequence, -1, &dev))
+    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], one_set ? nullptr : &feat[1], priors, results,
+                                           n_stereo, sequence, -1, &dev, session))
         return rc;
     float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
     std::fill(ms, ms + 5, 0.f);
@@ -1045,11 +1047,12 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
 static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
                                const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
-                               PlPoseResult* results, int32_t* n_stereo, bool sequence, const PlRectifier* rect = nullptr) {
+                               PlPoseResult* results, int32_t* n_stereo, bool sequence, const PlRectifier* rect = nullptr,
+                               PlStereoSession* session = nullptr) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    const int rc =
-        track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, rect, prev, curr, priors, results, n_stereo, sequence);
+    const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, rect, prev, curr, priors, results, n_stereo,
+                                    sequence, session);
     // after an error the line stages may still run on the second stream, and ORB on the first: the next call may reuse their
     // arenas
     const cudaError_t e = cudaStreamSynchronize(ctx->s_alt), e_main = cudaStreamSynchronize(ctx->s_main);
@@ -1098,6 +1101,118 @@ int plstvo_track_stereo_raw_images_sequence(PlContext* ctx, const PlCamera* cam,
                                             const PlStereoImages* frames, const PlPrior* priors, PlPoseResult* results,
                                             int32_t* n_stereo) {
     return track_images_common(ctx, cam, cfg, mcfg, scfg, ocfg, true, lcfg, frames, nullptr, priors, results, n_stereo, true, rect);
+}
+
+/* ---- stereo sessions: each stream's previous frame kept in HBM as its stereo features ---- */
+PlStereoSession* plstvo_stereo_session_create(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
+                                              const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                              const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlRectifier* rect,
+                                              int n_streams) {
+    if (!ctx) return nullptr;
+    LOCK(ctx);
+    auto bad = [&](int code, const char* msg) -> PlStereoSession* {
+        fail(ctx, code, msg);
+        return nullptr;
+    };
+    if (!cam || !cfg || !mcfg || !scfg || !ocfg) return bad(PLSTVO_E_INVALID, "null argument");
+    if (n_streams < 1) return bad(PLSTVO_E_INVALID, "n_streams must be at least 1");
+    if (orb_detect_check(ctx, ocfg)) return nullptr;
+    if (cfg->has_lines) {
+        if (!lcfg) return bad(PLSTVO_E_INVALID, "null lsd config");
+        if (lsd_check_config(ctx, lcfg)) return nullptr;
+    }
+    if (!grid_ok(mcfg->grid_rows, mcfg->grid_cols) || cam->width <= 0 || cam->height <= 0)
+        return bad(PLSTVO_E_INVALID, "bad grid or image size");
+    if (rect && rect->ctx != ctx) return bad(PLSTVO_E_INVALID, "the rectifier belongs to another context");
+    if (rect && (rect->width != cam->width || rect->height != cam->height))
+        return bad(PLSTVO_E_SIZE, "rectifier size differs from the camera's");
+    PlStereoSession* ss = new PlStereoSession();
+    ss->ctx = ctx;
+    ss->cam = *cam; ss->cfg = *cfg; ss->mc = *mcfg; ss->sc = *scfg; ss->oc = *ocfg;
+    ss->has_lc = lcfg != nullptr;
+    if (lcfg) ss->lc = *lcfg;
+    ss->rect = rect;
+    ss->n_streams = n_streams;
+    ss->live.assign((size_t)n_streams, 0);
+    ss->n_pt.assign((size_t)n_streams, 0);
+    ss->n_ls.assign((size_t)n_streams, 0);
+    ss->off_pt.assign((size_t)n_streams, 0);
+    ss->off_ls.assign((size_t)n_streams, 0);
+    return ss;
+}
+
+void plstvo_stereo_session_destroy(PlStereoSession* ss) {
+    if (!ss) return;
+    {
+        LOCK(ss->ctx);   // every call that reads the pools blocks, so none is using them once the lock is held
+        cudaSetDevice(ss->ctx->device);
+        ss->pool[0].buf.release();
+        ss->pool[1].buf.release();
+        ss->d_meta.release();
+    }
+    delete ss;
+}
+
+int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
+    if (!ss) return 0;
+    LOCK(ss->ctx);
+    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap);
+}
+
+namespace {
+// initialize (track == false) or insert for streams ids[0 .. n): the checks, then the images path in session mode; the pools
+// flip and the streams' counts are kept only when the whole call succeeded
+int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const int32_t* ids, const PlStereoImages* frames,
+                 const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
+    if (frames->B != n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from n");
+    if (n == 0) return 0;
+    if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
+    if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
+    std::vector<uint8_t> named((size_t)ss->n_streams, 0);
+    for (int k = 0; k < n; ++k) {
+        const int id = ids[k];
+        if (id < 0 || id >= ss->n_streams) return fail(ctx, PLSTVO_E_INVALID, "stream id outside [0, n_streams)");
+        if (named[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "duplicate stream id");
+        named[(size_t)id] = 1;
+        if (track && !ss->live[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "insert on a stream with no frame: initialize it first");
+    }
+    ss->track = track;
+    ss->n = n;
+    ss->ids = ids;
+    if (track) {   // the kept frames, compact in call order: the tracker's previous frames
+        ss->kept_off_pt.assign((size_t)n + 1, 0);
+        ss->kept_off_ls.assign((size_t)n + 1, 0);
+        for (int k = 0; k < n; ++k) {
+            const size_t id = (size_t)ids[k];
+            ss->kept_off_pt[(size_t)k + 1] = ss->kept_off_pt[(size_t)k] + ss->n_pt[id];
+            ss->kept_off_ls[(size_t)k + 1] = ss->kept_off_ls[(size_t)k] + ss->n_ls[id];
+            if (n_stereo) {
+                n_stereo[4 * (size_t)k] = ss->n_pt[id];
+                n_stereo[4 * (size_t)k + 1] = ss->n_ls[id];
+            }
+        }
+    }
+    const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, true, ss->has_lc ? &ss->lc : nullptr,
+                                       frames, nullptr, priors, results, n_stereo, false, ss->rect, ss);
+    if (rc == 0) session_commit(ss);
+    ss->ids = nullptr;   // the caller's array: not read after the call
+    return rc;
+}
+}  // namespace
+
+int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* ss, int n, const int32_t* ids, const PlStereoImages* frames,
+                                     int32_t* n_stereo) {
+    return session_call(ctx, ss, false, n, ids, frames, nullptr, nullptr, n_stereo);
+}
+
+int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* ss, int n, const int32_t* ids, const PlStereoImages* frames,
+                                 const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    return session_call(ctx, ss, true, n, ids, frames, priors, results, n_stereo);
 }
 
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {

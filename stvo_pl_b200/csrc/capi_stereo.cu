@@ -298,25 +298,32 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
 // sequence == false: B independent (prev, curr) pairs, four feature sets of B frames.
 // sequence == true : prev holds NF = B + 1 consecutive frames, pair p = (frame p, frame p + 1); two feature sets of NF frames,
 //                    every frame goes through the stereo step once and is lifted twice (as a previous and as a current frame).
+// session != null  : prev holds the NF = B new frames of the session's streams ids[0 .. B) (curr is unused).  Each new frame goes
+//                    through the stereo step once and is lifted twice: as the current frame of pair p into the workspace, and
+//                    in the previous-frame role into the session's next pool.  The streams' kept frames are gathered into the
+//                    workspace's previous-frame arrays (insert; initialize tracks nothing and takes no results).
 int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                 const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                                 const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                                const StereoDevInputs* dev) {
+                                const StereoDevInputs* dev, PlStereoSession* session) {
     // slot < 0: blocking (returns with the results in host memory); slot 0 / 1: enqueue only, results valid after plstvo_wait
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!cam || !cfg || !mc || !sc || !prev || (!sequence && !curr) || !results) return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    const bool one_set = sequence || session;       // two feature sets (points, lines of one frame set)
+    const bool track = !session || session->track;
+    if (!cam || !cfg || !mc || !sc || !prev || (!one_set && !curr) || (track && !results))
+        return fail(ctx, PLSTVO_E_INVALID, "null argument");
     const int NF = prev->B;                         // frames per feature set
     const int B = sequence ? NF - 1 : NF;           // pairs
-    if (NF < 0 || (!sequence && curr->B != NF)) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (NF < 0 || (!one_set && curr->B != NF)) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
     if (sequence && NF == 1) return 0;              // one frame: nothing to track
     const int rows = mc->grid_rows, cols = mc->grid_cols;
     if (!grid_ok(rows, cols) || cam->width <= 0 || cam->height <= 0)
         return fail(ctx, PLSTVO_E_INVALID, "bad grid or image size");
     if (NF == 0) return 0;
     CK(ctx, cudaSetDevice(ctx->device));
-    const int NSETS = sequence ? 2 : 4;
-    if (sequence) curr = prev;                      // sets 2, 3 below are unused
+    const int NSETS = one_set ? 2 : 4;
+    if (one_set) curr = prev;                       // sets 2, 3 below are unused
     // the four feature sets: {prev, curr} x {points, lines}
     struct Set {
         bool lines; const int32_t *l_off, *r_off; const float *xy_l, *xy_r, *ang; const int32_t* oct; const uint8_t *d1, *d2;
@@ -439,7 +446,8 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         for (int p = 0; p < NF; ++p) {
             ooff[k][p + 1] = ooff[k][p] + cnt[(size_t)k * NF + p];
             if (n_stereo) {
-                if (sequence) n_stereo[(size_t)p * 2 + k] = cnt[(size_t)k * NF + p];
+                if (sequence || !track) n_stereo[(size_t)p * 2 + k] = cnt[(size_t)k * NF + p];
+                else if (session) n_stereo[(size_t)p * 4 + 2 + k] = cnt[(size_t)k * NF + p];
                 else n_stereo[(size_t)p * 4 + k] = cnt[(size_t)k * NF + p];
             }
         }
@@ -450,12 +458,42 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             CK(ctx, a.up(sets[k].o_ooff2, ooff2[k].data(), (size_t)NF * 4, sh));
         }
     }
+    // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
+    // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
+    auto lift_prev_points = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
+        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
+                                  a.i32(st.o_m12), nullptr, nullptr, o.ptP, o.pts2, nullptr, o.pdesc, nullptr, a.i32(st.o_cnt), s,
+                                  out_off);
+    };
+    auto lift_prev_lines = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
+        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1, a.i32(st.o_roff),
+                                 st.g_xyr, a.i32(st.o_m12), o.spl, o.epl, nullptr, nullptr, o.sP, o.eP, nullptr, nullptr, o.s2,
+                                 o.lev, o.ldesc, nullptr, a.i32(st.o_cnt), s, out_off);
+    };
+    // session: the new frames' previous-frame role goes into the next pool, the untouched streams' kept frames follow it there
+    if (session) {
+        if (const int rc = session_plan(ctx, session, cnt, cnt + NF, s)) return rc;
+        const PrevRows& next = session->pool[session->cur ^ 1].rows;
+        CK(ctx, lift_prev_points(sets[0], next, session_out_off(session, false)));
+        CK(ctx, lift_prev_lines(sets[1], next, session_out_off(session, true)));
+        ctx->launches += 2;
+        if (const int rc = session_gather_others(ctx, session, s)) return rc;
+        if (!track) {
+            if (dev && dev->marks) {
+                CK(ctx, cudaEventRecord(dev->marks[1], s));
+                CK(ctx, cudaEventRecord(dev->marks[2], s));
+            }
+            if (slot < 0) CK(ctx, cudaStreamSynchronize(s));
+            return 0;
+        }
+    }
     // ---- the tracker's plan on the compact lists; the records are written straight into its buffers ----
     PlFrameBatch fp{}, fc{};
     fp.B = fc.B = B;
-    fp.pt_off = ooff[0].data(); fp.ls_off = ooff[1].data();
-    fc.pt_off = sequence ? ooff2[0].data() : ooff[2].data();
-    fc.ls_off = sequence ? ooff2[1].data() : ooff[3].data();
+    fp.pt_off = session ? session->kept_off_pt.data() : ooff[0].data();
+    fp.ls_off = session ? session->kept_off_ls.data() : ooff[1].data();
+    fc.pt_off = sequence ? ooff2[0].data() : session ? ooff[0].data() : ooff[2].data();
+    fc.ls_off = sequence ? ooff2[1].data() : session ? ooff[1].data() : ooff[3].data();
     Workspace& ws = slot < 0 ? ctx->ws : ctx->ws_async[slot];
     int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr);
     if (rc) return rc;
@@ -463,20 +501,6 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     cudaEvent_t planned = next_event(ctx);
     CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(s, planned, 0));
-    // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
-    // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
-    auto lift_prev_points = [&](const Set& st) -> cudaError_t {
-        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
-                                  a.i32(st.o_m12), nullptr, nullptr, ws.d_ptP.as<double>(), ws.d_pts2.as<double>(), nullptr,
-                                  ws.d_pdesc1.as<uint8_t>(), nullptr, a.i32(st.o_cnt), s, a.i32(st.o_ooff));
-    };
-    auto lift_prev_lines = [&](const Set& st) -> cudaError_t {
-        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1, a.i32(st.o_roff),
-                                 st.g_xyr, a.i32(st.o_m12), ws.d_lsspl.as<double>(), ws.d_lsepl.as<double>(), nullptr, nullptr,
-                                 ws.d_lssP.as<double>(), ws.d_lseP.as<double>(), nullptr, nullptr, ws.d_lss2.as<double>(),
-                                 ws.d_lslev.as<int32_t>(), ws.d_ldesc1.as<uint8_t>(), nullptr, a.i32(st.o_cnt), s,
-                                 a.i32(st.o_ooff));
-    };
     auto lift_curr_points = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
         return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
                                   st.g_xyr, a.i32(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
@@ -488,16 +512,24 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
                                  nullptr, ws.d_lsle.as<double>(), nullptr, nullptr, nullptr, ws.d_ldesc2.as<uint8_t>(), nullptr,
                                  a.i32(st.o_cnt) + first, s, a.i32(o_out));
     };
-    CK(ctx, lift_prev_points(sets[0]));
-    CK(ctx, lift_prev_lines(sets[1]));
+    if (session) {
+        if (const int rc2 = session_gather_named(ctx, session, workspace_prev_rows(ws), s)) return rc2;
+    } else {
+        const PrevRows wsr = workspace_prev_rows(ws);
+        CK(ctx, lift_prev_points(sets[0], wsr, a.i32(sets[0].o_ooff)));
+        CK(ctx, lift_prev_lines(sets[1], wsr, a.i32(sets[1].o_ooff)));
+    }
     if (sequence) {
         CK(ctx, lift_curr_points(sets[0], 1, sets[0].o_ooff2));
         CK(ctx, lift_curr_lines(sets[1], 1, sets[1].o_ooff2));
+    } else if (session) {
+        CK(ctx, lift_curr_points(sets[0], 0, sets[0].o_ooff));
+        CK(ctx, lift_curr_lines(sets[1], 0, sets[1].o_ooff));
     } else {
         CK(ctx, lift_curr_points(sets[2], 0, sets[2].o_ooff));
         CK(ctx, lift_curr_lines(sets[3], 0, sets[3].o_ooff));
     }
-    ctx->launches += 4;
+    ctx->launches += session ? 2 : 4;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
     rc = ws_launch_match(ctx, ws, 0, B, s);
     if (rc) return rc;

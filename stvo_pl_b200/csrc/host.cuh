@@ -371,6 +371,85 @@ int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t 
 int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_level, cudaStream_t s,
                     cudaEvent_t* marks = nullptr);
 
+// ---- session.cu: the previous-frame-role records of kept frames (plstvo_stereo_session_*) ----
+// Where the previous-frame role of a frame's stereo features is written: every array lift_points / lift_lines fill for a
+// frame that is tracked against (the workspace's d_ptP .. d_ldesc1, or a session pool), rows in CSR order.
+struct PrevRows {
+    double *ptP = nullptr, *pts2 = nullptr; uint8_t* pdesc = nullptr;                       // [n][3], [n], [n][32]
+    double *spl = nullptr, *epl = nullptr, *sP = nullptr, *eP = nullptr, *s2 = nullptr;      // [m][2] x2, [m][3] x2, [m]
+    int32_t* lev = nullptr; uint8_t* ldesc = nullptr;                                        // [m], [m][32]
+};
+constexpr size_t SESSION_PT_BYTES = 24 + 8 + 32;                   // bytes per kept stereo point
+constexpr size_t SESSION_LS_BYTES = 16 + 16 + 24 + 24 + 8 + 4 + 32;  // bytes per kept stereo line
+inline PrevRows workspace_prev_rows(const Workspace& ws) {
+    PrevRows r;
+    r.ptP = ws.d_ptP.as<double>(); r.pts2 = ws.d_pts2.as<double>(); r.pdesc = ws.d_pdesc1.as<uint8_t>();
+    r.spl = ws.d_lsspl.as<double>(); r.epl = ws.d_lsepl.as<double>(); r.sP = ws.d_lssP.as<double>();
+    r.eP = ws.d_lseP.as<double>(); r.s2 = ws.d_lss2.as<double>(); r.lev = ws.d_lslev.as<int32_t>();
+    r.ldesc = ws.d_ldesc1.as<uint8_t>();
+    return r;
+}
+// One session pool: the kept frames of every stream, point rows and line rows in stream-id order.
+struct SessionPool {
+    DevBuf buf;
+    size_t cap_pt = 0, cap_ls = 0;   // rows
+    PrevRows rows;
+    cudaError_t ensure(size_t n_pt, size_t n_ls);
+};
+// A block of consecutive rows moved by session_gather_kernel: point rows [src_pt, src_pt + n_pt) of the source to dst_pt ..
+// of the destination, and the same for lines.
+struct GatherSeg {
+    int32_t src_pt, dst_pt, n_pt, src_ls, dst_ls, n_ls;
+};
+cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s);
+
+}  // namespace plstvo
+
+// n_streams independent stereo streams, each with the previous-frame-role records of its kept frame in HBM
+// (plstvo_stereo_session_create).  pool[cur] holds the kept frames; a call writes pool[cur ^ 1] and flips cur when it succeeds.
+struct PlStereoSession {
+    PlContext* ctx = nullptr;
+    PlCamera cam{};
+    PlConfig cfg{};
+    PlStereoMatchConfig mc{};
+    PlStereoConfig sc{};
+    PlOrbDetectConfig oc{};
+    PlLsdConfig lc{};
+    bool has_lc = false;
+    const PlRectifier* rect = nullptr;
+    int n_streams = 0;
+    std::vector<uint8_t> live;              // [S] the stream has a kept frame
+    std::vector<int32_t> n_pt, n_ls;        // [S] its stereo points / lines
+    std::vector<int32_t> off_pt, off_ls;    // [S] its first rows in pool[cur]
+    plstvo::SessionPool pool[2];
+    int cur = 0;
+    plstvo::DevBuf d_meta;                  // this call's lift output offsets and gather segments
+    // ---- the call in progress (plstvo::session_plan), committed by plstvo::session_commit ----
+    bool track = false;                     // insert (true) or initialize
+    int n = 0;
+    const int32_t* ids = nullptr;
+    std::vector<int32_t> kept_off_pt, kept_off_ls;   // [n + 1] the named streams' kept frames, compact (insert)
+    std::vector<int32_t> next_off_pt, next_off_ls;   // [S] first rows in pool[cur ^ 1]
+    std::vector<int32_t> new_pt, new_ls;             // [n] the new frames' stereo points / lines
+    std::vector<int32_t> meta;                       // uploaded: out_off_pt [n], out_off_ls [n], GatherSeg named [n], others
+    int n_others = 0;
+};
+
+namespace plstvo {
+
+// Lays out pool[cur ^ 1] for the new frames' counts (new_pt, new_ls [n], call order) and the untouched streams' kept frames,
+// grows it if need be, and uploads the call's offsets and gather segments on s.  PLSTVO_E_TOO_LARGE: more than INT_MAX rows.
+int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s);
+// The two moves of a planned call, enqueued on s: the named streams' kept frames from pool[cur] into the workspace's
+// previous-frame arrays at kept_off_pt / kept_off_ls (insert), and the untouched streams' kept frames from pool[cur] into
+// pool[cur ^ 1].  The new frames' previous-frame role goes into pool[cur ^ 1] through the lift kernels, at session_out_off.
+int session_gather_named(PlContext* ctx, PlStereoSession* ss, const PrevRows& ws_rows, cudaStream_t s);
+int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s);
+// device offsets [n] of the new frames' first point / line rows in pool[cur ^ 1]
+const int32_t* session_out_off(const PlStereoSession* ss, bool lines);
+// the call succeeded: pool[cur ^ 1] becomes the kept frames
+void session_commit(PlStereoSession* ss);
+
 // ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
 // Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the
 // stream `lines_ready` was recorded on).  A set with on_device reads xy_l, xy_r, oct, d1, d2 from here instead of uploading
@@ -386,7 +465,7 @@ struct StereoDevInputs {
 int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                         const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                         const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                        const StereoDevInputs* dev = nullptr);
+                        const StereoDevInputs* dev = nullptr, PlStereoSession* session = nullptr);
 
 // ---- rectify.cu: rectifyImagesLR on the device, composed by the raw-images path ----
 struct ImgPart {   // consecutive host images of one size

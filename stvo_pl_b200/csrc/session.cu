@@ -1,0 +1,158 @@
+// session.cu — the device side of plstvo_stereo_session_*: the session's double-buffered pools of kept frames and the gather
+// kernel that moves a list of streams' previous-frame-role rows, byte for byte, from one CSR layout into another.
+#include <climits>
+#include <cstring>
+
+#include "host.cuh"
+
+namespace plstvo {
+
+namespace {
+
+constexpr int GATHER_THREADS = 256;
+constexpr int GATHER_ARRAYS = 10;   // PrevRows: 3 point arrays, 7 line arrays
+
+struct GatherArrays {
+    const uint32_t* src[GATHER_ARRAYS];
+    uint32_t* dst[GATHER_ARRAYS];
+};
+
+// 4-byte words per row of each PrevRows array, points first
+__constant__ int c_words[GATHER_ARRAYS] = {6, 2, 8, 4, 4, 6, 6, 2, 1, 8};
+
+// One block per segment: every word of the segment's point rows, then of its line rows, is copied unchanged.  Integer
+// copies only (no arithmetic on the values), so the kept records are the lift kernels' bytes.
+__global__ void __launch_bounds__(GATHER_THREADS) session_gather_kernel(GatherArrays a, const GatherSeg* __restrict__ segs) {
+    const GatherSeg g = segs[blockIdx.x];
+#pragma unroll 1
+    for (int k = 0; k < GATHER_ARRAYS; ++k) {
+        const bool pt = k < 3;
+        const int n = pt ? g.n_pt : g.n_ls;
+        if (n == 0) continue;
+        const int w = c_words[k];
+        const size_t words = (size_t)n * w;
+        const uint32_t* __restrict__ src = a.src[k] + (size_t)(pt ? g.src_pt : g.src_ls) * w;
+        uint32_t* __restrict__ dst = a.dst[k] + (size_t)(pt ? g.dst_pt : g.dst_ls) * w;
+        for (size_t i = threadIdx.x; i < words; i += GATHER_THREADS) dst[i] = src[i];
+    }
+}
+
+GatherArrays gather_arrays(const PrevRows& s, const PrevRows& d) {
+    GatherArrays a;
+    const void* sp[GATHER_ARRAYS] = {s.ptP, s.pts2, s.pdesc, s.spl, s.epl, s.sP, s.eP, s.s2, s.lev, s.ldesc};
+    void* dp[GATHER_ARRAYS] = {d.ptP, d.pts2, d.pdesc, d.spl, d.epl, d.sP, d.eP, d.s2, d.lev, d.ldesc};
+    for (int k = 0; k < GATHER_ARRAYS; ++k) {
+        a.src[k] = static_cast<const uint32_t*>(sp[k]);
+        a.dst[k] = static_cast<uint32_t*>(dp[k]);
+    }
+    return a;
+}
+
+// offsets into PlStereoSession::meta
+size_t meta_named(const PlStereoSession* ss) { return 2 * (size_t)ss->n; }
+size_t meta_others(const PlStereoSession* ss) { return meta_named(ss) + (size_t)ss->n * (sizeof(GatherSeg) / 4); }
+
+}  // namespace
+
+cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s) {
+    if (n_segs <= 0) return cudaSuccess;
+    session_gather_kernel<<<n_segs, GATHER_THREADS, 0, s>>>(gather_arrays(src, dst), segs);
+    return cudaGetLastError();
+}
+
+cudaError_t SessionPool::ensure(size_t n_pt, size_t n_ls) {
+    if (buf.p && n_pt <= cap_pt && n_ls <= cap_ls) return cudaSuccess;
+    const size_t want_pt = std::max(n_pt + n_pt / 4, cap_pt) + 64, want_ls = std::max(n_ls + n_ls / 4, cap_ls) + 64;
+    Arena a;
+    const size_t o_P = a.take(want_pt * 24), o_s2 = a.take(want_pt * 8), o_d = a.take(want_pt * 32);
+    const size_t o_spl = a.take(want_ls * 16), o_epl = a.take(want_ls * 16), o_sP = a.take(want_ls * 24);
+    const size_t o_eP = a.take(want_ls * 24), o_ls2 = a.take(want_ls * 8), o_lev = a.take(want_ls * 4);
+    const size_t o_ld = a.take(want_ls * 32);
+    cap_pt = cap_ls = 0;
+    rows = PrevRows{};
+    if (const cudaError_t e = a.alloc(buf)) return e;
+    rows.ptP = a.f64(o_P); rows.pts2 = a.f64(o_s2); rows.pdesc = a.u8(o_d);
+    rows.spl = a.f64(o_spl); rows.epl = a.f64(o_epl); rows.sP = a.f64(o_sP); rows.eP = a.f64(o_eP); rows.s2 = a.f64(o_ls2);
+    rows.lev = a.i32(o_lev); rows.ldesc = a.u8(o_ld);
+    cap_pt = want_pt;
+    cap_ls = want_ls;
+    return cudaSuccess;
+}
+
+int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s) {
+    const int S = ss->n_streams, n = ss->n;
+    std::vector<int> slot((size_t)S, -1);   // call position of each named stream
+    for (int k = 0; k < n; ++k) slot[(size_t)ss->ids[k]] = k;
+    ss->new_pt.assign(new_pt, new_pt + n);
+    ss->new_ls.assign(new_ls, new_ls + n);
+    ss->next_off_pt.assign((size_t)S, 0);
+    ss->next_off_ls.assign((size_t)S, 0);
+    std::vector<GatherSeg> others;
+    long long tp = 0, tl = 0;
+    for (int id = 0; id < S; ++id) {
+        const int k = slot[(size_t)id];
+        const int np = k >= 0 ? new_pt[k] : ss->live[(size_t)id] ? ss->n_pt[(size_t)id] : 0;
+        const int nl = k >= 0 ? new_ls[k] : ss->live[(size_t)id] ? ss->n_ls[(size_t)id] : 0;
+        ss->next_off_pt[(size_t)id] = (int32_t)tp;
+        ss->next_off_ls[(size_t)id] = (int32_t)tl;
+        if (k < 0 && (np || nl))
+            others.push_back(GatherSeg{ss->off_pt[(size_t)id], (int32_t)tp, np, ss->off_ls[(size_t)id], (int32_t)tl, nl});
+        tp += np;
+        tl += nl;
+        if (tp > INT_MAX || tl > INT_MAX) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than INT_MAX kept rows in one session");
+    }
+    CK(ctx, ss->pool[ss->cur ^ 1].ensure((size_t)tp, (size_t)tl));
+    // meta: out_off_pt [n], out_off_ls [n], the named streams' segments (kept frame -> the workspace, compact), the others'
+    std::vector<int32_t>& m = ss->meta;
+    m.assign(meta_others(ss), 0);
+    for (int k = 0; k < n; ++k) {
+        const int id = ss->ids[k];
+        m[(size_t)k] = ss->next_off_pt[(size_t)id];
+        m[(size_t)n + k] = ss->next_off_ls[(size_t)id];
+        if (ss->track) {
+            const GatherSeg g{ss->off_pt[(size_t)id], ss->kept_off_pt[(size_t)k], ss->n_pt[(size_t)id],
+                              ss->off_ls[(size_t)id], ss->kept_off_ls[(size_t)k], ss->n_ls[(size_t)id]};
+            memcpy(m.data() + meta_named(ss) + (size_t)k * (sizeof(GatherSeg) / 4), &g, sizeof g);
+        }
+    }
+    ss->n_others = (int)others.size();
+    const size_t o = m.size();
+    m.resize(o + others.size() * (sizeof(GatherSeg) / 4));
+    if (!others.empty()) memcpy(m.data() + o, others.data(), others.size() * sizeof(GatherSeg));
+    CK(ctx, ss->d_meta.ensure(m.size() * 4));
+    CK(ctx, cudaMemcpyAsync(ss->d_meta.p, m.data(), m.size() * 4, cudaMemcpyHostToDevice, s));
+    return 0;
+}
+
+int session_gather_named(PlContext* ctx, PlStereoSession* ss, const PrevRows& ws_rows, cudaStream_t s) {
+    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_named(ss));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ws_rows, segs, ss->n, s));
+    ctx->launches++;
+    return 0;
+}
+
+int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s) {
+    if (!ss->n_others) return 0;
+    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_others(ss));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ss->pool[ss->cur ^ 1].rows, segs, ss->n_others, s));
+    ctx->launches++;
+    return 0;
+}
+
+const int32_t* session_out_off(const PlStereoSession* ss, bool lines) {
+    return ss->d_meta.as<int32_t>() + (lines ? ss->n : 0);
+}
+
+void session_commit(PlStereoSession* ss) {
+    for (int k = 0; k < ss->n; ++k) {
+        const size_t id = (size_t)ss->ids[k];
+        ss->live[id] = 1;
+        ss->n_pt[id] = ss->new_pt[(size_t)k];
+        ss->n_ls[id] = ss->new_ls[(size_t)k];
+    }
+    ss->off_pt = ss->next_off_pt;
+    ss->off_ls = ss->next_off_ls;
+    ss->cur ^= 1;
+}
+
+}  // namespace plstvo

@@ -130,6 +130,12 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                                                               C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
                                                               C.POINTER(T.PlLsdConfig), vp, C.POINTER(T.PlStereoImages), vp, vp,
                                                               i32p]),
+        "plstvo_stereo_session_create": (vp, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig), C.POINTER(T.PlStereoConfig),
+                                              C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlLsdConfig), vp, C.c_int]),
+        "plstvo_stereo_session_destroy": (None, [vp]),
+        "plstvo_stereo_session_device_bytes": (C.c_int64, [vp]),
+        "plstvo_stereo_session_initialize": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), i32p]),
+        "plstvo_stereo_session_insert": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), vp, vp, i32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -156,7 +162,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_track_stereo_images_sequence", "plstvo_track_stereo_images_lsd_batch", "plstvo_track_stereo_images_lsd_sequence",
     "plstvo_track_stereo_images_stage_times", "plstvo_init_undistort_rectify_map", "plstvo_rectifier_create",
     "plstvo_rectifier_destroy", "plstvo_rectify_batch", "plstvo_rectify_kernel_times", "plstvo_track_stereo_raw_images_batch",
-    "plstvo_track_stereo_raw_images_sequence"]
+    "plstvo_track_stereo_raw_images_sequence", "plstvo_stereo_session_create", "plstvo_stereo_session_destroy",
+    "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -186,6 +193,33 @@ class Rectifier:
     def close(self):
         if self.handle:
             self.lib.plstvo_rectifier_destroy(self.handle)
+            self.handle = None
+
+
+class StereoSession:
+    """A PlStereoSession: n_streams stereo streams, each stream's previous frame kept in HBM as its stereo features
+    (Engine.stereo_session_create).  initialize / insert name any subset of the streams; close() or the owning Engine frees it."""
+
+    def __init__(self, eng: "Engine", handle, n_streams: int):
+        self.eng, self.handle, self.n_streams = eng, handle, n_streams
+
+    def initialize(self, ids, frames: dict):
+        """initialize(img_l, img_r) for streams ids: frames holds len(ids) frames (img_l / img_r uint8[n, H, W], optionally
+        fast_th [n]).  Returns n_stereo [n, 2]."""
+        return self.eng.stereo_session_initialize(self, ids, frames)
+
+    def insert(self, ids, frames: dict, priors=None, results=None):
+        """insertStereoPair + optimizePose for streams ids against their kept frames, which the new frames then replace.
+        Returns (results [n], n_stereo [n, 4])."""
+        return self.eng.stereo_session_insert(self, ids, frames, priors, results)
+
+    @property
+    def device_bytes(self) -> int:
+        return int(self.eng.lib.plstvo_stereo_session_device_bytes(self.handle)) if self.handle else 0
+
+    def close(self):
+        if self.handle:
+            self.eng.lib.plstvo_stereo_session_destroy(self.handle)
             self.handle = None
 
 
@@ -317,9 +351,12 @@ class Engine:
         self.ctx = ctx
         self.pinned = PinnedPool(self.lib)
         self._rectifiers = []
+        self._sessions = []
 
     def close(self):
         if self.ctx:
+            for ss in self._sessions:
+                ss.close()
             for r in self._rectifiers:
                 r.close()
             self.pinned.close()
@@ -776,6 +813,45 @@ class Engine:
             self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
             None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle, C.byref(fs),
             priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
+        del keep
+        return results, n_stereo
+
+    # ---- stereo sessions: many streams, each stream's previous frame kept on the device ----
+    def stereo_session_create(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], n_streams: int) -> StereoSession:
+        """A session of n_streams streams with these configs (copied; lcfg may be None where cfg.has_lines is 0) and rect
+        (None: the images are already rectified; it must outlive the session)."""
+        h = self.lib.plstvo_stereo_session_create(self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg),
+                                                  C.byref(ocfg), None if lcfg is None else C.byref(lcfg),
+                                                  None if rect is None else rect.handle, n_streams)
+        if not h:
+            raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
+        ss = StereoSession(self, h, n_streams)
+        self._sessions.append(ss)
+        return ss
+
+    def stereo_session_destroy(self, ss: StereoSession):
+        ss.close()
+        self._sessions = [x for x in self._sessions if x is not ss]
+
+    def stereo_session_initialize(self, ss: StereoSession, ids, frames: dict):
+        ids = np.ascontiguousarray(ids, np.int32)
+        fs, keep = T.stereo_images_as_c(frames)
+        n_stereo = np.zeros((len(ids), 2), np.int32)
+        self._ck(self.lib.plstvo_stereo_session_initialize(self.ctx, ss.handle, len(ids), _p(ids, T.c_int32_p), C.byref(fs),
+                                                           _p(n_stereo, T.c_int32_p)))
+        del keep
+        return n_stereo
+
+    def stereo_session_insert(self, ss: StereoSession, ids, frames: dict, priors=None, results=None):
+        ids = np.ascontiguousarray(ids, np.int32)
+        fs, keep = T.stereo_images_as_c(frames)
+        n = len(ids)
+        if results is None:
+            results = np.zeros(n, dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((n, 4), np.int32)
+        self._ck(self.lib.plstvo_stereo_session_insert(self.ctx, ss.handle, n, _p(ids, T.c_int32_p), C.byref(fs),
+                                                       priors.ctypes.data if priors is not None else None, results.ctypes.data,
+                                                       _p(n_stereo, T.c_int32_p)))
         del keep
         return results, n_stereo
 
