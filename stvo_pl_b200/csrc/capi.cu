@@ -946,21 +946,6 @@ int plstvo_batch_kernel_times(PlContext* ctx, PlDeviceBatch* db, int iters, doub
         tm += a;
         tsv += b;
     }
-    if (getenv("PLSTVO_PHASE_DEBUG") && ws.B > 0) {   // per-phase device cycles of K2 and of the GN loop kernel, averaged over the pairs
-        std::vector<long long> h((size_t)ws.B * PLSTVO_PHASE_SLOTS);
-        int rc2 = ws_phase_pass(ctx, ws, h.data());
-        if (rc2) return rc2;
-        static const char* names[8 + 11] = {"match_finalize", "gather", "gn_eval", "gn_serial", "gates_eig", "outliers", "final",
-                                            "sort_mad", "gl_wait", "gl_eval", "gl_fold", "gl_barrier", "gl_tests", "gl_close",
-                                            "gl_solve", "gl_increment", "gl_trailing", "gl_inv6", "gl_iterations"};
-        for (int k = 0; k < 8 + 2 * 11; ++k) {
-            double sum = 0;
-            for (int p = 0; p < ws.B; ++p) sum += (double)h[(size_t)p * PLSTVO_PHASE_SLOTS + k];
-            if (k < 8) fprintf(stderr, "[plstvo phase] %-15s %10.0f cycles/pair\n", names[k], sum / ws.B);
-            else fprintf(stderr, "[plstvo phase] %-15s stage %d %10.0f %s/pair\n", names[8 + (k - 8) % 11], 1 + (k - 8) / 11,
-                         sum / ws.B, (k - 8) % 11 == 10 ? "iterations" : "cycles");
-        }
-    }
     if (ms_match) *ms_match = tm / iters;
     if (ms_solve) *ms_solve = tsv / iters;
     if (n_tiles) *n_tiles = (int32_t)std::count_if(ws.problems.begin(), ws.problems.end(),

@@ -89,7 +89,7 @@ struct SolveParams {
     int32_t  cap_pt, cap_ls;  // capacity of the SoA arrays (max matched features per pair in this launch)
     int32_t  sort_cap;        // power of two >= max(cap_pt, cap_ls)
     int32_t  feat_in_smem;
-    long long* phase_cycles;  // optional [pairs][PLSTVO_PHASE_SLOTS] debug timers (PLSTVO_PHASE_DEBUG), else null
+    long long* phase_cycles;  // optional [pairs][PLSTVO_PHASE_SLOTS] cycle counters (plstvo_batch_phase_cycles), else null
     const int32_t* only_if;   // optional [pairs]: the CTA of pair p returns at once unless only_if[p] != 0
 };
 

@@ -19,15 +19,10 @@ constexpr int GS_STAGE_BYTES = 16384;
 constexpr int GS_STAGES = 6;
 constexpr int GS_NACC = ACC_N + 1;                     // 21 H + 6 g + e + count
 
-#ifdef GS_EXACT_MATH   // A/B build: IEEE division / square root instead of the approximate SFU forms
-__device__ __forceinline__ float gs_rcp(float x) { return __frcp_rn(x); }
-__device__ __forceinline__ float gs_sqrt(float x) { return __fsqrt_rn(x); }
-__device__ __forceinline__ float gs_rsqrt(float x) { return __frcp_rn(__fsqrt_rn(x)); }
-#else
+// the approximate SFU forms of division and square root
 __device__ __forceinline__ float gs_rcp(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float gs_sqrt(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float gs_rsqrt(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-#endif
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }

@@ -143,7 +143,7 @@ struct Workspace {
     DevBuf d_lssP, d_lseP, d_lsspl, d_lsepl, d_lss2, d_lslev, d_lsle;  // prev ...; curr le
     DevBuf d_priors, d_results, d_m12p, d_m12l, d_inlp, d_inll;
     DevBuf d_rowpart, d_colpart, d_problems, d_feat;
-    DevBuf d_phase;   // debug phase timers (PLSTVO_PHASE_DEBUG)
+    DevBuf d_phase;   // solver phase cycle counters (plstvo_batch_phase_cycles)
     // K1 (match_tc.cu): per-block value partials, work items
     std::vector<TcProblem> tc_problems;   // [2B], parallel to `problems`
     std::vector<TcItem> tc_items[2];      // work items of the point problems (long) and of the line problems (short)

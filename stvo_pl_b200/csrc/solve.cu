@@ -34,6 +34,18 @@ struct Feat {
 };
 constexpr int PT_ARRAYS = 6, LS_ARRAYS = 13;
 
+// the point and line arrays inside a list buffer fb of k2_feat_stride(cp, cl) doubles; flags and counts are the caller's to set.
+// Returned, not filled in through a reference: a callee that takes the address of K2's Feat costs K2 spill bytes.
+__device__ __forceinline__ Feat feat_view(double* fb, int cp, int cl) {
+    Feat f;
+    f.Px = fb; f.Py = fb + cp; f.Pz = fb + 2 * cp; f.pu = fb + 3 * cp; f.pv = fb + 4 * cp; f.pss = fb + 5 * cp;
+    double* lb = fb + PT_ARRAYS * (size_t)cp;
+    f.sX = lb; f.sY = lb + cl; f.sZ = lb + 2 * cl; f.eX = lb + 3 * cl; f.eY = lb + 4 * cl; f.eZ = lb + 5 * cl;
+    f.l0 = lb + 6 * cl; f.l1 = lb + 7 * cl; f.l2 = lb + 8 * cl; f.oa = lb + 9 * cl; f.ob = lb + 10 * cl;
+    f.oc = lb + 11 * cl; f.lss = lb + 12 * cl;
+    return f;
+}
+
 struct State {
     double red[K2_WARPS][32];
     double acc[32];          // reduced sums: H upper triangle (21), g (6), e (1), count (1)
@@ -1097,28 +1109,24 @@ __device__ __forceinline__ double unpack_normal_equations(State& st, int lane) {
     return st.acc[27] / st.acc[28];   // e /= (N_l + N_p)  (:692)
 }
 
-// warp 0: DT << DT * inverse_se3(expmap_se3(inc))  (:419); every lane computes, lanes 0..15 store
-__device__ __forceinline__ void apply_increment(double* DTs, const double* inc, int lane) {
-    double E[16], Ei[16], D[16], R[16];
+// the new pose of an increment in the calling thread's registers: R = D * inverse_se3(expmap_se3(inc))  (:419)
+__device__ __forceinline__ void increment_regs(const double* D, const double* inc, double* R) {
+    double E[16], Ei[16];
     expmap_se3(inc, E);
     inverse_se3(E, Ei);
-#pragma unroll
-    for (int i = 0; i < 16; i++) D[i] = DTs[i];
     mat4_mul(D, Ei, R);
+}
+
+// warp 0: DT << DT * inverse_se3(expmap_se3(inc))  (:419); every lane computes, lanes 0..15 store
+__device__ __forceinline__ void apply_increment(double* DTs, const double* inc, int lane) {
+    double R[16];
+    increment_regs(DTs, inc, R);
     __syncwarp();
     double mine = R[0];
 #pragma unroll
     for (int i = 1; i < 16; i++) mine = (lane == i) ? R[i] : mine;
     if (lane < 16) DTs[lane] = mine;
     __syncwarp();
-}
-
-// apply_increment's new pose in the calling thread's registers: R = D * inverse_se3(expmap_se3(inc)), the same operations
-__device__ __forceinline__ void increment_regs(const double* D, const double* inc, double* R) {
-    double E[16], Ei[16];
-    expmap_se3(inc, E);
-    inverse_se3(E, Ei);
-    mat4_mul(D, Ei, R);
 }
 
 // gaussNewtonOptimization (:394-431) and gaussNewtonOptimizationRobust (:433-480).
@@ -1205,6 +1213,39 @@ __device__ void gauss_newton(const Feat& f, State& st, double* sortbuf, const Ca
     __syncthreads();
 }
 
+// removeOutliers (:988-1067) after the median and MAD, for one list of n entries: the trimmed mean of the residuals, the threshold,
+// and the flags that go from 1 to 0, taken off n_inl (shared).  residual(i): entry i's residual, formed only for an entry still
+// flagged; drop(i): told of every flag cleared.  Block-wide.
+template <class Res, class Drop>
+__device__ __forceinline__ void outlier_flags(State& st, int n, double stdv, const PlConfig& cfg, uint8_t* inl, int& n_inl,
+                                              Res residual, Drop drop) {
+    const int tid = threadIdx.x, nth = blockDim.x;
+    // mean of the residuals below 2 stdv if there are enough of them, else plain mean (auxiliar.cpp:406-427)
+    double s[3] = {0.0, 0.0, 0.0};
+    for (int i = tid; i < n; i += nth) {
+        const double r = residual(i);
+        s[2] += r;
+        if (r < 2.0 * stdv) {
+            s[0] += r;
+            s[1] += 1.0;
+        }
+    }
+    block_sum<3>(st, s);
+    const int k = (int)s[1];
+    const double mean = (k >= (int)(0.2 * (double)n)) ? s[0] / (double)k : s[2] / (double)n;
+    const double th = cfg.inlier_k * stdv;
+    double removed[1] = {0.0};
+    for (int i = tid; i < n; i += nth)
+        if (inl[i] && fabs(residual(i) - mean) > th) {
+            inl[i] = 0;
+            removed[0] += 1.0;
+            drop(i);
+        }
+    block_sum<1>(st, removed);
+    if (tid == 0) n_inl -= (int)removed[0];
+    __syncthreads();
+}
+
 // removeOutliers (:988-1067) for LONG lists (the streamed solver: 8000 + 2000 entries): res_pt(i) / res_ls(i) = |e| sqrt(sigma2)
 // of matched feature i at the stage-1 pose, each formed ONCE, straight into shared memory; median and MAD by radix selection
 // (a full bitonic sort of 8192 doubles through shared memory costs 10x more).  Same order statistics, same flags as
@@ -1235,35 +1276,9 @@ __device__ void remove_outliers_select(const Feat& f, State& st, double* sortbuf
         const double mad = block_select_wide(sel, st, n, n / 2, [&](int i) -> double { return (double)fabsf((float)(sortbuf[i] - median)); });
         const double stdv = 1.4826 * mad;
         if (tid == 0) st.tc[7] += clock64() - t_s;
-        // mean of the residuals below 2 stdv if there are enough of them, else plain mean (auxiliar.cpp:406-427)
-        double s[3] = {0.0, 0.0, 0.0};
-        for (int i = tid; i < n; i += nth) {
-            const double r = residual(i);
-            s[2] += r;
-            if (r < 2.0 * stdv) {
-                s[0] += r;
-                s[1] += 1.0;
-            }
-        }
-        block_sum<3>(st, s);
-        const int k = (int)s[1];
-        const double mean = (k >= (int)(0.2 * (double)n)) ? s[0] / (double)k : s[2] / (double)n;
-        const double th = cfg.inlier_k * stdv;
-        double removed[1] = {0.0};
-        uint8_t* inl = type ? f.inl_l : f.inl_p;
-#pragma unroll 4
-        for (int i = tid; i < n; i += nth)
-            if (fabs(residual(i) - mean) > th && inl[i]) {
-                inl[i] = 0;
-                removed[0] += 1.0;
-                if (type == 0) drop_pt(i); else drop_ls(i);
-            }
-        block_sum<1>(st, removed);
-        if (tid == 0) {
-            if (type == 0) st.n_inl_p -= (int)removed[0];
-            else st.n_inl_l -= (int)removed[0];
-        }
-        __syncthreads();
+        outlier_flags(st, n, stdv, cfg, type ? f.inl_l : f.inl_p, type ? st.n_inl_l : st.n_inl_p, residual, [&](int i) {
+            if (type == 0) drop_pt(i); else drop_ls(i);
+        });
     }
 }
 
@@ -1291,33 +1306,7 @@ __device__ void remove_outliers(const Feat& f, State& st, double* sortbuf, const
         double median, stdv;
         median_mad(sortbuf, n, median, stdv);
         if (tid == 0) st.tc[7] += clock64() - t_s;
-        // mean of the residuals below 2 stdv if there are enough of them, else plain mean (auxiliar.cpp:406-427)
-        double s[3] = {0.0, 0.0, 0.0};
-        for (int i = tid; i < n; i += nth) {
-            const double r = residual(i);
-            s[2] += r;
-            if (r < 2.0 * stdv) {
-                s[0] += r;
-                s[1] += 1.0;
-            }
-        }
-        block_sum<3>(st, s);
-        const int k = (int)s[1];
-        const double mean = (k >= (int)(0.2 * (double)n)) ? s[0] / (double)k : s[2] / (double)n;
-        const double th = cfg.inlier_k * stdv;
-        double removed[1] = {0.0};
-        uint8_t* inl = type ? f.inl_l : f.inl_p;
-        for (int i = tid; i < n; i += nth)
-            if (inl[i] && fabs(residual(i) - mean) > th) {
-                inl[i] = 0;
-                removed[0] += 1.0;
-            }
-        block_sum<1>(st, removed);
-        if (tid == 0) {
-            if (type == 0) st.n_inl_p -= (int)removed[0];
-            else st.n_inl_l -= (int)removed[0];
-        }
-        __syncthreads();
+        outlier_flags(st, n, stdv, cfg, type ? f.inl_l : f.inl_p, type ? st.n_inl_l : st.n_inl_p, residual, [](int) {});
     }
 }
 
@@ -1610,6 +1599,50 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
     }
 }
 
+// warp 0: the initial pose of optimizePose (:317-326), the prior's DT if the motion model is on and the prior passes
+// isGoodSolution, else the identity; returns entry `lane` of it to lanes 0..15.  Stages the prior in st.DT0 and st.H.
+__device__ __forceinline__ double warp_initial_pose(State& st, const PlPrior* prior, const PlConfig& cfg, int lane) {
+    bool use_prior = false;
+    if (cfg.use_motion_model && prior) {
+        if (lane < 16) st.DT0[lane] = prior->DT[lane];
+        for (int i = lane; i < 36; i += 32) st.H[i] = prior->DT_cov[i];
+        __syncwarp();
+        use_prior = warp_is_good_solution(st.DT0, st.H, prior->err_norm, nullptr);
+        __syncwarp();
+    }
+    return (use_prior && lane < 16) ? st.DT0[lane] : ((lane % 5 == 0) ? 1.0 : 0.0);
+}
+
+// after a block barrier: the result record (cooperatively; sizeof(PlPoseResult) is a multiple of 8) and the inlier flags of the
+// np + nl list entries in the caller's indexing from slot first_p / first_l: entry k at midx[k] in mode 0, where the n1p + n1l
+// flags of the previous frame's features are cleared first, and at k in mode 1.  Block-wide; nth = blockDim.x as the kernel read
+// it on entry (read here instead, K2 spills more).
+__device__ __forceinline__ void write_result(const SolveParams& prm, int pair, const PlPoseResult& out, const uint8_t* flag_p,
+                                             const uint8_t* flag_l, const uint16_t* midx_p, const uint16_t* midx_l, int np, int nl,
+                                             int n1p, int n1l, size_t first_p, size_t first_l, int nth) {
+    const int tid = threadIdx.x;
+    __syncthreads();
+    const uint64_t* src = reinterpret_cast<const uint64_t*>(&out);
+    uint64_t* dst = reinterpret_cast<uint64_t*>(&prm.results[pair]);
+    for (int i = tid; i < (int)(sizeof(PlPoseResult) / 8); i += nth) dst[i] = src[i];
+    if (prm.mode == 0) {
+        if (prm.inlier_pt)
+            for (int i = tid; i < n1p; i += nth) prm.inlier_pt[first_p + i] = 0;
+        if (prm.inlier_ls)
+            for (int i = tid; i < n1l; i += nth) prm.inlier_ls[first_l + i] = 0;
+        __syncthreads();
+        if (prm.inlier_pt)
+            for (int k = tid; k < np; k += nth) prm.inlier_pt[first_p + midx_p[k]] = flag_p[k];
+        if (prm.inlier_ls)
+            for (int k = tid; k < nl; k += nth) prm.inlier_ls[first_l + midx_l[k]] = flag_l[k];
+    } else {
+        if (prm.inlier_pt)
+            for (int k = tid; k < np; k += nth) prm.inlier_pt[first_p + k] = flag_p[k];
+        if (prm.inlier_ls)
+            for (int k = tid; k < nl; k += nth) prm.inlier_ls[first_l + k] = flag_l[k];
+    }
+}
+
 __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveParams prm) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5;
@@ -1621,21 +1654,15 @@ __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveP
     size_t off = align_up(sizeof(State), 16);
     double* sortbuf = reinterpret_cast<double*>(smem + off);
     off += (size_t)prm.sort_cap * sizeof(double);
-    Feat f;
-    f.inl_p = smem + off;  off += align_up((size_t)prm.cap_pt, 16);
-    f.inl_l = smem + off;  off += align_up((size_t)prm.cap_ls, 16);
+    uint8_t* inl_p = smem + off;  off += align_up((size_t)prm.cap_pt, 16);
+    uint8_t* inl_l = smem + off;  off += align_up((size_t)prm.cap_ls, 16);
     uint16_t* midx_p = reinterpret_cast<uint16_t*>(smem + off);  off += align_up((size_t)prm.cap_pt * 2, 16);
     uint16_t* midx_l = reinterpret_cast<uint16_t*>(smem + off);  off += align_up((size_t)prm.cap_ls * 2, 16);
-    double* fb = prm.feat_in_smem ? reinterpret_cast<double*>(smem + off)
-                                  : prm.feat_scratch + (size_t)blockIdx.x * prm.feat_scratch_stride;
-    {
-        const int cp = prm.cap_pt, cl = prm.cap_ls;
-        f.Px = fb; f.Py = fb + cp; f.Pz = fb + 2 * cp; f.pu = fb + 3 * cp; f.pv = fb + 4 * cp; f.pss = fb + 5 * cp;
-        double* lb = fb + PT_ARRAYS * (size_t)cp;
-        f.sX = lb; f.sY = lb + cl; f.sZ = lb + 2 * cl; f.eX = lb + 3 * cl; f.eY = lb + 4 * cl; f.eZ = lb + 5 * cl;
-        f.l0 = lb + 6 * cl; f.l1 = lb + 7 * cl; f.l2 = lb + 8 * cl; f.oa = lb + 9 * cl; f.ob = lb + 10 * cl;
-        f.oc = lb + 11 * cl; f.lss = lb + 12 * cl;
-    }
+    Feat f = feat_view(prm.feat_in_smem ? reinterpret_cast<double*>(smem + off)
+                                        : prm.feat_scratch + (size_t)blockIdx.x * prm.feat_scratch_stride,
+                       prm.cap_pt, prm.cap_ls);
+    f.inl_p = inl_p;
+    f.inl_l = inl_l;
     const PlConfig& cfg = prm.cfg;
     const Cam cam = {prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
 
@@ -1662,18 +1689,10 @@ __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveP
             st.err = -1.0;
         }
         for (int i = lane; i < 36; i += 32) st.cov[i] = 0.0;
-        bool use_prior = false;
-        if (cfg.use_motion_model && prior) {   // :317-324
-            if (lane < 16) st.DT0[lane] = prior->DT[lane];
-            for (int i = lane; i < 36; i += 32) st.H[i] = prior->DT_cov[i];   // staging for the gate
-            __syncwarp();
-            use_prior = warp_is_good_solution(st.DT0, st.H, prior->err_norm, nullptr);
-            __syncwarp();
-        }
+        const double d = warp_initial_pose(st, prior, cfg, lane);
         if (lane < 16) {
-            const double v = use_prior ? st.DT0[lane] : ((lane % 5 == 0) ? 1.0 : 0.0);
-            st.DT0[lane] = v;
-            st.DT[lane] = v;
+            st.DT0[lane] = d;
+            st.DT[lane] = d;
         }
         if (lane == 0) st.ctrl = (st.n_inl_p + st.n_inl_l >= cfg.min_features) ? 1 : 0;
     }
@@ -1728,31 +1747,7 @@ __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveP
 
     // ---- pose finalisation (:372-391), warp 0 ----
     if (warp == 0) finalize_pose(st, prior, f, lane, prm.phase_cycles ? prm.phase_cycles + (size_t)pair * PLSTVO_PHASE_SLOTS : nullptr);
-    __syncthreads();
-    {   // result struct -> HBM, cooperatively (sizeof(PlPoseResult) is a multiple of 8)
-        const uint64_t* src = reinterpret_cast<const uint64_t*>(&st.out);
-        uint64_t* dst = reinterpret_cast<uint64_t*>(&prm.results[pair]);
-        for (int i = tid; i < (int)(sizeof(PlPoseResult) / 8); i += nth) dst[i] = src[i];
-    }
-    // ---- inlier flags back to the caller's indexing ----
-    if (prm.mode == 0) {
-        if (prm.inlier_pt) {
-            for (int i = tid; i < n1p; i += nth) prm.inlier_pt[out_p0 + i] = 0;
-        }
-        if (prm.inlier_ls) {
-            for (int i = tid; i < n1l; i += nth) prm.inlier_ls[out_l0 + i] = 0;
-        }
-        __syncthreads();
-        if (prm.inlier_pt)
-            for (int k = tid; k < f.np; k += nth) prm.inlier_pt[out_p0 + midx_p[k]] = f.inl_p[k];
-        if (prm.inlier_ls)
-            for (int k = tid; k < f.nl; k += nth) prm.inlier_ls[out_l0 + midx_l[k]] = f.inl_l[k];
-    } else {
-        if (prm.inlier_pt)
-            for (int k = tid; k < f.np; k += nth) prm.inlier_pt[out_p0 + k] = f.inl_p[k];
-        if (prm.inlier_ls)
-            for (int k = tid; k < f.nl; k += nth) prm.inlier_ls[out_l0 + k] = f.inl_l[k];
-    }
+    write_result(prm, pair, st.out, f.inl_p, f.inl_l, midx_p, midx_l, f.np, f.nl, n1p, n1l, out_p0, out_l0, nth);
 }
 
 // test hook: the warp-level 6x6 routines on caller-supplied matrices (one warp per problem)
@@ -1829,19 +1824,12 @@ __device__ __forceinline__ StreamView stream_view(const SolveParams& prm, const 
     v.sortbuf = reinterpret_cast<double*>(smem + align_up(sizeof(State), 16));
     v.slot_p = (size_t)(prm.mode == 0 ? prm.prev.pt_off[pair] : prm.matched.pt_off[pair]);
     v.slot_l = (size_t)(prm.mode == 0 ? prm.prev.ls_off[pair] : prm.matched.ls_off[pair]);
+    v.f = feat_view(prm.feat_scratch + (size_t)local * prm.feat_scratch_stride, prm.cap_pt, prm.cap_ls);
     v.f.inl_p = sb.flag_pt + v.slot_p;
     v.f.inl_l = sb.flag_ls + v.slot_l;
+    v.f.np = v.f.nl = 0;
     v.midx_p = sb.midx_pt + v.slot_p;
     v.midx_l = sb.midx_ls + v.slot_l;
-    double* fb = prm.feat_scratch + (size_t)local * prm.feat_scratch_stride;
-    const int cp = prm.cap_pt, cl = prm.cap_ls;
-    Feat& f = v.f;
-    f.Px = fb; f.Py = fb + cp; f.Pz = fb + 2 * cp; f.pu = fb + 3 * cp; f.pv = fb + 4 * cp; f.pss = fb + 5 * cp;
-    double* lb = fb + PT_ARRAYS * (size_t)cp;
-    f.sX = lb; f.sY = lb + cl; f.sZ = lb + 2 * cl; f.eX = lb + 3 * cl; f.eY = lb + 4 * cl; f.eZ = lb + 5 * cl;
-    f.l0 = lb + 6 * cl; f.l1 = lb + 7 * cl; f.l2 = lb + 8 * cl; f.oa = lb + 9 * cl; f.ob = lb + 10 * cl;
-    f.oc = lb + 11 * cl; f.lss = lb + 12 * cl;
-    f.np = f.nl = 0;
     return v;
 }
 
@@ -1874,16 +1862,8 @@ __global__ void __launch_bounds__(SPREP_THREADS, 3) stream_prepare_kernel(const 
     const PlPrior* prior = prm.priors ? &prm.priors[pair] : nullptr;
     StreamCtl& c = sb.ctl[local];
     if (warp == 0) {
-        bool use_prior = false;
-        if (cfg.use_motion_model && prior) {   // :317-324
-            if (lane < 16) st.DT0[lane] = prior->DT[lane];
-            for (int i = lane; i < 36; i += 32) st.H[i] = prior->DT_cov[i];
-            __syncwarp();
-            use_prior = warp_is_good_solution(st.DT0, st.H, prior->err_norm, nullptr);
-            __syncwarp();
-        }
+        const double d = warp_initial_pose(st, prior, cfg, lane);
         if (lane < 16) {
-            const double d = use_prior ? st.DT0[lane] : ((lane % 5 == 0) ? 1.0 : 0.0);
             c.DT0[lane] = d;
             sb.DT[(size_t)local * 16 + lane] = d;
         }
@@ -1945,18 +1925,12 @@ __device__ void exact_error_partial(const Feat& f, const double* DT, const Cam& 
 // the warps, runs the stop tests / 6x6 solve / SE(3) update in double and publishes the new pose.  No grid-wide step between
 // iterations: while one CTA of an SM solves its 6x6 system the other keeps the memory pipe busy, so the launch as a whole
 // streams at HBM speed.  One launch replaces max_iters x (sweep + reduce + step).
-#ifndef GL_FOLD_TILES
-#define GL_FOLD_TILES 4
-#endif
-constexpr int GL_FOLD = GL_FOLD_TILES;
-// CTA shape of the GN loop kernel: consumer warps, ring stages, CTAs per SM (three digits).  862 keeps a KITTI-size problem's
-// records resident in the ring.  434 (twice the problems in flight per SM, records re-streamed from L2 every iteration) was
-// measured: the kernel alone gets faster at C2 (0.262 -> 0.227 ms per 512 problems) but the pass as a whole does not (two solver
-// chains already run side by side), and C5's stage 2 gets slower (0.45 -> 0.51 ms).
-#ifndef GL_SHAPE
-#define GL_SHAPE 862
-#endif
-constexpr int GL_CWARPS = GL_SHAPE / 100, GL_STAGES = (GL_SHAPE / 10) % 10, GL_MINBLOCKS = GL_SHAPE % 10;
+constexpr int GL_FOLD = 4;   // the consumers fold their fp32 partials to fp64 every GL_FOLD tiles
+// CTA shape of the GN loop kernel: 8 consumer warps, 6 ring stages, 2 CTAs per SM ("862").  It keeps a KITTI-size problem's
+// records resident in the ring.  434 (4 warps, 3 stages, 4 CTAs: twice the problems in flight per SM, records re-streamed from L2
+// every iteration) was measured: the kernel alone gets faster at C2 (0.262 -> 0.227 ms per 512 problems) but the pass as a whole
+// does not (two solver chains already run side by side), and C5's stage 2 gets slower (0.45 -> 0.51 ms).
+constexpr int GL_CWARPS = 8, GL_STAGES = 6, GL_MINBLOCKS = 2;
 constexpr int GL_CONSUMERS = GL_CWARPS * 32, GL_THREADS = GL_CONSUMERS + 32;
 // relative half-width of the "could go either way" band of the error tests: it must hold the fp32-summed error's deviation from
 // the fp64 error at the same pose (measured > 1.5e-7) plus the trajectory's (0.8e-7 .. 5e-7 of err, tests/test_gpu_stream_decisions.py)
@@ -2203,20 +2177,11 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
             mark(GLP_TRAIL);
             int flags = s_flags;                // rewritten by warp 0 only after the next iteration's first barrier
             if (flags & GL_CLOSE) {            // block-uniform, rare (about one problem in a hundred, once)
-                Feat f;
-                {
-                    double* fb = feat_scratch + (size_t)p * feat_stride;
-                    const int cp = cap_pt, cl = cap_ls;
-                    f.Px = fb; f.Py = fb + cp; f.Pz = fb + 2 * cp; f.pu = fb + 3 * cp; f.pv = fb + 4 * cp; f.pss = fb + 5 * cp;
-                    double* lb = fb + PT_ARRAYS * (size_t)cp;
-                    f.sX = lb; f.sY = lb + cl; f.sZ = lb + 2 * cl; f.eX = lb + 3 * cl; f.eY = lb + 4 * cl; f.eZ = lb + 5 * cl;
-                    f.l0 = lb + 6 * cl; f.l1 = lb + 7 * cl; f.l2 = lb + 8 * cl; f.oa = lb + 9 * cl; f.ob = lb + 10 * cl;
-                    f.oc = lb + 11 * cl; f.lss = lb + 12 * cl;
-                    f.inl_p = sb.flag_pt + p0;
-                    f.inl_l = sb.flag_ls + l0;
-                    f.np = np;
-                    f.nl = nl;
-                }
+                Feat f = feat_view(feat_scratch + (size_t)p * feat_stride, cap_pt, cap_ls);
+                f.inl_p = sb.flag_pt + p0;
+                f.inl_l = sb.flag_ls + l0;
+                f.np = np;
+                f.nl = nl;
                 const Cam camd = {cam.fx, cam.fy, cam.cx, cam.cy};
                 double v[4];
                 exact_error_partial(f, sDT, camd, v[0], v[1]);
@@ -2400,30 +2365,8 @@ __global__ void __launch_bounds__(256) stream_finalize_kernel(const SolveParams 
         __syncwarp();
         finalize_pose(st, prior, f, lane, nullptr);
     }
-    __syncthreads();
-    {
-        const uint64_t* src = reinterpret_cast<const uint64_t*>(&st.out);
-        uint64_t* dst = reinterpret_cast<uint64_t*>(&prm.results[pair]);
-        for (int i = tid; i < (int)(sizeof(PlPoseResult) / 8); i += nth) dst[i] = src[i];
-    }
-    const uint8_t* fp = sb.flag_pt + slot_p;
-    const uint8_t* fl = sb.flag_ls + slot_l;
-    if (prm.mode == 0) {
-        if (prm.inlier_pt)
-            for (int i = tid; i < n1p; i += nth) prm.inlier_pt[slot_p + i] = 0;
-        if (prm.inlier_ls)
-            for (int i = tid; i < n1l; i += nth) prm.inlier_ls[slot_l + i] = 0;
-        __syncthreads();
-        if (prm.inlier_pt)
-            for (int k = tid; k < c.np; k += nth) prm.inlier_pt[slot_p + sb.midx_pt[slot_p + k]] = fp[k];
-        if (prm.inlier_ls)
-            for (int k = tid; k < c.nl; k += nth) prm.inlier_ls[slot_l + sb.midx_ls[slot_l + k]] = fl[k];
-    } else {
-        if (prm.inlier_pt)
-            for (int k = tid; k < c.np; k += nth) prm.inlier_pt[slot_p + k] = fp[k];
-        if (prm.inlier_ls)
-            for (int k = tid; k < c.nl; k += nth) prm.inlier_ls[slot_l + k] = fl[k];
-    }
+    write_result(prm, pair, st.out, sb.flag_pt + slot_p, sb.flag_ls + slot_l, sb.midx_pt + slot_p, sb.midx_ls + slot_l, f.np, f.nl,
+                 n1p, n1l, slot_p, slot_l, nth);
 }
 
 }  // namespace

@@ -12,7 +12,7 @@ import numpy as np
 from . import types as T
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("PLSTVO_LIB") or os.path.join(_HERE, "lib", "libplstvo_b200.so")   # PLSTVO_LIB: A/B builds
+LIB_PATH = os.environ.get("PLSTVO_LIB") or os.path.join(_HERE, "lib", "libplstvo_b200.so")   # PLSTVO_LIB: another build to load
 PHASE_SLOTS = 32   # PLSTVO_PHASE_SLOTS
 
 ERRORS = {-1: "PLSTVO_E_INVALID", -2: "PLSTVO_E_TOO_LARGE", -3: "PLSTVO_E_CUDA", -4: "PLSTVO_E_NO_DEVICE",

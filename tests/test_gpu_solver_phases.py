@@ -1,4 +1,4 @@
-"""The streamed solver's cycle counters (plstvo_batch_phase_cycles, PLSTVO_PHASE_DEBUG): the timed instantiation of the GN loop
+"""The streamed solver's cycle counters (plstvo_batch_phase_cycles): the timed instantiation of the GN loop
 kernel computes exactly what the shipped one computes on bench.py's C2 workload, and every phase it times is counted."""
 import os
 
@@ -19,7 +19,7 @@ def _same(a, b):
 
 
 @pytest.mark.gpu
-def test_phase_pass_matches_plain_pass(engine, monkeypatch):
+def test_phase_pass_matches_plain_pass(engine):
     prev, curr, _, cam = make_workload(512, 0)
     db = engine.upload(cam, workload_config(), prev, curr)
     try:
@@ -28,8 +28,7 @@ def test_phase_pass_matches_plain_pass(engine, monkeypatch):
         cyc = db.phase_cycles()
         timed = db.download()
         _same(plain, timed)
-        monkeypatch.setenv("PLSTVO_PHASE_DEBUG", "1")
-        db.kernel_times(iters=1)           # its last solve pass is the timed one
+        db.kernel_times(iters=1)           # a pass after the timed one computes the same again
         _same(plain, db.download())
     finally:
         db.free()

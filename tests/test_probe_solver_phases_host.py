@@ -41,6 +41,20 @@ def test_phase_table():
     assert s2["problems"] == 1 and s2["fold"]["median"] == 5
 
 
+def test_k2_table(capsys):
+    cyc = np.zeros((4, 32), np.int64)
+    cyc[0, :8] = [10, 20, 300, 40, 5, 60, 7, 30]
+    cyc[2, :8] = [30, 40, 500, 80, 15, 100, 9, 50]
+    cyc[3, P.GL_FIRST + P.GL_N - 1] = 4               # a streamed pair: its K2 slots stay zero
+    t = P.k2_table(cyc)
+    assert t["pairs"] == 2 and list(t)[1:] == P.K2_PHASES
+    assert t["gn_eval"]["median"] == 400 and t["sort_mad"]["median"] == 40 and t["match_finalize"]["p90"] == 28
+    P.print_k2_table(t, None)
+    out = capsys.readouterr().out
+    assert "K2: 2 pairs" in out and all(n in out for n in P.K2_PHASES)
+    assert P.k2_table(np.zeros((2, 32), np.int64)) == {"pairs": 0}
+
+
 def test_pass_report():
     def k(name, stream, a, b):
         return {"name": name, "stream": stream, "ts": a, "end": b}

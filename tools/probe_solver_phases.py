@@ -2,8 +2,8 @@
 
 Mode `phases` runs one solve pass with the GN loop kernel's cycle counters on (plstvo_batch_phase_cycles; the pass computes
 what the plain pass computes) and prints, per GN stage, the cycles of each phase per iteration (median and p90 over the
-problems of the batch), the iterations per stage, and the whole-kernel times of the other streamed-solver kernels (CUDA
-events).  Mode `trace` records a torch.profiler CUDA-activity trace of a few resident passes (what bench.py times) into the
+problems of the batch), the iterations per stage, K2's cycles per phase over the pairs it solved, and the whole-kernel times of
+the other streamed-solver kernels (CUDA events).  Mode `trace` records a torch.profiler CUDA-activity trace of a few resident passes (what bench.py times) into the
 output directory and reports, per pass and stream, when each kernel started and ended, and how much of the pass is solver
 time after the last matcher kernel has ended.  Both print the card, its power limit and the SM clock sampled in the run.
 
@@ -29,6 +29,8 @@ sys.path.insert(0, ROOT)
 PHASES = ["wait", "eval", "fold", "barrier", "tests", "close", "solve", "increment", "trailing", "inv6"]
 PER_CALL = {"wait", "inv6"}          # once per call (the first iteration's record load, the end-of-call covariance)
 GL_FIRST, GL_N = 8, 11                # include/plstvo.h, PLSTVO_PHASE_SLOTS
+# K2's slots 0 .. GL_FIRST - 1, cycles per pair (sort_mad is part of outliers)
+K2_PHASES = ["match_finalize", "gather", "gn_eval", "gn_serial", "gates_eig", "outliers", "final", "sort_mad"]
 MATCHER = ("tc_hamming_kernel", "tc_resolve_kernel")
 SOLVER = ("stream_prepare_kernel", "gn_loop_stream_kernel", "stream_outlier_kernel", "stream_finalize_kernel",
           "track_solve_kernel")
@@ -80,6 +82,30 @@ def phase_table(cyc):
     return out
 
 
+def k2_table(cyc):
+    """cyc: [B][PHASE_SLOTS] -> {phase: (median, p90) cycles per pair} of K2 over the pairs whose K2 slots are non-zero (the pairs
+    K2 solved: all of them when it is the solver, those handed back to it by the streamed solver otherwise)"""
+    blk = cyc[:, :len(K2_PHASES)].astype(np.float64)
+    ran = (blk != 0).any(axis=1)
+    tab = {"pairs": int(ran.sum())}
+    if ran.any():
+        for k, name in enumerate(K2_PHASES):
+            tab[name] = {"median": float(np.median(blk[ran, k])), "p90": float(np.percentile(blk[ran, k], 90))}
+    return tab
+
+
+def print_k2_table(tab, mhz):
+    if not tab["pairs"]:
+        print("K2: no pair ran")
+        return
+    print(f"K2: {tab['pairs']} pairs")
+    print(f"  {'phase':<20}{'median':>10}{'p90':>10}   cycles per pair" + (f" (us at {mhz:.0f} MHz)" if mhz else ""))
+    for name in K2_PHASES:
+        v = tab[name]
+        us = f"  {v['median'] / mhz:7.2f} us" if mhz else ""
+        print(f"  {name:<20}{v['median']:>10.0f}{v['p90']:>10.0f}{us}")
+
+
 def print_table(tab, mhz):
     for s, st in tab.items():
         if "iterations" not in st:
@@ -107,15 +133,17 @@ def run_phases(db, eng, out):
     clocks = clk.summary()
     np.save(os.path.join(out, "phase_cycles.npy"), cyc)
     tab = phase_table(cyc)
+    k2 = k2_table(cyc)
     kernels = {"stream_prepare_kernel": st["ms_lists"], "gn_loop_stream_kernel stage 1": st["ms_gn_stage1"],
                "stream_outlier_kernel": st["ms_outliers"], "gn_loop_stream_kernel stage 2": st["ms_gn_stage2"],
                "stream_finalize_kernel + handed-back problems":
                    max(st["ms_optimize_pose"] - st["ms_gn_stage1"] - st["ms_gn_stage2"] - st["ms_outliers"], 0.0)}
     print_table(tab, clocks.get("sm_mhz"))
+    print_k2_table(k2, clocks.get("sm_mhz"))
     print("whole kernels (ms, CUDA events, each stage alone over the batch):")
     for k, v in kernels.items():
         print(f"  {k:<48}{v:8.4f}")
-    return {"phases": tab, "kernels_ms": kernels, "clocks": clocks}
+    return {"phases": tab, "k2_phases": k2, "kernels_ms": kernels, "clocks": clocks}
 
 
 def trace_kernels(path):
