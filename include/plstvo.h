@@ -678,6 +678,51 @@ int  plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const in
  * eigenvalues) on n caller-supplied matrices: H [n][36] row-major, g [n][6] -> x [n][6], lad [n], inv [n][36], eig [n][6] */
 int  plstvo_debug_algebra(PlContext* ctx, int n, const double* H, const double* g, double* x, double* lad,
                           double* inv, double* eig);
+/* test hook for the device helpers both pose solvers use to decide and finish a problem, one warp per case, each run on
+ * the same inputs:
+ *   in  [n][PLSTVO_PH_IN]:  H[36] and g[6] (row-major; a solve), cov[36] (row-major; only its lower triangle is read),
+ *                           DT[16], err, Tfw_prev[16], Tfw_cov_prev[36] (isGoodSolution and the pose finalisation),
+ *                           xi[6] = [t; w] (expmap_se3), T[16] (inverse_se3, logmap_se3);
+ *   out [n][PLSTVO_PH_OUT]: the Cholesky fast path with log|det| (x, lad, ok) and without it (x, ok), its all-register
+ *                           copy on H's upper triangle (x, ok), the column-pivoted QR with log|det| (x, lad), the
+ *                           isGoodSolution shortcut's verdict, isGoodSolution without and with the eigenvalues (verdict,
+ *                           ascending eigenvalues), inverse_se3(T), logmap_se3(T), expmap_se3(xi), and the pose
+ *                           finalisation on (DT, cov, err, Tfw_prev, Tfw_cov_prev): good, err_norm, DT, Tfw, Tfw_cov,
+ *                           DT_cov_eig.  Flags are 0.0 / 1.0. */
+#define PLSTVO_PH_IN_H 0
+#define PLSTVO_PH_IN_G 36
+#define PLSTVO_PH_IN_COV 42
+#define PLSTVO_PH_IN_DT 78
+#define PLSTVO_PH_IN_ERR 94
+#define PLSTVO_PH_IN_TFW_PREV 95
+#define PLSTVO_PH_IN_TFW_COV_PREV 111
+#define PLSTVO_PH_IN_XI 147
+#define PLSTVO_PH_IN_T 153
+#define PLSTVO_PH_IN 169
+#define PLSTVO_PH_CHOL_X 0
+#define PLSTVO_PH_CHOL_LAD 6
+#define PLSTVO_PH_CHOL_OK 7
+#define PLSTVO_PH_CHOL0_X 8
+#define PLSTVO_PH_CHOL0_OK 14
+#define PLSTVO_PH_REGS_X 15
+#define PLSTVO_PH_REGS_OK 21
+#define PLSTVO_PH_QR_X 22
+#define PLSTVO_PH_QR_LAD 28
+#define PLSTVO_PH_SURELY 29
+#define PLSTVO_PH_GOOD_FAST 30
+#define PLSTVO_PH_GOOD_FULL 31
+#define PLSTVO_PH_EIG 32
+#define PLSTVO_PH_INV 38
+#define PLSTVO_PH_LOG 54
+#define PLSTVO_PH_EXP 60
+#define PLSTVO_PH_FIN_GOOD 76
+#define PLSTVO_PH_FIN_ERR 77
+#define PLSTVO_PH_FIN_DT 78
+#define PLSTVO_PH_FIN_TFW 94
+#define PLSTVO_PH_FIN_TFW_COV 110
+#define PLSTVO_PH_FIN_EIG 146
+#define PLSTVO_PH_OUT 152
+int  plstvo_debug_pose_helpers(PlContext* ctx, int n, const double* in, double* out);
 /* POPC issue-rate micro-benchmark: returns 32-bit popcounts per second on this device */
 int  plstvo_popc_rate(PlContext* ctx, double* popc_per_s);
 

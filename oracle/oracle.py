@@ -148,6 +148,8 @@ class Oracle:
         L.orc_unccomp_se3.argtypes = [dp, dp, dp, dp]
         L.orc_is_finite.restype = C.c_int
         L.orc_is_finite.argtypes = [dp, C.c_int]
+        L.orc_is_good_solution.restype = C.c_int
+        L.orc_is_good_solution.argtypes = [dp, dp, C.c_double]
         L.orc_vector_mean_stdv_mad.restype = None
         L.orc_vector_mean_stdv_mad.argtypes = [dp, C.c_int, dp, dp]
         L.orc_vector_stdv_mad.restype = C.c_double
@@ -378,6 +380,10 @@ class Oracle:
 
     def eig6_sym(self, A):
         return self._unary("orc_eig6_sym", A, 6)
+
+    def is_good_solution(self, DT, DT_cov, err) -> bool:
+        DT, DT_cov = self._d(DT).ravel(), self._d(DT_cov).ravel()
+        return bool(self.lib.orc_is_good_solution(self._dp(DT), self._dp(DT_cov), float(err)))
 
     def unccomp_se3(self, T1, c1, cinc):
         T1, c1, cinc = self._d(T1).ravel(), self._d(c1).ravel(), self._d(cinc).ravel()

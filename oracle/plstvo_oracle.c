@@ -453,8 +453,10 @@ void orc_eig6_sym(const double Ain[36], double w[6]) {
     }
     for (int i = 0; i < 6; i++) w[i] = A[i * 6 + i];
     qsort(w, 6, sizeof(double), cmp_double);
-    /* NaN input: qsort leaves an arbitrary order; the gate below only asks w[0] < 0 || w[5] > 1,
-     * both false for NaN, exactly like Eigen's NaN eigenvalues. */
+    /* NaN input: the sweep test above is false for a NaN off-diagonal mass, so the loop stops at once and w is A's
+     * diagonal, which can be finite; the gate below then judges that diagonal.  qsort leaves NaN entries in an arbitrary
+     * order, and a NaN w[0] or w[5] passes the gate (both comparisons false).  The device's Jacobi does the same
+     * (solve.cu: warp_eig6_sym).  This is NOT what Eigen's solver does with a NaN entry (DESIGN.md §3). */
 }
 
 /* ------------------------------------------------------------------------------------------------
@@ -1199,6 +1201,7 @@ static int is_good_solution(const double DT[16], const double DT_cov[36], double
     if (w[0] < 0.0 || w[5] > 1.0 || err < 0.0 || err > 1.0 || !orc_is_finite(DT, 16)) return 0;
     return 1;
 }
+int orc_is_good_solution(const double DT[16], const double DT_cov[36], double err) { return is_good_solution(DT, DT_cov, err); }
 
 /* removeOutliers (src/stereoFrameHandler.cpp:988-1067) */
 static int remove_outliers(OrcHandler* h, const double DT[16]) {

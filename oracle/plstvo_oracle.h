@@ -86,6 +86,7 @@ void   orc_logmap_se3(const double T[16], double x[6]);                 /* :143-
 void   orc_adjoint_se3(const double T[16], double Ad[36]);              /* :175-182 */
 void   orc_unccomp_se3(const double T1[16], const double c1[36], const double cinc[36], double out[36]); /* :192-197 */
 int    orc_is_finite(const double* x, int n);                           /* :353-355 */
+int    orc_is_good_solution(const double DT[16], const double DT_cov[36], double err);   /* isGoodSolution, :292-305 */
 void   orc_vector_mean_stdv_mad(const double* res, int n, double* mean, double* stdv); /* :387-430 */
 double orc_vector_stdv_mad(const double* res, int n);                   /* :444-460 */
 double orc_robust_weight_cauchy(double r);                              /* :556-559 */

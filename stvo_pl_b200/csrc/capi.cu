@@ -1081,6 +1081,24 @@ int plstvo_debug_algebra(PlContext* ctx, int n, const double* H, const double* g
     return 0;
 }
 
+int plstvo_debug_pose_helpers(PlContext* ctx, int n, const double* in, double* out) {
+    if (!ctx || n < 0 || !in || !out) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (n == 0) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    const size_t in_b = (size_t)n * PLSTVO_PH_IN * 8, out_b = (size_t)n * PLSTVO_PH_OUT * 8;
+    CK(ctx, ctx->scratch.ensure(in_b + out_b));
+    double* d = ctx->scratch.as<double>();
+    double* dout = d + (size_t)n * PLSTVO_PH_IN;
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, cudaMemcpyAsync(d, in, in_b, cudaMemcpyHostToDevice, s));
+    CK(ctx, launch_pose_helpers_selftest(d, n, dout, s));
+    ctx->launches++;
+    CK(ctx, cudaMemcpyAsync(out, dout, out_b, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return 0;
+}
+
 int plstvo_popc_rate(PlContext* ctx, double* popc_per_s) {
     if (!ctx || !popc_per_s) return PLSTVO_E_INVALID;
     LOCK(ctx);

@@ -134,6 +134,7 @@ cudaError_t launch_select_selftest(const double* v, const int32_t* off, const in
                                    double* out, cudaStream_t stream);
 cudaError_t launch_algebra_selftest(const double* H, const double* g, int n, double* x, double* lad, double* inv,
                                     double* eig, cudaStream_t stream);
+cudaError_t launch_pose_helpers_selftest(const double* in, int n, double* out, cudaStream_t stream);
 cudaError_t launch_popc_bench(uint32_t* out, int iters, int blocks, cudaStream_t stream);
 
 // ---- StVO::matchGrid (match_grid.cu) ---------------------------------------------------------------------------

@@ -1772,6 +1772,102 @@ __global__ void algebra_selftest_kernel(const double* __restrict__ H, const doub
     for (int i = lane; i < 36; i += 32) inv[(size_t)p * 36 + i] = sInv[i];
 }
 
+// test hook: the helpers both pose solvers decide and finish a problem with, on caller-supplied inputs (one warp per case;
+// layouts in include/plstvo.h, plstvo_debug_pose_helpers)
+__global__ void pose_helpers_selftest_kernel(const double* __restrict__ in, int n, double* __restrict__ out) {
+    __shared__ double sH[36], sg[6];
+    __shared__ State st;
+    __shared__ PlPrior pr;
+    const int lane = threadIdx.x & 31, p = blockIdx.x;
+    if (p >= n) return;
+    const double* q = in + (size_t)p * PLSTVO_PH_IN;
+    double* r = out + (size_t)p * PLSTVO_PH_OUT;
+    for (int i = lane; i < 36; i += 32) {
+        sH[i] = q[PLSTVO_PH_IN_H + i];
+        st.cov[i] = q[PLSTVO_PH_IN_COV + i];
+        pr.Tfw_cov[i] = q[PLSTVO_PH_IN_TFW_COV_PREV + i];
+    }
+    if (lane < 6) sg[lane] = q[PLSTVO_PH_IN_G + lane];
+    if (lane < 16) {
+        st.DT[lane] = q[PLSTVO_PH_IN_DT + lane];
+        pr.Tfw[lane] = q[PLSTVO_PH_IN_TFW_PREV + lane];
+    }
+    if (lane < 8) st.tc[lane] = 0;
+    if (lane == 0) {
+        st.err = q[PLSTVO_PH_IN_ERR];
+        st.n_inl_p = st.n_inl_l = 0;
+    }
+    __syncwarp();
+    double x[6], lad = 0.0, w[6], T[16], Y[16], v[6];
+    bool ok = warp_chol6_solve(sH, sg, x, &lad);
+    if (lane == 0) {
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_CHOL_X + i] = x[i];
+        r[PLSTVO_PH_CHOL_LAD] = lad;
+        r[PLSTVO_PH_CHOL_OK] = ok;
+    }
+    ok = warp_chol6_solve(sH, sg, x);
+    if (lane == 0) {
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_CHOL0_X + i] = x[i];
+        r[PLSTVO_PH_CHOL0_OK] = ok;
+    }
+    {
+        double Hu[21];
+        for (int i = 0; i < 6; i++)
+            for (int j = i; j < 6; j++) Hu[tri(i, j)] = sH[i * 6 + j];
+        ok = chol6_solve_regs(Hu, sg, x);
+        if (lane == 0) {
+            for (int i = 0; i < 6; i++) r[PLSTVO_PH_REGS_X + i] = x[i];
+            r[PLSTVO_PH_REGS_OK] = ok;
+        }
+    }
+    warp_qr6_solve<true>(sH, sg, x, lad);
+    if (lane == 0) {
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_QR_X + i] = x[i];
+        r[PLSTVO_PH_QR_LAD] = lad;
+    }
+    ok = cov_surely_inside_unit(st.cov);
+    if (lane == 0) r[PLSTVO_PH_SURELY] = ok;
+    ok = warp_is_good_solution(st.DT, st.cov, st.err, nullptr);
+    if (lane == 0) r[PLSTVO_PH_GOOD_FAST] = ok;
+    ok = warp_is_good_solution(st.DT, st.cov, st.err, w);
+    if (lane == 0) {
+        r[PLSTVO_PH_GOOD_FULL] = ok;
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_EIG + i] = w[i];
+    }
+    for (int i = 0; i < 16; i++) T[i] = q[PLSTVO_PH_IN_T + i];
+    inverse_se3(T, Y);
+    if (lane == 0)
+        for (int i = 0; i < 16; i++) r[PLSTVO_PH_INV + i] = Y[i];
+    logmap_se3(T, v);
+    if (lane == 0)
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_LOG + i] = v[i];
+    for (int i = 0; i < 6; i++) v[i] = q[PLSTVO_PH_IN_XI + i];
+    expmap_se3(v, Y);
+    if (lane == 0)
+        for (int i = 0; i < 16; i++) r[PLSTVO_PH_EXP + i] = Y[i];
+    Feat f;
+    f.np = f.nl = 0;
+    finalize_pose(st, &pr, f, lane, nullptr);
+    __syncwarp();
+    if (lane == 0) {
+        const PlPoseResult& o = st.out;
+        r[PLSTVO_PH_FIN_GOOD] = o.good;
+        r[PLSTVO_PH_FIN_ERR] = o.err_norm;
+        for (int i = 0; i < 16; i++) {
+            r[PLSTVO_PH_FIN_DT + i] = o.DT[i];
+            r[PLSTVO_PH_FIN_TFW + i] = o.Tfw[i];
+        }
+        for (int i = 0; i < 36; i++) r[PLSTVO_PH_FIN_TFW_COV + i] = o.Tfw_cov[i];
+        for (int i = 0; i < 6; i++) r[PLSTVO_PH_FIN_EIG + i] = o.DT_cov_eig[i];
+    }
+}
+
+cudaError_t launch_pose_helpers_selftest(const double* in, int n, double* out, cudaStream_t stream) {
+    if (n <= 0) return cudaSuccess;
+    pose_helpers_selftest_kernel<<<n, 32, 0, stream>>>(in, n, out);
+    return cudaGetLastError();
+}
+
 // test hook: the block-wide radix selection on caller-supplied lists (one 256-thread CTA per list, like the outlier pass); mode 0:
 // the k-th smallest value, mode 1: the k-th smallest of |x - pivot| rounded to float (the MAD form of src/auxiliar.cpp:399-402)
 __global__ void __launch_bounds__(256) select_selftest_kernel(const double* __restrict__ v, const int32_t* __restrict__ off,

@@ -87,6 +87,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_gn_eval_stream": (C.c_int, [vp, cam, cfg, mb, dp, C.c_int, dp, dp, dp, C.POINTER(C.c_float)]),
         "plstvo_popc_rate": (C.c_int, [vp, dp]),
         "plstvo_debug_algebra": (C.c_int, [vp, C.c_int, dp, dp, dp, dp, dp, dp]),
+        "plstvo_debug_pose_helpers": (C.c_int, [vp, C.c_int, dp, dp]),
         "plstvo_debug_select": (C.c_int, [vp, C.c_int, i32p, dp, i32p, dp, C.c_int, dp]),
         "plstvo_debug_tc_partials": (C.c_int, [vp, C.c_int, u8p, i32p, u8p, i32p, C.c_float, u32p, u32p, u32p, u32p]),
         "plstvo_default_orb_config": (None, [C.POINTER(T.PlOrbConfig)]),
@@ -154,7 +155,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_batch_run_timed", "plstvo_batch_download", "plstvo_batch_free", "plstvo_synchronize",
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
     "plstvo_batch_phase_cycles",
-    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_select", "plstvo_debug_tc_partials",
+    "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_pose_helpers",
+    "plstvo_debug_select", "plstvo_debug_tc_partials",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
     "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
@@ -974,6 +976,39 @@ class Engine:
         self._ck(self.lib.plstvo_debug_algebra(self.ctx, n, _p(H, T.c_double_p), _p(g, T.c_double_p), _p(x, T.c_double_p),
                                                _p(lad, T.c_double_p), _p(inv, T.c_double_p), _p(eig, T.c_double_p)))
         return x, lad, inv.reshape(n, 6, 6), eig
+
+    # plstvo_debug_pose_helpers' record layouts (include/plstvo.h, PLSTVO_PH_*): name -> (offset, shape)
+    PH_IN = {"H": (0, (6, 6)), "g": (36, (6,)), "cov": (42, (6, 6)), "DT": (78, (4, 4)), "err": (94, ()),
+             "Tfw_prev": (95, (4, 4)), "Tfw_cov_prev": (111, (6, 6)), "xi": (147, (6,)), "T": (153, (4, 4))}
+    PH_IN_SIZE = 169
+    PH_OUT = {"chol_x": (0, (6,)), "chol_lad": (6, ()), "chol_ok": (7, ()), "chol0_x": (8, (6,)), "chol0_ok": (14, ()),
+              "regs_x": (15, (6,)), "regs_ok": (21, ()), "qr_x": (22, (6,)), "qr_lad": (28, ()), "surely": (29, ()),
+              "good_fast": (30, ()), "good_full": (31, ()), "eig": (32, (6,)), "inv": (38, (4, 4)), "log": (54, (6,)),
+              "exp": (60, (4, 4)), "fin_good": (76, ()), "fin_err": (77, ()), "fin_DT": (78, (4, 4)), "fin_Tfw": (94, (4, 4)),
+              "fin_Tfw_cov": (110, (6, 6)), "fin_eig": (146, (6,))}
+    PH_OUT_SIZE = 152
+
+    def debug_pose_helpers(self, **inputs):
+        """The pose solvers' decision and finishing helpers (test hook), one case per row of the inputs: keyword arrays named as
+        in PH_IN with a leading case axis (missing ones are zero; Tfw_prev and T default to the identity).  Returns a dict of
+        the PH_OUT quantities with the same leading axis; flags as bool."""
+        n = len(next(iter(inputs.values())))
+        rec = np.zeros((n, self.PH_IN_SIZE))
+        for name in ("Tfw_prev", "T"):
+            rec[:, self.PH_IN[name][0]:self.PH_IN[name][0] + 16] = np.eye(4).ravel()
+        for name, a in inputs.items():
+            off, shape = self.PH_IN[name]
+            size = int(np.prod(shape, dtype=np.int64))
+            rec[:, off:off + size] = np.asarray(a, np.float64).reshape(n, size)
+        out = np.zeros((n, self.PH_OUT_SIZE))
+        self._ck(self.lib.plstvo_debug_pose_helpers(self.ctx, n, _p(rec, T.c_double_p), _p(out, T.c_double_p)))
+        res = {}
+        for name, (off, shape) in self.PH_OUT.items():
+            size = int(np.prod(shape, dtype=np.int64))
+            v = out[:, off:off + size].reshape((n,) + shape)
+            res[name] = v.astype(bool) if name in ("chol_ok", "chol0_ok", "regs_ok", "surely", "good_fast", "good_full",
+                                                   "fin_good") else v
+        return res
 
     def synchronize(self):
         self._ck(self.lib.plstvo_synchronize(self.ctx))

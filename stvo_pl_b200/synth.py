@@ -110,16 +110,17 @@ def _line_eq(s, e):
 
 
 def make_pair(shape: Shape, pair_index: int, *, n_pt=None, n_ls=None, overlap=0.7, bitflip=0.10,
-              noise_px=0.5, outlier_frac=0.10, tie_stress=False, seed_offset=0):
+              noise_px=0.5, outlier_frac=0.10, tie_stress=False, seed_offset=0, motion=None):
     """One (prev, curr) frame pair + ground-truth motion.  Returns (prev, curr, T_gt) with prev / curr dicts
-    of per-frame arrays.  `overlap` = fraction of curr rows that are noisy copies of a distinct prev row."""
+    of per-frame arrays.  `overlap` = fraction of curr rows that are noisy copies of a distinct prev row.  `motion` (optional,
+    4x4): the ground-truth motion to use instead of the drawn one (the rest of the pair is drawn as without it)."""
     cam = camera_for(shape.camera)
     n_pt = shape.n_pt if n_pt is None else n_pt
     n_ls = shape.n_ls if n_ls is None else n_ls
     rng = np.random.default_rng(BASE_SEED + 1000 * shape.config_id + pair_index + seed_offset)
     W, H = cam.width, cam.height
     xi = np.concatenate([rng.normal(shape.t_mean, shape.t_std), rng.normal(0.0, shape.w_std, 3)])
-    T_gt = expmap_se3(xi)  # prev-camera -> curr-camera coordinates (P' = R P + t, stereoFrameHandler.cpp:567)
+    T_gt = expmap_se3(xi) if motion is None else np.asarray(motion, np.float64)  # prev-camera -> curr-camera (P' = R P + t, :567)
 
     def depths(n):
         lo, hi = shape.depth

@@ -6,6 +6,7 @@ import re
 import subprocess
 import tempfile
 
+import numpy as np
 import pytest
 
 from conftest import ROOT
@@ -33,6 +34,20 @@ def test_every_declared_symbol_is_exported():
         assert hasattr(lib, n), f"{n} declared in include/plstvo.h but not exported"
     assert sorted(EXPORTED_SYMBOLS) == names          # the binding covers the whole header, nothing more
     assert load_library().plstvo_version() == 100
+
+
+def test_pose_helper_layouts_match_the_header():
+    """plstvo_debug_pose_helpers' record offsets in the binding are the header's PLSTVO_PH_* macros."""
+    txt = open(HEADER).read()
+    defs = {m.group(1): int(m.group(2)) for m in re.finditer(r"#define PLSTVO_PH_(\w+) (\d+)", txt)}
+    assert defs.pop("IN") == Engine.PH_IN_SIZE and defs.pop("OUT") == Engine.PH_OUT_SIZE
+    ins = {k[3:].lower(): v for k, v in defs.items() if k.startswith("IN_")}
+    outs = {k.lower(): v for k, v in defs.items() if not k.startswith("IN_")}
+    assert ins == {k.lower(): off for k, (off, _) in Engine.PH_IN.items()}
+    assert outs == {k.lower(): off for k, (off, _) in Engine.PH_OUT.items()}
+    for layout, size in ((Engine.PH_IN, Engine.PH_IN_SIZE), (Engine.PH_OUT, Engine.PH_OUT_SIZE)):
+        spans = sorted((off, off + int(np.prod(shape, dtype=np.int64))) for off, shape in layout.values())
+        assert spans[0][0] == 0 and spans[-1][1] == size and all(a[1] == b[0] for a, b in zip(spans, spans[1:]))
 
 
 def test_struct_layouts_match_the_header():
