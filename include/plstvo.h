@@ -496,24 +496,38 @@ int plstvo_init_undistort_rectify_map(const PlRectifyModel* model, int width, in
 typedef struct PlRectifier PlRectifier;
 PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, const int16_t* map1_l, const uint16_t* map2_l,
                                      const int16_t* map1_r, const uint16_t* map2_r);
+/* Images of `channels` interleaved 8-bit channels (3: BGR, 4: BGRA, as cv::imread gives them), [height][width][channels]
+ * per image.  With maps (all four non-NULL) the device computes cvtColor(remap(img), COLOR_BGR2GRAY) (Dataset::nextFrame's
+ * rectifyImagesLR, then the detectors' conversion); with all four NULL, cvtColor alone (the reference's dist == false
+ * copy).  The conversion is OpenCV 4.13's for 8-bit data, (3735 B + 19235 G + 9798 R + 2^14) >> 15; alpha is not read.
+ * The maps are held as plstvo_rectifier_create holds them.  Every call that takes a rectifier then takes such images in
+ * place of grey ones and reads nothing else of them.  Returns NULL on failure; PLSTVO_E_INVALID: channels other than 3 or
+ * 4, a size outside 1..32767, some but not all maps NULL (plstvo_last_error says which). */
+PlRectifier* plstvo_rectifier_create_color(PlContext* ctx, int width, int height, int channels,
+                                           const int16_t* map1_l, const uint16_t* map2_l,
+                                           const int16_t* map1_r, const uint16_t* map2_r);
 void plstvo_rectifier_destroy(PlRectifier* rect);
 /* rectifyImagesLR on B pairs: out_l[b] = cv::remap(img_l[b], map1_l, map2_l, INTER_LINEAR, BORDER_CONSTANT, 0), and the
- * same on the right; images [B][height][width] grey of the rectifier's size, host memory in and out.  The weights are
- * OpenCV's INTER_LINEAR table and the sum is rounded as cv::remap rounds it, so the result equals OpenCV's byte for byte.
- * PLSTVO_E_INVALID: a null pointer, B < 0, or a rectifier of another context.  Device memory: 2 bytes per pixel of the call
- * (raw and rectified), kept by the context for the next call. */
+ * same on the right; images [B][height][width][channels] of the rectifier's size and channels in, [B][height][width] grey
+ * out, host memory.  The weights are OpenCV's INTER_LINEAR table and the sum is rounded as cv::remap rounds it, so the result
+ * equals OpenCV's byte for byte.  A colour rectifier converts each remapped image (or, without maps, each image) with
+ * cvtColor(COLOR_BGR2GRAY), byte for byte too.  PLSTVO_E_INVALID: a null pointer, B < 0, or a rectifier of another context.
+ * Device memory: channels + 1 bytes per pixel of the call (raw and grey), kept by the context for the next call. */
 int plstvo_rectify_batch(PlContext* ctx, const PlRectifier* rect, int B, const uint8_t* img_l, const uint8_t* img_r,
                          uint8_t* out_l, uint8_t* out_r);
-/* Device time of the last remap on this context (plstvo_rectify_batch or a raw-images call), ms. */
+/* Device time of the last remap or colour preparation on this context (plstvo_rectify_batch or a raw-images call), ms. */
 int plstvo_rectify_kernel_times(PlContext* ctx, float* ms1);
 
 /* ---- raw stereo images in, pose out: Dataset::nextFrame's rectifyImagesLR, then the handler (plstvo_track_stereo_images_lsd_*)
  * The signatures of the _lsd_ calls plus rect.  Results and n_stereo equal, byte for byte, plstvo_rectify_batch on every pair
  * followed by plstvo_track_stereo_images_lsd_batch / _sequence on the rectified images.  rect == NULL: the _lsd_ call (the
- * reference's copy when dist is false).  The raw images go up once into a staging slot and the remap writes the device copy
- * that LSD, ORB and LBD read, so no rectified image crosses PCIe; stage slot [0] of plstvo_track_stereo_images_stage_times
- * then covers the upload and the remap.  Device memory besides the _lsd_ call's: the staging copy, 1 byte per pixel of the
- * call, and the rectifier's maps.  PLSTVO_E_SIZE: the rectifier's size differs from cam's (and so from the images');
+ * reference's copy when dist is false).  PlStereoImages' img_l / img_r are [B][height][width][channels] of the rectifier
+ * (colour images for a colour rectifier).  The raw images go up once into a staging slot and the remap (for colour images,
+ * the remap and the conversion to grey, or the conversion alone) writes the grey device copy that LSD, ORB and LBD read, so
+ * no rectified image crosses PCIe and no stage reads the caller's images; stage slot [0] of
+ * plstvo_track_stereo_images_stage_times then covers the upload and the remap.  Device memory besides the _lsd_ call's: the
+ * staging copy, channels bytes per pixel of the call, and the rectifier's maps.  PLSTVO_E_SIZE: the rectifier's size differs
+ * from cam's (and so from the images');
  * PLSTVO_E_INVALID: a rectifier of another context, and every code of the _lsd_ calls.  The context stays usable after any
  * error.  The call also updates what plstvo_rectify_kernel_times reports when the images are read. */
 int plstvo_track_stereo_raw_images_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mcfg,
@@ -537,7 +551,8 @@ int plstvo_track_stereo_raw_images_sequence(PlContext* ctx, const PlCamera* cam,
  * and serve as the next pair's previous frame unchanged.
  * The configs are copied at creation and fixed for the session's life (the kept records depend on cam and scfg, the
  * descriptors on ocfg and lcfg).  lcfg may be NULL where cfg->has_lines is 0.  rect (NULL: the images are already rectified)
- * must belong to ctx and outlive the session.  Returns NULL on failure (a null argument, n_streams < 1, the ORB / LSD config
+ * must belong to ctx and outlive the session; the frames of _initialize / _insert are [height][width][channels] of it, so a
+ * colour rectifier takes colour frames.  Returns NULL on failure (a null argument, n_streams < 1, the ORB / LSD config
  * checks of the _lsd_ calls, a bad grid, a rectifier of another context or of another size; plstvo_last_error says which).
  * Destroy a session before its context; plstvo_stereo_session_device_bytes is its device memory (pools and call tables). */
 typedef struct PlStereoSession PlStereoSession;

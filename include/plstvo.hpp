@@ -289,28 +289,44 @@ inline RectifyMaps initUndistortRectifyMap(const PlRectifyModel& model, int widt
     if (rc < 0) throw Error(rc, "initUndistortRectifyMap: unsupported model (coefficient count, singular P * R) or size");
     return m;
 }
-// A rig's maps resident in HBM (plstvo_rectifier_create); one map pair for both sides where only left is given.  Destroy it
+// A rig's maps resident in HBM (plstvo_rectifier_create); one map pair for both sides where only left is given.  The colour
+// forms (plstvo_rectifier_create_color) take images of `channels` interleaved channels (3: BGR, 4: BGRA, as cv::imread
+// gives them) and give the detectors cvtColor(remap(img), COLOR_BGR2GRAY), or without maps cvtColor alone.  Destroy it
 // before its Context.
 class Rectifier {
 public:
-    Rectifier(Context& c, const RectifyMaps& left, const RectifyMaps& right) : r_(create(c, left, right)) {}
-    Rectifier(Context& c, const RectifyMaps& both) : r_(create(c, both, both)) {}
+    Rectifier(Context& c, const RectifyMaps& left, const RectifyMaps& right) : r_(create(c, 1, left, right)) {}
+    Rectifier(Context& c, const RectifyMaps& both) : r_(create(c, 1, both, both)) {}
+    Rectifier(Context& c, int channels, const RectifyMaps& left, const RectifyMaps& right)
+        : r_(create(c, channels, left, right)), channels_(channels) {}
+    Rectifier(Context& c, int channels, const RectifyMaps& both) : r_(create(c, channels, both, both)), channels_(channels) {}
+    Rectifier(Context& c, int width, int height, int channels)
+        : r_(check(c, plstvo_rectifier_create_color(c.get(), width, height, channels, nullptr, nullptr, nullptr, nullptr))),
+          channels_(channels) {}
     ~Rectifier() { plstvo_rectifier_destroy(r_); }
     Rectifier(const Rectifier&) = delete;
     Rectifier& operator=(const Rectifier&) = delete;
     const PlRectifier* get() const { return r_; }
+    int channels() const { return channels_; }   // bytes per pixel of the images it takes
 private:
-    static PlRectifier* create(Context& c, const RectifyMaps& l, const RectifyMaps& r) {
-        if (l.width != r.width || l.height != r.height) throw Error(PLSTVO_E_SIZE, "Rectifier: the two sides' maps differ in size");
-        PlRectifier* p = plstvo_rectifier_create(c.get(), l.width, l.height, l.map1.data(), l.map2.data(), r.map1.data(),
-                                                 r.map2.data());
+    static PlRectifier* check(Context& c, PlRectifier* p) {
         if (!p) throw Error(PLSTVO_E_INVALID, plstvo_last_error(c.get()));
         return p;
     }
+    static PlRectifier* create(Context& c, int channels, const RectifyMaps& l, const RectifyMaps& r) {
+        if (l.width != r.width || l.height != r.height) throw Error(PLSTVO_E_SIZE, "Rectifier: the two sides' maps differ in size");
+        if (channels == 1)
+            return check(c, plstvo_rectifier_create(c.get(), l.width, l.height, l.map1.data(), l.map2.data(), r.map1.data(),
+                                                    r.map2.data()));
+        return check(c, plstvo_rectifier_create_color(c.get(), l.width, l.height, channels, l.map1.data(), l.map2.data(),
+                                                      r.map1.data(), r.map2.data()));
+    }
     PlRectifier* r_ = nullptr;
+    int channels_ = 1;
 };
 // PinholeStereoCamera::rectifyImagesLR on B pairs (plstvo_rectify_batch): out = cv::remap(img, maps, INTER_LINEAR), byte for
-// byte; [B][height][width] grey in and out.
+// byte; [B][height][width] grey in and out.  With a colour rectifier the input is [B][height][width][channels] and the output
+// the grey image cvtColor(..., COLOR_BGR2GRAY) makes of it.
 inline void rectifyImagesLR(Context& c, const Rectifier& r, const uint8_t* img_l, uint8_t* rec_l, const uint8_t* img_r,
                             uint8_t* rec_r, int B = 1) {
     c.check(plstvo_rectify_batch(c.get(), r.get(), B, img_l, img_r, rec_l, rec_r));
@@ -347,11 +363,12 @@ struct StereoRectification {
         s.one_map = true;
         return s;
     }
-    // the maps of both sides, uploaded once
-    Rectifier rectifier(Context& c) const {
+    // the maps of both sides, uploaded once; channels 3 or 4: a colour rectifier on these maps (images as cv::imread reads
+    // KITTI's image_2 / image_3, or EuRoC's with IMREAD_UNCHANGED)
+    Rectifier rectifier(Context& c, int channels = 1) const {
         const RectifyMaps l = initUndistortRectifyMap(left, cam.width, cam.height);
-        if (one_map) return Rectifier(c, l);
-        return Rectifier(c, l, initUndistortRectifyMap(right, cam.width, cam.height));
+        if (one_map) return Rectifier(c, channels, l);
+        return Rectifier(c, channels, l, initUndistortRectifyMap(right, cam.width, cam.height));
     }
 
 private:
@@ -827,14 +844,14 @@ private:
 };
 
 namespace detail {
-// n frames of one size, copied into the contiguous arrays a PlStereoImages of images alone points at
+// n frames of one size (channels bytes per pixel), copied into the contiguous arrays a PlStereoImages of images alone points at
 struct StereoImagesBatch {
     std::vector<uint8_t> img_l, img_r;
     std::vector<int32_t> th;
     PlStereoImages view{};
-    void pack(int width, int height, const std::vector<const uint8_t*>& l, const std::vector<const uint8_t*>& r,
+    void pack(int width, int height, int channels, const std::vector<const uint8_t*>& l, const std::vector<const uint8_t*>& r,
               const std::vector<int32_t>& fast_th, const char* who) {
-        const size_t px = (size_t)width * (size_t)height, n = l.size();
+        const size_t px = (size_t)width * (size_t)height * (size_t)channels, n = l.size();
         if (r.size() != n || fast_th.size() != n) throw Error(PLSTVO_E_INVALID, std::string(who) + ": ids and images differ in number");
         img_l.resize(n * px);
         img_r.resize(n * px);
@@ -873,7 +890,8 @@ public:
         : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, 1) {}
     // Raw images, as Dataset::nextFrame feeds the reference's handler (src/dataset.cpp:147-157): initialize / insertStereoPair
     // take the camera's images before rectifyImagesLR, and each call rectifies them on the device under rect; cam is the
-    // rectified camera (StereoRectification::cam).  rect must outlive the handler.
+    // rectified camera (StereoRectification::cam).  With a colour rectifier the images are [height][width][channels] (BGR or
+    // BGRA, as cv::imread gives them) and are converted to grey on the device after the remap.  rect must outlive the handler.
     StereoImageHandler(Context& ctx, const Rectifier& rect, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
                        const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
                        const HandlerConfig& hcfg = HandlerConfig{})
@@ -967,7 +985,7 @@ public:
                          const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc, int n_streams,
                          const HandlerConfig& hcfg = HandlerConfig{}, const Rectifier* rect = nullptr)
         : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, n_streams, rect),
-          streams_((size_t)n_streams) {
+          streams_((size_t)n_streams), channels_(rect ? rect->channels() : 1) {
         for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
     }
 
@@ -975,7 +993,7 @@ public:
     void initialize(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
                     const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
         const std::vector<int32_t> th(ids.size(), hcfg_.orb_fast_th);   // :38
-        pack_.pack(cam_.width, cam_.height, img_l, img_r, th, "StereoStreamsHandler::initialize");
+        pack_.pack(cam_.width, cam_.height, channels_, img_l, img_r, th, "StereoStreamsHandler::initialize");
         session_.initialize((int)ids.size(), ids.data(), pack_.view);
         for (size_t k = 0; k < ids.size(); ++k) {
             Stream& s = streams_[(size_t)ids[k]];
@@ -999,7 +1017,7 @@ public:
             th.push_back(s.orb_fast_th);
             priors.push_back(priorOf(s.prev_frame));
         }
-        pack_.pack(cam_.width, cam_.height, img_l, img_r, th, "StereoStreamsHandler::insertStereoPairs");
+        pack_.pack(cam_.width, cam_.height, channels_, img_l, img_r, th, "StereoStreamsHandler::insertStereoPairs");
         std::vector<PlPoseResult> res(ids.size());
         std::vector<int32_t> ns(4 * ids.size());
         session_.insert((int)ids.size(), ids.data(), pack_.view, priors.data(), res.data(), ns.data());
@@ -1043,6 +1061,7 @@ private:
     HandlerConfig hcfg_;
     StereoSession session_;
     std::vector<Stream> streams_;
+    int channels_ = 1;   // bytes per pixel of the images: the rectifier's channels
     detail::StereoImagesBatch pack_;
 };
 

@@ -909,6 +909,10 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
         for (int i = 0; i < NF; ++i)   // 0 = the configured threshold, as detectPointFeatures / plstvo::detectAndComputeORB
             th[(size_t)b * NF + i] = f->fast_th && f->fast_th[i] ? f->fast_th[i] : oc->fast_threshold;
     }
+    // the host images a stage may upload itself: none with a rectifier, whose images (colour ones too) only the rectifier
+    // reads; every stage then reads its grey device copy
+    const std::vector<ImgPart> no_parts;
+    const std::vector<ImgPart>& stage_parts = rect ? no_parts : iparts;
     bool run_lbd = false;
     auto count_lines = [&]() {
         for (int b = 0; b < nblk; ++b) lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
@@ -920,7 +924,8 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const uint8_t* d_images = nullptr;   // the device copy of the images the line stages read (null: LBD uploads its own)
     cudaEvent_t images_ready = nullptr;
     auto enqueue_lbd = [&]() -> int {
-        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_images, images_ready, iparts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_images, images_ready, stage_parts, ctx->s_alt, &d_seg, &d_ldesc))
+            return rc;
         CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
         return 0;
     };
@@ -954,7 +959,8 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     // LSD on the second stream.
     const bool lsd_first = run_lsd && pts && n_img < ctx->sm_count;
     CK(ctx, cudaEventRecord(ctx->img_ev[0], ctx->s_main));
-    // raw images: they go up into the rectifier's staging slot, and every stage reads the remap's device copy
+    // raw images: they go up into the rectifier's staging slot, and every stage reads the grey device copy the rectifier
+    // writes (the remap's, or for colour images the conversion's)
     const uint8_t* rectified = nullptr;
     cudaEvent_t rectified_ready = nullptr;
     if (rect && (pts || lns)) {
@@ -964,7 +970,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     }
     const uint8_t* orb_images = rectified;   // the device images ORB reads (null: ORB uploads them)
     if (lsd_first) {
-        if (const int rc = lsd_enqueue(ctx, lsd, rectified, nullptr, iparts, ctx->s_main)) return rc;
+        if (const int rc = lsd_enqueue(ctx, lsd, rectified, nullptr, stage_parts, ctx->s_main)) return rc;
         if (const int rc = lsd_lines(ctx->s_main)) return rc;
         orb_images = lsd.images;
     }
@@ -974,13 +980,14 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     auto lines_beside = [&](const uint8_t* d_img, cudaEvent_t ready) -> int {
         d_images = d_img;
         images_ready = ready;
-        return lsd_beside ? lsd_enqueue(ctx, lsd, d_img, ready, iparts, ctx->s_alt) : enqueue_lbd();
+        return lsd_beside ? lsd_enqueue(ctx, lsd, d_img, ready, stage_parts, ctx->s_alt) : enqueue_lbd();
     };
     OrbDetected orb;
     if (pts) {
         std::function<int(const uint8_t*, cudaEvent_t)> beside;
         if (lsd_beside || run_lbd) beside = lines_beside;
-        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, orb_images, iparts, th.data(), INT_MAX, beside, orb)) return rc;
+        if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, orb_images, stage_parts, th.data(), INT_MAX, beside, orb))
+            return rc;
     } else {
         orb.off.assign((size_t)n_img + 1, 0);
         if (lsd_beside || run_lbd)

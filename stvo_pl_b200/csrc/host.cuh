@@ -189,9 +189,9 @@ struct PlContext {
     plstvo::DevBuf lsd_trig;       // cos / sin table of the gradient angles (lsd.cu), built once
     bool lsd_ran = false;
     plstvo::Events<6> lsd_ev;
-    plstvo::DevBuf arena_rect;     // plstvo_rectify_batch / _raw_images_*: raw images (staging), rectified images
+    plstvo::DevBuf arena_rect;     // plstvo_rectify_batch / _raw_images_*: raw images (staging), rectified grey images
     bool rect_ran = false;
-    plstvo::Events<2> rect_ev;     // the remap kernel's start and end
+    plstvo::Events<2> rect_ev;     // the remap (or colour preparation) kernel's start and end
     // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
     plstvo::Events<4> img_ev;
     plstvo::Events<1> img_join;
@@ -208,10 +208,13 @@ struct PlContext {
 };
 
 // A rig's two CV_16SC2 + CV_16UC1 map pairs, resident in HBM (plstvo_rectifier_create).  Where both sides were given the same
-// maps they are held once and m1[1], m2[1] alias side 0.
+// maps they are held once and m1[1], m2[1] alias side 0.  A colour rectifier (plstvo_rectifier_create_color) takes images of
+// 3 or 4 interleaved channels and may hold no maps (maps false: the conversion to grey alone).
 struct PlRectifier {
     PlContext* ctx = nullptr;
     int width = 0, height = 0;
+    int channels = 1;
+    bool maps = true;
     plstvo::DevBuf map1[2], map2[2];
     const short2* m1[2] = {nullptr, nullptr};
     const uint16_t* m2[2] = {nullptr, nullptr};
@@ -471,8 +474,9 @@ int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg
 struct ImgPart {   // consecutive host images of one size
     const uint8_t* p; int n;
 };
-// Enqueues on stream s the upload of n_img raw images of rect's size (parts, in order) into arena_rect's staging slot and
-// their remap into its rectified slot (*d_out), in blocks of per_block images that alternate left, right maps.
+// Enqueues on stream s the upload of n_img raw images of rect's size and channels (parts, in order) into arena_rect's staging
+// slot and the grey device copy of them into its rectified slot (*d_out): their remap, in blocks of per_block images that
+// alternate left, right maps, and for a colour rectifier the conversion to grey after it.
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
                     cudaStream_t s, const uint8_t** d_out);
 

@@ -61,6 +61,112 @@ __global__ void __launch_bounds__(256) rectify_remap_kernel(const uint8_t* __res
     }
 }
 
+// cv::cvtColor(COLOR_BGR2GRAY) on 8-bit data, as cv2 4.13 computes it for every BGR triple (with and without IPP): 15-bit
+// coefficients that sum to 2^15, so B = G = R = v gives v back.
+__device__ __forceinline__ uint32_t bgr_to_grey(uint32_t b, uint32_t g, uint32_t r) {
+    return (3735u * b + 19235u * g + 9798u * r + (1u << 14)) >> 15;
+}
+
+// Byte k of a run of little-endian words (k a compile-time constant once the callers' loops unroll).
+__device__ __forceinline__ uint32_t byte_of(const uint32_t* w, int k) { return (w[k >> 2] >> (8 * (k & 3))) & 255u; }
+
+// cvtColor alone on n pixels of C interleaved channels (B, G, R[, A]), the whole batch as one run: the conversion does not
+// depend on where an image starts.  One thread converts 16 pixels: C 16-byte loads and one 16-byte store, all aligned
+// because the staging and the output slots start 256-byte aligned; the last partial group goes pixel by pixel.
+template <int C>
+__global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t n) {
+    const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 16;
+    if (p0 >= n) return;
+    if (p0 + 16 <= n) {
+        uint32_t w[4 * C];
+#pragma unroll
+        for (int k = 0; k < C; ++k) {
+            const uint4 v = __ldg(reinterpret_cast<const uint4*>(src + p0 * C) + k);
+            w[4 * k] = v.x; w[4 * k + 1] = v.y; w[4 * k + 2] = v.z; w[4 * k + 3] = v.w;
+        }
+        uint32_t o[4] = {0, 0, 0, 0};
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+            o[i >> 2] |= bgr_to_grey(byte_of(w, C * i), byte_of(w, C * i + 1), byte_of(w, C * i + 2)) << (8 * (i & 3));
+        *reinterpret_cast<uint4*>(dst + p0) = make_uint4(o[0], o[1], o[2], o[3]);
+    } else {
+        for (size_t p = p0; p < n; ++p) {
+            const uint8_t* s = src + p * C;
+            dst[p] = (uint8_t)bgr_to_grey(__ldg(s), __ldg(s + 1), __ldg(s + 2));
+        }
+    }
+}
+
+// remap_pixel on each of the first three channels of a C-channel image, then the conversion: cv::remap of a multi-channel
+// image interpolates every channel with the same weights as the one-channel remap, and the reference converts the remapped
+// image.  Alpha is not read: a 4-channel tap is one aligned 4-byte load, of which the top byte is dropped.
+template <int C>
+__device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
+    f &= 1023u;
+    const int ax = (int)(f & 31u), ay = (int)(f >> 5);
+    const int x = m.x, y = m.y;
+    const bool x0 = (unsigned)x < (unsigned)W, x1 = (unsigned)(x + 1) < (unsigned)W;
+    const bool y0 = (unsigned)y < (unsigned)H, y1 = (unsigned)(y + 1) < (unsigned)H;
+    const int w00 = (32 - ax) * (32 - ay), w01 = ax * (32 - ay), w10 = (32 - ax) * ay, w11 = ax * ay;
+    const ptrdiff_t row = (ptrdiff_t)W * C;
+    const uint8_t* r0 = S + ((ptrdiff_t)y * W + x) * C;
+    uint32_t ch[3];
+    if constexpr (C == 4) {
+        const uint32_t t00 = (x0 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0)) : 0u;
+        const uint32_t t01 = (x1 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + 4)) : 0u;
+        const uint32_t t10 = (x0 && y1) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + row)) : 0u;
+        const uint32_t t11 = (x1 && y1) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + row + 4)) : 0u;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const int sh = 8 * c;
+            const int sum = (int)((t00 >> sh) & 255u) * w00 + (int)((t01 >> sh) & 255u) * w01 +
+                            (int)((t10 >> sh) & 255u) * w10 + (int)((t11 >> sh) & 255u) * w11;
+            ch[c] = (uint32_t)((sum + 512) >> 10);
+        }
+    } else {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            const int v00 = (x0 && y0) ? __ldg(r0 + c) : 0, v01 = (x1 && y0) ? __ldg(r0 + C + c) : 0;
+            const int v10 = (x0 && y1) ? __ldg(r0 + row + c) : 0, v11 = (x1 && y1) ? __ldg(r0 + row + C + c) : 0;
+            ch[c] = (uint32_t)((v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + 512) >> 10);
+        }
+    }
+    return bgr_to_grey(ch[0], ch[1], ch[2]);
+}
+
+// rectify_remap_kernel's layout on C-channel images: one thread writes 4 consecutive grey pixels of one image from one
+// 16-byte map1 load and one 8-byte map2 load; image z of the staging slot starts at z * W * H * C.
+template <int C>
+__global__ void __launch_bounds__(256) color_remap_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
+                                                          const short2* __restrict__ m1l, const uint16_t* __restrict__ m2l,
+                                                          const short2* __restrict__ m1r, const uint16_t* __restrict__ m2r,
+                                                          int W, int H, int per_block, int z0) {
+    const int z = z0 + (int)blockIdx.y;
+    const size_t N = (size_t)W * H;
+    const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+    if (p0 >= N) return;
+    const bool right = (z / per_block) & 1;
+    const short2* m1 = right ? m1r : m1l;
+    const uint16_t* m2 = right ? m2r : m2l;
+    const uint8_t* S = src + (size_t)z * N * C;
+    uint8_t* D = dst + (size_t)z * N + p0;
+    if (p0 + 4 <= N) {
+        const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
+        const uint2 b = __ldg(reinterpret_cast<const uint2*>(m2 + p0));
+        short2 m[4];
+        memcpy(m, &a, sizeof a);
+        const uint32_t v = remap_grey<C>(S, W, H, m[0], b.x & 0xffffu) | remap_grey<C>(S, W, H, m[1], b.x >> 16) << 8 |
+                           remap_grey<C>(S, W, H, m[2], b.y & 0xffffu) << 16 | remap_grey<C>(S, W, H, m[3], b.y >> 16) << 24;
+        if (((uintptr_t)D & 3) == 0) {
+            *reinterpret_cast<uint32_t*>(D) = v;
+        } else {
+            D[0] = (uint8_t)v; D[1] = (uint8_t)(v >> 8); D[2] = (uint8_t)(v >> 16); D[3] = (uint8_t)(v >> 24);
+        }
+    } else {
+        for (size_t p = p0; p < N; ++p) D[p - p0] = (uint8_t)remap_grey<C>(S, W, H, __ldg(m1 + p), __ldg(m2 + p));
+    }
+}
+
 // cvRound (saturate_cast<int>(double)) on x86-64: round half to even; cvtsd2si gives INT_MIN for a result outside int, and for NaN
 int cv_round(double v) {
     const double r = nearbyint(v);
@@ -92,25 +198,52 @@ cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const u
     return cudaGetLastError();
 }
 
+// The grey device copy of n_img colour images (C channels): color_convert_kernel without maps, color_remap_kernel with.
+template <int C>
+cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool maps, const uint8_t* src, uint8_t* dst,
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches) {
+    if (!maps) {
+        const size_t groups = ((size_t)n_img * W * H + 15) / 16;
+        color_convert_kernel<C><<<(unsigned)((groups + 255) / 256), 256, 0, s>>>(src, dst, (size_t)n_img * W * H);
+        ++*launches;
+        return cudaGetLastError();
+    }
+    const size_t quads = ((size_t)W * H + 3) / 4;
+    const unsigned gx = (unsigned)((quads + 255) / 256);
+    for (int z0 = 0; z0 < n_img; z0 += 65535) {
+        const int nz = std::min(n_img - z0, 65535);
+        color_remap_kernel<C><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block, z0);
+        ++*launches;
+    }
+    return cudaGetLastError();
+}
+
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
                     cudaStream_t s, const uint8_t** d_out) {
-    const int W = rect->width, H = rect->height;
+    const int W = rect->width, H = rect->height, Ch = rect->channels;
     const size_t bytes = (size_t)n_img * W * H;
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, ctx->rect_ev.create());
     Arena a;
-    const size_t o_raw = a.take(bytes), o_out = a.take(bytes);
+    const size_t o_raw = a.take(bytes * Ch), o_out = a.take(bytes);
     CK(ctx, a.alloc(ctx->arena_rect));
     size_t o = o_raw;
     for (const ImgPart& ip : parts) {
-        const size_t b = (size_t)ip.n * W * H;
+        const size_t b = (size_t)ip.n * W * H * Ch;
         CK(ctx, a.up(o, ip.p, b, s));
         o += b;
     }
     int launches = 0;
     ctx->rect_ran = false;
     CK(ctx, cudaEventRecord(ctx->rect_ev[0], s));
-    CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches));
+    if (Ch == 1)
+        CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches));
+    else if (Ch == 3)
+        CK(ctx, launch_color_prepare<3>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
+                                        &launches));
+    else
+        CK(ctx, launch_color_prepare<4>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
+                                        &launches));
     CK(ctx, cudaEventRecord(ctx->rect_ev[1], s));
     ctx->rect_ran = true;
     ctx->launches += launches;
@@ -205,18 +338,12 @@ int plstvo_init_undistort_rectify_map(const PlRectifyModel* m, int width, int he
     return 0;
 }
 
-PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, const int16_t* map1_l, const uint16_t* map2_l,
-                                     const int16_t* map1_r, const uint16_t* map2_r) {
-    if (!ctx) return nullptr;
-    LOCK(ctx);
-    if (width < 1 || width > 32767 || height < 1 || height > 32767) {
-        fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
-        return nullptr;
-    }
-    if (!map1_l || !map2_l || !map1_r || !map2_r) {
-        fail(ctx, PLSTVO_E_INVALID, "null map");
-        return nullptr;
-    }
+}  // extern "C"
+
+namespace {
+// A checked rectifier of `channels` with the four maps uploaded, or none (all four null), under the context's lock.
+PlRectifier* rectifier_new(PlContext* ctx, int width, int height, int channels, const int16_t* map1_l, const uint16_t* map2_l,
+                           const int16_t* map1_r, const uint16_t* map2_r) {
     if (cudaSetDevice(ctx->device) != cudaSuccess) {
         fail(ctx, PLSTVO_E_CUDA, "cudaSetDevice failed");
         return nullptr;
@@ -225,6 +352,9 @@ PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, cons
     r->ctx = ctx;
     r->width = width;
     r->height = height;
+    r->channels = channels;
+    r->maps = map1_l != nullptr;
+    if (!r->maps) return r;
     const size_t N = (size_t)width * height;
     const bool shared = map1_l == map1_r && map2_l == map2_r;
     const int16_t* m1[2] = {map1_l, map1_r};
@@ -247,6 +377,44 @@ PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, cons
         r->m2[1] = r->m2[0];
     }
     return r;
+}
+}  // namespace
+
+extern "C" {
+
+PlRectifier* plstvo_rectifier_create(PlContext* ctx, int width, int height, const int16_t* map1_l, const uint16_t* map2_l,
+                                     const int16_t* map1_r, const uint16_t* map2_r) {
+    if (!ctx) return nullptr;
+    LOCK(ctx);
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) {
+        fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+        return nullptr;
+    }
+    if (!map1_l || !map2_l || !map1_r || !map2_r) {
+        fail(ctx, PLSTVO_E_INVALID, "null map");
+        return nullptr;
+    }
+    return rectifier_new(ctx, width, height, 1, map1_l, map2_l, map1_r, map2_r);
+}
+
+PlRectifier* plstvo_rectifier_create_color(PlContext* ctx, int width, int height, int channels, const int16_t* map1_l,
+                                           const uint16_t* map2_l, const int16_t* map1_r, const uint16_t* map2_r) {
+    if (!ctx) return nullptr;
+    LOCK(ctx);
+    if (channels != 3 && channels != 4) {
+        fail(ctx, PLSTVO_E_INVALID, "channels must be 3 (BGR) or 4 (BGRA)");
+        return nullptr;
+    }
+    if (width < 1 || width > 32767 || height < 1 || height > 32767) {
+        fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+        return nullptr;
+    }
+    const int given = (map1_l != nullptr) + (map2_l != nullptr) + (map1_r != nullptr) + (map2_r != nullptr);
+    if (given != 0 && given != 4) {
+        fail(ctx, PLSTVO_E_INVALID, "maps must be all four or none");
+        return nullptr;
+    }
+    return rectifier_new(ctx, width, height, channels, map1_l, map2_l, map1_r, map2_r);
 }
 
 void plstvo_rectifier_destroy(PlRectifier* rect) {

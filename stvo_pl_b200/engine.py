@@ -120,6 +120,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_track_stereo_images_stage_times": (C.c_int, [vp, fp]),
         "plstvo_init_undistort_rectify_map": (C.c_int, [C.POINTER(T.PlRectifyModel), C.c_int, C.c_int, i16p, u16p]),
         "plstvo_rectifier_create": (vp, [vp, C.c_int, C.c_int, i16p, u16p, i16p, u16p]),
+        "plstvo_rectifier_create_color": (vp, [vp, C.c_int, C.c_int, C.c_int, i16p, u16p, i16p, u16p]),
         "plstvo_rectifier_destroy": (None, [vp]),
         "plstvo_rectify_batch": (C.c_int, [vp, vp, C.c_int, u8p, u8p, u8p, u8p]),
         "plstvo_rectify_kernel_times": (C.c_int, [vp, fp]),
@@ -165,7 +166,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_track_stereo_images_stage_times", "plstvo_init_undistort_rectify_map", "plstvo_rectifier_create",
     "plstvo_rectifier_destroy", "plstvo_rectify_batch", "plstvo_rectify_kernel_times", "plstvo_track_stereo_raw_images_batch",
     "plstvo_track_stereo_raw_images_sequence", "plstvo_stereo_session_create", "plstvo_stereo_session_destroy",
-    "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert"]
+    "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert",
+    "plstvo_rectifier_create_color"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -187,10 +189,23 @@ def init_undistort_rectify_map(model: int, K, D, R, P, width: int, height: int, 
 
 
 class Rectifier:
-    """A PlRectifier: a rig's maps resident in HBM (Engine.rectifier_create); close() or the owning Engine frees it."""
+    """A PlRectifier: a rig's maps resident in HBM (Engine.rectifier_create), or for colour images (channels 3 or 4) the
+    conversion to grey with or without maps (Engine.rectifier_create_color); close() or the owning Engine frees it."""
 
-    def __init__(self, lib: C.CDLL, handle, width: int, height: int):
-        self.lib, self.handle, self.width, self.height = lib, handle, width, height
+    def __init__(self, lib: C.CDLL, handle, width: int, height: int, channels: int = 1):
+        self.lib, self.handle, self.width, self.height, self.channels = lib, handle, width, height, channels
+
+    def image_shape(self, B: int):
+        """The shape of B raw images this rectifier takes: uint8[B, H, W] grey, uint8[B, H, W, C] colour."""
+        return (B, self.height, self.width) + ((self.channels,) if self.channels > 1 else ())
+
+    def check_frames(self, *frame_sets):
+        """ValueError unless each dict's img_l / img_r hold images of this rectifier's size and channels."""
+        for fs in frame_sets:
+            il, ir = (np.asarray(fs[k]) for k in ("img_l", "img_r"))
+            if il.shape != ir.shape or il.shape != self.image_shape(il.shape[0] if il.ndim else 0):
+                raise ValueError(f"images must be uint8{list(self.image_shape(il.shape[0] if il.ndim else 0))} "
+                                 "(B images of the rectifier's size and channels), both sides alike")
 
     def close(self):
         if self.handle:
@@ -202,12 +217,17 @@ class StereoSession:
     """A PlStereoSession: n_streams stereo streams, each stream's previous frame kept in HBM as its stereo features
     (Engine.stereo_session_create).  initialize / insert name any subset of the streams; close() or the owning Engine frees it."""
 
-    def __init__(self, eng: "Engine", handle, n_streams: int):
-        self.eng, self.handle, self.n_streams = eng, handle, n_streams
+    def __init__(self, eng: "Engine", handle, n_streams: int, rect: Optional[Rectifier] = None):
+        self.eng, self.handle, self.n_streams, self.rect = eng, handle, n_streams, rect
+
+    def check_frames(self, frames: dict):
+        """ValueError unless a colour session's frames are colour images of its rectifier's size and channels."""
+        if self.rect is not None and self.rect.channels > 1:
+            self.rect.check_frames(frames)
 
     def initialize(self, ids, frames: dict):
-        """initialize(img_l, img_r) for streams ids: frames holds len(ids) frames (img_l / img_r uint8[n, H, W], optionally
-        fast_th [n]).  Returns n_stereo [n, 2]."""
+        """initialize(img_l, img_r) for streams ids: frames holds len(ids) frames (img_l / img_r uint8[n, H, W], or
+        uint8[n, H, W, C] with a colour rectifier, optionally fast_th [n]).  Returns n_stereo [n, 2]."""
         return self.eng.stereo_session_initialize(self, ids, frames)
 
     def insert(self, ids, frames: dict, priors=None, results=None):
@@ -763,19 +783,43 @@ class Engine:
         self._rectifiers.append(r)
         return r
 
+    def rectifier_create_color(self, width: int, height: int, channels: int, map1_l=None, map2_l=None, map1_r=None,
+                               map2_r=None) -> Rectifier:
+        """A rectifier of colour images (channels 3: BGR, 4: BGRA): cvtColor(remap(img), COLOR_BGR2GRAY) with the maps, the
+        conversion alone without them.  The right pair defaults to the left one (held once); no maps at all is the map-less
+        form."""
+        i16p, u16p = C.POINTER(C.c_int16), C.POINTER(C.c_uint16)
+        m1l = None if map1_l is None else np.ascontiguousarray(map1_l, np.int16)
+        m2l = None if map2_l is None else np.ascontiguousarray(map2_l, np.uint16)
+        m1r = m1l if map1_r is None else np.ascontiguousarray(map1_r, np.int16)
+        m2r = m2l if map2_r is None else np.ascontiguousarray(map2_r, np.uint16)
+        for m, shape in ((m1l, (height, width, 2)), (m2l, (height, width)), (m1r, (height, width, 2)), (m2r, (height, width))):
+            if m is not None and m.shape != shape:
+                raise ValueError("map shapes differ from the size")
+        h = self.lib.plstvo_rectifier_create_color(self.ctx, width, height, channels, _p(m1l, i16p), _p(m2l, u16p),
+                                                   _p(m1r, i16p), _p(m2r, u16p))
+        if not h:
+            raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
+        r = Rectifier(self.lib, h, width, height, channels)
+        self._rectifiers.append(r)
+        return r
+
     def rectifier_destroy(self, rect: Rectifier):
         rect.close()
         self._rectifiers = [r for r in self._rectifiers if r is not rect]
 
     def rectify_batch(self, rect: Rectifier, img_l, img_r):
-        """rectifyImagesLR on B pairs: (rectified left uint8[B, H, W], rectified right)."""
+        """rectifyImagesLR on B pairs: (rectified left uint8[B, H, W], rectified right).  A colour rectifier takes
+        uint8[B, H, W, C] and returns the grey images the reference's detectors see."""
         il = np.ascontiguousarray(img_l, np.uint8)
         ir = np.ascontiguousarray(img_r, np.uint8)
-        if il.ndim == 2:
+        if il.ndim == len(rect.image_shape(0)) - 1:
             il, ir = il[None], ir[None]
-        if il.shape != ir.shape or il.shape[1:] != (rect.height, rect.width):
+        if il.shape != ir.shape or il.shape != rect.image_shape(il.shape[0]):
+            if rect.channels > 1:
+                raise ValueError("images must be uint8[B, H, W, C] of the rectifier's size and channels, both sides alike")
             raise ValueError("images must be uint8[B, H, W] of the rectifier's size, both sides alike")
-        ol, orr = np.empty_like(il), np.empty_like(ir)
+        ol, orr = np.empty(il.shape[:3], np.uint8), np.empty(ir.shape[:3], np.uint8)
         self._ck(self.lib.plstvo_rectify_batch(self.ctx, rect.handle, il.shape[0], _p(il, T.c_uint8_p), _p(ir, T.c_uint8_p),
                                                _p(ol, T.c_uint8_p), _p(orr, T.c_uint8_p)))
         return ol, orr
@@ -789,7 +833,9 @@ class Engine:
     def track_stereo_raw_images_batch(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], prev: dict, curr: dict,
                                       priors=None, results=None):
         """track_stereo_images_lsd_batch on raw (distorted) images: rect's remap runs on the device first; rect None: the
-        _lsd_ call.  Returns (results, n_stereo[B, 4])."""
+        _lsd_ call.  A colour rectifier takes img_l / img_r uint8[B, H, W, C].  Returns (results, n_stereo[B, 4])."""
+        if rect is not None and rect.channels > 1:
+            rect.check_frames(prev, curr)
         ps, keep_p = T.stereo_images_as_c(prev)
         cs, keep_c = T.stereo_images_as_c(curr)
         B = ps.B
@@ -805,7 +851,10 @@ class Engine:
 
     def track_stereo_raw_images_sequence(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], frames: dict,
                                          priors=None, results=None):
-        """track_stereo_images_lsd_sequence on raw images, rectified on the device.  Returns (results, n_stereo[NF, 2])."""
+        """track_stereo_images_lsd_sequence on raw images, rectified on the device (colour ones converted to grey there).
+        Returns (results, n_stereo[NF, 2])."""
+        if rect is not None and rect.channels > 1:
+            rect.check_frames(frames)
         fs, keep = T.stereo_images_as_c(frames)
         NF = fs.B
         if results is None:
@@ -821,13 +870,14 @@ class Engine:
     # ---- stereo sessions: many streams, each stream's previous frame kept on the device ----
     def stereo_session_create(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], n_streams: int) -> StereoSession:
         """A session of n_streams streams with these configs (copied; lcfg may be None where cfg.has_lines is 0) and rect
-        (None: the images are already rectified; it must outlive the session)."""
+        (None: the images are already rectified; it must outlive the session).  With a colour rectifier the session takes
+        colour frames, uint8[n, H, W, C]."""
         h = self.lib.plstvo_stereo_session_create(self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg),
                                                   C.byref(ocfg), None if lcfg is None else C.byref(lcfg),
                                                   None if rect is None else rect.handle, n_streams)
         if not h:
             raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
-        ss = StereoSession(self, h, n_streams)
+        ss = StereoSession(self, h, n_streams, rect)
         self._sessions.append(ss)
         return ss
 
@@ -836,6 +886,7 @@ class Engine:
         self._sessions = [x for x in self._sessions if x is not ss]
 
     def stereo_session_initialize(self, ss: StereoSession, ids, frames: dict):
+        ss.check_frames(frames)
         ids = np.ascontiguousarray(ids, np.int32)
         fs, keep = T.stereo_images_as_c(frames)
         n_stereo = np.zeros((len(ids), 2), np.int32)
@@ -845,6 +896,7 @@ class Engine:
         return n_stereo
 
     def stereo_session_insert(self, ss: StereoSession, ids, frames: dict, priors=None, results=None):
+        ss.check_frames(frames)
         ids = np.ascontiguousarray(ids, np.int32)
         fs, keep = T.stereo_images_as_c(frames)
         n = len(ids)

@@ -178,11 +178,12 @@ STEREO_IMAGE_DTYPES = dict(img_l=np.uint8, img_r=np.uint8, fast_th=np.int32, ll_
 
 
 def stereo_images_as_c(d: dict):
-    """dict with img_l / img_r uint8[B, H, W] and optionally fast_th [B] and the key-line arrays (keys of STEREO_IMAGE_DTYPES;
-    a missing or None entry is passed as NULL) -> (PlStereoImages, keep-alive dict)."""
+    """dict with img_l / img_r uint8[B, H, W] (uint8[B, H, W, C] for a colour rectifier) and optionally fast_th [B] and the
+    key-line arrays (keys of STEREO_IMAGE_DTYPES; a missing or None entry is passed as NULL) -> (PlStereoImages, keep-alive
+    dict)."""
     keep = {k: None if d.get(k) is None else np.ascontiguousarray(d[k], dt) for k, dt in STEREO_IMAGE_DTYPES.items()}
     s = PlStereoImages()
-    B, H, W = keep["img_l"].shape
+    B, H, W = keep["img_l"].shape[:3]
     s.B, s.width, s.height = B, W, H
     for k, a in keep.items():
         typ = dict(PlStereoImages._fields_)[k]
