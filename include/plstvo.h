@@ -585,6 +585,33 @@ int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* s, int n, 
 int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* s, int n, const int32_t* ids, const PlStereoImages* frames,
                                  const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo);
 
+/* ---- reading a session call's frames back: StereoFrame::stereo_pt / stereo_ls and StereoFrameHandler::matched_pt / _ls
+ * of the last _initialize / _insert ----
+ * Outputs of plstvo_stereo_session_read.  Every pointer may be NULL (that array is not copied).  The point and line fields
+ * are what plstvo_match_stereo_points / _lines write for the call's n new frames, in call order, frame k's rows after frame
+ * k - 1's; the row counts are the call's n_stereo (initialize: columns 0, 1; insert: columns 2, 3).  pt_src / ls_src are
+ * their src_idx: the index in ORB's / LSD's output order for the left image.  m12_* and inlier_* (insert only) are what
+ * plstvo_track_batch writes, one row per feature of each named stream's kept (previous) frame in call order (the insert's
+ * n_stereo columns 0, 1), an m12 value indexing the stream's new frame's rows (or -1). */
+typedef struct PlStereoFrameOut {
+    double* pt_pl; double* pt_disp; double* pt_P; double* pt_sigma2; int32_t* pt_level; uint8_t* pdesc; int32_t* pt_src;
+    double* ls_spl; double* ls_epl; double* ls_sdisp; double* ls_edisp; double* ls_sP; double* ls_eP; double* ls_le;
+    double* ls_angle; double* ls_sigma2; int32_t* ls_level; uint8_t* ldesc; int32_t* ls_src;
+    int32_t* m12_pt; uint8_t* inlier_pt; int32_t* m12_ls; uint8_t* inlier_ls;
+} PlStereoFrameOut;
+/* Retention switch, off at creation.  on != 0 takes effect from the next _initialize / _insert: each successful call then
+ * keeps, in a session-owned device arena (counted by plstvo_stereo_session_device_bytes, untouched by other calls on the
+ * context), its new frames' full records (96 bytes per stereo point, 176 per stereo line) and, for an insert, the tracker's
+ * m12 and inlier rows (5 bytes per kept row).  Filling it costs two more lift launches per call and device-to-device copies.
+ * on == 0 frees the arena at once; with retention off a call's launches, device memory and results are those of a session
+ * never switched on.  Returns 0, or PLSTVO_E_INVALID for a null or foreign session. */
+int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* s, int on);
+/* Copies what the last call retained into out's non-NULL arrays (after an initialize, m12_* and inlier_* are left untouched)
+ * and returns that call's n.  PLSTVO_E_INVALID: ctx, s or out null, a session of another context, retention off, no call
+ * succeeded since retention was turned on, or the last call on the session failed (any failed call discards what was
+ * retained, so a read never mixes two calls). */
+int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* s, const PlStereoFrameOut* out);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

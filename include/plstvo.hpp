@@ -45,6 +45,10 @@ struct StereoFrame {
     std::vector<double> pt_P, pt_pl, pt_sigma2;                          // [n][3], [n][2], [n]
     std::vector<double> ls_sP, ls_eP, ls_le, ls_spl, ls_epl, ls_sigma2;  // [m][3] x3, [m][2] x2, [m]
     std::vector<int32_t> ls_level;                                       // [m]
+    // the rest of stereo_pt / stereo_ls, filled by the images handlers' keepFeatures (the tracker does not read them):
+    // disparities, ORB octave, start / end disparities, line angle, and each feature's index in ORB's / LSD's left-image order
+    std::vector<double> pt_disp, ls_sdisp, ls_edisp, ls_angle;          // [n], [m] x3
+    std::vector<int32_t> pt_level, pt_src, ls_src;                       // [n] x2, [m]
     int frame_idx = 0;
     // results published by optimizePose (src/stereoFrameHandler.cpp:372-391), row-major
     std::array<double, 16> Tfw{1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1}, DT = Tfw;
@@ -834,6 +838,46 @@ public:
                 int32_t* n_stereo = nullptr) {
         c_.check(plstvo_stereo_session_insert(c_.get(), s_, n, ids, &frames, priors, results, n_stereo));
     }
+    // plstvo_stereo_session_retain: keep each following call's frames and matches for read() (off frees them)
+    void retain(bool on) { c_.check(plstvo_stereo_session_retain(c_.get(), s_, on ? 1 : 0)); }
+    // plstvo_stereo_session_read of the last call, into out's vectors sized from that call's n and n_stereo ([n][2] after an
+    // initialize, [n][4] after an insert, as the call wrote it); out.m12_* / inlier_* are emptied after an initialize
+    struct Frames {
+        std::vector<double> pt_pl, pt_disp, pt_P, pt_sigma2;                                  // [N][2], [N], [N][3], [N]
+        std::vector<int32_t> pt_level, pt_src;                                                // [N] x2
+        std::vector<uint8_t> pdesc;                                                           // [N][32]
+        std::vector<double> ls_spl, ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2;
+        std::vector<int32_t> ls_level, ls_src;                                                // [M] x2
+        std::vector<uint8_t> ldesc;                                                           // [M][32]
+        std::vector<int32_t> m12_pt, m12_ls;                                                  // [kept points], [kept lines]
+        std::vector<uint8_t> inlier_pt, inlier_ls;
+    };
+    void read(int n, const int32_t* n_stereo, bool insert, Frames& out) const {
+        const int cols = insert ? 4 : 2;
+        size_t np = 0, nl = 0, kp = 0, kl = 0;
+        for (int k = 0; k < n; ++k) {
+            np += (size_t)n_stereo[cols * k + cols - 2];
+            nl += (size_t)n_stereo[cols * k + cols - 1];
+            if (insert) {
+                kp += (size_t)n_stereo[cols * k];
+                kl += (size_t)n_stereo[cols * k + 1];
+            }
+        }
+        out.pt_pl.resize(2 * np); out.pt_disp.resize(np); out.pt_P.resize(3 * np); out.pt_sigma2.resize(np);
+        out.pt_level.resize(np); out.pt_src.resize(np); out.pdesc.resize(32 * np);
+        out.ls_spl.resize(2 * nl); out.ls_epl.resize(2 * nl); out.ls_sdisp.resize(nl); out.ls_edisp.resize(nl);
+        out.ls_sP.resize(3 * nl); out.ls_eP.resize(3 * nl); out.ls_le.resize(3 * nl); out.ls_angle.resize(nl);
+        out.ls_sigma2.resize(nl); out.ls_level.resize(nl); out.ls_src.resize(nl); out.ldesc.resize(32 * nl);
+        out.m12_pt.assign(kp, -1); out.m12_ls.assign(kl, -1); out.inlier_pt.assign(kp, 0); out.inlier_ls.assign(kl, 0);
+        const PlStereoFrameOut o{out.pt_pl.data(), out.pt_disp.data(), out.pt_P.data(), out.pt_sigma2.data(),
+                                 out.pt_level.data(), out.pdesc.data(), out.pt_src.data(), out.ls_spl.data(), out.ls_epl.data(),
+                                 out.ls_sdisp.data(), out.ls_edisp.data(), out.ls_sP.data(), out.ls_eP.data(), out.ls_le.data(),
+                                 out.ls_angle.data(), out.ls_sigma2.data(), out.ls_level.data(), out.ldesc.data(),
+                                 out.ls_src.data(), out.m12_pt.data(), out.inlier_pt.data(), out.m12_ls.data(),
+                                 out.inlier_ls.data()};
+        if (c_.check(plstvo_stereo_session_read(c_.get(), s_, &o)) != n)
+            throw Error(PLSTVO_E_INVALID, "StereoSession::read: n differs from the last call's");
+    }
     int streams() const { return n_streams_; }
     int64_t deviceBytes() const { return plstvo_stereo_session_device_bytes(s_); }
     PlStereoSession* get() const { return s_; }
@@ -842,6 +886,22 @@ private:
     PlStereoSession* s_ = nullptr;
     int n_streams_ = 0;
 };
+
+namespace detail {
+// frame k's rows of a StereoSession::read into f's feature arrays: points [p0, p0 + np), lines [l0, l0 + nl)
+inline void frameFromRead(const StereoSession::Frames& r, size_t p0, size_t np, size_t l0, size_t nl, StereoFrame& f) {
+    auto cut = [](auto& dst, const auto& src, size_t first, size_t count, size_t w) {
+        dst.assign(src.begin() + (std::ptrdiff_t)(first * w), src.begin() + (std::ptrdiff_t)((first + count) * w));
+    };
+    cut(f.pt_pl, r.pt_pl, p0, np, 2); cut(f.pt_disp, r.pt_disp, p0, np, 1); cut(f.pt_P, r.pt_P, p0, np, 3);
+    cut(f.pt_sigma2, r.pt_sigma2, p0, np, 1); cut(f.pt_level, r.pt_level, p0, np, 1); cut(f.pt_src, r.pt_src, p0, np, 1);
+    cut(f.pdesc, r.pdesc, p0, np, 32);
+    cut(f.ls_spl, r.ls_spl, l0, nl, 2); cut(f.ls_epl, r.ls_epl, l0, nl, 2); cut(f.ls_sdisp, r.ls_sdisp, l0, nl, 1);
+    cut(f.ls_edisp, r.ls_edisp, l0, nl, 1); cut(f.ls_sP, r.ls_sP, l0, nl, 3); cut(f.ls_eP, r.ls_eP, l0, nl, 3);
+    cut(f.ls_le, r.ls_le, l0, nl, 3); cut(f.ls_angle, r.ls_angle, l0, nl, 1); cut(f.ls_sigma2, r.ls_sigma2, l0, nl, 1);
+    cut(f.ls_level, r.ls_level, l0, nl, 1); cut(f.ls_src, r.ls_src, l0, nl, 1); cut(f.ldesc, r.ldesc, l0, nl, 32);
+}
+}  // namespace detail
 
 namespace detail {
 // n frames of one size (channels bytes per pixel), copied into the contiguous arrays a PlStereoImages of images alone points at
@@ -881,7 +941,10 @@ inline PlOrbDetectConfig handlerOrbConfig(PlOrbDetectConfig oc) {
 // the kept frame with the prior f2fTracking builds from prev_frame, and keeps the new frame in its place.  The results equal
 // those of plstvo_track_stereo_raw_images_batch on (previous images, new images), byte for byte.  As in the reference's loop,
 // updateFrame follows each insertStereoPair: the device already holds the new frame as the previous one.  prev_frame /
-// curr_frame hold the pose state; their feature arrays stay empty.
+// curr_frame hold the pose state; their feature arrays stay empty unless keepFeatures(true) is on.  Then initialize fills
+// prev_frame's arrays and insertStereoPair curr_frame's, with matches_pt / _ls and inlier_pt / _ls as StereoFrameHandler
+// has them, all read back from the device after the call (StereoSession::read): such a frame can be given to the
+// features-in StereoFrameHandler as it is.
 class StereoImageHandler {
 public:
     StereoImageHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
@@ -901,13 +964,24 @@ public:
         orb_fast_th = hcfg_.orb_fast_th;                 // :38
         images(img_l, img_r);
         const int32_t id = 0;
-        session_.initialize(1, &id, frame_);
+        int32_t ns[2] = {0, 0};
+        session_.initialize(1, &id, frame_, ns);
         frame_ = PlStereoImages{};
         prev_frame = StereoFrame{};
         prev_frame.frame_idx = idx;
         for (int i = 0; i < 36; ++i) prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+        if (keep_) {
+            session_.read(1, ns, false, read_);
+            detail::frameFromRead(read_, 0, (size_t)ns[0], 0, (size_t)ns[1], prev_frame);
+        }
         kf = KeyframeTest{};                             // :48-51
         has_prev_ = true;
+    }
+    // keep each frame's stereo features and the matches on the host after every call (off by default); effective from the
+    // next initialize / insertStereoPair
+    void keepFeatures(bool on) {
+        session_.retain(on);
+        keep_ = on;
     }
     void insertStereoPair(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // :54-60
         if (!has_prev_) throw Error(PLSTVO_E_INVALID, "initialize() first");
@@ -923,6 +997,14 @@ public:
         const PlStereoImages f = frame_;
         frame_ = PlStereoImages{};
         session_.insert(1, &id, f, &prior, &result_, n_stereo.data());
+        if (keep_) {
+            session_.read(1, n_stereo.data(), true, read_);
+            detail::frameFromRead(read_, 0, (size_t)n_stereo[2], 0, (size_t)n_stereo[3], curr_frame);
+            matches_pt = std::move(read_.m12_pt);
+            matches_ls = std::move(read_.m12_ls);
+            inlier_pt = std::move(read_.inlier_pt);
+            inlier_ls = std::move(read_.inlier_ls);
+        }
         n_inliers_pt = result_.n_matched_pt;             // :126-128
         n_inliers_ls = result_.n_matched_ls;
         n_inliers = n_inliers_pt + n_inliers_ls;
@@ -945,6 +1027,8 @@ public:
 
     StereoFrame prev_frame, curr_frame;
     std::array<int32_t, 4> n_stereo{};                   // stereo points, lines of prev, then of curr, in the last call
+    std::vector<int32_t> matches_pt, matches_ls;         // keepFeatures: prev index -> curr index or -1
+    std::vector<uint8_t> inlier_pt, inlier_ls;           // keepFeatures: per prev feature, matched and still an inlier
     int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
     int orb_fast_th = 20;                                // include/stereoFrameHandler.h:62
     KeyframeTest kf;
@@ -963,6 +1047,8 @@ private:
     PlStereoImages frame_{};
     int32_t th_ = 0;
     bool has_prev_ = false;
+    bool keep_ = false;
+    StereoSession::Frames read_;
 };
 
 // Many StereoImageHandlers at once: one per stream (camera) of a session, each with the reference handler's state, and one
@@ -975,6 +1061,8 @@ public:
     struct Stream {
         StereoFrame prev_frame, curr_frame;
         std::array<int32_t, 4> n_stereo{};               // stereo points, lines of prev, then of curr, in the stream's last insert
+        std::vector<int32_t> matches_pt, matches_ls;     // keepFeatures: prev index -> curr index or -1
+        std::vector<uint8_t> inlier_pt, inlier_ls;       // keepFeatures: per prev feature, matched and still an inlier
         int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
         int orb_fast_th = 20;
         KeyframeTest kf;
@@ -994,13 +1082,21 @@ public:
                     const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
         const std::vector<int32_t> th(ids.size(), hcfg_.orb_fast_th);   // :38
         pack_.pack(cam_.width, cam_.height, channels_, img_l, img_r, th, "StereoStreamsHandler::initialize");
-        session_.initialize((int)ids.size(), ids.data(), pack_.view);
+        std::vector<int32_t> ns(2 * ids.size());
+        session_.initialize((int)ids.size(), ids.data(), pack_.view, ns.data());
+        if (keep_) session_.read((int)ids.size(), ns.data(), false, read_);
+        size_t p0 = 0, l0 = 0;
         for (size_t k = 0; k < ids.size(); ++k) {
             Stream& s = streams_[(size_t)ids[k]];
             s.orb_fast_th = hcfg_.orb_fast_th;
             s.prev_frame = StereoFrame{};
             s.prev_frame.frame_idx = k < idx.size() ? idx[k] : 0;
             for (int i = 0; i < 36; ++i) s.prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+            if (keep_) {
+                detail::frameFromRead(read_, p0, (size_t)ns[2 * k], l0, (size_t)ns[2 * k + 1], s.prev_frame);
+                p0 += (size_t)ns[2 * k];
+                l0 += (size_t)ns[2 * k + 1];
+            }
             s.curr_frame = StereoFrame{};
             s.kf = KeyframeTest{};                       // :48-51
             s.has_prev = true;
@@ -1021,12 +1117,28 @@ public:
         std::vector<PlPoseResult> res(ids.size());
         std::vector<int32_t> ns(4 * ids.size());
         session_.insert((int)ids.size(), ids.data(), pack_.view, priors.data(), res.data(), ns.data());
+        if (keep_) session_.read((int)ids.size(), ns.data(), true, read_);
+        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
         for (size_t k = 0; k < ids.size(); ++k) {
             Stream& s = streams_[(size_t)ids[k]];
             s.curr_frame = StereoFrame{};
             s.curr_frame.frame_idx = k < idx.size() ? idx[k] : 0;
             s.result = res[k];
             std::copy(ns.begin() + 4 * k, ns.begin() + 4 * k + 4, s.n_stereo.begin());
+            if (keep_) {
+                const size_t kp = (size_t)ns[4 * k], kl = (size_t)ns[4 * k + 1], np = (size_t)ns[4 * k + 2], nl = (size_t)ns[4 * k + 3];
+                detail::frameFromRead(read_, p0, np, l0, nl, s.curr_frame);
+                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
+                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
+                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                p0 += np;
+                l0 += nl;
+                kp0 += kp;
+                kl0 += kl;
+            }
             s.n_inliers_pt = s.result.n_matched_pt;      // :126-128
             s.n_inliers_ls = s.result.n_matched_ls;
             s.n_inliers = s.n_inliers_pt + s.n_inliers_ls;
@@ -1048,6 +1160,12 @@ public:
     bool needNewKF(int id) { Stream& s = at(id); return s.kf.needNewKF(hcfg_, s.curr_frame); }
     void currFrameIsKF(int id) { Stream& s = at(id); s.kf.currFrameIsKF(s.curr_frame); }
 
+    // StereoImageHandler::keepFeatures for every stream: initialize fills the named streams' prev_frame arrays,
+    // insertStereoPairs their curr_frame arrays and matches_pt / _ls, inlier_pt / _ls
+    void keepFeatures(bool on) {
+        session_.retain(on);
+        keep_ = on;
+    }
     Stream& stream(int id) { return at(id); }
     int streams() const { return (int)streams_.size(); }
     const StereoSession& session() const { return session_; }
@@ -1063,6 +1181,8 @@ private:
     std::vector<Stream> streams_;
     int channels_ = 1;   // bytes per pixel of the images: the rectifier's channels
     detail::StereoImagesBatch pack_;
+    bool keep_ = false;
+    StereoSession::Frames read_;
 };
 
 }  // namespace plstvo

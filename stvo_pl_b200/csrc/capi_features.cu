@@ -1156,6 +1156,7 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
         ss->pool[0].buf.release();
         ss->pool[1].buf.release();
         ss->d_meta.release();
+        ss->kept.buf.release();
     }
     delete ss;
 }
@@ -1163,7 +1164,46 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
 int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
     if (!ss) return 0;
     LOCK(ss->ctx);
-    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap);
+    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap);
+}
+
+int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (on && ss->retain) return 0;   // already on: what the last call retained stays readable
+    ss->retain = on != 0;
+    ss->kept.valid = false;
+    if (!on) {
+        CK(ctx, cudaSetDevice(ctx->device));
+        ss->kept.buf.release();   // every call that wrote it blocked until done
+    }
+    return 0;
+}
+
+int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* ss, const PlStereoFrameOut* out) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss || !out) return fail(ctx, PLSTVO_E_INVALID, "null session or output");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (!ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
+    const SessionRetained& kr = ss->kept;
+    if (!kr.valid) return fail(ctx, PLSTVO_E_INVALID, "nothing retained: no call succeeded since retention was turned on, or the last call failed");
+    CK(ctx, cudaSetDevice(ctx->device));
+    using R = SessionRetained;
+    void* dst[R::N_ARRAYS] = {out->pt_pl, out->pt_disp, out->pt_P, out->pt_sigma2, out->pt_level, out->pdesc, out->pt_src,
+                              out->ls_spl, out->ls_epl, out->ls_sdisp, out->ls_edisp, out->ls_sP, out->ls_eP, out->ls_le,
+                              out->ls_angle, out->ls_sigma2, out->ls_level, out->ldesc, out->ls_src,
+                              out->m12_pt, out->inlier_pt, out->m12_ls, out->inlier_ls};
+    const int n_arrays = kr.track ? R::N_ARRAYS : R::M12_PT;   // after an initialize the tracker's arrays are left untouched
+    cudaStream_t s = ctx->s_main;
+    for (int k = 0; k < n_arrays; ++k) {
+        const size_t bytes = kr.rows[k] * (size_t)R::row_bytes[k];
+        if (dst[k] && bytes) CK(ctx, cudaMemcpyAsync(dst[k], kr.at<uint8_t>(k), bytes, cudaMemcpyDeviceToHost, s));
+    }
+    CK(ctx, cudaStreamSynchronize(s));
+    return kr.n;
 }
 
 namespace {
@@ -1175,9 +1215,17 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     LOCK(ctx);
     if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
     if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    ss->kept.valid = false;   // a failed call discards what the last one retained
     if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
     if (frames->B != n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from n");
-    if (n == 0) return 0;
+    if (n == 0) {
+        if (ss->retain) {   // an empty call succeeds and retains nothing
+            ss->kept.track = track;
+            ss->kept.n = 0;
+            ss->kept.valid = ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
+        }
+        return 0;
+    }
     if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
     if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
     std::vector<uint8_t> named((size_t)ss->n_streams, 0);
@@ -1206,7 +1254,14 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     }
     const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, true, ss->has_lc ? &ss->lc : nullptr,
                                        frames, nullptr, priors, results, n_stereo, false, ss->rect, ss);
-    if (rc == 0) session_commit(ss);
+    if (rc == 0) {
+        session_commit(ss);
+        if (ss->retain) {
+            ss->kept.track = track;
+            ss->kept.n = n;
+            ss->kept.valid = true;
+        }
+    }
     ss->ids = nullptr;   // the caller's array: not read after the call
     return rc;
 }

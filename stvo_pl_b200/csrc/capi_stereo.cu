@@ -478,6 +478,32 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         CK(ctx, lift_prev_lines(sets[1], next, session_out_off(session, true)));
         ctx->launches += 2;
         if (const int rc = session_gather_others(ctx, session, s)) return rc;
+        if (session->retain) {   // plstvo_stereo_session_read: every record of the new frames, compact in call order
+            SessionRetained& kr = session->kept;
+            CK(ctx, kr.lay_out((size_t)ooff[0][NF], (size_t)ooff[1][NF], track ? (size_t)session->kept_off_pt[NF] : 0,
+                               track ? (size_t)session->kept_off_ls[NF] : 0));
+            cudaEvent_t offsets_up = next_event(ctx);   // sets[k].o_ooff, uploaded on sh above
+            CK(ctx, cudaEventRecord(offsets_up, sh));
+            CK(ctx, cudaStreamWaitEvent(s, offsets_up, 0));
+            using R = SessionRetained;
+            const Set& sp = sets[0];
+            const Set& sl = sets[1];
+            const cudaError_t e_pt =
+                launch_lift_points(*cam, *sc, NF, a.i32(sp.o_loff), sp.g_xyl, sp.g_oct, sp.g_d1, a.i32(sp.o_roff), sp.g_xyr,
+                                   a.i32(sp.o_m12), kr.at<double>(R::PT_PL), kr.at<double>(R::PT_DISP), kr.at<double>(R::PT_P),
+                                   kr.at<double>(R::PT_S2), kr.at<int32_t>(R::PT_LEVEL), kr.at<uint8_t>(R::PT_DESC),
+                                   kr.at<int32_t>(R::PT_SRC), a.i32(sp.o_cnt), s, a.i32(sp.o_ooff));
+            CK(ctx, e_pt);
+            const cudaError_t e_ls =
+                launch_lift_lines(*cam, *sc, NF, a.i32(sl.o_loff), sl.g_xyl, a.f32(sl.o_ang), sl.g_oct, sl.g_d1,
+                                  a.i32(sl.o_roff), sl.g_xyr, a.i32(sl.o_m12), kr.at<double>(R::LS_SPL), kr.at<double>(R::LS_EPL),
+                                  kr.at<double>(R::LS_SDISP), kr.at<double>(R::LS_EDISP), kr.at<double>(R::LS_SP),
+                                  kr.at<double>(R::LS_EP), kr.at<double>(R::LS_LE), kr.at<double>(R::LS_ANGLE),
+                                  kr.at<double>(R::LS_S2), kr.at<int32_t>(R::LS_LEVEL), kr.at<uint8_t>(R::LS_DESC),
+                                  kr.at<int32_t>(R::LS_SRC), a.i32(sl.o_cnt), s, a.i32(sl.o_ooff));
+            CK(ctx, e_ls);
+            ctx->launches += 2;
+        }
         if (!track) {
             if (dev && dev->marks) {
                 CK(ctx, cudaEventRecord(dev->marks[1], s));
@@ -536,6 +562,15 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     rc = ws_launch_solve(ctx, ws, 0, B, true, s);
     if (rc) return rc;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[2], s));
+    if (session && session->retain) {   // the tracker's rows, indexed by the kept frames' features (fp's offsets)
+        const SessionRetained& kr = session->kept;
+        const DevBuf* src[4] = {&ws.d_m12p, &ws.d_inlp, &ws.d_m12l, &ws.d_inll};
+        for (int k = 0; k < 4; ++k) {
+            const int r = SessionRetained::M12_PT + k;
+            const size_t bytes = kr.rows[r] * (size_t)SessionRetained::row_bytes[r];
+            if (bytes) CK(ctx, cudaMemcpyAsync(kr.at<uint8_t>(r), src[k]->p, bytes, cudaMemcpyDeviceToDevice, s));
+        }
+    }
     CK(ctx, cudaMemcpyAsync(results, ws.d_results.p, (size_t)B * sizeof(PlPoseResult), cudaMemcpyDeviceToHost, s));
     if (slot < 0) CK(ctx, cudaStreamSynchronize(s));
     return 0;

@@ -406,6 +406,25 @@ struct GatherSeg {
 };
 cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s);
 
+// The records a session call retains for plstvo_stereo_session_read (plstvo_stereo_session_retain): the new frames' full
+// point and line records and the insert's m12 / inlier rows, one array each in PlStereoFrameOut's field order, rows in call
+// order.  lay_out() sizes the arena for one call; valid is set only when that call succeeded.
+struct SessionRetained {
+    enum {   // arrays, points first
+        PT_PL, PT_DISP, PT_P, PT_S2, PT_LEVEL, PT_DESC, PT_SRC,
+        LS_SPL, LS_EPL, LS_SDISP, LS_EDISP, LS_SP, LS_EP, LS_LE, LS_ANGLE, LS_S2, LS_LEVEL, LS_DESC, LS_SRC,
+        M12_PT, INL_PT, M12_LS, INL_LS, N_ARRAYS
+    };
+    static const int row_bytes[N_ARRAYS];
+    DevBuf buf;
+    size_t off[N_ARRAYS] = {};
+    size_t rows[N_ARRAYS] = {};   // of every array: the new frames' points / lines, the kept frames' points / lines
+    bool valid = false, track = false;
+    int n = 0;
+    cudaError_t lay_out(size_t new_pt, size_t new_ls, size_t kept_pt, size_t kept_ls);
+    template <typename T> T* at(int k) const { return reinterpret_cast<T*>(buf.as<uint8_t>() + off[k]); }
+};
+
 }  // namespace plstvo
 
 // n_streams independent stereo streams, each with the previous-frame-role records of its kept frame in HBM
@@ -436,6 +455,9 @@ struct PlStereoSession {
     std::vector<int32_t> new_pt, new_ls;             // [n] the new frames' stereo points / lines
     std::vector<int32_t> meta;                       // uploaded: out_off_pt [n], out_off_ls [n], GatherSeg named [n], others
     int n_others = 0;
+    // ---- plstvo_stereo_session_retain / _read ----
+    bool retain = false;
+    plstvo::SessionRetained kept;                    // the last call's records while retain is on
 };
 
 namespace plstvo {

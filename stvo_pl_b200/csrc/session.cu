@@ -79,6 +79,19 @@ cudaError_t SessionPool::ensure(size_t n_pt, size_t n_ls) {
     return cudaSuccess;
 }
 
+const int SessionRetained::row_bytes[SessionRetained::N_ARRAYS] = {16, 8, 24, 8, 4, 32, 4,
+                                                                   16, 16, 8, 8, 24, 24, 24, 8, 8, 4, 32, 4,
+                                                                   4, 1, 4, 1};
+
+cudaError_t SessionRetained::lay_out(size_t new_pt, size_t new_ls, size_t kept_pt, size_t kept_ls) {
+    Arena a;
+    for (int k = 0; k < N_ARRAYS; ++k) {
+        rows[k] = k < LS_SPL ? new_pt : k < M12_PT ? new_ls : (k == M12_PT || k == INL_PT) ? kept_pt : kept_ls;
+        off[k] = a.take(rows[k] * (size_t)row_bytes[k]);
+    }
+    return a.alloc(buf);
+}
+
 int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s) {
     const int S = ss->n_streams, n = ss->n;
     std::vector<int> slot((size_t)S, -1);   // call position of each named stream

@@ -138,6 +138,8 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_stereo_session_device_bytes": (C.c_int64, [vp]),
         "plstvo_stereo_session_initialize": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), i32p]),
         "plstvo_stereo_session_insert": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), vp, vp, i32p]),
+        "plstvo_stereo_session_retain": (C.c_int, [vp, vp, C.c_int]),
+        "plstvo_stereo_session_read": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut)]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -167,7 +169,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_rectifier_destroy", "plstvo_rectify_batch", "plstvo_rectify_kernel_times", "plstvo_track_stereo_raw_images_batch",
     "plstvo_track_stereo_raw_images_sequence", "plstvo_stereo_session_create", "plstvo_stereo_session_destroy",
     "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert",
-    "plstvo_rectifier_create_color"]
+    "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -219,6 +221,7 @@ class StereoSession:
 
     def __init__(self, eng: "Engine", handle, n_streams: int, rect: Optional[Rectifier] = None):
         self.eng, self.handle, self.n_streams, self.rect = eng, handle, n_streams, rect
+        self.last = None   # the last call, if it succeeded: (insert, n_stereo), which sizes read()'s arrays
 
     def check_frames(self, frames: dict):
         """ValueError unless a colour session's frames are colour images of its rectifier's size and channels."""
@@ -234,6 +237,40 @@ class StereoSession:
         """insertStereoPair + optimizePose for streams ids against their kept frames, which the new frames then replace.
         Returns (results [n], n_stereo [n, 4])."""
         return self.eng.stereo_session_insert(self, ids, frames, priors, results)
+
+    def retain(self, on: bool):
+        """plstvo_stereo_session_retain: from the next initialize / insert on, keep each call's new frames and matches on the
+        device for read(); off frees them."""
+        self.eng._ck(self.eng.lib.plstvo_stereo_session_retain(self.eng.ctx, self.handle, 1 if on else 0))
+
+    def read(self):
+        """plstvo_stereo_session_read of the last call: (pt, ls, m12_pt, inlier_pt, m12_ls, inlier_ls).  pt / ls hold the new
+        frames' records in call order under the keys of Engine.match_stereo_points / _lines (counts: each frame's rows); the
+        tracker's rows are indexed by the kept frames' features in call order, and are None after an initialize."""
+        track, ns = self.last if self.last is not None else (False, np.zeros((0, 2), np.int32))
+        n = len(ns)
+        np_, nl = int(ns[:, -2].sum()), int(ns[:, -1].sum())
+        pt = self.eng.stereo_outputs(np_, n, lines=False)
+        ls = self.eng.stereo_outputs(nl, n, lines=True)
+        for d, col in ((pt, -2), (ls, -1)):
+            del d["m12"]
+            d["counts"][...] = ns[:, col]
+        kp, kl = (int(ns[:, 0].sum()), int(ns[:, 1].sum())) if track else (0, 0)
+        m12_pt, m12_ls = np.full(kp, -1, np.int32), np.full(kl, -1, np.int32)
+        inl_pt, inl_ls = np.zeros(kp, np.uint8), np.zeros(kl, np.uint8)
+        o = T.PlStereoFrameOut()
+        for f, key in T.FRAME_OUT_POINT_KEYS.items():
+            setattr(o, f, pt[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
+        for f, key in T.FRAME_OUT_LINE_KEYS.items():
+            setattr(o, f, ls[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
+        o.m12_pt, o.m12_ls = m12_pt.ctypes.data_as(T.c_int32_p), m12_ls.ctypes.data_as(T.c_int32_p)
+        o.inlier_pt, o.inlier_ls = inl_pt.ctypes.data_as(T.c_uint8_p), inl_ls.ctypes.data_as(T.c_uint8_p)
+        got = self.eng._ck(self.eng.lib.plstvo_stereo_session_read(self.eng.ctx, self.handle, C.byref(o)))
+        if got != n:
+            raise PlstvoError(-1, f"plstvo_stereo_session_read returned {got} frames, the last call had {n}")
+        if not track:
+            return pt, ls, None, None, None, None
+        return pt, ls, m12_pt, inl_pt, m12_ls, inl_ls
 
     @property
     def device_bytes(self) -> int:
@@ -890,9 +927,11 @@ class Engine:
         ids = np.ascontiguousarray(ids, np.int32)
         fs, keep = T.stereo_images_as_c(frames)
         n_stereo = np.zeros((len(ids), 2), np.int32)
+        ss.last = None
         self._ck(self.lib.plstvo_stereo_session_initialize(self.ctx, ss.handle, len(ids), _p(ids, T.c_int32_p), C.byref(fs),
                                                            _p(n_stereo, T.c_int32_p)))
         del keep
+        ss.last = (False, n_stereo.copy())
         return n_stereo
 
     def stereo_session_insert(self, ss: StereoSession, ids, frames: dict, priors=None, results=None):
@@ -903,10 +942,12 @@ class Engine:
         if results is None:
             results = np.zeros(n, dtype=T.POSE_RESULT_DTYPE)
         n_stereo = np.zeros((n, 4), np.int32)
+        ss.last = None
         self._ck(self.lib.plstvo_stereo_session_insert(self.ctx, ss.handle, n, _p(ids, T.c_int32_p), C.byref(fs),
                                                        priors.ctypes.data if priors is not None else None, results.ctypes.data,
                                                        _p(n_stereo, T.c_int32_p)))
         del keep
+        ss.last = (True, n_stereo.copy())
         return results, n_stereo
 
     def track_stereo_images_stage_times(self):

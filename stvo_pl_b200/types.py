@@ -173,6 +173,23 @@ class PlStereoImages(C.Structure):
                 ("angle_l", c_float_p), ("angle_r", c_float_p), ("npix_l", c_int32_p), ("npix_r", c_int32_p)]
 
 
+class PlStereoFrameOut(C.Structure):
+    """Destinations of plstvo_stereo_session_read (PlStereoFrameOut, include/plstvo.h); a NULL field is not copied."""
+    _fields_ = [("pt_pl", c_double_p), ("pt_disp", c_double_p), ("pt_P", c_double_p), ("pt_sigma2", c_double_p),
+                ("pt_level", c_int32_p), ("pdesc", c_uint8_p), ("pt_src", c_int32_p),
+                ("ls_spl", c_double_p), ("ls_epl", c_double_p), ("ls_sdisp", c_double_p), ("ls_edisp", c_double_p),
+                ("ls_sP", c_double_p), ("ls_eP", c_double_p), ("ls_le", c_double_p), ("ls_angle", c_double_p),
+                ("ls_sigma2", c_double_p), ("ls_level", c_int32_p), ("ldesc", c_uint8_p), ("ls_src", c_int32_p),
+                ("m12_pt", c_int32_p), ("inlier_pt", c_uint8_p), ("m12_ls", c_int32_p), ("inlier_ls", c_uint8_p)]
+
+
+# PlStereoFrameOut's point / line fields and the keys of Engine.match_stereo_points / _lines' outputs they correspond to
+FRAME_OUT_POINT_KEYS = dict(pt_pl="pl", pt_disp="disp", pt_P="P", pt_sigma2="sigma2", pt_level="level", pdesc="desc",
+                            pt_src="src_idx")
+FRAME_OUT_LINE_KEYS = dict(ls_spl="spl", ls_epl="epl", ls_sdisp="sdisp", ls_edisp="edisp", ls_sP="sP", ls_eP="eP", ls_le="le",
+                           ls_angle="angle", ls_sigma2="sigma2", ls_level="level", ldesc="desc", ls_src="src_idx")
+
+
 STEREO_IMAGE_DTYPES = dict(img_l=np.uint8, img_r=np.uint8, fast_th=np.int32, ll_off=np.int32, lr_off=np.int32, seg_l=np.float32,
                            seg_r=np.float32, angle_l=np.float32, angle_r=np.float32, npix_l=np.int32, npix_r=np.int32)
 
