@@ -560,6 +560,23 @@ PlStereoSession* plstvo_stereo_session_create(PlContext* ctx, const PlCamera* ca
                                               const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
                                               const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg, const PlRectifier* rect,
                                               int n_streams);
+/* A session whose stream i is tracked under its own camera cams[i] and prepared by its own rectifier rects[i]: N
+ * StereoFrameHandlers, each built on its own PinholeStereoCamera (app/imagesStVO.cpp:66,86, src/stereoFrameHandler.cpp:29).
+ * Every camera must have one width / height (PLSTVO_E_SIZE otherwise); the configs are those of plstvo_stereo_session_create.
+ * rects == NULL (or every entry NULL): no stream is remapped.  In a grey session rects[i] == NULL takes stream i's images as
+ * given.  Every non-NULL rectifier must belong to ctx (PLSTVO_E_INVALID) and have the cameras' size (PLSTVO_E_SIZE), and all
+ * must have one channel count (PLSTVO_E_INVALID).  A colour session needs a colour rectifier for every stream
+ * (PLSTVO_E_INVALID for a NULL entry): give one without maps where a camera needs no remap.  Rectifiers must outlive the
+ * session.  _initialize, _insert, _retain, _read, _device_bytes and _destroy work on it unchanged.
+ * Contract: without rectifiers, each stream's results, n_stereo and _read rows equal, byte for byte, those of a
+ * plstvo_stereo_session_create session with that stream's camera driven through the same calls; with rectifiers, those of
+ * the same session without them fed each stream's frames after plstvo_rectify_batch with its rectifier.  Device memory
+ * besides the plain session's: a call table of n cameras (48 bytes each, counted by plstvo_stereo_session_device_bytes) and,
+ * with rectifiers, a table of 2 n map pointers beside the call's staged images. */
+PlStereoSession* plstvo_stereo_session_create_cams(PlContext* ctx, const PlCamera* cams /* [n_streams] */, const PlConfig* cfg,
+                                                   const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                                   const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                                   const PlRectifier* const* rects /* [n_streams] or NULL */, int n_streams);
 void    plstvo_stereo_session_destroy(PlStereoSession* s);
 int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* s);
 /* StereoFrameHandler::initialize(img_l, img_r) for streams ids[0 .. n) (any subset of [0, n_streams), any order, no
@@ -636,6 +653,15 @@ int plstvo_track_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
                        const PlFrameBatch* prev, const PlFrameBatch* curr, const PlPrior* priors,
                        PlPoseResult* results, int32_t* m12_pt, int32_t* m12_ls,
                        uint8_t* inlier_pt, uint8_t* inlier_ls);
+
+/* plstvo_track_batch with pair p solved under cams[p] (B cameras: several calibrated rigs in one batch).  Row p of every
+ * output equals row p of plstvo_track_batch on the same inputs with cam = cams[p], byte for byte: matching does not read the
+ * camera, the solver plan depends on B and the list lengths only, and each pair is solved on its own.  Same H2D / compute /
+ * D2H pipeline and errors as plstvo_track_batch (PLSTVO_E_INVALID for cams NULL); device memory besides its: B x 48 bytes. */
+int plstvo_track_batch_cams(PlContext* ctx, const PlCamera* cams /* [B] */, const PlConfig* cfg,
+                            const PlFrameBatch* prev, const PlFrameBatch* curr, const PlPrior* priors,
+                            PlPoseResult* results, int32_t* m12_pt, int32_t* m12_ls,
+                            uint8_t* inlier_pt, uint8_t* inlier_ls);
 
 /* Streaming form of plstvo_track_batch: enqueues the batch (H2D, kernels, D2H) and returns a ticket >= 0 without
  * waiting, so that the caller can submit batch k+1 (its H2D then overlaps the kernels of batch k) before it waits for

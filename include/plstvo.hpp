@@ -826,6 +826,20 @@ public:
         s_ = plstvo_stereo_session_create(c.get(), &cam, &cfg, &mc, &sc, &oc, &lc, rect ? rect->get() : nullptr, n_streams);
         if (!s_) throw Error(PLSTVO_E_INVALID, plstvo_last_error(c.get()));
     }
+    // plstvo_stereo_session_create_cams: stream i tracked under cams[i] and prepared by rects[i] (rects empty: no stream is
+    // remapped; a null entry in a grey session: that stream's images as given).  The rectifiers must outlive the session.
+    StereoSession(Context& c, const std::vector<PlCamera>& cams, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                  const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                  const std::vector<const Rectifier*>& rects = {})
+        : c_(c), n_streams_((int)cams.size()) {
+        if (!rects.empty() && rects.size() != cams.size())
+            throw Error(PLSTVO_E_INVALID, "StereoSession: one rectifier (or null) per camera");
+        std::vector<const PlRectifier*> r;
+        for (const Rectifier* x : rects) r.push_back(x ? x->get() : nullptr);
+        s_ = plstvo_stereo_session_create_cams(c.get(), cams.data(), &cfg, &mc, &sc, &oc, &lc, r.empty() ? nullptr : r.data(),
+                                               (int)cams.size());
+        if (!s_) throw Error(PLSTVO_E_INVALID, plstvo_last_error(c.get()));
+    }
     ~StereoSession() { plstvo_stereo_session_destroy(s_); }
     StereoSession(const StereoSession&) = delete;
     StereoSession& operator=(const StereoSession&) = delete;
@@ -1074,6 +1088,20 @@ public:
                          const HandlerConfig& hcfg = HandlerConfig{}, const Rectifier* rect = nullptr)
         : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, n_streams, rect),
           streams_((size_t)n_streams), channels_(rect ? rect->channels() : 1) {
+        for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
+    }
+    // One camera per stream, as one PinholeStereoCamera per StereoFrameHandler in the reference, and optionally one rectifier
+    // per stream (StereoSession's cams constructor).  The cameras share one image size.
+    StereoStreamsHandler(Context& ctx, const std::vector<PlCamera>& cams, const PlConfig& cfg, const PlStereoMatchConfig& mc,
+                         const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
+                         const HandlerConfig& hcfg = HandlerConfig{}, const std::vector<const Rectifier*>& rects = {})
+        : cam_(cams.at(0)), hcfg_(hcfg), session_(ctx, cams, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, rects),
+          streams_(cams.size()) {
+        for (const Rectifier* r : rects)
+            if (r) {
+                channels_ = r->channels();
+                break;
+            }
         for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
     }
 

@@ -91,8 +91,10 @@ StreamBufs stream_bufs_at(const StreamBufs& sb, int p0) {
 // Launches the planned solver on pairs [p0, p1) of a batch of B: prm filled but for the solver's fields, feat the batch's
 // global list scratch (pl.feat_stride doubles per pair), slots_pt / slots_ls the record slots of the streamed solver's arena.
 // marks: 4 events recorded between the solver's stages (instrumentation only).
+// cams (optional, device, [B]): the camera of each pair instead of prm.cam.
 int launch_solver(PlContext* ctx, SolveParams prm, const SolvePlan& pl, double* feat, DevBuf& stream_arena, int B,
-                  size_t slots_pt, size_t slots_ls, int p0, int p1, cudaStream_t s, cudaEvent_t* marks = nullptr) {
+                  size_t slots_pt, size_t slots_ls, int p0, int p1, cudaStream_t s, cudaEvent_t* marks = nullptr,
+                  const PlCamera* cams = nullptr) {
     prm.first_pair = p0;
     prm.feat_scratch = pl.feat_in_smem ? nullptr : feat + (size_t)p0 * pl.feat_stride;
     prm.feat_scratch_stride = pl.feat_stride;
@@ -107,13 +109,13 @@ int launch_solver(PlContext* ctx, SolveParams prm, const SolvePlan& pl, double* 
         prm.feat_scratch = feat + (size_t)p0 * pl.feat_stride;
         prm.feat_in_smem = 0;
         int nl = 0;
-        CK(ctx, launch_stream_solve(prm, p1 - p0, stream_bufs_at(sb, p0), s, &nl, marks));
+        CK(ctx, launch_stream_solve(prm, p1 - p0, stream_bufs_at(sb, p0), s, &nl, marks, cams));
         ctx->launches += nl;
         return 0;
     }
     if (marks)   // fused kernel: list building, both GN stages and the outlier pass are inside K2
         for (int k = 0; k < 4; ++k) CK(ctx, cudaEventRecord(marks[k], s));
-    CK(ctx, launch_track_solve(prm, p1 - p0, s));
+    CK(ctx, launch_track_solve(prm, p1 - p0, s, cams));
     ctx->launches++;
     return 0;
 }
@@ -149,9 +151,11 @@ int validate_frames(PlContext* ctx, const PlFrameBatch* prev, const PlFrameBatch
 namespace plstvo {
 
 // Builds the plan of a batch of pairs and sizes every device buffer.  `with_features` = track mode.
+// d_cams (optional): the device camera of each pair, which the solver then reads instead of cam.
 int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfig* cfg, const PlFrameBatch* prev,
-               const PlFrameBatch* curr, bool with_features, bool has_priors) {
+               const PlFrameBatch* curr, bool with_features, bool has_priors, const PlCamera* d_cams) {
     const int B = prev->B;
+    ws.d_cams = d_cams;
     // Same shapes and matching parameters as the previous call on this workspace (a video stream, a benchmark loop):
     // the plan, the partial buffers and their device copies are still valid — skip the rebuild and its uploads.
     if (ws.planned && ws.B == B && ws.planned_features == with_features && ws.sm_planned == ctx->sm_count &&
@@ -383,7 +387,7 @@ int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_lev
     prm.inlier_ls = ws.d_inll.as<uint8_t>();
     prm.phase_cycles = ws.d_phase.as<long long>();
     return launch_solver(ctx, prm, ws.solver, ws.d_feat.as<double>(), ws.d_stream, ws.B, (size_t)ws.p_off1[ws.B],
-                         (size_t)ws.l_off1[ws.B], p0, p1, s, marks);
+                         (size_t)ws.l_off1[ws.B], p0, p1, s, marks, ws.d_cams);
 }
 
 #define D2H(ctx, dst, src, elem_bytes, first, count, stream)                                                 \
@@ -741,13 +745,18 @@ int plstvo_optimize_pose(PlContext* ctx, const PlCamera* cam, const PlConfig* cf
     return 0;
 }
 
-// enqueue one batch on the context's streams: chunked H2D -> K1 -> K2 -> D2H, nothing is waited for
+// enqueue one batch on the context's streams: chunked H2D -> K1 -> K2 -> D2H, nothing is waited for.  cams (optional, host,
+// [B]): pair p is solved under cams[p] instead of cam.
 static int track_enqueue(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfig* cfg,
                          const PlFrameBatch* prev, const PlFrameBatch* curr, const PlPrior* priors,
                          PlPoseResult* results, int32_t* m12_pt, int32_t* m12_ls, uint8_t* inlier_pt,
-                         uint8_t* inlier_ls, bool pipelined) {
+                         uint8_t* inlier_ls, bool pipelined, const PlCamera* cams = nullptr) {
     const int B = prev->B;
-    int rc = ws_prepare(ctx, ws, cam, cfg, prev, curr, true, priors != nullptr);
+    if (cams) {   // ahead of the first chunk's uploads on the same stream, so every chunk's solver sees it
+        CK(ctx, ws.d_pair_cams.ensure((size_t)B * sizeof(PlCamera)));
+        CK(ctx, cudaMemcpyAsync(ws.d_pair_cams.p, cams, (size_t)B * sizeof(PlCamera), cudaMemcpyHostToDevice, ctx->s_h2d));
+    }
+    int rc = ws_prepare(ctx, ws, cam, cfg, prev, curr, true, priors != nullptr, cams ? ws.d_pair_cams.as<PlCamera>() : nullptr);
     if (rc) return rc;
     const bool have_level = prev->ls_level != nullptr;
     const std::vector<int> bounds = chunk_schedule(B, ctx->sm_count, pipelined);
@@ -784,6 +793,22 @@ int plstvo_track_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg,
     rc = track_enqueue(ctx, ctx->ws, cam, cfg, prev, curr, priors, results, m12_pt, m12_ls, inlier_pt, inlier_ls, false);
     if (rc) return rc;
     CK(ctx, cudaStreamSynchronize(ctx->s_d2h));   // every chunk's D2H waited for its compute, which waited for its H2D
+    return 0;
+}
+
+int plstvo_track_batch_cams(PlContext* ctx, const PlCamera* cams, const PlConfig* cfg, const PlFrameBatch* prev,
+                            const PlFrameBatch* curr, const PlPrior* priors, PlPoseResult* results, int32_t* m12_pt,
+                            int32_t* m12_ls, uint8_t* inlier_pt, uint8_t* inlier_ls) {
+    if (!ctx || !cams || !cfg) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    CK(ctx, cudaSetDevice(ctx->device));
+    int rc = validate_frames(ctx, prev, curr, true);
+    if (rc) return rc;
+    if (prev->B == 0) return 0;
+    rc = track_enqueue(ctx, ctx->ws, &cams[0], cfg, prev, curr, priors, results, m12_pt, m12_ls, inlier_pt, inlier_ls, false,
+                       cams);
+    if (rc) return rc;
+    CK(ctx, cudaStreamSynchronize(ctx->s_d2h));
     return 0;
 }
 

@@ -964,7 +964,12 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const uint8_t* rectified = nullptr;
     cudaEvent_t rectified_ready = nullptr;
     if (rect && (pts || lns)) {
-        if (const int rc = rectify_enqueue(ctx, rect, n_img, NF, iparts, ctx->s_main, &rectified)) return rc;
+        std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
+        if (session && !session->rects.empty())
+            for (int k = 0; k < NF; ++k) call_rects.push_back(session->rects[(size_t)session->ids[k]]);
+        if (const int rc = rectify_enqueue(ctx, rect, n_img, NF, iparts, ctx->s_main, &rectified,
+                                           call_rects.empty() ? nullptr : call_rects.data()))
+            return rc;
         rectified_ready = next_event(ctx);
         CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
     }
@@ -1148,6 +1153,45 @@ PlStereoSession* plstvo_stereo_session_create(PlContext* ctx, const PlCamera* ca
     return ss;
 }
 
+PlStereoSession* plstvo_stereo_session_create_cams(PlContext* ctx, const PlCamera* cams, const PlConfig* cfg,
+                                                   const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
+                                                   const PlOrbDetectConfig* ocfg, const PlLsdConfig* lcfg,
+                                                   const PlRectifier* const* rects, int n_streams) {
+    if (!ctx) return nullptr;
+    LOCK(ctx);
+    auto bad = [&](int code, const char* msg) -> PlStereoSession* {
+        fail(ctx, code, msg);
+        return nullptr;
+    };
+    if (!cams) return bad(PLSTVO_E_INVALID, "null cameras");
+    if (n_streams < 1) return bad(PLSTVO_E_INVALID, "n_streams must be at least 1");
+    for (int i = 1; i < n_streams; ++i)
+        if (cams[i].width != cams[0].width || cams[i].height != cams[0].height)
+            return bad(PLSTVO_E_SIZE, "the cameras differ in image size");
+    // the rectifier the images path sizes its staging by (the first one given), after every entry is checked against it
+    const PlRectifier* first = nullptr;
+    bool any_null = false;
+    for (int i = 0; rects && i < n_streams; ++i) {
+        const PlRectifier* r = rects[i];
+        if (!r) {
+            any_null = true;
+            continue;
+        }
+        if (r->ctx != ctx) return bad(PLSTVO_E_INVALID, "a rectifier belongs to another context");
+        if (r->width != cams[0].width || r->height != cams[0].height)
+            return bad(PLSTVO_E_SIZE, "rectifier size differs from the cameras'");
+        if (first && r->channels != first->channels) return bad(PLSTVO_E_INVALID, "the rectifiers differ in channel count");
+        if (!first) first = r;
+    }
+    if (first && first->channels > 1 && any_null)
+        return bad(PLSTVO_E_INVALID, "a colour session needs a colour rectifier for every stream (one without maps converts only)");
+    PlStereoSession* ss = plstvo_stereo_session_create(ctx, &cams[0], cfg, mcfg, scfg, ocfg, lcfg, first, n_streams);
+    if (!ss) return nullptr;
+    ss->cams.assign(cams, cams + n_streams);
+    if (first) ss->rects.assign(rects, rects + n_streams);   // all null: no stream is remapped, as with rects == NULL
+    return ss;
+}
+
 void plstvo_stereo_session_destroy(PlStereoSession* ss) {
     if (!ss) return;
     {
@@ -1157,6 +1201,7 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
         ss->pool[1].buf.release();
         ss->d_meta.release();
         ss->kept.buf.release();
+        ss->d_cams.release();
     }
     delete ss;
 }
@@ -1164,7 +1209,7 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
 int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
     if (!ss) return 0;
     LOCK(ss->ctx);
-    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap);
+    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap + ss->d_cams.cap);
 }
 
 int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {

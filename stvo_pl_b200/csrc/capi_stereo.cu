@@ -458,17 +458,26 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             CK(ctx, a.up(sets[k].o_ooff2, ooff2[k].data(), (size_t)NF * 4, sh));
         }
     }
+    // a cams session: the camera of each new frame (its stream's), for pass 2's lifts and for the solver (pair p = frame p)
+    const PlCamera* d_cams = nullptr;
+    if (session && !session->cams.empty()) {
+        std::vector<PlCamera> fc((size_t)NF);
+        for (int k = 0; k < NF; ++k) fc[(size_t)k] = session->cams[(size_t)session->ids[k]];
+        CK(ctx, session->d_cams.ensure((size_t)NF * sizeof(PlCamera)));
+        CK(ctx, cudaMemcpyAsync(session->d_cams.p, fc.data(), (size_t)NF * sizeof(PlCamera), cudaMemcpyHostToDevice, s));
+        d_cams = session->d_cams.as<PlCamera>();
+    }
     // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
     // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
     auto lift_prev_points = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
         return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
                                   a.i32(st.o_m12), nullptr, nullptr, o.ptP, o.pts2, nullptr, o.pdesc, nullptr, a.i32(st.o_cnt), s,
-                                  out_off);
+                                  out_off, d_cams);
     };
     auto lift_prev_lines = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
         return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1, a.i32(st.o_roff),
                                  st.g_xyr, a.i32(st.o_m12), o.spl, o.epl, nullptr, nullptr, o.sP, o.eP, nullptr, nullptr, o.s2,
-                                 o.lev, o.ldesc, nullptr, a.i32(st.o_cnt), s, out_off);
+                                 o.lev, o.ldesc, nullptr, a.i32(st.o_cnt), s, out_off, d_cams);
     };
     // session: the new frames' previous-frame role goes into the next pool, the untouched streams' kept frames follow it there
     if (session) {
@@ -492,7 +501,7 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
                 launch_lift_points(*cam, *sc, NF, a.i32(sp.o_loff), sp.g_xyl, sp.g_oct, sp.g_d1, a.i32(sp.o_roff), sp.g_xyr,
                                    a.i32(sp.o_m12), kr.at<double>(R::PT_PL), kr.at<double>(R::PT_DISP), kr.at<double>(R::PT_P),
                                    kr.at<double>(R::PT_S2), kr.at<int32_t>(R::PT_LEVEL), kr.at<uint8_t>(R::PT_DESC),
-                                   kr.at<int32_t>(R::PT_SRC), a.i32(sp.o_cnt), s, a.i32(sp.o_ooff));
+                                   kr.at<int32_t>(R::PT_SRC), a.i32(sp.o_cnt), s, a.i32(sp.o_ooff), d_cams);
             CK(ctx, e_pt);
             const cudaError_t e_ls =
                 launch_lift_lines(*cam, *sc, NF, a.i32(sl.o_loff), sl.g_xyl, a.f32(sl.o_ang), sl.g_oct, sl.g_d1,
@@ -500,7 +509,7 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
                                   kr.at<double>(R::LS_SDISP), kr.at<double>(R::LS_EDISP), kr.at<double>(R::LS_SP),
                                   kr.at<double>(R::LS_EP), kr.at<double>(R::LS_LE), kr.at<double>(R::LS_ANGLE),
                                   kr.at<double>(R::LS_S2), kr.at<int32_t>(R::LS_LEVEL), kr.at<uint8_t>(R::LS_DESC),
-                                  kr.at<int32_t>(R::LS_SRC), a.i32(sl.o_cnt), s, a.i32(sl.o_ooff));
+                                  kr.at<int32_t>(R::LS_SRC), a.i32(sl.o_cnt), s, a.i32(sl.o_ooff), d_cams);
             CK(ctx, e_ls);
             ctx->launches += 2;
         }
@@ -521,7 +530,7 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     fc.pt_off = sequence ? ooff2[0].data() : session ? ooff[0].data() : ooff[2].data();
     fc.ls_off = sequence ? ooff2[1].data() : session ? ooff[1].data() : ooff[3].data();
     Workspace& ws = slot < 0 ? ctx->ws : ctx->ws_async[slot];
-    int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr);
+    int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr, d_cams);
     if (rc) return rc;
     if (priors) CK(ctx, cudaMemcpyAsync(ws.d_priors.p, priors, (size_t)B * sizeof(PlPrior), cudaMemcpyHostToDevice, ctx->s_h2d));
     cudaEvent_t planned = next_event(ctx);
@@ -530,13 +539,13 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     auto lift_curr_points = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
         return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
                                   st.g_xyr, a.i32(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
-                                  ws.d_pdesc2.as<uint8_t>(), nullptr, a.i32(st.o_cnt) + first, s, a.i32(o_out));
+                                  ws.d_pdesc2.as<uint8_t>(), nullptr, a.i32(st.o_cnt) + first, s, a.i32(o_out), d_cams);
     };
     auto lift_curr_lines = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
         return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
                                  a.i32(st.o_roff) + first, st.g_xyr, a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr,
                                  nullptr, ws.d_lsle.as<double>(), nullptr, nullptr, nullptr, ws.d_ldesc2.as<uint8_t>(), nullptr,
-                                 a.i32(st.o_cnt) + first, s, a.i32(o_out));
+                                 a.i32(st.o_cnt) + first, s, a.i32(o_out), d_cams);
     };
     if (session) {
         if (const int rc2 = session_gather_named(ctx, session, workspace_prev_rows(ws), s)) return rc2;

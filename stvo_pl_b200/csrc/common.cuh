@@ -119,9 +119,12 @@ struct StreamBufs {
     int32_t* queue;           // problem queues of the persistent GN kernel (one int per launch of a solve: [2] per chunk)
     int32_t  sm_count;
 };
-// prm.feat_scratch must hold k2_feat_stride() doubles per pair; prm.feat_in_smem must be 0
+// prm.feat_scratch must hold k2_feat_stride() doubles per pair; prm.feat_in_smem must be 0.  cams (optional, device): the
+// camera of each pair, indexed by pair (prm.first_pair + p for the launch's pair p), instead of prm.cam; it selects the
+// kernels' instantiations that read it (a separate kernel parameter, after the existing ones).
 cudaError_t launch_stream_solve(const SolveParams& prm, int n_pairs, const StreamBufs& sb, cudaStream_t stream, int* launches,
-                                cudaEvent_t* marks = nullptr);   // marks: 4 events (see solve.cu), instrumentation only
+                                cudaEvent_t* marks = nullptr,    // marks: 4 events (see solve.cu), instrumentation only
+                                const PlCamera* cams = nullptr);
 
 size_t k2_smem_bytes(int cap_pt, int cap_ls, int sort_cap, bool feat_in_smem);
 size_t k2_feat_stride(int cap_pt, int cap_ls);   // doubles of global feature scratch per pair
@@ -129,7 +132,7 @@ size_t k2_feat_stride(int cap_pt, int cap_ls);   // doubles of global feature sc
 // kernel launchers (defined in match.cu / solve.cu)
 cudaError_t launch_match_finalize(const MatchProblem* problems, int n_problems, int max_n2, int32_t* counts,
                                   cudaStream_t stream);
-cudaError_t launch_track_solve(const SolveParams& prm, int n_pairs, cudaStream_t stream);
+cudaError_t launch_track_solve(const SolveParams& prm, int n_pairs, cudaStream_t stream, const PlCamera* cams = nullptr);
 cudaError_t launch_select_selftest(const double* v, const int32_t* off, const int32_t* ks, const double* pivot, int mode, int n_lists,
                                    double* out, cudaStream_t stream);
 cudaError_t launch_algebra_selftest(const double* H, const double* g, int n, double* x, double* lad, double* inv,
@@ -175,13 +178,14 @@ cudaError_t launch_lift_points(const PlCamera& cam, const PlStereoConfig& sc, in
                                const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off, const float* kp_r,
                                const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P, double* pt_sigma2,
                                int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts, cudaStream_t s,
-                               const int32_t* out_off = nullptr);   // out_off: compact output offsets per frame (else l_off); null outputs are skipped
+                               const int32_t* out_off = nullptr,    // out_off: compact output offsets per frame (else l_off); null outputs are skipped
+                               const PlCamera* cams = nullptr);     // cams: device camera of each frame (else cam)
 cudaError_t launch_lift_lines(const PlCamera& cam, const PlStereoConfig& sc, int B, const int32_t* l_off, const float* seg_l,
                               const float* ang_l, const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off,
                               const float* seg_r, const int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp,
                               double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le, double* ls_angle,
                               double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts,
-                              cudaStream_t s, const int32_t* out_off = nullptr);
+                              cudaStream_t s, const int32_t* out_off = nullptr, const PlCamera* cams = nullptr);
 
 // orb.cu: ORB description (pyramid, blur, border filter, angle, rBRIEF) of a batch of images of one size
 constexpr int ORB_MAX_LEVELS = 32;
@@ -288,9 +292,15 @@ cudaError_t launch_lbd(int n_img, int W, int H, const uint8_t* images, const int
                        cudaEvent_t* ev, int* launches);   // dir: (cosf, sinf) of each angle; ev[0..2]: start, gradients, descriptors
 
 // rectify.cu: cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of n_img grey W x H images on CV_16SC2 + CV_16UC1 maps; image z takes
-// the right maps (m1[1], m2[1]) where (z / per_block) is odd, the left ones otherwise
+// the right maps (m1[1], m2[1]) where (z / per_block) is odd, the left ones otherwise.  With a map table (device, [per_block][2])
+// image z takes maps[2 (z % per_block) + side] instead, and an entry with null maps is copied.
+struct RemapMaps {
+    const short2* m1;
+    const uint16_t* m2;
+};
 cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const uint8_t* src, uint8_t* dst,
-                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches);
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches,
+                                 const RemapMaps* maps = nullptr);
 
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);

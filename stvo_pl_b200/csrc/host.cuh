@@ -150,6 +150,8 @@ struct Workspace {
     std::vector<int32_t> item_start[2];   // [B+1] first work item of each pair in either list
     DevBuf d_tcprob, d_tcitems[2], d_rowp, d_colp, d_sched;
     DevBuf d_stream;       // arena of the streamed solver (frames too large for K2's shared memory)
+    const PlCamera* d_cams = nullptr;   // optional device camera of each pair [B] (ws_prepare), else cam for every pair
+    DevBuf d_pair_cams;    // plstvo_track_batch_cams: the caller's cameras, uploaded
 };
 
 }  // namespace plstvo
@@ -369,7 +371,7 @@ struct GridScratch {
 
 // ---- capi.cu: the tracker's plan and launches, composed by the stereo paths ----
 int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfig* cfg, const PlFrameBatch* prev,
-               const PlFrameBatch* curr, bool with_features, bool has_priors);
+               const PlFrameBatch* curr, bool with_features, bool has_priors, const PlCamera* d_cams = nullptr);
 int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t s, cudaEvent_t* marks = nullptr);
 int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_level, cudaStream_t s,
                     cudaEvent_t* marks = nullptr);
@@ -439,6 +441,10 @@ struct PlStereoSession {
     PlLsdConfig lc{};
     bool has_lc = false;
     const PlRectifier* rect = nullptr;
+    // plstvo_stereo_session_create_cams: stream i's camera and rectifier (empty: cam and rect for every stream)
+    std::vector<PlCamera> cams;
+    std::vector<const PlRectifier*> rects;
+    plstvo::DevBuf d_cams;                  // this call's camera of each new frame, call order (cams sessions)
     int n_streams = 0;
     std::vector<uint8_t> live;              // [S] the stream has a kept frame
     std::vector<int32_t> n_pt, n_ls;        // [S] its stereo points / lines
@@ -498,8 +504,10 @@ struct ImgPart {   // consecutive host images of one size
 };
 // Enqueues on stream s the upload of n_img raw images of rect's size and channels (parts, in order) into arena_rect's staging
 // slot and the grey device copy of them into its rectified slot (*d_out): their remap, in blocks of per_block images that
-// alternate left, right maps, and for a colour rectifier the conversion to grey after it.
+// alternate left, right maps, and for a colour rectifier the conversion to grey after it.  rects (optional, [per_block], of
+// rect's size and channels): image z is prepared by rects[z % per_block] instead, a null entry or one without maps copying
+// (grey) or converting (colour) the image.
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
-                    cudaStream_t s, const uint8_t** d_out);
+                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects = nullptr);
 
 }  // namespace plstvo

@@ -63,18 +63,21 @@ __device__ int block_scan_flag(int flag, int* s_warp, int* s_base, int* total_ro
     return pos;
 }
 
+// CAMS: frame f is back-projected under cams[f], else under cam.
+template <bool CAMS>
 __global__ void __launch_bounds__(LF_THREADS)
 lift_points_kernel(PlCamera cam, PlStereoConfig sc, const int32_t* __restrict__ l_off, const float* __restrict__ kp_l,
                    const int32_t* __restrict__ oct_l, const uint8_t* __restrict__ desc_l, const int32_t* __restrict__ r_off,
                    const float* __restrict__ kp_r, const int32_t* __restrict__ m12, double* pt_pl, double* pt_disp,
                    double* pt_P, double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx,
-                   int32_t* counts, const int32_t* __restrict__ out_off) {
+                   int32_t* counts, const int32_t* __restrict__ out_off, const PlCamera* __restrict__ cams) {
     // out_off == nullptr: frame f's records start at element l_off[f] of every output; else at out_off[f] (compact layout).
     // Output pointers may be null (not wanted); with all of them null the kernel only counts.
     __shared__ int s_warp[LF_THREADS / 32], s_base;
     const int f = blockIdx.x, tid = threadIdx.x;
     const int a0 = l_off[f], n = l_off[f + 1] - a0, b0 = r_off[f];
     const size_t o0 = out_off ? (size_t)out_off[f] : (size_t)a0;
+    if constexpr (CAMS) cam = cams[f];
     if (tid == 0) s_base = 0;
     __syncthreads();
     for (int base = 0; base < n; base += LF_THREADS) {
@@ -117,17 +120,20 @@ lift_points_kernel(PlCamera cam, PlStereoConfig sc, const int32_t* __restrict__ 
     if (tid == 0) counts[f] = s_base;
 }
 
+template <bool CAMS>
 __global__ void __launch_bounds__(LF_THREADS)
 lift_lines_kernel(PlCamera cam, PlStereoConfig sc, const int32_t* __restrict__ l_off, const float* __restrict__ seg_l,
                   const float* __restrict__ ang_l, const int32_t* __restrict__ oct_l, const uint8_t* __restrict__ desc_l,
                   const int32_t* __restrict__ r_off, const float* __restrict__ seg_r, const int32_t* __restrict__ m12,
                   double* ls_spl, double* ls_epl, double* ls_sdisp, double* ls_edisp, double* ls_sP, double* ls_eP,
                   double* ls_le, double* ls_angle, double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out,
-                  int32_t* src_idx, int32_t* counts, const int32_t* __restrict__ out_off) {
+                  int32_t* src_idx, int32_t* counts, const int32_t* __restrict__ out_off,
+                  const PlCamera* __restrict__ cams) {
     __shared__ int s_warp[LF_THREADS / 32], s_base;
     const int f = blockIdx.x, tid = threadIdx.x;
     const int a0 = l_off[f], n = l_off[f + 1] - a0, b0 = r_off[f];
     const size_t o0 = out_off ? (size_t)out_off[f] : (size_t)a0;
+    if constexpr (CAMS) cam = cams[f];
     if (tid == 0) s_base = 0;
     __syncthreads();
     for (int base = 0; base < n; base += LF_THREADS) {
@@ -246,10 +252,14 @@ cudaError_t launch_lift_points(const PlCamera& cam, const PlStereoConfig& sc, in
                                const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off, const float* kp_r,
                                const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P, double* pt_sigma2,
                                int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts, cudaStream_t s,
-                               const int32_t* out_off) {
+                               const int32_t* out_off, const PlCamera* cams) {
     if (B <= 0) return cudaSuccess;
-    lift_points_kernel<<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, pt_pl, pt_disp, pt_P,
-                                                pt_sigma2, pt_level, pdesc_out, src_idx, counts, out_off);
+    if (cams)
+        lift_points_kernel<true><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, pt_pl, pt_disp,
+                                                          pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts, out_off, cams);
+    else
+        lift_points_kernel<false><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, pt_pl, pt_disp,
+                                                           pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts, out_off, nullptr);
     return cudaGetLastError();
 }
 
@@ -258,11 +268,16 @@ cudaError_t launch_lift_lines(const PlCamera& cam, const PlStereoConfig& sc, int
                               const float* seg_r, const int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp,
                               double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le, double* ls_angle,
                               double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts,
-                              cudaStream_t s, const int32_t* out_off) {
+                              cudaStream_t s, const int32_t* out_off, const PlCamera* cams) {
     if (B <= 0) return cudaSuccess;
-    lift_lines_kernel<<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, ls_spl, ls_epl,
-                                               ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2, ls_level,
-                                               ldesc_out, src_idx, counts, out_off);
+    if (cams)
+        lift_lines_kernel<true><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, ls_spl,
+                                                         ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
+                                                         ls_level, ldesc_out, src_idx, counts, out_off, cams);
+    else
+        lift_lines_kernel<false><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, ls_spl,
+                                                          ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
+                                                          ls_level, ldesc_out, src_idx, counts, out_off, nullptr);
     return cudaGetLastError();
 }
 

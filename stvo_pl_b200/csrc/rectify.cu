@@ -28,13 +28,24 @@ __device__ __forceinline__ uint32_t remap_pixel(const uint8_t* __restrict__ S, i
     return (uint32_t)((sum + 512) >> 10);
 }
 
+// 4 bytes from 4-byte aligned D on, else byte by byte
+__device__ __forceinline__ void store4(uint8_t* D, uint32_t v) {
+    if (((uintptr_t)D & 3) == 0) {
+        *reinterpret_cast<uint32_t*>(D) = v;
+    } else {
+        D[0] = (uint8_t)v; D[1] = (uint8_t)(v >> 8); D[2] = (uint8_t)(v >> 16); D[3] = (uint8_t)(v >> 24);
+    }
+}
+
 // One thread writes 4 consecutive pixels of one image (flat index p0 .. p0 + 3 of W*H): one 16-byte map1 load, one 8-byte
 // map2 load, 16 byte gathers on the read-only path and one 4-byte store where the output is 4-byte aligned.  blockIdx.y is
-// the image within a slice of at most 65535 starting at z0.
+// the image within a slice of at most 65535 starting at z0.  TABLE: image z takes maps[2 (z % per_block) + side] instead of
+// the launch's two map pairs, and an entry without maps copies the image.
+template <bool TABLE>
 __global__ void __launch_bounds__(256) rectify_remap_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
                                                             const short2* __restrict__ m1l, const uint16_t* __restrict__ m2l,
                                                             const short2* __restrict__ m1r, const uint16_t* __restrict__ m2r,
-                                                            int W, int H, int per_block, int z0) {
+                                                            int W, int H, int per_block, int z0, const RemapMaps* __restrict__ maps) {
     const int z = z0 + (int)blockIdx.y;
     const size_t N = (size_t)W * H;
     const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -44,6 +55,19 @@ __global__ void __launch_bounds__(256) rectify_remap_kernel(const uint8_t* __res
     const uint16_t* m2 = right ? m2r : m2l;
     const uint8_t* S = src + (size_t)z * N;
     uint8_t* D = dst + (size_t)z * N + p0;
+    if constexpr (TABLE) {
+        const RemapMaps mp = maps[2 * (z % per_block) + (right ? 1 : 0)];
+        m1 = mp.m1;
+        m2 = mp.m2;
+        if (!m1) {
+            const size_t e = p0 + 4 <= N ? p0 + 4 : N;
+            if (e - p0 == 4)
+                store4(D, (uint32_t)S[p0] | (uint32_t)S[p0 + 1] << 8 | (uint32_t)S[p0 + 2] << 16 | (uint32_t)S[p0 + 3] << 24);
+            else
+                for (size_t p = p0; p < e; ++p) D[p - p0] = S[p];
+            return;
+        }
+    }
     if (p0 + 4 <= N) {   // the maps start 256-byte aligned, so p0 % 4 == 0 aligns both vector loads
         const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
         const uint2 b = __ldg(reinterpret_cast<const uint2*>(m2 + p0));
@@ -136,11 +160,12 @@ __device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, in
 
 // rectify_remap_kernel's layout on C-channel images: one thread writes 4 consecutive grey pixels of one image from one
 // 16-byte map1 load and one 8-byte map2 load; image z of the staging slot starts at z * W * H * C.
-template <int C>
+// TABLE: the maps of image z as in rectify_remap_kernel; an entry without maps converts the image only.
+template <int C, bool TABLE>
 __global__ void __launch_bounds__(256) color_remap_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
                                                           const short2* __restrict__ m1l, const uint16_t* __restrict__ m2l,
                                                           const short2* __restrict__ m1r, const uint16_t* __restrict__ m2r,
-                                                          int W, int H, int per_block, int z0) {
+                                                          int W, int H, int per_block, int z0, const RemapMaps* __restrict__ maps) {
     const int z = z0 + (int)blockIdx.y;
     const size_t N = (size_t)W * H;
     const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -150,6 +175,24 @@ __global__ void __launch_bounds__(256) color_remap_kernel(const uint8_t* __restr
     const uint16_t* m2 = right ? m2r : m2l;
     const uint8_t* S = src + (size_t)z * N * C;
     uint8_t* D = dst + (size_t)z * N + p0;
+    if constexpr (TABLE) {
+        const RemapMaps mp = maps[2 * (z % per_block) + (right ? 1 : 0)];
+        m1 = mp.m1;
+        m2 = mp.m2;
+        if (!m1) {
+            const size_t e = p0 + 4 <= N ? p0 + 4 : N;
+            uint32_t v = 0;
+            for (size_t p = p0; p < e; ++p) {
+                const uint8_t* q = S + p * C;
+                v |= bgr_to_grey(__ldg(q), __ldg(q + 1), __ldg(q + 2)) << (8 * (p - p0));
+            }
+            if (e - p0 == 4)
+                store4(D, v);
+            else
+                for (size_t p = p0; p < e; ++p) D[p - p0] = (uint8_t)(v >> (8 * (p - p0)));
+            return;
+        }
+    }
     if (p0 + 4 <= N) {
         const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
         const uint2 b = __ldg(reinterpret_cast<const uint2*>(m2 + p0));
@@ -187,21 +230,40 @@ void store_map(double u, double v, bool vec, int16_t* m1, uint16_t* m2) {
 namespace plstvo {
 
 cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const uint8_t* src, uint8_t* dst,
-                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches) {
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches,
+                                 const RemapMaps* maps) {
     const size_t quads = ((size_t)W * H + 3) / 4;
     const unsigned gx = (unsigned)((quads + 255) / 256);
     for (int z0 = 0; z0 < n_img; z0 += 65535) {
         const int nz = std::min(n_img - z0, 65535);
-        rectify_remap_kernel<<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block, z0);
+        if (maps)
+            rectify_remap_kernel<true><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, nullptr, nullptr, nullptr, nullptr, W, H,
+                                                                              per_block, z0, maps);
+        else
+            rectify_remap_kernel<false><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H,
+                                                                               per_block, z0, nullptr);
         ++*launches;
     }
     return cudaGetLastError();
 }
 
-// The grey device copy of n_img colour images (C channels): color_convert_kernel without maps, color_remap_kernel with.
+// The grey device copy of n_img colour images (C channels): color_convert_kernel without maps, color_remap_kernel with;
+// with a map table (per-image maps or none) its instantiation that reads it.
 template <int C>
 cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool maps, const uint8_t* src, uint8_t* dst,
-                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches) {
+                                 const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches,
+                                 const RemapMaps* table) {
+    if (table) {
+        const size_t quads = ((size_t)W * H + 3) / 4;
+        const unsigned gx = (unsigned)((quads + 255) / 256);
+        for (int z0 = 0; z0 < n_img; z0 += 65535) {
+            const int nz = std::min(n_img - z0, 65535);
+            color_remap_kernel<C, true><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, nullptr, nullptr, nullptr, nullptr, W, H,
+                                                                                per_block, z0, table);
+            ++*launches;
+        }
+        return cudaGetLastError();
+    }
     if (!maps) {
         const size_t groups = ((size_t)n_img * W * H + 15) / 16;
         color_convert_kernel<C><<<(unsigned)((groups + 255) / 256), 256, 0, s>>>(src, dst, (size_t)n_img * W * H);
@@ -212,21 +274,29 @@ cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool ma
     const unsigned gx = (unsigned)((quads + 255) / 256);
     for (int z0 = 0; z0 < n_img; z0 += 65535) {
         const int nz = std::min(n_img - z0, 65535);
-        color_remap_kernel<C><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block, z0);
+        color_remap_kernel<C, false><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block,
+                                                                             z0, nullptr);
         ++*launches;
     }
     return cudaGetLastError();
 }
 
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
-                    cudaStream_t s, const uint8_t** d_out) {
+                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects) {
     const int W = rect->width, H = rect->height, Ch = rect->channels;
     const size_t bytes = (size_t)n_img * W * H;
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, ctx->rect_ev.create());
+    std::vector<RemapMaps> table(rects ? 2 * (size_t)per_block : 0, RemapMaps{nullptr, nullptr});
+    for (size_t k = 0; k < table.size() / 2; ++k)
+        if (const PlRectifier* r = rects[k])
+            if (r->maps)
+                for (int side = 0; side < 2; ++side) table[2 * k + side] = RemapMaps{r->m1[side], r->m2[side]};
     Arena a;
-    const size_t o_raw = a.take(bytes * Ch), o_out = a.take(bytes);
+    const size_t o_raw = a.take(bytes * Ch), o_out = a.take(bytes), o_tab = a.take(table.size() * sizeof(RemapMaps));
     CK(ctx, a.alloc(ctx->arena_rect));
+    CK(ctx, a.up(o_tab, table.data(), table.size() * sizeof(RemapMaps), s));
+    const RemapMaps* d_tab = rects ? a.at<RemapMaps>(o_tab) : nullptr;
     size_t o = o_raw;
     for (const ImgPart& ip : parts) {
         const size_t b = (size_t)ip.n * W * H * Ch;
@@ -237,13 +307,13 @@ int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_
     ctx->rect_ran = false;
     CK(ctx, cudaEventRecord(ctx->rect_ev[0], s));
     if (Ch == 1)
-        CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches));
+        CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches, d_tab));
     else if (Ch == 3)
         CK(ctx, launch_color_prepare<3>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
-                                        &launches));
+                                        &launches, d_tab));
     else
         CK(ctx, launch_color_prepare<4>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
-                                        &launches));
+                                        &launches, d_tab));
     CK(ctx, cudaEventRecord(ctx->rect_ev[1], s));
     ctx->rect_ran = true;
     ctx->launches += launches;

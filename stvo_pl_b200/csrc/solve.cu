@@ -601,6 +601,14 @@ struct Cam {
     double fx, fy, cx, cy;
 };
 
+// The camera of pair `pair` in a per-pair table, read once into registers.  The kernels' CAMS instantiations take it; the
+// others read the launch's one camera from the constant bank, spelled at each kernel as before (a shared helper for both
+// changes how ptxas allocates K2's registers).
+__device__ __forceinline__ Cam table_cam(const PlCamera* cams, int pair) {
+    const PlCamera* c = cams + pair;
+    return Cam{__ldg(&c->fx), __ldg(&c->fy), __ldg(&c->cx), __ldg(&c->cy)};
+}
+
 __device__ __forceinline__ void transform(const double* DT, double x, double y, double z, double& X, double& Y, double& Z) {
     X = (DT[0] * x + DT[1] * y + DT[2] * z) + DT[3];   // DT.block(0,0,3,3) * P + DT.col(3).head(3)  (:567)
     Y = (DT[4] * x + DT[5] * y + DT[6] * z) + DT[7];
@@ -1643,7 +1651,8 @@ __device__ __forceinline__ void write_result(const SolveParams& prm, int pair, c
     }
 }
 
-__global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveParams prm) {
+template <bool CAMS>
+__global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveParams prm, const PlCamera* __restrict__ cams) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5;
     const int pair = prm.first_pair + blockIdx.x;
@@ -1664,7 +1673,7 @@ __global__ void __launch_bounds__(K2_THREADS, 1) track_solve_kernel(const SolveP
     f.inl_p = inl_p;
     f.inl_l = inl_l;
     const PlConfig& cfg = prm.cfg;
-    const Cam cam = {prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
+    const Cam cam = CAMS ? table_cam(cams, pair) : Cam{prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
 
     if (tid == 0)
         for (int i = 0; i < 8; i++) st.tc[i] = 0;
@@ -1934,7 +1943,9 @@ __device__ __forceinline__ StreamView stream_view(const SolveParams& prm, const 
 // 256-thread CTAs, up to three per SM: list building is a chain of short block-wide steps (see stream_outlier_kernel)
 constexpr int SPREP_THREADS = 256;
 __host__ __device__ inline size_t stream_prepare_smem(int sort_cap) { return align_up(sizeof(State), 16) + (size_t)sort_cap * sizeof(double); }
-__global__ void __launch_bounds__(SPREP_THREADS, 3) stream_prepare_kernel(const SolveParams prm, const StreamBufs sb) {
+template <bool CAMS>
+__global__ void __launch_bounds__(SPREP_THREADS, 3) stream_prepare_kernel(const SolveParams prm, const StreamBufs sb,
+                                                                                const PlCamera* __restrict__ cams) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, local = blockIdx.x;
     const int pair = prm.first_pair + local;
@@ -1950,7 +1961,8 @@ __global__ void __launch_bounds__(SPREP_THREADS, 3) stream_prepare_kernel(const 
         rs.on = true;
         rs.pt = sb.rec_pt + 2 * v.slot_p;
         rs.ls = sb.rec_ls + 4 * v.slot_l;
-        rs.cam = GsCamD{prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
+        const Cam c = CAMS ? table_cam(cams, pair) : Cam{prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
+        rs.cam = GsCamD{c.fx, c.fy, c.cx, c.cy};
         build_matched_lists(prm, pair, st, v.sortbuf, v.f, v.midx_p, v.midx_l, n1p, n1l, out_p0, out_l0, t_ph, rs);
     }
     __syncthreads();
@@ -2052,11 +2064,13 @@ __device__ __forceinline__ void fold_level(float* v, int lane) {
     }
 }
 
-template <bool PHASES>
+// CAMS: problem p is solved under cams[p] (the launch's pairs from its first), else under cam.
+template <bool PHASES, bool CAMS>
 __global__ void __launch_bounds__(GL_THREADS, GL_MINBLOCKS)
 gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __restrict__ pt_off, const int32_t* __restrict__ ls_off,
                       const StreamBufs sb, int n, int max_iters, int* __restrict__ queue, double* __restrict__ feat_scratch,
-                      size_t feat_stride, int cap_pt, int cap_ls, long long* __restrict__ phase) {
+                      size_t feat_stride, int cap_pt, int cap_ls, long long* __restrict__ phase,
+                      const PlCamera* __restrict__ cams) {
     extern __shared__ __align__(128) uint8_t ring[];
     __shared__ __align__(8) uint64_t full[GL_STAGES], empty[GL_STAGES];
     __shared__ double red[GL_CWARPS + 1][32], sH[36], sg[8], sDT[16], sDTprev[16], sC[36], s_exact[4];
@@ -2096,6 +2110,11 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
         if (!live) continue;
         StreamCtl& c = sb.ctl[p];
         const int np = sb.cnt_pt[p], nl = sb.cnt_ls[p], p0 = pt_off[p], l0 = ls_off[p];
+        if constexpr (CAMS) {   // every thread sets its own copy: no barrier needed before the consumers read it
+            const PlCamera& q = cams[p];
+            P.fx = (float)q.fx; P.fy = (float)q.fy; P.cx = (float)q.cx; P.cy = (float)q.cy;
+            P.fx_h = P.fx / P.h;
+        }
         const int ptiles = (np + GS_PT_TILE - 1) / GS_PT_TILE, n_tiles = ptiles + (nl + GS_LS_TILE - 1) / GS_LS_TILE;
         // a problem whose records fit the ring (KITTI-size: 4 point tiles + 2 line tiles) is loaded ONCE per GN call and
         // re-evaluated from shared memory; longer lists stream through the ring every iteration
@@ -2278,7 +2297,7 @@ gn_loop_stream_kernel(const PlCamera cam, const PlConfig cfg, const int32_t* __r
                 f.inl_l = sb.flag_ls + l0;
                 f.np = np;
                 f.nl = nl;
-                const Cam camd = {cam.fx, cam.fy, cam.cx, cam.cy};
+                const Cam camd = CAMS ? table_cam(cams, p) : Cam{cam.fx, cam.fy, cam.cx, cam.cy};
                 double v[4];
                 exact_error_partial(f, sDT, camd, v[0], v[1]);
                 exact_error_partial(f, sDTprev, camd, v[2], v[3]);   // (unused when it == 0: there is no previous pose yet)
@@ -2349,7 +2368,9 @@ constexpr int SO_THREADS = 256;
 __host__ __device__ inline size_t stream_outlier_smem(int sort_cap) {
     return align_up(sizeof(State), 16) + (size_t)sort_cap * sizeof(double) + sel_scratch_bytes();
 }
-__global__ void __launch_bounds__(SO_THREADS, 3) stream_outlier_kernel(const SolveParams prm, const StreamBufs sb) {
+template <bool CAMS>
+__global__ void __launch_bounds__(SO_THREADS, 3) stream_outlier_kernel(const SolveParams prm, const StreamBufs sb,
+                                                                         const PlCamera* __restrict__ cams) {
     extern __shared__ __align__(16) uint8_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, local = blockIdx.x;
     const int pair = prm.first_pair + local;
@@ -2361,7 +2382,7 @@ __global__ void __launch_bounds__(SO_THREADS, 3) stream_outlier_kernel(const Sol
     v.f.np = c.np;
     v.f.nl = c.nl;
     const PlConfig& cfg = prm.cfg;
-    const Cam cam = {prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
+    const Cam cam = CAMS ? table_cam(cams, pair) : Cam{prm.cam.fx, prm.cam.fy, prm.cam.cx, prm.cam.cy};
     // the lists live in HBM here: every residual is formed ONCE (same fp64 arithmetic as K2's), straight into shared memory
     if (warp == 0) {
         if (lane == 0) {
@@ -2467,32 +2488,35 @@ __global__ void __launch_bounds__(256) stream_finalize_kernel(const SolveParams 
 
 }  // namespace
 
-cudaError_t launch_stream_solve(const SolveParams& prm_in, int n_pairs, const StreamBufs& sb, cudaStream_t stream, int* launches,
-                                cudaEvent_t* marks) {
-    if (n_pairs <= 0) return cudaSuccess;
+namespace {
+
+template <bool CAMS>
+cudaError_t stream_solve(const SolveParams& prm_in, int n_pairs, const StreamBufs& sb, cudaStream_t stream, int* launches,
+                         cudaEvent_t* marks, const PlCamera* pair_cams) {
     SolveParams prm = prm_in;
     prm.feat_in_smem = 0;
     prm.only_if = nullptr;
     static size_t conf_a[64] = {}, conf_b[64] = {};
     const size_t smem_prep = stream_prepare_smem(prm.sort_cap);
-    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(stream_prepare_kernel), smem_prep, conf_a);
+    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(stream_prepare_kernel<CAMS>), smem_prep, conf_a);
     if (e != cudaSuccess) return e;
     const size_t smem_out = stream_outlier_smem(prm.sort_cap);
-    e = ensure_dynamic_smem(reinterpret_cast<const void*>(stream_outlier_kernel), smem_out, conf_b);
+    e = ensure_dynamic_smem(reinterpret_cast<const void*>(stream_outlier_kernel<CAMS>), smem_out, conf_b);
     if (e != cudaSuccess) return e;
     int nl = 0;
-    stream_prepare_kernel<<<n_pairs, SPREP_THREADS, smem_prep, stream>>>(prm, sb);
+    stream_prepare_kernel<CAMS><<<n_pairs, SPREP_THREADS, smem_prep, stream>>>(prm, sb, pair_cams);
     ++nl;
     // instrumentation (optional): lists built | GN stage 1 done | outlier pass done | GN stage 2 done
     if (marks) cudaEventRecord(marks[0], stream);
     const int32_t* off_p = prm.mode == 0 ? prm.prev.pt_off + prm.first_pair : prm.matched.pt_off + prm.first_pair;
     const int32_t* off_l = prm.mode == 0 ? prm.prev.ls_off + prm.first_pair : prm.matched.ls_off + prm.first_pair;
+    const PlCamera* cams = CAMS ? pair_cams + prm.first_pair : nullptr;   // the GN loop indexes its problems from 0
     static size_t conf_c[64] = {}, conf_d[64] = {};
     const size_t ring = (size_t)GL_STAGES * GS_STAGE_BYTES;
-    e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<false>), ring, conf_c);
+    e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<false, CAMS>), ring, conf_c);
     if (e != cudaSuccess) return e;
     if (prm.phase_cycles) {
-        e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<true>), ring, conf_d);
+        e = ensure_dynamic_smem(reinterpret_cast<const void*>(gn_loop_stream_kernel<true, CAMS>), ring, conf_d);
         if (e != cudaSuccess) return e;
     }
     int gn_calls = 0;
@@ -2503,13 +2527,15 @@ cudaError_t launch_stream_solve(const SolveParams& prm_in, int n_pairs, const St
         const int grid = n_pairs < GL_MINBLOCKS * sb.sm_count ? n_pairs : GL_MINBLOCKS * sb.sm_count;
         if (prm.phase_cycles) {
             long long* ph = prm.phase_cycles + (size_t)prm.first_pair * PLSTVO_PHASE_SLOTS + GLP_FIRST + gn_calls * GLP_N;
-            gn_loop_stream_kernel<true><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs, max_iters, q,
-                                                                            prm.feat_scratch, (size_t)prm.feat_scratch_stride,
-                                                                            prm.cap_pt, prm.cap_ls, ph);
+            gn_loop_stream_kernel<true, CAMS><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs,
+                                                                                  max_iters, q, prm.feat_scratch,
+                                                                                  (size_t)prm.feat_scratch_stride, prm.cap_pt,
+                                                                                  prm.cap_ls, ph, cams);
         } else {
-            gn_loop_stream_kernel<false><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs, max_iters, q,
-                                                                             prm.feat_scratch, (size_t)prm.feat_scratch_stride,
-                                                                             prm.cap_pt, prm.cap_ls, nullptr);
+            gn_loop_stream_kernel<false, CAMS><<<grid, GL_THREADS, ring, stream>>>(prm.cam, prm.cfg, off_p, off_l, sb, n_pairs,
+                                                                                   max_iters, q, prm.feat_scratch,
+                                                                                   (size_t)prm.feat_scratch_stride, prm.cap_pt,
+                                                                                   prm.cap_ls, nullptr, cams);
         }
         ++gn_calls;
         nl += 1;
@@ -2517,7 +2543,7 @@ cudaError_t launch_stream_solve(const SolveParams& prm_in, int n_pairs, const St
     };
     if ((e = gn(prm.cfg.max_iters)) != cudaSuccess) return e;
     if (marks) cudaEventRecord(marks[1], stream);
-    stream_outlier_kernel<<<n_pairs, SO_THREADS, smem_out, stream>>>(prm, sb);
+    stream_outlier_kernel<CAMS><<<n_pairs, SO_THREADS, smem_out, stream>>>(prm, sb, pair_cams);
     if (marks) cudaEventRecord(marks[2], stream);
     if ((e = gn(prm.cfg.max_iters_ref)) != cudaSuccess) return e;
     if (marks) cudaEventRecord(marks[3], stream);
@@ -2527,20 +2553,34 @@ cudaError_t launch_stream_solve(const SolveParams& prm_in, int n_pairs, const St
     // whatever left the common path: the whole problem again in K2 (global-scratch form)
     SolveParams k2 = prm;
     k2.only_if = sb.active;
-    e = launch_track_solve(k2, n_pairs, stream);
+    e = launch_track_solve(k2, n_pairs, stream, pair_cams);
     ++nl;
     if (launches) *launches = nl;
     return e != cudaSuccess ? e : cudaGetLastError();
 }
 
-cudaError_t launch_track_solve(const SolveParams& prm, int n_pairs, cudaStream_t stream) {
-    if (n_pairs <= 0) return cudaSuccess;
+template <bool CAMS>
+cudaError_t track_solve(const SolveParams& prm, int n_pairs, cudaStream_t stream, const PlCamera* cams) {
     const size_t smem = k2_smem_bytes(prm.cap_pt, prm.cap_ls, prm.sort_cap, prm.feat_in_smem != 0);
     static size_t configured[64] = {};
-    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(track_solve_kernel), smem, configured);
+    cudaError_t e = ensure_dynamic_smem(reinterpret_cast<const void*>(track_solve_kernel<CAMS>), smem, configured);
     if (e != cudaSuccess) return e;
-    track_solve_kernel<<<n_pairs, K2_THREADS, smem, stream>>>(prm);
+    track_solve_kernel<CAMS><<<n_pairs, K2_THREADS, smem, stream>>>(prm, cams);
     return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_stream_solve(const SolveParams& prm, int n_pairs, const StreamBufs& sb, cudaStream_t stream, int* launches,
+                                cudaEvent_t* marks, const PlCamera* cams) {
+    if (n_pairs <= 0) return cudaSuccess;
+    return cams ? stream_solve<true>(prm, n_pairs, sb, stream, launches, marks, cams)
+                : stream_solve<false>(prm, n_pairs, sb, stream, launches, marks, nullptr);
+}
+
+cudaError_t launch_track_solve(const SolveParams& prm, int n_pairs, cudaStream_t stream, const PlCamera* cams) {
+    if (n_pairs <= 0) return cudaSuccess;
+    return cams ? track_solve<true>(prm, n_pairs, stream, cams) : track_solve<false>(prm, n_pairs, stream, nullptr);
 }
 
 }  // namespace plstvo

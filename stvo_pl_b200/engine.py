@@ -70,6 +70,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_f2f_tracking": (C.c_int, [vp, cfg, fb, fb, i32p, i32p, i32p]),
         "plstvo_optimize_pose": (C.c_int, [vp, cam, cfg, mb, vp, vp, u8p, u8p]),
         "plstvo_track_batch": (C.c_int, [vp, cam, cfg, fb, fb, vp, vp, i32p, i32p, u8p, u8p]),
+        "plstvo_track_batch_cams": (C.c_int, [vp, cam, cfg, fb, fb, vp, vp, i32p, i32p, u8p, u8p]),
         "plstvo_track_batch_async": (C.c_int, [vp, cam, cfg, fb, fb, vp, vp, i32p, i32p, u8p, u8p]),
         "plstvo_wait": (C.c_int, [vp, C.c_int]),
         "plstvo_batch_upload": (C.c_int, [vp, cam, cfg, fb, fb, vp, C.POINTER(vp)]),
@@ -134,6 +135,9 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
                                                               i32p]),
         "plstvo_stereo_session_create": (vp, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig), C.POINTER(T.PlStereoConfig),
                                               C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlLsdConfig), vp, C.c_int]),
+        "plstvo_stereo_session_create_cams": (vp, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig),
+                                                   C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig),
+                                                   C.POINTER(T.PlLsdConfig), C.POINTER(vp), C.c_int]),
         "plstvo_stereo_session_destroy": (None, [vp]),
         "plstvo_stereo_session_device_bytes": (C.c_int64, [vp]),
         "plstvo_stereo_session_initialize": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), i32p]),
@@ -169,7 +173,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_rectifier_destroy", "plstvo_rectify_batch", "plstvo_rectify_kernel_times", "plstvo_track_stereo_raw_images_batch",
     "plstvo_track_stereo_raw_images_sequence", "plstvo_stereo_session_create", "plstvo_stereo_session_destroy",
     "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert",
-    "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read"]
+    "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read",
+    "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -918,6 +923,30 @@ class Engine:
         self._sessions.append(ss)
         return ss
 
+    def stereo_session_create_cams(self, cams, cfg, mcfg, scfg, ocfg, lcfg, rects, n_streams: int) -> StereoSession:
+        """A session whose stream i is tracked under cams[i] (n_streams PlCamera of one image size) and prepared by rects[i]
+        (rects None: no stream is remapped; in a grey session an entry None takes that stream's images as given; a colour
+        session needs a colour rectifier for every stream).  The rectifiers must outlive the session."""
+        cams = list(cams)
+        if len(cams) != n_streams:
+            raise ValueError("one camera per stream")
+        carr = (T.PlCamera * max(n_streams, 1))(*cams)
+        rarr = None
+        first = None
+        if rects is not None:
+            rects = list(rects)
+            if len(rects) != n_streams:
+                raise ValueError("one rectifier (or None) per stream")
+            rarr = (C.c_void_p * n_streams)(*[None if r is None else r.handle for r in rects])
+            first = next((r for r in rects if r is not None), None)
+        h = self.lib.plstvo_stereo_session_create_cams(self.ctx, carr, C.byref(cfg), C.byref(mcfg), C.byref(scfg),
+                                                       C.byref(ocfg), None if lcfg is None else C.byref(lcfg), rarr, n_streams)
+        if not h:
+            raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
+        ss = StereoSession(self, h, n_streams, first)
+        self._sessions.append(ss)
+        return ss
+
     def stereo_session_destroy(self, ss: StereoSession):
         ss.close()
         self._sessions = [x for x in self._sessions if x is not ss]
@@ -985,6 +1014,24 @@ class Engine:
         pc, cc = prev.as_c(), curr.as_c()
         self._ck(self.lib.plstvo_track_batch(
             self.ctx, C.byref(cam), C.byref(cfg), C.byref(pc), C.byref(cc),
+            priors.ctypes.data if priors is not None else None, out["results"].ctypes.data,
+            _p(out["m12_pt"], T.c_int32_p), _p(out["m12_ls"], T.c_int32_p), _p(out["inlier_pt"], T.c_uint8_p),
+            _p(out["inlier_ls"], T.c_uint8_p)))
+        return out
+
+    def track_batch_cams(self, cams, cfg, prev: T.FrameBatch, curr: T.FrameBatch, priors=None, out=None):
+        """track_batch with pair p solved under cams[p] (B PlCamera)."""
+        cams = list(cams)
+        if len(cams) != prev.B:
+            raise ValueError("one camera per pair")
+        carr = (T.PlCamera * max(prev.B, 1))(*cams)
+        if out is None:
+            out = dict(results=np.zeros(prev.B, dtype=T.POSE_RESULT_DTYPE),
+                       m12_pt=np.full(prev.n_pt, -1, np.int32), m12_ls=np.full(prev.n_ls, -1, np.int32),
+                       inlier_pt=np.zeros(prev.n_pt, np.uint8), inlier_ls=np.zeros(prev.n_ls, np.uint8))
+        pc, cc = prev.as_c(), curr.as_c()
+        self._ck(self.lib.plstvo_track_batch_cams(
+            self.ctx, carr, C.byref(cfg), C.byref(pc), C.byref(cc),
             priors.ctypes.data if priors is not None else None, out["results"].ctypes.data,
             _p(out["m12_pt"], T.c_int32_p), _p(out["m12_ls"], T.c_int32_p), _p(out["inlier_pt"], T.c_uint8_p),
             _p(out["inlier_ls"], T.c_uint8_p)))
