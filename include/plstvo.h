@@ -629,6 +629,57 @@ int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* s, int on);
  * retained, so a read never mixes two calls). */
 int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* s, const PlStereoFrameOut* out);
 
+/* ---- running the handler's frame loop over many frames per stream in one call (app/imagesStVO.cpp:88-124) ----
+ * The Config values of updateFrame's adaptive FAST threshold (include/config.h:50, :67-71; src/config.cpp:52, :72-76).
+ * fast_err_th is a float, as updateFrame reads it (src/stereoFrameHandler.cpp:72). */
+typedef struct PlHandlerConfig {
+    int32_t adaptative_fast;
+    int32_t fast_min_th, fast_max_th, fast_inc_th, fast_feat_th;
+    float   fast_err_th;
+} PlHandlerConfig;
+void plstvo_default_handler_config(PlHandlerConfig* h);   /* 1, 5, 50, 5, 50, 0.5f (src/config.cpp) */
+void plstvo_kitti_handler_config(PlHandlerConfig* h);     /* 1, 7, 30, 5, 50, 0.5f (config/config/config_kitti.yaml) */
+/* T steps of StereoFrameHandler's loop (insertStereoPair, optimizePose, updateFrame) for streams ids[0 .. n), each of which
+ * must hold a frame.  frames holds B = T * n frames, step-major: frame t * n + k is stream ids[k]'s frame of step t; its
+ * fast_th and key-line fields must be NULL.  Contract: the call equals, byte for byte, T calls of
+ * plstvo_stereo_session_insert on the same session, where the call of step t takes step t's n frames with
+ *   thresholds th_t:  th_0[k] = fast_th0[k] (fast_th0 NULL or an entry 0: ocfg->fast_threshold, as the images calls map it);
+ *                     th_{t+1}[k] = updateFastThreshold(h, th_t[k], curr_frame, results[t][k].n_inliers_pt) (plstvo.hpp);
+ *   priors:           priors at t = 0 (NULL as for insert), then priorOf of the frame publishPose(results[t - 1][k]) fills.
+ * Under it, results ([T][n]), n_stereo ([T][n][4], optional), the threshold rows (fast_th [T + 1][n], optional: row t = th_t,
+ * row T the threshold the next frame would take), the kept frames (a further insert gives the same bytes) and, with
+ * retention on, what plstvo_stereo_session_read returns (the last step, as if it had been an insert) are equal.  Streams not
+ * named are untouched.  T = 0 returns 0 and changes nothing; fast_th's row 0 (= row T) is still written.  A second run
+ * continues a first exactly when given fast_th0 = row T and priors built from the last results, so the caller splits a long
+ * sequence into calls of the T that fits.
+ * Schedule: all 2 n T images go up once and are rectified / converted once; LSD and LBD run once over all of them; then each
+ * step runs ORB at the device threshold row, the stereo step, tracking, and session_handler_kernel, which writes the next
+ * threshold row and the next priors on the device.  Per step, the host hops are an insert's: ORB's key-point counts and the
+ * stereo step's survivor counts.  The results, n_stereo rows and thresholds come down once, at the end.
+ * Device memory besides the session's pools: every image of the call is resident at once: LSD's 35 bytes or so per scaled
+ * pixel (as the _lsd_ calls), the grey copy's 1 byte per pixel, and with a rectifier its staging copy's channels bytes per
+ * pixel; LBD's outputs for all the call's key lines; and a table of T n results and 2 (T + 1) n thresholds.  The caller picks
+ * T to fit.  plstvo_track_stereo_images_stage_times then covers the whole call: [0] uploads and preparation, [1] ORB summed
+ * over the steps, [2] LSD + LBD, [3] the stereo step summed, [4] tracking and the threshold / prior update summed; the
+ * kernel-time calls report their last launches.
+ * Checks before any work, each leaving the session and context usable: PLSTVO_E_INVALID for h NULL; h out of range
+ * (fast_min_th < 1, fast_min_th > fast_max_th, fast_max_th > 255, fast_inc_th < 0, fast_feat_th < 0, a non-finite
+ * fast_err_th; the floor of 1 keeps a threshold of 0 from meaning the configured one); a non-NULL frames->fast_th or key-line
+ * field; a fast_th0 entry, or an ocfg->fast_threshold it maps to, outside [0, 255] (the rule sees what ORB uses); T < 0; more
+ * than 65535 images (2 n T); a session whose ocfg.n_features exceeds PLSTVO_MAX_FEATURES (so no step can fail on a feature
+ * limit); and insert's id, liveness and config checks.  PLSTVO_E_SIZE: frames->B != T * n, and insert's size codes.
+ * LSD's key-line limit (PLSTVO_E_TOO_LARGE) is found before step 0, since LSD runs first.
+ * Not checked before any work: the limits the T inserts would meet step by step (matchGrid's 128 candidates in one query
+ * window, the per-pair solver's list capacity, more than INT_MAX kept rows) and CUDA failures.  Such an error part-way
+ * returns its code with the named streams holding the frames of the last completed step, but results, fast_th and
+ * n_stereo are then unspecified and the number of completed steps is not returned, so the caller cannot continue exactly
+ * from there: it re-initialises those streams and continues with per-frame inserts or a new run.  For a CUDA failure this
+ * is not verified, since nothing provokes one safely. */
+int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* s, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
+                              const PlStereoImages* frames, const int32_t* fast_th0 /* [n] or NULL */,
+                              const PlPrior* priors /* [n] or NULL */, PlPoseResult* results /* [T][n] */,
+                              int32_t* fast_th /* [T + 1][n] or NULL */, int32_t* n_stereo /* [T][n][4] or NULL */);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

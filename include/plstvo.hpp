@@ -674,6 +674,10 @@ struct HandlerConfig {
     float fast_err_th = 0.5f;
     int orb_fast_th = 20;
     double min_entropy_ratio = 0.85, max_kf_t_dist = 5.0, max_kf_r_dist = 15.0;
+    // the adaptive threshold's values, as plstvo_stereo_session_run takes them
+    PlHandlerConfig device() const {
+        return PlHandlerConfig{adaptative_fast ? 1 : 0, fast_min_th, fast_max_th, fast_inc_th, fast_feat_th, fast_err_th};
+    }
 };
 
 // StereoFrameHandler::updateFrame's adaptive FAST threshold (src/stereoFrameHandler.cpp:66-86): the threshold the caller's
@@ -851,6 +855,12 @@ public:
     void insert(int n, const int32_t* ids, const PlStereoImages& frames, const PlPrior* priors, PlPoseResult* results,
                 int32_t* n_stereo = nullptr) {
         c_.check(plstvo_stereo_session_insert(c_.get(), s_, n, ids, &frames, priors, results, n_stereo));
+    }
+    // plstvo_stereo_session_run: T steps of insert + optimizePose + updateFrame for streams ids[0 .. n), frames B = T * n
+    // step-major; results [T][n], fast_th [T + 1][n] and n_stereo [T][n][4] optional
+    void run(const PlHandlerConfig& h, int n, const int32_t* ids, int T, const PlStereoImages& frames, const int32_t* fast_th0,
+             const PlPrior* priors, PlPoseResult* results, int32_t* fast_th = nullptr, int32_t* n_stereo = nullptr) {
+        c_.check(plstvo_stereo_session_run(c_.get(), s_, &h, n, ids, T, &frames, fast_th0, priors, results, fast_th, n_stereo));
     }
     // plstvo_stereo_session_retain: keep each following call's frames and matches for read() (off frees them)
     void retain(bool on) { c_.check(plstvo_stereo_session_retain(c_.get(), s_, on ? 1 : 0)); }
@@ -1171,6 +1181,72 @@ public:
             s.n_inliers_ls = s.result.n_matched_ls;
             s.n_inliers = s.n_inliers_pt + s.n_inliers_ls;
         }
+    }
+    // T frames per named stream in one session call (plstvo_stereo_session_run): img_l[t][k] / img_r[t][k] is stream ids[k]'s
+    // frame of step t.  Each stream then stands as after T rounds of insertStereoPairs, optimizePose and updateFrame: its
+    // prev_frame holds the last step's published pose, orb_fast_th the next frame's threshold, n_inliers* and n_stereo the
+    // last step's, and per-frame calls can follow.  results (optional) receives [T][n] results.  The key-frame test is not
+    // run (needNewKF reads each step's curr_frame); keepFeatures' arrays hold the last step.
+    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
+                               const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results = nullptr) {
+        const size_t n = ids.size(), T = img_l.size();
+        if (img_r.size() != T) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: T differs between sides");
+        std::vector<int32_t> th0;
+        std::vector<PlPrior> priors;
+        std::vector<const uint8_t*> l, r;
+        for (int32_t id : ids) {
+            const Stream& s = at(id);
+            if (!s.has_prev) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: initialize() the stream first");
+            th0.push_back(s.orb_fast_th);
+            priors.push_back(priorOf(s.prev_frame));
+        }
+        for (size_t t = 0; t < T; ++t) {
+            if (img_l[t].size() != n || img_r[t].size() != n)
+                throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: one image per stream and step");
+            l.insert(l.end(), img_l[t].begin(), img_l[t].end());
+            r.insert(r.end(), img_r[t].begin(), img_r[t].end());
+        }
+        if (T == 0 || n == 0) return;
+        pack_.pack(cam_.width, cam_.height, channels_, l, r, std::vector<int32_t>(n * T, 0),
+                   "StereoStreamsHandler::insertStereoSequences");
+        PlStereoImages frames = pack_.view;
+        frames.fast_th = nullptr;
+        std::vector<PlPoseResult> res(n * T);
+        std::vector<int32_t> th((T + 1) * n), ns(4 * n * T);
+        // th0 of 0 would mean the session's configured threshold, which the handler's ORB config sets to 0 as well
+        session_.run(hcfg_.device(), (int)n, ids.data(), (int)T, frames, th0.data(), priors.data(), res.data(), th.data(),
+                     ns.data());
+        if (keep_) session_.read((int)n, ns.data() + 4 * n * (T - 1), true, read_);
+        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
+        for (size_t k = 0; k < n; ++k) {
+            Stream& s = streams_[(size_t)ids[k]];
+            const PlPoseResult& last = res[(T - 1) * n + k];
+            s.result = last;
+            std::copy(ns.begin() + 4 * ((T - 1) * n + k), ns.begin() + 4 * ((T - 1) * n + k) + 4, s.n_stereo.begin());
+            s.prev_frame = StereoFrame{};
+            if (keep_) {
+                const size_t kp = (size_t)s.n_stereo[0], kl = (size_t)s.n_stereo[1], np = (size_t)s.n_stereo[2],
+                             nl = (size_t)s.n_stereo[3];
+                detail::frameFromRead(read_, p0, np, l0, nl, s.prev_frame);
+                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
+                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
+                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                p0 += np;
+                l0 += nl;
+                kp0 += kp;
+                kl0 += kl;
+            }
+            publishPose(last, s.prev_frame);   // optimizePose, then updateFrame moved curr_frame into prev_frame
+            s.curr_frame = StereoFrame{};
+            s.n_inliers_pt = last.n_inliers_pt;
+            s.n_inliers_ls = last.n_inliers_ls;
+            s.n_inliers = last.n_inliers;
+            s.orb_fast_th = th[T * n + k];
+        }
+        if (results) *results = std::move(res);
     }
     void optimizePose(int id) {                          // :307-392
         Stream& s = at(id);

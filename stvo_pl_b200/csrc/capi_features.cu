@@ -327,6 +327,18 @@ int orb_detect_check(PlContext* ctx, const PlOrbDetectConfig* cfg) {
     return 0;
 }
 
+// ORB's pyramid for images of width x height under a checked detect config: oc (scale_factor rounded to float, as ORB::create
+// takes it) and the levels' geometry and resize tables.  PLSTVO_E_INVALID where the pyramid cannot be built.
+int orb_detect_levels(PlContext* ctx, const PlOrbDetectConfig* cfg, int width, int height, PlOrbConfig& oc, OrbDevLevels& L,
+                      std::vector<int32_t>& tabs, std::vector<size_t>& tab_off) {
+    oc = cfg->orb;
+    oc.scale_factor = (double)(float)oc.scale_factor;   // ORB::create takes a float scale factor
+    if (oc.n_levels > 1 && !(oc.scale_factor > 1.0)) return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1 in float");
+    L = OrbDevLevels{};
+    if (!orb_levels(&oc, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    return 0;
+}
+
 // key points of an ORB detect call, left in HBM (CSR by image, arena_orb_kp) with the host copy of the offsets
 struct OrbDetected {
     std::vector<int32_t> off;   // [n_img + 1]; also written in full when the call fails with PLSTVO_E_TOO_LARGE
@@ -336,20 +348,19 @@ struct OrbDetected {
 };
 
 // Enqueues detection and description of n_img (> 0) images on s_main, for a checked config and per-image FAST thresholds th
-// (clamped here): either device images already written on s_main (d_img) or host images (parts, in order) that go up into
-// arena_orb.  `beside` (optional) is called with the device images and an event that completes once they are on the device,
+// (clamped here), or d_th: device thresholds in [0, 255] written on s_main, read as they are: either device images already
+// written on s_main (d_img) or host images (parts, in order) that go up into arena_orb.  `beside` (optional) is called with the device images and an event that completes once they are on the device,
 // after the pyramid and FAST launches are enqueued and before the first offsets readback blocks this thread: work enqueued
 // there on another stream overlaps those stages.
 int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, int width, int height, const uint8_t* d_img,
                        const std::vector<ImgPart>& parts, const int32_t* fast_th, int capacity,
-                       const std::function<int(const uint8_t*, cudaEvent_t)>& beside, OrbDetected& out) {
-    PlOrbConfig oc = cfg->orb;
-    oc.scale_factor = (double)(float)oc.scale_factor;   // ORB::create takes a float scale factor
-    if (oc.n_levels > 1 && !(oc.scale_factor > 1.0)) return fail(ctx, PLSTVO_E_INVALID, "scale_factor must be > 1 in float");
-    OrbDevLevels L{};
+                       const std::function<int(const uint8_t*, cudaEvent_t)>& beside, OrbDetected& out,
+                       const int32_t* d_th = nullptr) {
+    PlOrbConfig oc;
+    OrbDevLevels L;
     std::vector<int32_t> tabs;
     std::vector<size_t> tab_off;
-    if (!orb_levels(&oc, width, height, L, tabs, tab_off)) return fail(ctx, PLSTVO_E_INVALID, "a pyramid level has zero size");
+    if (const int rc = orb_detect_levels(ctx, cfg, width, height, oc, L, tabs, tab_off)) return rc;
     const int nl = L.n;
     const bool harris = cfg->score_type == 0;
     OrbDetectLevels D{};
@@ -376,8 +387,8 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
         D.harris_scale4 = hs * hs * hs * hs;
     }
     const int R = D.row0[nl];
-    std::vector<int32_t> th((size_t)n_img);
-    for (int i = 0; i < n_img; ++i) th[i] = std::min(std::max(fast_th[i], 0), 255);
+    std::vector<int32_t> th(d_th ? 0 : (size_t)n_img);
+    for (size_t i = 0; i < th.size(); ++i) th[i] = std::min(std::max(fast_th[i], 0), 255);
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, orb_init(ctx));
     const size_t img_bytes = (size_t)n_img * width * height, NL = (size_t)n_img * nl;
@@ -406,14 +417,14 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
         CK(ctx, cudaEventRecord(uploaded, s));
     }
     CK(ctx, a.up(o_tab, tabs.data(), tabs.size() * 4, s));
-    CK(ctx, a.up(o_th, th.data(), (size_t)n_img * 4, s));
+    CK(ctx, a.up(o_th, th.data(), th.size() * 4, s));
     const std::vector<const int32_t*> rs_tab = orb_resize_tabs(a.i32(o_tab), tab_off, nl);
     cudaEvent_t* ev = ctx->orb_det_ev.ev;   // [0] start, [1] pyramid + blur, [2] FAST + NMS, [3] selection, [4] angle + descriptor
     int launches = 0;
     CK(ctx, cudaEventRecord(ev[0], s));
     launch_orb_pyramid(L, n_img, img, a.u8(o_raw), a.u8(o_blur), rs_tab.data(), s, &launches);
     CK(ctx, cudaEventRecord(ev[1], s));
-    launch_orb_fast_select(L, D, n_img, img, a.u8(o_raw), a.i32(o_th), a.u8(o_score),
+    launch_orb_fast_select(L, D, n_img, img, a.u8(o_raw), d_th ? d_th : a.i32(o_th), a.u8(o_score),
                            a.at<uint32_t>(o_hist), a.i32(o_cut), a.i32(o_rcnt), a.i32(o_rbase), a.i32(o_icnt), a.i32(o_soff), s,
                            ev[2], &launches);
     CK(ctx, cudaGetLastError());
@@ -838,6 +849,107 @@ int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
 }
 
 /* ---- stereo images -> pose: ORB, LSD and LBD feed the stereo step and the tracker without leaving HBM ---- */
+namespace {
+// LSD's key lines of nblk blocks of nf images each, the arrays a LineSrc per block points at
+struct DetectedLines {
+    std::vector<std::vector<int32_t>> off, npix;
+    std::vector<std::vector<float>> seg, angle;
+};
+
+// LSD's host continuation on stream s (where its device half ran), then one LineSrc per block appended to lsrc, with the
+// images calls' key-line checks
+int lsd_line_sources(PlContext* ctx, const PlLsdConfig* lc, const LsdLaunch& lsd, cudaStream_t s, int nblk, int nf,
+                     DetectedLines& d, std::vector<LineSrc>& lsrc) {
+    std::vector<std::vector<KeyLine>> kls;
+    if (const int rc = lsd_finish(ctx, lc, lsd, s, kls)) return rc;
+    for (const std::vector<KeyLine>& k : kls)
+        if (k.size() > (size_t)PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+    d.off.assign((size_t)nblk, {});
+    d.npix.assign((size_t)nblk, {});
+    d.seg.assign((size_t)nblk, {});
+    d.angle.assign((size_t)nblk, {});
+    for (int b = 0; b < nblk; ++b) {
+        std::vector<int32_t>& off = d.off[(size_t)b];
+        off.assign(1, 0);
+        for (int i = 0; i < nf; ++i) off.push_back(off.back() + (int32_t)kls[(size_t)b * nf + i].size());
+        const size_t m = (size_t)off.back();
+        d.seg[(size_t)b].resize(4 * m);
+        d.angle[(size_t)b].resize(m);
+        d.npix[(size_t)b].resize(m);
+        lsd_rows(kls, b * nf, nf, d.seg[(size_t)b].data(), d.angle[(size_t)b].data(), d.npix[(size_t)b].data(), nullptr, nullptr);
+        lsrc.push_back(LineSrc{nf, off.data(), d.seg[(size_t)b].data(), d.angle[(size_t)b].data(), d.npix[(size_t)b].data()});
+    }
+    for (const LineSrc& l : lsrc)
+        if (const int rc = lbd_check_lines(ctx, l)) return rc;
+    return 0;
+}
+
+// One frame set of the stereo step (nf frames) on device inputs: the points of ORB's image blocks ob and ob + 1 (left,
+// right, nf images each) and the lines of line blocks lb and lb + 1 (LBD's rows from lbase[lb], lbase[lb + 1]), offsets
+// rebased to 0 into pl_off / pr_off.  lines: the frames have key lines (lsrc valid); run_lbd: LBD ran (d_seg, d_ldesc valid).
+void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const std::vector<LineSrc>& lsrc, int lb, bool lines,
+                       bool run_lbd, const std::vector<int32_t>& lbase, const float* d_seg, const uint8_t* d_ldesc, int nf,
+                       const std::vector<int32_t>& none, std::vector<int32_t>& pl_off, std::vector<int32_t>& pr_off,
+                       PlStereoFeatures& F, StereoDevInputs::Set& P, StereoDevInputs::Set& Ls) {
+    const size_t kl = orb.off[(size_t)ob * nf], kr = orb.off[(size_t)(ob + 1) * nf];
+    pl_off.resize((size_t)nf + 1);
+    pr_off.resize((size_t)nf + 1);
+    for (int i = 0; i <= nf; ++i) {
+        pl_off[i] = orb.off[(size_t)ob * nf + i] - (int32_t)kl;
+        pr_off[i] = orb.off[(size_t)(ob + 1) * nf + i] - (int32_t)kr;
+    }
+    F = PlStereoFeatures{};
+    F.B = nf;
+    F.pl_off = pl_off.data(); F.pr_off = pr_off.data();
+    F.ll_off = lines ? lsrc[(size_t)lb].off : none.data(); F.lr_off = lines ? lsrc[(size_t)lb + 1].off : none.data();
+    F.angle_l = lines ? lsrc[(size_t)lb].angle : nullptr;
+    P = StereoDevInputs::Set{};
+    P.on_device = true;
+    if (pts) {
+        P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
+        P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
+    }
+    Ls = StereoDevInputs::Set{};
+    Ls.on_device = true;   // oct stays null: key lines of octave 0
+    if (run_lbd) {
+        Ls.xy_l = d_seg + 4 * (size_t)lbase[(size_t)lb]; Ls.xy_r = d_seg + 4 * (size_t)lbase[(size_t)lb + 1];
+        Ls.d1 = d_ldesc + 32 * (size_t)lbase[(size_t)lb]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[(size_t)lb + 1];
+    }
+}
+
+bool key_lines_given(const PlStereoImages* f) {
+    return f->ll_off || f->lr_off || f->seg_l || f->seg_r || f->angle_l || f->angle_r || f->npix_l || f->npix_r;
+}
+
+// The image checks of an images call or a session run, before any work, on frame sets fs[0 .. nfs) holding n_img > 0 images
+// in all: every image of the camera's size and present where a stage runs, and with lines the size range and, given lc, LSD's
+// plan of all n_img images
+int images_check(PlContext* ctx, int W, int H, bool pts, bool lns, const PlStereoImages* const* fs, int nfs,
+                 const PlLsdConfig* lc, int n_img, LsdLaunch& lsd) {
+    for (int j = 0; j < nfs; ++j) {
+        // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
+        if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
+        if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
+    }
+    if (lns) {
+        if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
+        if (lc)
+            if (const int rc = lsd_plan(ctx, lc, n_img, W, H, lsd)) return rc;
+    }
+    return 0;
+}
+
+// Enqueues on s the grey device copy of n_img raw images (parts) in blocks of n images alternating left, right: the remap /
+// colour conversion of rect, or with a session of per-stream rectifiers, stream ids[k]'s rectifier for image k of each block
+int rectify_call(PlContext* ctx, const PlRectifier* rect, const PlStereoSession* session, const int32_t* ids, int n, int n_img,
+                 const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out) {
+    std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
+    if (session && !session->rects.empty())
+        for (int k = 0; k < n; ++k) call_rects.push_back(session->rects[(size_t)ids[k]]);
+    return rectify_enqueue(ctx, rect, n_img, n, parts, s, d_out, call_rects.empty() ? nullptr : call_rects.data());
+}
+}  // namespace
+
 // The images go up once, in blocks of NF images: sequence [left][right], batch [prev left][prev right][curr left][curr right].
 // Every feature set of the stereo step is then a contiguous slice of ORB's CSR output and of LBD's rows.  The key lines are
 // the caller's, or (detect_lines) LSD's, detected on the same device copy of the images: ORB's, or LSD's own when ORB does
@@ -862,11 +974,9 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0, run_lsd = detect_lines && lns;
     const int W = cam->width, H = cam->height;
     if (detect_lines) {
-        for (int j = 0; j < nfs; ++j) {
-            const PlStereoImages* f = fs[j];
-            if (f->ll_off || f->lr_off || f->seg_l || f->seg_r || f->angle_l || f->angle_r || f->npix_l || f->npix_r)
+        for (int j = 0; j < nfs; ++j)
+            if (key_lines_given(fs[j]))
                 return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the call detects its own key lines");
-        }
         if (run_lsd) {
             if (!lc) return fail(ctx, PLSTVO_E_INVALID, "null lsd config");
             if (const int rc = lsd_check_config(ctx, lc)) return rc;
@@ -877,23 +987,14 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     std::vector<LineSrc> lsrc;   // key lines per image block
     LsdLaunch lsd{};
     if (NF > 0) {
-        for (int j = 0; j < nfs; ++j) {
-            // the reference's grid scale is cols / img.cols (src/stereoFrame.cpp:47-48), the stereo step's cols / cam->width
-            if (fs[j]->width != W || fs[j]->height != H) return fail(ctx, PLSTVO_E_SIZE, "image size differs from the camera's");
-            if ((pts || lns) && (!fs[j]->img_l || !fs[j]->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images");
-        }
-        if (lns) {
-            if (W < 1 || W > 32767 || H < 1 || H > 32767) return fail(ctx, PLSTVO_E_INVALID, "width and height must be 1..32767");
-            if (run_lsd) {
-                if (const int rc = lsd_plan(ctx, lc, n_img, W, H, lsd)) return rc;
-            } else {
-                for (int j = 0; j < nfs; ++j) {
-                    lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
-                    lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
-                }
-                for (const LineSrc& l : lsrc)
-                    if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        if (const int rc = images_check(ctx, W, H, pts, lns, fs, nfs, run_lsd ? lc : nullptr, n_img, lsd)) return rc;
+        if (lns && !run_lsd) {
+            for (int j = 0; j < nfs; ++j) {
+                lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
+                lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
             }
+            for (const LineSrc& l : lsrc)
+                if (const int rc = lbd_check_lines(ctx, l)) return rc;
         }
     }
     if (NF == 0 || (sequence && NF == 1)) return 0;
@@ -929,27 +1030,10 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
         CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
         return 0;
     };
-    // LSD's key lines per image block, what lsrc points at: LSD's host continuation on stream s (where its device half ran),
-    // then the key-line checks of the images call
-    std::vector<int32_t> det_off[4], det_npix[4];
-    std::vector<float> det_seg[4], det_angle[4];
+    // LSD's key lines per image block, what lsrc points at
+    DetectedLines det;
     auto lsd_lines = [&](cudaStream_t s) -> int {
-        std::vector<std::vector<KeyLine>> kls;
-        if (const int rc = lsd_finish(ctx, lc, lsd, s, kls)) return rc;
-        for (const std::vector<KeyLine>& k : kls)
-            if (k.size() > (size_t)PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
-        for (int b = 0; b < nblk; ++b) {
-            det_off[b].assign(1, 0);
-            for (int i = 0; i < NF; ++i) det_off[b].push_back(det_off[b].back() + (int32_t)kls[(size_t)b * NF + i].size());
-            const size_t m = (size_t)det_off[b].back();
-            det_seg[b].resize(4 * m);
-            det_angle[b].resize(m);
-            det_npix[b].resize(m);
-            lsd_rows(kls, b * NF, NF, det_seg[b].data(), det_angle[b].data(), det_npix[b].data(), nullptr, nullptr);
-            lsrc.push_back(LineSrc{NF, det_off[b].data(), det_seg[b].data(), det_angle[b].data(), det_npix[b].data()});
-        }
-        for (const LineSrc& l : lsrc)
-            if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        if (const int rc = lsd_line_sources(ctx, lc, lsd, s, nblk, NF, det, lsrc)) return rc;
         count_lines();
         return 0;
     };
@@ -964,11 +1048,8 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const uint8_t* rectified = nullptr;
     cudaEvent_t rectified_ready = nullptr;
     if (rect && (pts || lns)) {
-        std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
-        if (session && !session->rects.empty())
-            for (int k = 0; k < NF; ++k) call_rects.push_back(session->rects[(size_t)session->ids[k]]);
-        if (const int rc = rectify_enqueue(ctx, rect, n_img, NF, iparts, ctx->s_main, &rectified,
-                                           call_rects.empty() ? nullptr : call_rects.data()))
+        if (const int rc = rectify_call(ctx, rect, session, session ? session->ids : nullptr, NF, n_img, iparts, ctx->s_main,
+                                        &rectified))
             return rc;
         rectified_ready = next_event(ctx);
         CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
@@ -1008,33 +1089,9 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
     PlStereoFeatures feat[2]{};
     StereoDevInputs dev;
-    for (int j = 0; j < nfs; ++j) {
-        const int bl = 2 * j, br = 2 * j + 1;
-        const size_t kl = orb.off[(size_t)bl * NF], kr = orb.off[(size_t)br * NF];
-        pl_off[j].resize((size_t)NF + 1);
-        pr_off[j].resize((size_t)NF + 1);
-        for (int i = 0; i <= NF; ++i) {
-            pl_off[j][i] = orb.off[(size_t)bl * NF + i] - (int32_t)kl;
-            pr_off[j][i] = orb.off[(size_t)br * NF + i] - (int32_t)kr;
-        }
-        PlStereoFeatures& F = feat[j];
-        F.B = NF;
-        F.pl_off = pl_off[j].data(); F.pr_off = pr_off[j].data();
-        F.ll_off = lns ? lsrc[bl].off : none.data(); F.lr_off = lns ? lsrc[br].off : none.data();
-        F.angle_l = lns ? lsrc[bl].angle : nullptr;
-        StereoDevInputs::Set& P = dev.set[2 * j];
-        P.on_device = true;
-        if (pts) {
-            P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
-            P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
-        }
-        StereoDevInputs::Set& Ls = dev.set[2 * j + 1];
-        Ls.on_device = true;   // oct stays null: key lines of octave 0
-        if (run_lbd) {
-            Ls.xy_l = d_seg + 4 * (size_t)lbase[bl]; Ls.xy_r = d_seg + 4 * (size_t)lbase[br];
-            Ls.d1 = d_ldesc + 32 * (size_t)lbase[bl]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[br];
-        }
-    }
+    for (int j = 0; j < nfs; ++j)
+        stereo_set_inputs(orb, 2 * j, pts, lsrc, 2 * j, lns, run_lbd, lbase, d_seg, d_ldesc, NF, none, pl_off[j], pr_off[j],
+                          feat[j], dev.set[2 * j], dev.set[2 * j + 1]);
     dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
     dev.marks = ctx->img_ev.ev + 1;
     if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], one_set ? nullptr : &feat[1], priors, results,
@@ -1252,6 +1309,39 @@ int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* ss, const 
 }
 
 namespace {
+// the named streams of a call: ids in range, no duplicates, and for an insert each holding a frame
+int session_check_ids(PlContext* ctx, const PlStereoSession* ss, bool track, int n, const int32_t* ids) {
+    std::vector<uint8_t> named((size_t)ss->n_streams, 0);
+    for (int k = 0; k < n; ++k) {
+        const int id = ids[k];
+        if (id < 0 || id >= ss->n_streams) return fail(ctx, PLSTVO_E_INVALID, "stream id outside [0, n_streams)");
+        if (named[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "duplicate stream id");
+        named[(size_t)id] = 1;
+        if (track && !ss->live[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "insert on a stream with no frame: initialize it first");
+    }
+    return 0;
+}
+
+// the call in progress on checked streams; for an insert, their kept frames compact in call order (the tracker's previous
+// frames) and their counts into n_stereo's columns 0, 1
+void session_begin(PlStereoSession* ss, bool track, int n, const int32_t* ids, int32_t* n_stereo) {
+    ss->track = track;
+    ss->n = n;
+    ss->ids = ids;
+    if (!track) return;
+    ss->kept_off_pt.assign((size_t)n + 1, 0);
+    ss->kept_off_ls.assign((size_t)n + 1, 0);
+    for (int k = 0; k < n; ++k) {
+        const size_t id = (size_t)ids[k];
+        ss->kept_off_pt[(size_t)k + 1] = ss->kept_off_pt[(size_t)k] + ss->n_pt[id];
+        ss->kept_off_ls[(size_t)k + 1] = ss->kept_off_ls[(size_t)k] + ss->n_ls[id];
+        if (n_stereo) {
+            n_stereo[4 * (size_t)k] = ss->n_pt[id];
+            n_stereo[4 * (size_t)k + 1] = ss->n_ls[id];
+        }
+    }
+}
+
 // initialize (track == false) or insert for streams ids[0 .. n): the checks, then the images path in session mode; the pools
 // flip and the streams' counts are kept only when the whole call succeeded
 int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const int32_t* ids, const PlStereoImages* frames,
@@ -1273,30 +1363,8 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     }
     if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
     if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
-    std::vector<uint8_t> named((size_t)ss->n_streams, 0);
-    for (int k = 0; k < n; ++k) {
-        const int id = ids[k];
-        if (id < 0 || id >= ss->n_streams) return fail(ctx, PLSTVO_E_INVALID, "stream id outside [0, n_streams)");
-        if (named[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "duplicate stream id");
-        named[(size_t)id] = 1;
-        if (track && !ss->live[(size_t)id]) return fail(ctx, PLSTVO_E_INVALID, "insert on a stream with no frame: initialize it first");
-    }
-    ss->track = track;
-    ss->n = n;
-    ss->ids = ids;
-    if (track) {   // the kept frames, compact in call order: the tracker's previous frames
-        ss->kept_off_pt.assign((size_t)n + 1, 0);
-        ss->kept_off_ls.assign((size_t)n + 1, 0);
-        for (int k = 0; k < n; ++k) {
-            const size_t id = (size_t)ids[k];
-            ss->kept_off_pt[(size_t)k + 1] = ss->kept_off_pt[(size_t)k] + ss->n_pt[id];
-            ss->kept_off_ls[(size_t)k + 1] = ss->kept_off_ls[(size_t)k] + ss->n_ls[id];
-            if (n_stereo) {
-                n_stereo[4 * (size_t)k] = ss->n_pt[id];
-                n_stereo[4 * (size_t)k + 1] = ss->n_ls[id];
-            }
-        }
-    }
+    if (const int rc = session_check_ids(ctx, ss, track, n, ids)) return rc;
+    session_begin(ss, track, n, ids, n_stereo);
     const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, true, ss->has_lc ? &ss->lc : nullptr,
                                        frames, nullptr, priors, results, n_stereo, false, ss->rect, ss);
     if (rc == 0) {
@@ -1320,6 +1388,235 @@ int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* ss, int n,
 int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* ss, int n, const int32_t* ids, const PlStereoImages* frames,
                                  const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
     return session_call(ctx, ss, true, n, ids, frames, priors, results, n_stereo);
+}
+
+/* ---- stereo sessions: the handler's frame loop over T frames per stream in one call ---- */
+void plstvo_default_handler_config(PlHandlerConfig* h) {
+    if (!h) return;
+    h->adaptative_fast = 1; h->fast_min_th = 5; h->fast_max_th = 50; h->fast_inc_th = 5; h->fast_feat_th = 50;
+    h->fast_err_th = 0.5f;
+}
+
+void plstvo_kitti_handler_config(PlHandlerConfig* h) {
+    if (!h) return;
+    plstvo_default_handler_config(h);
+    h->fast_min_th = 7; h->fast_max_th = 30;
+}
+
+namespace {
+// plstvo_stereo_session_run after the context lock: the checks, then the state-independent stages once over every image
+// (upload, rectifier, LSD, LBD) and the steps (ORB at the device threshold row, the stereo step, tracking, the handler
+// update), each committed to the session as an insert is.  The caller synchronises both streams afterwards.
+int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
+                const PlStereoImages* frames, const int32_t* fast_th0, const PlPrior* priors, PlPoseResult* results,
+                int32_t* fast_th, int32_t* n_stereo) {
+    if (!h) return fail(ctx, PLSTVO_E_INVALID, "null handler config");
+    if (h->fast_min_th < 1 || h->fast_min_th > h->fast_max_th || h->fast_max_th > 255 || h->fast_inc_th < 0 ||
+        h->fast_feat_th < 0 || !std::isfinite(h->fast_err_th))
+        return fail(ctx, PLSTVO_E_INVALID, "handler config out of range");
+    if (T < 0) return fail(ctx, PLSTVO_E_INVALID, "negative T");
+    if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
+    if ((long long)frames->B != (long long)T * n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from T * n");
+    if (frames->fast_th || key_lines_given(frames))
+        return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th and the key-line fields must be null: the run sets its thresholds and detects its key lines");
+    const PlOrbDetectConfig* oc = &ss->oc;
+    std::vector<int32_t> th0((size_t)2 * n);   // row 0 of the threshold table, [left n][right n]
+    for (int k = 0; k < n; ++k) {
+        if (fast_th0 && (fast_th0[k] < 0 || fast_th0[k] > 255)) return fail(ctx, PLSTVO_E_INVALID, "fast_th0 outside [0, 255]");
+        th0[(size_t)k] = th0[(size_t)n + k] = fast_th0 && fast_th0[k] ? fast_th0[k] : oc->fast_threshold;
+        if (th0[(size_t)k] < 0 || th0[(size_t)k] > 255)
+            return fail(ctx, PLSTVO_E_INVALID, "ocfg->fast_threshold outside [0, 255] where fast_th0 leaves it");
+    }
+    if (T == 0) {   // nothing runs; row T of the thresholds is row 0
+        if (fast_th) std::copy(th0.begin(), th0.begin() + n, fast_th);
+        return 0;
+    }
+    if (n > 0 && (!ids || !results)) return fail(ctx, PLSTVO_E_INVALID, "null ids or results");
+    if (2LL * n * T > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
+    if (const int rc = session_check_ids(ctx, ss, true, n, ids)) return rc;
+    if (oc->n_features > PLSTVO_MAX_FEATURES)
+        return fail(ctx, PLSTVO_E_INVALID, "ocfg.n_features exceeds PLSTVO_MAX_FEATURES: a step could fail on a feature limit");
+    const PlCamera& cam = ss->cam;
+    const bool pts = ss->cfg.has_points != 0, lns = ss->cfg.has_lines != 0;
+    const int W = cam.width, H = cam.height, n_img = 2 * n * T;
+    // the insert's checks (track_images_run) before any work: ORB's and LSD's plans, image sizes and pointers
+    if (const int rc = orb_detect_check(ctx, oc)) return rc;
+    if (pts && n > 0) {
+        PlOrbConfig orb_cfg;
+        OrbDevLevels levels;
+        std::vector<int32_t> tabs;
+        std::vector<size_t> tab_off;
+        if (const int rc = orb_detect_levels(ctx, oc, W, H, orb_cfg, levels, tabs, tab_off)) return rc;
+    }
+    LsdLaunch lsd{};
+    if (n > 0) {   // the session was created with an LSD config wherever it has lines
+        if (const int rc = images_check(ctx, W, H, pts, lns, &frames, 1, lns ? &ss->lc : nullptr, n_img, lsd)) return rc;
+    }
+    if (n == 0) {   // T empty inserts: they succeed and retain nothing
+        if (ss->retain) {
+            ss->kept.track = true;
+            ss->kept.n = 0;
+            ss->kept.valid = ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
+        }
+        return 0;
+    }
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, ctx->img_ev.create());
+    CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
+    ctx->img_timed = false;
+    Events<2> run_ev;      // the call's start, the end of its uploads and preparation
+    Events<3> marks[2];    // stereo step start, its end, tracking end, of even and odd steps
+    CK(ctx, run_ev.create());
+    CK(ctx, marks[0].create());
+    CK(ctx, marks[1].create());
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, cudaEventRecord(run_ev[0], s));
+    const size_t px = (size_t)W * H, step_px = 2 * (size_t)n * px;
+    const PlRectifier* rect = ss->rect;
+    const bool prepare = rect && (pts || lns);
+    // the threshold table [T + 1][2 n] (row t: step t's ORB thresholds, left and right), the results [T][n], and without a
+    // rectifier the grey images, step-major: step t's n left images, then its n right images
+    Arena a;
+    const size_t o_img = a.take(prepare || !(pts || lns) ? 0 : (size_t)n_img * px), o_th = a.take((size_t)(T + 1) * 2 * n * 4),
+                 o_res = a.take((size_t)T * n * sizeof(PlPoseResult));
+    CK(ctx, a.alloc(ctx->arena_run));
+    CK(ctx, a.up(o_th, th0.data(), th0.size() * 4, s));
+    const int32_t* d_th = a.i32(o_th);
+    const int ch = rect ? rect->channels : 1;
+    std::vector<ImgPart> iparts;
+    for (int t = 0; t < T; ++t) {
+        iparts.push_back(ImgPart{frames->img_l + (size_t)t * n * px * ch, n});
+        iparts.push_back(ImgPart{frames->img_r + (size_t)t * n * px * ch, n});
+    }
+    const uint8_t* d_img = nullptr;
+    if (prepare) {
+        if (const int rc = rectify_call(ctx, rect, ss, ids, n, n_img, iparts, s, &d_img)) return rc;
+    } else if (pts || lns) {
+        size_t o = o_img;
+        for (const ImgPart& ip : iparts) {
+            CK(ctx, a.up(o, ip.p, (size_t)ip.n * px, s));
+            o += (size_t)ip.n * px;
+        }
+        d_img = a.u8(o_img);
+    }
+    CK(ctx, cudaEventRecord(run_ev[1], s));
+    // the lines of every image: LSD alone on the main stream, then LBD on the second stream beside step 0's ORB; line
+    // blocks 2 t, 2 t + 1 are step t's left and right images
+    const int nblk = 2 * T;
+    std::vector<LineSrc> lsrc;
+    DetectedLines det;
+    std::vector<int32_t> lbase((size_t)nblk + 1, 0);
+    const float* d_seg = nullptr;
+    const uint8_t* d_ldesc = nullptr;
+    bool run_lbd = false;
+    if (lns) {
+        if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
+        if (const int rc = lsd_line_sources(ctx, &ss->lc, lsd, s, nblk, n, det, lsrc)) return rc;
+        for (int b = 0; b < nblk; ++b) lbase[(size_t)b + 1] = lbase[(size_t)b] + lsrc[(size_t)b].off[n];
+        run_lbd = lbase[(size_t)nblk] > 0;
+        if (run_lbd) {
+            cudaEvent_t ready = next_event(ctx);
+            CK(ctx, cudaEventRecord(ready, s));
+            if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, {}, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+            CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
+        }
+    }
+    float* ms = ctx->img_ms;
+    std::fill(ms, ms + 5, 0.f);
+    auto add_ms = [&](int k, cudaEvent_t from, cudaEvent_t to) -> int {
+        float v = 0;
+        CK(ctx, cudaEventElapsedTime(&v, from, to));
+        ms[k] += v;
+        return 0;
+    };
+    const bool keep = ss->retain;
+    std::vector<int32_t> none((size_t)n + 1, 0), pl_off, pr_off;
+    for (int t = 0; t < T; ++t) {
+        int32_t* ns = n_stereo ? n_stereo + (size_t)t * 4 * n : nullptr;
+        session_begin(ss, true, n, ids, ns);
+        OrbDetected orb;
+        if (pts) {
+            if (const int rc = orb_detect_enqueue(ctx, oc, 2 * n, W, H, d_img + (size_t)t * step_px, {}, nullptr, INT_MAX,
+                                                  nullptr, orb, d_th + (size_t)t * 2 * n))
+                return rc;
+        } else {
+            orb.off.assign((size_t)2 * n + 1, 0);
+        }
+        PlStereoFeatures feat;
+        StereoDevInputs dev;
+        stereo_set_inputs(orb, 0, pts, lsrc, 2 * t, lns, run_lbd, lbase, d_seg, d_ldesc, n, none, pl_off, pr_off, feat,
+                          dev.set[0], dev.set[1]);
+        dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
+        cudaEvent_t* mk = marks[t % 2].ev;
+        dev.marks = mk;
+        dev.priors_resident = t > 0;   // step t - 1's handler update wrote them
+        dev.tracked = [&](const Workspace& ws) -> int {
+            CK(ctx, launch_session_handler(*h, n, ws.d_results.as<PlPoseResult>(), d_th + (size_t)t * 2 * n,
+                                           a.i32(o_th) + (size_t)(t + 1) * 2 * n, ws.d_priors.as<PlPrior>(),
+                                           a.at<PlPoseResult>(o_res) + (size_t)t * n, s));
+            ctx->launches++;
+            CK(ctx, cudaEventRecord(mk[2], s));
+            // An insert ends synchronised; a step does not, and the next step's stereo step and tracker plan upload into the
+            // same arenas on s_h2d (offsets, line angles, problem tables) while this step's lifts and solver may still read
+            // them on s_main.  Every later upload on s_h2d waits for this step's end.
+            cudaEvent_t step_done = next_event(ctx);
+            CK(ctx, cudaEventRecord(step_done, s));
+            CK(ctx, cudaStreamWaitEvent(ctx->s_h2d, step_done, 0));
+            return 0;
+        };
+        ss->retain = keep && t == T - 1;   // the retention arena holds the last step
+        const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, &feat, nullptr, t == 0 ? priors : nullptr,
+                                           results + (size_t)t * n, ns, false, -1, &dev, ss);
+        ss->retain = keep;
+        if (rc) return rc;
+        session_commit(ss);
+        // the stereo step's count readback synchronised the main stream: this step's ORB and the last step are done
+        if (pts)
+            if (const int rc2 = add_ms(1, ctx->orb_det_ev[0], ctx->orb_det_ev[4])) return rc2;
+        if (t > 0) {
+            const cudaEvent_t* pm = marks[(t - 1) % 2].ev;
+            if (const int rc2 = add_ms(3, pm[0], pm[1])) return rc2;
+            if (const int rc2 = add_ms(4, pm[1], pm[2])) return rc2;
+        }
+    }
+    CK(ctx, a.down(results, o_res, (size_t)T * n * sizeof(PlPoseResult), s));
+    if (fast_th)
+        CK(ctx, cudaMemcpy2DAsync(fast_th, (size_t)n * 4, d_th, (size_t)2 * n * 4, (size_t)n * 4, (size_t)T + 1,
+                                  cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    CK(ctx, cudaStreamSynchronize(ctx->s_alt));
+    const cudaEvent_t* pm = marks[(T - 1) % 2].ev;
+    if (const int rc = add_ms(3, pm[0], pm[1])) return rc;
+    if (const int rc = add_ms(4, pm[1], pm[2])) return rc;
+    if (const int rc = add_ms(0, run_ev[0], run_ev[1])) return rc;
+    if (lns)
+        if (const int rc = add_ms(2, ctx->lsd_ev[0], run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5])) return rc;
+    ctx->img_timed = true;
+    if (keep) {
+        ss->kept.track = true;
+        ss->kept.n = n;
+        ss->kept.valid = true;
+    }
+    return 0;
+}
+}  // namespace
+
+int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
+                              const PlStereoImages* frames, const int32_t* fast_th0, const PlPrior* priors,
+                              PlPoseResult* results, int32_t* fast_th, int32_t* n_stereo) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo);
+    ss->ids = nullptr;   // the caller's array: not read after the call
+    if (rc) {
+        ss->kept.valid = false;   // a failed call discards what the last one retained
+        // the line stages may still run on the second stream, and a step on the first: the next call may reuse their arenas
+        cudaStreamSynchronize(ctx->s_alt);
+        cudaStreamSynchronize(ctx->s_main);
+    }
+    return rc;
 }
 
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {

@@ -530,9 +530,11 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     fc.pt_off = sequence ? ooff2[0].data() : session ? ooff[0].data() : ooff[2].data();
     fc.ls_off = sequence ? ooff2[1].data() : session ? ooff[1].data() : ooff[3].data();
     Workspace& ws = slot < 0 ? ctx->ws : ctx->ws_async[slot];
-    int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr, d_cams);
+    const bool resident = dev && dev->priors_resident;   // ws_prepare keeps d_priors: B is the run's n at every step
+    int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr || resident, d_cams);
     if (rc) return rc;
-    if (priors) CK(ctx, cudaMemcpyAsync(ws.d_priors.p, priors, (size_t)B * sizeof(PlPrior), cudaMemcpyHostToDevice, ctx->s_h2d));
+    if (priors && !resident)
+        CK(ctx, cudaMemcpyAsync(ws.d_priors.p, priors, (size_t)B * sizeof(PlPrior), cudaMemcpyHostToDevice, ctx->s_h2d));
     cudaEvent_t planned = next_event(ctx);
     CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(s, planned, 0));
@@ -580,6 +582,7 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             if (bytes) CK(ctx, cudaMemcpyAsync(kr.at<uint8_t>(r), src[k]->p, bytes, cudaMemcpyDeviceToDevice, s));
         }
     }
+    if (dev && dev->tracked) return dev->tracked(ws);
     CK(ctx, cudaMemcpyAsync(results, ws.d_results.p, (size_t)B * sizeof(PlPoseResult), cudaMemcpyDeviceToHost, s));
     if (slot < 0) CK(ctx, cudaStreamSynchronize(s));
     return 0;

@@ -5,6 +5,7 @@
 
 #include <algorithm>
 #include <cstdio>
+#include <functional>
 #include <initializer_list>
 #include <mutex>
 #include <string>
@@ -197,6 +198,7 @@ struct PlContext {
     // plstvo_track_stereo_images_*: [0] first upload, [1] stereo step start, [2] its end, [3] tracking end; the join of the LBD stream
     plstvo::Events<4> img_ev;
     plstvo::Events<1> img_join;
+    plstvo::DevBuf arena_run;      // plstvo_stereo_session_run: grey images (no rectifier), threshold and results tables
     float img_ms[5] = {0, 0, 0, 0, 0};
     bool img_timed = false;
     // pinned host scratch (small tables and counters that must not block the enqueueing thread), same indexing as the arenas
@@ -480,6 +482,11 @@ int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s);
 const int32_t* session_out_off(const PlStereoSession* ss, bool lines);
 // the call succeeded: pool[cur ^ 1] becomes the kept frames
 void session_commit(PlStereoSession* ss);
+// updateFrame's threshold and the next prior of one session-run step, on s for n streams: from the step's results (ws's
+// d_results), th [2 n] (row t of the run's threshold table) -> th + 2 n (row t + 1, both halves), priors [n] (ws's d_priors),
+// and the results copied to res_out [n]
+cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPoseResult* results, const int32_t* th,
+                                   int32_t* th_next, PlPrior* priors, PlPoseResult* res_out, cudaStream_t s);
 
 // ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
 // Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the
@@ -492,6 +499,9 @@ struct StereoDevInputs {
     } set[4];
     cudaEvent_t lines_ready = nullptr;   // waited on before the first line set's stereo step
     cudaEvent_t* marks = nullptr;        // [3] timing events: stereo step start, its end, tracking end (all on s_main)
+    bool priors_resident = false;        // the workspace's d_priors already holds this call's priors (a session run's steps)
+    // set: called on s_main once the solver is enqueued, in place of the results' download (results are then not written)
+    std::function<int(const Workspace&)> tracked;
 };
 int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                         const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,

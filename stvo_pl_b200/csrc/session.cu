@@ -48,6 +48,41 @@ GatherArrays gather_arrays(const PrevRows& s, const PrevRows& d) {
     return a;
 }
 
+// updateFrame of one stream after a session-run step (src/stereoFrameHandler.cpp:62-86, :317-326, :377-378), as
+// plstvo.hpp's updateFastThreshold, publishPose and priorOf compute it on the host: comparisons and integer arithmetic only.
+// th_next is written into both halves of the next row (ORB reads one threshold per image: [left n][right n]).
+__global__ void session_handler_kernel(PlHandlerConfig h, int n, const PlPoseResult* __restrict__ results,
+                                       const int32_t* __restrict__ th, int32_t* __restrict__ th_next,
+                                       PlPrior* __restrict__ priors, PlPoseResult* __restrict__ res_out) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const PlPoseResult& r = results[k];
+    const int t = th[k];
+    int next = t;
+    if (h.adaptative_fast) {
+        bool identity = true;   // Eigen's operator==: every coefficient compared exactly
+        for (int i = 0; i < 16; ++i) identity = identity && r.DT[i] == ((i % 5 == 0) ? 1.0 : 0.0);
+        const int inc = h.fast_inc_th, feat = h.fast_feat_th, n_in = r.n_inliers_pt;
+        if (identity || r.err_norm > (double)h.fast_err_th || n_in < feat) next = max(h.fast_min_th, t - 2 * inc);
+        else if (n_in < feat * 2) next = max(h.fast_min_th, t - inc);
+        else if (n_in > feat * 3) next = min(h.fast_max_th, t + inc);
+        // the reference's last branch (> 4 feat: + 2 inc, :84-85) is unreachable behind "> 3 feat"
+    }
+    th_next[k] = next;
+    th_next[n + k] = next;
+    PlPrior& p = priors[k];
+    for (int i = 0; i < 16; ++i) {
+        p.Tfw[i] = r.Tfw[i];
+        p.DT[i] = r.DT[i];
+    }
+    for (int i = 0; i < 36; ++i) {
+        p.Tfw_cov[i] = r.Tfw_cov[i];
+        p.DT_cov[i] = r.DT_cov[i];
+    }
+    p.err_norm = r.err_norm;
+    res_out[k] = r;
+}
+
 // offsets into PlStereoSession::meta
 size_t meta_named(const PlStereoSession* ss) { return 2 * (size_t)ss->n; }
 size_t meta_others(const PlStereoSession* ss) { return meta_named(ss) + (size_t)ss->n * (sizeof(GatherSeg) / 4); }
@@ -57,6 +92,13 @@ size_t meta_others(const PlStereoSession* ss) { return meta_named(ss) + (size_t)
 cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s) {
     if (n_segs <= 0) return cudaSuccess;
     session_gather_kernel<<<n_segs, GATHER_THREADS, 0, s>>>(gather_arrays(src, dst), segs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPoseResult* results, const int32_t* th,
+                                   int32_t* th_next, PlPrior* priors, PlPoseResult* res_out, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    session_handler_kernel<<<(n + 127) / 128, 128, 0, s>>>(h, n, results, th, th_next, priors, res_out);
     return cudaGetLastError();
 }
 

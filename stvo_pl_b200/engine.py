@@ -144,6 +144,10 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_stereo_session_insert": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), vp, vp, i32p]),
         "plstvo_stereo_session_retain": (C.c_int, [vp, vp, C.c_int]),
         "plstvo_stereo_session_read": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut)]),
+        "plstvo_default_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
+        "plstvo_kitti_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
+        "plstvo_stereo_session_run": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), C.c_int, i32p, C.c_int,
+                                                C.POINTER(T.PlStereoImages), i32p, vp, vp, i32p, i32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -174,7 +178,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_track_stereo_raw_images_sequence", "plstvo_stereo_session_create", "plstvo_stereo_session_destroy",
     "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert",
     "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read",
-    "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams"]
+    "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams", "plstvo_default_handler_config",
+    "plstvo_kitti_handler_config", "plstvo_stereo_session_run"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -242,6 +247,14 @@ class StereoSession:
         """insertStereoPair + optimizePose for streams ids against their kept frames, which the new frames then replace.
         Returns (results [n], n_stereo [n, 4])."""
         return self.eng.stereo_session_insert(self, ids, frames, priors, results)
+
+    def run(self, hcfg, ids, T_: int, frames: dict, fast_th0=None, priors=None):
+        """plstvo_stereo_session_run: T_ steps of the handler's loop (insert, optimizePose, updateFrame) for streams ids, the
+        FAST threshold and the prior carried from step to step on the device.  hcfg: a T.PlHandlerConfig or a
+        handler.HandlerConfig.  frames holds T_ * len(ids) frames, step-major (no fast_th); fast_th0 and priors (optional)
+        one entry per stream.  Returns (results [T_, n], fast_th [T_ + 1, n], n_stereo [T_, n, 4]); fast_th's last row is
+        the next frame's threshold (for T_ = 0, fast_th0 with 0 mapped to the configured threshold)."""
+        return self.eng.stereo_session_run(self, hcfg, ids, T_, frames, fast_th0, priors)
 
     def retain(self, on: bool):
         """plstvo_stereo_session_retain: from the next initialize / insert on, keep each call's new frames and matches on the
@@ -978,6 +991,34 @@ class Engine:
         del keep
         ss.last = (True, n_stereo.copy())
         return results, n_stereo
+
+    def handler_config(self, kitti: bool = False):
+        """plstvo_default_handler_config / plstvo_kitti_handler_config."""
+        h = T.PlHandlerConfig()
+        (self.lib.plstvo_kitti_handler_config if kitti else self.lib.plstvo_default_handler_config)(C.byref(h))
+        return h
+
+    def stereo_session_run(self, ss: StereoSession, hcfg, ids, T_: int, frames: dict, fast_th0=None, priors=None):
+        ss.check_frames(frames)
+        h = hcfg if isinstance(hcfg, T.PlHandlerConfig) else T.handler_config(hcfg)
+        ids = np.ascontiguousarray(ids, np.int32)
+        fs, keep = T.stereo_images_as_c(frames)
+        n = len(ids)
+        th0 = None if fast_th0 is None else np.ascontiguousarray(fast_th0, np.int32).reshape(-1)
+        pri = None if priors is None else np.ascontiguousarray(priors, T.PRIOR_DTYPE).reshape(-1)
+        if (th0 is not None and len(th0) != n) or (pri is not None and len(pri) != n):
+            raise ValueError("fast_th0 and priors take one entry per stream of ids")
+        results = np.zeros((T_, n), dtype=T.POSE_RESULT_DTYPE)
+        fast_th = np.zeros((T_ + 1, n), np.int32)
+        n_stereo = np.zeros((T_, n, 4), np.int32)
+        last, ss.last = ss.last, None
+        self._ck(self.lib.plstvo_stereo_session_run(self.ctx, ss.handle, C.byref(h), n, _p(ids, T.c_int32_p), T_, C.byref(fs),
+                                                    _p(th0, T.c_int32_p), None if pri is None else pri.ctypes.data,
+                                                    results.ctypes.data, _p(fast_th, T.c_int32_p), _p(n_stereo, T.c_int32_p)))
+        del keep
+        # read() returns the last step, as if it had been an insert; T_ = 0 changes nothing
+        ss.last = (True, n_stereo[-1].copy()) if T_ > 0 else last
+        return results, fast_th, n_stereo
 
     def track_stereo_images_stage_times(self):
         """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB; after the LSD form, the lines: LSD's first launch

@@ -235,6 +235,18 @@ POSE_RESULT_DTYPE = np.dtype([
     ("iters_stage2", "i4"), ("reserved", "i4")])
 assert POSE_RESULT_DTYPE.itemsize == C.sizeof(PlPoseResult)
 
+class PlHandlerConfig(C.Structure):
+    """updateFrame's adaptive FAST threshold (Config::adaptativeFAST, fastMinTh .. fastErrTh) of plstvo_stereo_session_run."""
+    _fields_ = [("adaptative_fast", C.c_int32), ("fast_min_th", C.c_int32), ("fast_max_th", C.c_int32),
+                ("fast_inc_th", C.c_int32), ("fast_feat_th", C.c_int32), ("fast_err_th", C.c_float)]
+
+
+def handler_config(h) -> "PlHandlerConfig":
+    """The PlHandlerConfig of a handler.HandlerConfig (or any object with its fields)."""
+    return PlHandlerConfig(int(bool(h.adaptative_fast)), h.fast_min_th, h.fast_max_th, h.fast_inc_th, h.fast_feat_th,
+                           float(h.fast_err_th))
+
+
 PRIOR_DTYPE = np.dtype([("Tfw", "f8", (4, 4)), ("Tfw_cov", "f8", (6, 6)), ("DT", "f8", (4, 4)),
                         ("DT_cov", "f8", (6, 6)), ("err_norm", "f8")])
 assert PRIOR_DTYPE.itemsize == C.sizeof(PlPrior)
