@@ -680,6 +680,63 @@ int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* s, const PlHandle
                               const PlPrior* priors /* [n] or NULL */, PlPoseResult* results /* [T][n] */,
                               int32_t* fast_th /* [T + 1][n] or NULL */, int32_t* n_stereo /* [T][n][4] or NULL */);
 
+/* ---- the same loop with the PL-SLAM key-frame test (needNewKF / currFrameIsKF, src/stereoFrameHandler.cpp:1136-1218) ----
+ * The Config values of needNewKF (include/config.h:39-41, :108-110; defaults src/config.cpp:40-42).  -inf / +inf switch a
+ * criterion off; NaN is refused. */
+typedef struct PlKeyframeConfig {
+    double min_entropy_ratio, max_kf_t_dist, max_kf_r_dist;
+} PlKeyframeConfig;
+void plstvo_default_keyframe_config(PlKeyframeConfig* k);   /* 0.85, 5.0, 15.0 */
+/* One stream's key-frame state, the handler's SLAM variables (include/stereoFrameHandler.h:81-86), as plstvo.hpp's
+ * KeyframeTest holds them.  T_prevKF and cov_prevKF_currF are row-major. */
+typedef struct PlKeyframeState {
+    int32_t prev_f_iskf, N_prevKF_currF;
+    double  entropy_first_prevKF;
+    double  T_prevKF[16];
+    double  cov_prevKF_currF[36];
+} PlKeyframeState;
+void plstvo_initial_keyframe_state(PlKeyframeState* s);     /* what initialize() leaves (:48-51): 1, 0, 0.0, I, 0 */
+/* One stream's needNewKF at one step: the decision, N_prevKF_currF as needNewKF leaves it (before currFrameIsKF resets it),
+ * and the test's entropy of the accumulated covariance, its ratio to the key frame's, and the distance t (m) and angle r
+ * (degrees) to the previous key frame. */
+typedef struct PlKeyframeResult {
+    int32_t new_kf, N_prevKF_currF;
+    double  entropy_curr, entropy_ratio, t, r;
+} PlKeyframeResult;
+/* plstvo_stereo_session_run with, per named stream and step, needNewKF after optimizePose and currFrameIsKF where it fires,
+ * before updateFrame.  Contract: the call equals T calls of plstvo_stereo_session_insert on the same session as the run's
+ * contract states them, except that the prior of step t + 1 is priorOf of the published frame with Tfw = I and Tfw_cov = I
+ * where kf[t][k].new_kf is 1, and that each step's results go through plstvo.hpp's KeyframeTest::needNewKF, starting from
+ * kf_state[k].  Under it results (optimizePose's rows, Tfw before any reset), n_stereo and fast_th are byte for byte the
+ * loop's; kf[t][k].new_kf and .N_prevKF_currF are the host test's; the four diagnostics agree with it to the last few ulps
+ * (the device's log and acos are CUDA's); and kf_state comes back as the host test stands after step T - 1.
+ * A second call continues a first exactly when given fast_th0 = row T, the returned kf_state, and priors built from the last
+ * results with that reset applied.
+ * The test runs in session_keyframe_kernel, one thread per stream after session_handler_kernel: one launch per step more
+ * than plstvo_stereo_session_run, in fp64 without fused multiply-adds.
+ * Retention (plstvo_stereo_session_retain on): the call keeps, for every (step, stream) whose frame became a key frame,
+ * that frame's new stereo points and lines, the same bytes as an insert of that frame retains; plstvo_stereo_session_read
+ * still returns the last step.  The device arena grows by each step's new rows of every named stream, 96 bytes per stereo
+ * point and 176 per stereo line, in one allocation per step with the session's usual slack (a quarter more, plus 256-byte
+ * alignment per array; counted by plstvo_stereo_session_device_bytes), and every step is retained as an insert
+ * is, so a retained call costs two lift launches, the tracker's row copies and one copy launch more per step.
+ * Checks before any work: those of plstvo_stereo_session_run, and PLSTVO_E_INVALID for k, kf_state or kf NULL, a NaN in k,
+ * and a kf_state entry with prev_f_iskf outside {0, 1} or N_prevKF_currF < 0.  A failed call leaves kf_state untouched and
+ * discards the key frames (as it discards what _read returns); so does any other call on the session. */
+int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* s, const PlHandlerConfig* h, const PlKeyframeConfig* k,
+                                        int n, const int32_t* ids, int T, const PlStereoImages* frames,
+                                        const int32_t* fast_th0 /* [n] or NULL */, const PlPrior* priors /* [n] or NULL */,
+                                        PlKeyframeState* kf_state /* [n] in / out */, PlPoseResult* results /* [T][n] */,
+                                        PlKeyframeResult* kf /* [T][n] */, int32_t* fast_th /* [T + 1][n] or NULL */,
+                                        int32_t* n_stereo /* [T][n][4] or NULL */);
+/* Copies the key frames the last plstvo_stereo_session_run_keyframes kept into out's non-NULL point and line arrays, in
+ * (step, call position) order, key frame j's rows after key frame j - 1's (m12_* / inlier_* are not read), and writes
+ * rows [n_kf][4]: step, stream id, stereo points, stereo lines (rows may be NULL to learn n_kf).  Returns n_kf.
+ * PLSTVO_E_INVALID: ctx, s or out null, a session of another context, retention off, or no key frames kept (the last call
+ * on the session was not a successful run_keyframes). */
+int plstvo_stereo_session_read_keyframes(PlContext* ctx, const PlStereoSession* s, const PlStereoFrameOut* out,
+                                         int32_t* rows /* [n_kf][4] or NULL */);
+
 /* ---- include/stereoFrameHandler.h surface ----------------------------------------------------- */
 /* StereoFrameHandler::f2fTracking (src/stereoFrameHandler.cpp:106-180) for B independent
  * (prev, curr) pairs: descriptor matching for points and lines; m12_* hold problem-local indices

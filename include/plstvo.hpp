@@ -678,6 +678,8 @@ struct HandlerConfig {
     PlHandlerConfig device() const {
         return PlHandlerConfig{adaptative_fast ? 1 : 0, fast_min_th, fast_max_th, fast_inc_th, fast_feat_th, fast_err_th};
     }
+    // the key-frame test's values, as plstvo_stereo_session_run_keyframes takes them
+    PlKeyframeConfig keyframes() const { return PlKeyframeConfig{min_entropy_ratio, max_kf_t_dist, max_kf_r_dist}; }
 };
 
 // StereoFrameHandler::updateFrame's adaptive FAST threshold (src/stereoFrameHandler.cpp:66-86): the threshold the caller's
@@ -723,6 +725,25 @@ struct KeyframeTest {
             return true;
         N_prevKF_currF++;
         return false;
+    }
+    // the state as plstvo_stereo_session_run_keyframes takes and returns it (the diagnostics are not part of it)
+    PlKeyframeState state() const {
+        PlKeyframeState s{};
+        s.prev_f_iskf = prev_f_iskf ? 1 : 0;
+        s.N_prevKF_currF = N_prevKF_currF;
+        s.entropy_first_prevKF = entropy_first_prevKF;
+        std::copy(T_prevKF.begin(), T_prevKF.end(), s.T_prevKF);
+        std::copy(cov_prevKF_currF.begin(), cov_prevKF_currF.end(), s.cov_prevKF_currF);
+        return s;
+    }
+    static KeyframeTest fromState(const PlKeyframeState& s) {
+        KeyframeTest k;
+        k.prev_f_iskf = s.prev_f_iskf != 0;
+        k.N_prevKF_currF = s.N_prevKF_currF;
+        k.entropy_first_prevKF = s.entropy_first_prevKF;
+        std::copy(s.T_prevKF, s.T_prevKF + 16, k.T_prevKF.begin());
+        std::copy(s.cov_prevKF_currF, s.cov_prevKF_currF + 36, k.cov_prevKF_currF.begin());
+        return k;
     }
     void currFrameIsKF(StereoFrame& curr_frame) {        // :1189-1218 (feature idx renumbering is the caller's: dense order already)
         curr_frame.Tfw = se3::identity4();
@@ -862,6 +883,14 @@ public:
              const PlPrior* priors, PlPoseResult* results, int32_t* fast_th = nullptr, int32_t* n_stereo = nullptr) {
         c_.check(plstvo_stereo_session_run(c_.get(), s_, &h, n, ids, T, &frames, fast_th0, priors, results, fast_th, n_stereo));
     }
+    // plstvo_stereo_session_run_keyframes: run() with needNewKF / currFrameIsKF per stream and step; kf_state [n] in / out,
+    // kf [T][n]
+    void runKeyframes(const PlHandlerConfig& h, const PlKeyframeConfig& k, int n, const int32_t* ids, int T,
+                      const PlStereoImages& frames, const int32_t* fast_th0, const PlPrior* priors, PlKeyframeState* kf_state,
+                      PlPoseResult* results, PlKeyframeResult* kf, int32_t* fast_th = nullptr, int32_t* n_stereo = nullptr) {
+        c_.check(plstvo_stereo_session_run_keyframes(c_.get(), s_, &h, &k, n, ids, T, &frames, fast_th0, priors, kf_state,
+                                                     results, kf, fast_th, n_stereo));
+    }
     // plstvo_stereo_session_retain: keep each following call's frames and matches for read() (off frees them)
     void retain(bool on) { c_.check(plstvo_stereo_session_retain(c_.get(), s_, on ? 1 : 0)); }
     // plstvo_stereo_session_read of the last call, into out's vectors sized from that call's n and n_stereo ([n][2] after an
@@ -877,6 +906,32 @@ public:
         std::vector<uint8_t> inlier_pt, inlier_ls;
     };
     void read(int n, const int32_t* n_stereo, bool insert, Frames& out) const {
+        const PlStereoFrameOut o = outputs(n, n_stereo, insert, out);
+        if (c_.check(plstvo_stereo_session_read(c_.get(), s_, &o)) != n)
+            throw Error(PLSTVO_E_INVALID, "StereoSession::read: n differs from the last call's");
+    }
+    // plstvo_stereo_session_run_keyframes' key frames (retention on) into out's point and line vectors; rows [n_kf][4]: step,
+    // stream id, points, lines.  out.m12_* / inlier_* are emptied.
+    void readKeyframes(Frames& out, std::vector<int32_t>& rows) const {
+        PlStereoFrameOut none{};
+        const int n_kf = c_.check(plstvo_stereo_session_read_keyframes(c_.get(), s_, &none, nullptr));
+        rows.assign(4 * (size_t)n_kf, 0);
+        c_.check(plstvo_stereo_session_read_keyframes(c_.get(), s_, &none, rows.data()));
+        std::vector<int32_t> ns(2 * (size_t)n_kf, 0);   // as an initialize's n_stereo: points, lines
+        for (int j = 0; j < n_kf; ++j) {
+            ns[2 * (size_t)j] = rows[4 * (size_t)j + 2];
+            ns[2 * (size_t)j + 1] = rows[4 * (size_t)j + 3];
+        }
+        const PlStereoFrameOut o = outputs(n_kf, ns.data(), false, out);
+        if (c_.check(plstvo_stereo_session_read_keyframes(c_.get(), s_, &o, nullptr)) != n_kf)
+            throw Error(PLSTVO_E_INVALID, "StereoSession::readKeyframes: the number of key frames changed");
+    }
+    int streams() const { return n_streams_; }
+    int64_t deviceBytes() const { return plstvo_stereo_session_device_bytes(s_); }
+    PlStereoSession* get() const { return s_; }
+private:
+    // out's vectors sized for n frames of n_stereo ([n][4] with insert, else [n][2]; the tracker's rows with insert only)
+    static PlStereoFrameOut outputs(int n, const int32_t* n_stereo, bool insert, Frames& out) {
         const int cols = insert ? 4 : 2;
         size_t np = 0, nl = 0, kp = 0, kl = 0;
         for (int k = 0; k < n; ++k) {
@@ -893,19 +948,13 @@ public:
         out.ls_sP.resize(3 * nl); out.ls_eP.resize(3 * nl); out.ls_le.resize(3 * nl); out.ls_angle.resize(nl);
         out.ls_sigma2.resize(nl); out.ls_level.resize(nl); out.ls_src.resize(nl); out.ldesc.resize(32 * nl);
         out.m12_pt.assign(kp, -1); out.m12_ls.assign(kl, -1); out.inlier_pt.assign(kp, 0); out.inlier_ls.assign(kl, 0);
-        const PlStereoFrameOut o{out.pt_pl.data(), out.pt_disp.data(), out.pt_P.data(), out.pt_sigma2.data(),
+        return PlStereoFrameOut{out.pt_pl.data(), out.pt_disp.data(), out.pt_P.data(), out.pt_sigma2.data(),
                                  out.pt_level.data(), out.pdesc.data(), out.pt_src.data(), out.ls_spl.data(), out.ls_epl.data(),
                                  out.ls_sdisp.data(), out.ls_edisp.data(), out.ls_sP.data(), out.ls_eP.data(), out.ls_le.data(),
                                  out.ls_angle.data(), out.ls_sigma2.data(), out.ls_level.data(), out.ldesc.data(),
                                  out.ls_src.data(), out.m12_pt.data(), out.inlier_pt.data(), out.m12_ls.data(),
                                  out.inlier_ls.data()};
-        if (c_.check(plstvo_stereo_session_read(c_.get(), s_, &o)) != n)
-            throw Error(PLSTVO_E_INVALID, "StereoSession::read: n differs from the last call's");
     }
-    int streams() const { return n_streams_; }
-    int64_t deviceBytes() const { return plstvo_stereo_session_device_bytes(s_); }
-    PlStereoSession* get() const { return s_; }
-private:
     Context& c_;
     PlStereoSession* s_ = nullptr;
     int n_streams_ = 0;
@@ -1186,67 +1235,28 @@ public:
     // frame of step t.  Each stream then stands as after T rounds of insertStereoPairs, optimizePose and updateFrame: its
     // prev_frame holds the last step's published pose, orb_fast_th the next frame's threshold, n_inliers* and n_stereo the
     // last step's, and per-frame calls can follow.  results (optional) receives [T][n] results.  The key-frame test is not
-    // run (needNewKF reads each step's curr_frame); keepFeatures' arrays hold the last step.
+    // run here: the overload below runs it inside the call.  keepFeatures' arrays hold the last step.
     void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
                                const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results = nullptr) {
-        const size_t n = ids.size(), T = img_l.size();
-        if (img_r.size() != T) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: T differs between sides");
-        std::vector<int32_t> th0;
-        std::vector<PlPrior> priors;
-        std::vector<const uint8_t*> l, r;
-        for (int32_t id : ids) {
-            const Stream& s = at(id);
-            if (!s.has_prev) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: initialize() the stream first");
-            th0.push_back(s.orb_fast_th);
-            priors.push_back(priorOf(s.prev_frame));
-        }
-        for (size_t t = 0; t < T; ++t) {
-            if (img_l[t].size() != n || img_r[t].size() != n)
-                throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: one image per stream and step");
-            l.insert(l.end(), img_l[t].begin(), img_l[t].end());
-            r.insert(r.end(), img_r[t].begin(), img_r[t].end());
-        }
-        if (T == 0 || n == 0) return;
-        pack_.pack(cam_.width, cam_.height, channels_, l, r, std::vector<int32_t>(n * T, 0),
-                   "StereoStreamsHandler::insertStereoSequences");
-        PlStereoImages frames = pack_.view;
-        frames.fast_th = nullptr;
-        std::vector<PlPoseResult> res(n * T);
-        std::vector<int32_t> th((T + 1) * n), ns(4 * n * T);
-        // th0 of 0 would mean the session's configured threshold, which the handler's ORB config sets to 0 as well
-        session_.run(hcfg_.device(), (int)n, ids.data(), (int)T, frames, th0.data(), priors.data(), res.data(), th.data(),
-                     ns.data());
-        if (keep_) session_.read((int)n, ns.data() + 4 * n * (T - 1), true, read_);
-        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
-        for (size_t k = 0; k < n; ++k) {
-            Stream& s = streams_[(size_t)ids[k]];
-            const PlPoseResult& last = res[(T - 1) * n + k];
-            s.result = last;
-            std::copy(ns.begin() + 4 * ((T - 1) * n + k), ns.begin() + 4 * ((T - 1) * n + k) + 4, s.n_stereo.begin());
-            s.prev_frame = StereoFrame{};
-            if (keep_) {
-                const size_t kp = (size_t)s.n_stereo[0], kl = (size_t)s.n_stereo[1], np = (size_t)s.n_stereo[2],
-                             nl = (size_t)s.n_stereo[3];
-                detail::frameFromRead(read_, p0, np, l0, nl, s.prev_frame);
-                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
-                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
-                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                p0 += np;
-                l0 += nl;
-                kp0 += kp;
-                kl0 += kl;
-            }
-            publishPose(last, s.prev_frame);   // optimizePose, then updateFrame moved curr_frame into prev_frame
-            s.curr_frame = StereoFrame{};
-            s.n_inliers_pt = last.n_inliers_pt;
-            s.n_inliers_ls = last.n_inliers_ls;
-            s.n_inliers = last.n_inliers;
-            s.orb_fast_th = th[T * n + k];
-        }
-        if (results) *results = std::move(res);
+        run(ids, img_l, img_r, results, nullptr, nullptr);
+    }
+    // A key frame of that overload: stream id, step, and with keepFeatures its new stereo points and lines (pose fields as
+    // published, Tfw before currFrameIsKF's reset)
+    struct KeyFrame {
+        int stream = 0, step = 0;
+        StereoFrame frame;
+    };
+    // The same with the PL-SLAM test (plstvo_stereo_session_run_keyframes): per stream and step, needNewKF after optimizePose
+    // and currFrameIsKF where it fires, from and back into each stream's kf.  A stream whose last step was a key frame has
+    // prev_frame.Tfw = I and Tfw_cov = I, as currFrameIsKF leaves curr_frame.  Returns the [T][n] tests; results (optional)
+    // receives [T][n] results, and keyframes (optional, with keepFeatures on) each key frame in (step, call position) order.
+    std::vector<PlKeyframeResult> insertStereoSequences(const std::vector<int32_t>& ids,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_l,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_r,
+                                                        std::vector<PlPoseResult>* results, std::vector<KeyFrame>* keyframes) {
+        std::vector<PlKeyframeResult> kf;
+        run(ids, img_l, img_r, results, &kf, keyframes);
+        return kf;
     }
     void optimizePose(int id) {                          // :307-392
         Stream& s = at(id);
@@ -1275,6 +1285,109 @@ public:
     const StereoSession& session() const { return session_; }
 
 private:
+    // the two insertStereoSequences: kf null runs plstvo_stereo_session_run, else plstvo_stereo_session_run_keyframes
+    void run(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
+             const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results,
+             std::vector<PlKeyframeResult>* kf, std::vector<KeyFrame>* keyframes) {
+        const size_t n = ids.size(), T = img_l.size();
+        if (img_r.size() != T) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: T differs between sides");
+        std::vector<int32_t> th0;
+        std::vector<PlPrior> priors;
+        std::vector<PlKeyframeState> state;
+        std::vector<const uint8_t*> l, r;
+        for (int32_t id : ids) {
+            const Stream& s = at(id);
+            if (!s.has_prev) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: initialize() the stream first");
+            th0.push_back(s.orb_fast_th);
+            priors.push_back(priorOf(s.prev_frame));
+            state.push_back(s.kf.state());
+        }
+        if (kf) kf->clear();
+        if (keyframes) keyframes->clear();
+        for (size_t t = 0; t < T; ++t) {
+            if (img_l[t].size() != n || img_r[t].size() != n)
+                throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: one image per stream and step");
+            l.insert(l.end(), img_l[t].begin(), img_l[t].end());
+            r.insert(r.end(), img_r[t].begin(), img_r[t].end());
+        }
+        if (T == 0 || n == 0) return;
+        pack_.pack(cam_.width, cam_.height, channels_, l, r, std::vector<int32_t>(n * T, 0),
+                   "StereoStreamsHandler::insertStereoSequences");
+        PlStereoImages frames = pack_.view;
+        frames.fast_th = nullptr;
+        std::vector<PlPoseResult> res(n * T);
+        std::vector<int32_t> th((T + 1) * n), ns(4 * n * T);
+        // th0 of 0 would mean the session's configured threshold, which the handler's ORB config sets to 0 as well
+        if (kf) {
+            kf->resize(n * T);
+            session_.runKeyframes(hcfg_.device(), hcfg_.keyframes(), (int)n, ids.data(), (int)T, frames, th0.data(),
+                                  priors.data(), state.data(), res.data(), kf->data(), th.data(), ns.data());
+            if (keyframes && keep_) {
+                std::vector<int32_t> rows;
+                session_.readKeyframes(read_, rows);
+                size_t p0 = 0, l0 = 0;
+                for (size_t j = 0; j < rows.size() / 4; ++j) {
+                    KeyFrame f;
+                    f.step = rows[4 * j];
+                    f.stream = rows[4 * j + 1];
+                    const size_t np = (size_t)rows[4 * j + 2], nl = (size_t)rows[4 * j + 3];
+                    detail::frameFromRead(read_, p0, np, l0, nl, f.frame);
+                    p0 += np;
+                    l0 += nl;
+                    size_t k = 0;
+                    while (ids[k] != f.stream) ++k;
+                    publishPose(res[(size_t)f.step * n + k], f.frame);
+                    keyframes->push_back(std::move(f));
+                }
+            }
+        } else {
+            session_.run(hcfg_.device(), (int)n, ids.data(), (int)T, frames, th0.data(), priors.data(), res.data(), th.data(),
+                         ns.data());
+        }
+        if (keep_) session_.read((int)n, ns.data() + 4 * n * (T - 1), true, read_);
+        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
+        for (size_t k = 0; k < n; ++k) {
+            Stream& s = streams_[(size_t)ids[k]];
+            const PlPoseResult& last = res[(T - 1) * n + k];
+            s.result = last;
+            std::copy(ns.begin() + 4 * ((T - 1) * n + k), ns.begin() + 4 * ((T - 1) * n + k) + 4, s.n_stereo.begin());
+            s.prev_frame = StereoFrame{};
+            if (keep_) {
+                const size_t kp = (size_t)s.n_stereo[0], kl = (size_t)s.n_stereo[1], np = (size_t)s.n_stereo[2],
+                             nl = (size_t)s.n_stereo[3];
+                detail::frameFromRead(read_, p0, np, l0, nl, s.prev_frame);
+                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
+                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
+                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
+                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
+                p0 += np;
+                l0 += nl;
+                kp0 += kp;
+                kl0 += kl;
+            }
+            publishPose(last, s.prev_frame);   // optimizePose, then updateFrame moved curr_frame into prev_frame
+            if (kf) {
+                s.kf = KeyframeTest::fromState(state[k]);
+                const PlKeyframeResult& kl = (*kf)[(T - 1) * n + k];
+                s.kf.entropy_curr = kl.entropy_curr;
+                s.kf.entropy_ratio = kl.entropy_ratio;
+                s.kf.kf_t = kl.t;
+                s.kf.kf_r = kl.r;
+                if (kl.new_kf) {   // currFrameIsKF on the frame that became prev_frame
+                    s.prev_frame.Tfw = se3::identity4();
+                    for (int i = 0; i < 36; ++i) s.prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+                }
+            }
+            s.curr_frame = StereoFrame{};
+            s.n_inliers_pt = last.n_inliers_pt;
+            s.n_inliers_ls = last.n_inliers_ls;
+            s.n_inliers = last.n_inliers;
+            s.orb_fast_th = th[T * n + k];
+        }
+        if (results) *results = std::move(res);
+    }
     Stream& at(int id) {
         if (id < 0 || id >= (int)streams_.size()) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: stream id out of range");
         return streams_[(size_t)id];

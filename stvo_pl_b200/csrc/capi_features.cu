@@ -1259,6 +1259,7 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
         ss->d_meta.release();
         ss->kept.buf.release();
         ss->d_cams.release();
+        ss->kf_steps.clear();
     }
     delete ss;
 }
@@ -1266,8 +1267,21 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
 int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
     if (!ss) return 0;
     LOCK(ss->ctx);
-    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap + ss->d_cams.cap);
+    size_t kf = 0;
+    for (const auto& c : ss->kf_steps) kf += c->buf.cap;
+    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap + ss->d_cams.cap + kf);
 }
+
+namespace {
+// every call on a session but the reads discards the key frames a run_keyframes kept (the chunks' frees wait for the device)
+void session_drop_keyframes(PlStereoSession* ss) {
+    ss->kf_valid = false;
+    if (!ss->kf_steps.empty()) cudaSetDevice(ss->ctx->device);
+    ss->kf_steps.clear();
+    ss->kf_rows.clear();
+    ss->kf_off.clear();
+}
+}  // namespace
 
 int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
     if (!ctx) return PLSTVO_E_INVALID;
@@ -1276,6 +1290,7 @@ int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
     if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
     if (on && ss->retain) return 0;   // already on: what the last call retained stays readable
     ss->retain = on != 0;
+    session_drop_keyframes(ss);
     ss->kept.valid = false;
     if (!on) {
         CK(ctx, cudaSetDevice(ctx->device));
@@ -1351,6 +1366,7 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
     if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
     ss->kept.valid = false;   // a failed call discards what the last one retained
+    session_drop_keyframes(ss);
     if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
     if (frames->B != n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from n");
     if (n == 0) {
@@ -1406,10 +1422,13 @@ void plstvo_kitti_handler_config(PlHandlerConfig* h) {
 namespace {
 // plstvo_stereo_session_run after the context lock: the checks, then the state-independent stages once over every image
 // (upload, rectifier, LSD, LBD) and the steps (ORB at the device threshold row, the stereo step, tracking, the handler
-// update), each committed to the session as an insert is.  The caller synchronises both streams afterwards.
+// update), each committed to the session as an insert is.  The caller synchronises both streams afterwards.  With kc
+// (plstvo_stereo_session_run_keyframes) each step also runs the key-frame test from kf_state's streams and, with retention
+// on, keeps every step's records and copies the key frames' into the session's chunks; kf_state is written on success only.
 int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
                 const PlStereoImages* frames, const int32_t* fast_th0, const PlPrior* priors, PlPoseResult* results,
-                int32_t* fast_th, int32_t* n_stereo) {
+                int32_t* fast_th, int32_t* n_stereo, const PlKeyframeConfig* kc = nullptr, PlKeyframeState* kf_state = nullptr,
+                PlKeyframeResult* kf = nullptr) {
     if (!h) return fail(ctx, PLSTVO_E_INVALID, "null handler config");
     if (h->fast_min_th < 1 || h->fast_min_th > h->fast_max_th || h->fast_max_th > 255 || h->fast_inc_th < 0 ||
         h->fast_feat_th < 0 || !std::isfinite(h->fast_err_th))
@@ -1479,8 +1498,20 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     Arena a;
     const size_t o_img = a.take(prepare || !(pts || lns) ? 0 : (size_t)n_img * px), o_th = a.take((size_t)(T + 1) * 2 * n * 4),
                  o_res = a.take((size_t)T * n * sizeof(PlPoseResult));
+    const bool keep = ss->retain;
+    // the key-frame test: the streams' states [n], the decisions [T][n], and with retention each step's call-order offsets
+    // of the new rows [T][2][n + 1]
+    size_t o_kfs = 0, o_kfr = 0, o_kfoff = 0;
+    if (kc) {
+        o_kfs = a.take((size_t)n * sizeof(PlKeyframeState));
+        o_kfr = a.take((size_t)T * n * sizeof(PlKeyframeResult));
+        o_kfoff = a.take(keep ? (size_t)T * 2 * (n + 1) * 4 : 0);
+    }
     CK(ctx, a.alloc(ctx->arena_run));
     CK(ctx, a.up(o_th, th0.data(), th0.size() * 4, s));
+    if (kc) CK(ctx, a.up(o_kfs, kf_state, (size_t)n * sizeof(PlKeyframeState), s));
+    const double k_entropy = 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0)));   // KeyframeTest::needNewKF's constant
+    std::vector<int32_t> kf_off(kc && keep ? (size_t)T * 2 * (n + 1) : 0, 0);   // [T][2][n + 1], as uploaded
     const int32_t* d_th = a.i32(o_th);
     const int ch = rect ? rect->channels : 1;
     std::vector<ImgPart> iparts;
@@ -1529,7 +1560,6 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         ms[k] += v;
         return 0;
     };
-    const bool keep = ss->retain;
     std::vector<int32_t> none((size_t)n + 1, 0), pl_off, pr_off;
     for (int t = 0; t < T; ++t) {
         int32_t* ns = n_stereo ? n_stereo + (size_t)t * 4 * n : nullptr;
@@ -1555,6 +1585,32 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
                                            a.i32(o_th) + (size_t)(t + 1) * 2 * n, ws.d_priors.as<PlPrior>(),
                                            a.at<PlPoseResult>(o_res) + (size_t)t * n, s));
             ctx->launches++;
+            if (kc) {
+                PlKeyframeResult* d_kf = a.at<PlKeyframeResult>(o_kfr) + (size_t)t * n;
+                CK(ctx, launch_session_keyframe(*kc, k_entropy, n, ws.d_results.as<PlPoseResult>(), a.at<PlKeyframeState>(o_kfs),
+                                                d_kf, ws.d_priors.as<PlPrior>(), s));
+                ctx->launches++;
+                if (keep) {   // the key frames' rows, from this step's retention arena into its own chunk
+                    int32_t* off = kf_off.data() + (size_t)t * 2 * (n + 1);
+                    for (int k = 0; k < n; ++k) {
+                        off[k + 1] = off[k] + ss->new_pt[(size_t)k];
+                        off[n + 2 + k] = off[n + 1 + k] + ss->new_ls[(size_t)k];
+                    }
+                    const size_t o = o_kfoff + (size_t)t * 2 * (n + 1) * 4;
+                    CK(ctx, a.up(o, off, (size_t)2 * (n + 1) * 4, s));
+                    ss->kf_steps.push_back(std::unique_ptr<SessionRetained>(new SessionRetained()));
+                    SessionRetained& c = *ss->kf_steps.back();
+                    CK(ctx, c.lay_out((size_t)off[n], (size_t)off[2 * n + 1], 0, 0));
+                    KeyframeCopyArrays ca;
+                    for (int j = 0; j < KeyframeCopyArrays::N; ++j) {
+                        ca.src[j] = ss->kept.at<uint32_t>(j);
+                        ca.dst[j] = c.at<uint32_t>(j);
+                        ca.words[j] = SessionRetained::row_bytes[j] / 4;
+                    }
+                    CK(ctx, launch_session_keyframe_copy(ca, a.i32(o), d_kf, n, s));
+                    ctx->launches++;
+                }
+            }
             CK(ctx, cudaEventRecord(mk[2], s));
             // An insert ends synchronised; a step does not, and the next step's stereo step and tracker plan upload into the
             // same arenas on s_h2d (offsets, line angles, problem tables) while this step's lifts and solver may still read
@@ -1564,7 +1620,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
             CK(ctx, cudaStreamWaitEvent(ctx->s_h2d, step_done, 0));
             return 0;
         };
-        ss->retain = keep && t == T - 1;   // the retention arena holds the last step
+        ss->retain = keep && (kc || t == T - 1);   // the retention arena holds the last step (every step for the key frames)
         const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, &feat, nullptr, t == 0 ? priors : nullptr,
                                            results + (size_t)t * n, ns, false, -1, &dev, ss);
         ss->retain = keep;
@@ -1580,6 +1636,11 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         }
     }
     CK(ctx, a.down(results, o_res, (size_t)T * n * sizeof(PlPoseResult), s));
+    std::vector<PlKeyframeState> kfs_out(kc ? (size_t)n : 0);
+    if (kc) {
+        CK(ctx, a.down(kf, o_kfr, (size_t)T * n * sizeof(PlKeyframeResult), s));
+        CK(ctx, a.down(kfs_out.data(), o_kfs, (size_t)n * sizeof(PlKeyframeState), s));
+    }
     if (fast_th)
         CK(ctx, cudaMemcpy2DAsync(fast_th, (size_t)n * 4, d_th, (size_t)2 * n * 4, (size_t)n * 4, (size_t)T + 1,
                                   cudaMemcpyDeviceToHost, s));
@@ -1597,6 +1658,16 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         ss->kept.n = n;
         ss->kept.valid = true;
     }
+    if (kc) {
+        std::copy(kfs_out.begin(), kfs_out.end(), kf_state);
+        for (int t = 0; keep && t < T; ++t)
+            for (int k = 0; k < n; ++k) {
+                if (!kf[(size_t)t * n + k].new_kf) continue;
+                const int32_t* off = kf_off.data() + (size_t)t * 2 * (n + 1);
+                ss->kf_rows.insert(ss->kf_rows.end(), {t, ids[k], off[k + 1] - off[k], off[n + 2 + k] - off[n + 1 + k]});
+                ss->kf_off.insert(ss->kf_off.end(), {off[k], off[n + 1 + k]});
+            }
+    }
     return 0;
 }
 }  // namespace
@@ -1608,6 +1679,7 @@ int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* ss, const PlHandl
     LOCK(ctx);
     if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
     if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    session_drop_keyframes(ss);
     const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo);
     ss->ids = nullptr;   // the caller's array: not read after the call
     if (rc) {
@@ -1617,6 +1689,83 @@ int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* ss, const PlHandl
         cudaStreamSynchronize(ctx->s_main);
     }
     return rc;
+}
+
+/* ---- the same loop with the key-frame test ---- */
+void plstvo_default_keyframe_config(PlKeyframeConfig* k) {
+    if (!k) return;
+    k->min_entropy_ratio = 0.85; k->max_kf_t_dist = 5.0; k->max_kf_r_dist = 15.0;
+}
+
+void plstvo_initial_keyframe_state(PlKeyframeState* s) {
+    if (!s) return;
+    memset(s, 0, sizeof *s);
+    s->prev_f_iskf = 1;
+    for (int i = 0; i < 4; ++i) s->T_prevKF[5 * i] = 1.0;
+}
+
+int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, const PlKeyframeConfig* k,
+                                        int n, const int32_t* ids, int T, const PlStereoImages* frames, const int32_t* fast_th0,
+                                        const PlPrior* priors, PlKeyframeState* kf_state, PlPoseResult* results,
+                                        PlKeyframeResult* kf, int32_t* fast_th, int32_t* n_stereo) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    ss->kept.valid = false;   // what the last call retained, and its key frames, are discarded by this one
+    session_drop_keyframes(ss);
+    if (!k || !kf_state || !kf) return fail(ctx, PLSTVO_E_INVALID, "null key-frame config, state or results");
+    if (std::isnan(k->min_entropy_ratio) || std::isnan(k->max_kf_t_dist) || std::isnan(k->max_kf_r_dist))
+        return fail(ctx, PLSTVO_E_INVALID, "NaN in the key-frame config");
+    for (int i = 0; i < n; ++i)
+        if ((kf_state[i].prev_f_iskf != 0 && kf_state[i].prev_f_iskf != 1) || kf_state[i].N_prevKF_currF < 0)
+            return fail(ctx, PLSTVO_E_INVALID, "key-frame state with prev_f_iskf outside {0, 1} or a negative N_prevKF_currF");
+    const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo, k, kf_state, kf);
+    ss->ids = nullptr;   // the caller's array: not read after the call
+    if (rc) {
+        ss->kept.valid = false;
+        session_drop_keyframes(ss);
+        cudaStreamSynchronize(ctx->s_alt);
+        cudaStreamSynchronize(ctx->s_main);
+        return rc;
+    }
+    ss->kf_valid = ss->retain;
+    return 0;
+}
+
+int plstvo_stereo_session_read_keyframes(PlContext* ctx, const PlStereoSession* ss, const PlStereoFrameOut* out, int32_t* rows) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss || !out) return fail(ctx, PLSTVO_E_INVALID, "null session or output");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (!ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
+    if (!ss->kf_valid) return fail(ctx, PLSTVO_E_INVALID, "no key frames kept: the last call on the session was not a successful run_keyframes");
+    CK(ctx, cudaSetDevice(ctx->device));
+    using R = SessionRetained;
+    uint8_t* dst[R::M12_PT] = {(uint8_t*)out->pt_pl, (uint8_t*)out->pt_disp, (uint8_t*)out->pt_P, (uint8_t*)out->pt_sigma2,
+                               (uint8_t*)out->pt_level, out->pdesc, (uint8_t*)out->pt_src, (uint8_t*)out->ls_spl,
+                               (uint8_t*)out->ls_epl, (uint8_t*)out->ls_sdisp, (uint8_t*)out->ls_edisp, (uint8_t*)out->ls_sP,
+                               (uint8_t*)out->ls_eP, (uint8_t*)out->ls_le, (uint8_t*)out->ls_angle, (uint8_t*)out->ls_sigma2,
+                               (uint8_t*)out->ls_level, out->ldesc, (uint8_t*)out->ls_src};
+    const int n_kf = (int)(ss->kf_rows.size() / 4);
+    cudaStream_t s = ctx->s_main;
+    size_t at_pt = 0, at_ls = 0;   // rows copied so far
+    for (int j = 0; j < n_kf; ++j) {
+        const int32_t* r = ss->kf_rows.data() + 4 * (size_t)j;
+        const R& c = *ss->kf_steps[(size_t)r[0]];
+        for (int a = 0; a < R::M12_PT; ++a) {
+            const bool pt = a < R::LS_SPL;
+            const size_t w = (size_t)R::row_bytes[a], rows_j = (size_t)(pt ? r[2] : r[3]);
+            const size_t from = (size_t)ss->kf_off[2 * (size_t)j + (pt ? 0 : 1)], to = pt ? at_pt : at_ls;
+            if (dst[a] && rows_j)
+                CK(ctx, cudaMemcpyAsync(dst[a] + to * w, c.at<uint8_t>(a) + from * w, rows_j * w, cudaMemcpyDeviceToHost, s));
+        }
+        at_pt += (size_t)r[2];
+        at_ls += (size_t)r[3];
+    }
+    CK(ctx, cudaStreamSynchronize(s));
+    if (rows) std::copy(ss->kf_rows.begin(), ss->kf_rows.end(), rows);
+    return n_kf;
 }
 
 int plstvo_track_stereo_images_stage_times(PlContext* ctx, float ms5[5]) {

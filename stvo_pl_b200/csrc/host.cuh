@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <functional>
 #include <initializer_list>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -466,6 +467,11 @@ struct PlStereoSession {
     // ---- plstvo_stereo_session_retain / _read ----
     bool retain = false;
     plstvo::SessionRetained kept;                    // the last call's records while retain is on
+    // ---- plstvo_stereo_session_run_keyframes / _read_keyframes: per step, every named stream's new rows (the key frames'
+    // filled), and the key frames' rows [n_kf][4] (step, stream id, points, lines) with their chunk offsets [n_kf][2] ----
+    std::vector<std::unique_ptr<plstvo::SessionRetained>> kf_steps;
+    std::vector<int32_t> kf_rows, kf_off;
+    bool kf_valid = false;
 };
 
 namespace plstvo {
@@ -487,6 +493,21 @@ void session_commit(PlStereoSession* ss);
 // and the results copied to res_out [n]
 cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPoseResult* results, const int32_t* th,
                                    int32_t* th_next, PlPrior* priors, PlPoseResult* res_out, cudaStream_t s);
+// keyframe.cu: needNewKF / currFrameIsKF of one session-run step on s for n streams: from the step's results (ws's
+// d_results) and state [n] (updated in place) -> out [n]; where it fires, priors [n] (ws's d_priors, after the handler
+// update) take Tfw = I, Tfw_cov = I.  k_entropy = 3 (1 + log 2 pi), as the host computes it.
+cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
+                                    PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s);
+// The point and line arrays of SessionRetained (the first LS_SPL are points), as 4-byte words
+struct KeyframeCopyArrays {
+    enum { N = 19, N_PT = 7 };
+    const uint32_t* src[N];
+    uint32_t* dst[N];
+    int words[N];
+};
+// the rows of the streams kf[k].new_kf marks, for n streams at call-order offsets off ([n + 1] points, [n + 1] lines)
+cudaError_t launch_session_keyframe_copy(const KeyframeCopyArrays& a, const int32_t* off, const PlKeyframeResult* kf, int n,
+                                         cudaStream_t s);
 
 // ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
 // Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the

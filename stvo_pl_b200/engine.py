@@ -148,6 +148,11 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_kitti_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
         "plstvo_stereo_session_run": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), C.c_int, i32p, C.c_int,
                                                 C.POINTER(T.PlStereoImages), i32p, vp, vp, i32p, i32p]),
+        "plstvo_default_keyframe_config": (None, [vp]),
+        "plstvo_initial_keyframe_state": (None, [vp]),
+        "plstvo_stereo_session_run_keyframes": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), vp, C.c_int, i32p, C.c_int,
+                                                          C.POINTER(T.PlStereoImages), i32p, vp, vp, vp, vp, i32p, i32p]),
+        "plstvo_stereo_session_read_keyframes": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut), i32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -179,7 +184,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_stereo_session_device_bytes", "plstvo_stereo_session_initialize", "plstvo_stereo_session_insert",
     "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read",
     "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams", "plstvo_default_handler_config",
-    "plstvo_kitti_handler_config", "plstvo_stereo_session_run"]
+    "plstvo_kitti_handler_config", "plstvo_stereo_session_run", "plstvo_default_keyframe_config",
+    "plstvo_initial_keyframe_state", "plstvo_stereo_session_run_keyframes", "plstvo_stereo_session_read_keyframes"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -255,6 +261,36 @@ class StereoSession:
         one entry per stream.  Returns (results [T_, n], fast_th [T_ + 1, n], n_stereo [T_, n, 4]); fast_th's last row is
         the next frame's threshold (for T_ = 0, fast_th0 with 0 mapped to the configured threshold)."""
         return self.eng.stereo_session_run(self, hcfg, ids, T_, frames, fast_th0, priors)
+
+    def run_keyframes(self, hcfg, kcfg, ids, T_: int, frames: dict, kf_state, fast_th0=None, priors=None):
+        """plstvo_stereo_session_run_keyframes: run() with the key-frame test (needNewKF, then currFrameIsKF where it fires)
+        after each step's optimizePose.  kcfg: a T.KEYFRAME_CONFIG_DTYPE record or a handler.HandlerConfig; kf_state: one
+        T.KEYFRAME_STATE_DTYPE record per stream (handler.KeyframeTest.to_state()), updated in place on success.  Returns
+        (results [T_, n], kf [T_, n] of T.KEYFRAME_RESULT_DTYPE, fast_th [T_ + 1, n], n_stereo [T_, n, 4])."""
+        return self.eng.stereo_session_run_keyframes(self, hcfg, kcfg, ids, T_, frames, kf_state, fast_th0, priors)
+
+    def read_keyframes(self):
+        """plstvo_stereo_session_read_keyframes: (rows [n_kf, 4] of step, stream id, points, lines; pt; ls), pt / ls holding
+        the key frames' records in (step, call position) order under the keys of read()'s."""
+        lib, ctx = self.eng.lib, self.eng.ctx
+        empty = T.PlStereoFrameOut()
+        n_kf = self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(empty), None))
+        rows = np.zeros((n_kf, 4), np.int32)
+        self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(empty), _p(rows, T.c_int32_p)))
+        pt = self.eng.stereo_outputs(int(rows[:, 2].sum()), n_kf, lines=False)
+        ls = self.eng.stereo_outputs(int(rows[:, 3].sum()), n_kf, lines=True)
+        for d, col in ((pt, 2), (ls, 3)):
+            del d["m12"]
+            d["counts"][...] = rows[:, col]
+        o = T.PlStereoFrameOut()
+        for f, key in T.FRAME_OUT_POINT_KEYS.items():
+            setattr(o, f, pt[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
+        for f, key in T.FRAME_OUT_LINE_KEYS.items():
+            setattr(o, f, ls[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
+        got = self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(o), None))
+        if got != n_kf:
+            raise PlstvoError(-1, f"plstvo_stereo_session_read_keyframes returned {got} key frames, then {n_kf}")
+        return rows, pt, ls
 
     def retain(self, on: bool):
         """plstvo_stereo_session_retain: from the next initialize / insert on, keep each call's new frames and matches on the
@@ -1019,6 +1055,47 @@ class Engine:
         # read() returns the last step, as if it had been an insert; T_ = 0 changes nothing
         ss.last = (True, n_stereo[-1].copy()) if T_ > 0 else last
         return results, fast_th, n_stereo
+
+    def keyframe_config(self):
+        """plstvo_default_keyframe_config: one T.KEYFRAME_CONFIG_DTYPE record."""
+        k = np.zeros(1, T.KEYFRAME_CONFIG_DTYPE)
+        self.lib.plstvo_default_keyframe_config(k.ctypes.data)
+        return k
+
+    def initial_keyframe_state(self, n: int = 1):
+        """plstvo_initial_keyframe_state for n streams: T.KEYFRAME_STATE_DTYPE [n]."""
+        s = np.zeros(n, T.KEYFRAME_STATE_DTYPE)
+        for i in range(n):
+            self.lib.plstvo_initial_keyframe_state(s[i:].ctypes.data)
+        return s
+
+    def stereo_session_run_keyframes(self, ss: StereoSession, hcfg, kcfg, ids, T_: int, frames: dict, kf_state, fast_th0=None,
+                                     priors=None):
+        ss.check_frames(frames)
+        h = hcfg if isinstance(hcfg, T.PlHandlerConfig) else T.handler_config(hcfg)
+        k = (np.ascontiguousarray(kcfg, T.KEYFRAME_CONFIG_DTYPE).reshape(-1) if isinstance(kcfg, np.ndarray)
+             else T.keyframe_config(kcfg))
+        ids = np.ascontiguousarray(ids, np.int32)
+        fs, keep = T.stereo_images_as_c(frames)
+        n = len(ids)
+        th0 = None if fast_th0 is None else np.ascontiguousarray(fast_th0, np.int32).reshape(-1)
+        pri = None if priors is None else np.ascontiguousarray(priors, T.PRIOR_DTYPE).reshape(-1)
+        if not (isinstance(kf_state, np.ndarray) and kf_state.dtype == T.KEYFRAME_STATE_DTYPE and kf_state.flags.c_contiguous):
+            raise ValueError("kf_state: a contiguous T.KEYFRAME_STATE_DTYPE array, updated in place")
+        if (th0 is not None and len(th0) != n) or (pri is not None and len(pri) != n) or kf_state.size != n:
+            raise ValueError("fast_th0, priors and kf_state take one entry per stream of ids")
+        results = np.zeros((T_, n), dtype=T.POSE_RESULT_DTYPE)
+        kf = np.zeros((T_, n), dtype=T.KEYFRAME_RESULT_DTYPE)
+        fast_th = np.zeros((T_ + 1, n), np.int32)
+        n_stereo = np.zeros((T_, n, 4), np.int32)
+        last, ss.last = ss.last, None
+        self._ck(self.lib.plstvo_stereo_session_run_keyframes(
+            self.ctx, ss.handle, C.byref(h), k.ctypes.data, n, _p(ids, T.c_int32_p), T_, C.byref(fs), _p(th0, T.c_int32_p),
+            None if pri is None else pri.ctypes.data, kf_state.ctypes.data, results.ctypes.data, kf.ctypes.data,
+            _p(fast_th, T.c_int32_p), _p(n_stereo, T.c_int32_p)))
+        del keep
+        ss.last = (True, n_stereo[-1].copy()) if T_ > 0 else last
+        return results, kf, fast_th, n_stereo
 
     def track_stereo_images_stage_times(self):
         """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB; after the LSD form, the lines: LSD's first launch

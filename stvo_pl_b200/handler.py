@@ -131,6 +131,23 @@ class KeyframeTest:
         self.N_prevKF_currF += 1
         return False
 
+    def to_state(self) -> np.ndarray:
+        """This test's state as one PlKeyframeState record (T.KEYFRAME_STATE_DTYPE), for StereoSession.run_keyframes."""
+        s = np.zeros(1, T.KEYFRAME_STATE_DTYPE)
+        s["prev_f_iskf"], s["N_prevKF_currF"] = int(bool(self.prev_f_iskf)), self.N_prevKF_currF
+        s["entropy_first_prevKF"], s["T_prevKF"][0], s["cov_prevKF_currF"][0] = self.entropy_first_prevKF, self.T_prevKF, self.cov_prevKF_currF
+        return s
+
+    @classmethod
+    def from_state(cls, s) -> "KeyframeTest":
+        """The test standing in PlKeyframeState s (a T.KEYFRAME_STATE_DTYPE record); the diagnostics start at 0."""
+        s = np.asarray(s, T.KEYFRAME_STATE_DTYPE).reshape(-1)[0]
+        k = cls()
+        k.prev_f_iskf, k.N_prevKF_currF = bool(s["prev_f_iskf"]), int(s["N_prevKF_currF"])
+        k.entropy_first_prevKF = float(s["entropy_first_prevKF"])
+        k.T_prevKF, k.cov_prevKF_currF = np.array(s["T_prevKF"], float), np.array(s["cov_prevKF_currF"], float)
+        return k
+
     def currFrameIsKF(self, frame):
         frame.Tfw, frame.Tfw_cov = np.eye(4), np.eye(6)
         self.T_prevKF, self.cov_prevKF_currF = np.eye(4), np.zeros((6, 6))

@@ -251,6 +251,18 @@ PRIOR_DTYPE = np.dtype([("Tfw", "f8", (4, 4)), ("Tfw_cov", "f8", (6, 6)), ("DT",
                         ("DT_cov", "f8", (6, 6)), ("err_norm", "f8")])
 assert PRIOR_DTYPE.itemsize == C.sizeof(PlPrior)
 
+# plstvo_stereo_session_run_keyframes: needNewKF's thresholds, one stream's key-frame state, one stream's test at one step
+KEYFRAME_CONFIG_DTYPE = np.dtype([("min_entropy_ratio", "f8"), ("max_kf_t_dist", "f8"), ("max_kf_r_dist", "f8")])
+KEYFRAME_STATE_DTYPE = np.dtype([("prev_f_iskf", "i4"), ("N_prevKF_currF", "i4"), ("entropy_first_prevKF", "f8"),
+                                 ("T_prevKF", "f8", (4, 4)), ("cov_prevKF_currF", "f8", (6, 6))])
+KEYFRAME_RESULT_DTYPE = np.dtype([("new_kf", "i4"), ("N_prevKF_currF", "i4"), ("entropy_curr", "f8"), ("entropy_ratio", "f8"),
+                                  ("t", "f8"), ("r", "f8")])
+
+
+def keyframe_config(h) -> np.ndarray:
+    """The PlKeyframeConfig (KEYFRAME_CONFIG_DTYPE, one record) of a handler.HandlerConfig (or any object with its fields)."""
+    return np.array([(h.min_entropy_ratio, h.max_kf_t_dist, h.max_kf_r_dist)], KEYFRAME_CONFIG_DTYPE)
+
 ST_REFINED, ST_ROBUST_FALLBACK, ST_FEW_BEFORE, ST_FEW_AFTER = 0, 1, 2, 3
 
 
