@@ -1281,6 +1281,14 @@ void session_drop_keyframes(PlStereoSession* ss) {
     ss->kf_rows.clear();
     ss->kf_off.clear();
 }
+
+// the caller's arrays of a PlStereoFrameOut, indexed by records.h's arrays
+RecPtrs frame_out_records(const PlStereoFrameOut* o) {
+    return RecPtrs::from(PT_PL, {o->pt_pl, o->pt_disp, o->pt_P, o->pt_sigma2, o->pt_level, o->pdesc, o->pt_src,
+                                 o->ls_spl, o->ls_epl, o->ls_sdisp, o->ls_edisp, o->ls_sP, o->ls_eP, o->ls_le, o->ls_angle,
+                                 o->ls_sigma2, o->ls_level, o->ldesc, o->ls_src, o->m12_pt, o->inlier_pt, o->m12_ls,
+                                 o->inlier_ls});
+}
 }  // namespace
 
 int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
@@ -1308,16 +1316,12 @@ int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* ss, const 
     const SessionRetained& kr = ss->kept;
     if (!kr.valid) return fail(ctx, PLSTVO_E_INVALID, "nothing retained: no call succeeded since retention was turned on, or the last call failed");
     CK(ctx, cudaSetDevice(ctx->device));
-    using R = SessionRetained;
-    void* dst[R::N_ARRAYS] = {out->pt_pl, out->pt_disp, out->pt_P, out->pt_sigma2, out->pt_level, out->pdesc, out->pt_src,
-                              out->ls_spl, out->ls_epl, out->ls_sdisp, out->ls_edisp, out->ls_sP, out->ls_eP, out->ls_le,
-                              out->ls_angle, out->ls_sigma2, out->ls_level, out->ldesc, out->ls_src,
-                              out->m12_pt, out->inlier_pt, out->m12_ls, out->inlier_ls};
-    const int n_arrays = kr.track ? R::N_ARRAYS : R::M12_PT;   // after an initialize the tracker's arrays are left untouched
+    const RecPtrs dst = frame_out_records(out);
+    const int n_arrays = kr.track ? N_REC : M12_PT;   // after an initialize the tracker's arrays are left untouched
     cudaStream_t s = ctx->s_main;
     for (int k = 0; k < n_arrays; ++k) {
-        const size_t bytes = kr.rows[k] * (size_t)R::row_bytes[k];
-        if (dst[k] && bytes) CK(ctx, cudaMemcpyAsync(dst[k], kr.at<uint8_t>(k), bytes, cudaMemcpyDeviceToHost, s));
+        const size_t bytes = kr.rows[k] * (size_t)REC_BYTES[k];
+        if (dst.p[k] && bytes) CK(ctx, cudaMemcpyAsync(dst.p[k], kr.rec.p[k], bytes, cudaMemcpyDeviceToHost, s));
     }
     CK(ctx, cudaStreamSynchronize(s));
     return kr.n;
@@ -1499,19 +1503,19 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     const size_t o_img = a.take(prepare || !(pts || lns) ? 0 : (size_t)n_img * px), o_th = a.take((size_t)(T + 1) * 2 * n * 4),
                  o_res = a.take((size_t)T * n * sizeof(PlPoseResult));
     const bool keep = ss->retain;
-    // the key-frame test: the streams' states [n], the decisions [T][n], and with retention each step's call-order offsets
-    // of the new rows [T][2][n + 1]
-    size_t o_kfs = 0, o_kfr = 0, o_kfoff = 0;
+    // the key-frame test: the streams' states [n], the decisions [T][n], and with retention each step's segments of the new
+    // rows [T][n] (call order)
+    size_t o_kfs = 0, o_kfr = 0, o_kfseg = 0;
     if (kc) {
         o_kfs = a.take((size_t)n * sizeof(PlKeyframeState));
         o_kfr = a.take((size_t)T * n * sizeof(PlKeyframeResult));
-        o_kfoff = a.take(keep ? (size_t)T * 2 * (n + 1) * 4 : 0);
+        o_kfseg = a.take(keep ? (size_t)T * n * sizeof(GatherSeg) : 0);
     }
     CK(ctx, a.alloc(ctx->arena_run));
     CK(ctx, a.up(o_th, th0.data(), th0.size() * 4, s));
     if (kc) CK(ctx, a.up(o_kfs, kf_state, (size_t)n * sizeof(PlKeyframeState), s));
     const double k_entropy = 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0)));   // KeyframeTest::needNewKF's constant
-    std::vector<int32_t> kf_off(kc && keep ? (size_t)T * 2 * (n + 1) : 0, 0);   // [T][2][n + 1], as uploaded
+    std::vector<GatherSeg> kf_segs(kc && keep ? (size_t)T * n : 0);   // [T][n], as uploaded
     const int32_t* d_th = a.i32(o_th);
     const int ch = rect ? rect->channels : 1;
     std::vector<ImgPart> iparts;
@@ -1590,24 +1594,20 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
                 CK(ctx, launch_session_keyframe(*kc, k_entropy, n, ws.d_results.as<PlPoseResult>(), a.at<PlKeyframeState>(o_kfs),
                                                 d_kf, ws.d_priors.as<PlPrior>(), s));
                 ctx->launches++;
-                if (keep) {   // the key frames' rows, from this step's retention arena into its own chunk
-                    int32_t* off = kf_off.data() + (size_t)t * 2 * (n + 1);
+                if (keep) {   // the key frames' rows, from this step's retention arena into its own chunk, at the same rows
+                    GatherSeg* seg = kf_segs.data() + (size_t)t * n;
+                    int32_t np = 0, nl = 0;
                     for (int k = 0; k < n; ++k) {
-                        off[k + 1] = off[k] + ss->new_pt[(size_t)k];
-                        off[n + 2 + k] = off[n + 1 + k] + ss->new_ls[(size_t)k];
+                        seg[k] = GatherSeg{np, np, ss->new_pt[(size_t)k], nl, nl, ss->new_ls[(size_t)k]};
+                        np += seg[k].n_pt;
+                        nl += seg[k].n_ls;
                     }
-                    const size_t o = o_kfoff + (size_t)t * 2 * (n + 1) * 4;
-                    CK(ctx, a.up(o, off, (size_t)2 * (n + 1) * 4, s));
+                    const size_t o = o_kfseg + (size_t)t * n * sizeof(GatherSeg);
+                    CK(ctx, a.up(o, seg, (size_t)n * sizeof(GatherSeg), s));
                     ss->kf_steps.push_back(std::unique_ptr<SessionRetained>(new SessionRetained()));
                     SessionRetained& c = *ss->kf_steps.back();
-                    CK(ctx, c.lay_out((size_t)off[n], (size_t)off[2 * n + 1], 0, 0));
-                    KeyframeCopyArrays ca;
-                    for (int j = 0; j < KeyframeCopyArrays::N; ++j) {
-                        ca.src[j] = ss->kept.at<uint32_t>(j);
-                        ca.dst[j] = c.at<uint32_t>(j);
-                        ca.words[j] = SessionRetained::row_bytes[j] / 4;
-                    }
-                    CK(ctx, launch_session_keyframe_copy(ca, a.i32(o), d_kf, n, s));
+                    CK(ctx, c.lay_out((size_t)np, (size_t)nl, 0, 0));
+                    CK(ctx, launch_session_gather(ss->kept.rec, c.rec, false, a.at<GatherSeg>(o), n, s, d_kf));
                     ctx->launches++;
                 }
             }
@@ -1663,9 +1663,9 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         for (int t = 0; keep && t < T; ++t)
             for (int k = 0; k < n; ++k) {
                 if (!kf[(size_t)t * n + k].new_kf) continue;
-                const int32_t* off = kf_off.data() + (size_t)t * 2 * (n + 1);
-                ss->kf_rows.insert(ss->kf_rows.end(), {t, ids[k], off[k + 1] - off[k], off[n + 2 + k] - off[n + 1 + k]});
-                ss->kf_off.insert(ss->kf_off.end(), {off[k], off[n + 1 + k]});
+                const GatherSeg& g = kf_segs[(size_t)t * n + k];
+                ss->kf_rows.insert(ss->kf_rows.end(), {t, ids[k], g.n_pt, g.n_ls});
+                ss->kf_off.insert(ss->kf_off.end(), {g.src_pt, g.src_ls});
             }
     }
     return 0;
@@ -1741,24 +1741,20 @@ int plstvo_stereo_session_read_keyframes(PlContext* ctx, const PlStereoSession* 
     if (!ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
     if (!ss->kf_valid) return fail(ctx, PLSTVO_E_INVALID, "no key frames kept: the last call on the session was not a successful run_keyframes");
     CK(ctx, cudaSetDevice(ctx->device));
-    using R = SessionRetained;
-    uint8_t* dst[R::M12_PT] = {(uint8_t*)out->pt_pl, (uint8_t*)out->pt_disp, (uint8_t*)out->pt_P, (uint8_t*)out->pt_sigma2,
-                               (uint8_t*)out->pt_level, out->pdesc, (uint8_t*)out->pt_src, (uint8_t*)out->ls_spl,
-                               (uint8_t*)out->ls_epl, (uint8_t*)out->ls_sdisp, (uint8_t*)out->ls_edisp, (uint8_t*)out->ls_sP,
-                               (uint8_t*)out->ls_eP, (uint8_t*)out->ls_le, (uint8_t*)out->ls_angle, (uint8_t*)out->ls_sigma2,
-                               (uint8_t*)out->ls_level, out->ldesc, (uint8_t*)out->ls_src};
+    const RecPtrs dst = frame_out_records(out);
     const int n_kf = (int)(ss->kf_rows.size() / 4);
     cudaStream_t s = ctx->s_main;
     size_t at_pt = 0, at_ls = 0;   // rows copied so far
     for (int j = 0; j < n_kf; ++j) {
         const int32_t* r = ss->kf_rows.data() + 4 * (size_t)j;
-        const R& c = *ss->kf_steps[(size_t)r[0]];
-        for (int a = 0; a < R::M12_PT; ++a) {
-            const bool pt = a < R::LS_SPL;
-            const size_t w = (size_t)R::row_bytes[a], rows_j = (size_t)(pt ? r[2] : r[3]);
+        const SessionRetained& c = *ss->kf_steps[(size_t)r[0]];
+        for (int a = 0; a < N_LIFT; ++a) {
+            const bool pt = rec_is_point(a);
+            const size_t w = (size_t)REC_BYTES[a], rows_j = (size_t)(pt ? r[2] : r[3]);
             const size_t from = (size_t)ss->kf_off[2 * (size_t)j + (pt ? 0 : 1)], to = pt ? at_pt : at_ls;
-            if (dst[a] && rows_j)
-                CK(ctx, cudaMemcpyAsync(dst[a] + to * w, c.at<uint8_t>(a) + from * w, rows_j * w, cudaMemcpyDeviceToHost, s));
+            if (dst.p[a] && rows_j)
+                CK(ctx, cudaMemcpyAsync(dst.at<uint8_t>(a) + to * w, c.rec.at<uint8_t>(a) + from * w, rows_j * w,
+                                        cudaMemcpyDeviceToHost, s));
         }
         at_pt += (size_t)r[2];
         at_ls += (size_t)r[3];

@@ -95,8 +95,9 @@ int plstvo_stereo_lift_points(PlContext* ctx, const PlCamera* cam, const PlStere
     Arena a;
     const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_kpl = a.take(N1 * 8);
     const size_t o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_kpr = a.take(N2 * 8), o_m12 = a.take(N1 * 4);
-    const size_t o_pl = a.take(N1 * 16), o_disp = a.take(N1 * 8), o_P = a.take(N1 * 24), o_s2 = a.take(N1 * 8);
-    const size_t o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32), o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    size_t o_rec[N_REC];
+    take_records(a, N1, PT_PL, LS_SPL, o_rec);
+    const size_t o_cnt = a.take((size_t)B * 4);
     CK(ctx, a.alloc(ctx->arena_lift_pt));
     cudaStream_t s = ctx->s_main;
     CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
@@ -107,16 +108,10 @@ int plstvo_stereo_lift_points(PlContext* ctx, const PlCamera* cam, const PlStere
     CK(ctx, a.up(o_kpr, kp_r, N2 * 8, s));
     CK(ctx, a.up(o_m12, m12, N1 * 4, s));
     CK(ctx, launch_lift_points(*cam, *scfg, B, a.i32(o_loff), a.f32(o_kpl), a.i32(o_oct), a.u8(o_desc), a.i32(o_roff),
-                               a.f32(o_kpr), a.i32(o_m12), a.f64(o_pl), a.f64(o_disp), a.f64(o_P), a.f64(o_s2), a.i32(o_lvl),
-                               a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+                               a.f32(o_kpr), a.i32(o_m12), arena_records(a, o_rec, PT_PL, LS_SPL), a.i32(o_cnt), s));
     ctx->launches++;
-    CK(ctx, a.down(pt_pl, o_pl, N1 * 16, s));
-    CK(ctx, a.down(pt_disp, o_disp, N1 * 8, s));
-    CK(ctx, a.down(pt_P, o_P, N1 * 24, s));
-    CK(ctx, a.down(pt_sigma2, o_s2, N1 * 8, s));
-    CK(ctx, a.down(pt_level, o_lvl, N1 * 4, s));
-    CK(ctx, a.down(pdesc_out, o_dout, N1 * 32, s));
-    CK(ctx, a.down(src_idx, o_src, N1 * 4, s));
+    const RecPtrs out = RecPtrs::from(PT_PL, {pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx});
+    CK(ctx, down_records(a, out, o_rec, N1, PT_PL, LS_SPL, s));
     return counts_total(ctx, s, B, a.i32(o_cnt), counts);
 }
 
@@ -138,10 +133,10 @@ int plstvo_stereo_lift_lines(PlContext* ctx, const PlCamera* cam, const PlStereo
     Arena a;
     const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_segl = a.take(N1 * 16);
     const size_t o_ang = a.take(N1 * 4), o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_segr = a.take(N2 * 16);
-    const size_t o_m12 = a.take(N1 * 4), o_spl = a.take(N1 * 16), o_epl = a.take(N1 * 16), o_sd = a.take(N1 * 8);
-    const size_t o_ed = a.take(N1 * 8), o_sP = a.take(N1 * 24), o_eP = a.take(N1 * 24), o_le = a.take(N1 * 24);
-    const size_t o_angd = a.take(N1 * 8), o_s2 = a.take(N1 * 8), o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32);
-    const size_t o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
+    const size_t o_m12 = a.take(N1 * 4);
+    size_t o_rec[N_REC];
+    take_records(a, N1, LS_SPL, N_LIFT, o_rec);
+    const size_t o_cnt = a.take((size_t)B * 4);
     CK(ctx, a.alloc(ctx->arena_lift_ls));
     cudaStream_t s = ctx->s_main;
     CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
@@ -153,22 +148,12 @@ int plstvo_stereo_lift_lines(PlContext* ctx, const PlCamera* cam, const PlStereo
     CK(ctx, a.up(o_segr, seg_r, N2 * 16, s));
     CK(ctx, a.up(o_m12, m12, N1 * 4, s));
     CK(ctx, launch_lift_lines(*cam, *scfg, B, a.i32(o_loff), a.f32(o_segl), a.f32(o_ang), a.i32(o_oct), a.u8(o_desc),
-                              a.i32(o_roff), a.f32(o_segr), a.i32(o_m12), a.f64(o_spl), a.f64(o_epl), a.f64(o_sd), a.f64(o_ed),
-                              a.f64(o_sP), a.f64(o_eP), a.f64(o_le), a.f64(o_angd), a.f64(o_s2), a.i32(o_lvl), a.u8(o_dout),
-                              a.i32(o_src), a.i32(o_cnt), s));
+                              a.i32(o_roff), a.f32(o_segr), a.i32(o_m12), arena_records(a, o_rec, LS_SPL, N_LIFT), a.i32(o_cnt),
+                              s));
     ctx->launches++;
-    CK(ctx, a.down(ls_spl, o_spl, N1 * 16, s));
-    CK(ctx, a.down(ls_epl, o_epl, N1 * 16, s));
-    CK(ctx, a.down(ls_sdisp, o_sd, N1 * 8, s));
-    CK(ctx, a.down(ls_edisp, o_ed, N1 * 8, s));
-    CK(ctx, a.down(ls_sP, o_sP, N1 * 24, s));
-    CK(ctx, a.down(ls_eP, o_eP, N1 * 24, s));
-    CK(ctx, a.down(ls_le, o_le, N1 * 24, s));
-    CK(ctx, a.down(ls_angle, o_angd, N1 * 8, s));
-    CK(ctx, a.down(ls_sigma2, o_s2, N1 * 8, s));
-    CK(ctx, a.down(ls_level, o_lvl, N1 * 4, s));
-    CK(ctx, a.down(ldesc_out, o_dout, N1 * 32, s));
-    CK(ctx, a.down(src_idx, o_src, N1 * 4, s));
+    const RecPtrs out = RecPtrs::from(LS_SPL, {ls_spl, ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
+                                               ls_level, ldesc_out, src_idx});
+    CK(ctx, down_records(a, out, o_rec, N1, LS_SPL, N_LIFT, s));
     return counts_total(ctx, s, B, a.i32(o_cnt), counts);
 }
 
@@ -180,15 +165,11 @@ void plstvo_default_stereo_match_config(PlStereoMatchConfig* c) {   // include/s
 }
 
 namespace {
-struct StereoOut {   // host destinations of the lifted records (points use the first seven)
-    int32_t* m12; double *a_pl, *a_disp, *a_P, *a_s2; int32_t* level; uint8_t* desc; int32_t *src, *counts;
-    double *epl, *edisp, *eP, *le, *angle;   // lines only
-};
-
+// out: the host destinations of the kind's lifted records
 int match_stereo_common(PlContext* ctx, bool lines, const PlCamera* cam, const PlStereoMatchConfig* mc, const PlStereoConfig* sc,
                         int B, const int32_t* l_off, const float* xy_l, const float* angle_l, const int32_t* octave_l,
-                        const uint8_t* desc_l, const int32_t* r_off, const float* xy_r, const uint8_t* desc_r,
-                        const StereoOut& out) {
+                        const uint8_t* desc_l, const int32_t* r_off, const float* xy_r, const uint8_t* desc_r, int32_t* m12,
+                        const RecPtrs& out, int32_t* counts) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
     if (!cam || !mc || !sc || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
@@ -212,10 +193,10 @@ int match_stereo_common(PlContext* ctx, bool lines, const PlCamera* cam, const P
     const GridScratch g(a, rows, cols, B, N1, N2, N2 * grid_cells_per_train(lines, rows, cols), !lines, lines);
     const size_t o_prob = a.take((size_t)B * sizeof(GridProblem));
     // lifted records
-    const size_t o_pl = a.take(N1 * 16), o_disp = a.take(N1 * 8), o_P = a.take(N1 * 24), o_s2 = a.take(N1 * 8);
-    const size_t o_lvl = a.take(N1 * 4), o_dout = a.take(N1 * 32), o_src = a.take(N1 * 4), o_cnt = a.take((size_t)B * 4);
-    const size_t o_epl = a.take(lines ? N1 * 16 : 0), o_edisp = a.take(lines ? N1 * 8 : 0), o_eP = a.take(lines ? N1 * 24 : 0);
-    const size_t o_le = a.take(lines ? N1 * 24 : 0), o_angd = a.take(lines ? N1 * 8 : 0);
+    const int first = lines ? LS_SPL : PT_PL, last = lines ? N_LIFT : LS_SPL;
+    size_t o_rec[N_REC];
+    take_records(a, N1, first, last, o_rec);
+    const size_t o_cnt = a.take((size_t)B * 4);
     CK(ctx, a.alloc(ctx->arena_stereo));
     std::vector<GridProblem> probs((size_t)B);
     g.fill(probs.data(), B, lines, l_off, r_off, a.u8(o_d1), a.u8(o_d2), a.i32(o_m12), a.i32(o_gcnt));
@@ -242,32 +223,17 @@ int match_stereo_common(PlContext* ctx, bool lines, const PlCamera* cam, const P
                    mc->min_ratio_12_p, mc->line_sim_th};
     CK(ctx, launch_match_grid(a.at<GridProblem>(o_prob), B, prm, lines, s));
     // 3. lifting, reading the match list where matchGrid left it
+    const RecPtrs rec = arena_records(a, o_rec, first, last);
     if (lines)
         CK(ctx, launch_lift_lines(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.f32(o_ang), a.i32(o_oct), a.u8(o_d1),
-                                  a.i32(o_roff), a.f32(o_xyr), a.i32(o_m12), a.f64(o_pl), a.f64(o_epl), a.f64(o_disp),
-                                  a.f64(o_edisp), a.f64(o_P), a.f64(o_eP), a.f64(o_le), a.f64(o_angd), a.f64(o_s2),
-                                  a.i32(o_lvl), a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+                                  a.i32(o_roff), a.f32(o_xyr), a.i32(o_m12), rec, a.i32(o_cnt), s));
     else
         CK(ctx, launch_lift_points(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.i32(o_oct), a.u8(o_d1), a.i32(o_roff),
-                                   a.f32(o_xyr), a.i32(o_m12), a.f64(o_pl), a.f64(o_disp), a.f64(o_P), a.f64(o_s2),
-                                   a.i32(o_lvl), a.u8(o_dout), a.i32(o_src), a.i32(o_cnt), s));
+                                   a.f32(o_xyr), a.i32(o_m12), rec, a.i32(o_cnt), s));
     ctx->launches += 3;
-    CK(ctx, a.down(out.m12, o_m12, N1 * 4, s));
-    CK(ctx, a.down(out.a_pl, o_pl, N1 * 16, s));
-    CK(ctx, a.down(out.a_disp, o_disp, N1 * 8, s));
-    CK(ctx, a.down(out.a_P, o_P, N1 * 24, s));
-    CK(ctx, a.down(out.a_s2, o_s2, N1 * 8, s));
-    CK(ctx, a.down(out.level, o_lvl, N1 * 4, s));
-    CK(ctx, a.down(out.desc, o_dout, N1 * 32, s));
-    CK(ctx, a.down(out.src, o_src, N1 * 4, s));
-    if (lines) {
-        CK(ctx, a.down(out.epl, o_epl, N1 * 16, s));
-        CK(ctx, a.down(out.edisp, o_edisp, N1 * 8, s));
-        CK(ctx, a.down(out.eP, o_eP, N1 * 24, s));
-        CK(ctx, a.down(out.le, o_le, N1 * 24, s));
-        CK(ctx, a.down(out.angle, o_angd, N1 * 8, s));
-    }
-    return counts_total(ctx, s, B, a.i32(o_cnt), out.counts, a.i32(o_gcnt));
+    CK(ctx, a.down(m12, o_m12, N1 * 4, s));
+    CK(ctx, down_records(a, out, o_rec, N1, first, last, s));
+    return counts_total(ctx, s, B, a.i32(o_cnt), counts, a.i32(o_gcnt));
 }
 }  // namespace
 
@@ -276,9 +242,9 @@ int plstvo_match_stereo_points(PlContext* ctx, const PlCamera* cam, const PlSter
                                const int32_t* r_off, const float* kp_r, const uint8_t* desc_r, int32_t* m12, double* pt_pl,
                                double* pt_disp, double* pt_P, double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out,
                                int32_t* src_idx, int32_t* counts) {
-    const StereoOut out{m12, pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts,
-                        nullptr, nullptr, nullptr, nullptr, nullptr};
-    return match_stereo_common(ctx, false, cam, mcfg, scfg, B, l_off, kp_l, nullptr, octave_l, desc_l, r_off, kp_r, desc_r, out);
+    const RecPtrs out = RecPtrs::from(PT_PL, {pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx});
+    return match_stereo_common(ctx, false, cam, mcfg, scfg, B, l_off, kp_l, nullptr, octave_l, desc_l, r_off, kp_r, desc_r, m12,
+                               out, counts);
 }
 
 int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
@@ -287,9 +253,10 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
                               int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp, double* ls_edisp, double* ls_sP,
                               double* ls_eP, double* ls_le, double* ls_angle, double* ls_sigma2, int32_t* ls_level,
                               uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts) {
-    const StereoOut out{m12, ls_spl, ls_sdisp, ls_sP, ls_sigma2, ls_level, ldesc_out, src_idx, counts,
-                        ls_epl, ls_edisp, ls_eP, ls_le, ls_angle};
-    return match_stereo_common(ctx, true, cam, mcfg, scfg, B, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, desc_r, out);
+    const RecPtrs out = RecPtrs::from(LS_SPL, {ls_spl, ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
+                                               ls_level, ldesc_out, src_idx});
+    return match_stereo_common(ctx, true, cam, mcfg, scfg, B, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, desc_r, m12,
+                               out, counts);
 }
 
 }  // extern "C"
@@ -380,6 +347,16 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     }
     cudaStream_t s = ctx->s_main, sh = ctx->s_h2d;   // uploads of set k + 1 run under the kernels of set k
     // (this slot's arena is free: a blocking call ends synchronised, an async slot is reused only after its event completed)
+    // the lifting of frames [first, first + nf) of a set into o's entries of its kind (all null: counts only), at out_off
+    auto lift = [&](const Set& st, int nf, int first, const RecPtrs& o, const int32_t* out_off,
+                    const PlCamera* cams) -> cudaError_t {
+        if (st.lines)
+            return launch_lift_lines(*cam, *sc, nf, a.i32(st.o_loff) + first, st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
+                                     a.i32(st.o_roff) + first, st.g_xyr, a.i32(st.o_m12), o, a.i32(st.o_cnt) + first, s,
+                                     out_off, cams);
+        return launch_lift_points(*cam, *sc, nf, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
+                                  st.g_xyr, a.i32(st.o_m12), o, a.i32(st.o_cnt) + first, s, out_off, cams);
+    };
     const double inv_w = cols / static_cast<double>(cam->width), inv_h = rows / static_cast<double>(cam->height);
     const GridParams gprm{rows, cols, GRID_CAP, mc->best_lr_matches ? 1 : 0, PlGridWindow{mc->matching_s_ws, 0, 0, 0},
                           mc->min_ratio_12_p, mc->line_sim_th};
@@ -418,21 +395,14 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             CK(ctx, cudaStreamWaitEvent(s, dev->lines_ready, 0));
             joined = true;
         }
-        if (st.lines) {
+        if (st.lines)
             CK(ctx, launch_stereo_cells_lines((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
                                               a.f64(g.tline), a.f64(g.tdir), s));
-            CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, true, s));
-            CK(ctx, launch_lift_lines(*cam, *sc, NF, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
-                                      a.i32(st.o_roff), st.g_xyr, a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr,
-                                      nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, a.i32(st.o_cnt), s));
-        } else {
+        else
             CK(ctx, launch_stereo_cells_points((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
                                                a.i32(g.tcell), s));
-            CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, false, s));
-            CK(ctx, launch_lift_points(*cam, *sc, NF, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
-                                       a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                       a.i32(st.o_cnt), s));
-        }
+        CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, st.lines, s));
+        CK(ctx, lift(st, NF, 0, RecPtrs{}, nullptr, nullptr));
         ctx->launches += 3;
         CK(ctx, cudaMemcpyAsync(cnt + (size_t)k * NF, a.u8(st.o_cnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
         CK(ctx, cudaMemcpyAsync(gcnt + (size_t)k * NF, a.u8(st.o_gcnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
@@ -467,24 +437,13 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         CK(ctx, cudaMemcpyAsync(session->d_cams.p, fc.data(), (size_t)NF * sizeof(PlCamera), cudaMemcpyHostToDevice, s));
         d_cams = session->d_cams.as<PlCamera>();
     }
-    // pass 2: the same lifting kernels, now writing at the compact offsets (prev role: P, sigma2, segments, level; curr role: pl, le).
-    // `first` = first frame of the role inside its set (sequence mode: the current-frame role starts at frame 1).
-    auto lift_prev_points = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
-        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff), st.g_xyr,
-                                  a.i32(st.o_m12), nullptr, nullptr, o.ptP, o.pts2, nullptr, o.pdesc, nullptr, a.i32(st.o_cnt), s,
-                                  out_off, d_cams);
-    };
-    auto lift_prev_lines = [&](const Set& st, const PrevRows& o, const int32_t* out_off) -> cudaError_t {
-        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff), st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1, a.i32(st.o_roff),
-                                 st.g_xyr, a.i32(st.o_m12), o.spl, o.epl, nullptr, nullptr, o.sP, o.eP, nullptr, nullptr, o.s2,
-                                 o.lev, o.ldesc, nullptr, a.i32(st.o_cnt), s, out_off, d_cams);
-    };
+    // pass 2: the same lifting kernels, now writing at the compact offsets: the previous-frame role (a pool's or the
+    // workspace's PREV_ROLE entries), the current-frame role (curr_rows below) and retention (every array)
     // session: the new frames' previous-frame role goes into the next pool, the untouched streams' kept frames follow it there
     if (session) {
         if (const int rc = session_plan(ctx, session, cnt, cnt + NF, s)) return rc;
-        const PrevRows& next = session->pool[session->cur ^ 1].rows;
-        CK(ctx, lift_prev_points(sets[0], next, session_out_off(session, false)));
-        CK(ctx, lift_prev_lines(sets[1], next, session_out_off(session, true)));
+        for (int k = 0; k < 2; ++k)
+            CK(ctx, lift(sets[k], B, 0, session->pool[session->cur ^ 1].rows, session_out_off(session, k == 1), d_cams));
         ctx->launches += 2;
         if (const int rc = session_gather_others(ctx, session, s)) return rc;
         if (session->retain) {   // plstvo_stereo_session_read: every record of the new frames, compact in call order
@@ -494,23 +453,7 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             cudaEvent_t offsets_up = next_event(ctx);   // sets[k].o_ooff, uploaded on sh above
             CK(ctx, cudaEventRecord(offsets_up, sh));
             CK(ctx, cudaStreamWaitEvent(s, offsets_up, 0));
-            using R = SessionRetained;
-            const Set& sp = sets[0];
-            const Set& sl = sets[1];
-            const cudaError_t e_pt =
-                launch_lift_points(*cam, *sc, NF, a.i32(sp.o_loff), sp.g_xyl, sp.g_oct, sp.g_d1, a.i32(sp.o_roff), sp.g_xyr,
-                                   a.i32(sp.o_m12), kr.at<double>(R::PT_PL), kr.at<double>(R::PT_DISP), kr.at<double>(R::PT_P),
-                                   kr.at<double>(R::PT_S2), kr.at<int32_t>(R::PT_LEVEL), kr.at<uint8_t>(R::PT_DESC),
-                                   kr.at<int32_t>(R::PT_SRC), a.i32(sp.o_cnt), s, a.i32(sp.o_ooff), d_cams);
-            CK(ctx, e_pt);
-            const cudaError_t e_ls =
-                launch_lift_lines(*cam, *sc, NF, a.i32(sl.o_loff), sl.g_xyl, a.f32(sl.o_ang), sl.g_oct, sl.g_d1,
-                                  a.i32(sl.o_roff), sl.g_xyr, a.i32(sl.o_m12), kr.at<double>(R::LS_SPL), kr.at<double>(R::LS_EPL),
-                                  kr.at<double>(R::LS_SDISP), kr.at<double>(R::LS_EDISP), kr.at<double>(R::LS_SP),
-                                  kr.at<double>(R::LS_EP), kr.at<double>(R::LS_LE), kr.at<double>(R::LS_ANGLE),
-                                  kr.at<double>(R::LS_S2), kr.at<int32_t>(R::LS_LEVEL), kr.at<uint8_t>(R::LS_DESC),
-                                  kr.at<int32_t>(R::LS_SRC), a.i32(sl.o_cnt), s, a.i32(sl.o_ooff), d_cams);
-            CK(ctx, e_ls);
+            for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], NF, 0, kr.rec, a.i32(sets[k].o_ooff), d_cams));
             ctx->launches += 2;
         }
         if (!track) {
@@ -538,33 +481,21 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     cudaEvent_t planned = next_event(ctx);
     CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(s, planned, 0));
-    auto lift_curr_points = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
-        return launch_lift_points(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
-                                  st.g_xyr, a.i32(st.o_m12), ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, nullptr,
-                                  ws.d_pdesc2.as<uint8_t>(), nullptr, a.i32(st.o_cnt) + first, s, a.i32(o_out), d_cams);
-    };
-    auto lift_curr_lines = [&](const Set& st, int first, size_t o_out) -> cudaError_t {
-        return launch_lift_lines(*cam, *sc, B, a.i32(st.o_loff) + first, st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
-                                 a.i32(st.o_roff) + first, st.g_xyr, a.i32(st.o_m12), nullptr, nullptr, nullptr, nullptr, nullptr,
-                                 nullptr, ws.d_lsle.as<double>(), nullptr, nullptr, nullptr, ws.d_ldesc2.as<uint8_t>(), nullptr,
-                                 a.i32(st.o_cnt) + first, s, a.i32(o_out), d_cams);
-    };
     if (session) {
         if (const int rc2 = session_gather_named(ctx, session, workspace_prev_rows(ws), s)) return rc2;
     } else {
-        const PrevRows wsr = workspace_prev_rows(ws);
-        CK(ctx, lift_prev_points(sets[0], wsr, a.i32(sets[0].o_ooff)));
-        CK(ctx, lift_prev_lines(sets[1], wsr, a.i32(sets[1].o_ooff)));
+        for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], B, 0, workspace_prev_rows(ws), a.i32(sets[k].o_ooff), d_cams));
     }
-    if (sequence) {
-        CK(ctx, lift_curr_points(sets[0], 1, sets[0].o_ooff2));
-        CK(ctx, lift_curr_lines(sets[1], 1, sets[1].o_ooff2));
-    } else if (session) {
-        CK(ctx, lift_curr_points(sets[0], 0, sets[0].o_ooff));
-        CK(ctx, lift_curr_lines(sets[1], 0, sets[1].o_ooff));
-    } else {
-        CK(ctx, lift_curr_points(sets[2], 0, sets[2].o_ooff));
-        CK(ctx, lift_curr_lines(sets[3], 0, sets[3].o_ooff));
+    // the current-frame role: the set's frames from `first` on (sequence mode: the second frame)
+    RecPtrs curr_rows;
+    curr_rows.p[PT_PL] = ws.d_ptpl.p;
+    curr_rows.p[PT_DESC] = ws.d_pdesc2.p;
+    curr_rows.p[LS_LE] = ws.d_lsle.p;
+    curr_rows.p[LS_DESC] = ws.d_ldesc2.p;
+    const int first = sequence ? 1 : 0;
+    for (int k = 0; k < 2; ++k) {
+        const Set& st = sets[one_set ? k : 2 + k];
+        CK(ctx, lift(st, B, first, curr_rows, a.i32(sequence ? st.o_ooff2 : st.o_ooff), d_cams));
     }
     ctx->launches += session ? 2 : 4;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
@@ -577,9 +508,9 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         const SessionRetained& kr = session->kept;
         const DevBuf* src[4] = {&ws.d_m12p, &ws.d_inlp, &ws.d_m12l, &ws.d_inll};
         for (int k = 0; k < 4; ++k) {
-            const int r = SessionRetained::M12_PT + k;
-            const size_t bytes = kr.rows[r] * (size_t)SessionRetained::row_bytes[r];
-            if (bytes) CK(ctx, cudaMemcpyAsync(kr.at<uint8_t>(r), src[k]->p, bytes, cudaMemcpyDeviceToDevice, s));
+            const int r = M12_PT + k;
+            const size_t bytes = kr.rows[r] * (size_t)REC_BYTES[r];
+            if (bytes) CK(ctx, cudaMemcpyAsync(kr.rec.p[r], src[k]->p, bytes, cudaMemcpyDeviceToDevice, s));
         }
     }
     if (dev && dev->tracked) return dev->tracked(ws);

@@ -8,6 +8,7 @@
 #include <mutex>
 
 #include "../../include/plstvo.h"
+#include "records.h"
 
 namespace plstvo {
 
@@ -173,19 +174,17 @@ cudaError_t launch_stereo_cells_points(int n_l, int n_r, double inv_w, double in
                                        int32_t* q_cell, int32_t* t_cell, cudaStream_t s);
 cudaError_t launch_stereo_cells_lines(int n_l, int n_r, double inv_w, double inv_h, const float* seg_l, const float* seg_r,
                                       int32_t* q_line, double* t_line, double* t_dir, cudaStream_t s);
-// lift.cu: stereo matches -> PointFeature / LineFeature records (src/stereoFrame.cpp:149-172, :348-397)
+// lift.cu: stereo matches -> PointFeature / LineFeature records (src/stereoFrame.cpp:149-172, :348-397).  out: the device
+// arrays PT_PL .. PT_SRC (points) or LS_SPL .. LS_SRC (lines), null entries skipped (all null: count only).
 cudaError_t launch_lift_points(const PlCamera& cam, const PlStereoConfig& sc, int B, const int32_t* l_off, const float* kp_l,
                                const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off, const float* kp_r,
-                               const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P, double* pt_sigma2,
-                               int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts, cudaStream_t s,
-                               const int32_t* out_off = nullptr,    // out_off: compact output offsets per frame (else l_off); null outputs are skipped
+                               const int32_t* m12, const RecPtrs& out, int32_t* counts, cudaStream_t s,
+                               const int32_t* out_off = nullptr,    // out_off: compact output offsets per frame (else l_off)
                                const PlCamera* cams = nullptr);     // cams: device camera of each frame (else cam)
 cudaError_t launch_lift_lines(const PlCamera& cam, const PlStereoConfig& sc, int B, const int32_t* l_off, const float* seg_l,
                               const float* ang_l, const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off,
-                              const float* seg_r, const int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp,
-                              double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le, double* ls_angle,
-                              double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts,
-                              cudaStream_t s, const int32_t* out_off = nullptr, const PlCamera* cams = nullptr);
+                              const float* seg_r, const int32_t* m12, const RecPtrs& out, int32_t* counts, cudaStream_t s,
+                              const int32_t* out_off = nullptr, const PlCamera* cams = nullptr);
 
 // orb.cu: ORB description (pyramid, blur, border filter, angle, rBRIEF) of a batch of images of one size
 constexpr int ORB_MAX_LEVELS = 32;

@@ -379,29 +379,40 @@ int ws_launch_match(PlContext* ctx, Workspace& ws, int p0, int p1, cudaStream_t 
 int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_level, cudaStream_t s,
                     cudaEvent_t* marks = nullptr);
 
-// ---- session.cu: the previous-frame-role records of kept frames (plstvo_stereo_session_*) ----
-// Where the previous-frame role of a frame's stereo features is written: every array lift_points / lift_lines fill for a
-// frame that is tracked against (the workspace's d_ptP .. d_ldesc1, or a session pool), rows in CSR order.
-struct PrevRows {
-    double *ptP = nullptr, *pts2 = nullptr; uint8_t* pdesc = nullptr;                       // [n][3], [n], [n][32]
-    double *spl = nullptr, *epl = nullptr, *sP = nullptr, *eP = nullptr, *s2 = nullptr;      // [m][2] x2, [m][3] x2, [m]
-    int32_t* lev = nullptr; uint8_t* ldesc = nullptr;                                        // [m], [m][32]
-};
-constexpr size_t SESSION_PT_BYTES = 24 + 8 + 32;                   // bytes per kept stereo point
-constexpr size_t SESSION_LS_BYTES = 16 + 16 + 24 + 24 + 8 + 4 + 32;  // bytes per kept stereo line
-inline PrevRows workspace_prev_rows(const Workspace& ws) {
-    PrevRows r;
-    r.ptP = ws.d_ptP.as<double>(); r.pts2 = ws.d_pts2.as<double>(); r.pdesc = ws.d_pdesc1.as<uint8_t>();
-    r.spl = ws.d_lsspl.as<double>(); r.epl = ws.d_lsepl.as<double>(); r.sP = ws.d_lssP.as<double>();
-    r.eP = ws.d_lseP.as<double>(); r.s2 = ws.d_lss2.as<double>(); r.lev = ws.d_lslev.as<int32_t>();
-    r.ldesc = ws.d_ldesc1.as<uint8_t>();
+// ---- the lifted records (records.h) on an arena ----
+// Slices of `rows` rows for the record arrays [first, last), taken in table order; off[k] receives array k's offset.
+inline void take_records(Arena& a, size_t rows, int first, int last, size_t* off) {
+    for (int k = first; k < last; ++k) off[k] = a.take(rows * (size_t)REC_BYTES[k]);
+}
+// the allocated arena's slices off[first .. last)
+inline RecPtrs arena_records(const Arena& a, const size_t* off, int first, int last) {
+    RecPtrs r;
+    for (int k = first; k < last; ++k) r.p[k] = a.u8(off[k]);
     return r;
 }
-// One session pool: the kept frames of every stream, point rows and line rows in stream-id order.
+// downloads `rows` rows of each array [first, last) into dst's non-null entries
+inline cudaError_t down_records(const Arena& a, const RecPtrs& dst, const size_t* off, size_t rows, int first, int last,
+                                cudaStream_t s) {
+    for (int k = first; k < last; ++k)
+        if (const cudaError_t e = a.down(dst.p[k], off[k], rows * (size_t)REC_BYTES[k], s)) return e;
+    return cudaSuccess;
+}
+
+// ---- session.cu: the previous-frame-role records of kept frames (plstvo_stereo_session_*) ----
+// The workspace's previous-frame buffers, the PREV_ROLE entries of a RecPtrs
+inline RecPtrs workspace_prev_rows(const Workspace& ws) {
+    RecPtrs r;
+    r.p[PT_P] = ws.d_ptP.p; r.p[PT_S2] = ws.d_pts2.p; r.p[PT_DESC] = ws.d_pdesc1.p;
+    r.p[LS_SPL] = ws.d_lsspl.p; r.p[LS_EPL] = ws.d_lsepl.p; r.p[LS_SP] = ws.d_lssP.p; r.p[LS_EP] = ws.d_lseP.p;
+    r.p[LS_S2] = ws.d_lss2.p; r.p[LS_LEVEL] = ws.d_lslev.p; r.p[LS_DESC] = ws.d_ldesc1.p;
+    return r;
+}
+// One session pool: the kept frames of every stream in the previous-frame role (the PREV_ROLE entries of rows), point rows
+// and line rows in stream-id order.
 struct SessionPool {
     DevBuf buf;
     size_t cap_pt = 0, cap_ls = 0;   // rows
-    PrevRows rows;
+    RecPtrs rows;
     cudaError_t ensure(size_t n_pt, size_t n_ls);
 };
 // A block of consecutive rows moved by session_gather_kernel: point rows [src_pt, src_pt + n_pt) of the source to dst_pt ..
@@ -409,25 +420,21 @@ struct SessionPool {
 struct GatherSeg {
     int32_t src_pt, dst_pt, n_pt, src_ls, dst_ls, n_ls;
 };
-cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s);
+// One block per segment, copying the rows of the PREV_ROLE arrays (prev_role) or of every lifted array (else), unchanged.
+// gate (optional, [n_segs]): segment k is copied only where gate[k].new_kf is set.
+cudaError_t launch_session_gather(const RecPtrs& src, const RecPtrs& dst, bool prev_role, const GatherSeg* segs, int n_segs,
+                                  cudaStream_t s, const PlKeyframeResult* gate = nullptr);
 
 // The records a session call retains for plstvo_stereo_session_read (plstvo_stereo_session_retain): the new frames' full
-// point and line records and the insert's m12 / inlier rows, one array each in PlStereoFrameOut's field order, rows in call
-// order.  lay_out() sizes the arena for one call; valid is set only when that call succeeded.
+// point and line records and the insert's m12 / inlier rows, every array of records.h, rows in call order.  lay_out() sizes
+// the arena for one call; valid is set only when that call succeeded.
 struct SessionRetained {
-    enum {   // arrays, points first
-        PT_PL, PT_DISP, PT_P, PT_S2, PT_LEVEL, PT_DESC, PT_SRC,
-        LS_SPL, LS_EPL, LS_SDISP, LS_EDISP, LS_SP, LS_EP, LS_LE, LS_ANGLE, LS_S2, LS_LEVEL, LS_DESC, LS_SRC,
-        M12_PT, INL_PT, M12_LS, INL_LS, N_ARRAYS
-    };
-    static const int row_bytes[N_ARRAYS];
     DevBuf buf;
-    size_t off[N_ARRAYS] = {};
-    size_t rows[N_ARRAYS] = {};   // of every array: the new frames' points / lines, the kept frames' points / lines
+    RecPtrs rec;               // where each array starts
+    size_t rows[N_REC] = {};   // of every array: the new frames' points / lines, the kept frames' points / lines
     bool valid = false, track = false;
     int n = 0;
     cudaError_t lay_out(size_t new_pt, size_t new_ls, size_t kept_pt, size_t kept_ls);
-    template <typename T> T* at(int k) const { return reinterpret_cast<T*>(buf.as<uint8_t>() + off[k]); }
 };
 
 }  // namespace plstvo
@@ -482,7 +489,7 @@ int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, con
 // The two moves of a planned call, enqueued on s: the named streams' kept frames from pool[cur] into the workspace's
 // previous-frame arrays at kept_off_pt / kept_off_ls (insert), and the untouched streams' kept frames from pool[cur] into
 // pool[cur ^ 1].  The new frames' previous-frame role goes into pool[cur ^ 1] through the lift kernels, at session_out_off.
-int session_gather_named(PlContext* ctx, PlStereoSession* ss, const PrevRows& ws_rows, cudaStream_t s);
+int session_gather_named(PlContext* ctx, PlStereoSession* ss, const RecPtrs& ws_rows, cudaStream_t s);
 int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s);
 // device offsets [n] of the new frames' first point / line rows in pool[cur ^ 1]
 const int32_t* session_out_off(const PlStereoSession* ss, bool lines);
@@ -498,16 +505,6 @@ cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPose
 // update) take Tfw = I, Tfw_cov = I.  k_entropy = 3 (1 + log 2 pi), as the host computes it.
 cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
                                     PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s);
-// The point and line arrays of SessionRetained (the first LS_SPL are points), as 4-byte words
-struct KeyframeCopyArrays {
-    enum { N = 19, N_PT = 7 };
-    const uint32_t* src[N];
-    uint32_t* dst[N];
-    int words[N];
-};
-// the rows of the streams kf[k].new_kf marks, for n streams at call-order offsets off ([n + 1] points, [n + 1] lines)
-cudaError_t launch_session_keyframe_copy(const KeyframeCopyArrays& a, const int32_t* off, const PlKeyframeResult* kf, int n,
-                                         cudaStream_t s);
 
 // ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
 // Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the

@@ -1,6 +1,6 @@
 // keyframe.cu — the PL-SLAM key-frame test of a session run on the device (plstvo_stereo_session_run_keyframes): needNewKF
-// and currFrameIsKF of every named stream after each step's optimizePose, and the copy of the key frames' records into the
-// run's retention chunks.
+// and currFrameIsKF of every named stream after each step's optimizePose.  (session_gather_kernel copies the key frames'
+// records into the run's retention chunks.)
 //
 // Precision: every operation follows plstvo.hpp's se3 helpers and KeyframeTest::needNewKF in fp64, in the header's order,
 // with its pivoting, loop order and divisions.  Each a * b + c is spelled __dadd_rn(__dmul_rn(a, b), c) so that nvcc forms
@@ -188,36 +188,12 @@ __global__ void session_keyframe_kernel(PlKeyframeConfig cfg, double k_entropy, 
     }
 }
 
-constexpr int KF_COPY_THREADS = 256;
-
-// One block per named stream: a key frame's rows of every point and line array, unchanged, from the step's retention arena
-// into the step's key-frame chunk at the same call-order offsets (off: point offsets [n + 1], then line offsets [n + 1]).
-__global__ void __launch_bounds__(KF_COPY_THREADS) session_keyframe_copy_kernel(KeyframeCopyArrays a, const int32_t* __restrict__ off,
-                                                                                 const PlKeyframeResult* __restrict__ kf, int n) {
-    const int k = blockIdx.x;
-    if (!kf[k].new_kf) return;
-#pragma unroll 1
-    for (int j = 0; j < KeyframeCopyArrays::N; ++j) {
-        const int32_t* o = off + (j < KeyframeCopyArrays::N_PT ? 0 : n + 1);
-        const int w = a.words[j];
-        const size_t first = (size_t)o[k] * w, last = (size_t)o[k + 1] * w;
-        for (size_t i = first + threadIdx.x; i < last; i += KF_COPY_THREADS) a.dst[j][i] = a.src[j][i];
-    }
-}
-
 }  // namespace
 
 cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
                                     PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     session_keyframe_kernel<<<(n + 63) / 64, 64, 0, s>>>(cfg, k_entropy, n, results, state, out, priors);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_session_keyframe_copy(const KeyframeCopyArrays& a, const int32_t* off, const PlKeyframeResult* kf, int n,
-                                         cudaStream_t s) {
-    if (n <= 0) return cudaSuccess;
-    session_keyframe_copy_kernel<<<n, KF_COPY_THREADS, 0, s>>>(a, off, kf, n);
     return cudaGetLastError();
 }
 

@@ -250,34 +250,28 @@ cudaError_t launch_stereo_cells_lines(int n_l, int n_r, double inv_w, double inv
 
 cudaError_t launch_lift_points(const PlCamera& cam, const PlStereoConfig& sc, int B, const int32_t* l_off, const float* kp_l,
                                const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off, const float* kp_r,
-                               const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P, double* pt_sigma2,
-                               int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts, cudaStream_t s,
-                               const int32_t* out_off, const PlCamera* cams) {
+                               const int32_t* m12, const RecPtrs& out, int32_t* counts, cudaStream_t s, const int32_t* out_off,
+                               const PlCamera* cams) {
     if (B <= 0) return cudaSuccess;
-    if (cams)
-        lift_points_kernel<true><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, pt_pl, pt_disp,
-                                                          pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts, out_off, cams);
-    else
-        lift_points_kernel<false><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, pt_pl, pt_disp,
-                                                           pt_P, pt_sigma2, pt_level, pdesc_out, src_idx, counts, out_off, nullptr);
+    const auto kernel = cams ? lift_points_kernel<true> : lift_points_kernel<false>;
+    kernel<<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, kp_l, oct_l, desc_l, r_off, kp_r, m12, out.at<double>(PT_PL),
+                                    out.at<double>(PT_DISP), out.at<double>(PT_P), out.at<double>(PT_S2),
+                                    out.at<int32_t>(PT_LEVEL), out.at<uint8_t>(PT_DESC), out.at<int32_t>(PT_SRC), counts,
+                                    out_off, cams);
     return cudaGetLastError();
 }
 
 cudaError_t launch_lift_lines(const PlCamera& cam, const PlStereoConfig& sc, int B, const int32_t* l_off, const float* seg_l,
                               const float* ang_l, const int32_t* oct_l, const uint8_t* desc_l, const int32_t* r_off,
-                              const float* seg_r, const int32_t* m12, double* ls_spl, double* ls_epl, double* ls_sdisp,
-                              double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le, double* ls_angle,
-                              double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts,
-                              cudaStream_t s, const int32_t* out_off, const PlCamera* cams) {
+                              const float* seg_r, const int32_t* m12, const RecPtrs& out, int32_t* counts, cudaStream_t s,
+                              const int32_t* out_off, const PlCamera* cams) {
     if (B <= 0) return cudaSuccess;
-    if (cams)
-        lift_lines_kernel<true><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, ls_spl,
-                                                         ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
-                                                         ls_level, ldesc_out, src_idx, counts, out_off, cams);
-    else
-        lift_lines_kernel<false><<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, ls_spl,
-                                                          ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
-                                                          ls_level, ldesc_out, src_idx, counts, out_off, nullptr);
+    const auto kernel = cams ? lift_lines_kernel<true> : lift_lines_kernel<false>;
+    kernel<<<B, LF_THREADS, 0, s>>>(cam, sc, l_off, seg_l, ang_l, oct_l, desc_l, r_off, seg_r, m12, out.at<double>(LS_SPL),
+                                    out.at<double>(LS_EPL), out.at<double>(LS_SDISP), out.at<double>(LS_EDISP),
+                                    out.at<double>(LS_SP), out.at<double>(LS_EP), out.at<double>(LS_LE),
+                                    out.at<double>(LS_ANGLE), out.at<double>(LS_S2), out.at<int32_t>(LS_LEVEL),
+                                    out.at<uint8_t>(LS_DESC), out.at<int32_t>(LS_SRC), counts, out_off, cams);
     return cudaGetLastError();
 }
 

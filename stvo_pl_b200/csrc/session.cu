@@ -10,42 +10,38 @@ namespace plstvo {
 namespace {
 
 constexpr int GATHER_THREADS = 256;
-constexpr int GATHER_ARRAYS = 10;   // PrevRows: 3 point arrays, 7 line arrays
 
-struct GatherArrays {
-    const uint32_t* src[GATHER_ARRAYS];
-    uint32_t* dst[GATHER_ARRAYS];
+constexpr bool lifted_rows_are_words() {
+    for (int k = 0; k < N_LIFT; ++k)
+        if (REC_BYTES[k] % 4) return false;
+    return true;
+}
+static_assert(lifted_rows_are_words(), "the gather copies 4-byte words");
+
+struct GatherArrays {   // arrays 0 .. n_pt - 1 hold point rows, n_pt .. n - 1 line rows
+    int n, n_pt;
+    const uint32_t* src[N_LIFT];
+    uint32_t* dst[N_LIFT];
+    int words[N_LIFT];   // 4-byte words per row
 };
-
-// 4-byte words per row of each PrevRows array, points first
-__constant__ int c_words[GATHER_ARRAYS] = {6, 2, 8, 4, 4, 6, 6, 2, 1, 8};
 
 // One block per segment: every word of the segment's point rows, then of its line rows, is copied unchanged.  Integer
 // copies only (no arithmetic on the values), so the kept records are the lift kernels' bytes.
-__global__ void __launch_bounds__(GATHER_THREADS) session_gather_kernel(GatherArrays a, const GatherSeg* __restrict__ segs) {
+__global__ void __launch_bounds__(GATHER_THREADS) session_gather_kernel(GatherArrays a, const GatherSeg* __restrict__ segs,
+                                                                        const PlKeyframeResult* __restrict__ gate) {
+    if (gate && !gate[blockIdx.x].new_kf) return;
     const GatherSeg g = segs[blockIdx.x];
 #pragma unroll 1
-    for (int k = 0; k < GATHER_ARRAYS; ++k) {
-        const bool pt = k < 3;
+    for (int k = 0; k < a.n; ++k) {
+        const bool pt = k < a.n_pt;
         const int n = pt ? g.n_pt : g.n_ls;
         if (n == 0) continue;
-        const int w = c_words[k];
+        const int w = a.words[k];
         const size_t words = (size_t)n * w;
         const uint32_t* __restrict__ src = a.src[k] + (size_t)(pt ? g.src_pt : g.src_ls) * w;
         uint32_t* __restrict__ dst = a.dst[k] + (size_t)(pt ? g.dst_pt : g.dst_ls) * w;
         for (size_t i = threadIdx.x; i < words; i += GATHER_THREADS) dst[i] = src[i];
     }
-}
-
-GatherArrays gather_arrays(const PrevRows& s, const PrevRows& d) {
-    GatherArrays a;
-    const void* sp[GATHER_ARRAYS] = {s.ptP, s.pts2, s.pdesc, s.spl, s.epl, s.sP, s.eP, s.s2, s.lev, s.ldesc};
-    void* dp[GATHER_ARRAYS] = {d.ptP, d.pts2, d.pdesc, d.spl, d.epl, d.sP, d.eP, d.s2, d.lev, d.ldesc};
-    for (int k = 0; k < GATHER_ARRAYS; ++k) {
-        a.src[k] = static_cast<const uint32_t*>(sp[k]);
-        a.dst[k] = static_cast<uint32_t*>(dp[k]);
-    }
-    return a;
 }
 
 // updateFrame of one stream after a session-run step (src/stereoFrameHandler.cpp:62-86, :317-326, :377-378), as
@@ -89,9 +85,20 @@ size_t meta_others(const PlStereoSession* ss) { return meta_named(ss) + (size_t)
 
 }  // namespace
 
-cudaError_t launch_session_gather(const PrevRows& src, const PrevRows& dst, const GatherSeg* segs, int n_segs, cudaStream_t s) {
+cudaError_t launch_session_gather(const RecPtrs& src, const RecPtrs& dst, bool prev_role, const GatherSeg* segs, int n_segs,
+                                  cudaStream_t s, const PlKeyframeResult* gate) {
     if (n_segs <= 0) return cudaSuccess;
-    session_gather_kernel<<<n_segs, GATHER_THREADS, 0, s>>>(gather_arrays(src, dst), segs);
+    GatherArrays a;
+    a.n = prev_role ? N_PREV : N_LIFT;
+    a.n_pt = 0;
+    for (int j = 0; j < a.n; ++j) {
+        const int k = prev_role ? PREV_ROLE[j] : j;
+        a.n_pt += rec_is_point(k);
+        a.src[j] = src.at<const uint32_t>(k);
+        a.dst[j] = dst.at<uint32_t>(k);
+        a.words[j] = REC_BYTES[k] / 4;
+    }
+    session_gather_kernel<<<n_segs, GATHER_THREADS, 0, s>>>(a, segs, gate);
     return cudaGetLastError();
 }
 
@@ -106,32 +113,27 @@ cudaError_t SessionPool::ensure(size_t n_pt, size_t n_ls) {
     if (buf.p && n_pt <= cap_pt && n_ls <= cap_ls) return cudaSuccess;
     const size_t want_pt = std::max(n_pt + n_pt / 4, cap_pt) + 64, want_ls = std::max(n_ls + n_ls / 4, cap_ls) + 64;
     Arena a;
-    const size_t o_P = a.take(want_pt * 24), o_s2 = a.take(want_pt * 8), o_d = a.take(want_pt * 32);
-    const size_t o_spl = a.take(want_ls * 16), o_epl = a.take(want_ls * 16), o_sP = a.take(want_ls * 24);
-    const size_t o_eP = a.take(want_ls * 24), o_ls2 = a.take(want_ls * 8), o_lev = a.take(want_ls * 4);
-    const size_t o_ld = a.take(want_ls * 32);
+    size_t off[N_REC];
+    for (int k : PREV_ROLE) off[k] = a.take((rec_is_point(k) ? want_pt : want_ls) * (size_t)REC_BYTES[k]);
     cap_pt = cap_ls = 0;
-    rows = PrevRows{};
+    rows = RecPtrs{};
     if (const cudaError_t e = a.alloc(buf)) return e;
-    rows.ptP = a.f64(o_P); rows.pts2 = a.f64(o_s2); rows.pdesc = a.u8(o_d);
-    rows.spl = a.f64(o_spl); rows.epl = a.f64(o_epl); rows.sP = a.f64(o_sP); rows.eP = a.f64(o_eP); rows.s2 = a.f64(o_ls2);
-    rows.lev = a.i32(o_lev); rows.ldesc = a.u8(o_ld);
+    for (int k : PREV_ROLE) rows.p[k] = a.u8(off[k]);
     cap_pt = want_pt;
     cap_ls = want_ls;
     return cudaSuccess;
 }
 
-const int SessionRetained::row_bytes[SessionRetained::N_ARRAYS] = {16, 8, 24, 8, 4, 32, 4,
-                                                                   16, 16, 8, 8, 24, 24, 24, 8, 8, 4, 32, 4,
-                                                                   4, 1, 4, 1};
-
 cudaError_t SessionRetained::lay_out(size_t new_pt, size_t new_ls, size_t kept_pt, size_t kept_ls) {
     Arena a;
-    for (int k = 0; k < N_ARRAYS; ++k) {
+    size_t off[N_REC];
+    for (int k = 0; k < N_REC; ++k) {
         rows[k] = k < LS_SPL ? new_pt : k < M12_PT ? new_ls : (k == M12_PT || k == INL_PT) ? kept_pt : kept_ls;
-        off[k] = a.take(rows[k] * (size_t)row_bytes[k]);
+        off[k] = a.take(rows[k] * (size_t)REC_BYTES[k]);
     }
-    return a.alloc(buf);
+    const cudaError_t e = a.alloc(buf);
+    rec = arena_records(a, off, 0, N_REC);
+    return e;
 }
 
 int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s) {
@@ -179,9 +181,9 @@ int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, con
     return 0;
 }
 
-int session_gather_named(PlContext* ctx, PlStereoSession* ss, const PrevRows& ws_rows, cudaStream_t s) {
+int session_gather_named(PlContext* ctx, PlStereoSession* ss, const RecPtrs& ws_rows, cudaStream_t s) {
     const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_named(ss));
-    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ws_rows, segs, ss->n, s));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ws_rows, true, segs, ss->n, s));
     ctx->launches++;
     return 0;
 }
@@ -189,7 +191,7 @@ int session_gather_named(PlContext* ctx, PlStereoSession* ss, const PrevRows& ws
 int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s) {
     if (!ss->n_others) return 0;
     const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_others(ss));
-    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ss->pool[ss->cur ^ 1].rows, segs, ss->n_others, s));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ss->pool[ss->cur ^ 1].rows, true, segs, ss->n_others, s));
     ctx->launches++;
     return 0;
 }

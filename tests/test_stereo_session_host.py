@@ -70,13 +70,26 @@ def test_session_create_parameter_order():
                          C.POINTER(T.PlStereoConfig), C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlLsdConfig)]
 
 
-def test_kept_record_sizes_in_the_header():
-    """The header states bytes per kept point and line; they are the previous-frame-role record sizes."""
+def test_header_record_sizes_match_the_record_table(tmp_path):
+    """The header states bytes per kept point and line, per retained point and line, and per retained tracker row; they are
+    the sizes the record table (csrc/records.h) gives the previous-frame role, the lifted records and the m12 / inlier rows."""
     txt = re.sub(r"\s*\n\s*\*?\s*", " ", open(HEADER).read())
     assert "per kept stereo point 64 bytes" in txt and "per kept stereo line 124 bytes" in txt
-    assert 24 + 8 + 32 == 64 and 16 + 16 + 24 + 24 + 8 + 4 + 32 == 124
-    host = open(os.path.join(ROOT, "stvo_pl_b200", "csrc", "host.cuh")).read()
-    assert "SESSION_PT_BYTES = 24 + 8 + 32" in host and "SESSION_LS_BYTES = 16 + 16 + 24 + 24 + 8 + 4 + 32" in host
+    assert "(96 bytes per stereo point, 176 per stereo line)" in txt and "(5 bytes per kept row)" in txt
+    src = tmp_path / "sizes.cpp"
+    src.write_text('''#include <cstdio>
+#include "records.h"
+using namespace plstvo;
+int main() {
+    std::printf("%d %d %d %d %d %d\\n", prev_row_bytes(true), prev_row_bytes(false), rec_row_bytes(PT_PL, LS_SPL),
+                rec_row_bytes(LS_SPL, N_LIFT), rec_row_bytes(M12_PT, M12_LS), rec_row_bytes(M12_LS, N_REC));
+}
+''')
+    exe = str(tmp_path / "sizes")
+    subprocess.run(["g++", "-std=c++17", "-Wall", "-Werror", "-I", os.path.join(ROOT, "stvo_pl_b200", "csrc"), str(src),
+                    "-o", exe], check=True)
+    out = subprocess.run([exe], capture_output=True, text=True, check=True).stdout.split()
+    assert out == ["64", "124", "96", "176", "5", "5"], out
 
 
 def test_streams_example_compiles_and_links(tmp_path):
