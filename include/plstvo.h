@@ -387,6 +387,24 @@ int plstvo_lsd_detect_batch(PlContext* ctx, const PlLsdConfig* cfg, int n_img, i
 /* Device time of the last plstvo_lsd_detect_batch on this context, ms: [0] blur and resize, [1] gradient and seed order,
  * [2] region growing, [3] the host's region angles, [4] rectangles. */
 int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5);
+/* The KeyLine step of the reference's FLD line branch (Config::useFLDLines, src/stereoFrame.cpp:260-299) for one image of
+ * width x height: seg [n_seg][4] is cv::ximgproc::FastLineDetector::detect's output on fld_img, as Vec4f (start x, y, end
+ * x, y), in its order.  The caller runs FLD: createFastLineDetector(min_line_length * min(width, height)) on fld_img, the
+ * grey image, or for a colour image cvtColor(img, COLOR_RGB2GRAY) (the branch's CV_RGB2GRAY).  Where n_seg > n_features and
+ * n_features != 0 the segments are sorted by sort_flines_by_length (include/auxiliar.h:149-154: the double
+ * sqrt(pow(dx, 2.0) + pow(dy, 2.0)), strict >, libstdc++'s std::sort on the given order, so equal lengths land where the
+ * reference puts them) and truncated to n_features.  Each kept segment becomes a key line, byte for byte the reference's:
+ * kl_seg the segment as given (no clamp to the image: the LSD branch's checkLineExtremes does not apply), kl_length
+ * (float)sqrt(pow(dx, 2) + pow(dy, 2)), kl_angle atan2 of the float differences (std::atan2(float, float), glibc's
+ * atan2f), kl_response length / max(width, height), kl_npix cv::LineIterator(fld_img, start, end).count on the unclamped
+ * endpoints (after LineIterator's own clipping; 0 for a segment whose rounded endpoints both leave the image on one side).
+ * Such a line is returned as the reference computes it, and plstvo_lbd_compute_batch and the sessions then refuse it
+ * (numOfPixels 1..32767), as the images calls do.  Any output may be NULL; the arrays hold min(n_seg, n_features) rows
+ * (n_seg where n_features is 0).  Host code, no context or GPU.  Returns the number of key lines; PLSTVO_E_INVALID for
+ * width or height outside 1..32767, n_features < 0, n_seg < 0, seg NULL with n_seg > 0, or a coordinate that is not finite or
+ * lies outside [-2^31, 2^31) (where cvRound, which LineIterator rounds with, leaves int; FastLineDetector never gives one). */
+int plstvo_fld_key_lines(int width, int height, int n_features, int n_seg, const float* seg, float* kl_seg, float* kl_angle,
+                         int32_t* kl_npix, float* kl_response, float* kl_length);
 
 /* ---- stereo images in, pose out: StereoFrame::extractStereoFeatures (src/stereoFrame.cpp:59-118, :182-243) with LSD left
  * to the caller, then matchStereoPoints / matchStereoLines, f2fTracking and optimizePose (plstvo_track_stereo_images_lsd_*
@@ -601,6 +619,25 @@ int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* s, int n, 
  * (initialize too, its tracking slot then empty). */
 int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* s, int n, const int32_t* ids, const PlStereoImages* frames,
                                  const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo);
+/* The reference's FLD line branch (use_fld_lines, src/stereoFrame.cpp:244-304) on a session: on != 0 makes _initialize,
+ * _insert, _run and _run_keyframes take each frame's key lines from the caller instead of running LSD, off (the state at
+ * creation) restores LSD.  Legal only while no stream holds a frame (PLSTVO_E_INVALID otherwise, the session unchanged), so
+ * every kept frame of a session was described one way; it works on _create and _create_cams sessions alike, and lcfg,
+ * checked at creation as before, is not read while it is on.
+ * With it on, wherever cfg->has_lines is set the frames' key-line fields (ll_off .. npix_r) are required and hold what the
+ * images call takes (plstvo_fld_key_lines' rows: sPointInOctave / ePointInOctave, angle, numOfPixels), frame-major for
+ * _initialize / _insert and step-major over the T n frames of a run, with plstvo_lbd_compute_batch's key-line checks
+ * (PLSTVO_E_INVALID for a missing or malformed field or a numOfPixels outside 1..32767; PLSTVO_E_TOO_LARGE for more than
+ * PLSTVO_MAX_FEATURES lines in one image); where has_lines is 0 they must be NULL (PLSTVO_E_INVALID).  Each such error
+ * leaves the session usable.  LSD does not run and LBD describes the given lines; a run describes all 2 n T images' lines in
+ * one LBD pass and keeps no LSD arena.  Contract: an insert equals plstvo_track_stereo_images_batch with the session's
+ * configs, prev = each named stream's kept images and key lines at their thresholds, curr = frames, the same priors; the
+ * runs equal T such inserts as plstvo_stereo_session_run states it.  Retention, _read, _read_keyframes (ls_src: the row
+ * in the caller's key lines of the image) work unchanged.
+ * A colour session computes the branch's fld_img = cvtColor(img, CV_RGB2GRAY) of each remapped (or unmapped) image beside
+ * the COLOR_BGR2GRAY copy ORB reads, in the same launch, and LBD reads it: one byte per pixel of the call more of the
+ * rectifier's staging. */
+int plstvo_stereo_session_use_fld_lines(PlContext* ctx, PlStereoSession* s, int on);
 
 /* ---- reading a session call's frames back: StereoFrame::stereo_pt / stereo_ls and StereoFrameHandler::matched_pt / _ls
  * of the last _initialize / _insert ----

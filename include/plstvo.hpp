@@ -221,6 +221,29 @@ inline int detectLSD(Context& c, const PlLsdConfig& cfg, const uint8_t* image, i
         return n;
     }
 }
+// The FLD branch's key lines of one width x height image (src/stereoFrame.cpp:260-299, plstvo_fld_key_lines): seg is
+// FastLineDetector::detect's vector<Vec4f> as [n][4] floats, in its order; the caller ran
+// createFastLineDetector(cfg.min_line_length * min(width, height)) on fld_img.  kl.seg, kl.angle and kl.octave (all 0) are
+// replaced by the key lines in the reference's order and kl.desc is cleared; num_pixels, response and length (if given)
+// likewise.  Host code.  Returns the line count.
+inline int fldKeyLines(int width, int height, int n_features, const std::vector<float>& seg, KeyLines& kl,
+                       std::vector<int32_t>& num_pixels, std::vector<float>* response = nullptr,
+                       std::vector<float>* length = nullptr) {
+    if (seg.size() % 4) throw Error(PLSTVO_E_INVALID, "fldKeyLines: seg must hold 4 floats per segment");
+    const int n = (int)(seg.size() / 4), m = n_features > 0 ? std::min(n, n_features) : n;
+    std::vector<float> resp((size_t)m), len((size_t)m);
+    kl.seg.resize(4 * (size_t)m);
+    kl.angle.resize((size_t)m);
+    num_pixels.resize((size_t)m);
+    const int k = plstvo_fld_key_lines(width, height, n_features, n, seg.data(), kl.seg.data(), kl.angle.data(),
+                                       num_pixels.data(), resp.data(), len.data());
+    if (k < 0) throw Error(k, "fldKeyLines: width or height outside 1..32767, or n_features < 0");
+    kl.octave.assign((size_t)k, 0);
+    kl.desc.clear();
+    if (response) *response = std::move(resp);
+    if (length) *length = std::move(len);
+    return k;
+}
 // One stereo frame as StereoFrame::extractStereoFeatures starts it (src/stereoFrame.cpp:59-118, :182-243): the two grey images
 // (row-major, width * height bytes each) and the key lines LSD kept on each (octave 0: start / end point [m][4], KeyLine::angle,
 // KeyLine::numOfPixels).  fast_th 0: the config's FAST threshold.
@@ -891,6 +914,10 @@ public:
         c_.check(plstvo_stereo_session_run_keyframes(c_.get(), s_, &h, &k, n, ids, T, &frames, fast_th0, priors, kf_state,
                                                      results, kf, fast_th, n_stereo));
     }
+    // plstvo_stereo_session_use_fld_lines: the reference's FLD line branch, before any stream is initialised.  On, every call
+    // takes each frame's key lines in frames' key-line fields (fldKeyLines' rows; step-major for run / runKeyframes) and
+    // LSD does not run.
+    void useFLDLines(bool on) { c_.check(plstvo_stereo_session_use_fld_lines(c_.get(), s_, on ? 1 : 0)); }
     // plstvo_stereo_session_retain: keep each following call's frames and matches for read() (off frees them)
     void retain(bool on) { c_.check(plstvo_stereo_session_retain(c_.get(), s_, on ? 1 : 0)); }
     // plstvo_stereo_session_read of the last call, into out's vectors sized from that call's n and n_stereo ([n][2] after an
@@ -995,6 +1022,32 @@ struct StereoImagesBatch {
         }
         th = fast_th;
         view = PlStereoImages{(int32_t)n, width, height, img_l.data(), img_r.data(), th.data()};
+    }
+    // the FLD branch's key lines of the packed frames: image k's FastLineDetector segments seg_l[k] / seg_r[k] ([m][4] floats,
+    // FLD's order) through fldKeyLines, into the view's key-line fields
+    std::vector<int32_t> ll_off, lr_off, npix_l, npix_r;
+    std::vector<float> seg_l, seg_r, angle_l, angle_r;
+    void addFLDLines(int width, int height, int n_features, const std::vector<std::vector<float>>& fl,
+                     const std::vector<std::vector<float>>& fr, const char* who) {
+        if (fl.size() != (size_t)view.B || fr.size() != (size_t)view.B)
+            throw Error(PLSTVO_E_INVALID, std::string(who) + ": one segment list per image");
+        ll_off.assign(1, 0); lr_off.assign(1, 0);
+        npix_l.clear(); npix_r.clear(); seg_l.clear(); seg_r.clear(); angle_l.clear(); angle_r.clear();
+        KeyLines kl;
+        std::vector<int32_t> npix;
+        for (size_t k = 0; k < fl.size(); ++k)
+            for (int side = 0; side < 2; ++side) {
+                fldKeyLines(width, height, n_features, (side ? fr : fl)[k], kl, npix);
+                std::vector<int32_t>& off = side ? lr_off : ll_off;
+                off.push_back(off.back() + (int32_t)npix.size());
+                (side ? seg_r : seg_l).insert((side ? seg_r : seg_l).end(), kl.seg.begin(), kl.seg.end());
+                (side ? angle_r : angle_l).insert((side ? angle_r : angle_l).end(), kl.angle.begin(), kl.angle.end());
+                (side ? npix_r : npix_l).insert((side ? npix_r : npix_l).end(), npix.begin(), npix.end());
+            }
+        view.ll_off = ll_off.data(); view.lr_off = lr_off.data();
+        view.seg_l = seg_l.data(); view.seg_r = seg_r.data();
+        view.angle_l = angle_l.data(); view.angle_r = angle_r.data();
+        view.npix_l = npix_l.data(); view.npix_r = npix_r.data();
     }
 };
 // the handler's ORB config: a frame's fast_th of 0 stands for the config's threshold; with that set to 0 too, every frame is
@@ -1146,7 +1199,8 @@ public:
                          const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc, int n_streams,
                          const HandlerConfig& hcfg = HandlerConfig{}, const Rectifier* rect = nullptr)
         : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, n_streams, rect),
-          streams_((size_t)n_streams), channels_(rect ? rect->channels() : 1) {
+          streams_((size_t)n_streams), channels_(rect ? rect->channels() : 1), lsd_nfeatures_(lc.n_features),
+          has_lines_(cfg.has_lines != 0) {
         for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
     }
     // One camera per stream, as one PinholeStereoCamera per StereoFrameHandler in the reference, and optionally one rectifier
@@ -1155,7 +1209,7 @@ public:
                          const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
                          const HandlerConfig& hcfg = HandlerConfig{}, const std::vector<const Rectifier*>& rects = {})
         : cam_(cams.at(0)), hcfg_(hcfg), session_(ctx, cams, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, rects),
-          streams_(cams.size()) {
+          streams_(cams.size()), lsd_nfeatures_(lc.n_features), has_lines_(cfg.has_lines != 0) {
         for (const Rectifier* r : rects)
             if (r) {
                 channels_ = r->channels();
@@ -1164,11 +1218,99 @@ public:
         for (Stream& s : streams_) s.orb_fast_th = hcfg_.orb_fast_th;
     }
 
+    // The reference's FLD line branch (use_fld_lines, StereoSession::useFLDLines), before any stream is initialised: on, every
+    // call takes each image's FastLineDetector segments (Segments: FLD's vector<Vec4f> as [m][4] floats, in its order, found on
+    // fld_img: the grey image, or cvtColor(img, CV_RGB2GRAY) of a colour one, rectified where the handler remaps) beside its
+    // images, through the overloads below, and runs fldKeyLines on them with lc.n_features; LSD does not run.  Where cfg has
+    // no lines the segments are not read.
+    using Segments = std::vector<float>;
+    void useFLDLines(bool on) {
+        session_.useFLDLines(on);
+        fld_ = on;
+    }
     // initialize(img_l[k], img_r[k], idx[k]) of stream ids[k], in one session call (idx optional)
     void initialize(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
                     const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
+        initialize(ids, img_l, img_r, nullptr, nullptr, idx);
+    }
+    // the same on the FLD branch: seg_l[k] / seg_r[k] are the segments of img_l[k] / img_r[k]
+    void initialize(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                    const std::vector<const uint8_t*>& img_r, const std::vector<Segments>& seg_l,
+                    const std::vector<Segments>& seg_r, const std::vector<int>& idx = {}) {
+        initialize(ids, img_l, img_r, &seg_l, &seg_r, idx);
+    }
+    // insertStereoPair(img_l[k], img_r[k], idx[k]) of stream ids[k]: f2fTracking of every named stream in one session call
+    void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                           const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
+        insertStereoPairs(ids, img_l, img_r, nullptr, nullptr, idx);
+    }
+    // the same on the FLD branch: seg_l[k] / seg_r[k] are the segments of img_l[k] / img_r[k]
+    void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                           const std::vector<const uint8_t*>& img_r, const std::vector<Segments>& seg_l,
+                           const std::vector<Segments>& seg_r, const std::vector<int>& idx = {}) {
+        insertStereoPairs(ids, img_l, img_r, &seg_l, &seg_r, idx);
+    }
+    // T frames per named stream in one session call (plstvo_stereo_session_run): img_l[t][k] / img_r[t][k] is stream ids[k]'s
+    // frame of step t.  Each stream then stands as after T rounds of insertStereoPairs, optimizePose and updateFrame: its
+    // prev_frame holds the last step's published pose, orb_fast_th the next frame's threshold, n_inliers* and n_stereo the
+    // last step's, and per-frame calls can follow.  results (optional) receives [T][n] results.  The key-frame test is not
+    // run here: the overload below runs it inside the call.  keepFeatures' arrays hold the last step.
+    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
+                               const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results = nullptr) {
+        run(ids, img_l, img_r, nullptr, nullptr, results, nullptr, nullptr);
+    }
+    // the same on the FLD branch: seg_l[t][k] / seg_r[t][k] are the segments of img_l[t][k] / img_r[t][k]
+    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
+                               const std::vector<std::vector<const uint8_t*>>& img_r,
+                               const std::vector<std::vector<Segments>>& seg_l, const std::vector<std::vector<Segments>>& seg_r,
+                               std::vector<PlPoseResult>* results = nullptr) {
+        run(ids, img_l, img_r, &seg_l, &seg_r, results, nullptr, nullptr);
+    }
+    // A key frame of the key-frame overloads: stream id, step, and with keepFeatures its new stereo points and lines (pose
+    // fields as published, Tfw before currFrameIsKF's reset)
+    struct KeyFrame {
+        int stream = 0, step = 0;
+        StereoFrame frame;
+    };
+    // The same with the PL-SLAM test (plstvo_stereo_session_run_keyframes): per stream and step, needNewKF after optimizePose
+    // and currFrameIsKF where it fires, from and back into each stream's kf.  A stream whose last step was a key frame has
+    // prev_frame.Tfw = I and Tfw_cov = I, as currFrameIsKF leaves curr_frame.  Returns the [T][n] tests; results (optional)
+    // receives [T][n] results, and keyframes (optional, with keepFeatures on) each key frame in (step, call position) order.
+    std::vector<PlKeyframeResult> insertStereoSequences(const std::vector<int32_t>& ids,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_l,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_r,
+                                                        std::vector<PlPoseResult>* results, std::vector<KeyFrame>* keyframes) {
+        std::vector<PlKeyframeResult> kf;
+        run(ids, img_l, img_r, nullptr, nullptr, results, &kf, keyframes);
+        return kf;
+    }
+    // the same on the FLD branch, segments as in the plain FLD overload
+    std::vector<PlKeyframeResult> insertStereoSequences(const std::vector<int32_t>& ids,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_l,
+                                                        const std::vector<std::vector<const uint8_t*>>& img_r,
+                                                        const std::vector<std::vector<Segments>>& seg_l,
+                                                        const std::vector<std::vector<Segments>>& seg_r,
+                                                        std::vector<PlPoseResult>* results, std::vector<KeyFrame>* keyframes) {
+        std::vector<PlKeyframeResult> kf;
+        run(ids, img_l, img_r, &seg_l, &seg_r, results, &kf, keyframes);
+        return kf;
+    }
+
+private:
+    // the FLD branch's key lines of the packed frames (fl / fr null: none given)
+    void attachLines(const std::vector<Segments>* fl, const std::vector<Segments>* fr, const char* who) {
+        if (!fl != !fr) throw Error(PLSTVO_E_INVALID, std::string(who) + ": segments for both sides or neither");
+        if (fl && !fld_) throw Error(PLSTVO_E_INVALID, std::string(who) + ": segments given: useFLDLines(true) first");
+        if (!fl && fld_ && has_lines_)
+            throw Error(PLSTVO_E_INVALID, std::string(who) + ": the FLD branch takes each image's segments");
+        if (fl && has_lines_) pack_.addFLDLines(cam_.width, cam_.height, lsd_nfeatures_, *fl, *fr, who);
+    }
+    void initialize(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
+                    const std::vector<const uint8_t*>& img_r, const std::vector<Segments>* fl, const std::vector<Segments>* fr,
+                    const std::vector<int>& idx) {
         const std::vector<int32_t> th(ids.size(), hcfg_.orb_fast_th);   // :38
         pack_.pack(cam_.width, cam_.height, channels_, img_l, img_r, th, "StereoStreamsHandler::initialize");
+        attachLines(fl, fr, "StereoStreamsHandler::initialize");
         std::vector<int32_t> ns(2 * ids.size());
         session_.initialize((int)ids.size(), ids.data(), pack_.view, ns.data());
         if (keep_) session_.read((int)ids.size(), ns.data(), false, read_);
@@ -1189,9 +1331,9 @@ public:
             s.has_prev = true;
         }
     }
-    // insertStereoPair(img_l[k], img_r[k], idx[k]) of stream ids[k]: f2fTracking of every named stream in one session call
     void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
-                           const std::vector<const uint8_t*>& img_r, const std::vector<int>& idx = {}) {
+                           const std::vector<const uint8_t*>& img_r, const std::vector<Segments>* fl,
+                           const std::vector<Segments>* fr, const std::vector<int>& idx) {
         std::vector<int32_t> th;
         std::vector<PlPrior> priors;
         for (int32_t id : ids) {
@@ -1201,6 +1343,7 @@ public:
             priors.push_back(priorOf(s.prev_frame));
         }
         pack_.pack(cam_.width, cam_.height, channels_, img_l, img_r, th, "StereoStreamsHandler::insertStereoPairs");
+        attachLines(fl, fr, "StereoStreamsHandler::insertStereoPairs");
         std::vector<PlPoseResult> res(ids.size());
         std::vector<int32_t> ns(4 * ids.size());
         session_.insert((int)ids.size(), ids.data(), pack_.view, priors.data(), res.data(), ns.data());
@@ -1231,33 +1374,8 @@ public:
             s.n_inliers = s.n_inliers_pt + s.n_inliers_ls;
         }
     }
-    // T frames per named stream in one session call (plstvo_stereo_session_run): img_l[t][k] / img_r[t][k] is stream ids[k]'s
-    // frame of step t.  Each stream then stands as after T rounds of insertStereoPairs, optimizePose and updateFrame: its
-    // prev_frame holds the last step's published pose, orb_fast_th the next frame's threshold, n_inliers* and n_stereo the
-    // last step's, and per-frame calls can follow.  results (optional) receives [T][n] results.  The key-frame test is not
-    // run here: the overload below runs it inside the call.  keepFeatures' arrays hold the last step.
-    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
-                               const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results = nullptr) {
-        run(ids, img_l, img_r, results, nullptr, nullptr);
-    }
-    // A key frame of that overload: stream id, step, and with keepFeatures its new stereo points and lines (pose fields as
-    // published, Tfw before currFrameIsKF's reset)
-    struct KeyFrame {
-        int stream = 0, step = 0;
-        StereoFrame frame;
-    };
-    // The same with the PL-SLAM test (plstvo_stereo_session_run_keyframes): per stream and step, needNewKF after optimizePose
-    // and currFrameIsKF where it fires, from and back into each stream's kf.  A stream whose last step was a key frame has
-    // prev_frame.Tfw = I and Tfw_cov = I, as currFrameIsKF leaves curr_frame.  Returns the [T][n] tests; results (optional)
-    // receives [T][n] results, and keyframes (optional, with keepFeatures on) each key frame in (step, call position) order.
-    std::vector<PlKeyframeResult> insertStereoSequences(const std::vector<int32_t>& ids,
-                                                        const std::vector<std::vector<const uint8_t*>>& img_l,
-                                                        const std::vector<std::vector<const uint8_t*>>& img_r,
-                                                        std::vector<PlPoseResult>* results, std::vector<KeyFrame>* keyframes) {
-        std::vector<PlKeyframeResult> kf;
-        run(ids, img_l, img_r, results, &kf, keyframes);
-        return kf;
-    }
+
+public:
     void optimizePose(int id) {                          // :307-392
         Stream& s = at(id);
         publishPose(s.result, s.curr_frame);
@@ -1285,9 +1403,11 @@ public:
     const StereoSession& session() const { return session_; }
 
 private:
-    // the two insertStereoSequences: kf null runs plstvo_stereo_session_run, else plstvo_stereo_session_run_keyframes
+    // the insertStereoSequences: kf null runs plstvo_stereo_session_run, else plstvo_stereo_session_run_keyframes; fl / fr
+    // (FLD branch) [T][n] segments
     void run(const std::vector<int32_t>& ids, const std::vector<std::vector<const uint8_t*>>& img_l,
-             const std::vector<std::vector<const uint8_t*>>& img_r, std::vector<PlPoseResult>* results,
+             const std::vector<std::vector<const uint8_t*>>& img_r, const std::vector<std::vector<Segments>>* fl,
+             const std::vector<std::vector<Segments>>* fr, std::vector<PlPoseResult>* results,
              std::vector<PlKeyframeResult>* kf, std::vector<KeyFrame>* keyframes) {
         const size_t n = ids.size(), T = img_l.size();
         if (img_r.size() != T) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: T differs between sides");
@@ -1313,6 +1433,16 @@ private:
         if (T == 0 || n == 0) return;
         pack_.pack(cam_.width, cam_.height, channels_, l, r, std::vector<int32_t>(n * T, 0),
                    "StereoStreamsHandler::insertStereoSequences");
+        std::vector<Segments> sl, sr;   // step-major, as the images
+        if (fl && fr) {
+            if (fl->size() != T || fr->size() != T)
+                throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: one segment list per image");
+            for (size_t t = 0; t < T; ++t) {
+                sl.insert(sl.end(), (*fl)[t].begin(), (*fl)[t].end());
+                sr.insert(sr.end(), (*fr)[t].begin(), (*fr)[t].end());
+            }
+        }
+        attachLines(fl ? &sl : nullptr, fr ? &sr : nullptr, "StereoStreamsHandler::insertStereoSequences");
         PlStereoImages frames = pack_.view;
         frames.fast_th = nullptr;
         std::vector<PlPoseResult> res(n * T);
@@ -1397,6 +1527,9 @@ private:
     StereoSession session_;
     std::vector<Stream> streams_;
     int channels_ = 1;   // bytes per pixel of the images: the rectifier's channels
+    int lsd_nfeatures_ = 0;   // lsd_nfeatures, the FLD branch's truncation
+    bool has_lines_ = true;
+    bool fld_ = false;        // useFLDLines
     detail::StereoImagesBatch pack_;
     bool keep_ = false;
     StereoSession::Frames read_;

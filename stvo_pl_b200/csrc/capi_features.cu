@@ -629,6 +629,22 @@ int line_iterator_count(int W, int H, const float* e) {
     return (int)std::max(std::llabs(x2 - x1), std::llabs(y2 - y1)) + 1;
 }
 
+// The KeyLine both line branches build from a segment e (start x, y, end x, y) of a W x H image, octave 0: lineLength
+// (float)sqrt(pow(dx, 2) + pow(dy, 2)) of the float differences (the squares are exact in double), angle atan2 of the float
+// differences, response lineLength / max(cols, rows), numOfPixels LineIterator's count on e.  Unqualified atan2 of two
+// floats binds to std::atan2(float, float) in both branches (LSDDetector_custom.cpp and stereoFrame.cpp include <math.h>'s
+// C++ form and `using namespace std`), the C library's atan2f, evaluated here with the same library.
+KeyLine key_line(int W, int H, const float* e) {
+    KeyLine kl;
+    memcpy(kl.seg, e, sizeof kl.seg);
+    const double dx = (double)(e[0] - e[2]), dy = (double)(e[1] - e[3]);
+    kl.length = (float)sqrt(dx * dx + dy * dy);
+    kl.npix = line_iterator_count(W, H, e);
+    kl.angle = atan2f(e[3] - e[1], e[2] - e[0]);
+    kl.response = kl.length / (float)std::max(W, H);
+    return kl;
+}
+
 // LSDDetectorC::detectImpl's KeyLine step for one octave (3rdparty/line_descriptor/src/LSDDetector_custom.cpp:266-308)
 // and detectLineFeatures' sort-and-truncate (src/stereoFrame.cpp:232-241), on the host: a few hundred lines per image, and
 // atan2f is the C library's.  std::sort is the reference's own (libstdc++) sort, so equal responses keep its order.
@@ -641,21 +657,34 @@ void lsd_keylines(int W, int H, const float4* raw, int n, double min_length, int
             if (e[c] < 0) e[c] = 0;
             if (e[c] >= lim) e[c] = (float)lim - 1.0f;
         }
-        const double dx = (double)(e[0] - e[2]), dy = (double)(e[1] - e[3]);
-        const double length = (float)sqrt(dx * dx + dy * dy);   // (float)sqrt(pow(.., 2) + pow(.., 2)); the squares are exact
-        if (!(length > min_length)) continue;
-        KeyLine kl;
-        memcpy(kl.seg, e, sizeof e);
-        kl.length = (float)length;
-        kl.npix = line_iterator_count(W, H, e);
-        kl.angle = atan2f(e[3] - e[1], e[2] - e[0]);
-        kl.response = kl.length / (float)std::max(W, H);
+        const KeyLine kl = key_line(W, H, e);
+        if (!((double)kl.length > min_length)) continue;
         out.push_back(kl);
     }
     if ((int)out.size() > n_features && n_features != 0) {
         std::sort(out.begin(), out.end(), [](const KeyLine& a, const KeyLine& b) { return a.response > b.response; });
         out.resize((size_t)n_features);
     }
+}
+
+// detectLineFeatures' FLD branch after fld->detect (src/stereoFrame.cpp:260-299): FastLineDetector's segments seg [n][4]
+// sorted by sort_flines_by_length (include/auxiliar.h:149-154: sqrt(pow(d, 2.0) + ..) in double, strict >) where there are
+// more than n_features (!= 0) of them, truncated, then each made a KeyLine on the unclamped endpoints.  The sort runs on the
+// segments in the caller's order with libstdc++'s std::sort, as the reference sorts its vector<Vec4f>, so equal lengths
+// land where the reference puts them.
+void fld_keylines(int W, int H, const float* seg, int n, int n_features, std::vector<KeyLine>& out) {
+    struct Seg {
+        float v[4];
+    };
+    std::vector<Seg> s((size_t)n);
+    if (n) memcpy(s.data(), seg, (size_t)n * sizeof(Seg));
+    if (n > n_features && n_features != 0) {
+        auto len = [](const Seg& a) { return sqrt(pow(a.v[0] - a.v[2], 2.0) + pow(a.v[1] - a.v[3], 2.0)); };
+        std::sort(s.begin(), s.end(), [&](const Seg& a, const Seg& b) { return len(a) > len(b); });
+        s.resize((size_t)n_features);
+    }
+    out.clear();
+    for (const Seg& e : s) out.push_back(key_line(W, H, e.v));
 }
 
 int lsd_check_config(PlContext* ctx, const PlLsdConfig* c) {
@@ -848,6 +877,21 @@ int plstvo_lsd_kernel_times(PlContext* ctx, float* ms5) {
     return 0;
 }
 
+int plstvo_fld_key_lines(int width, int height, int n_features, int n_seg, const float* seg, float* kl_seg, float* kl_angle,
+                         int32_t* kl_npix, float* kl_response, float* kl_length) {
+    if (width < 1 || width > 32767 || height < 1 || height > 32767 || n_features < 0 || n_seg < 0 || (n_seg && !seg))
+        return PLSTVO_E_INVALID;
+    // LineIterator rounds with cvRound, which equals lrintf only on finite values inside int (it gives INT_MIN elsewhere), and
+    // the sort needs ordered lengths: such coordinates are refused rather than counted differently
+    for (size_t k = 0; k < 4 * (size_t)n_seg; ++k)
+        if (!(seg[k] >= -2147483648.0f && seg[k] < 2147483648.0f)) return PLSTVO_E_INVALID;
+    std::vector<KeyLine> kls;
+    fld_keylines(width, height, seg, n_seg, n_features, kls);
+    const std::vector<std::vector<KeyLine>> one{std::move(kls)};
+    lsd_rows(one, 0, 1, kl_seg, kl_angle, kl_npix, kl_response, kl_length);
+    return (int)one[0].size();
+}
+
 /* ---- stereo images -> pose: ORB, LSD and LBD feed the stereo step and the tracker without leaving HBM ---- */
 namespace {
 // LSD's key lines of nblk blocks of nf images each, the arrays a LineSrc per block points at
@@ -940,13 +984,16 @@ int images_check(PlContext* ctx, int W, int H, bool pts, bool lns, const PlStere
 }
 
 // Enqueues on s the grey device copy of n_img raw images (parts) in blocks of n images alternating left, right: the remap /
-// colour conversion of rect, or with a session of per-stream rectifiers, stream ids[k]'s rectifier for image k of each block
+// colour conversion of rect, or with a session of per-stream rectifiers, stream ids[k]'s rectifier for image k of each block.
+// A colour session on the FLD branch with lines also gets the RGB2GRAY plane LBD reads (*d_lbd; else null).
 int rectify_call(PlContext* ctx, const PlRectifier* rect, const PlStereoSession* session, const int32_t* ids, int n, int n_img,
-                 const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out) {
+                 const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out, const uint8_t** d_lbd) {
     std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
     if (session && !session->rects.empty())
         for (int k = 0; k < n; ++k) call_rects.push_back(session->rects[(size_t)ids[k]]);
-    return rectify_enqueue(ctx, rect, n_img, n, parts, s, d_out, call_rects.empty() ? nullptr : call_rects.data());
+    const bool rgb = session && session->fld && session->cfg.has_lines && rect->channels > 1;
+    return rectify_enqueue(ctx, rect, n_img, n, parts, s, d_out, call_rects.empty() ? nullptr : call_rects.data(),
+                           rgb ? d_lbd : nullptr);
 }
 }  // namespace
 
@@ -1023,9 +1070,11 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const float* d_seg = nullptr;
     const uint8_t* d_ldesc = nullptr;
     const uint8_t* d_images = nullptr;   // the device copy of the images the line stages read (null: LBD uploads its own)
+    const uint8_t* d_rgb = nullptr;      // a colour FLD session's RGB2GRAY plane, which LBD reads instead
     cudaEvent_t images_ready = nullptr;
     auto enqueue_lbd = [&]() -> int {
-        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_images, images_ready, stage_parts, ctx->s_alt, &d_seg, &d_ldesc))
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_rgb ? d_rgb : d_images, images_ready, stage_parts, ctx->s_alt, &d_seg,
+                                       &d_ldesc))
             return rc;
         CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
         return 0;
@@ -1049,7 +1098,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     cudaEvent_t rectified_ready = nullptr;
     if (rect && (pts || lns)) {
         if (const int rc = rectify_call(ctx, rect, session, session ? session->ids : nullptr, NF, n_img, iparts, ctx->s_main,
-                                        &rectified))
+                                        &rectified, &d_rgb))
             return rc;
         rectified_ready = next_event(ctx);
         CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
@@ -1384,9 +1433,13 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
     if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
     if (const int rc = session_check_ids(ctx, ss, track, n, ids)) return rc;
+    if (ss->fld && !ss->cfg.has_lines && key_lines_given(frames))
+        return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the session has no lines");
     session_begin(ss, track, n, ids, n_stereo);
-    const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, true, ss->has_lc ? &ss->lc : nullptr,
-                                       frames, nullptr, priors, results, n_stereo, false, ss->rect, ss);
+    // the FLD branch: the caller's key lines (the images call's checks), LSD and its config unused
+    const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, !ss->fld,
+                                       !ss->fld && ss->has_lc ? &ss->lc : nullptr, frames, nullptr, priors, results, n_stereo,
+                                       false, ss->rect, ss);
     if (rc == 0) {
         session_commit(ss);
         if (ss->retain) {
@@ -1408,6 +1461,17 @@ int plstvo_stereo_session_initialize(PlContext* ctx, PlStereoSession* ss, int n,
 int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* ss, int n, const int32_t* ids, const PlStereoImages* frames,
                                  const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
     return session_call(ctx, ss, true, n, ids, frames, priors, results, n_stereo);
+}
+
+int plstvo_stereo_session_use_fld_lines(PlContext* ctx, PlStereoSession* ss, int on) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    for (uint8_t l : ss->live)
+        if (l) return fail(ctx, PLSTVO_E_INVALID, "a stream holds a frame: switch the line branch before any stream is initialised");
+    ss->fld = on != 0;
+    return 0;
 }
 
 /* ---- stereo sessions: the handler's frame loop over T frames per stream in one call ---- */
@@ -1440,8 +1504,12 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (T < 0) return fail(ctx, PLSTVO_E_INVALID, "negative T");
     if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
     if ((long long)frames->B != (long long)T * n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from T * n");
-    if (frames->fast_th || key_lines_given(frames))
+    const bool lns = ss->cfg.has_lines != 0, fld = ss->fld && lns;   // fld: the caller's key lines, step-major
+    if (!ss->fld && (frames->fast_th || key_lines_given(frames)))
         return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th and the key-line fields must be null: the run sets its thresholds and detects its key lines");
+    if (ss->fld && frames->fast_th) return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th must be null: the run sets its thresholds");
+    if (ss->fld && !lns && key_lines_given(frames))
+        return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the session has no lines");
     const PlOrbDetectConfig* oc = &ss->oc;
     std::vector<int32_t> th0((size_t)2 * n);   // row 0 of the threshold table, [left n][right n]
     for (int k = 0; k < n; ++k) {
@@ -1460,7 +1528,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (oc->n_features > PLSTVO_MAX_FEATURES)
         return fail(ctx, PLSTVO_E_INVALID, "ocfg.n_features exceeds PLSTVO_MAX_FEATURES: a step could fail on a feature limit");
     const PlCamera& cam = ss->cam;
-    const bool pts = ss->cfg.has_points != 0, lns = ss->cfg.has_lines != 0;
+    const bool pts = ss->cfg.has_points != 0;
     const int W = cam.width, H = cam.height, n_img = 2 * n * T;
     // the insert's checks (track_images_run) before any work: ORB's and LSD's plans, image sizes and pointers
     if (const int rc = orb_detect_check(ctx, oc)) return rc;
@@ -1473,7 +1541,25 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     }
     LsdLaunch lsd{};
     if (n > 0) {   // the session was created with an LSD config wherever it has lines
-        if (const int rc = images_check(ctx, W, H, pts, lns, &frames, 1, lns ? &ss->lc : nullptr, n_img, lsd)) return rc;
+        if (const int rc = images_check(ctx, W, H, pts, lns, &frames, 1, lns && !fld ? &ss->lc : nullptr, n_img, lsd)) return rc;
+    }
+    // the caller's key lines as line blocks: 2 t, 2 t + 1 are step t's left and right images, offsets rebased to 0
+    const int nblk = 2 * T;
+    std::vector<LineSrc> lsrc;
+    DetectedLines det;
+    if (fld && n > 0) {
+        const LineSrc given[2] = {LineSrc{n * T, frames->ll_off, frames->seg_l, frames->angle_l, frames->npix_l},
+                                  LineSrc{n * T, frames->lr_off, frames->seg_r, frames->angle_r, frames->npix_r}};
+        for (const LineSrc& l : given)
+            if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        det.off.assign((size_t)nblk, {});
+        for (int b = 0; b < nblk; ++b) {
+            const LineSrc& l = given[b % 2];
+            const int32_t* o = l.off + (size_t)(b / 2) * n;
+            std::vector<int32_t>& off = det.off[(size_t)b];
+            for (int i = 0; i <= n; ++i) off.push_back(o[i] - o[0]);
+            lsrc.push_back(LineSrc{n, off.data(), l.seg + 4 * (size_t)o[0], l.angle + o[0], l.npix + o[0]});
+        }
     }
     if (n == 0) {   // T empty inserts: they succeed and retain nothing
         if (ss->retain) {
@@ -1524,8 +1610,9 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         iparts.push_back(ImgPart{frames->img_r + (size_t)t * n * px * ch, n});
     }
     const uint8_t* d_img = nullptr;
+    const uint8_t* d_rgb = nullptr;   // a colour FLD session's RGB2GRAY plane, which LBD reads
     if (prepare) {
-        if (const int rc = rectify_call(ctx, rect, ss, ids, n, n_img, iparts, s, &d_img)) return rc;
+        if (const int rc = rectify_call(ctx, rect, ss, ids, n, n_img, iparts, s, &d_img, &d_rgb)) return rc;
     } else if (pts || lns) {
         size_t o = o_img;
         for (const ImgPart& ip : iparts) {
@@ -1535,24 +1622,24 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         d_img = a.u8(o_img);
     }
     CK(ctx, cudaEventRecord(run_ev[1], s));
-    // the lines of every image: LSD alone on the main stream, then LBD on the second stream beside step 0's ORB; line
-    // blocks 2 t, 2 t + 1 are step t's left and right images
-    const int nblk = 2 * T;
-    std::vector<LineSrc> lsrc;
-    DetectedLines det;
+    // the lines of every image: LSD alone on the main stream (FLD: the caller's), then LBD on the second stream beside step
+    // 0's ORB
     std::vector<int32_t> lbase((size_t)nblk + 1, 0);
     const float* d_seg = nullptr;
     const uint8_t* d_ldesc = nullptr;
     bool run_lbd = false;
     if (lns) {
-        if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
-        if (const int rc = lsd_line_sources(ctx, &ss->lc, lsd, s, nblk, n, det, lsrc)) return rc;
+        if (!fld) {
+            if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
+            if (const int rc = lsd_line_sources(ctx, &ss->lc, lsd, s, nblk, n, det, lsrc)) return rc;
+        }
         for (int b = 0; b < nblk; ++b) lbase[(size_t)b + 1] = lbase[(size_t)b] + lsrc[(size_t)b].off[n];
         run_lbd = lbase[(size_t)nblk] > 0;
         if (run_lbd) {
             cudaEvent_t ready = next_event(ctx);
             CK(ctx, cudaEventRecord(ready, s));
-            if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, {}, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+            if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_rgb ? d_rgb : d_img, ready, {}, ctx->s_alt, &d_seg, &d_ldesc))
+                return rc;
             CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
         }
     }
@@ -1650,8 +1737,10 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (const int rc = add_ms(3, pm[0], pm[1])) return rc;
     if (const int rc = add_ms(4, pm[1], pm[2])) return rc;
     if (const int rc = add_ms(0, run_ev[0], run_ev[1])) return rc;
-    if (lns)
+    if (lns && !fld)
         if (const int rc = add_ms(2, ctx->lsd_ev[0], run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5])) return rc;
+    if (fld && run_lbd)
+        if (const int rc = add_ms(2, ctx->lbd_ev[0], ctx->lbd_ev[2])) return rc;
     ctx->img_timed = true;
     if (keep) {
         ss->kept.track = true;

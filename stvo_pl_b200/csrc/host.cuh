@@ -450,6 +450,7 @@ struct PlStereoSession {
     PlOrbDetectConfig oc{};
     PlLsdConfig lc{};
     bool has_lc = false;
+    bool fld = false;                       // plstvo_stereo_session_use_fld_lines: the caller's key lines, no LSD
     const PlRectifier* rect = nullptr;
     // plstvo_stereo_session_create_cams: stream i's camera and rectifier (empty: cam and rect for every stream)
     std::vector<PlCamera> cams;
@@ -534,8 +535,10 @@ struct ImgPart {   // consecutive host images of one size
 // slot and the grey device copy of them into its rectified slot (*d_out): their remap, in blocks of per_block images that
 // alternate left, right maps, and for a colour rectifier the conversion to grey after it.  rects (optional, [per_block], of
 // rect's size and channels): image z is prepared by rects[z % per_block] instead, a null entry or one without maps copying
-// (grey) or converting (colour) the image.
+// (grey) or converting (colour) the image.  d_rgb (optional, colour rectifiers only): the same launch also writes the
+// COLOR_RGB2GRAY conversion of each remapped (or unmapped) image into a second grey slot, *d_rgb.
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
-                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects = nullptr);
+                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects = nullptr,
+                    const uint8_t** d_rgb = nullptr);
 
 }  // namespace plstvo

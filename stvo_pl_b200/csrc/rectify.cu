@@ -91,14 +91,20 @@ __device__ __forceinline__ uint32_t bgr_to_grey(uint32_t b, uint32_t g, uint32_t
     return (3735u * b + 19235u * g + 9798u * r + (1u << 14)) >> 15;
 }
 
+// cv::cvtColor(COLOR_RGB2GRAY) on 8-bit data: the same fixed point with the first and third channels swapped.  The
+// reference's FLD branch converts a colour image with it (src/stereoFrame.cpp:251) and LBD then reads that image.
+__device__ __forceinline__ uint32_t rgb_to_grey(uint32_t r, uint32_t g, uint32_t b) { return bgr_to_grey(b, g, r); }
+
 // Byte k of a run of little-endian words (k a compile-time constant once the callers' loops unroll).
 __device__ __forceinline__ uint32_t byte_of(const uint32_t* w, int k) { return (w[k >> 2] >> (8 * (k & 3))) & 255u; }
 
 // cvtColor alone on n pixels of C interleaved channels (B, G, R[, A]), the whole batch as one run: the conversion does not
 // depend on where an image starts.  One thread converts 16 pixels: C 16-byte loads and one 16-byte store, all aligned
 // because the staging and the output slots start 256-byte aligned; the last partial group goes pixel by pixel.
-template <int C>
-__global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t n) {
+// RGB: the same pixels' rgb_to_grey also go to dst_rgb (read once, two bytes written per pixel).
+template <int C, bool RGB = false>
+__global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, size_t n,
+                                                            uint8_t* __restrict__ dst_rgb) {
     const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 16;
     if (p0 >= n) return;
     if (p0 + 16 <= n) {
@@ -113,10 +119,18 @@ __global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __res
         for (int i = 0; i < 16; ++i)
             o[i >> 2] |= bgr_to_grey(byte_of(w, C * i), byte_of(w, C * i + 1), byte_of(w, C * i + 2)) << (8 * (i & 3));
         *reinterpret_cast<uint4*>(dst + p0) = make_uint4(o[0], o[1], o[2], o[3]);
+        if constexpr (RGB) {
+            uint32_t q[4] = {0, 0, 0, 0};
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+                q[i >> 2] |= rgb_to_grey(byte_of(w, C * i), byte_of(w, C * i + 1), byte_of(w, C * i + 2)) << (8 * (i & 3));
+            *reinterpret_cast<uint4*>(dst_rgb + p0) = make_uint4(q[0], q[1], q[2], q[3]);
+        }
     } else {
         for (size_t p = p0; p < n; ++p) {
             const uint8_t* s = src + p * C;
             dst[p] = (uint8_t)bgr_to_grey(__ldg(s), __ldg(s + 1), __ldg(s + 2));
+            if constexpr (RGB) dst_rgb[p] = (uint8_t)rgb_to_grey(__ldg(s), __ldg(s + 1), __ldg(s + 2));
         }
     }
 }
@@ -125,7 +139,7 @@ __global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __res
 // image interpolates every channel with the same weights as the one-channel remap, and the reference converts the remapped
 // image.  Alpha is not read: a 4-channel tap is one aligned 4-byte load, of which the top byte is dropped.
 template <int C>
-__device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
+__device__ __forceinline__ void remap_channels(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f, uint32_t ch[3]) {
     f &= 1023u;
     const int ax = (int)(f & 31u), ay = (int)(f >> 5);
     const int x = m.x, y = m.y;
@@ -134,7 +148,6 @@ __device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, in
     const int w00 = (32 - ax) * (32 - ay), w01 = ax * (32 - ay), w10 = (32 - ax) * ay, w11 = ax * ay;
     const ptrdiff_t row = (ptrdiff_t)W * C;
     const uint8_t* r0 = S + ((ptrdiff_t)y * W + x) * C;
-    uint32_t ch[3];
     if constexpr (C == 4) {
         const uint32_t t00 = (x0 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0)) : 0u;
         const uint32_t t01 = (x1 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + 4)) : 0u;
@@ -155,17 +168,25 @@ __device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, in
             ch[c] = (uint32_t)((v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + 512) >> 10);
         }
     }
+}
+
+template <int C>
+__device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
+    uint32_t ch[3];
+    remap_channels<C>(S, W, H, m, f, ch);
     return bgr_to_grey(ch[0], ch[1], ch[2]);
 }
 
 // rectify_remap_kernel's layout on C-channel images: one thread writes 4 consecutive grey pixels of one image from one
 // 16-byte map1 load and one 8-byte map2 load; image z of the staging slot starts at z * W * H * C.
 // TABLE: the maps of image z as in rectify_remap_kernel; an entry without maps converts the image only.
-template <int C, bool TABLE>
+// RGB: each remapped (or unmapped) pixel's rgb_to_grey also goes to dst_rgb, at the same index as its dst byte.
+template <int C, bool TABLE, bool RGB = false>
 __global__ void __launch_bounds__(256) color_remap_kernel(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst,
                                                           const short2* __restrict__ m1l, const uint16_t* __restrict__ m2l,
                                                           const short2* __restrict__ m1r, const uint16_t* __restrict__ m2r,
-                                                          int W, int H, int per_block, int z0, const RemapMaps* __restrict__ maps) {
+                                                          int W, int H, int per_block, int z0, const RemapMaps* __restrict__ maps,
+                                                          uint8_t* __restrict__ dst_rgb) {
     const int z = z0 + (int)blockIdx.y;
     const size_t N = (size_t)W * H;
     const size_t p0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
@@ -181,17 +202,50 @@ __global__ void __launch_bounds__(256) color_remap_kernel(const uint8_t* __restr
         m2 = mp.m2;
         if (!m1) {
             const size_t e = p0 + 4 <= N ? p0 + 4 : N;
-            uint32_t v = 0;
+            uint32_t v = 0, v2 = 0;
             for (size_t p = p0; p < e; ++p) {
                 const uint8_t* q = S + p * C;
                 v |= bgr_to_grey(__ldg(q), __ldg(q + 1), __ldg(q + 2)) << (8 * (p - p0));
+                if constexpr (RGB) v2 |= rgb_to_grey(__ldg(q), __ldg(q + 1), __ldg(q + 2)) << (8 * (p - p0));
             }
-            if (e - p0 == 4)
+            if (e - p0 == 4) {
                 store4(D, v);
-            else
+                if constexpr (RGB) store4(dst_rgb + (size_t)z * N + p0, v2);
+            } else {
                 for (size_t p = p0; p < e; ++p) D[p - p0] = (uint8_t)(v >> (8 * (p - p0)));
+                if constexpr (RGB)
+                    for (size_t p = p0; p < e; ++p) dst_rgb[(size_t)z * N + p] = (uint8_t)(v2 >> (8 * (p - p0)));
+            }
             return;
         }
+    }
+    if constexpr (RGB) {   // both conversions of each remapped pixel's three channels
+        uint8_t* D2 = dst_rgb + (size_t)z * N + p0;
+        if (p0 + 4 <= N) {   // the maps as the grey form loads them: one 16-byte map1 and one 8-byte map2 load
+            const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
+            const uint2 b = __ldg(reinterpret_cast<const uint2*>(m2 + p0));
+            short2 m[4];
+            memcpy(m, &a, sizeof a);
+            const uint32_t f[4] = {b.x & 0xffffu, b.x >> 16, b.y & 0xffffu, b.y >> 16};
+            uint32_t v = 0, v2 = 0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                uint32_t ch[3];
+                remap_channels<C>(S, W, H, m[i], f[i], ch);
+                v |= bgr_to_grey(ch[0], ch[1], ch[2]) << (8 * i);
+                v2 |= rgb_to_grey(ch[0], ch[1], ch[2]) << (8 * i);
+            }
+            store4(D, v);
+            store4(D2, v2);
+        } else {
+            for (size_t p = p0; p < N; ++p) {
+                uint32_t ch[3];
+                remap_channels<C>(S, W, H, __ldg(m1 + p), __ldg(m2 + p), ch);
+                D[p - p0] = (uint8_t)bgr_to_grey(ch[0], ch[1], ch[2]);
+                D2[p - p0] = (uint8_t)rgb_to_grey(ch[0], ch[1], ch[2]);
+            }
+        }
+        return;
     }
     if (p0 + 4 <= N) {
         const int4 a = __ldg(reinterpret_cast<const int4*>(m1 + p0));
@@ -249,24 +303,25 @@ cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const u
 
 // The grey device copy of n_img colour images (C channels): color_convert_kernel without maps, color_remap_kernel with;
 // with a map table (per-image maps or none) its instantiation that reads it.
-template <int C>
+// RGB: the instantiations that also write the COLOR_RGB2GRAY plane dst_rgb.
+template <int C, bool RGB>
 cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool maps, const uint8_t* src, uint8_t* dst,
                                  const short2* const m1[2], const uint16_t* const m2[2], cudaStream_t s, int* launches,
-                                 const RemapMaps* table) {
+                                 const RemapMaps* table, uint8_t* dst_rgb) {
     if (table) {
         const size_t quads = ((size_t)W * H + 3) / 4;
         const unsigned gx = (unsigned)((quads + 255) / 256);
         for (int z0 = 0; z0 < n_img; z0 += 65535) {
             const int nz = std::min(n_img - z0, 65535);
-            color_remap_kernel<C, true><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, nullptr, nullptr, nullptr, nullptr, W, H,
-                                                                                per_block, z0, table);
+            color_remap_kernel<C, true, RGB><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, nullptr, nullptr, nullptr, nullptr, W,
+                                                                                     H, per_block, z0, table, dst_rgb);
             ++*launches;
         }
         return cudaGetLastError();
     }
     if (!maps) {
         const size_t groups = ((size_t)n_img * W * H + 15) / 16;
-        color_convert_kernel<C><<<(unsigned)((groups + 255) / 256), 256, 0, s>>>(src, dst, (size_t)n_img * W * H);
+        color_convert_kernel<C, RGB><<<(unsigned)((groups + 255) / 256), 256, 0, s>>>(src, dst, (size_t)n_img * W * H, dst_rgb);
         ++*launches;
         return cudaGetLastError();
     }
@@ -274,15 +329,15 @@ cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool ma
     const unsigned gx = (unsigned)((quads + 255) / 256);
     for (int z0 = 0; z0 < n_img; z0 += 65535) {
         const int nz = std::min(n_img - z0, 65535);
-        color_remap_kernel<C, false><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H, per_block,
-                                                                             z0, nullptr);
+        color_remap_kernel<C, false, RGB><<<dim3(gx, (unsigned)nz), 256, 0, s>>>(src, dst, m1[0], m2[0], m1[1], m2[1], W, H,
+                                                                                  per_block, z0, nullptr, dst_rgb);
         ++*launches;
     }
     return cudaGetLastError();
 }
 
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
-                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects) {
+                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects, const uint8_t** d_rgb) {
     const int W = rect->width, H = rect->height, Ch = rect->channels;
     const size_t bytes = (size_t)n_img * W * H;
     CK(ctx, cudaSetDevice(ctx->device));
@@ -293,7 +348,9 @@ int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_
             if (r->maps)
                 for (int side = 0; side < 2; ++side) table[2 * k + side] = RemapMaps{r->m1[side], r->m2[side]};
     Arena a;
+    const bool rgb = d_rgb && Ch > 1;
     const size_t o_raw = a.take(bytes * Ch), o_out = a.take(bytes), o_tab = a.take(table.size() * sizeof(RemapMaps));
+    const size_t o_rgb = a.take(rgb ? bytes : 0);
     CK(ctx, a.alloc(ctx->arena_rect));
     CK(ctx, a.up(o_tab, table.data(), table.size() * sizeof(RemapMaps), s));
     const RemapMaps* d_tab = rects ? a.at<RemapMaps>(o_tab) : nullptr;
@@ -308,16 +365,23 @@ int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_
     CK(ctx, cudaEventRecord(ctx->rect_ev[0], s));
     if (Ch == 1)
         CK(ctx, launch_rectify_remap(n_img, per_block, W, H, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s, &launches, d_tab));
+    else if (Ch == 3 && rgb)
+        CK(ctx, (launch_color_prepare<3, true>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2,
+                                              s, &launches, d_tab, a.u8(o_rgb))));
     else if (Ch == 3)
-        CK(ctx, launch_color_prepare<3>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
-                                        &launches, d_tab));
+        CK(ctx, (launch_color_prepare<3, false>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2,
+                                               s, &launches, d_tab, nullptr)));
+    else if (rgb)
+        CK(ctx, (launch_color_prepare<4, true>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2,
+                                              s, &launches, d_tab, a.u8(o_rgb))));
     else
-        CK(ctx, launch_color_prepare<4>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2, s,
-                                        &launches, d_tab));
+        CK(ctx, (launch_color_prepare<4, false>(n_img, per_block, W, H, rect->maps, a.u8(o_raw), a.u8(o_out), rect->m1, rect->m2,
+                                               s, &launches, d_tab, nullptr)));
     CK(ctx, cudaEventRecord(ctx->rect_ev[1], s));
     ctx->rect_ran = true;
     ctx->launches += launches;
     *d_out = a.u8(o_out);
+    if (d_rgb) *d_rgb = rgb ? a.u8(o_rgb) : nullptr;
     return 0;
 }
 

@@ -105,6 +105,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_lsd_detect_batch": (C.c_int, [vp, C.POINTER(T.PlLsdConfig), C.c_int, C.c_int, C.c_int, u8p, C.c_int, i32p, fp, fp,
                                               i32p, fp, fp]),
         "plstvo_lsd_kernel_times": (C.c_int, [vp, fp]),
+        "plstvo_fld_key_lines": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, fp, fp, fp, i32p, fp, fp]),
         "plstvo_track_stereo_images_batch": (C.c_int, [vp, cam, cfg, C.POINTER(T.PlStereoMatchConfig), C.POINTER(T.PlStereoConfig),
                                                        C.POINTER(T.PlOrbDetectConfig), C.POINTER(T.PlStereoImages),
                                                        C.POINTER(T.PlStereoImages), vp, vp, i32p]),
@@ -143,6 +144,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_stereo_session_initialize": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), i32p]),
         "plstvo_stereo_session_insert": (C.c_int, [vp, vp, C.c_int, i32p, C.POINTER(T.PlStereoImages), vp, vp, i32p]),
         "plstvo_stereo_session_retain": (C.c_int, [vp, vp, C.c_int]),
+        "plstvo_stereo_session_use_fld_lines": (C.c_int, [vp, vp, C.c_int]),
         "plstvo_stereo_session_read": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut)]),
         "plstvo_default_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
         "plstvo_kitti_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
@@ -185,11 +187,30 @@ EXPORTED_SYMBOLS = [
     "plstvo_rectifier_create_color", "plstvo_stereo_session_retain", "plstvo_stereo_session_read",
     "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams", "plstvo_default_handler_config",
     "plstvo_kitti_handler_config", "plstvo_stereo_session_run", "plstvo_default_keyframe_config",
-    "plstvo_initial_keyframe_state", "plstvo_stereo_session_run_keyframes", "plstvo_stereo_session_read_keyframes"]
+    "plstvo_initial_keyframe_state", "plstvo_stereo_session_run_keyframes", "plstvo_stereo_session_read_keyframes",
+    "plstvo_fld_key_lines", "plstvo_stereo_session_use_fld_lines"]
 
 
 def _p(a: Optional[np.ndarray], typ):
     return C.cast(None, typ) if a is None else a.ctypes.data_as(typ)
+
+
+def fld_key_lines(width: int, height: int, n_features: int, seg, lib: Optional[C.CDLL] = None):
+    """plstvo_fld_key_lines (host code, no GPU): the reference's FLD-branch key lines of one width x height image from
+    FastLineDetector's segments seg float32[n, 4] in its order.  Returns dict(seg [m, 4], angle, npix, response, length), m =
+    min(n, n_features) (n where n_features is 0), in the reference's order."""
+    lib = lib or load_library()
+    seg = np.ascontiguousarray(seg, np.float32).reshape(-1, 4)
+    m = len(seg) if n_features == 0 else min(len(seg), max(int(n_features), 0))
+    out = dict(seg=np.zeros((m, 4), np.float32), angle=np.zeros(m, np.float32), npix=np.zeros(m, np.int32),
+               response=np.zeros(m, np.float32), length=np.zeros(m, np.float32))
+    rc = lib.plstvo_fld_key_lines(width, height, n_features, len(seg), _p(seg, T.c_float_p), _p(out["seg"], T.c_float_p),
+                                  _p(out["angle"], T.c_float_p), _p(out["npix"], T.c_int32_p),
+                                  _p(out["response"], T.c_float_p), _p(out["length"], T.c_float_p))
+    if rc < 0:
+        raise PlstvoError(rc, "plstvo_fld_key_lines rejected the size, n_features or the segments")
+    assert rc == m
+    return out
 
 
 def init_undistort_rectify_map(model: int, K, D, R, P, width: int, height: int, lib: Optional[C.CDLL] = None):
@@ -291,6 +312,12 @@ class StereoSession:
         if got != n_kf:
             raise PlstvoError(-1, f"plstvo_stereo_session_read_keyframes returned {got} key frames, then {n_kf}")
         return rows, pt, ls
+
+    def use_fld_lines(self, on: bool):
+        """plstvo_stereo_session_use_fld_lines: the reference's FLD line branch.  On, every call takes each frame's key lines
+        from frames under the images call's keys (ll_off / lr_off, seg_l / seg_r, angle_l / angle_r, npix_l / npix_r, e.g.
+        from fld_key_lines; step-major for run / run_keyframes) instead of running LSD.  Only while no stream holds a frame."""
+        self.eng._ck(self.eng.lib.plstvo_stereo_session_use_fld_lines(self.eng.ctx, self.handle, 1 if on else 0))
 
     def retain(self, on: bool):
         """plstvo_stereo_session_retain: from the next initialize / insert on, keep each call's new frames and matches on the
@@ -665,6 +692,10 @@ class Engine:
         for k in ("seg", "angle", "npix", "response", "length"):
             out[k] = out[k][:total]
         return total, out
+
+    def fld_key_lines(self, width: int, height: int, n_features: int, seg):
+        """Module-level fld_key_lines on this engine's library."""
+        return fld_key_lines(width, height, n_features, seg, self.lib)
 
     def lsd_kernel_times(self):
         """Device ms of the last lsd_detect_batch: blur + resize, gradient + seed order, region growing, the host's region
