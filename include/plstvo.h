@@ -887,6 +887,17 @@ int  plstvo_debug_select(PlContext* ctx, int n_lists, const int32_t* off, const 
 int  plstvo_debug_tc_partials(PlContext* ctx, int B, const uint8_t* d1, const int32_t* off1, const uint8_t* d2,
                               const int32_t* off2, float nnr, uint32_t* rowp, uint32_t* colp, uint32_t* rowkey,
                               uint32_t* colkey);
+/* test hook: both grey planes of the colour preparation a colour FLD session runs (the upload, then the remap and the
+ * conversions of the same launch), on B pairs of host images img_l, img_r [B][height][width][channels] of a colour rectifier
+ * rect.  rects (NULL, or [B] as plstvo_stereo_session_create_cams takes them, one per pair): pair b is prepared by rects[b]
+ * instead of rect, a NULL entry or one without maps converting only.  Out, host, left images then right:
+ *   grey [2][B][height][width]: cvtColor(remap(img), COLOR_BGR2GRAY), what ORB and LSD read (plstvo_rectify_batch's output);
+ *   rgb  [2][B][height][width]: cvtColor(remap(img), COLOR_RGB2GRAY), what LBD reads on the FLD branch.
+ * Without maps the remap is left out.  PLSTVO_E_INVALID (plstvo_last_error says which): a null pointer, B < 1, a rectifier
+ * of another context, a grey rectifier, a table entry of another size or channel count than rect.  The call also updates
+ * what plstvo_rectify_kernel_times reports. */
+int  plstvo_debug_color_planes(PlContext* ctx, const PlRectifier* rect, const PlRectifier* const* rects, int B,
+                               const uint8_t* img_l, const uint8_t* img_r, uint8_t* grey, uint8_t* rgb);
 /* test hook for the on-chip 6x6 routines of the solver (ColPivHouseholderQR solve + log|det|, inverse, symmetric
  * eigenvalues) on n caller-supplied matrices: H [n][36] row-major, g [n][6] -> x [n][6], lad [n], inv [n][36], eig [n][6] */
 int  plstvo_debug_algebra(PlContext* ctx, int n, const double* H, const double* g, double* x, double* lad,

@@ -579,6 +579,33 @@ int plstvo_rectify_batch(PlContext* ctx, const PlRectifier* rect, int B, const u
     return 0;
 }
 
+int plstvo_debug_color_planes(PlContext* ctx, const PlRectifier* rect, const PlRectifier* const* rects, int B,
+                              const uint8_t* img_l, const uint8_t* img_r, uint8_t* grey, uint8_t* rgb) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!rect || !img_l || !img_r || !grey || !rgb) return fail(ctx, PLSTVO_E_INVALID, "null argument");
+    if (B < 1) return fail(ctx, PLSTVO_E_INVALID, "B must be at least 1");
+    if (rect->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the rectifier belongs to another context");
+    if (rect->channels == 1) return fail(ctx, PLSTVO_E_INVALID, "a grey rectifier has no RGB plane");
+    for (int b = 0; rects && b < B; ++b) {
+        const PlRectifier* r = rects[b];
+        if (!r) continue;
+        if (r->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "a table rectifier belongs to another context");
+        if (r->width != rect->width || r->height != rect->height)
+            return fail(ctx, PLSTVO_E_INVALID, "a table rectifier's size differs from rect's");
+        if (r->channels != rect->channels) return fail(ctx, PLSTVO_E_INVALID, "a table rectifier's channels differ from rect's");
+    }
+    cudaStream_t s = ctx->s_main;
+    const uint8_t *d_grey = nullptr, *d_rgb = nullptr;
+    if (const int rc = rectify_enqueue(ctx, rect, 2 * B, B, {ImgPart{img_l, B}, ImgPart{img_r, B}}, s, &d_grey, rects, &d_rgb))
+        return rc;
+    const size_t bytes = 2 * (size_t)B * rect->width * rect->height;
+    CK(ctx, cudaMemcpyAsync(grey, d_grey, bytes, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaMemcpyAsync(rgb, d_rgb, bytes, cudaMemcpyDeviceToHost, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return 0;
+}
+
 int plstvo_rectify_kernel_times(PlContext* ctx, float* ms1) {
     if (!ctx || !ms1) return PLSTVO_E_INVALID;
     LOCK(ctx);

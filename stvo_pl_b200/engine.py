@@ -91,6 +91,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_debug_pose_helpers": (C.c_int, [vp, C.c_int, dp, dp]),
         "plstvo_debug_select": (C.c_int, [vp, C.c_int, i32p, dp, i32p, dp, C.c_int, dp]),
         "plstvo_debug_tc_partials": (C.c_int, [vp, C.c_int, u8p, i32p, u8p, i32p, C.c_float, u32p, u32p, u32p, u32p]),
+        "plstvo_debug_color_planes": (C.c_int, [vp, vp, C.POINTER(vp), C.c_int, u8p, u8p, u8p, u8p]),
         "plstvo_default_orb_config": (None, [C.POINTER(T.PlOrbConfig)]),
         "plstvo_orb_compute_batch": (C.c_int, [vp, C.POINTER(T.PlOrbConfig), C.c_int, C.c_int, C.c_int, u8p, i32p, fp, i32p, fp,
                                                fp, u8p, i32p, i32p]),
@@ -174,7 +175,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
     "plstvo_batch_phase_cycles",
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_pose_helpers",
-    "plstvo_debug_select", "plstvo_debug_tc_partials",
+    "plstvo_debug_select", "plstvo_debug_tc_partials", "plstvo_debug_color_planes",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
     "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
@@ -1255,6 +1256,27 @@ class Engine:
                                                    _p(off2, T.c_int32_p), C.c_float(nnr), _p(rowp, u32p), _p(colp, u32p),
                                                    _p(rowkey, u32p), _p(colkey, u32p)))
         return rowp, colp, rowkey, colkey
+
+    def debug_color_planes(self, rect: Rectifier, img_l, img_r, rects=None):
+        """Both grey planes of a colour FLD session's preparation (test hook) on B pairs uint8[B, H, W, C] of the colour
+        rectifier rect; rects (None, or one Rectifier or None per pair): pair b prepared by rects[b], None converting only.
+        Returns (grey, rgb), each uint8[2, B, H, W] (left images, then right): COLOR_BGR2GRAY and COLOR_RGB2GRAY of each
+        remapped image."""
+        il = np.ascontiguousarray(img_l, np.uint8)
+        ir = np.ascontiguousarray(img_r, np.uint8)
+        B = il.shape[0] if il.ndim else 0
+        if il.shape != ir.shape or il.shape != rect.image_shape(B):
+            raise ValueError("images must be uint8[B, H, W, C] of the rectifier's size and channels, both sides alike")
+        H, W = rect.height, rect.width
+        rarr = None
+        if rects is not None:
+            if len(rects) != B:
+                raise ValueError("one rectifier (or None) per pair")
+            rarr = (C.c_void_p * max(B, 1))(*[None if r is None else r.handle for r in rects])
+        grey, rgb = np.zeros((2, B, H, W), np.uint8), np.zeros((2, B, H, W), np.uint8)
+        self._ck(self.lib.plstvo_debug_color_planes(self.ctx, rect.handle, rarr, B, _p(il, T.c_uint8_p), _p(ir, T.c_uint8_p),
+                                                    _p(grey, T.c_uint8_p), _p(rgb, T.c_uint8_p)))
+        return grey, rgb
 
     def debug_algebra(self, H, g):
         """On-chip 6x6 routines (test hook): returns x = H^-1 g (col-pivot QR), log|det H|, inv(H), eigvals(H)."""
