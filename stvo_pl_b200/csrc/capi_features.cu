@@ -894,47 +894,82 @@ int plstvo_fld_key_lines(int width, int height, int n_features, int n_seg, const
 
 /* ---- stereo images -> pose: ORB, LSD and LBD feed the stereo step and the tracker without leaving HBM ---- */
 namespace {
-// LSD's key lines of nblk blocks of nf images each, the arrays a LineSrc per block points at
-struct DetectedLines {
-    std::vector<std::vector<int32_t>> off, npix;
-    std::vector<std::vector<float>> seg, angle;
+// A call's key lines in blocks of nf images, block 2 s + side holding step (or frame set) s's left (side 0) or right images:
+// the LineSrc each block gives LBD and the stereo step, and where LBD leaves the blocks' rows
+struct LineBlocks {
+    std::vector<LineSrc> lsrc;                     // per block: into the caller's arrays, or into LSD's below
+    std::vector<std::vector<int32_t>> off;         // per block: its offsets, rebased to 0
+    std::vector<int32_t> lsd_off, lsd_npix;        // LSD's key lines of every image of the call
+    std::vector<float> lsd_seg, lsd_angle;
+    std::vector<int32_t> lbase{0};                 // [blocks + 1] each block's first row in LBD's output
+    bool run_lbd = false;                          // some block has a key line
+    const float* d_seg = nullptr;                  // LBD's rows (once describe() ran): segments and descriptors
+    const uint8_t* d_ldesc = nullptr;
+    cudaEvent_t joined = nullptr;                  // recorded on the second stream after LBD
+
+    // The caller's key lines of frame sets fs[0 .. nfs), steps x nf frames each: both sides of every set checked whole, then
+    // cut into one block per step and side
+    int cut(PlContext* ctx, const PlStereoImages* const* fs, int nfs, int steps, int nf) {
+        std::vector<LineSrc> whole;
+        for (int j = 0; j < nfs; ++j) {
+            whole.push_back(LineSrc{steps * nf, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
+            whole.push_back(LineSrc{steps * nf, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
+        }
+        for (const LineSrc& l : whole)
+            if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        off.assign(whole.size() * steps, {});
+        for (size_t b = 0; b < off.size(); ++b)   // frame set b / (2 steps), step b / 2 % steps, side b % 2
+            add_block(b, whole[b / (2 * steps) * 2 + b % 2], b / 2 % steps * nf, nf);
+        return 0;
+    }
+
+    // LSD's key lines of nblk blocks of nf images: its host continuation on stream s (where its device half ran), with the
+    // images calls' key-line checks
+    int take_lsd(PlContext* ctx, const PlLsdConfig* lc, const LsdLaunch& lsd, cudaStream_t s, int nblk, int nf) {
+        std::vector<std::vector<KeyLine>> kls;
+        if (const int rc = lsd_finish(ctx, lc, lsd, s, kls)) return rc;
+        lsd_off.assign(1, 0);
+        for (const std::vector<KeyLine>& k : kls) {
+            if (k.size() > (size_t)PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
+            lsd_off.push_back(lsd_off.back() + (int32_t)k.size());
+        }
+        const size_t m = (size_t)lsd_off.back();
+        lsd_seg.resize(4 * m);
+        lsd_angle.resize(m);
+        lsd_npix.resize(m);
+        lsd_rows(kls, 0, (int)kls.size(), lsd_seg.data(), lsd_angle.data(), lsd_npix.data(), nullptr, nullptr);
+        const LineSrc all{(int)kls.size(), lsd_off.data(), lsd_seg.data(), lsd_angle.data(), lsd_npix.data()};
+        if (const int rc = lbd_check_lines(ctx, all)) return rc;
+        off.assign((size_t)nblk, {});
+        for (int b = 0; b < nblk; ++b) add_block(b, all, (size_t)b * nf, nf);
+        return 0;
+    }
+
+    // block b (the next one): nf images of l from image i0 on
+    void add_block(size_t b, const LineSrc& l, size_t i0, int nf) {
+        const int32_t* o = l.off + i0;
+        for (int i = 0; i <= nf; ++i) off[b].push_back(o[i] - o[0]);
+        lsrc.push_back(LineSrc{nf, off[b].data(), l.seg + 4 * (size_t)o[0], l.angle + o[0], l.npix + o[0]});
+        lbase.push_back(lbase.back() + off[b][(size_t)nf]);
+        run_lbd = lbase.back() > 0;
+    }
+
+    // LBD on every block's key lines, enqueued on the second stream (device images d_img, ready once `ready` has completed,
+    // or host images parts), then the join
+    int describe(PlContext* ctx, int W, int H, const uint8_t* d_img, cudaEvent_t ready, const std::vector<ImgPart>& parts) {
+        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_img, ready, parts, ctx->s_alt, &d_seg, &d_ldesc)) return rc;
+        CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
+        joined = ctx->img_join[0];
+        return 0;
+    }
 };
 
-// LSD's host continuation on stream s (where its device half ran), then one LineSrc per block appended to lsrc, with the
-// images calls' key-line checks
-int lsd_line_sources(PlContext* ctx, const PlLsdConfig* lc, const LsdLaunch& lsd, cudaStream_t s, int nblk, int nf,
-                     DetectedLines& d, std::vector<LineSrc>& lsrc) {
-    std::vector<std::vector<KeyLine>> kls;
-    if (const int rc = lsd_finish(ctx, lc, lsd, s, kls)) return rc;
-    for (const std::vector<KeyLine>& k : kls)
-        if (k.size() > (size_t)PLSTVO_MAX_FEATURES) return fail(ctx, PLSTVO_E_TOO_LARGE, "more than 65535 key lines in one image");
-    d.off.assign((size_t)nblk, {});
-    d.npix.assign((size_t)nblk, {});
-    d.seg.assign((size_t)nblk, {});
-    d.angle.assign((size_t)nblk, {});
-    for (int b = 0; b < nblk; ++b) {
-        std::vector<int32_t>& off = d.off[(size_t)b];
-        off.assign(1, 0);
-        for (int i = 0; i < nf; ++i) off.push_back(off.back() + (int32_t)kls[(size_t)b * nf + i].size());
-        const size_t m = (size_t)off.back();
-        d.seg[(size_t)b].resize(4 * m);
-        d.angle[(size_t)b].resize(m);
-        d.npix[(size_t)b].resize(m);
-        lsd_rows(kls, b * nf, nf, d.seg[(size_t)b].data(), d.angle[(size_t)b].data(), d.npix[(size_t)b].data(), nullptr, nullptr);
-        lsrc.push_back(LineSrc{nf, off.data(), d.seg[(size_t)b].data(), d.angle[(size_t)b].data(), d.npix[(size_t)b].data()});
-    }
-    for (const LineSrc& l : lsrc)
-        if (const int rc = lbd_check_lines(ctx, l)) return rc;
-    return 0;
-}
-
-// One frame set of the stereo step (nf frames) on device inputs: the points of ORB's image blocks ob and ob + 1 (left,
-// right, nf images each) and the lines of line blocks lb and lb + 1 (LBD's rows from lbase[lb], lbase[lb + 1]), offsets
-// rebased to 0 into pl_off / pr_off.  lines: the frames have key lines (lsrc valid); run_lbd: LBD ran (d_seg, d_ldesc valid).
-void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const std::vector<LineSrc>& lsrc, int lb, bool lines,
-                       bool run_lbd, const std::vector<int32_t>& lbase, const float* d_seg, const uint8_t* d_ldesc, int nf,
+// One frame set of the stereo step (nf frames) on device inputs, into dev.set[k] (points) and dev.set[k + 1] (lines): the
+// points of ORB's image blocks ob and ob + 1 (left, right, nf images each) and the key lines of line blocks lb and lb + 1,
+// offsets rebased to 0 into pl_off / pr_off.  none: nf + 1 zero offsets, for frames without key lines.
+void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const LineBlocks& lines, int lb, int nf,
                        const std::vector<int32_t>& none, std::vector<int32_t>& pl_off, std::vector<int32_t>& pr_off,
-                       PlStereoFeatures& F, StereoDevInputs::Set& P, StereoDevInputs::Set& Ls) {
+                       PlStereoFeatures& F, StereoDevInputs& dev, int k) {
     const size_t kl = orb.off[(size_t)ob * nf], kr = orb.off[(size_t)(ob + 1) * nf];
     pl_off.resize((size_t)nf + 1);
     pr_off.resize((size_t)nf + 1);
@@ -942,27 +977,47 @@ void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const std::vect
         pl_off[i] = orb.off[(size_t)ob * nf + i] - (int32_t)kl;
         pr_off[i] = orb.off[(size_t)(ob + 1) * nf + i] - (int32_t)kr;
     }
+    const bool has_lines = !lines.lsrc.empty();
     F = PlStereoFeatures{};
     F.B = nf;
     F.pl_off = pl_off.data(); F.pr_off = pr_off.data();
-    F.ll_off = lines ? lsrc[(size_t)lb].off : none.data(); F.lr_off = lines ? lsrc[(size_t)lb + 1].off : none.data();
-    F.angle_l = lines ? lsrc[(size_t)lb].angle : nullptr;
+    F.ll_off = has_lines ? lines.lsrc[(size_t)lb].off : none.data();
+    F.lr_off = has_lines ? lines.lsrc[(size_t)lb + 1].off : none.data();
+    F.angle_l = has_lines ? lines.lsrc[(size_t)lb].angle : nullptr;
+    StereoDevInputs::Set& P = dev.set[k];
     P = StereoDevInputs::Set{};
     P.on_device = true;
     if (pts) {
         P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
         P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
     }
+    StereoDevInputs::Set& Ls = dev.set[k + 1];
     Ls = StereoDevInputs::Set{};
     Ls.on_device = true;   // oct stays null: key lines of octave 0
-    if (run_lbd) {
-        Ls.xy_l = d_seg + 4 * (size_t)lbase[(size_t)lb]; Ls.xy_r = d_seg + 4 * (size_t)lbase[(size_t)lb + 1];
-        Ls.d1 = d_ldesc + 32 * (size_t)lbase[(size_t)lb]; Ls.d2 = d_ldesc + 32 * (size_t)lbase[(size_t)lb + 1];
+    if (lines.run_lbd) {
+        const size_t l0 = (size_t)lines.lbase[(size_t)lb], l1 = (size_t)lines.lbase[(size_t)lb + 1];
+        Ls.xy_l = lines.d_seg + 4 * l0; Ls.xy_r = lines.d_seg + 4 * l1;
+        Ls.d1 = lines.d_ldesc + 32 * l0; Ls.d2 = lines.d_ldesc + 32 * l1;
     }
+    dev.lines_ready = lines.joined;
 }
 
-bool key_lines_given(const PlStereoImages* f) {
-    return f->ll_off || f->lr_off || f->seg_l || f->seg_r || f->angle_l || f->angle_r || f->npix_l || f->npix_r;
+// The key-line field rules of a call on frame sets fs[0 .. nfs): the fields are null where the call detects its own key lines
+// (detect) and in a session without lines (no_lines); a session run (run) sets its own FAST thresholds, so frames->fast_th is
+// null there too
+int check_key_line_fields(PlContext* ctx, const PlStereoImages* const* fs, int nfs, bool detect, bool no_lines, bool run) {
+    bool given = false;
+    for (int j = 0; j < nfs; ++j) {
+        const PlStereoImages* f = fs[j];
+        given = given || f->ll_off || f->lr_off || f->seg_l || f->seg_r || f->angle_l || f->angle_r || f->npix_l || f->npix_r;
+    }
+    if (run && (fs[0]->fast_th || (detect && given)))
+        return fail(ctx, PLSTVO_E_INVALID,
+                    detect ? "frames->fast_th and the key-line fields must be null: the run sets its thresholds and detects its key lines"
+                           : "frames->fast_th must be null: the run sets its thresholds");
+    if (given && detect) return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the call detects its own key lines");
+    if (given && no_lines) return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the session has no lines");
+    return 0;
 }
 
 // The image checks of an images call or a session run, before any work, on frame sets fs[0 .. nfs) holding n_img > 0 images
@@ -984,14 +1039,15 @@ int images_check(PlContext* ctx, int W, int H, bool pts, bool lns, const PlStere
 }
 
 // Enqueues on s the grey device copy of n_img raw images (parts) in blocks of n images alternating left, right: the remap /
-// colour conversion of rect, or with a session of per-stream rectifiers, stream ids[k]'s rectifier for image k of each block.
-// A colour session on the FLD branch with lines also gets the RGB2GRAY plane LBD reads (*d_lbd; else null).
-int rectify_call(PlContext* ctx, const PlRectifier* rect, const PlStereoSession* session, const int32_t* ids, int n, int n_img,
+// colour conversion of rect, or in a session call with per-stream rectifiers, stream ids[k]'s rectifier for image k of each
+// block.  A colour session on the FLD branch with lines also gets the RGB2GRAY plane LBD reads (*d_lbd; else null).
+int rectify_call(PlContext* ctx, const PlRectifier* rect, const SessionCall* call, int n, int n_img,
                  const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out, const uint8_t** d_lbd) {
+    const PlStereoSession* ss = call ? call->ss : nullptr;
     std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
-    if (session && !session->rects.empty())
-        for (int k = 0; k < n; ++k) call_rects.push_back(session->rects[(size_t)ids[k]]);
-    const bool rgb = session && session->fld && session->cfg.has_lines && rect->channels > 1;
+    if (ss && !ss->rects.empty())
+        for (int k = 0; k < n; ++k) call_rects.push_back(ss->rects[(size_t)call->ids[k]]);
+    const bool rgb = ss && ss->fld && ss->cfg.has_lines && rect->channels > 1;
     return rectify_enqueue(ctx, rect, n_img, n, parts, s, d_out, call_rects.empty() ? nullptr : call_rects.data(),
                            rgb ? d_lbd : nullptr);
 }
@@ -1005,9 +1061,9 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
                             const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
                             const PlRectifier* rect, const PlStereoImages* prev, const PlStereoImages* curr,
                             const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence,
-                            PlStereoSession* session = nullptr) {
-    const bool one_set = sequence || session;   // one frame set: a sequence, or a session's new frames
-    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!one_set && !curr) || (!results && (!session || session->track)))
+                            SessionCall* call = nullptr) {
+    const bool one_set = sequence || call;   // one frame set: a sequence, or a session's new frames
+    if (!cam || !cfg || !mc || !sc || !oc || !prev || (!one_set && !curr) || (!results && (!call || call->track)))
         return fail(ctx, PLSTVO_E_INVALID, "null argument");
     if (rect && rect->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the rectifier belongs to another context");
     if (rect && (rect->width != cam->width || rect->height != cam->height))
@@ -1020,29 +1076,19 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const PlStereoImages* fs[2] = {prev, curr};
     const bool pts = cfg->has_points != 0, lns = cfg->has_lines != 0, run_lsd = detect_lines && lns;
     const int W = cam->width, H = cam->height;
-    if (detect_lines) {
-        for (int j = 0; j < nfs; ++j)
-            if (key_lines_given(fs[j]))
-                return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the call detects its own key lines");
-        if (run_lsd) {
-            if (!lc) return fail(ctx, PLSTVO_E_INVALID, "null lsd config");
-            if (const int rc = lsd_check_config(ctx, lc)) return rc;
-            if (2L * nfs * NF > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
-        }
+    if (const int rc = check_key_line_fields(ctx, fs, nfs, detect_lines, false, false)) return rc;
+    if (run_lsd) {
+        if (!lc) return fail(ctx, PLSTVO_E_INVALID, "null lsd config");
+        if (const int rc = lsd_check_config(ctx, lc)) return rc;
+        if (2L * nfs * NF > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
     }
     const int nblk = 2 * nfs, n_img = nblk * NF;
-    std::vector<LineSrc> lsrc;   // key lines per image block
+    LineBlocks lines;   // key lines per image block: one frame set's left, right images
     LsdLaunch lsd{};
     if (NF > 0) {
         if (const int rc = images_check(ctx, W, H, pts, lns, fs, nfs, run_lsd ? lc : nullptr, n_img, lsd)) return rc;
-        if (lns && !run_lsd) {
-            for (int j = 0; j < nfs; ++j) {
-                lsrc.push_back(LineSrc{NF, fs[j]->ll_off, fs[j]->seg_l, fs[j]->angle_l, fs[j]->npix_l});
-                lsrc.push_back(LineSrc{NF, fs[j]->lr_off, fs[j]->seg_r, fs[j]->angle_r, fs[j]->npix_r});
-            }
-            for (const LineSrc& l : lsrc)
-                if (const int rc = lbd_check_lines(ctx, l)) return rc;
-        }
+        if (lns && !run_lsd)
+            if (const int rc = lines.cut(ctx, fs, nfs, 1, NF)) return rc;
     }
     if (NF == 0 || (sequence && NF == 1)) return 0;
     CK(ctx, cudaSetDevice(ctx->device));
@@ -1050,7 +1096,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
     ctx->img_timed = false;
     std::vector<ImgPart> iparts;
-    std::vector<int32_t> th((size_t)n_img), lbase((size_t)nblk + 1, 0);
+    std::vector<int32_t> th((size_t)n_img);
     for (int b = 0; b < nblk; ++b) {
         const PlStereoImages* f = fs[b / 2];
         iparts.push_back(ImgPart{b % 2 ? f->img_r : f->img_l, NF});
@@ -1061,31 +1107,10 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     // reads; every stage then reads its grey device copy
     const std::vector<ImgPart> no_parts;
     const std::vector<ImgPart>& stage_parts = rect ? no_parts : iparts;
-    bool run_lbd = false;
-    auto count_lines = [&]() {
-        for (int b = 0; b < nblk; ++b) lbase[b + 1] = lbase[b] + (lns ? lsrc[b].off[NF] : 0);
-        run_lbd = lbase[nblk] > 0;
-    };
-    if (!run_lsd) count_lines();
-    const float* d_seg = nullptr;
-    const uint8_t* d_ldesc = nullptr;
     const uint8_t* d_images = nullptr;   // the device copy of the images the line stages read (null: LBD uploads its own)
     const uint8_t* d_rgb = nullptr;      // a colour FLD session's RGB2GRAY plane, which LBD reads instead
     cudaEvent_t images_ready = nullptr;
-    auto enqueue_lbd = [&]() -> int {
-        if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_rgb ? d_rgb : d_images, images_ready, stage_parts, ctx->s_alt, &d_seg,
-                                       &d_ldesc))
-            return rc;
-        CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
-        return 0;
-    };
-    // LSD's key lines per image block, what lsrc points at
-    DetectedLines det;
-    auto lsd_lines = [&](cudaStream_t s) -> int {
-        if (const int rc = lsd_line_sources(ctx, lc, lsd, s, nblk, NF, det, lsrc)) return rc;
-        count_lines();
-        return 0;
-    };
+    auto enqueue_lbd = [&]() { return lines.describe(ctx, W, H, d_rgb ? d_rgb : d_images, images_ready, stage_parts); };
     // With fewer images than SMs, LSD's one-warp and one-thread-per-image stages (seed order, region growing) are the whole
     // critical path and lose more beside ORB than ORB takes (BASELINE.md), so LSD runs first on the main stream, alone, and ORB
     // reads its device copy of the images; LBD then runs beside ORB as for the caller's key lines.  With more, ORB runs beside
@@ -1097,8 +1122,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const uint8_t* rectified = nullptr;
     cudaEvent_t rectified_ready = nullptr;
     if (rect && (pts || lns)) {
-        if (const int rc = rectify_call(ctx, rect, session, session ? session->ids : nullptr, NF, n_img, iparts, ctx->s_main,
-                                        &rectified, &d_rgb))
+        if (const int rc = rectify_call(ctx, rect, call, NF, n_img, iparts, ctx->s_main, &rectified, &d_rgb))
             return rc;
         rectified_ready = next_event(ctx);
         CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
@@ -1106,7 +1130,7 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const uint8_t* orb_images = rectified;   // the device images ORB reads (null: ORB uploads them)
     if (lsd_first) {
         if (const int rc = lsd_enqueue(ctx, lsd, rectified, nullptr, stage_parts, ctx->s_main)) return rc;
-        if (const int rc = lsd_lines(ctx->s_main)) return rc;
+        if (const int rc = lines.take_lsd(ctx, lc, lsd, ctx->s_main, nblk, NF)) return rc;
         orb_images = lsd.images;
     }
     const bool lsd_beside = run_lsd && !lsd_first;
@@ -1120,18 +1144,18 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     OrbDetected orb;
     if (pts) {
         std::function<int(const uint8_t*, cudaEvent_t)> beside;
-        if (lsd_beside || run_lbd) beside = lines_beside;
+        if (lsd_beside || lines.run_lbd) beside = lines_beside;
         if (const int rc = orb_detect_enqueue(ctx, oc, n_img, W, H, orb_images, stage_parts, th.data(), INT_MAX, beside, orb))
             return rc;
     } else {
         orb.off.assign((size_t)n_img + 1, 0);
-        if (lsd_beside || run_lbd)
+        if (lsd_beside || lines.run_lbd)
             if (const int rc = lines_beside(rectified, rectified_ready)) return rc;
     }
     if (lsd_beside) {   // LSD's host continuation (while ORB's selection and descriptors run), then LBD on the same stream
-        if (const int rc = lsd_lines(ctx->s_alt)) return rc;
+        if (const int rc = lines.take_lsd(ctx, lc, lsd, ctx->s_alt, nblk, NF)) return rc;
         d_images = lsd.images;   // ORB's copy, or LSD's own when ORB does not run
-        if (run_lbd)
+        if (lines.run_lbd)
             if (const int rc = enqueue_lbd()) return rc;
     }
     // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
@@ -1139,17 +1163,16 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     PlStereoFeatures feat[2]{};
     StereoDevInputs dev;
     for (int j = 0; j < nfs; ++j)
-        stereo_set_inputs(orb, 2 * j, pts, lsrc, 2 * j, lns, run_lbd, lbase, d_seg, d_ldesc, NF, none, pl_off[j], pr_off[j],
-                          feat[j], dev.set[2 * j], dev.set[2 * j + 1]);
-    dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
+        stereo_set_inputs(orb, 2 * j, pts, lines, 2 * j, NF, none, pl_off[j], pr_off[j], feat[j], dev, 2 * j);
     dev.marks = ctx->img_ev.ev + 1;
     if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], one_set ? nullptr : &feat[1], priors, results,
-                                           n_stereo, sequence, -1, &dev, session))
+                                           n_stereo, sequence, -1, &dev, call))
         return rc;
     float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
     std::fill(ms, ms + 5, 0.f);
     // uploads end where the first stage starts: LSD waits for the images, LBD on the caller's lines for the images and its key
     // lines, ORB for the images only
+    const bool run_lbd = lines.run_lbd;
     const cudaEvent_t up_end = run_lsd ? ctx->lsd_ev[0] : run_lbd ? ctx->lbd_ev[0] : pts ? ctx->orb_det_ev[0] : nullptr;
     if (up_end) CK(ctx, cudaEventElapsedTime(&ms[0], ctx->img_ev[0], up_end));
     if (pts) CK(ctx, cudaEventElapsedTime(&ms[1], ctx->orb_det_ev[0], ctx->orb_det_ev[4]));
@@ -1166,11 +1189,11 @@ static int track_images_common(PlContext* ctx, const PlCamera* cam, const PlConf
                                const PlStereoConfig* sc, const PlOrbDetectConfig* oc, bool detect_lines, const PlLsdConfig* lc,
                                const PlStereoImages* prev, const PlStereoImages* curr, const PlPrior* priors,
                                PlPoseResult* results, int32_t* n_stereo, bool sequence, const PlRectifier* rect = nullptr,
-                               PlStereoSession* session = nullptr) {
+                               SessionCall* call = nullptr) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
     const int rc = track_images_run(ctx, cam, cfg, mc, sc, oc, detect_lines, lc, rect, prev, curr, priors, results, n_stereo,
-                                    sequence, session);
+                                    sequence, call);
     // after an error the line stages may still run on the second stream, and ORB on the first: the next call may reuse their
     // arenas
     const cudaError_t e = cudaStreamSynchronize(ctx->s_alt), e_main = cudaStreamSynchronize(ctx->s_main);
@@ -1322,6 +1345,14 @@ int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
 }
 
 namespace {
+// every session entry point, after the context lock: a session of this context (a read passes ss null where its output is
+// null, with its own message)
+int session_check(PlContext* ctx, const PlStereoSession* ss, const char* null_msg = "null session") {
+    if (!ss) return fail(ctx, PLSTVO_E_INVALID, null_msg);
+    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    return 0;
+}
+
 // every call on a session but the reads discards the key frames a run_keyframes kept (the chunks' frees wait for the device)
 void session_drop_keyframes(PlStereoSession* ss) {
     ss->kf_valid = false;
@@ -1329,6 +1360,32 @@ void session_drop_keyframes(PlStereoSession* ss) {
     ss->kf_steps.clear();
     ss->kf_rows.clear();
     ss->kf_off.clear();
+}
+
+// The start and the end of a call that changes the session: initialize / insert, run and run_keyframes.  The start drops the
+// key frames and, with discard, invalidates what the last call retained.  The end of a failed call (rc) does both and
+// synchronises both streams: the line stages may still run on the second stream, and ORB or a step on the first, and the
+// next call may reuse their arenas.  The end of a successful one marks the retention arena as the call's (track, n): an empty
+// call (n = 0) retains nothing, and a run of T = 0 (ran false) leaves it as it was.
+void session_start(PlStereoSession* ss, bool discard) {
+    if (discard) ss->kept.valid = false;
+    session_drop_keyframes(ss);
+}
+
+int session_finish(PlContext* ctx, PlStereoSession* ss, int rc, bool track, int n, bool ran = true) {
+    if (rc) {
+        ss->kept.valid = false;
+        session_drop_keyframes(ss);
+        cudaStreamSynchronize(ctx->s_alt);
+        cudaStreamSynchronize(ctx->s_main);
+        return rc;
+    }
+    if (ran && ss->retain) {
+        ss->kept.track = track;
+        ss->kept.n = n;
+        ss->kept.valid = n > 0 || ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
+    }
+    return 0;
 }
 
 // the caller's arrays of a PlStereoFrameOut, indexed by records.h's arrays
@@ -1343,8 +1400,7 @@ RecPtrs frame_out_records(const PlStereoFrameOut* o) {
 int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (const int rc = session_check(ctx, ss)) return rc;
     if (on && ss->retain) return 0;   // already on: what the last call retained stays readable
     ss->retain = on != 0;
     session_drop_keyframes(ss);
@@ -1359,8 +1415,7 @@ int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
 int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* ss, const PlStereoFrameOut* out) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss || !out) return fail(ctx, PLSTVO_E_INVALID, "null session or output");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (const int rc = session_check(ctx, out ? ss : nullptr, "null session or output")) return rc;
     if (!ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
     const SessionRetained& kr = ss->kept;
     if (!kr.valid) return fail(ctx, PLSTVO_E_INVALID, "nothing retained: no call succeeded since retention was turned on, or the last call failed");
@@ -1390,66 +1445,48 @@ int session_check_ids(PlContext* ctx, const PlStereoSession* ss, bool track, int
     return 0;
 }
 
-// the call in progress on checked streams; for an insert, their kept frames compact in call order (the tracker's previous
-// frames) and their counts into n_stereo's columns 0, 1
-void session_begin(PlStereoSession* ss, bool track, int n, const int32_t* ids, int32_t* n_stereo) {
-    ss->track = track;
-    ss->n = n;
-    ss->ids = ids;
-    if (!track) return;
-    ss->kept_off_pt.assign((size_t)n + 1, 0);
-    ss->kept_off_ls.assign((size_t)n + 1, 0);
+// A call (or run step) on checked streams ids[0 .. n), filling the retention arena while retention is on; for an insert, the
+// streams' kept frames compact in call order (the tracker's previous frames)
+SessionCall session_begin(PlStereoSession* ss, bool track, int n, const int32_t* ids) {
+    SessionCall c{ss, track, ss->retain, n, ids};
+    if (!track) return c;
+    c.kept_off_pt.assign((size_t)n + 1, 0);
+    c.kept_off_ls.assign((size_t)n + 1, 0);
     for (int k = 0; k < n; ++k) {
         const size_t id = (size_t)ids[k];
-        ss->kept_off_pt[(size_t)k + 1] = ss->kept_off_pt[(size_t)k] + ss->n_pt[id];
-        ss->kept_off_ls[(size_t)k + 1] = ss->kept_off_ls[(size_t)k] + ss->n_ls[id];
-        if (n_stereo) {
-            n_stereo[4 * (size_t)k] = ss->n_pt[id];
-            n_stereo[4 * (size_t)k + 1] = ss->n_ls[id];
-        }
+        c.kept_off_pt[(size_t)k + 1] = c.kept_off_pt[(size_t)k] + ss->n_pt[id];
+        c.kept_off_ls[(size_t)k + 1] = c.kept_off_ls[(size_t)k] + ss->n_ls[id];
     }
+    return c;
 }
 
-// initialize (track == false) or insert for streams ids[0 .. n): the checks, then the images path in session mode; the pools
-// flip and the streams' counts are kept only when the whole call succeeded
+// initialize (track == false) or insert for streams ids[0 .. n) after the session's start: the checks, then the images path
+// with the call's record; the pools flip and the streams' counts are kept only when the whole call succeeded
+int session_images(PlContext* ctx, PlStereoSession* ss, bool track, int n, const int32_t* ids, const PlStereoImages* frames,
+                   const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
+    if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
+    if (frames->B != n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from n");
+    if (n == 0) return 0;
+    if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
+    if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
+    if (const int rc = session_check_ids(ctx, ss, track, n, ids)) return rc;
+    if (const int rc = check_key_line_fields(ctx, &frames, 1, false, ss->fld && !ss->cfg.has_lines, false)) return rc;
+    SessionCall call = session_begin(ss, track, n, ids);
+    // the FLD branch: the caller's key lines (the images call's checks), LSD and its config unused
+    const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, !ss->fld,
+                                       !ss->fld && ss->has_lc ? &ss->lc : nullptr, frames, nullptr, priors, results, n_stereo,
+                                       false, ss->rect, &call);
+    if (rc == 0) session_commit(call);
+    return rc;
+}
+
 int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const int32_t* ids, const PlStereoImages* frames,
                  const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
-    ss->kept.valid = false;   // a failed call discards what the last one retained
-    session_drop_keyframes(ss);
-    if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
-    if (frames->B != n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from n");
-    if (n == 0) {
-        if (ss->retain) {   // an empty call succeeds and retains nothing
-            ss->kept.track = track;
-            ss->kept.n = 0;
-            ss->kept.valid = ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
-        }
-        return 0;
-    }
-    if (!ids) return fail(ctx, PLSTVO_E_INVALID, "null ids");
-    if (2L * n > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
-    if (const int rc = session_check_ids(ctx, ss, track, n, ids)) return rc;
-    if (ss->fld && !ss->cfg.has_lines && key_lines_given(frames))
-        return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the session has no lines");
-    session_begin(ss, track, n, ids, n_stereo);
-    // the FLD branch: the caller's key lines (the images call's checks), LSD and its config unused
-    const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, !ss->fld,
-                                       !ss->fld && ss->has_lc ? &ss->lc : nullptr, frames, nullptr, priors, results, n_stereo,
-                                       false, ss->rect, ss);
-    if (rc == 0) {
-        session_commit(ss);
-        if (ss->retain) {
-            ss->kept.track = track;
-            ss->kept.n = n;
-            ss->kept.valid = true;
-        }
-    }
-    ss->ids = nullptr;   // the caller's array: not read after the call
-    return rc;
+    if (const int rc = session_check(ctx, ss)) return rc;
+    session_start(ss, true);
+    return session_finish(ctx, ss, session_images(ctx, ss, track, n, ids, frames, priors, results, n_stereo), track, n);
 }
 }  // namespace
 
@@ -1466,8 +1503,7 @@ int plstvo_stereo_session_insert(PlContext* ctx, PlStereoSession* ss, int n, con
 int plstvo_stereo_session_use_fld_lines(PlContext* ctx, PlStereoSession* ss, int on) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (const int rc = session_check(ctx, ss)) return rc;
     for (uint8_t l : ss->live)
         if (l) return fail(ctx, PLSTVO_E_INVALID, "a stream holds a frame: switch the line branch before any stream is initialised");
     ss->fld = on != 0;
@@ -1490,7 +1526,7 @@ void plstvo_kitti_handler_config(PlHandlerConfig* h) {
 namespace {
 // plstvo_stereo_session_run after the context lock: the checks, then the state-independent stages once over every image
 // (upload, rectifier, LSD, LBD) and the steps (ORB at the device threshold row, the stereo step, tracking, the handler
-// update), each committed to the session as an insert is.  The caller synchronises both streams afterwards.  With kc
+// update), each committed to the session as an insert is.  session_finish synchronises both streams after a failure.  With kc
 // (plstvo_stereo_session_run_keyframes) each step also runs the key-frame test from kf_state's streams and, with retention
 // on, keeps every step's records and copies the key frames' into the session's chunks; kf_state is written on success only.
 int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
@@ -1505,11 +1541,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
     if ((long long)frames->B != (long long)T * n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from T * n");
     const bool lns = ss->cfg.has_lines != 0, fld = ss->fld && lns;   // fld: the caller's key lines, step-major
-    if (!ss->fld && (frames->fast_th || key_lines_given(frames)))
-        return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th and the key-line fields must be null: the run sets its thresholds and detects its key lines");
-    if (ss->fld && frames->fast_th) return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th must be null: the run sets its thresholds");
-    if (ss->fld && !lns && key_lines_given(frames))
-        return fail(ctx, PLSTVO_E_INVALID, "key-line fields must be null: the session has no lines");
+    if (const int rc = check_key_line_fields(ctx, &frames, 1, !ss->fld, ss->fld && !lns, true)) return rc;
     const PlOrbDetectConfig* oc = &ss->oc;
     std::vector<int32_t> th0((size_t)2 * n);   // row 0 of the threshold table, [left n][right n]
     for (int k = 0; k < n; ++k) {
@@ -1543,32 +1575,12 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (n > 0) {   // the session was created with an LSD config wherever it has lines
         if (const int rc = images_check(ctx, W, H, pts, lns, &frames, 1, lns && !fld ? &ss->lc : nullptr, n_img, lsd)) return rc;
     }
-    // the caller's key lines as line blocks: 2 t, 2 t + 1 are step t's left and right images, offsets rebased to 0
+    // the key lines as line blocks: 2 t, 2 t + 1 are step t's left and right images (FLD: the caller's, cut here)
     const int nblk = 2 * T;
-    std::vector<LineSrc> lsrc;
-    DetectedLines det;
-    if (fld && n > 0) {
-        const LineSrc given[2] = {LineSrc{n * T, frames->ll_off, frames->seg_l, frames->angle_l, frames->npix_l},
-                                  LineSrc{n * T, frames->lr_off, frames->seg_r, frames->angle_r, frames->npix_r}};
-        for (const LineSrc& l : given)
-            if (const int rc = lbd_check_lines(ctx, l)) return rc;
-        det.off.assign((size_t)nblk, {});
-        for (int b = 0; b < nblk; ++b) {
-            const LineSrc& l = given[b % 2];
-            const int32_t* o = l.off + (size_t)(b / 2) * n;
-            std::vector<int32_t>& off = det.off[(size_t)b];
-            for (int i = 0; i <= n; ++i) off.push_back(o[i] - o[0]);
-            lsrc.push_back(LineSrc{n, off.data(), l.seg + 4 * (size_t)o[0], l.angle + o[0], l.npix + o[0]});
-        }
-    }
-    if (n == 0) {   // T empty inserts: they succeed and retain nothing
-        if (ss->retain) {
-            ss->kept.track = true;
-            ss->kept.n = 0;
-            ss->kept.valid = ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
-        }
-        return 0;
-    }
+    LineBlocks lines;
+    if (fld && n > 0)
+        if (const int rc = lines.cut(ctx, &frames, 1, T, n)) return rc;
+    if (n == 0) return 0;   // T empty inserts
     CK(ctx, cudaSetDevice(ctx->device));
     CK(ctx, ctx->img_ev.create());
     CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
@@ -1611,8 +1623,9 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     }
     const uint8_t* d_img = nullptr;
     const uint8_t* d_rgb = nullptr;   // a colour FLD session's RGB2GRAY plane, which LBD reads
+    SessionCall step = session_begin(ss, true, n, ids);   // step 0's; each later step's follows the commit of the one before
     if (prepare) {
-        if (const int rc = rectify_call(ctx, rect, ss, ids, n, n_img, iparts, s, &d_img, &d_rgb)) return rc;
+        if (const int rc = rectify_call(ctx, rect, &step, n, n_img, iparts, s, &d_img, &d_rgb)) return rc;
     } else if (pts || lns) {
         size_t o = o_img;
         for (const ImgPart& ip : iparts) {
@@ -1624,24 +1637,14 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     CK(ctx, cudaEventRecord(run_ev[1], s));
     // the lines of every image: LSD alone on the main stream (FLD: the caller's), then LBD on the second stream beside step
     // 0's ORB
-    std::vector<int32_t> lbase((size_t)nblk + 1, 0);
-    const float* d_seg = nullptr;
-    const uint8_t* d_ldesc = nullptr;
-    bool run_lbd = false;
-    if (lns) {
-        if (!fld) {
-            if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
-            if (const int rc = lsd_line_sources(ctx, &ss->lc, lsd, s, nblk, n, det, lsrc)) return rc;
-        }
-        for (int b = 0; b < nblk; ++b) lbase[(size_t)b + 1] = lbase[(size_t)b] + lsrc[(size_t)b].off[n];
-        run_lbd = lbase[(size_t)nblk] > 0;
-        if (run_lbd) {
-            cudaEvent_t ready = next_event(ctx);
-            CK(ctx, cudaEventRecord(ready, s));
-            if (const int rc = lbd_enqueue(ctx, W, H, lsrc, d_rgb ? d_rgb : d_img, ready, {}, ctx->s_alt, &d_seg, &d_ldesc))
-                return rc;
-            CK(ctx, cudaEventRecord(ctx->img_join[0], ctx->s_alt));
-        }
+    if (lns && !fld) {
+        if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
+        if (const int rc = lines.take_lsd(ctx, &ss->lc, lsd, s, nblk, n)) return rc;
+    }
+    if (lines.run_lbd) {
+        cudaEvent_t ready = next_event(ctx);
+        CK(ctx, cudaEventRecord(ready, s));
+        if (const int rc = lines.describe(ctx, W, H, d_rgb ? d_rgb : d_img, ready, {})) return rc;
     }
     float* ms = ctx->img_ms;
     std::fill(ms, ms + 5, 0.f);
@@ -1653,8 +1656,8 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     };
     std::vector<int32_t> none((size_t)n + 1, 0), pl_off, pr_off;
     for (int t = 0; t < T; ++t) {
-        int32_t* ns = n_stereo ? n_stereo + (size_t)t * 4 * n : nullptr;
-        session_begin(ss, true, n, ids, ns);
+        if (t > 0) step = session_begin(ss, true, n, ids);
+        step.retain = keep && (kc || t == T - 1);   // the retention arena holds the last step (every step for the key frames)
         OrbDetected orb;
         if (pts) {
             if (const int rc = orb_detect_enqueue(ctx, oc, 2 * n, W, H, d_img + (size_t)t * step_px, {}, nullptr, INT_MAX,
@@ -1665,9 +1668,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         }
         PlStereoFeatures feat;
         StereoDevInputs dev;
-        stereo_set_inputs(orb, 0, pts, lsrc, 2 * t, lns, run_lbd, lbase, d_seg, d_ldesc, n, none, pl_off, pr_off, feat,
-                          dev.set[0], dev.set[1]);
-        dev.lines_ready = run_lbd ? ctx->img_join[0] : nullptr;
+        stereo_set_inputs(orb, 0, pts, lines, 2 * t, n, none, pl_off, pr_off, feat, dev, 0);
         cudaEvent_t* mk = marks[t % 2].ev;
         dev.marks = mk;
         dev.priors_resident = t > 0;   // step t - 1's handler update wrote them
@@ -1685,7 +1686,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
                     GatherSeg* seg = kf_segs.data() + (size_t)t * n;
                     int32_t np = 0, nl = 0;
                     for (int k = 0; k < n; ++k) {
-                        seg[k] = GatherSeg{np, np, ss->new_pt[(size_t)k], nl, nl, ss->new_ls[(size_t)k]};
+                        seg[k] = GatherSeg{np, np, step.new_pt[(size_t)k], nl, nl, step.new_ls[(size_t)k]};
                         np += seg[k].n_pt;
                         nl += seg[k].n_ls;
                     }
@@ -1707,12 +1708,11 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
             CK(ctx, cudaStreamWaitEvent(ctx->s_h2d, step_done, 0));
             return 0;
         };
-        ss->retain = keep && (kc || t == T - 1);   // the retention arena holds the last step (every step for the key frames)
+        int32_t* ns = n_stereo ? n_stereo + (size_t)t * 4 * n : nullptr;
         const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, &feat, nullptr, t == 0 ? priors : nullptr,
-                                           results + (size_t)t * n, ns, false, -1, &dev, ss);
-        ss->retain = keep;
+                                           results + (size_t)t * n, ns, false, -1, &dev, &step);
         if (rc) return rc;
-        session_commit(ss);
+        session_commit(step);
         // the stereo step's count readback synchronised the main stream: this step's ORB and the last step are done
         if (pts)
             if (const int rc2 = add_ms(1, ctx->orb_det_ev[0], ctx->orb_det_ev[4])) return rc2;
@@ -1738,15 +1738,10 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     if (const int rc = add_ms(4, pm[1], pm[2])) return rc;
     if (const int rc = add_ms(0, run_ev[0], run_ev[1])) return rc;
     if (lns && !fld)
-        if (const int rc = add_ms(2, ctx->lsd_ev[0], run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5])) return rc;
-    if (fld && run_lbd)
+        if (const int rc = add_ms(2, ctx->lsd_ev[0], lines.run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5])) return rc;
+    if (fld && lines.run_lbd)
         if (const int rc = add_ms(2, ctx->lbd_ev[0], ctx->lbd_ev[2])) return rc;
     ctx->img_timed = true;
-    if (keep) {
-        ss->kept.track = true;
-        ss->kept.n = n;
-        ss->kept.valid = true;
-    }
     if (kc) {
         std::copy(kfs_out.begin(), kfs_out.end(), kf_state);
         for (int t = 0; keep && t < T; ++t)
@@ -1766,18 +1761,10 @@ int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* ss, const PlHandl
                               PlPoseResult* results, int32_t* fast_th, int32_t* n_stereo) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
-    session_drop_keyframes(ss);
+    if (const int rc = session_check(ctx, ss)) return rc;
+    session_start(ss, false);   // a run of T = 0 leaves what the last call retained readable
     const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo);
-    ss->ids = nullptr;   // the caller's array: not read after the call
-    if (rc) {
-        ss->kept.valid = false;   // a failed call discards what the last one retained
-        // the line stages may still run on the second stream, and a step on the first: the next call may reuse their arenas
-        cudaStreamSynchronize(ctx->s_alt);
-        cudaStreamSynchronize(ctx->s_main);
-    }
-    return rc;
+    return session_finish(ctx, ss, rc, true, n, T > 0);
 }
 
 /* ---- the same loop with the key-frame test ---- */
@@ -1799,10 +1786,8 @@ int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* ss, con
                                         PlKeyframeResult* kf, int32_t* fast_th, int32_t* n_stereo) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss) return fail(ctx, PLSTVO_E_INVALID, "null session");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
-    ss->kept.valid = false;   // what the last call retained, and its key frames, are discarded by this one
-    session_drop_keyframes(ss);
+    if (const int rc = session_check(ctx, ss)) return rc;
+    session_start(ss, true);   // what the last call retained is discarded, also by a run of T = 0
     if (!k || !kf_state || !kf) return fail(ctx, PLSTVO_E_INVALID, "null key-frame config, state or results");
     if (std::isnan(k->min_entropy_ratio) || std::isnan(k->max_kf_t_dist) || std::isnan(k->max_kf_r_dist))
         return fail(ctx, PLSTVO_E_INVALID, "NaN in the key-frame config");
@@ -1810,23 +1795,14 @@ int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* ss, con
         if ((kf_state[i].prev_f_iskf != 0 && kf_state[i].prev_f_iskf != 1) || kf_state[i].N_prevKF_currF < 0)
             return fail(ctx, PLSTVO_E_INVALID, "key-frame state with prev_f_iskf outside {0, 1} or a negative N_prevKF_currF");
     const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo, k, kf_state, kf);
-    ss->ids = nullptr;   // the caller's array: not read after the call
-    if (rc) {
-        ss->kept.valid = false;
-        session_drop_keyframes(ss);
-        cudaStreamSynchronize(ctx->s_alt);
-        cudaStreamSynchronize(ctx->s_main);
-        return rc;
-    }
-    ss->kf_valid = ss->retain;
-    return 0;
+    if (session_finish(ctx, ss, rc, true, n, T > 0) == 0) ss->kf_valid = ss->retain;
+    return rc;
 }
 
 int plstvo_stereo_session_read_keyframes(PlContext* ctx, const PlStereoSession* ss, const PlStereoFrameOut* out, int32_t* rows) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    if (!ss || !out) return fail(ctx, PLSTVO_E_INVALID, "null session or output");
-    if (ss->ctx != ctx) return fail(ctx, PLSTVO_E_INVALID, "the session belongs to another context");
+    if (const int rc = session_check(ctx, out ? ss : nullptr, "null session or output")) return rc;
     if (!ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
     if (!ss->kf_valid) return fail(ctx, PLSTVO_E_INVALID, "no key frames kept: the last call on the session was not a successful run_keyframes");
     CK(ctx, cudaSetDevice(ctx->device));

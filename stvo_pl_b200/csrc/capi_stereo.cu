@@ -265,19 +265,19 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
 // sequence == false: B independent (prev, curr) pairs, four feature sets of B frames.
 // sequence == true : prev holds NF = B + 1 consecutive frames, pair p = (frame p, frame p + 1); two feature sets of NF frames,
 //                    every frame goes through the stereo step once and is lifted twice (as a previous and as a current frame).
-// session != null  : prev holds the NF = B new frames of the session's streams ids[0 .. B) (curr is unused).  Each new frame goes
-//                    through the stereo step once and is lifted twice: as the current frame of pair p into the workspace, and
-//                    in the previous-frame role into the session's next pool.  The streams' kept frames are gathered into the
-//                    workspace's previous-frame arrays (insert; initialize tracks nothing and takes no results).
+// call != null     : prev holds the NF = B new frames of a session call's streams ids[0 .. B) (curr is unused).  Each new frame
+//                    goes through the stereo step once and is lifted twice: as the current frame of pair p into the workspace,
+//                    and in the previous-frame role into the session's next pool.  The streams' kept frames are gathered into
+//                    the workspace's previous-frame arrays (insert; initialize tracks nothing and takes no results).
 int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                 const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                                 const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                                const StereoDevInputs* dev, PlStereoSession* session) {
+                                const StereoDevInputs* dev, SessionCall* call) {
     // slot < 0: blocking (returns with the results in host memory); slot 0 / 1: enqueue only, results valid after plstvo_wait
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
-    const bool one_set = sequence || session;       // two feature sets (points, lines of one frame set)
-    const bool track = !session || session->track;
+    const bool one_set = sequence || call;          // two feature sets (points, lines of one frame set)
+    const bool track = !call || call->track;
     if (!cam || !cfg || !mc || !sc || !prev || (!one_set && !curr) || (track && !results))
         return fail(ctx, PLSTVO_E_INVALID, "null argument");
     const int NF = prev->B;                         // frames per feature set
@@ -417,8 +417,12 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             ooff[k][p + 1] = ooff[k][p] + cnt[(size_t)k * NF + p];
             if (n_stereo) {
                 if (sequence || !track) n_stereo[(size_t)p * 2 + k] = cnt[(size_t)k * NF + p];
-                else if (session) n_stereo[(size_t)p * 4 + 2 + k] = cnt[(size_t)k * NF + p];
-                else n_stereo[(size_t)p * 4 + k] = cnt[(size_t)k * NF + p];
+                else if (!call) n_stereo[(size_t)p * 4 + k] = cnt[(size_t)k * NF + p];
+                else {   // an insert: the kept frame's counts, then the new frame's
+                    const std::vector<int32_t>& kept = k ? call->kept_off_ls : call->kept_off_pt;
+                    n_stereo[(size_t)p * 4 + k] = kept[(size_t)p + 1] - kept[(size_t)p];
+                    n_stereo[(size_t)p * 4 + 2 + k] = cnt[(size_t)k * NF + p];
+                }
             }
         }
         CK(ctx, a.up(sets[k].o_ooff, ooff[k].data(), (size_t)(NF + 1) * 4, sh));
@@ -429,27 +433,28 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         }
     }
     // a cams session: the camera of each new frame (its stream's), for pass 2's lifts and for the solver (pair p = frame p)
+    PlStereoSession* const ss = call ? call->ss : nullptr;
     const PlCamera* d_cams = nullptr;
-    if (session && !session->cams.empty()) {
+    if (ss && !ss->cams.empty()) {
         std::vector<PlCamera> fc((size_t)NF);
-        for (int k = 0; k < NF; ++k) fc[(size_t)k] = session->cams[(size_t)session->ids[k]];
-        CK(ctx, session->d_cams.ensure((size_t)NF * sizeof(PlCamera)));
-        CK(ctx, cudaMemcpyAsync(session->d_cams.p, fc.data(), (size_t)NF * sizeof(PlCamera), cudaMemcpyHostToDevice, s));
-        d_cams = session->d_cams.as<PlCamera>();
+        for (int k = 0; k < NF; ++k) fc[(size_t)k] = ss->cams[(size_t)call->ids[k]];
+        CK(ctx, ss->d_cams.ensure((size_t)NF * sizeof(PlCamera)));
+        CK(ctx, cudaMemcpyAsync(ss->d_cams.p, fc.data(), (size_t)NF * sizeof(PlCamera), cudaMemcpyHostToDevice, s));
+        d_cams = ss->d_cams.as<PlCamera>();
     }
     // pass 2: the same lifting kernels, now writing at the compact offsets: the previous-frame role (a pool's or the
     // workspace's PREV_ROLE entries), the current-frame role (curr_rows below) and retention (every array)
     // session: the new frames' previous-frame role goes into the next pool, the untouched streams' kept frames follow it there
-    if (session) {
-        if (const int rc = session_plan(ctx, session, cnt, cnt + NF, s)) return rc;
+    if (call) {
+        if (const int rc = session_plan(ctx, *call, cnt, cnt + NF, s)) return rc;
         for (int k = 0; k < 2; ++k)
-            CK(ctx, lift(sets[k], B, 0, session->pool[session->cur ^ 1].rows, session_out_off(session, k == 1), d_cams));
+            CK(ctx, lift(sets[k], B, 0, ss->pool[ss->cur ^ 1].rows, session_out_off(*call, k == 1), d_cams));
         ctx->launches += 2;
-        if (const int rc = session_gather_others(ctx, session, s)) return rc;
-        if (session->retain) {   // plstvo_stereo_session_read: every record of the new frames, compact in call order
-            SessionRetained& kr = session->kept;
-            CK(ctx, kr.lay_out((size_t)ooff[0][NF], (size_t)ooff[1][NF], track ? (size_t)session->kept_off_pt[NF] : 0,
-                               track ? (size_t)session->kept_off_ls[NF] : 0));
+        if (const int rc = session_gather_others(ctx, *call, s)) return rc;
+        if (call->retain) {   // plstvo_stereo_session_read: every record of the new frames, compact in call order
+            SessionRetained& kr = ss->kept;
+            CK(ctx, kr.lay_out((size_t)ooff[0][NF], (size_t)ooff[1][NF], track ? (size_t)call->kept_off_pt[NF] : 0,
+                               track ? (size_t)call->kept_off_ls[NF] : 0));
             cudaEvent_t offsets_up = next_event(ctx);   // sets[k].o_ooff, uploaded on sh above
             CK(ctx, cudaEventRecord(offsets_up, sh));
             CK(ctx, cudaStreamWaitEvent(s, offsets_up, 0));
@@ -468,10 +473,10 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     // ---- the tracker's plan on the compact lists; the records are written straight into its buffers ----
     PlFrameBatch fp{}, fc{};
     fp.B = fc.B = B;
-    fp.pt_off = session ? session->kept_off_pt.data() : ooff[0].data();
-    fp.ls_off = session ? session->kept_off_ls.data() : ooff[1].data();
-    fc.pt_off = sequence ? ooff2[0].data() : session ? ooff[0].data() : ooff[2].data();
-    fc.ls_off = sequence ? ooff2[1].data() : session ? ooff[1].data() : ooff[3].data();
+    fp.pt_off = call ? call->kept_off_pt.data() : ooff[0].data();
+    fp.ls_off = call ? call->kept_off_ls.data() : ooff[1].data();
+    fc.pt_off = sequence ? ooff2[0].data() : call ? ooff[0].data() : ooff[2].data();
+    fc.ls_off = sequence ? ooff2[1].data() : call ? ooff[1].data() : ooff[3].data();
     Workspace& ws = slot < 0 ? ctx->ws : ctx->ws_async[slot];
     const bool resident = dev && dev->priors_resident;   // ws_prepare keeps d_priors: B is the run's n at every step
     int rc = ws_prepare(ctx, ws, cam, cfg, &fp, &fc, true, priors != nullptr || resident, d_cams);
@@ -481,8 +486,8 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     cudaEvent_t planned = next_event(ctx);
     CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(s, planned, 0));
-    if (session) {
-        if (const int rc2 = session_gather_named(ctx, session, workspace_prev_rows(ws), s)) return rc2;
+    if (call) {
+        if (const int rc2 = session_gather_named(ctx, *call, workspace_prev_rows(ws), s)) return rc2;
     } else {
         for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], B, 0, workspace_prev_rows(ws), a.i32(sets[k].o_ooff), d_cams));
     }
@@ -497,15 +502,15 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
         const Set& st = sets[one_set ? k : 2 + k];
         CK(ctx, lift(st, B, first, curr_rows, a.i32(sequence ? st.o_ooff2 : st.o_ooff), d_cams));
     }
-    ctx->launches += session ? 2 : 4;
+    ctx->launches += call ? 2 : 4;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
     rc = ws_launch_match(ctx, ws, 0, B, s);
     if (rc) return rc;
     rc = ws_launch_solve(ctx, ws, 0, B, true, s);
     if (rc) return rc;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[2], s));
-    if (session && session->retain) {   // the tracker's rows, indexed by the kept frames' features (fp's offsets)
-        const SessionRetained& kr = session->kept;
+    if (call && call->retain) {   // the tracker's rows, indexed by the kept frames' features (fp's offsets)
+        const SessionRetained& kr = ss->kept;
         const DevBuf* src[4] = {&ws.d_m12p, &ws.d_inlp, &ws.d_m12l, &ws.d_inll};
         for (int k = 0; k < 4; ++k) {
             const int r = M12_PT + k;

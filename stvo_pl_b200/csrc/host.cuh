@@ -462,16 +462,7 @@ struct PlStereoSession {
     std::vector<int32_t> off_pt, off_ls;    // [S] its first rows in pool[cur]
     plstvo::SessionPool pool[2];
     int cur = 0;
-    plstvo::DevBuf d_meta;                  // this call's lift output offsets and gather segments
-    // ---- the call in progress (plstvo::session_plan), committed by plstvo::session_commit ----
-    bool track = false;                     // insert (true) or initialize
-    int n = 0;
-    const int32_t* ids = nullptr;
-    std::vector<int32_t> kept_off_pt, kept_off_ls;   // [n + 1] the named streams' kept frames, compact (insert)
-    std::vector<int32_t> next_off_pt, next_off_ls;   // [S] first rows in pool[cur ^ 1]
-    std::vector<int32_t> new_pt, new_ls;             // [n] the new frames' stereo points / lines
-    std::vector<int32_t> meta;                       // uploaded: out_off_pt [n], out_off_ls [n], GatherSeg named [n], others
-    int n_others = 0;
+    plstvo::DevBuf d_meta;                  // a call's lift output offsets and gather segments
     // ---- plstvo_stereo_session_retain / _read ----
     bool retain = false;
     plstvo::SessionRetained kept;                    // the last call's records while retain is on
@@ -484,18 +475,33 @@ struct PlStereoSession {
 
 namespace plstvo {
 
+// One call on a session, or one step of a session run, on the entry point's stack: the streams it names, and the plan
+// session_plan makes for them, committed to the session by session_commit.
+struct SessionCall {
+    PlStereoSession* ss = nullptr;
+    bool track = false;                     // insert (true) or initialize
+    bool retain = false;                    // the call fills the session's retention arena
+    int n = 0;
+    const int32_t* ids = nullptr;           // the caller's array
+    std::vector<int32_t> kept_off_pt, kept_off_ls;   // [n + 1] the named streams' kept frames, compact (insert)
+    std::vector<int32_t> next_off_pt, next_off_ls;   // [S] first rows in pool[cur ^ 1]
+    std::vector<int32_t> new_pt, new_ls;             // [n] the new frames' stereo points / lines
+    std::vector<int32_t> meta;                       // uploaded: out_off_pt [n], out_off_ls [n], GatherSeg named [n], others
+    int n_others = 0;
+};
+
 // Lays out pool[cur ^ 1] for the new frames' counts (new_pt, new_ls [n], call order) and the untouched streams' kept frames,
 // grows it if need be, and uploads the call's offsets and gather segments on s.  PLSTVO_E_TOO_LARGE: more than INT_MAX rows.
-int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s);
+int session_plan(PlContext* ctx, SessionCall& c, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s);
 // The two moves of a planned call, enqueued on s: the named streams' kept frames from pool[cur] into the workspace's
 // previous-frame arrays at kept_off_pt / kept_off_ls (insert), and the untouched streams' kept frames from pool[cur] into
 // pool[cur ^ 1].  The new frames' previous-frame role goes into pool[cur ^ 1] through the lift kernels, at session_out_off.
-int session_gather_named(PlContext* ctx, PlStereoSession* ss, const RecPtrs& ws_rows, cudaStream_t s);
-int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s);
+int session_gather_named(PlContext* ctx, const SessionCall& c, const RecPtrs& ws_rows, cudaStream_t s);
+int session_gather_others(PlContext* ctx, const SessionCall& c, cudaStream_t s);
 // device offsets [n] of the new frames' first point / line rows in pool[cur ^ 1]
-const int32_t* session_out_off(const PlStereoSession* ss, bool lines);
+const int32_t* session_out_off(const SessionCall& c, bool lines);
 // the call succeeded: pool[cur ^ 1] becomes the kept frames
-void session_commit(PlStereoSession* ss);
+void session_commit(const SessionCall& c);
 // updateFrame's threshold and the next prior of one session-run step, on s for n streams: from the step's results (ws's
 // d_results), th [2 n] (row t of the run's threshold table) -> th + 2 n (row t + 1, both halves), priors [n] (ws's d_priors),
 // and the results copied to res_out [n]
@@ -525,7 +531,7 @@ struct StereoDevInputs {
 int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                         const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                         const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                        const StereoDevInputs* dev = nullptr, PlStereoSession* session = nullptr);
+                        const StereoDevInputs* dev = nullptr, SessionCall* call = nullptr);
 
 // ---- rectify.cu: rectifyImagesLR on the device, composed by the raw-images path ----
 struct ImgPart {   // consecutive host images of one size

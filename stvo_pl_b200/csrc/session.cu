@@ -79,9 +79,9 @@ __global__ void session_handler_kernel(PlHandlerConfig h, int n, const PlPoseRes
     res_out[k] = r;
 }
 
-// offsets into PlStereoSession::meta
-size_t meta_named(const PlStereoSession* ss) { return 2 * (size_t)ss->n; }
-size_t meta_others(const PlStereoSession* ss) { return meta_named(ss) + (size_t)ss->n * (sizeof(GatherSeg) / 4); }
+// offsets into SessionCall::meta
+size_t meta_named(const SessionCall& c) { return 2 * (size_t)c.n; }
+size_t meta_others(const SessionCall& c) { return meta_named(c) + (size_t)c.n * (sizeof(GatherSeg) / 4); }
 
 }  // namespace
 
@@ -136,22 +136,23 @@ cudaError_t SessionRetained::lay_out(size_t new_pt, size_t new_ls, size_t kept_p
     return e;
 }
 
-int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s) {
-    const int S = ss->n_streams, n = ss->n;
+int session_plan(PlContext* ctx, SessionCall& c, const int32_t* new_pt, const int32_t* new_ls, cudaStream_t s) {
+    PlStereoSession* ss = c.ss;
+    const int S = ss->n_streams, n = c.n;
     std::vector<int> slot((size_t)S, -1);   // call position of each named stream
-    for (int k = 0; k < n; ++k) slot[(size_t)ss->ids[k]] = k;
-    ss->new_pt.assign(new_pt, new_pt + n);
-    ss->new_ls.assign(new_ls, new_ls + n);
-    ss->next_off_pt.assign((size_t)S, 0);
-    ss->next_off_ls.assign((size_t)S, 0);
+    for (int k = 0; k < n; ++k) slot[(size_t)c.ids[k]] = k;
+    c.new_pt.assign(new_pt, new_pt + n);
+    c.new_ls.assign(new_ls, new_ls + n);
+    c.next_off_pt.assign((size_t)S, 0);
+    c.next_off_ls.assign((size_t)S, 0);
     std::vector<GatherSeg> others;
     long long tp = 0, tl = 0;
     for (int id = 0; id < S; ++id) {
         const int k = slot[(size_t)id];
         const int np = k >= 0 ? new_pt[k] : ss->live[(size_t)id] ? ss->n_pt[(size_t)id] : 0;
         const int nl = k >= 0 ? new_ls[k] : ss->live[(size_t)id] ? ss->n_ls[(size_t)id] : 0;
-        ss->next_off_pt[(size_t)id] = (int32_t)tp;
-        ss->next_off_ls[(size_t)id] = (int32_t)tl;
+        c.next_off_pt[(size_t)id] = (int32_t)tp;
+        c.next_off_ls[(size_t)id] = (int32_t)tl;
         if (k < 0 && (np || nl))
             others.push_back(GatherSeg{ss->off_pt[(size_t)id], (int32_t)tp, np, ss->off_ls[(size_t)id], (int32_t)tl, nl});
         tp += np;
@@ -160,19 +161,19 @@ int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, con
     }
     CK(ctx, ss->pool[ss->cur ^ 1].ensure((size_t)tp, (size_t)tl));
     // meta: out_off_pt [n], out_off_ls [n], the named streams' segments (kept frame -> the workspace, compact), the others'
-    std::vector<int32_t>& m = ss->meta;
-    m.assign(meta_others(ss), 0);
+    std::vector<int32_t>& m = c.meta;
+    m.assign(meta_others(c), 0);
     for (int k = 0; k < n; ++k) {
-        const int id = ss->ids[k];
-        m[(size_t)k] = ss->next_off_pt[(size_t)id];
-        m[(size_t)n + k] = ss->next_off_ls[(size_t)id];
-        if (ss->track) {
-            const GatherSeg g{ss->off_pt[(size_t)id], ss->kept_off_pt[(size_t)k], ss->n_pt[(size_t)id],
-                              ss->off_ls[(size_t)id], ss->kept_off_ls[(size_t)k], ss->n_ls[(size_t)id]};
-            memcpy(m.data() + meta_named(ss) + (size_t)k * (sizeof(GatherSeg) / 4), &g, sizeof g);
+        const int id = c.ids[k];
+        m[(size_t)k] = c.next_off_pt[(size_t)id];
+        m[(size_t)n + k] = c.next_off_ls[(size_t)id];
+        if (c.track) {
+            const GatherSeg g{ss->off_pt[(size_t)id], c.kept_off_pt[(size_t)k], ss->n_pt[(size_t)id],
+                              ss->off_ls[(size_t)id], c.kept_off_ls[(size_t)k], ss->n_ls[(size_t)id]};
+            memcpy(m.data() + meta_named(c) + (size_t)k * (sizeof(GatherSeg) / 4), &g, sizeof g);
         }
     }
-    ss->n_others = (int)others.size();
+    c.n_others = (int)others.size();
     const size_t o = m.size();
     m.resize(o + others.size() * (sizeof(GatherSeg) / 4));
     if (!others.empty()) memcpy(m.data() + o, others.data(), others.size() * sizeof(GatherSeg));
@@ -181,34 +182,37 @@ int session_plan(PlContext* ctx, PlStereoSession* ss, const int32_t* new_pt, con
     return 0;
 }
 
-int session_gather_named(PlContext* ctx, PlStereoSession* ss, const RecPtrs& ws_rows, cudaStream_t s) {
-    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_named(ss));
-    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ws_rows, true, segs, ss->n, s));
+int session_gather_named(PlContext* ctx, const SessionCall& c, const RecPtrs& ws_rows, cudaStream_t s) {
+    const PlStereoSession* ss = c.ss;
+    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_named(c));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ws_rows, true, segs, c.n, s));
     ctx->launches++;
     return 0;
 }
 
-int session_gather_others(PlContext* ctx, PlStereoSession* ss, cudaStream_t s) {
-    if (!ss->n_others) return 0;
-    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_others(ss));
-    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ss->pool[ss->cur ^ 1].rows, true, segs, ss->n_others, s));
+int session_gather_others(PlContext* ctx, const SessionCall& c, cudaStream_t s) {
+    if (!c.n_others) return 0;
+    const PlStereoSession* ss = c.ss;
+    const GatherSeg* segs = reinterpret_cast<const GatherSeg*>(ss->d_meta.as<int32_t>() + meta_others(c));
+    CK(ctx, launch_session_gather(ss->pool[ss->cur].rows, ss->pool[ss->cur ^ 1].rows, true, segs, c.n_others, s));
     ctx->launches++;
     return 0;
 }
 
-const int32_t* session_out_off(const PlStereoSession* ss, bool lines) {
-    return ss->d_meta.as<int32_t>() + (lines ? ss->n : 0);
+const int32_t* session_out_off(const SessionCall& c, bool lines) {
+    return c.ss->d_meta.as<int32_t>() + (lines ? c.n : 0);
 }
 
-void session_commit(PlStereoSession* ss) {
-    for (int k = 0; k < ss->n; ++k) {
-        const size_t id = (size_t)ss->ids[k];
+void session_commit(const SessionCall& c) {
+    PlStereoSession* ss = c.ss;
+    for (int k = 0; k < c.n; ++k) {
+        const size_t id = (size_t)c.ids[k];
         ss->live[id] = 1;
-        ss->n_pt[id] = ss->new_pt[(size_t)k];
-        ss->n_ls[id] = ss->new_ls[(size_t)k];
+        ss->n_pt[id] = c.new_pt[(size_t)k];
+        ss->n_ls[id] = c.new_ls[(size_t)k];
     }
-    ss->off_pt = ss->next_off_pt;
-    ss->off_ls = ss->next_off_ls;
+    ss->off_pt = c.next_off_pt;
+    ss->off_ls = c.next_off_ls;
     ss->cur ^= 1;
 }
 
