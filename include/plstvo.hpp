@@ -717,6 +717,11 @@ inline int updateFastThreshold(const HandlerConfig& c, int orb_fast_th, const St
     return orb_fast_th;   // the reference's last branch (> 4 feat: + 2 inc, :84-85) is unreachable behind "> 3 feat"
 }
 
+// the identity 6x6 covariance that initialize and currFrameIsKF give a frame's Tfw_cov (src/stereoFrameHandler.cpp:45, :1195)
+inline void identityCov(std::array<double, 36>& cov) {
+    for (int i = 0; i < 36; ++i) cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+}
+
 // Key-frame test on the accumulated pose entropy (src/stereoFrameHandler.cpp:1136-1218; state include/stereoFrameHandler.h:81-86)
 struct KeyframeTest {
     bool prev_f_iskf = true;
@@ -770,7 +775,7 @@ struct KeyframeTest {
     }
     void currFrameIsKF(StereoFrame& curr_frame) {        // :1189-1218 (feature idx renumbering is the caller's: dense order already)
         curr_frame.Tfw = se3::identity4();
-        for (int i = 0; i < 36; ++i) curr_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+        identityCov(curr_frame.Tfw_cov);
         T_prevKF = curr_frame.Tfw;
         cov_prevKF_currF.fill(0.0);
         prev_f_iskf = true;
@@ -798,17 +803,52 @@ inline void publishPose(const PlPoseResult& r, StereoFrame& curr_frame) {
     curr_frame.err_norm = r.err_norm;
 }
 
+// One stream's state of the reference's handler (include/stereoFrameHandler.h:56-86) and the steps on it that do not depend
+// on how the frame reached the device: every handler below holds one per stream and drives it through these.
+struct HandlerState {
+    StereoFrame prev_frame, curr_frame;
+    // the images handlers fill these with keepFeatures on only
+    std::vector<int32_t> matches_pt, matches_ls;         // prev index -> curr index or -1
+    std::vector<uint8_t> inlier_pt, inlier_ls;           // per prev feature: matched and still an inlier
+    int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
+    int orb_fast_th = 20;                                // include/stereoFrameHandler.h:62
+    KeyframeTest kf;
+
+    void initialize(const HandlerConfig& hcfg, StereoFrame frame) {   // src/stereoFrameHandler.cpp:35-52
+        orb_fast_th = hcfg.orb_fast_th;                  // :38 (the threshold the first frame is detected with)
+        prev_frame = std::move(frame);
+        identityCov(prev_frame.Tfw_cov);
+        kf = KeyframeTest{};                             // :48-51
+    }
+    void tracked(const PlPoseResult& r) {                // f2fTracking's matched counts (:126-128)
+        n_inliers_pt = r.n_matched_pt;
+        n_inliers_ls = r.n_matched_ls;
+        n_inliers = n_inliers_pt + n_inliers_ls;
+    }
+    void optimizePose(const PlPoseResult& r) {           // :307-392: publish what the device computed
+        publishPose(r, curr_frame);
+        n_inliers_pt = r.n_inliers_pt;
+        n_inliers_ls = r.n_inliers_ls;
+        n_inliers = r.n_inliers;
+    }
+    void updateFrame(const HandlerConfig& hcfg) {        // :62-102
+        orb_fast_th = updateFastThreshold(hcfg, orb_fast_th, curr_frame, n_inliers_pt);   // :66-86
+        prev_frame = std::move(curr_frame);
+        curr_frame = StereoFrame{};
+    }
+    // key-frame test (:1136-1218), PL-SLAM hooks: state in `kf`
+    bool needNewKF(const HandlerConfig& hcfg) { return kf.needNewKF(hcfg, curr_frame); }
+    void currFrameIsKF() { kf.currFrameIsKF(curr_frame); }
+};
+
 // StereoFrameHandler surface: initialize / insertStereoPair / optimizePose / updateFrame (app/imagesStVO.cpp:88-124)
-class StereoFrameHandler {
+class StereoFrameHandler : public HandlerState {
 public:
     StereoFrameHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const HandlerConfig& hcfg = HandlerConfig{})
         : ctx_(ctx), cam_(cam), cfg_(cfg), hcfg_(hcfg) {}
 
-    void initialize(StereoFrame frame) {                 // src/stereoFrameHandler.cpp:35-52
-        orb_fast_th = hcfg_.orb_fast_th;                 // :38 (the caller extracts features with this threshold)
-        prev_frame = std::move(frame);
-        for (int i = 0; i < 36; ++i) prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
-        kf = KeyframeTest{};                             // :48-51
+    void initialize(StereoFrame frame) {                 // the caller extracts features with orb_fast_th from here on
+        HandlerState::initialize(hcfg_, std::move(frame));
         has_prev_ = true;
     }
     void insertStereoPair(StereoFrame frame) {           // :54-60 (feature extraction is the caller's)
@@ -826,33 +866,12 @@ public:
         inlier_ls.assign(prev_frame.n_ls(), 0);
         ctx_.check(plstvo_track_batch(ctx_.get(), &cam_, &cfg_, &prev, &curr, &prior, &result_, matches_pt.data(),
                                       matches_ls.data(), inlier_pt.data(), inlier_ls.data()));
-        n_inliers_pt = result_.n_matched_pt;             // :126-128
-        n_inliers_ls = result_.n_matched_ls;
-        n_inliers = n_inliers_pt + n_inliers_ls;
+        tracked(result_);
     }
-    void optimizePose() {                                // :307-392: publish what the device computed
-        publishPose(result_, curr_frame);
-        n_inliers_pt = result_.n_inliers_pt;
-        n_inliers_ls = result_.n_inliers_ls;
-        n_inliers = result_.n_inliers;
-    }
-    void updateFrame() {                                 // :62-102
-        orb_fast_th = updateFastThreshold(hcfg_, orb_fast_th, curr_frame, n_inliers_pt);   // :66-86
-        prev_frame = std::move(curr_frame);
-        curr_frame = StereoFrame{};
-    }
-
-    // key-frame test (:1136-1218), PL-SLAM hooks: state in `kf`
-    bool needNewKF() { return kf.needNewKF(hcfg_, curr_frame); }
-    void currFrameIsKF() { kf.currFrameIsKF(curr_frame); }
+    void optimizePose() { HandlerState::optimizePose(result_); }
+    void updateFrame() { HandlerState::updateFrame(hcfg_); }
+    bool needNewKF() { return HandlerState::needNewKF(hcfg_); }
     const PlPoseResult& result() const { return result_; }
-
-    StereoFrame prev_frame, curr_frame;
-    std::vector<int32_t> matches_pt, matches_ls;         // prev index -> curr index or -1
-    std::vector<uint8_t> inlier_pt, inlier_ls;           // per prev feature: matched and still an inlier
-    int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
-    int orb_fast_th = 20;                                // include/stereoFrameHandler.h:62
-    KeyframeTest kf;
 
 private:
     Context& ctx_;
@@ -931,6 +950,29 @@ public:
         std::vector<uint8_t> ldesc;                                                           // [M][32]
         std::vector<int32_t> m12_pt, m12_ls;                                                  // [kept points], [kept lines]
         std::vector<uint8_t> inlier_pt, inlier_ls;
+        // The 19 lifted arrays, once, in PlStereoFrameOut's field order: f(this struct's member, StereoFrame's,
+        // PlStereoFrameOut's, values per row, point (true) or line array) for each
+        template <typename F> static void records(F&& f) {
+            f(&Frames::pt_pl, &StereoFrame::pt_pl, &PlStereoFrameOut::pt_pl, 2, true);
+            f(&Frames::pt_disp, &StereoFrame::pt_disp, &PlStereoFrameOut::pt_disp, 1, true);
+            f(&Frames::pt_P, &StereoFrame::pt_P, &PlStereoFrameOut::pt_P, 3, true);
+            f(&Frames::pt_sigma2, &StereoFrame::pt_sigma2, &PlStereoFrameOut::pt_sigma2, 1, true);
+            f(&Frames::pt_level, &StereoFrame::pt_level, &PlStereoFrameOut::pt_level, 1, true);
+            f(&Frames::pdesc, &StereoFrame::pdesc, &PlStereoFrameOut::pdesc, 32, true);
+            f(&Frames::pt_src, &StereoFrame::pt_src, &PlStereoFrameOut::pt_src, 1, true);
+            f(&Frames::ls_spl, &StereoFrame::ls_spl, &PlStereoFrameOut::ls_spl, 2, false);
+            f(&Frames::ls_epl, &StereoFrame::ls_epl, &PlStereoFrameOut::ls_epl, 2, false);
+            f(&Frames::ls_sdisp, &StereoFrame::ls_sdisp, &PlStereoFrameOut::ls_sdisp, 1, false);
+            f(&Frames::ls_edisp, &StereoFrame::ls_edisp, &PlStereoFrameOut::ls_edisp, 1, false);
+            f(&Frames::ls_sP, &StereoFrame::ls_sP, &PlStereoFrameOut::ls_sP, 3, false);
+            f(&Frames::ls_eP, &StereoFrame::ls_eP, &PlStereoFrameOut::ls_eP, 3, false);
+            f(&Frames::ls_le, &StereoFrame::ls_le, &PlStereoFrameOut::ls_le, 3, false);
+            f(&Frames::ls_angle, &StereoFrame::ls_angle, &PlStereoFrameOut::ls_angle, 1, false);
+            f(&Frames::ls_sigma2, &StereoFrame::ls_sigma2, &PlStereoFrameOut::ls_sigma2, 1, false);
+            f(&Frames::ls_level, &StereoFrame::ls_level, &PlStereoFrameOut::ls_level, 1, false);
+            f(&Frames::ldesc, &StereoFrame::ldesc, &PlStereoFrameOut::ldesc, 32, false);
+            f(&Frames::ls_src, &StereoFrame::ls_src, &PlStereoFrameOut::ls_src, 1, false);
+        }
     };
     void read(int n, const int32_t* n_stereo, bool insert, Frames& out) const {
         const PlStereoFrameOut o = outputs(n, n_stereo, insert, out);
@@ -969,18 +1011,15 @@ private:
                 kl += (size_t)n_stereo[cols * k + 1];
             }
         }
-        out.pt_pl.resize(2 * np); out.pt_disp.resize(np); out.pt_P.resize(3 * np); out.pt_sigma2.resize(np);
-        out.pt_level.resize(np); out.pt_src.resize(np); out.pdesc.resize(32 * np);
-        out.ls_spl.resize(2 * nl); out.ls_epl.resize(2 * nl); out.ls_sdisp.resize(nl); out.ls_edisp.resize(nl);
-        out.ls_sP.resize(3 * nl); out.ls_eP.resize(3 * nl); out.ls_le.resize(3 * nl); out.ls_angle.resize(nl);
-        out.ls_sigma2.resize(nl); out.ls_level.resize(nl); out.ls_src.resize(nl); out.ldesc.resize(32 * nl);
+        PlStereoFrameOut o{};
+        Frames::records([&](auto frames, auto, auto field, size_t per_row, bool point) {
+            (out.*frames).resize(per_row * (point ? np : nl));
+            o.*field = (out.*frames).data();
+        });
         out.m12_pt.assign(kp, -1); out.m12_ls.assign(kl, -1); out.inlier_pt.assign(kp, 0); out.inlier_ls.assign(kl, 0);
-        return PlStereoFrameOut{out.pt_pl.data(), out.pt_disp.data(), out.pt_P.data(), out.pt_sigma2.data(),
-                                 out.pt_level.data(), out.pdesc.data(), out.pt_src.data(), out.ls_spl.data(), out.ls_epl.data(),
-                                 out.ls_sdisp.data(), out.ls_edisp.data(), out.ls_sP.data(), out.ls_eP.data(), out.ls_le.data(),
-                                 out.ls_angle.data(), out.ls_sigma2.data(), out.ls_level.data(), out.ldesc.data(),
-                                 out.ls_src.data(), out.m12_pt.data(), out.inlier_pt.data(), out.m12_ls.data(),
-                                 out.inlier_ls.data()};
+        o.m12_pt = out.m12_pt.data(); o.inlier_pt = out.inlier_pt.data();
+        o.m12_ls = out.m12_ls.data(); o.inlier_ls = out.inlier_ls.data();
+        return o;
     }
     Context& c_;
     PlStereoSession* s_ = nullptr;
@@ -988,18 +1027,45 @@ private:
 };
 
 namespace detail {
-// frame k's rows of a StereoSession::read into f's feature arrays: points [p0, p0 + np), lines [l0, l0 + nl)
-inline void frameFromRead(const StereoSession::Frames& r, size_t p0, size_t np, size_t l0, size_t nl, StereoFrame& f) {
-    auto cut = [](auto& dst, const auto& src, size_t first, size_t count, size_t w) {
-        dst.assign(src.begin() + (std::ptrdiff_t)(first * w), src.begin() + (std::ptrdiff_t)((first + count) * w));
-    };
-    cut(f.pt_pl, r.pt_pl, p0, np, 2); cut(f.pt_disp, r.pt_disp, p0, np, 1); cut(f.pt_P, r.pt_P, p0, np, 3);
-    cut(f.pt_sigma2, r.pt_sigma2, p0, np, 1); cut(f.pt_level, r.pt_level, p0, np, 1); cut(f.pt_src, r.pt_src, p0, np, 1);
-    cut(f.pdesc, r.pdesc, p0, np, 32);
-    cut(f.ls_spl, r.ls_spl, l0, nl, 2); cut(f.ls_epl, r.ls_epl, l0, nl, 2); cut(f.ls_sdisp, r.ls_sdisp, l0, nl, 1);
-    cut(f.ls_edisp, r.ls_edisp, l0, nl, 1); cut(f.ls_sP, r.ls_sP, l0, nl, 3); cut(f.ls_eP, r.ls_eP, l0, nl, 3);
-    cut(f.ls_le, r.ls_le, l0, nl, 3); cut(f.ls_angle, r.ls_angle, l0, nl, 1); cut(f.ls_sigma2, r.ls_sigma2, l0, nl, 1);
-    cut(f.ls_level, r.ls_level, l0, nl, 1); cut(f.ls_src, r.ls_src, l0, nl, 1); cut(f.ldesc, r.ldesc, l0, nl, 32);
+// A StereoSession::read (or readKeyframes) taken apart in call order: each call takes the next frame's rows.
+struct ReadCursor {
+    const StereoSession::Frames& r;
+    size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;   // rows taken: points, lines, then the tracker's kept points, lines
+
+    // the next frame's np points and nl lines into f's feature arrays
+    void frameFromRead(size_t np, size_t nl, StereoFrame& f) {
+        StereoSession::Frames::records([&](auto frames, auto frame, auto, size_t per_row, bool point) {
+            const auto& src = r.*frames;
+            const size_t first = point ? p0 : l0, count = point ? np : nl;
+            (f.*frame).assign(src.begin() + (std::ptrdiff_t)(first * per_row),
+                              src.begin() + (std::ptrdiff_t)((first + count) * per_row));
+        });
+        p0 += np;
+        l0 += nl;
+    }
+    // the next kept frame's tracker rows (kp points, kl lines) into s's matches and inlier flags
+    void tracked(size_t kp, size_t kl, HandlerState& s) {
+        auto cut = [](auto& dst, const auto& src, size_t first, size_t count) {
+            dst.assign(src.begin() + (std::ptrdiff_t)first, src.begin() + (std::ptrdiff_t)(first + count));
+        };
+        cut(s.matches_pt, r.m12_pt, kp0, kp);
+        cut(s.inlier_pt, r.inlier_pt, kp0, kp);
+        cut(s.matches_ls, r.m12_ls, kl0, kl);
+        cut(s.inlier_ls, r.inlier_ls, kl0, kl);
+        kp0 += kp;
+        kl0 += kl;
+    }
+};
+// One call's StereoSession::read split into its streams, given in call order: stream k's `frame` takes frame k's rows and,
+// after an insert (n_stereo of 4 columns, else 2), its matches_pt / _ls and inlier_pt / _ls its kept frame's tracker rows.
+inline void splitRead(const StereoSession::Frames& r, const int32_t* n_stereo, int cols,
+                      const std::vector<HandlerState*>& streams, StereoFrame HandlerState::*frame) {
+    ReadCursor c{r};
+    for (size_t k = 0; k < streams.size(); ++k) {
+        const int32_t* ns = n_stereo + cols * k;
+        c.frameFromRead((size_t)ns[cols - 2], (size_t)ns[cols - 1], streams[k]->*frame);
+        if (cols == 4) c.tracked((size_t)ns[0], (size_t)ns[1], *streams[k]);
+    }
 }
 }  // namespace detail
 
@@ -1071,7 +1137,7 @@ inline PlOrbDetectConfig handlerOrbConfig(PlOrbDetectConfig oc) {
 // prev_frame's arrays and insertStereoPair curr_frame's, with matches_pt / _ls and inlier_pt / _ls as StereoFrameHandler
 // has them, all read back from the device after the call (StereoSession::read): such a frame can be given to the
 // features-in StereoFrameHandler as it is.
-class StereoImageHandler {
+class StereoImageHandler : public HandlerState {
 public:
     StereoImageHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
                        const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc,
@@ -1087,20 +1153,23 @@ public:
         : cam_(cam), hcfg_(hcfg), session_(ctx, cam, cfg, mc, sc, detail::handlerOrbConfig(oc), lc, 1, &rect) {}
 
     void initialize(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // src/stereoFrameHandler.cpp:35-52
-        orb_fast_th = hcfg_.orb_fast_th;                 // :38
+        // :38, set here already because images() takes the first frame's threshold from it; HandlerState::initialize sets
+        // the same value again below
+        orb_fast_th = hcfg_.orb_fast_th;
         images(img_l, img_r);
         const int32_t id = 0;
         int32_t ns[2] = {0, 0};
         session_.initialize(1, &id, frame_, ns);
         frame_ = PlStereoImages{};
-        prev_frame = StereoFrame{};
-        prev_frame.frame_idx = idx;
-        for (int i = 0; i < 36; ++i) prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+        StereoFrame frame;
+        frame.frame_idx = idx;
+        // resets prev_frame and kf before the read below: should that read throw, kf is reset already (prev_frame would be
+        // reset either way, as the device already holds the new frame)
+        HandlerState::initialize(hcfg_, std::move(frame));
         if (keep_) {
             session_.read(1, ns, false, read_);
-            detail::frameFromRead(read_, 0, (size_t)ns[0], 0, (size_t)ns[1], prev_frame);
+            detail::splitRead(read_, ns, 2, {this}, &HandlerState::prev_frame);
         }
-        kf = KeyframeTest{};                             // :48-51
         has_prev_ = true;
     }
     // keep each frame's stereo features and the matches on the host after every call (off by default); effective from the
@@ -1125,39 +1194,16 @@ public:
         session_.insert(1, &id, f, &prior, &result_, n_stereo.data());
         if (keep_) {
             session_.read(1, n_stereo.data(), true, read_);
-            detail::frameFromRead(read_, 0, (size_t)n_stereo[2], 0, (size_t)n_stereo[3], curr_frame);
-            matches_pt = std::move(read_.m12_pt);
-            matches_ls = std::move(read_.m12_ls);
-            inlier_pt = std::move(read_.inlier_pt);
-            inlier_ls = std::move(read_.inlier_ls);
+            detail::splitRead(read_, n_stereo.data(), 4, {this}, &HandlerState::curr_frame);
         }
-        n_inliers_pt = result_.n_matched_pt;             // :126-128
-        n_inliers_ls = result_.n_matched_ls;
-        n_inliers = n_inliers_pt + n_inliers_ls;
+        tracked(result_);
     }
-    void optimizePose() {                                // :307-392: publish what the device computed
-        publishPose(result_, curr_frame);
-        n_inliers_pt = result_.n_inliers_pt;
-        n_inliers_ls = result_.n_inliers_ls;
-        n_inliers = result_.n_inliers;
-    }
-    void updateFrame() {                                 // :62-102
-        orb_fast_th = updateFastThreshold(hcfg_, orb_fast_th, curr_frame, n_inliers_pt);   // :66-86
-        prev_frame = std::move(curr_frame);
-        curr_frame = StereoFrame{};
-    }
-
-    bool needNewKF() { return kf.needNewKF(hcfg_, curr_frame); }
-    void currFrameIsKF() { kf.currFrameIsKF(curr_frame); }
+    void optimizePose() { HandlerState::optimizePose(result_); }
+    void updateFrame() { HandlerState::updateFrame(hcfg_); }
+    bool needNewKF() { return HandlerState::needNewKF(hcfg_); }
     const PlPoseResult& result() const { return result_; }
 
-    StereoFrame prev_frame, curr_frame;
     std::array<int32_t, 4> n_stereo{};                   // stereo points, lines of prev, then of curr, in the last call
-    std::vector<int32_t> matches_pt, matches_ls;         // keepFeatures: prev index -> curr index or -1
-    std::vector<uint8_t> inlier_pt, inlier_ls;           // keepFeatures: per prev feature, matched and still an inlier
-    int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
-    int orb_fast_th = 20;                                // include/stereoFrameHandler.h:62
-    KeyframeTest kf;
 
 private:
     // the caller's images for the next session call, detected at orb_fast_th (they are read during that call only)
@@ -1184,14 +1230,8 @@ private:
 // reference's loop: insertStereoPairs, then optimizePose, needNewKF / currFrameIsKF if wanted, and updateFrame.
 class StereoStreamsHandler {
 public:
-    struct Stream {
-        StereoFrame prev_frame, curr_frame;
+    struct Stream : HandlerState {
         std::array<int32_t, 4> n_stereo{};               // stereo points, lines of prev, then of curr, in the stream's last insert
-        std::vector<int32_t> matches_pt, matches_ls;     // keepFeatures: prev index -> curr index or -1
-        std::vector<uint8_t> inlier_pt, inlier_ls;       // keepFeatures: per prev feature, matched and still an inlier
-        int n_inliers = 0, n_inliers_pt = 0, n_inliers_ls = 0;
-        int orb_fast_th = 20;
-        KeyframeTest kf;
         PlPoseResult result{};
         bool has_prev = false;
     };
@@ -1314,22 +1354,15 @@ private:
         std::vector<int32_t> ns(2 * ids.size());
         session_.initialize((int)ids.size(), ids.data(), pack_.view, ns.data());
         if (keep_) session_.read((int)ids.size(), ns.data(), false, read_);
-        size_t p0 = 0, l0 = 0;
         for (size_t k = 0; k < ids.size(); ++k) {
             Stream& s = streams_[(size_t)ids[k]];
-            s.orb_fast_th = hcfg_.orb_fast_th;
-            s.prev_frame = StereoFrame{};
-            s.prev_frame.frame_idx = k < idx.size() ? idx[k] : 0;
-            for (int i = 0; i < 36; ++i) s.prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
-            if (keep_) {
-                detail::frameFromRead(read_, p0, (size_t)ns[2 * k], l0, (size_t)ns[2 * k + 1], s.prev_frame);
-                p0 += (size_t)ns[2 * k];
-                l0 += (size_t)ns[2 * k + 1];
-            }
-            s.curr_frame = StereoFrame{};
-            s.kf = KeyframeTest{};                       // :48-51
+            StereoFrame frame;
+            frame.frame_idx = k < idx.size() ? idx[k] : 0;
+            s.initialize(hcfg_, std::move(frame));
+            s.curr_frame = StereoFrame{};   // here only: the single handlers' initialize leaves curr_frame as it was
             s.has_prev = true;
         }
+        if (keep_) detail::splitRead(read_, ns.data(), 2, named(ids), &HandlerState::prev_frame);
     }
     void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
                            const std::vector<const uint8_t*>& img_r, const std::vector<Segments>* fl,
@@ -1348,49 +1381,22 @@ private:
         std::vector<int32_t> ns(4 * ids.size());
         session_.insert((int)ids.size(), ids.data(), pack_.view, priors.data(), res.data(), ns.data());
         if (keep_) session_.read((int)ids.size(), ns.data(), true, read_);
-        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
         for (size_t k = 0; k < ids.size(); ++k) {
             Stream& s = streams_[(size_t)ids[k]];
             s.curr_frame = StereoFrame{};
             s.curr_frame.frame_idx = k < idx.size() ? idx[k] : 0;
             s.result = res[k];
             std::copy(ns.begin() + 4 * k, ns.begin() + 4 * k + 4, s.n_stereo.begin());
-            if (keep_) {
-                const size_t kp = (size_t)ns[4 * k], kl = (size_t)ns[4 * k + 1], np = (size_t)ns[4 * k + 2], nl = (size_t)ns[4 * k + 3];
-                detail::frameFromRead(read_, p0, np, l0, nl, s.curr_frame);
-                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
-                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
-                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                p0 += np;
-                l0 += nl;
-                kp0 += kp;
-                kl0 += kl;
-            }
-            s.n_inliers_pt = s.result.n_matched_pt;      // :126-128
-            s.n_inliers_ls = s.result.n_matched_ls;
-            s.n_inliers = s.n_inliers_pt + s.n_inliers_ls;
+            s.tracked(s.result);
         }
+        if (keep_) detail::splitRead(read_, ns.data(), 4, named(ids), &HandlerState::curr_frame);
     }
 
 public:
-    void optimizePose(int id) {                          // :307-392
-        Stream& s = at(id);
-        publishPose(s.result, s.curr_frame);
-        s.n_inliers_pt = s.result.n_inliers_pt;
-        s.n_inliers_ls = s.result.n_inliers_ls;
-        s.n_inliers = s.result.n_inliers;
-    }
-    void updateFrame(int id) {                           // :62-102
-        Stream& s = at(id);
-        s.orb_fast_th = updateFastThreshold(hcfg_, s.orb_fast_th, s.curr_frame, s.n_inliers_pt);   // :66-86
-        s.prev_frame = std::move(s.curr_frame);
-        s.curr_frame = StereoFrame{};
-    }
-    bool needNewKF(int id) { Stream& s = at(id); return s.kf.needNewKF(hcfg_, s.curr_frame); }
-    void currFrameIsKF(int id) { Stream& s = at(id); s.kf.currFrameIsKF(s.curr_frame); }
+    void optimizePose(int id) { Stream& s = at(id); s.optimizePose(s.result); }
+    void updateFrame(int id) { at(id).updateFrame(hcfg_); }
+    bool needNewKF(int id) { return at(id).needNewKF(hcfg_); }
+    void currFrameIsKF(int id) { at(id).currFrameIsKF(); }
 
     // StereoImageHandler::keepFeatures for every stream: initialize fills the named streams' prev_frame arrays,
     // insertStereoPairs their curr_frame arrays and matches_pt / _ls, inlier_pt / _ls
@@ -1455,15 +1461,12 @@ private:
             if (keyframes && keep_) {
                 std::vector<int32_t> rows;
                 session_.readKeyframes(read_, rows);
-                size_t p0 = 0, l0 = 0;
+                detail::ReadCursor c{read_};
                 for (size_t j = 0; j < rows.size() / 4; ++j) {
                     KeyFrame f;
                     f.step = rows[4 * j];
                     f.stream = rows[4 * j + 1];
-                    const size_t np = (size_t)rows[4 * j + 2], nl = (size_t)rows[4 * j + 3];
-                    detail::frameFromRead(read_, p0, np, l0, nl, f.frame);
-                    p0 += np;
-                    l0 += nl;
+                    c.frameFromRead((size_t)rows[4 * j + 2], (size_t)rows[4 * j + 3], f.frame);
                     size_t k = 0;
                     while (ids[k] != f.stream) ++k;
                     publishPose(res[(size_t)f.step * n + k], f.frame);
@@ -1474,30 +1477,20 @@ private:
             session_.run(hcfg_.device(), (int)n, ids.data(), (int)T, frames, th0.data(), priors.data(), res.data(), th.data(),
                          ns.data());
         }
-        if (keep_) session_.read((int)n, ns.data() + 4 * n * (T - 1), true, read_);
-        size_t p0 = 0, l0 = 0, kp0 = 0, kl0 = 0;
+        const int32_t* ns_last = ns.data() + 4 * n * (T - 1);
+        if (keep_) session_.read((int)n, ns_last, true, read_);
         for (size_t k = 0; k < n; ++k) {
             Stream& s = streams_[(size_t)ids[k]];
             const PlPoseResult& last = res[(T - 1) * n + k];
             s.result = last;
-            std::copy(ns.begin() + 4 * ((T - 1) * n + k), ns.begin() + 4 * ((T - 1) * n + k) + 4, s.n_stereo.begin());
-            s.prev_frame = StereoFrame{};
-            if (keep_) {
-                const size_t kp = (size_t)s.n_stereo[0], kl = (size_t)s.n_stereo[1], np = (size_t)s.n_stereo[2],
-                             nl = (size_t)s.n_stereo[3];
-                detail::frameFromRead(read_, p0, np, l0, nl, s.prev_frame);
-                s.matches_pt.assign(read_.m12_pt.begin() + (std::ptrdiff_t)kp0, read_.m12_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.matches_ls.assign(read_.m12_ls.begin() + (std::ptrdiff_t)kl0, read_.m12_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                s.inlier_pt.assign(read_.inlier_pt.begin() + (std::ptrdiff_t)kp0,
-                                   read_.inlier_pt.begin() + (std::ptrdiff_t)(kp0 + kp));
-                s.inlier_ls.assign(read_.inlier_ls.begin() + (std::ptrdiff_t)kl0,
-                                   read_.inlier_ls.begin() + (std::ptrdiff_t)(kl0 + kl));
-                p0 += np;
-                l0 += nl;
-                kp0 += kp;
-                kl0 += kl;
-            }
-            publishPose(last, s.prev_frame);   // optimizePose, then updateFrame moved curr_frame into prev_frame
+            std::copy(ns_last + 4 * k, ns_last + 4 * k + 4, s.n_stereo.begin());
+            // the last step's optimizePose (so n_inliers* are its inlier counts, not f2fTracking's matched counts) and
+            // updateFrame, with the threshold the device carried
+            s.curr_frame = StereoFrame{};
+            s.optimizePose(last);
+            s.prev_frame = std::move(s.curr_frame);
+            s.curr_frame = StereoFrame{};
+            s.orb_fast_th = th[T * n + k];
             if (kf) {
                 s.kf = KeyframeTest::fromState(state[k]);
                 const PlKeyframeResult& kl = (*kf)[(T - 1) * n + k];
@@ -1505,22 +1498,24 @@ private:
                 s.kf.entropy_ratio = kl.entropy_ratio;
                 s.kf.kf_t = kl.t;
                 s.kf.kf_r = kl.r;
-                if (kl.new_kf) {   // currFrameIsKF on the frame that became prev_frame
+                if (kl.new_kf) {   // currFrameIsKF on the frame that became prev_frame: its Tfw / Tfw_cov (kf is the device's)
                     s.prev_frame.Tfw = se3::identity4();
-                    for (int i = 0; i < 36; ++i) s.prev_frame.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+                    identityCov(s.prev_frame.Tfw_cov);
                 }
             }
-            s.curr_frame = StereoFrame{};
-            s.n_inliers_pt = last.n_inliers_pt;
-            s.n_inliers_ls = last.n_inliers_ls;
-            s.n_inliers = last.n_inliers;
-            s.orb_fast_th = th[T * n + k];
         }
+        if (keep_) detail::splitRead(read_, ns_last, 4, named(ids), &HandlerState::prev_frame);
         if (results) *results = std::move(res);
     }
     Stream& at(int id) {
         if (id < 0 || id >= (int)streams_.size()) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler: stream id out of range");
         return streams_[(size_t)id];
+    }
+    // the streams ids name, in call order
+    std::vector<HandlerState*> named(const std::vector<int32_t>& ids) {
+        std::vector<HandlerState*> s;
+        for (int32_t id : ids) s.push_back(&at(id));
+        return s;
     }
     PlCamera cam_;
     HandlerConfig hcfg_;

@@ -196,6 +196,11 @@ def _p(a: Optional[np.ndarray], typ):
     return C.cast(None, typ) if a is None else a.ctypes.data_as(typ)
 
 
+def _record_ptrs(out: dict, records):
+    """Pointers to out's arrays (Engine.stereo_outputs' keys) of the given lifted records, in their C argument order."""
+    return [_p(out[r.key], r.ctype) for r in records]
+
+
 def fld_key_lines(width: int, height: int, n_features: int, seg, lib: Optional[C.CDLL] = None):
     """plstvo_fld_key_lines (host code, no GPU): the reference's FLD-branch key lines of one width x height image from
     FastLineDetector's segments seg float32[n, 4] in its order.  Returns dict(seg [m, 4], angle, npix, response, length), m =
@@ -299,16 +304,7 @@ class StereoSession:
         n_kf = self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(empty), None))
         rows = np.zeros((n_kf, 4), np.int32)
         self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(empty), _p(rows, T.c_int32_p)))
-        pt = self.eng.stereo_outputs(int(rows[:, 2].sum()), n_kf, lines=False)
-        ls = self.eng.stereo_outputs(int(rows[:, 3].sum()), n_kf, lines=True)
-        for d, col in ((pt, 2), (ls, 3)):
-            del d["m12"]
-            d["counts"][...] = rows[:, col]
-        o = T.PlStereoFrameOut()
-        for f, key in T.FRAME_OUT_POINT_KEYS.items():
-            setattr(o, f, pt[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
-        for f, key in T.FRAME_OUT_LINE_KEYS.items():
-            setattr(o, f, ls[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
+        pt, ls, o = self._frame_out(rows[:, 2:])
         got = self.eng._ck(lib.plstvo_stereo_session_read_keyframes(ctx, self.handle, C.byref(o), None))
         if got != n_kf:
             raise PlstvoError(-1, f"plstvo_stereo_session_read_keyframes returned {got} key frames, then {n_kf}")
@@ -331,20 +327,10 @@ class StereoSession:
         tracker's rows are indexed by the kept frames' features in call order, and are None after an initialize."""
         track, ns = self.last if self.last is not None else (False, np.zeros((0, 2), np.int32))
         n = len(ns)
-        np_, nl = int(ns[:, -2].sum()), int(ns[:, -1].sum())
-        pt = self.eng.stereo_outputs(np_, n, lines=False)
-        ls = self.eng.stereo_outputs(nl, n, lines=True)
-        for d, col in ((pt, -2), (ls, -1)):
-            del d["m12"]
-            d["counts"][...] = ns[:, col]
+        pt, ls, o = self._frame_out(ns[:, -2:])
         kp, kl = (int(ns[:, 0].sum()), int(ns[:, 1].sum())) if track else (0, 0)
         m12_pt, m12_ls = np.full(kp, -1, np.int32), np.full(kl, -1, np.int32)
         inl_pt, inl_ls = np.zeros(kp, np.uint8), np.zeros(kl, np.uint8)
-        o = T.PlStereoFrameOut()
-        for f, key in T.FRAME_OUT_POINT_KEYS.items():
-            setattr(o, f, pt[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
-        for f, key in T.FRAME_OUT_LINE_KEYS.items():
-            setattr(o, f, ls[key].ctypes.data_as(dict(T.PlStereoFrameOut._fields_)[f]))
         o.m12_pt, o.m12_ls = m12_pt.ctypes.data_as(T.c_int32_p), m12_ls.ctypes.data_as(T.c_int32_p)
         o.inlier_pt, o.inlier_ls = inl_pt.ctypes.data_as(T.c_uint8_p), inl_ls.ctypes.data_as(T.c_uint8_p)
         got = self.eng._ck(self.eng.lib.plstvo_stereo_session_read(self.eng.ctx, self.handle, C.byref(o)))
@@ -353,6 +339,19 @@ class StereoSession:
         if not track:
             return pt, ls, None, None, None, None
         return pt, ls, m12_pt, inl_pt, m12_ls, inl_ls
+
+    def _frame_out(self, counts):
+        """The point and line dicts of read() for frames of counts [n, 2] (points, lines each) and a PlStereoFrameOut whose
+        lifted fields point at them (the tracker's left NULL)."""
+        pt = self.eng.stereo_outputs(int(counts[:, 0].sum()), len(counts), lines=False)
+        ls = self.eng.stereo_outputs(int(counts[:, 1].sum()), len(counts), lines=True)
+        for d, col in ((pt, 0), (ls, 1)):
+            del d["m12"]
+            d["counts"][...] = counts[:, col]
+        o = T.PlStereoFrameOut()
+        for r in T.FRAME_OUT_RECORDS:
+            setattr(o, r.field, (pt if r.point else ls)[r.key].ctypes.data_as(r.ctype))
+        return pt, ls, o
 
     @property
     def device_bytes(self) -> int:
@@ -577,14 +576,12 @@ class Engine:
         octave_l, m12 = np.ascontiguousarray(octave_l, np.int32), np.ascontiguousarray(m12, np.int32)
         desc_l = np.ascontiguousarray(desc_l, np.uint8).reshape(-1, 32)
         B, n = len(l_off) - 1, len(kp_l)
-        out = dict(pl=np.zeros((n, 2)), disp=np.zeros(n), P=np.zeros((n, 3)), sigma2=np.zeros(n), level=np.zeros(n, np.int32),
-                   desc=np.zeros((n, 32), np.uint8), src_idx=np.full(n, -1, np.int32), counts=np.zeros(B, np.int32))
+        out = self.stereo_outputs(n, B, lines=False)
+        del out["m12"]
         total = self._ck(self.lib.plstvo_stereo_lift_points(
             self.ctx, C.byref(cam), C.byref(scfg), B, _p(l_off, T.c_int32_p), _p(kp_l, T.c_float_p), _p(octave_l, T.c_int32_p),
             _p(desc_l, T.c_uint8_p), _p(r_off, T.c_int32_p), _p(kp_r, T.c_float_p), _p(m12, T.c_int32_p),
-            _p(out["pl"], T.c_double_p), _p(out["disp"], T.c_double_p), _p(out["P"], T.c_double_p),
-            _p(out["sigma2"], T.c_double_p), _p(out["level"], T.c_int32_p), _p(out["desc"], T.c_uint8_p),
-            _p(out["src_idx"], T.c_int32_p), _p(out["counts"], T.c_int32_p)))
+            *_record_ptrs(out, T.FRAME_OUT_POINT_RECORDS), _p(out["counts"], T.c_int32_p)))
         return total, out
 
     def orb_compute_batch(self, cfg: T.PlOrbConfig, images, kp_off, kp_xy, kp_octave, kp_angle=None):
@@ -713,18 +710,12 @@ class Engine:
         octave_l, m12 = np.ascontiguousarray(octave_l, np.int32), np.ascontiguousarray(m12, np.int32)
         desc_l = np.ascontiguousarray(desc_l, np.uint8).reshape(-1, 32)
         B, n = len(l_off) - 1, len(seg_l)
-        out = dict(spl=np.zeros((n, 2)), epl=np.zeros((n, 2)), sdisp=np.zeros(n), edisp=np.zeros(n), sP=np.zeros((n, 3)),
-                   eP=np.zeros((n, 3)), le=np.zeros((n, 3)), angle=np.zeros(n), sigma2=np.zeros(n),
-                   level=np.zeros(n, np.int32), desc=np.zeros((n, 32), np.uint8), src_idx=np.full(n, -1, np.int32),
-                   counts=np.zeros(B, np.int32))
+        out = self.stereo_outputs(n, B, lines=True)
+        del out["m12"]
         total = self._ck(self.lib.plstvo_stereo_lift_lines(
             self.ctx, C.byref(cam), C.byref(scfg), B, _p(l_off, T.c_int32_p), _p(seg_l, T.c_float_p), _p(angle_l, T.c_float_p),
             _p(octave_l, T.c_int32_p), _p(desc_l, T.c_uint8_p), _p(r_off, T.c_int32_p), _p(seg_r, T.c_float_p),
-            _p(m12, T.c_int32_p), _p(out["spl"], T.c_double_p), _p(out["epl"], T.c_double_p), _p(out["sdisp"], T.c_double_p),
-            _p(out["edisp"], T.c_double_p), _p(out["sP"], T.c_double_p), _p(out["eP"], T.c_double_p),
-            _p(out["le"], T.c_double_p), _p(out["angle"], T.c_double_p), _p(out["sigma2"], T.c_double_p),
-            _p(out["level"], T.c_int32_p), _p(out["desc"], T.c_uint8_p), _p(out["src_idx"], T.c_int32_p),
-            _p(out["counts"], T.c_int32_p)))
+            _p(m12, T.c_int32_p), *_record_ptrs(out, T.FRAME_OUT_LINE_RECORDS), _p(out["counts"], T.c_int32_p)))
         return total, out
 
     def match_stereo_points(self, cam, mcfg: T.PlStereoMatchConfig, scfg: T.PlStereoConfig, l_off, kp_l, octave_l, desc_l,
@@ -741,24 +732,17 @@ class Engine:
         total = self._ck(self.lib.plstvo_match_stereo_points(
             self.ctx, C.byref(cam), C.byref(mcfg), C.byref(scfg), B, _p(l_off, T.c_int32_p), _p(kp_l, T.c_float_p),
             _p(octave_l, T.c_int32_p), _p(desc_l, T.c_uint8_p), _p(r_off, T.c_int32_p), _p(kp_r, T.c_float_p),
-            _p(desc_r, T.c_uint8_p), _p(out["m12"], T.c_int32_p), _p(out["pl"], T.c_double_p), _p(out["disp"], T.c_double_p),
-            _p(out["P"], T.c_double_p), _p(out["sigma2"], T.c_double_p), _p(out["level"], T.c_int32_p),
-            _p(out["desc"], T.c_uint8_p), _p(out["src_idx"], T.c_int32_p), _p(out["counts"], T.c_int32_p)))
+            _p(desc_r, T.c_uint8_p), _p(out["m12"], T.c_int32_p), *_record_ptrs(out, T.FRAME_OUT_POINT_RECORDS),
+            _p(out["counts"], T.c_int32_p)))
         return total, out
 
     def stereo_outputs(self, n: int, B: int, lines: bool, pinned: bool = False) -> dict:
         """Output arrays of match_stereo_points / _lines for n left features in B frames (pinned=True: cudaMallocHost)."""
         mk = (lambda shape, dt: self.pinned.empty(shape, dt)) if pinned else (lambda shape, dt: np.zeros(shape, dt))
-        if lines:
-            spec = dict(m12=((n,), np.int32), spl=((n, 2), np.float64), epl=((n, 2), np.float64), sdisp=((n,), np.float64),
-                        edisp=((n,), np.float64), sP=((n, 3), np.float64), eP=((n, 3), np.float64), le=((n, 3), np.float64),
-                        angle=((n,), np.float64), sigma2=((n,), np.float64), level=((n,), np.int32), desc=((n, 32), np.uint8),
-                        src_idx=((n,), np.int32), counts=((B,), np.int32))
-        else:
-            spec = dict(m12=((n,), np.int32), pl=((n, 2), np.float64), disp=((n,), np.float64), P=((n, 3), np.float64),
-                        sigma2=((n,), np.float64), level=((n,), np.int32), desc=((n, 32), np.uint8), src_idx=((n,), np.int32),
-                        counts=((B,), np.int32))
-        out = {k: mk(shape, dt) for k, (shape, dt) in spec.items()}
+        out = dict(m12=mk((n,), np.int32))
+        for r in T.FRAME_OUT_LINE_RECORDS if lines else T.FRAME_OUT_POINT_RECORDS:
+            out[r.key] = mk((n,) + r.row, r.dtype)
+        out["counts"] = mk((B,), np.int32)
         out["m12"][...] = -1
         out["src_idx"][...] = -1
         return out
@@ -776,28 +760,30 @@ class Engine:
         total = self._ck(self.lib.plstvo_match_stereo_lines(
             self.ctx, C.byref(cam), C.byref(mcfg), C.byref(scfg), B, _p(l_off, T.c_int32_p), _p(seg_l, T.c_float_p),
             _p(angle_l, T.c_float_p), _p(octave_l, T.c_int32_p), _p(desc_l, T.c_uint8_p), _p(r_off, T.c_int32_p),
-            _p(seg_r, T.c_float_p), _p(desc_r, T.c_uint8_p), _p(out["m12"], T.c_int32_p), _p(out["spl"], T.c_double_p),
-            _p(out["epl"], T.c_double_p), _p(out["sdisp"], T.c_double_p), _p(out["edisp"], T.c_double_p),
-            _p(out["sP"], T.c_double_p), _p(out["eP"], T.c_double_p), _p(out["le"], T.c_double_p), _p(out["angle"], T.c_double_p),
-            _p(out["sigma2"], T.c_double_p), _p(out["level"], T.c_int32_p), _p(out["desc"], T.c_uint8_p),
-            _p(out["src_idx"], T.c_int32_p), _p(out["counts"], T.c_int32_p)))
+            _p(seg_r, T.c_float_p), _p(desc_r, T.c_uint8_p), _p(out["m12"], T.c_int32_p),
+            *_record_ptrs(out, T.FRAME_OUT_LINE_RECORDS), _p(out["counts"], T.c_int32_p)))
         return total, out
+
+    def _track_stereo(self, fn, cam, cfg, mcfg, scfg, more, frame_sets, as_c, priors, results):
+        """One blocking track_stereo_* call: fn(ctx, cam, cfg, mcfg, scfg, *more, one struct per frame set, priors, results,
+        n_stereo).  frame_sets: (prev, curr) of B pairs, giving results [B] and n_stereo [B, 4], or (frames,) of NF
+        consecutive frames, giving results [NF - 1] and n_stereo [NF, 2]; as_c makes each set's struct and keep-alive arrays."""
+        structs = [as_c(f) for f in frame_sets]
+        B, pairs = structs[0][0].B, len(frame_sets) == 2
+        if results is None:
+            results = np.zeros(B if pairs else max(B - 1, 0), dtype=T.POSE_RESULT_DTYPE)
+        n_stereo = np.zeros((B, 4 if pairs else 2), np.int32)
+        self._ck(fn(self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), *more,
+                    *(C.byref(s) for s, _ in structs), priors.ctypes.data if priors is not None else None, results.ctypes.data,
+                    _p(n_stereo, T.c_int32_p)))
+        return results, n_stereo
 
     def track_stereo_batch(self, cam, cfg, mcfg, scfg, prev: dict, curr: dict, priors=None, results=None):
         """Raw stereo features of B (prev, curr) frame pairs -> poses: matchStereoPoints / Lines for both frames, f2fTracking and
         optimizePose, the lifted records resident in HBM.  prev / curr: dicts with the PlStereoFeatures fields.
         Returns (results, n_stereo[B, 4])."""
-        ps, keep_p = T.stereo_features_as_c(prev)
-        cs, keep_c = T.stereo_features_as_c(curr)
-        B = ps.B
-        if results is None:
-            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((B, 4), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_batch(self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ps),
-                                                    C.byref(cs), priors.ctypes.data if priors is not None else None,
-                                                    results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep_p, keep_c
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_batch, cam, cfg, mcfg, scfg, (), (prev, curr),
+                                  T.stereo_features_as_c, priors, results)
 
     def track_stereo_batch_async(self, cam, cfg, mcfg, scfg, prev_c, curr_c, results, n_stereo, priors=None) -> int:
         """Streaming form: prev_c / curr_c are PlStereoFeatures structs built once by T.stereo_features_as_c over PINNED arrays
@@ -814,78 +800,36 @@ class Engine:
     def track_stereo_sequence(self, cam, cfg, mcfg, scfg, frames: dict, priors=None, results=None):
         """NF consecutive frames of raw stereo features -> NF - 1 poses (pair p = frames p, p + 1); every frame goes through the
         stereo step once.  Returns (results, n_stereo[NF, 2])."""
-        fs, keep = T.stereo_features_as_c(frames)
-        NF = fs.B
-        if results is None:
-            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((NF, 2), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_sequence(self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg),
-                                                       C.byref(fs), priors.ctypes.data if priors is not None else None,
-                                                       results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_sequence, cam, cfg, mcfg, scfg, (), (frames,),
+                                  T.stereo_features_as_c, priors, results)
 
     def track_stereo_images_batch(self, cam, cfg, mcfg, scfg, ocfg, prev: dict, curr: dict, priors=None, results=None):
         """Stereo images and key lines of B (prev, curr) frame pairs -> poses: ORB detection, LBD description, the stereo step,
         f2fTracking and optimizePose, feature data resident in HBM.  prev / curr: dicts with img_l / img_r uint8[B, H, W] and
         the other PlStereoImages fields (see T.stereo_images_as_c).  Returns (results, n_stereo[B, 4])."""
-        ps, keep_p = T.stereo_images_as_c(prev)
-        cs, keep_c = T.stereo_images_as_c(curr)
-        B = ps.B
-        if results is None:
-            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((B, 4), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_images_batch(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg), C.byref(ps), C.byref(cs),
-            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep_p, keep_c
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_images_batch, cam, cfg, mcfg, scfg, (C.byref(ocfg),),
+                                  (prev, curr), T.stereo_images_as_c, priors, results)
 
     def track_stereo_images_sequence(self, cam, cfg, mcfg, scfg, ocfg, frames: dict, priors=None, results=None):
         """NF consecutive stereo frames (images and key lines) -> NF - 1 poses; every frame's images are detected and described
         once.  Returns (results, n_stereo[NF, 2])."""
-        fs, keep = T.stereo_images_as_c(frames)
-        NF = fs.B
-        if results is None:
-            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((NF, 2), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_images_sequence(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg), C.byref(fs),
-            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_images_sequence, cam, cfg, mcfg, scfg, (C.byref(ocfg),),
+                                  (frames,), T.stereo_images_as_c, priors, results)
 
     def track_stereo_images_lsd_batch(self, cam, cfg, mcfg, scfg, ocfg, lcfg, prev: dict, curr: dict, priors=None, results=None):
         """Stereo images alone of B (prev, curr) frame pairs -> poses: LSD detection inside the call, then what
         track_stereo_images_batch does.  prev / curr: dicts with img_l / img_r uint8[B, H, W] and optionally fast_th [B], no
         key-line arrays.  lcfg may be None where cfg.has_lines is 0.  Returns (results, n_stereo[B, 4])."""
-        ps, keep_p = T.stereo_images_as_c(prev)
-        cs, keep_c = T.stereo_images_as_c(curr)
-        B = ps.B
-        if results is None:
-            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((B, 4), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_images_lsd_batch(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
-            None if lcfg is None else C.byref(lcfg), C.byref(ps), C.byref(cs), priors.ctypes.data if priors is not None else None,
-            results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep_p, keep_c
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_images_lsd_batch, cam, cfg, mcfg, scfg,
+                                  (C.byref(ocfg), None if lcfg is None else C.byref(lcfg)), (prev, curr), T.stereo_images_as_c,
+                                  priors, results)
 
     def track_stereo_images_lsd_sequence(self, cam, cfg, mcfg, scfg, ocfg, lcfg, frames: dict, priors=None, results=None):
         """NF consecutive stereo frames (images alone) -> NF - 1 poses, LSD inside the call; every frame's images are detected
         and described once.  Returns (results, n_stereo[NF, 2])."""
-        fs, keep = T.stereo_images_as_c(frames)
-        NF = fs.B
-        if results is None:
-            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((NF, 2), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_images_lsd_sequence(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
-            None if lcfg is None else C.byref(lcfg), C.byref(fs), priors.ctypes.data if priors is not None else None,
-            results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_images_lsd_sequence, cam, cfg, mcfg, scfg,
+                                  (C.byref(ocfg), None if lcfg is None else C.byref(lcfg)), (frames,), T.stereo_images_as_c,
+                                  priors, results)
 
     # ---- rectification: PinholeStereoCamera::rectifyImagesLR ----
     def rectifier_create(self, map1_l, map2_l, map1_r=None, map2_r=None) -> Rectifier:
@@ -959,18 +903,9 @@ class Engine:
         _lsd_ call.  A colour rectifier takes img_l / img_r uint8[B, H, W, C].  Returns (results, n_stereo[B, 4])."""
         if rect is not None and rect.channels > 1:
             rect.check_frames(prev, curr)
-        ps, keep_p = T.stereo_images_as_c(prev)
-        cs, keep_c = T.stereo_images_as_c(curr)
-        B = ps.B
-        if results is None:
-            results = np.zeros(B, dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((B, 4), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_raw_images_batch(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
-            None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle, C.byref(ps), C.byref(cs),
-            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep_p, keep_c
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_raw_images_batch, cam, cfg, mcfg, scfg,
+                                  (C.byref(ocfg), None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle),
+                                  (prev, curr), T.stereo_images_as_c, priors, results)
 
     def track_stereo_raw_images_sequence(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], frames: dict,
                                          priors=None, results=None):
@@ -978,17 +913,9 @@ class Engine:
         Returns (results, n_stereo[NF, 2])."""
         if rect is not None and rect.channels > 1:
             rect.check_frames(frames)
-        fs, keep = T.stereo_images_as_c(frames)
-        NF = fs.B
-        if results is None:
-            results = np.zeros(max(NF - 1, 0), dtype=T.POSE_RESULT_DTYPE)
-        n_stereo = np.zeros((NF, 2), np.int32)
-        self._ck(self.lib.plstvo_track_stereo_raw_images_sequence(
-            self.ctx, C.byref(cam), C.byref(cfg), C.byref(mcfg), C.byref(scfg), C.byref(ocfg),
-            None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle, C.byref(fs),
-            priors.ctypes.data if priors is not None else None, results.ctypes.data, _p(n_stereo, T.c_int32_p)))
-        del keep
-        return results, n_stereo
+        return self._track_stereo(self.lib.plstvo_track_stereo_raw_images_sequence, cam, cfg, mcfg, scfg,
+                                  (C.byref(ocfg), None if lcfg is None else C.byref(lcfg), None if rect is None else rect.handle),
+                                  (frames,), T.stereo_images_as_c, priors, results)
 
     # ---- stereo sessions: many streams, each stream's previous frame kept on the device ----
     def stereo_session_create(self, cam, cfg, mcfg, scfg, ocfg, lcfg, rect: Optional[Rectifier], n_streams: int) -> StereoSession:

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass, field
-from typing import Optional, Sequence
+from typing import NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -173,21 +173,49 @@ class PlStereoImages(C.Structure):
                 ("angle_l", c_float_p), ("angle_r", c_float_p), ("npix_l", c_int32_p), ("npix_r", c_int32_p)]
 
 
+_C_PTR = {np.float64: c_double_p, np.int32: c_int32_p, np.uint8: c_uint8_p}
+
+
+class FrameRecord(NamedTuple):
+    """One lifted array: its PlStereoFrameOut field, its key in Engine.stereo_outputs' dicts, dtype, shape of one row, and
+    whether it is a point (True) or a line array."""
+    field: str
+    key: str
+    dtype: type
+    row: tuple
+    point: bool
+
+    @property
+    def ctype(self):
+        return _C_PTR[self.dtype]
+
+
+# The 19 lifted arrays, once, in PlStereoFrameOut's field order (include/plstvo.h): the lifting and matchStereo calls write
+# them in this order, and plstvo_stereo_session_read / _read_keyframes fill them.
+FRAME_OUT_RECORDS = tuple(FrameRecord(*r) for r in (
+    ("pt_pl", "pl", np.float64, (2,), True), ("pt_disp", "disp", np.float64, (), True),
+    ("pt_P", "P", np.float64, (3,), True), ("pt_sigma2", "sigma2", np.float64, (), True),
+    ("pt_level", "level", np.int32, (), True), ("pdesc", "desc", np.uint8, (DESC_BYTES,), True),
+    ("pt_src", "src_idx", np.int32, (), True),
+    ("ls_spl", "spl", np.float64, (2,), False), ("ls_epl", "epl", np.float64, (2,), False),
+    ("ls_sdisp", "sdisp", np.float64, (), False), ("ls_edisp", "edisp", np.float64, (), False),
+    ("ls_sP", "sP", np.float64, (3,), False), ("ls_eP", "eP", np.float64, (3,), False),
+    ("ls_le", "le", np.float64, (3,), False), ("ls_angle", "angle", np.float64, (), False),
+    ("ls_sigma2", "sigma2", np.float64, (), False), ("ls_level", "level", np.int32, (), False),
+    ("ldesc", "desc", np.uint8, (DESC_BYTES,), False), ("ls_src", "src_idx", np.int32, (), False)))
+FRAME_OUT_POINT_RECORDS = tuple(r for r in FRAME_OUT_RECORDS if r.point)
+FRAME_OUT_LINE_RECORDS = tuple(r for r in FRAME_OUT_RECORDS if not r.point)
+
+
 class PlStereoFrameOut(C.Structure):
     """Destinations of plstvo_stereo_session_read (PlStereoFrameOut, include/plstvo.h); a NULL field is not copied."""
-    _fields_ = [("pt_pl", c_double_p), ("pt_disp", c_double_p), ("pt_P", c_double_p), ("pt_sigma2", c_double_p),
-                ("pt_level", c_int32_p), ("pdesc", c_uint8_p), ("pt_src", c_int32_p),
-                ("ls_spl", c_double_p), ("ls_epl", c_double_p), ("ls_sdisp", c_double_p), ("ls_edisp", c_double_p),
-                ("ls_sP", c_double_p), ("ls_eP", c_double_p), ("ls_le", c_double_p), ("ls_angle", c_double_p),
-                ("ls_sigma2", c_double_p), ("ls_level", c_int32_p), ("ldesc", c_uint8_p), ("ls_src", c_int32_p),
-                ("m12_pt", c_int32_p), ("inlier_pt", c_uint8_p), ("m12_ls", c_int32_p), ("inlier_ls", c_uint8_p)]
+    _fields_ = [(r.field, r.ctype) for r in FRAME_OUT_RECORDS] + [
+        ("m12_pt", c_int32_p), ("inlier_pt", c_uint8_p), ("m12_ls", c_int32_p), ("inlier_ls", c_uint8_p)]
 
 
 # PlStereoFrameOut's point / line fields and the keys of Engine.match_stereo_points / _lines' outputs they correspond to
-FRAME_OUT_POINT_KEYS = dict(pt_pl="pl", pt_disp="disp", pt_P="P", pt_sigma2="sigma2", pt_level="level", pdesc="desc",
-                            pt_src="src_idx")
-FRAME_OUT_LINE_KEYS = dict(ls_spl="spl", ls_epl="epl", ls_sdisp="sdisp", ls_edisp="edisp", ls_sP="sP", ls_eP="eP", ls_le="le",
-                           ls_angle="angle", ls_sigma2="sigma2", ls_level="level", ldesc="desc", ls_src="src_idx")
+FRAME_OUT_POINT_KEYS = {r.field: r.key for r in FRAME_OUT_POINT_RECORDS}
+FRAME_OUT_LINE_KEYS = {r.field: r.key for r in FRAME_OUT_LINE_RECORDS}
 
 
 STEREO_IMAGE_DTYPES = dict(img_l=np.uint8, img_r=np.uint8, fast_th=np.int32, ll_off=np.int32, lr_off=np.int32, seg_l=np.float32,
