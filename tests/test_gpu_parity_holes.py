@@ -176,20 +176,24 @@ def test_robust_mode_flag_differences_are_counted(engine, oracle):
 def test_near_singular_normal_equations_take_the_qr_path(engine, oracle):
     """Ill-conditioned H (all points at nearly the same depth and direction: rotation and translation barely separable):
     K2's Cholesky fast path must hand over to the column-pivoted QR where the two would differ; the result follows the
-    oracle (ColPivHouseholderQR semantics, src/stereoFrameHandler.cpp:417-418)."""
+    oracle (ColPivHouseholderQR semantics, src/stereoFrameHandler.cpp:417-418).  The patch is 1.4 px wide at 1 m, so H at
+    the prior has kappa ~7e13 and a Cholesky pivot below 1e-13 max diag: the device refuses it (a 15 px patch at 40 m has
+    kappa ~5e12 but pivots near 5e-10 max diag, which the Cholesky accepts)."""
     cfg = T.kitti_config()
     cfg.has_lines = 0
     rng = np.random.default_rng(3)
     n = 60
     cam = T.kitti_camera()
-    u, v = rng.uniform(600, 615, n), rng.uniform(180, 190, n)      # a tiny patch of the image, one depth
-    d = np.full(n, cam.b * cam.fx / 40.0)
+    u, v = rng.uniform(300, 301.4, n), rng.uniform(180, 180.93, n)  # a tiny patch of the image, one depth
+    d = np.full(n, cam.b * cam.fx / 1.0)
     P = synth.back_projection(cam, u, v, d)
     Tgt = synth.expmap_se3(np.array([0.01, 0.0, -0.3, 0.001, -0.002, 0.0005]))
     obs = synth.projection(cam, P @ Tgt[:3, :3].T + Tgt[:3, 3]) + rng.normal(0, 0.05, (n, 2))
     m = T.MatchedBatch(pt_off=[0, n], ls_off=[0, 0], pt_P=P, pt_pl_obs=obs, pt_sigma2=np.ones(n), ls_sP=np.zeros((0, 3)),
                        ls_eP=np.zeros((0, 3)), ls_le_obs=np.zeros((0, 3)), ls_spl=np.zeros((0, 2)), ls_epl=np.zeros((0, 2)),
                        ls_sigma2=np.zeros(0))
+    H, g, _ = oracle.optimize_functions(cam, cfg, m, 0, np.eye(4))
+    assert not engine.debug_pose_helpers(H=H[None], g=g[None])["chol_ok"][0]      # the QR solves, not the Cholesky
     res, ip, il = engine.optimize_pose(cam, cfg, m)
     rc, res_o, ip_o, il_o = oracle.optimize_pose(cam, cfg, m)
     assert res[0]["good"] == res_o[0]["good"] and res[0]["status"] == res_o[0]["status"]
