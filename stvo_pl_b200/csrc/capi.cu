@@ -2,6 +2,7 @@
 // matching and tracking, throughput mode, instrumentation.  The stereo step is in capi_stereo.cu, feature extraction in
 // capi_features.cu, what they share in host.cuh.  No CPU compute path exists in this library: without a CUDA
 // device plstvo_create() fails with PLSTVO_E_NO_DEVICE and every other entry point needs a context.
+#include <array>
 #include <cstdlib>
 #include <cstring>
 
@@ -146,6 +147,56 @@ int validate_frames(PlContext* ctx, const PlFrameBatch* prev, const PlFrameBatch
     return 0;
 }
 
+// ---- the callers' arrays by records.h array ----
+struct HostRec {
+    int k;
+    const void* src;
+};
+// a PlFrameBatch in the previous-frame role (PREV_ROLE) and in the current-frame role (CURR_ROLE)
+std::array<HostRec, N_PREV> prev_fields(const PlFrameBatch* f) {
+    return {{{PT_P, f->pt_P}, {PT_S2, f->pt_sigma2}, {PT_DESC, f->pdesc}, {LS_SPL, f->ls_spl}, {LS_EPL, f->ls_epl},
+             {LS_SP, f->ls_sP}, {LS_EP, f->ls_eP}, {LS_S2, f->ls_sigma2}, {LS_LEVEL, f->ls_level}, {LS_DESC, f->ldesc}}};
+}
+std::array<HostRec, 4> curr_fields(const PlFrameBatch* f) {
+    return {{{PT_PL, f->pt_pl}, {PT_DESC, f->pdesc}, {LS_LE, f->ls_le}, {LS_DESC, f->ldesc}}};
+}
+// explicit matched lists: the observations pl_obs and le_obs are current-frame rows, PT_PL and LS_LE
+std::array<HostRec, 11> matched_fields(const PlMatchedBatch* m) {
+    return {{{PT_P, m->pt_P}, {PT_PL, m->pt_pl_obs}, {PT_S2, m->pt_sigma2}, {INL_PT, m->pt_inlier}, {LS_SP, m->ls_sP},
+             {LS_EP, m->ls_eP}, {LS_LE, m->ls_le_obs}, {LS_SPL, m->ls_spl}, {LS_EPL, m->ls_epl}, {LS_S2, m->ls_sigma2},
+             {INL_LS, m->ls_inlier}}};
+}
+
+// the arrays matching-only calls (plstvo_match_batch, plstvo_f2f_tracking) size and move: the descriptors and m12
+constexpr bool matching_rec(int k) { return k == PT_DESC || k == LS_DESC || k == M12_PT || k == M12_LS; }
+
+// rows [first, first + count) of w bytes each, from an array of such rows to another; nothing for a null end or no rows
+cudaError_t copy_rows(void* dst, const void* src, size_t w, size_t first, size_t count, cudaMemcpyKind kind, cudaStream_t s) {
+    if (!dst || !src || !count) return cudaSuccess;
+    return cudaMemcpyAsync(static_cast<uint8_t*>(dst) + first * w, static_cast<const uint8_t*>(src) + first * w, count * w,
+                           kind, s);
+}
+
+// Uploads explicit lists m on s into dst: the offsets and every array of the PlMatchedBatch table, each buffer at least 16
+// bytes (an empty list's too).  *rows: those arrays, a null entry for inlier flags the caller did not give (all true).
+int upload_matched(PlContext* ctx, const PlMatchedBatch* m, FrameBufs& dst, cudaStream_t s, RecPtrs* rows) {
+    const int B = m->B;
+    const size_t n_pt = m->pt_off[B], n_ls = m->ls_off[B], off_bytes = (size_t)(B + 1) * 4;
+    CK(ctx, dst.pt_off.ensure(std::max<size_t>(off_bytes, 16)));
+    CK(ctx, cudaMemcpyAsync(dst.pt_off.p, m->pt_off, off_bytes, cudaMemcpyHostToDevice, s));
+    CK(ctx, dst.ls_off.ensure(std::max<size_t>(off_bytes, 16)));
+    CK(ctx, cudaMemcpyAsync(dst.ls_off.p, m->ls_off, off_bytes, cudaMemcpyHostToDevice, s));
+    *rows = RecPtrs{};
+    for (const HostRec& e : matched_fields(m)) {
+        DevBuf& buf = dst.rec[e.k];
+        const size_t bytes = (rec_is_point(e.k) ? n_pt : n_ls) * REC_BYTES[e.k];
+        CK(ctx, buf.ensure(std::max<size_t>(bytes, 16)));
+        if (e.src && bytes) CK(ctx, cudaMemcpyAsync(buf.p, e.src, bytes, cudaMemcpyHostToDevice, s));
+        if (e.src || (e.k != INL_PT && e.k != INL_LS)) rows->p[e.k] = buf.p;
+    }
+    return 0;
+}
+
 }  // namespace
 
 namespace plstvo {
@@ -233,13 +284,14 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     if (with_features && !ws.solver.fits)
         return fail(ctx, PLSTVO_E_TOO_LARGE, "frame too large for the per-pair solver's shared memory");
 
-    // --- device storage ---
-    CK(ctx, ws.d_pdesc1.ensure(np1 * 32));
-    CK(ctx, ws.d_pdesc2.ensure(np2 * 32));
-    CK(ctx, ws.d_ldesc1.ensure(nl1 * 32));
-    CK(ctx, ws.d_ldesc2.ensure(nl2 * 32));
-    CK(ctx, ws.d_m12p.ensure(np1 * 4));
-    CK(ctx, ws.d_m12l.ensure(nl1 * 4));
+    // --- device storage: matching-only calls size the descriptors and m12, tracking every array of both roles ---
+    auto grow = [&](FrameBufs& side, int k, size_t n_pt, size_t n_ls) {
+        return with_features || matching_rec(k) ? side.rec[k].ensure((rec_is_point(k) ? n_pt : n_ls) * REC_BYTES[k])
+                                                : cudaSuccess;
+    };
+    for (int k : PREV_ROLE) CK(ctx, grow(ws.prev, k, np1, nl1));
+    for (int k = M12_PT; k < N_REC; ++k) CK(ctx, grow(ws.prev, k, np1, nl1));   // the tracker's rows
+    for (int k : CURR_ROLE) CK(ctx, grow(ws.curr, k, np2, nl2));
     CK(ctx, ws.d_rowpart.ensure(row_elems * sizeof(uint2)));
     CK(ctx, ws.d_colpart.ensure(col_elems * sizeof(uint2)));
     CK(ctx, ws.d_problems.ensure(ws.problems.size() * sizeof(MatchProblem)));
@@ -252,24 +304,10 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
         CK(ctx, cudaMemsetAsync(ws.d_sched.p, 0, 64, ctx->s_h2d));
     }
     if (with_features) {
-        CK(ctx, ws.d_poff1.ensure((B + 1) * 4));
-        CK(ctx, ws.d_poff2.ensure((B + 1) * 4));
-        CK(ctx, ws.d_loff1.ensure((B + 1) * 4));
-        CK(ctx, ws.d_loff2.ensure((B + 1) * 4));
-        CK(ctx, ws.d_ptP.ensure(np1 * 24));
-        CK(ctx, ws.d_pts2.ensure(np1 * 8));
-        CK(ctx, ws.d_ptpl.ensure(np2 * 16));
-        CK(ctx, ws.d_lssP.ensure(nl1 * 24));
-        CK(ctx, ws.d_lseP.ensure(nl1 * 24));
-        CK(ctx, ws.d_lsspl.ensure(nl1 * 16));
-        CK(ctx, ws.d_lsepl.ensure(nl1 * 16));
-        CK(ctx, ws.d_lss2.ensure(nl1 * 8));
-        CK(ctx, ws.d_lslev.ensure(nl1 * 4));
-        CK(ctx, ws.d_lsle.ensure(nl2 * 24));
+        for (DevBuf* off : {&ws.prev.pt_off, &ws.curr.pt_off, &ws.prev.ls_off, &ws.curr.ls_off})
+            CK(ctx, off->ensure((B + 1) * 4));
         CK(ctx, ws.d_priors.ensure((size_t)B * sizeof(PlPrior)));
         CK(ctx, ws.d_results.ensure((size_t)B * sizeof(PlPoseResult)));
-        CK(ctx, ws.d_inlp.ensure(np1));
-        CK(ctx, ws.d_inll.ensure(nl1));
         if (ws.solver.feat_stride) CK(ctx, ws.d_feat.ensure((size_t)B * ws.solver.feat_stride * sizeof(double)));
     }
     // --- fix up pointers, upload the plan ---
@@ -278,15 +316,11 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
             MatchProblem& pr = ws.problems[(size_t)2 * p + type];
             pr.rowpart = ws.d_rowpart.as<uint2>() + reinterpret_cast<size_t>(pr.rowpart);
             pr.colpart = ws.d_colpart.as<uint2>() + reinterpret_cast<size_t>(pr.colpart);
-            if (type == 0) {
-                pr.d1 = ws.d_pdesc1.as<uint8_t>() + (size_t)ws.p_off1[p] * 32;
-                pr.d2 = ws.d_pdesc2.as<uint8_t>() + (size_t)ws.p_off2[p] * 32;
-                pr.m12 = ws.d_m12p.as<int32_t>() + ws.p_off1[p];
-            } else {
-                pr.d1 = ws.d_ldesc1.as<uint8_t>() + (size_t)ws.l_off1[p] * 32;
-                pr.d2 = ws.d_ldesc2.as<uint8_t>() + (size_t)ws.l_off2[p] * 32;
-                pr.m12 = ws.d_m12l.as<int32_t>() + ws.l_off1[p];
-            }
+            const int kd = type ? LS_DESC : PT_DESC, km = type ? M12_LS : M12_PT;
+            const size_t r1 = type ? ws.l_off1[p] : ws.p_off1[p], r2 = type ? ws.l_off2[p] : ws.p_off2[p];
+            pr.d1 = ws.prev.rec[kd].as<uint8_t>() + r1 * REC_BYTES[kd];
+            pr.d2 = ws.curr.rec[kd].as<uint8_t>() + r2 * REC_BYTES[kd];
+            pr.m12 = ws.prev.rec[km].as<int32_t>() + r1;
             // the matcher expands the rows of the workspace's own 32-byte-row arenas (16-byte aligned loads)
             TcProblem& tp = ws.tc_problems[(size_t)2 * p + type];
             tp.d1 = pr.d1;
@@ -307,10 +341,10 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
         CK(ctx, cudaMemcpyAsync(ws.d_problems.p, ws.problems.data(), ws.problems.size() * sizeof(MatchProblem),
                                 cudaMemcpyHostToDevice, s));
     if (with_features) {
-        CK(ctx, cudaMemcpyAsync(ws.d_poff1.p, ws.p_off1.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
-        CK(ctx, cudaMemcpyAsync(ws.d_poff2.p, ws.p_off2.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
-        CK(ctx, cudaMemcpyAsync(ws.d_loff1.p, ws.l_off1.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
-        CK(ctx, cudaMemcpyAsync(ws.d_loff2.p, ws.l_off2.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
+        CK(ctx, cudaMemcpyAsync(ws.prev.pt_off.p, ws.p_off1.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
+        CK(ctx, cudaMemcpyAsync(ws.curr.pt_off.p, ws.p_off2.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
+        CK(ctx, cudaMemcpyAsync(ws.prev.ls_off.p, ws.l_off1.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
+        CK(ctx, cudaMemcpyAsync(ws.curr.ls_off.p, ws.l_off2.data(), (B + 1) * 4, cudaMemcpyHostToDevice, s));
     }
     ws.planned = true;
     ws.planned_features = with_features;
@@ -318,36 +352,23 @@ int ws_prepare(PlContext* ctx, Workspace& ws, const PlCamera* cam, const PlConfi
     return 0;
 }
 
-#define H2D(ctx, dst, src, elem_bytes, first, count, stream)                                                 \
-    do {                                                                                                     \
-        if ((count) > 0 && (src) != nullptr)                                                                 \
-            CK(ctx, cudaMemcpyAsync((dst).as<uint8_t>() + (size_t)(first) * (elem_bytes),                    \
-                                    reinterpret_cast<const uint8_t*>(src) + (size_t)(first) * (elem_bytes),  \
-                                    (size_t)(count) * (elem_bytes), cudaMemcpyHostToDevice, stream));        \
-    } while (0)
-
 // descriptors (+ features when with_features) of pairs [p0, p1) host -> device
 int ws_upload_range(PlContext* ctx, Workspace& ws, const PlFrameBatch* prev, const PlFrameBatch* curr,
                     const PlPrior* priors, int p0, int p1, bool with_features, cudaStream_t s) {
-    const int a = ws.p_off1[p0], an = ws.p_off1[p1] - a, b = ws.p_off2[p0], bn = ws.p_off2[p1] - b;
-    const int c = ws.l_off1[p0], cn = ws.l_off1[p1] - c, d = ws.l_off2[p0], dn = ws.l_off2[p1] - d;
-    H2D(ctx, ws.d_pdesc1, prev->pdesc, 32, a, an, s);
-    H2D(ctx, ws.d_pdesc2, curr->pdesc, 32, b, bn, s);
-    H2D(ctx, ws.d_ldesc1, prev->ldesc, 32, c, cn, s);
-    H2D(ctx, ws.d_ldesc2, curr->ldesc, 32, d, dn, s);
-    if (with_features) {
-        H2D(ctx, ws.d_ptP, prev->pt_P, 24, a, an, s);
-        H2D(ctx, ws.d_pts2, prev->pt_sigma2, 8, a, an, s);
-        H2D(ctx, ws.d_ptpl, curr->pt_pl, 16, b, bn, s);
-        H2D(ctx, ws.d_lssP, prev->ls_sP, 24, c, cn, s);
-        H2D(ctx, ws.d_lseP, prev->ls_eP, 24, c, cn, s);
-        H2D(ctx, ws.d_lsspl, prev->ls_spl, 16, c, cn, s);
-        H2D(ctx, ws.d_lsepl, prev->ls_epl, 16, c, cn, s);
-        H2D(ctx, ws.d_lss2, prev->ls_sigma2, 8, c, cn, s);
-        H2D(ctx, ws.d_lslev, prev->ls_level, 4, c, cn, s);
-        H2D(ctx, ws.d_lsle, curr->ls_le, 24, d, dn, s);
-        if (priors) H2D(ctx, ws.d_priors, priors, sizeof(PlPrior), p0, p1 - p0, s);
-    }
+    auto up = [&](FrameBufs& side, const auto& fields, const std::vector<int32_t>& pt_off, const std::vector<int32_t>& ls_off) {
+        for (const HostRec& e : fields) {
+            const std::vector<int32_t>& off = rec_is_point(e.k) ? pt_off : ls_off;
+            if (with_features || matching_rec(e.k))
+                if (const cudaError_t err = copy_rows(side.rec[e.k].p, e.src, REC_BYTES[e.k], off[p0], off[p1] - off[p0],
+                                                      cudaMemcpyHostToDevice, s))
+                    return err;
+        }
+        return cudaSuccess;
+    };
+    CK(ctx, up(ws.prev, prev_fields(prev), ws.p_off1, ws.l_off1));
+    CK(ctx, up(ws.curr, curr_fields(curr), ws.p_off2, ws.l_off2));
+    if (with_features)
+        CK(ctx, copy_rows(ws.d_priors.p, priors, sizeof(PlPrior), p0, p1 - p0, cudaMemcpyHostToDevice, s));
     return 0;
 }
 
@@ -373,39 +394,28 @@ int ws_launch_solve(PlContext* ctx, Workspace& ws, int p0, int p1, bool have_lev
     prm.cam = ws.cam;
     prm.cfg = ws.cfg;
     prm.mode = 0;
-    prm.prev = FrameDev{ws.d_poff1.as<int32_t>(), ws.d_loff1.as<int32_t>(), nullptr, nullptr,
-                        ws.d_ptP.as<double>(), nullptr, ws.d_pts2.as<double>(), ws.d_lssP.as<double>(),
-                        ws.d_lseP.as<double>(), nullptr, ws.d_lsspl.as<double>(), ws.d_lsepl.as<double>(),
-                        ws.d_lss2.as<double>(), have_level ? ws.d_lslev.as<int32_t>() : nullptr};
-    prm.curr = FrameDev{ws.d_poff2.as<int32_t>(), ws.d_loff2.as<int32_t>(), nullptr, nullptr, nullptr,
-                        ws.d_ptpl.as<double>(), nullptr, nullptr, nullptr, ws.d_lsle.as<double>(), nullptr,
-                        nullptr, nullptr, nullptr};
+    RecPtrs prev = ws.prev.rows(PREV_ROLE);
+    if (!have_level) prev.p[LS_LEVEL] = nullptr;
+    prm.prev = rows_dev(ws.prev.pt_off, ws.prev.ls_off, prev);
+    prm.curr = rows_dev(ws.curr.pt_off, ws.curr.ls_off, ws.curr.rows(CURR_ROLE));
     prm.problems = ws.d_problems.as<MatchProblem>();
     prm.priors = ws.has_priors ? ws.d_priors.as<PlPrior>() : nullptr;
     prm.results = ws.d_results.as<PlPoseResult>();
-    prm.inlier_pt = ws.d_inlp.as<uint8_t>();
-    prm.inlier_ls = ws.d_inll.as<uint8_t>();
+    prm.inlier_pt = ws.prev.rec[INL_PT].as<uint8_t>();
+    prm.inlier_ls = ws.prev.rec[INL_LS].as<uint8_t>();
     prm.phase_cycles = ws.d_phase.as<long long>();
     return launch_solver(ctx, prm, ws.solver, ws.d_feat.as<double>(), ws.d_stream, ws.B, (size_t)ws.p_off1[ws.B],
                          (size_t)ws.l_off1[ws.B], p0, p1, s, marks, ws.d_cams);
 }
 
-#define D2H(ctx, dst, src, elem_bytes, first, count, stream)                                                 \
-    do {                                                                                                     \
-        if ((count) > 0 && (dst) != nullptr)                                                                 \
-            CK(ctx, cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + (size_t)(first) * (elem_bytes),        \
-                                    (src).as<uint8_t>() + (size_t)(first) * (elem_bytes),                    \
-                                    (size_t)(count) * (elem_bytes), cudaMemcpyDeviceToHost, stream));        \
-    } while (0)
-
 int ws_download_range(PlContext* ctx, Workspace& ws, int p0, int p1, PlPoseResult* results, int32_t* m12_pt,
                       int32_t* m12_ls, uint8_t* inl_pt, uint8_t* inl_ls, cudaStream_t s) {
-    const int a = ws.p_off1[p0], an = ws.p_off1[p1] - a, c = ws.l_off1[p0], cn = ws.l_off1[p1] - c;
-    D2H(ctx, results, ws.d_results, sizeof(PlPoseResult), p0, p1 - p0, s);
-    D2H(ctx, m12_pt, ws.d_m12p, 4, a, an, s);
-    D2H(ctx, m12_ls, ws.d_m12l, 4, c, cn, s);
-    D2H(ctx, inl_pt, ws.d_inlp, 1, a, an, s);
-    D2H(ctx, inl_ls, ws.d_inll, 1, c, cn, s);
+    CK(ctx, copy_rows(results, ws.d_results.p, sizeof(PlPoseResult), p0, p1 - p0, cudaMemcpyDeviceToHost, s));
+    const RecPtrs dst = RecPtrs::from(M12_PT, {m12_pt, inl_pt, m12_ls, inl_ls});
+    for (int k = M12_PT; k < N_REC; ++k) {   // the tracker's rows, per previous-frame feature
+        const std::vector<int32_t>& off = rec_is_point(k) ? ws.p_off1 : ws.l_off1;
+        CK(ctx, copy_rows(dst.p[k], ws.prev.rec[k].p, REC_BYTES[k], off[p0], off[p1] - off[p0], cudaMemcpyDeviceToHost, s));
+    }
     return 0;
 }
 
@@ -592,7 +602,7 @@ int plstvo_match_batch(PlContext* ctx, int B, const uint8_t* d1, const int32_t* 
     CK(ctx, cudaMemcpyAsync(d_pts, pts.data(), (size_t)B * sizeof(MatchProblem), cudaMemcpyHostToDevice, ctx->s_main));
     CK(ctx, launch_match_finalize(d_pts, B, ws.max_n2, d_counts, ctx->s_main));
     ctx->launches++;
-    CK(ctx, cudaMemcpyAsync(m12, ws.d_m12p.p, (size_t)off1[B] * 4, cudaMemcpyDeviceToHost, ctx->s_main));
+    if ((rc = ws_download_range(ctx, ws, 0, B, nullptr, m12, nullptr, nullptr, nullptr, ctx->s_main))) return rc;
     return counts_total(ctx, ctx->s_main, B, d_counts, counts);
 }
 
@@ -669,10 +679,7 @@ int plstvo_f2f_tracking(PlContext* ctx, const PlConfig* cfg, const PlFrameBatch*
     CK(ctx, launch_match_finalize(ws.d_problems.as<MatchProblem>(), 2 * B, ws.max_n2, ctx->scratch.as<int32_t>(),
                                   ctx->s_main));
     ctx->launches++;
-    if (m12_pt && prev->pt_off[B])
-        CK(ctx, cudaMemcpyAsync(m12_pt, ws.d_m12p.p, (size_t)prev->pt_off[B] * 4, cudaMemcpyDeviceToHost, ctx->s_main));
-    if (m12_ls && prev->ls_off[B])
-        CK(ctx, cudaMemcpyAsync(m12_ls, ws.d_m12l.p, (size_t)prev->ls_off[B] * 4, cudaMemcpyDeviceToHost, ctx->s_main));
+    if ((rc = ws_download_range(ctx, ws, 0, B, nullptr, m12_pt, m12_ls, nullptr, nullptr, ctx->s_main))) return rc;
     if (n_matched)
         CK(ctx, cudaMemcpyAsync(n_matched, ctx->scratch.p, (size_t)2 * B * 4, cudaMemcpyDeviceToHost, ctx->s_main));
     CK(ctx, cudaStreamSynchronize(ctx->s_main));
@@ -706,16 +713,8 @@ int plstvo_optimize_pose(PlContext* ctx, const PlCamera* cam, const PlConfig* cf
     Workspace& ws = ctx->ws;
     ws.planned = false;   // the explicit-list path reuses the workspace's buffers with its own layout
     cudaStream_t s = ctx->s_main;
-    struct Up { DevBuf* buf; const void* src; size_t bytes; };
-    Up ups[] = {{&ws.d_poff1, m->pt_off, (size_t)(B + 1) * 4}, {&ws.d_loff1, m->ls_off, (size_t)(B + 1) * 4},
-                {&ws.d_ptP, m->pt_P, n * 24}, {&ws.d_ptpl, m->pt_pl_obs, n * 16}, {&ws.d_pts2, m->pt_sigma2, n * 8},
-                {&ws.d_inlp, m->pt_inlier, n}, {&ws.d_lssP, m->ls_sP, l * 24}, {&ws.d_lseP, m->ls_eP, l * 24},
-                {&ws.d_lsle, m->ls_le_obs, l * 24}, {&ws.d_lsspl, m->ls_spl, l * 16}, {&ws.d_lsepl, m->ls_epl, l * 16},
-                {&ws.d_lss2, m->ls_sigma2, l * 8}, {&ws.d_inll, m->ls_inlier, l}};
-    for (auto& u : ups) {
-        CK(ctx, u.buf->ensure(std::max<size_t>(u.bytes, 16)));
-        if (u.src && u.bytes) CK(ctx, cudaMemcpyAsync(u.buf->p, u.src, u.bytes, cudaMemcpyHostToDevice, s));
-    }
+    RecPtrs lists;
+    if (const int rc = upload_matched(ctx, m, ws.prev, s, &lists)) return rc;
     CK(ctx, ws.d_results.ensure((size_t)B * sizeof(PlPoseResult)));
     CK(ctx, ws.d_priors.ensure((size_t)B * sizeof(PlPrior)));
     if (priors) CK(ctx, cudaMemcpyAsync(ws.d_priors.p, priors, (size_t)B * sizeof(PlPrior), cudaMemcpyHostToDevice, s));
@@ -727,12 +726,7 @@ int plstvo_optimize_pose(PlContext* ctx, const PlCamera* cam, const PlConfig* cf
     prm.cam = *cam;
     prm.cfg = *cfg;
     prm.mode = 1;
-    prm.matched = MatchedDev{ws.d_poff1.as<int32_t>(), ws.d_loff1.as<int32_t>(), ws.d_ptP.as<double>(),
-                             ws.d_ptpl.as<double>(), ws.d_pts2.as<double>(),
-                             m->pt_inlier ? ws.d_inlp.as<uint8_t>() : nullptr, ws.d_lssP.as<double>(),
-                             ws.d_lseP.as<double>(), ws.d_lsle.as<double>(), ws.d_lsspl.as<double>(),
-                             ws.d_lsepl.as<double>(), ws.d_lss2.as<double>(),
-                             m->ls_inlier ? ws.d_inll.as<uint8_t>() : nullptr};
+    prm.prev = prm.curr = rows_dev(ws.prev.pt_off, ws.prev.ls_off, lists);
     prm.priors = priors ? ws.d_priors.as<PlPrior>() : nullptr;
     prm.results = ws.d_results.as<PlPoseResult>();
     prm.inlier_pt = ctx->gn_out[0].as<uint8_t>();
@@ -1154,21 +1148,9 @@ int plstvo_gn_eval_stream(PlContext* ctx, const PlCamera* cam, const PlConfig* c
     CK(ctx, cudaSetDevice(ctx->device));
     const size_t n = m->pt_off[B], l = m->ls_off[B];
     cudaStream_t s = ctx->s_main;
-    struct Up { const void* src; size_t bytes; };
-    const Up ups[8 + 5] = {{m->pt_off, (size_t)(B + 1) * 4}, {m->ls_off, (size_t)(B + 1) * 4}, {m->pt_P, n * 24},
-                           {m->pt_pl_obs, n * 16}, {m->pt_sigma2, n * 8}, {m->ls_sP, l * 24}, {m->ls_eP, l * 24},
-                           {m->ls_le_obs, l * 24}, {m->ls_spl, l * 16}, {m->ls_epl, l * 16}, {m->ls_sigma2, l * 8},
-                           {m->pt_inlier, n}, {m->ls_inlier, l}};
-    DevBuf* bufs = ctx->gs_in;   // resident inputs of the roofline run (context lifetime)
-    for (int i = 0; i < 13; ++i) {
-        CK(ctx, bufs[i].ensure(std::max<size_t>(ups[i].bytes, 16)));
-        if (ups[i].src && ups[i].bytes)
-            CK(ctx, cudaMemcpyAsync(bufs[i].p, ups[i].src, ups[i].bytes, cudaMemcpyHostToDevice, s));
-    }
-    MatchedDev md{bufs[0].as<int32_t>(), bufs[1].as<int32_t>(), bufs[2].as<double>(), bufs[3].as<double>(),
-                  bufs[4].as<double>(), m->pt_inlier ? bufs[11].as<uint8_t>() : nullptr, bufs[5].as<double>(),
-                  bufs[6].as<double>(), bufs[7].as<double>(), bufs[8].as<double>(), bufs[9].as<double>(),
-                  bufs[10].as<double>(), m->ls_inlier ? bufs[12].as<uint8_t>() : nullptr};
+    RecPtrs lists;   // resident inputs of the roofline run (context lifetime)
+    if (const int rc = upload_matched(ctx, m, ctx->gs_in, s, &lists)) return rc;
+    const RowsDev md = rows_dev(ctx->gs_in.pt_off, ctx->gs_in.ls_off, lists);
     // fp32-packed records (SURVEY 8(a) A4/A5: 32 B per point, 64 B per line), packed once on the device
     DevBuf &rec_pt = ctx->gs_rec_pt, &rec_ls = ctx->gs_rec_ls;
     CK(ctx, rec_pt.ensure(std::max<size_t>(n * 32, 32)));
@@ -1193,7 +1175,7 @@ int plstvo_gn_eval_stream(PlContext* ctx, const PlCamera* cam, const PlConfig* c
     CK(ctx, ev.create());
     const cudaEvent_t e0 = ev[0], e1 = ev[1];
     auto sweep = [&]() {
-        return launch_gn_eval_stream(*cam, *cfg, bufs[0].as<int32_t>(), bufs[1].as<int32_t>(), rec_pt.as<float4>(),
+        return launch_gn_eval_stream(*cam, *cfg, md.pt_off, md.ls_off, rec_pt.as<float4>(),
                                      rec_ls.as<float4>(), B, ctx->gn_in[0].as<double>(), ctx->gn_in[1].as<double>(), bpp,
                                      ctx->sm_count, dH, dg, de, s);
     };

@@ -487,20 +487,15 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     CK(ctx, cudaEventRecord(planned, ctx->s_h2d));
     CK(ctx, cudaStreamWaitEvent(s, planned, 0));
     if (call) {
-        if (const int rc2 = session_gather_named(ctx, *call, workspace_prev_rows(ws), s)) return rc2;
+        if (const int rc2 = session_gather_named(ctx, *call, ws.prev.rows(PREV_ROLE), s)) return rc2;
     } else {
-        for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], B, 0, workspace_prev_rows(ws), a.i32(sets[k].o_ooff), d_cams));
+        for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], B, 0, ws.prev.rows(PREV_ROLE), a.i32(sets[k].o_ooff), d_cams));
     }
     // the current-frame role: the set's frames from `first` on (sequence mode: the second frame)
-    RecPtrs curr_rows;
-    curr_rows.p[PT_PL] = ws.d_ptpl.p;
-    curr_rows.p[PT_DESC] = ws.d_pdesc2.p;
-    curr_rows.p[LS_LE] = ws.d_lsle.p;
-    curr_rows.p[LS_DESC] = ws.d_ldesc2.p;
     const int first = sequence ? 1 : 0;
     for (int k = 0; k < 2; ++k) {
         const Set& st = sets[one_set ? k : 2 + k];
-        CK(ctx, lift(st, B, first, curr_rows, a.i32(sequence ? st.o_ooff2 : st.o_ooff), d_cams));
+        CK(ctx, lift(st, B, first, ws.curr.rows(CURR_ROLE), a.i32(sequence ? st.o_ooff2 : st.o_ooff), d_cams));
     }
     ctx->launches += call ? 2 : 4;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
@@ -511,11 +506,9 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[2], s));
     if (call && call->retain) {   // the tracker's rows, indexed by the kept frames' features (fp's offsets)
         const SessionRetained& kr = ss->kept;
-        const DevBuf* src[4] = {&ws.d_m12p, &ws.d_inlp, &ws.d_m12l, &ws.d_inll};
-        for (int k = 0; k < 4; ++k) {
-            const int r = M12_PT + k;
+        for (int r = M12_PT; r < N_REC; ++r) {
             const size_t bytes = kr.rows[r] * (size_t)REC_BYTES[r];
-            if (bytes) CK(ctx, cudaMemcpyAsync(kr.rec.p[r], src[k]->p, bytes, cudaMemcpyDeviceToDevice, s));
+            if (bytes) CK(ctx, cudaMemcpyAsync(kr.rec.p[r], ws.prev.rec[r].p, bytes, cudaMemcpyDeviceToDevice, s));
         }
     }
     if (dev && dev->tracked) return dev->tracked(ws);

@@ -37,15 +37,16 @@ constexpr int K2_THREADS = 512;   // one pair per SM at a time: at a few pairs p
 constexpr int K2_WARPS   = K2_THREADS / 32;
 constexpr int ACC_N      = 28;    // 21 (upper triangle of J J^T w) + 6 (J r w) + 1 (r^2 w)
 
-// device copies of the PlFrameBatch arrays (all frames of a batch concatenated)
-struct FrameDev {
+// The rows the solver reads (device copies, all frames or lists of a batch concatenated): a frame's records.h arrays
+// (PlFrameBatch), or explicit matched lists (PlMatchedBatch: pt_pl and ls_le are the observations pl_obs and le_obs).  A
+// null array is one not supplied (ls_level: level 0 everywhere; the inlier flags: all true).  Built by rows_dev (host.cuh).
+struct RowsDev {
     const int32_t* pt_off;
     const int32_t* ls_off;
-    const uint8_t* pdesc;
-    const uint8_t* ldesc;
     const double*  pt_P;
     const double*  pt_pl;
     const double*  pt_sigma2;
+    const uint8_t* pt_inlier;
     const double*  ls_sP;
     const double*  ls_eP;
     const double*  ls_le;
@@ -53,22 +54,6 @@ struct FrameDev {
     const double*  ls_epl;
     const double*  ls_sigma2;
     const int32_t* ls_level;
-};
-
-// device copy of PlMatchedBatch (explicit matched lists)
-struct MatchedDev {
-    const int32_t* pt_off;
-    const int32_t* ls_off;
-    const double*  pt_P;
-    const double*  pt_pl_obs;
-    const double*  pt_sigma2;
-    const uint8_t* pt_inlier;
-    const double*  ls_sP;
-    const double*  ls_eP;
-    const double*  ls_le_obs;
-    const double*  ls_spl;
-    const double*  ls_epl;
-    const double*  ls_sigma2;
     const uint8_t* ls_inlier;
 };
 
@@ -77,8 +62,7 @@ struct SolveParams {
     PlConfig cfg;
     int32_t  mode;            // 0: track (match partials -> mutual -> gather -> optimizePose); 1: explicit lists
     int32_t  first_pair;      // pair index of blockIdx.x == 0
-    FrameDev prev, curr;      // mode 0
-    MatchedDev matched;       // mode 1
+    RowsDev  prev, curr;      // mode 1: both the explicit lists (entry i's observation is current row i)
     const MatchProblem* problems;   // mode 0: [2 * pair + {0: points, 1: lines}]
     const PlPrior* priors;    // may be null
     PlPoseResult*  results;
@@ -304,7 +288,7 @@ cudaError_t launch_rectify_remap(int n_img, int per_block, int W, int H, const u
 // GN evaluation streamed from HBM (roofline kernel of config C5): fp32-packed records, TMA-staged tiles
 int gn_stream_tiles(int n_pt, int n_ls);
 int gn_stream_partials_per_slice();   // fp64 partial records one slice writes (one per consumer warp)   // 16 KB tiles of one problem (512 points or 256 lines each)
-cudaError_t launch_pack_records(const MatchedDev& m, const PlCamera& cam, int B, int n_pt, int n_ls, float4* pt, float4* ls,
+cudaError_t launch_pack_records(const RowsDev& m, const PlCamera& cam, int B, int n_pt, int n_ls, float4* pt, float4* ls,
                                 cudaStream_t stream);
 cudaError_t launch_gn_eval_stream(const PlCamera& cam, const PlConfig& cfg, const int32_t* pt_off, const int32_t* ls_off,
                                   const float4* pt, const float4* ls, int B, const double* DT, double* partial,

@@ -38,7 +38,7 @@ __device__ __forceinline__ int gs_find_problem(const int32_t* __restrict__ off, 
 }
 
 // device-side packing of the double arrays into the tile-planar fp32 records
-__global__ void pack_records_kernel(MatchedDev m, PlCamera cam, int B, int n_pt, int n_ls, float4* __restrict__ pt,
+__global__ void pack_records_kernel(RowsDev m, PlCamera cam, int B, int n_pt, int n_ls, float4* __restrict__ pt,
                                     float4* __restrict__ ls) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const GsCamD c = {cam.fx, cam.fy, cam.cx, cam.cy};
@@ -47,7 +47,7 @@ __global__ void pack_records_kernel(MatchedDev m, PlCamera cam, int B, int n_pt,
         const int j = i - p0, t = j / GS_PT_TILE, r = j % GS_PT_TILE, cnt = min(GS_PT_TILE, np - t * GS_PT_TILE);
         float4* base = pt + 2 * (size_t)(p0 + t * GS_PT_TILE);
         const size_t a = (size_t)i;
-        gs_pack_point(c, m.pt_P[3 * a], m.pt_P[3 * a + 1], m.pt_P[3 * a + 2], m.pt_pl_obs[2 * a], m.pt_pl_obs[2 * a + 1],
+        gs_pack_point(c, m.pt_P[3 * a], m.pt_P[3 * a + 1], m.pt_P[3 * a + 2], m.pt_pl[2 * a], m.pt_pl[2 * a + 1],
                       sqrt(m.pt_sigma2[a]), !(m.pt_inlier && !m.pt_inlier[a]), base[r], base[cnt + r]);
     }
     if (i < n_ls) {
@@ -59,7 +59,7 @@ __global__ void pack_records_kernel(MatchedDev m, PlCamera cam, int B, int n_pt,
         double oa, ob, oc;
         overlap_coeffs(su, sv, eu, ev, oa, ob, oc);
         gs_pack_line(c, m.ls_sP[3 * a], m.ls_sP[3 * a + 1], m.ls_sP[3 * a + 2], m.ls_eP[3 * a], m.ls_eP[3 * a + 1], m.ls_eP[3 * a + 2],
-                     m.ls_le_obs[3 * a], m.ls_le_obs[3 * a + 1], m.ls_le_obs[3 * a + 2], oa, ob, oc, sqrt(m.ls_sigma2[a]),
+                     m.ls_le[3 * a], m.ls_le[3 * a + 1], m.ls_le[3 * a + 2], oa, ob, oc, sqrt(m.ls_sigma2[a]),
                      !(m.ls_inlier && !m.ls_inlier[a]), base[r], base[cnt + r], base[2 * cnt + r], base[3 * cnt + r]);
     }
 }
@@ -225,7 +225,7 @@ int gn_stream_tiles(int n_pt, int n_ls) {
     return (n_pt + GS_PT_TILE - 1) / GS_PT_TILE + (n_ls + GS_LS_TILE - 1) / GS_LS_TILE;
 }
 
-cudaError_t launch_pack_records(const MatchedDev& m, const PlCamera& cam, int B, int n_pt, int n_ls, float4* pt, float4* ls,
+cudaError_t launch_pack_records(const RowsDev& m, const PlCamera& cam, int B, int n_pt, int n_ls, float4* pt, float4* ls,
                                 cudaStream_t stream) {
     const int n = n_pt > n_ls ? n_pt : n_ls;
     if (n <= 0 || B <= 0) return cudaSuccess;

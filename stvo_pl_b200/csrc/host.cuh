@@ -123,6 +123,40 @@ struct SolvePlan {
     size_t feat_stride = 0;    // doubles of global list scratch per pair (0: none needed)
 };
 
+// One side of the tracker's device storage: the CSR offsets of its points and lines and one buffer per records.h array, each
+// grown on demand to the rows of the call that uses it (a workspace's previous and current frame; explicit matched lists).
+// Only the arrays a side's calls use are ever allocated; the others stay null.
+struct FrameBufs {
+    DevBuf pt_off, ls_off;
+    DevBuf rec[N_REC];
+    // the buffers of the arrays in role, the other entries null
+    template <int N> RecPtrs rows(const int (&role)[N]) const {
+        RecPtrs r;
+        for (int k : role) r.p[k] = rec[k].p;
+        return r;
+    }
+};
+
+// the solver's view of rows r (device) under offsets pt_off / ls_off
+inline RowsDev rows_dev(const DevBuf& pt_off, const DevBuf& ls_off, const RecPtrs& r) {
+    RowsDev v;
+    v.pt_off = pt_off.as<int32_t>();
+    v.ls_off = ls_off.as<int32_t>();
+    v.pt_P = r.at<double>(PT_P);
+    v.pt_pl = r.at<double>(PT_PL);
+    v.pt_sigma2 = r.at<double>(PT_S2);
+    v.pt_inlier = r.at<uint8_t>(INL_PT);
+    v.ls_sP = r.at<double>(LS_SP);
+    v.ls_eP = r.at<double>(LS_EP);
+    v.ls_le = r.at<double>(LS_LE);
+    v.ls_spl = r.at<double>(LS_SPL);
+    v.ls_epl = r.at<double>(LS_EPL);
+    v.ls_sigma2 = r.at<double>(LS_S2);
+    v.ls_level = r.at<int32_t>(LS_LEVEL);
+    v.ls_inlier = r.at<uint8_t>(INL_LS);
+    return v;
+}
+
 // Work plan + device storage of one batch of frame pairs (also the body of PlDeviceBatch)
 struct Workspace {
     int B = 0;
@@ -138,12 +172,10 @@ struct Workspace {
     std::vector<MatchProblem> problems;   // [2B]: points, lines
     int max_n2 = 0;
     SolvePlan solver;
-    // device storage
-    DevBuf d_poff1, d_poff2, d_loff1, d_loff2;
-    DevBuf d_pdesc1, d_pdesc2, d_ldesc1, d_ldesc2;
-    DevBuf d_ptP, d_pts2, d_ptpl;                                      // prev P, prev sigma2, curr pl
-    DevBuf d_lssP, d_lseP, d_lsspl, d_lsepl, d_lss2, d_lslev, d_lsle;  // prev ...; curr le
-    DevBuf d_priors, d_results, d_m12p, d_m12l, d_inlp, d_inll;
+    // device storage: the previous frame's PREV_ROLE arrays and the tracker's m12 and inlier rows, the current frame's
+    // CURR_ROLE arrays (plstvo_optimize_pose: its explicit lists in prev)
+    FrameBufs prev, curr;
+    DevBuf d_priors, d_results;
     DevBuf d_rowpart, d_colpart, d_problems, d_feat;
     DevBuf d_phase;   // solver phase cycle counters (plstvo_batch_phase_cycles)
     // K1 (match_tc.cu): per-block value partials, work items
@@ -178,7 +210,8 @@ struct PlContext {
     // per-entry-point device arenas (context-owned: a process may hold one context per GPU)
     plstvo::DevBuf arena_grid, arena_lift_pt, arena_lift_ls, arena_stereo;
     plstvo::DevBuf arena_track_stereo[3];   // [0]: blocking calls, [1 + slot]: plstvo_track_stereo_*_async
-    plstvo::DevBuf gs_in[13], gs_rec_pt, gs_rec_ls;   // resident inputs / packed records of the streamed evaluator
+    plstvo::FrameBufs gs_in;       // resident inputs of the streamed evaluator (plstvo_gn_eval_stream): explicit lists
+    plstvo::DevBuf gs_rec_pt, gs_rec_ls;   // their packed records
     plstvo::DevBuf arena_orb;      // plstvo_orb_compute_batch: images, level buffers, key points, outputs
     bool orb_tables = false;
     plstvo::Events<4> orb_ev;
@@ -399,14 +432,6 @@ inline cudaError_t down_records(const Arena& a, const RecPtrs& dst, const size_t
 }
 
 // ---- session.cu: the previous-frame-role records of kept frames (plstvo_stereo_session_*) ----
-// The workspace's previous-frame buffers, the PREV_ROLE entries of a RecPtrs
-inline RecPtrs workspace_prev_rows(const Workspace& ws) {
-    RecPtrs r;
-    r.p[PT_P] = ws.d_ptP.p; r.p[PT_S2] = ws.d_pts2.p; r.p[PT_DESC] = ws.d_pdesc1.p;
-    r.p[LS_SPL] = ws.d_lsspl.p; r.p[LS_EPL] = ws.d_lsepl.p; r.p[LS_SP] = ws.d_lssP.p; r.p[LS_EP] = ws.d_lseP.p;
-    r.p[LS_S2] = ws.d_lss2.p; r.p[LS_LEVEL] = ws.d_lslev.p; r.p[LS_DESC] = ws.d_ldesc1.p;
-    return r;
-}
 // One session pool: the kept frames of every stream in the previous-frame role (the PREV_ROLE entries of rows), point rows
 // and line rows in stream-id order.
 struct SessionPool {

@@ -1476,11 +1476,53 @@ __device__ int compaction_plan(State& st, const int32_t* __restrict__ m12, int n
     return total;
 }
 
+// One matched point / line into list slot k: previous-frame row a of P, observed at current-frame row b of C (mode 1: the
+// explicit lists' entry a, b = a), initial inlier flag inl.  The line weight is the level rule of track mode (level_rule) or
+// the explicit lists' sigma2 as given.
+__device__ __forceinline__ void gather_point(const RowsDev& P, const RowsDev& C, Feat& f, const RecordSink& rs, int k, int np,
+                                             size_t a, size_t b, bool inl) {
+    const double x = P.pt_P[3 * a], y = P.pt_P[3 * a + 1], z = P.pt_P[3 * a + 2];
+    const double u = C.pt_pl[2 * b], v = C.pt_pl[2 * b + 1];    // pl_obs = curr pl (:148)
+    const double pss = sqrt(P.pt_sigma2[a]);                     // PointFeature::safeCopy keeps sigma2
+    f.Px[k] = x; f.Py[k] = y; f.Pz[k] = z;
+    f.pu[k] = u; f.pv[k] = v;
+    f.pss[k] = pss;
+    f.inl_p[k] = inl ? 1 : 0;
+    if (rs.on) sink_point(rs, k, np, x, y, z, u, v, pss, inl);
+}
+__device__ __forceinline__ void gather_line(const RowsDev& P, const RowsDev& C, Feat& f, const RecordSink& rs, int k, int nl,
+                                            size_t a, size_t b, bool inl, bool level_rule, double lsd_scale) {
+    const double sx = P.ls_sP[3 * a], sy = P.ls_sP[3 * a + 1], sz = P.ls_sP[3 * a + 2];
+    const double ex = P.ls_eP[3 * a], ey = P.ls_eP[3 * a + 1], ez = P.ls_eP[3 * a + 2];
+    const double l0 = C.ls_le[3 * b], l1 = C.ls_le[3 * b + 1], l2 = C.ls_le[3 * b + 2];   // le_obs = curr le (:175)
+    double oa, ob, oc;
+    overlap_coeffs(P.ls_spl[2 * a], P.ls_spl[2 * a + 1], P.ls_epl[2 * a], P.ls_epl[2 * a + 1], oa, ob, oc);
+    double lss;
+    if (level_rule) {
+        // LineFeature::safeCopy -> ctor re-applies the level rule (src/stereoFeatures.cpp:117-135):
+        // sigma2' = 1 / (sigma2 * lsdScale^level)^2
+        double s2 = P.ls_sigma2[a];
+        const int level = P.ls_level ? P.ls_level[a] : 0;
+        for (int l = 0; l < level; l++) s2 *= lsd_scale;
+        lss = sqrt(1.0 / (s2 * s2));
+    } else {
+        lss = sqrt(P.ls_sigma2[a]);
+    }
+    f.sX[k] = sx; f.sY[k] = sy; f.sZ[k] = sz;
+    f.eX[k] = ex; f.eY[k] = ey; f.eZ[k] = ez;
+    f.l0[k] = l0; f.l1[k] = l1; f.l2[k] = l2;
+    f.oa[k] = oa; f.ob[k] = ob; f.oc[k] = oc;
+    f.lss[k] = lss;
+    f.inl_l[k] = inl ? 1 : 0;
+    if (rs.on) sink_line(rs, k, nl, sx, sy, sz, ex, ey, ez, l0, l1, l2, oa, ob, oc, lss, inl);
+}
+
 __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st, double* sortbuf, Feat& f, uint16_t* midx_p,
                                     uint16_t* midx_l, int& n1p, int& n1l, size_t& out_p0, size_t& out_l0, long long& t_ph,
                                     const RecordSink& rs) {
     const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5, nw = nth >> 5;
-    const PlConfig& cfg = prm.cfg;
+    const RowsDev& P = prm.prev;
+    const RowsDev& C = prm.curr;
     if (prm.mode == 0) {
         // ---- A. finish the matching: ratio test, mutual filter -> m12 (global) ----
         const MatchProblem pp = prm.problems[2 * pair], pl = prm.problems[2 * pair + 1];
@@ -1492,8 +1534,6 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
         t_ph = clock64();
 
         // ---- B. f2fTracking glue: ordered compaction of the matched features into SoA (and, streamed solver, fp32 records) ----
-        const FrameDev& P = prm.prev;
-        const FrameDev& C = prm.curr;
         int* cc = reinterpret_cast<int*>(sortbuf);
         const int a0 = P.pt_off[pair], b0 = C.pt_off[pair];
         n1p = P.pt_off[pair + 1] - a0;
@@ -1507,16 +1547,8 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
                 const unsigned bal = __ballot_sync(FULL_MASK, i2 >= 0);
                 if (i2 >= 0) {
                     const int k = cc[ch] + __popc(bal & ((1u << lane) - 1u));
-                    const double* p3 = P.pt_P + 3 * (size_t)(a0 + i);
-                    const double* o2 = C.pt_pl + 2 * (size_t)(b0 + i2);    // pl_obs = curr pl (:148)
-                    const double x = p3[0], y = p3[1], z = p3[2], u = o2[0], v = o2[1];
-                    const double pss = sqrt(P.pt_sigma2[a0 + i]);          // PointFeature::safeCopy keeps sigma2
-                    f.Px[k] = x; f.Py[k] = y; f.Pz[k] = z;
-                    f.pu[k] = u; f.pv[k] = v;
-                    f.pss[k] = pss;
-                    f.inl_p[k] = 1;
+                    gather_point(P, C, f, rs, k, np, (size_t)(a0 + i), (size_t)(b0 + i2), true);
                     midx_p[k] = (uint16_t)i;
-                    if (rs.on) sink_point(rs, k, np, x, y, z, u, v, pss, true);
                 }
             }
             f.np = np;
@@ -1534,27 +1566,8 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
                 const unsigned bal = __ballot_sync(FULL_MASK, i2 >= 0);
                 if (i2 >= 0) {
                     const int k = cc[ch] + __popc(bal & ((1u << lane) - 1u));
-                    const size_t a = (size_t)(c0 + i);
-                    const double sx = P.ls_sP[3 * a], sy = P.ls_sP[3 * a + 1], sz = P.ls_sP[3 * a + 2];
-                    const double ex = P.ls_eP[3 * a], ey = P.ls_eP[3 * a + 1], ez = P.ls_eP[3 * a + 2];
-                    const double* le = C.ls_le + 3 * (size_t)(d0 + i2);    // le_obs = curr le (:175)
-                    const double l0 = le[0], l1 = le[1], l2 = le[2];
-                    double oa, ob, oc;
-                    overlap_coeffs(P.ls_spl[2 * a], P.ls_spl[2 * a + 1], P.ls_epl[2 * a], P.ls_epl[2 * a + 1], oa, ob, oc);
-                    // LineFeature::safeCopy -> ctor re-applies the level rule (src/stereoFeatures.cpp:117-135):
-                    // sigma2' = 1 / (sigma2 * lsdScale^level)^2
-                    double s2 = P.ls_sigma2[a];
-                    const int level = P.ls_level ? P.ls_level[a] : 0;
-                    for (int l = 0; l < level; l++) s2 *= cfg.lsd_scale;
-                    const double lss = sqrt(1.0 / (s2 * s2));
-                    f.sX[k] = sx; f.sY[k] = sy; f.sZ[k] = sz;
-                    f.eX[k] = ex; f.eY[k] = ey; f.eZ[k] = ez;
-                    f.l0[k] = l0; f.l1[k] = l1; f.l2[k] = l2;
-                    f.oa[k] = oa; f.ob[k] = ob; f.oc[k] = oc;
-                    f.lss[k] = lss;
-                    f.inl_l[k] = 1;
+                    gather_line(P, C, f, rs, k, nl, (size_t)(c0 + i), (size_t)(d0 + i2), true, true, prm.cfg.lsd_scale);
                     midx_l[k] = (uint16_t)i;
-                    if (rs.on) sink_line(rs, k, nl, sx, sy, sz, ex, ey, ez, l0, l1, l2, oa, ob, oc, lss, true);
                 }
             }
             f.nl = nl;
@@ -1564,40 +1577,19 @@ __device__ void build_matched_lists(const SolveParams& prm, int pair, State& st,
             st.n_inl_l = f.nl;
         }
     } else {
-        // ---- explicit matched lists ----
-        const MatchedDev& M = prm.matched;
-        const int a0 = M.pt_off[pair], c0 = M.ls_off[pair];
-        n1p = f.np = M.pt_off[pair + 1] - a0;
-        n1l = f.nl = M.ls_off[pair + 1] - c0;
+        // ---- explicit matched lists: entry i is slot i, its observation current row i ----
+        const int a0 = P.pt_off[pair], c0 = P.ls_off[pair];
+        n1p = f.np = P.pt_off[pair + 1] - a0;
+        n1l = f.nl = P.ls_off[pair + 1] - c0;
         out_p0 = (size_t)a0;
         out_l0 = (size_t)c0;
         for (int i = tid; i < f.np; i += nth) {
             const size_t a = (size_t)(a0 + i);
-            const double x = M.pt_P[3 * a], y = M.pt_P[3 * a + 1], z = M.pt_P[3 * a + 2];
-            const double u = M.pt_pl_obs[2 * a], v = M.pt_pl_obs[2 * a + 1], pss = sqrt(M.pt_sigma2[a]);
-            const bool inl = M.pt_inlier ? (M.pt_inlier[a] != 0) : true;
-            f.Px[i] = x; f.Py[i] = y; f.Pz[i] = z;
-            f.pu[i] = u; f.pv[i] = v;
-            f.pss[i] = pss;
-            f.inl_p[i] = inl ? 1 : 0;
-            if (rs.on) sink_point(rs, i, f.np, x, y, z, u, v, pss, inl);
+            gather_point(P, C, f, rs, i, f.np, a, a, P.pt_inlier ? (P.pt_inlier[a] != 0) : true);
         }
         for (int i = tid; i < f.nl; i += nth) {
             const size_t a = (size_t)(c0 + i);
-            const double sx = M.ls_sP[3 * a], sy = M.ls_sP[3 * a + 1], sz = M.ls_sP[3 * a + 2];
-            const double ex = M.ls_eP[3 * a], ey = M.ls_eP[3 * a + 1], ez = M.ls_eP[3 * a + 2];
-            const double l0 = M.ls_le_obs[3 * a], l1 = M.ls_le_obs[3 * a + 1], l2 = M.ls_le_obs[3 * a + 2];
-            double oa, ob, oc;
-            overlap_coeffs(M.ls_spl[2 * a], M.ls_spl[2 * a + 1], M.ls_epl[2 * a], M.ls_epl[2 * a + 1], oa, ob, oc);
-            const double lss = sqrt(M.ls_sigma2[a]);
-            const bool inl = M.ls_inlier ? (M.ls_inlier[a] != 0) : true;
-            f.sX[i] = sx; f.sY[i] = sy; f.sZ[i] = sz;
-            f.eX[i] = ex; f.eY[i] = ey; f.eZ[i] = ez;
-            f.l0[i] = l0; f.l1[i] = l1; f.l2[i] = l2;
-            f.oa[i] = oa; f.ob[i] = ob; f.oc[i] = oc;
-            f.lss[i] = lss;
-            f.inl_l[i] = inl ? 1 : 0;
-            if (rs.on) sink_line(rs, i, f.nl, sx, sy, sz, ex, ey, ez, l0, l1, l2, oa, ob, oc, lss, inl);
+            gather_line(P, C, f, rs, i, f.nl, a, a, P.ls_inlier ? (P.ls_inlier[a] != 0) : true, false, 0.0);
         }
         // the reference sets n_inliers from the list sizes; explicit flags only matter to the evaluator
         if (tid == 0) {
@@ -1927,8 +1919,8 @@ __device__ __forceinline__ StreamView stream_view(const SolveParams& prm, const 
     StreamView v;
     v.st = reinterpret_cast<State*>(smem);
     v.sortbuf = reinterpret_cast<double*>(smem + align_up(sizeof(State), 16));
-    v.slot_p = (size_t)(prm.mode == 0 ? prm.prev.pt_off[pair] : prm.matched.pt_off[pair]);
-    v.slot_l = (size_t)(prm.mode == 0 ? prm.prev.ls_off[pair] : prm.matched.ls_off[pair]);
+    v.slot_p = (size_t)prm.prev.pt_off[pair];
+    v.slot_l = (size_t)prm.prev.ls_off[pair];
     v.f = feat_view(prm.feat_scratch + (size_t)local * prm.feat_scratch_stride, prm.cap_pt, prm.cap_ls);
     v.f.inl_p = sb.flag_pt + v.slot_p;
     v.f.inl_l = sb.flag_ls + v.slot_l;
@@ -2462,10 +2454,10 @@ __global__ void __launch_bounds__(256) stream_finalize_kernel(const SolveParams 
     Feat f;
     f.np = c.np;
     f.nl = c.nl;
-    const size_t slot_p = (size_t)(prm.mode == 0 ? prm.prev.pt_off[pair] : prm.matched.pt_off[pair]);
-    const size_t slot_l = (size_t)(prm.mode == 0 ? prm.prev.ls_off[pair] : prm.matched.ls_off[pair]);
-    const int n1p = prm.mode == 0 ? prm.prev.pt_off[pair + 1] - (int)slot_p : c.np;
-    const int n1l = prm.mode == 0 ? prm.prev.ls_off[pair + 1] - (int)slot_l : c.nl;
+    const size_t slot_p = (size_t)prm.prev.pt_off[pair];
+    const size_t slot_l = (size_t)prm.prev.ls_off[pair];
+    const int n1p = prm.prev.pt_off[pair + 1] - (int)slot_p;   // mode 1: the list lengths
+    const int n1l = prm.prev.ls_off[pair + 1] - (int)slot_l;
     const PlPrior* prior = prm.priors ? &prm.priors[pair] : nullptr;
     if (warp == 0) {
         if (lane < 16) st.DT[lane] = sb.DT[(size_t)local * 16 + lane];
@@ -2508,8 +2500,8 @@ cudaError_t stream_solve(const SolveParams& prm_in, int n_pairs, const StreamBuf
     ++nl;
     // instrumentation (optional): lists built | GN stage 1 done | outlier pass done | GN stage 2 done
     if (marks) cudaEventRecord(marks[0], stream);
-    const int32_t* off_p = prm.mode == 0 ? prm.prev.pt_off + prm.first_pair : prm.matched.pt_off + prm.first_pair;
-    const int32_t* off_l = prm.mode == 0 ? prm.prev.ls_off + prm.first_pair : prm.matched.ls_off + prm.first_pair;
+    const int32_t* off_p = prm.prev.pt_off + prm.first_pair;
+    const int32_t* off_l = prm.prev.ls_off + prm.first_pair;
     const PlCamera* cams = CAMS ? pair_cams + prm.first_pair : nullptr;   // the GN loop indexes its problems from 0
     static size_t conf_c[64] = {}, conf_d[64] = {};
     const size_t ring = (size_t)GL_STAGES * GS_STAGE_BYTES;
