@@ -964,12 +964,12 @@ struct LineBlocks {
     }
 };
 
-// One frame set of the stereo step (nf frames) on device inputs, into dev.set[k] (points) and dev.set[k + 1] (lines): the
-// points of ORB's image blocks ob and ob + 1 (left, right, nf images each) and the key lines of line blocks lb and lb + 1,
-// offsets rebased to 0 into pl_off / pr_off.  none: nf + 1 zero offsets, for frames without key lines.
+// One frame set of the stereo step (nf frames) on device inputs, into fs[0] (points) and fs[1] (lines): the points of ORB's
+// image blocks ob and ob + 1 (left, right, nf images each) and the key lines of line blocks lb and lb + 1, offsets rebased to
+// 0 into pl_off / pr_off.  none: nf + 1 zero offsets, for frames without key lines.
 void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const LineBlocks& lines, int lb, int nf,
                        const std::vector<int32_t>& none, std::vector<int32_t>& pl_off, std::vector<int32_t>& pr_off,
-                       PlStereoFeatures& F, StereoDevInputs& dev, int k) {
+                       StereoSet* fs) {
     const size_t kl = orb.off[(size_t)ob * nf], kr = orb.off[(size_t)(ob + 1) * nf];
     pl_off.resize((size_t)nf + 1);
     pr_off.resize((size_t)nf + 1);
@@ -977,29 +977,22 @@ void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const LineBlock
         pl_off[i] = orb.off[(size_t)ob * nf + i] - (int32_t)kl;
         pr_off[i] = orb.off[(size_t)(ob + 1) * nf + i] - (int32_t)kr;
     }
-    const bool has_lines = !lines.lsrc.empty();
-    F = PlStereoFeatures{};
-    F.B = nf;
-    F.pl_off = pl_off.data(); F.pr_off = pr_off.data();
-    F.ll_off = has_lines ? lines.lsrc[(size_t)lb].off : none.data();
-    F.lr_off = has_lines ? lines.lsrc[(size_t)lb + 1].off : none.data();
-    F.angle_l = has_lines ? lines.lsrc[(size_t)lb].angle : nullptr;
-    StereoDevInputs::Set& P = dev.set[k];
-    P = StereoDevInputs::Set{};
-    P.on_device = true;
+    StereoSet& P = fs[0];
+    P = StereoSet{false, nf, pl_off.data(), pr_off.data(), nullptr, true};
     if (pts) {
         P.xy_l = orb.xy + 2 * kl; P.xy_r = orb.xy + 2 * kr; P.oct = orb.octave + kl;
         P.d1 = orb.desc + 32 * kl; P.d2 = orb.desc + 32 * kr;
     }
-    StereoDevInputs::Set& Ls = dev.set[k + 1];
-    Ls = StereoDevInputs::Set{};
-    Ls.on_device = true;   // oct stays null: key lines of octave 0
+    StereoSet& Ls = fs[1];   // oct stays null: key lines of octave 0
+    Ls = StereoSet{true, nf, none.data(), none.data(), nullptr, true};
+    if (!lines.lsrc.empty()) {
+        Ls.l_off = lines.lsrc[(size_t)lb].off; Ls.r_off = lines.lsrc[(size_t)lb + 1].off; Ls.ang = lines.lsrc[(size_t)lb].angle;
+    }
     if (lines.run_lbd) {
         const size_t l0 = (size_t)lines.lbase[(size_t)lb], l1 = (size_t)lines.lbase[(size_t)lb + 1];
         Ls.xy_l = lines.d_seg + 4 * l0; Ls.xy_r = lines.d_seg + 4 * l1;
         Ls.d1 = lines.d_ldesc + 32 * l0; Ls.d2 = lines.d_ldesc + 32 * l1;
     }
-    dev.lines_ready = lines.joined;
 }
 
 // The key-line field rules of a call on frame sets fs[0 .. nfs): the fields are null where the call detects its own key lines
@@ -1160,12 +1153,12 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     }
     // the feature sets: slices of ORB's and LBD's outputs, offsets rebased to 0
     std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
-    PlStereoFeatures feat[2]{};
+    StereoSet sets[2][2];
+    for (int j = 0; j < nfs; ++j) stereo_set_inputs(orb, 2 * j, pts, lines, 2 * j, NF, none, pl_off[j], pr_off[j], sets[j]);
     StereoDevInputs dev;
-    for (int j = 0; j < nfs; ++j)
-        stereo_set_inputs(orb, 2 * j, pts, lines, 2 * j, NF, none, pl_off[j], pr_off[j], feat[j], dev, 2 * j);
+    dev.lines_ready = lines.joined;
     dev.marks = ctx->img_ev.ev + 1;
-    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, &feat[0], one_set ? nullptr : &feat[1], priors, results,
+    if (const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, sets[0], one_set ? nullptr : sets[1], priors, results,
                                            n_stereo, sequence, -1, &dev, call))
         return rc;
     float* ms = ctx->img_ms;   // the call ended synchronised: every event has completed
@@ -1666,9 +1659,10 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
         } else {
             orb.off.assign((size_t)2 * n + 1, 0);
         }
-        PlStereoFeatures feat;
+        StereoSet sets[2];
+        stereo_set_inputs(orb, 0, pts, lines, 2 * t, n, none, pl_off, pr_off, sets);
         StereoDevInputs dev;
-        stereo_set_inputs(orb, 0, pts, lines, 2 * t, n, none, pl_off, pr_off, feat, dev, 0);
+        dev.lines_ready = lines.joined;
         cudaEvent_t* mk = marks[t % 2].ev;
         dev.marks = mk;
         dev.priors_resident = t > 0;   // step t - 1's handler update wrote them
@@ -1709,7 +1703,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
             return 0;
         };
         int32_t* ns = n_stereo ? n_stereo + (size_t)t * 4 * n : nullptr;
-        const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, &feat, nullptr, t == 0 ? priors : nullptr,
+        const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, sets, nullptr, t == 0 ? priors : nullptr,
                                            results + (size_t)t * n, ns, false, -1, &dev, &step);
         if (rc) return rc;
         session_commit(step);

@@ -12,6 +12,114 @@ int check_stereo_offsets(PlContext* ctx, int B, const int32_t* l_off, const int3
 
 }  // namespace
 
+namespace plstvo {
+
+int StereoSet::check(PlContext* ctx) {
+    if (const int rc = check_stereo_offsets(ctx, nf, l_off, r_off)) return rc;
+    N1 = l_off[nf];
+    N2 = r_off[nf];
+    if ((N1 && (!xy_l || (!oct && !on_device) || !d1 || (lines && !ang) || (lift_only && !m12))) ||
+        (N2 && (!xy_r || (!d2 && !lift_only))))
+        return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    return 0;
+}
+
+void StereoSet::take(Arena& a) {
+    const size_t cw = lines ? 4 : 2;   // floats per key point / segment
+    auto host = [&](const void* p, size_t bytes) { return a.take(p && !on_device ? bytes : 0); };
+    o_loff = a.take((size_t)(nf + 1) * 4);
+    o_roff = a.take((size_t)(nf + 1) * 4);
+    o_xyl = host(xy_l, N1 * cw * 4);
+    o_xyr = host(xy_r, N2 * cw * 4);
+    o_ang = a.take(lines ? N1 * 4 : 0);
+    o_oct = a.take(on_device && oct ? 0 : N1 * 4);
+    o_d1 = host(d1, N1 * 32);
+    o_d2 = host(d2, N2 * 32);
+    o_m12 = a.take(N1 * 4);
+    o_cnt = a.take((size_t)nf * 4);
+    o_gcnt = a.take(lift_only ? 0 : (size_t)nf * 4);
+    o_prob = a.take(lift_only ? 0 : (size_t)nf * sizeof(GridProblem));
+}
+
+cudaError_t StereoSet::upload(const Arena& a, cudaStream_t s, const GridScratch* g, GridProblem* probs) const {
+    const size_t cw = lines ? 4 : 2;
+    if (g) g->fill(probs, nf, lines, l_off, r_off, in(a, d1, o_d1), in(a, d2, o_d2), a.i32(o_m12), a.i32(o_gcnt));
+    cudaError_t e = cudaSuccess;
+    auto up = [&](size_t o, const void* src, size_t bytes) { if (!e) e = a.up(o, src, bytes, s); };
+    up(o_loff, l_off, (size_t)(nf + 1) * 4);
+    up(o_roff, r_off, (size_t)(nf + 1) * 4);
+    if (lines) up(o_ang, ang, N1 * 4);
+    if (!on_device) {
+        up(o_xyl, xy_l, N1 * cw * 4);
+        up(o_xyr, xy_r, N2 * cw * 4);
+        up(o_oct, oct, N1 * 4);
+        up(o_d1, d1, N1 * 32);
+        up(o_d2, d2, N2 * 32);
+    } else if (!oct && N1 && !e) {
+        e = cudaMemsetAsync(a.u8(o_oct), 0, N1 * 4, s);   // key lines of octave 0
+    }
+    up(o_m12, m12, N1 * 4);
+    if (g) up(o_prob, probs, (size_t)nf * sizeof(GridProblem));
+    return e;
+}
+
+cudaError_t StereoSet::match(const Arena& a, const GridScratch& g, const PlCamera& cam, const PlStereoMatchConfig& mc,
+                             cudaStream_t s) const {
+    // grid coordinates (src/stereoFrame.cpp:47-48: inv_width = GRID_COLS / image width, inv_height = GRID_ROWS / image height)
+    const int rows = mc.grid_rows, cols = mc.grid_cols;
+    const double inv_w = cols / static_cast<double>(cam.width), inv_h = rows / static_cast<double>(cam.height);
+    const float *kl = in(a, xy_l, o_xyl), *kr = in(a, xy_r, o_xyr);
+    const int n1 = (int)N1, n2 = (int)N2;
+    const cudaError_t e =
+        lines ? launch_stereo_cells_lines(n1, n2, inv_w, inv_h, kl, kr, a.i32(g.qcell), a.f64(g.tline), a.f64(g.tdir), s)
+              : launch_stereo_cells_points(n1, n2, inv_w, inv_h, kl, kr, a.i32(g.qcell), a.i32(g.tcell), s);
+    if (e) return e;
+    // matchGrid with the stereo window (:141-143, :340-342: matching_s_ws cells to the left, same row)
+    const GridParams prm{rows, cols, GRID_CAP, mc.best_lr_matches ? 1 : 0, PlGridWindow{mc.matching_s_ws, 0, 0, 0},
+                         mc.min_ratio_12_p, mc.line_sim_th};
+    return launch_match_grid(a.at<GridProblem>(o_prob), nf, prm, lines, s);
+}
+
+cudaError_t StereoSet::lift(const Arena& a, const PlCamera& cam, const PlStereoConfig& sc, int n, int first,
+                            const RecPtrs& out, cudaStream_t s, const int32_t* out_off, const PlCamera* cams) const {
+    const int32_t *lo = a.i32(o_loff) + first, *ro = a.i32(o_roff) + first, *o = in(a, oct, o_oct);
+    const float *kl = in(a, xy_l, o_xyl), *kr = in(a, xy_r, o_xyr);
+    const uint8_t* dl = in(a, d1, o_d1);
+    int32_t* cnt = a.i32(o_cnt) + first;
+    if (lines)
+        return launch_lift_lines(cam, sc, n, lo, kl, a.f32(o_ang), o, dl, ro, kr, a.i32(o_m12), out, cnt, s, out_off, cams);
+    return launch_lift_points(cam, sc, n, lo, kl, o, dl, ro, kr, a.i32(o_m12), out, cnt, s, out_off, cams);
+}
+
+}  // namespace plstvo
+
+namespace {
+
+// stand-alone lifting of st (lift_only) into out (host)
+int stereo_lift(PlContext* ctx, const PlCamera* cam, const PlStereoConfig* scfg, StereoSet st, const RecPtrs& out,
+                int32_t* counts) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (!cam || !scfg || st.nf < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
+    if (st.nf == 0) return 0;
+    if (const int rc = st.check(ctx)) return rc;
+    CK(ctx, cudaSetDevice(ctx->device));
+    Arena a;
+    st.take(a);
+    const int first = st.lines ? LS_SPL : PT_PL, last = st.lines ? N_LIFT : LS_SPL;
+    size_t o_rec[N_REC];
+    take_records(a, st.N1, first, last, o_rec);
+    CK(ctx, a.alloc(st.lines ? ctx->arena_lift_ls : ctx->arena_lift_pt));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, st.upload(a, s));
+    CK(ctx, st.lift(a, *cam, *scfg, st.nf, 0, arena_records(a, o_rec, first, last), s));
+    ctx->launches++;
+    CK(ctx, down_records(a, out, o_rec, st.N1, first, last, s));
+    return counts_total(ctx, s, st.nf, a.i32(st.o_cnt), counts);
+}
+
+}  // namespace
+
 extern "C" {
 
 // ---- matchGrid (stereo step) -------------------------------------------------------------------------------------
@@ -83,36 +191,9 @@ int plstvo_stereo_lift_points(PlContext* ctx, const PlCamera* cam, const PlStere
                               const float* kp_l, const int32_t* octave_l, const uint8_t* desc_l, const int32_t* r_off,
                               const float* kp_r, const int32_t* m12, double* pt_pl, double* pt_disp, double* pt_P,
                               double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out, int32_t* src_idx, int32_t* counts) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!cam || !scfg || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
-    if (B == 0) return 0;
-    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
-    const size_t N1 = l_off[B], N2 = r_off[B];
-    if (N1 && (!kp_l || !octave_l || !desc_l || !m12)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-    if (N2 && !kp_r) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-    CK(ctx, cudaSetDevice(ctx->device));
-    Arena a;
-    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_kpl = a.take(N1 * 8);
-    const size_t o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_kpr = a.take(N2 * 8), o_m12 = a.take(N1 * 4);
-    size_t o_rec[N_REC];
-    take_records(a, N1, PT_PL, LS_SPL, o_rec);
-    const size_t o_cnt = a.take((size_t)B * 4);
-    CK(ctx, a.alloc(ctx->arena_lift_pt));
-    cudaStream_t s = ctx->s_main;
-    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_kpl, kp_l, N1 * 8, s));
-    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
-    CK(ctx, a.up(o_desc, desc_l, N1 * 32, s));
-    CK(ctx, a.up(o_kpr, kp_r, N2 * 8, s));
-    CK(ctx, a.up(o_m12, m12, N1 * 4, s));
-    CK(ctx, launch_lift_points(*cam, *scfg, B, a.i32(o_loff), a.f32(o_kpl), a.i32(o_oct), a.u8(o_desc), a.i32(o_roff),
-                               a.f32(o_kpr), a.i32(o_m12), arena_records(a, o_rec, PT_PL, LS_SPL), a.i32(o_cnt), s));
-    ctx->launches++;
+    const StereoSet st{false, B, l_off, r_off, nullptr, false, kp_l, kp_r, octave_l, desc_l, nullptr, true, m12};
     const RecPtrs out = RecPtrs::from(PT_PL, {pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx});
-    CK(ctx, down_records(a, out, o_rec, N1, PT_PL, LS_SPL, s));
-    return counts_total(ctx, s, B, a.i32(o_cnt), counts);
+    return stereo_lift(ctx, cam, scfg, st, out, counts);
 }
 
 int plstvo_stereo_lift_lines(PlContext* ctx, const PlCamera* cam, const PlStereoConfig* scfg, int B, const int32_t* l_off,
@@ -121,40 +202,10 @@ int plstvo_stereo_lift_lines(PlContext* ctx, const PlCamera* cam, const PlStereo
                              double* ls_sdisp, double* ls_edisp, double* ls_sP, double* ls_eP, double* ls_le,
                              double* ls_angle, double* ls_sigma2, int32_t* ls_level, uint8_t* ldesc_out, int32_t* src_idx,
                              int32_t* counts) {
-    if (!ctx) return PLSTVO_E_INVALID;
-    LOCK(ctx);
-    if (!cam || !scfg || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
-    if (B == 0) return 0;
-    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
-    const size_t N1 = l_off[B], N2 = r_off[B];
-    if (N1 && (!seg_l || !angle_l || !octave_l || !desc_l || !m12)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-    if (N2 && !seg_r) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-    CK(ctx, cudaSetDevice(ctx->device));
-    Arena a;
-    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_segl = a.take(N1 * 16);
-    const size_t o_ang = a.take(N1 * 4), o_oct = a.take(N1 * 4), o_desc = a.take(N1 * 32), o_segr = a.take(N2 * 16);
-    const size_t o_m12 = a.take(N1 * 4);
-    size_t o_rec[N_REC];
-    take_records(a, N1, LS_SPL, N_LIFT, o_rec);
-    const size_t o_cnt = a.take((size_t)B * 4);
-    CK(ctx, a.alloc(ctx->arena_lift_ls));
-    cudaStream_t s = ctx->s_main;
-    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_segl, seg_l, N1 * 16, s));
-    CK(ctx, a.up(o_ang, angle_l, N1 * 4, s));
-    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
-    CK(ctx, a.up(o_desc, desc_l, N1 * 32, s));
-    CK(ctx, a.up(o_segr, seg_r, N2 * 16, s));
-    CK(ctx, a.up(o_m12, m12, N1 * 4, s));
-    CK(ctx, launch_lift_lines(*cam, *scfg, B, a.i32(o_loff), a.f32(o_segl), a.f32(o_ang), a.i32(o_oct), a.u8(o_desc),
-                              a.i32(o_roff), a.f32(o_segr), a.i32(o_m12), arena_records(a, o_rec, LS_SPL, N_LIFT), a.i32(o_cnt),
-                              s));
-    ctx->launches++;
+    const StereoSet st{true, B, l_off, r_off, angle_l, false, seg_l, seg_r, octave_l, desc_l, nullptr, true, m12};
     const RecPtrs out = RecPtrs::from(LS_SPL, {ls_spl, ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
                                                ls_level, ldesc_out, src_idx});
-    CK(ctx, down_records(a, out, o_rec, N1, LS_SPL, N_LIFT, s));
-    return counts_total(ctx, s, B, a.i32(o_cnt), counts);
+    return stereo_lift(ctx, cam, scfg, st, out, counts);
 }
 
 // ---- matchStereoPoints / matchStereoLines in one device pass (src/stereoFrame.cpp:120-173, :309-398) ----------------
@@ -165,75 +216,36 @@ void plstvo_default_stereo_match_config(PlStereoMatchConfig* c) {   // include/s
 }
 
 namespace {
-// out: the host destinations of the kind's lifted records
-int match_stereo_common(PlContext* ctx, bool lines, const PlCamera* cam, const PlStereoMatchConfig* mc, const PlStereoConfig* sc,
-                        int B, const int32_t* l_off, const float* xy_l, const float* angle_l, const int32_t* octave_l,
-                        const uint8_t* desc_l, const int32_t* r_off, const float* xy_r, const uint8_t* desc_r, int32_t* m12,
-                        const RecPtrs& out, int32_t* counts) {
+// out: the host destinations of the set's lifted records
+int match_stereo_common(PlContext* ctx, const PlCamera* cam, const PlStereoMatchConfig* mc, const PlStereoConfig* sc,
+                        StereoSet st, int32_t* m12, const RecPtrs& out, int32_t* counts) {
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
+    const int B = st.nf;
     if (!cam || !mc || !sc || B < 0) return fail(ctx, PLSTVO_E_INVALID, "null camera / config or negative batch size");
     const int rows = mc->grid_rows, cols = mc->grid_cols;
     if (!grid_ok(rows, cols) || cam->width <= 0 || cam->height <= 0)
         return fail(ctx, PLSTVO_E_INVALID, "bad grid or image size");
     if (B == 0) return 0;
-    if (const int rc = check_stereo_offsets(ctx, B, l_off, r_off)) return rc;
-    const size_t N1 = l_off[B], N2 = r_off[B];
-    if (N1 && (!xy_l || !octave_l || !desc_l || (lines && !angle_l))) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-    if (N2 && (!xy_r || !desc_r)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
+    if (const int rc = st.check(ctx)) return rc;
     CK(ctx, cudaSetDevice(ctx->device));
-    const int cw = lines ? 4 : 2;                 // floats per feature (segment / key point) and ints per query cell record
     Arena a;
-    // raw inputs
-    const size_t o_loff = a.take((size_t)(B + 1) * 4), o_roff = a.take((size_t)(B + 1) * 4), o_xyl = a.take(N1 * cw * 4);
-    const size_t o_xyr = a.take(N2 * cw * 4), o_ang = a.take(lines ? N1 * 4 : 0), o_oct = a.take(N1 * 4);
-    const size_t o_d1 = a.take(N1 * 32), o_d2 = a.take(N2 * 32);
-    // matchGrid
-    const size_t o_m12 = a.take(N1 * 4), o_gcnt = a.take((size_t)B * 4);
-    const GridScratch g(a, rows, cols, B, N1, N2, N2 * grid_cells_per_train(lines, rows, cols), !lines, lines);
-    const size_t o_prob = a.take((size_t)B * sizeof(GridProblem));
-    // lifted records
-    const int first = lines ? LS_SPL : PT_PL, last = lines ? N_LIFT : LS_SPL;
+    st.take(a);
+    const GridScratch g(a, rows, cols, B, st.N1, st.N2, st.N2 * grid_cells_per_train(st.lines, rows, cols), !st.lines, st.lines);
+    const int first = st.lines ? LS_SPL : PT_PL, last = st.lines ? N_LIFT : LS_SPL;
     size_t o_rec[N_REC];
-    take_records(a, N1, first, last, o_rec);
-    const size_t o_cnt = a.take((size_t)B * 4);
+    take_records(a, st.N1, first, last, o_rec);
     CK(ctx, a.alloc(ctx->arena_stereo));
     std::vector<GridProblem> probs((size_t)B);
-    g.fill(probs.data(), B, lines, l_off, r_off, a.u8(o_d1), a.u8(o_d2), a.i32(o_m12), a.i32(o_gcnt));
     cudaStream_t s = ctx->s_main;
-    CK(ctx, a.up(o_loff, l_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_roff, r_off, (size_t)(B + 1) * 4, s));
-    CK(ctx, a.up(o_xyl, xy_l, N1 * cw * 4, s));
-    CK(ctx, a.up(o_xyr, xy_r, N2 * cw * 4, s));
-    if (lines) CK(ctx, a.up(o_ang, angle_l, N1 * 4, s));
-    CK(ctx, a.up(o_oct, octave_l, N1 * 4, s));
-    CK(ctx, a.up(o_d1, desc_l, N1 * 32, s));
-    CK(ctx, a.up(o_d2, desc_r, N2 * 32, s));
-    CK(ctx, a.up(o_prob, probs.data(), (size_t)B * sizeof(GridProblem), s));
-    // 1. grid coordinates (:47-48: inv_width = GRID_COLS / image width, inv_height = GRID_ROWS / image height)
-    const double inv_w = cols / static_cast<double>(cam->width), inv_h = rows / static_cast<double>(cam->height);
-    if (lines)
-        CK(ctx, launch_stereo_cells_lines((int)N1, (int)N2, inv_w, inv_h, a.f32(o_xyl), a.f32(o_xyr), a.i32(g.qcell),
-                                          a.f64(g.tline), a.f64(g.tdir), s));
-    else
-        CK(ctx, launch_stereo_cells_points((int)N1, (int)N2, inv_w, inv_h, a.f32(o_xyl), a.f32(o_xyr), a.i32(g.qcell),
-                                           a.i32(g.tcell), s));
-    // 2. matchGrid with the stereo window (:141-143, :340-342: matching_s_ws cells to the left, same row)
-    GridParams prm{rows, cols, GRID_CAP, mc->best_lr_matches ? 1 : 0, PlGridWindow{mc->matching_s_ws, 0, 0, 0},
-                   mc->min_ratio_12_p, mc->line_sim_th};
-    CK(ctx, launch_match_grid(a.at<GridProblem>(o_prob), B, prm, lines, s));
-    // 3. lifting, reading the match list where matchGrid left it
-    const RecPtrs rec = arena_records(a, o_rec, first, last);
-    if (lines)
-        CK(ctx, launch_lift_lines(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.f32(o_ang), a.i32(o_oct), a.u8(o_d1),
-                                  a.i32(o_roff), a.f32(o_xyr), a.i32(o_m12), rec, a.i32(o_cnt), s));
-    else
-        CK(ctx, launch_lift_points(*cam, *sc, B, a.i32(o_loff), a.f32(o_xyl), a.i32(o_oct), a.u8(o_d1), a.i32(o_roff),
-                                   a.f32(o_xyr), a.i32(o_m12), rec, a.i32(o_cnt), s));
+    CK(ctx, st.upload(a, s, &g, probs.data()));
+    CK(ctx, st.match(a, g, *cam, *mc, s));
+    // lifting, reading the match list where matchGrid left it
+    CK(ctx, st.lift(a, *cam, *sc, B, 0, arena_records(a, o_rec, first, last), s));
     ctx->launches += 3;
-    CK(ctx, a.down(m12, o_m12, N1 * 4, s));
-    CK(ctx, down_records(a, out, o_rec, N1, first, last, s));
-    return counts_total(ctx, s, B, a.i32(o_cnt), counts, a.i32(o_gcnt));
+    CK(ctx, a.down(m12, st.o_m12, st.N1 * 4, s));
+    CK(ctx, down_records(a, out, o_rec, st.N1, first, last, s));
+    return counts_total(ctx, s, B, a.i32(st.o_cnt), counts, a.i32(st.o_gcnt));
 }
 }  // namespace
 
@@ -243,8 +255,8 @@ int plstvo_match_stereo_points(PlContext* ctx, const PlCamera* cam, const PlSter
                                double* pt_disp, double* pt_P, double* pt_sigma2, int32_t* pt_level, uint8_t* pdesc_out,
                                int32_t* src_idx, int32_t* counts) {
     const RecPtrs out = RecPtrs::from(PT_PL, {pt_pl, pt_disp, pt_P, pt_sigma2, pt_level, pdesc_out, src_idx});
-    return match_stereo_common(ctx, false, cam, mcfg, scfg, B, l_off, kp_l, nullptr, octave_l, desc_l, r_off, kp_r, desc_r, m12,
-                               out, counts);
+    const StereoSet st{false, B, l_off, r_off, nullptr, false, kp_l, kp_r, octave_l, desc_l, desc_r};
+    return match_stereo_common(ctx, cam, mcfg, scfg, st, m12, out, counts);
 }
 
 int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStereoMatchConfig* mcfg, const PlStereoConfig* scfg,
@@ -255,8 +267,8 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
                               uint8_t* ldesc_out, int32_t* src_idx, int32_t* counts) {
     const RecPtrs out = RecPtrs::from(LS_SPL, {ls_spl, ls_epl, ls_sdisp, ls_edisp, ls_sP, ls_eP, ls_le, ls_angle, ls_sigma2,
                                                ls_level, ldesc_out, src_idx});
-    return match_stereo_common(ctx, true, cam, mcfg, scfg, B, l_off, seg_l, angle_l, octave_l, desc_l, r_off, seg_r, desc_r, m12,
-                               out, counts);
+    const StereoSet st{true, B, l_off, r_off, angle_l, false, seg_l, seg_r, octave_l, desc_l, desc_r};
+    return match_stereo_common(ctx, cam, mcfg, scfg, st, m12, out, counts);
 }
 
 }  // extern "C"
@@ -270,9 +282,9 @@ int plstvo_match_stereo_lines(PlContext* ctx, const PlCamera* cam, const PlStere
 //                    and in the previous-frame role into the session's next pool.  The streams' kept frames are gathered into
 //                    the workspace's previous-frame arrays (insert; initialize tracks nothing and takes no results).
 int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
-                                const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
-                                const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                                const StereoDevInputs* dev, SessionCall* call) {
+                                const PlStereoConfig* sc, const StereoSet* prev, const StereoSet* curr, const PlPrior* priors,
+                                PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot, const StereoDevInputs* dev,
+                                SessionCall* call) {
     // slot < 0: blocking (returns with the results in host memory); slot 0 / 1: enqueue only, results valid after plstvo_wait
     if (!ctx) return PLSTVO_E_INVALID;
     LOCK(ctx);
@@ -280,9 +292,9 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     const bool track = !call || call->track;
     if (!cam || !cfg || !mc || !sc || !prev || (!one_set && !curr) || (track && !results))
         return fail(ctx, PLSTVO_E_INVALID, "null argument");
-    const int NF = prev->B;                         // frames per feature set
+    const int NF = prev[0].nf;                      // frames per feature set
     const int B = sequence ? NF - 1 : NF;           // pairs
-    if (NF < 0 || (!one_set && curr->B != NF)) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
+    if (NF < 0 || (!one_set && curr[0].nf != NF)) return fail(ctx, PLSTVO_E_SIZE, "prev and curr hold different numbers of frames");
     if (sequence && NF == 1) return 0;              // one frame: nothing to track
     const int rows = mc->grid_rows, cols = mc->grid_cols;
     if (!grid_ok(rows, cols) || cam->width <= 0 || cam->height <= 0)
@@ -291,45 +303,15 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     CK(ctx, cudaSetDevice(ctx->device));
     const int NSETS = one_set ? 2 : 4;
     if (one_set) curr = prev;                       // sets 2, 3 below are unused
-    // the four feature sets: {prev, curr} x {points, lines}
-    struct Set {
-        bool lines; const int32_t *l_off, *r_off; const float *xy_l, *xy_r, *ang; const int32_t* oct; const uint8_t *d1, *d2;
-        size_t N1, N2, o_loff, o_roff, o_xyl, o_xyr, o_ang, o_oct, o_d1, o_d2, o_m12, o_cnt, o_gcnt, o_ooff, o_ooff2, o_prob;
-        bool on_device;
-        const float *g_xyl, *g_xyr; const int32_t* g_oct; const uint8_t *g_d1, *g_d2;   // where the kernels read the inputs
-    };
-    Set sets[4] = {
-        {false, prev->pl_off, prev->pr_off, prev->kp_l, prev->kp_r, nullptr, prev->poct_l, prev->pdesc_l, prev->pdesc_r},
-        {true, prev->ll_off, prev->lr_off, prev->seg_l, prev->seg_r, prev->angle_l, prev->loct_l, prev->ldesc_l, prev->ldesc_r},
-        {false, curr->pl_off, curr->pr_off, curr->kp_l, curr->kp_r, nullptr, curr->poct_l, curr->pdesc_l, curr->pdesc_r},
-        {true, curr->ll_off, curr->lr_off, curr->seg_l, curr->seg_r, curr->angle_l, curr->loct_l, curr->ldesc_l, curr->ldesc_r}};
-    if (dev)
-        for (int k = 0; k < NSETS; ++k)
-            if (dev->set[k].on_device) {
-                const StereoDevInputs::Set& d = dev->set[k];
-                Set& st = sets[k];
-                st.xy_l = d.xy_l; st.xy_r = d.xy_r; st.oct = d.oct; st.d1 = d.d1; st.d2 = d.d2;
-            }
+    StereoSet sets[4] = {prev[0], prev[1], curr[0], curr[1]};   // {prev, curr} x {points, lines}
     Arena a;
-    size_t maxN1 = 0, maxN2 = 0, max_items = 0;
+    size_t maxN1 = 0, maxN2 = 0, max_items = 0, o_ooff[4], o_ooff2[4];
     for (int k = 0; k < NSETS; ++k) {
-        Set& st = sets[k];
-        st.on_device = dev && dev->set[k].on_device;
-        if (const int rc = check_stereo_offsets(ctx, NF, st.l_off, st.r_off)) return rc;
-        st.N1 = st.l_off[NF];
-        st.N2 = st.r_off[NF];
-        if (st.N1 && (!st.xy_l || (!st.oct && !st.on_device) || !st.d1 || (st.lines && !st.ang)))
-            return fail(ctx, PLSTVO_E_INVALID, "null input array");
-        if (st.N2 && (!st.xy_r || !st.d2)) return fail(ctx, PLSTVO_E_INVALID, "null input array");
-        const int cw = st.lines ? 4 : 2;
-        const size_t host = st.on_device ? 0 : 1;   // device-resident inputs take no arena space (but zero octaves do)
-        st.o_loff = a.take((size_t)(NF + 1) * 4); st.o_roff = a.take((size_t)(NF + 1) * 4);
-        st.o_xyl = a.take(host * st.N1 * cw * 4); st.o_xyr = a.take(host * st.N2 * cw * 4); st.o_ang = a.take(st.lines ? st.N1 * 4 : 0);
-        st.o_oct = a.take(st.on_device && st.oct ? 0 : st.N1 * 4); st.o_d1 = a.take(host * st.N1 * 32);
-        st.o_d2 = a.take(host * st.N2 * 32); st.o_m12 = a.take(st.N1 * 4);
-        st.o_cnt = a.take((size_t)NF * 4); st.o_gcnt = a.take((size_t)NF * 4); st.o_ooff = a.take((size_t)(NF + 1) * 4);
-        st.o_ooff2 = a.take((size_t)(NF + 1) * 4);
-        st.o_prob = a.take((size_t)NF * sizeof(GridProblem));
+        StereoSet& st = sets[k];
+        if (const int rc = st.check(ctx)) return rc;
+        st.take(a);
+        o_ooff[k] = a.take((size_t)(NF + 1) * 4);
+        o_ooff2[k] = a.take((size_t)(NF + 1) * 4);
         maxN1 = std::max(maxN1, st.N1);
         maxN2 = std::max(maxN2, st.N2);
         max_items = std::max(max_items, st.N2 * grid_cells_per_train(st.lines, rows, cols));
@@ -337,29 +319,8 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     // matchGrid scratch, shared by the four sets (they run one after the other on one stream)
     const GridScratch g(a, rows, cols, NF, maxN1, maxN2, max_items, true, true);
     CK(ctx, a.alloc(ctx->arena_track_stereo[slot + 1]));
-    for (int k = 0; k < NSETS; ++k) {
-        Set& st = sets[k];
-        st.g_xyl = st.on_device ? st.xy_l : a.f32(st.o_xyl);
-        st.g_xyr = st.on_device ? st.xy_r : a.f32(st.o_xyr);
-        st.g_oct = st.on_device && st.oct ? st.oct : a.i32(st.o_oct);
-        st.g_d1 = st.on_device ? st.d1 : a.u8(st.o_d1);
-        st.g_d2 = st.on_device ? st.d2 : a.u8(st.o_d2);
-    }
     cudaStream_t s = ctx->s_main, sh = ctx->s_h2d;   // uploads of set k + 1 run under the kernels of set k
     // (this slot's arena is free: a blocking call ends synchronised, an async slot is reused only after its event completed)
-    // the lifting of frames [first, first + nf) of a set into o's entries of its kind (all null: counts only), at out_off
-    auto lift = [&](const Set& st, int nf, int first, const RecPtrs& o, const int32_t* out_off,
-                    const PlCamera* cams) -> cudaError_t {
-        if (st.lines)
-            return launch_lift_lines(*cam, *sc, nf, a.i32(st.o_loff) + first, st.g_xyl, a.f32(st.o_ang), st.g_oct, st.g_d1,
-                                     a.i32(st.o_roff) + first, st.g_xyr, a.i32(st.o_m12), o, a.i32(st.o_cnt) + first, s,
-                                     out_off, cams);
-        return launch_lift_points(*cam, *sc, nf, a.i32(st.o_loff) + first, st.g_xyl, st.g_oct, st.g_d1, a.i32(st.o_roff) + first,
-                                  st.g_xyr, a.i32(st.o_m12), o, a.i32(st.o_cnt) + first, s, out_off, cams);
-    };
-    const double inv_w = cols / static_cast<double>(cam->width), inv_h = rows / static_cast<double>(cam->height);
-    const GridParams gprm{rows, cols, GRID_CAP, mc->best_lr_matches ? 1 : 0, PlGridWindow{mc->matching_s_ws, 0, 0, 0},
-                          mc->min_ratio_12_p, mc->line_sim_th};
     // pinned staging: 4 problem tables + 2 x 4 x B counters (pageable copies would block this thread on the stream)
     const size_t prob_bytes = ((size_t)NF * sizeof(GridProblem) + 255) / 256 * 256;
     PinnedBuf& staging = ctx->h_staging[slot + 1];
@@ -371,23 +332,8 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     bool joined = false;
     // ---- pass 1: cells -> matchGrid -> lifting filters (count only) per set ----
     for (int k = 0; k < NSETS; ++k) {
-        Set& st = sets[k];
-        const int cw = st.lines ? 4 : 2;
-        GridProblem* probs = reinterpret_cast<GridProblem*>(hst + (size_t)k * prob_bytes);
-        g.fill(probs, NF, st.lines, st.l_off, st.r_off, st.g_d1, st.g_d2, a.i32(st.o_m12), a.i32(st.o_gcnt));
-        CK(ctx, a.up(st.o_loff, st.l_off, (size_t)(NF + 1) * 4, sh));
-        CK(ctx, a.up(st.o_roff, st.r_off, (size_t)(NF + 1) * 4, sh));
-        if (st.lines) CK(ctx, a.up(st.o_ang, st.ang, st.N1 * 4, sh));
-        if (!st.on_device) {
-            CK(ctx, a.up(st.o_xyl, st.xy_l, st.N1 * cw * 4, sh));
-            CK(ctx, a.up(st.o_xyr, st.xy_r, st.N2 * cw * 4, sh));
-            CK(ctx, a.up(st.o_oct, st.oct, st.N1 * 4, sh));
-            CK(ctx, a.up(st.o_d1, st.d1, st.N1 * 32, sh));
-            CK(ctx, a.up(st.o_d2, st.d2, st.N2 * 32, sh));
-        } else if (!st.oct && st.N1) {
-            CK(ctx, cudaMemsetAsync(a.u8(st.o_oct), 0, st.N1 * 4, sh));   // key lines of octave 0
-        }
-        CK(ctx, a.up(st.o_prob, probs, (size_t)NF * sizeof(GridProblem), sh));
+        const StereoSet& st = sets[k];
+        CK(ctx, st.upload(a, sh, &g, reinterpret_cast<GridProblem*>(hst + (size_t)k * prob_bytes)));
         cudaEvent_t uploaded = next_event(ctx);
         CK(ctx, cudaEventRecord(uploaded, sh));
         CK(ctx, cudaStreamWaitEvent(s, uploaded, 0));
@@ -395,14 +341,8 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             CK(ctx, cudaStreamWaitEvent(s, dev->lines_ready, 0));
             joined = true;
         }
-        if (st.lines)
-            CK(ctx, launch_stereo_cells_lines((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
-                                              a.f64(g.tline), a.f64(g.tdir), s));
-        else
-            CK(ctx, launch_stereo_cells_points((int)st.N1, (int)st.N2, inv_w, inv_h, st.g_xyl, st.g_xyr, a.i32(g.qcell),
-                                               a.i32(g.tcell), s));
-        CK(ctx, launch_match_grid(a.at<GridProblem>(st.o_prob), NF, gprm, st.lines, s));
-        CK(ctx, lift(st, NF, 0, RecPtrs{}, nullptr, nullptr));
+        CK(ctx, st.match(a, g, *cam, *mc, s));
+        CK(ctx, st.lift(a, *cam, *sc, NF, 0, RecPtrs{}, s));
         ctx->launches += 3;
         CK(ctx, cudaMemcpyAsync(cnt + (size_t)k * NF, a.u8(st.o_cnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
         CK(ctx, cudaMemcpyAsync(gcnt + (size_t)k * NF, a.u8(st.o_gcnt), (size_t)NF * 4, cudaMemcpyDeviceToHost, s));
@@ -425,11 +365,11 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
                 }
             }
         }
-        CK(ctx, a.up(sets[k].o_ooff, ooff[k].data(), (size_t)(NF + 1) * 4, sh));
+        CK(ctx, a.up(o_ooff[k], ooff[k].data(), (size_t)(NF + 1) * 4, sh));
         if (sequence) {
             ooff2[k].assign((size_t)NF, 0);          // frames 1 .. NF - 1 as current frames: offsets relative to frame 1
             for (int p = 0; p < NF; ++p) ooff2[k][p] = ooff[k][p + 1] - ooff[k][1];
-            CK(ctx, a.up(sets[k].o_ooff2, ooff2[k].data(), (size_t)NF * 4, sh));
+            CK(ctx, a.up(o_ooff2[k], ooff2[k].data(), (size_t)NF * 4, sh));
         }
     }
     // a cams session: the camera of each new frame (its stream's), for pass 2's lifts and for the solver (pair p = frame p)
@@ -448,17 +388,17 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     if (call) {
         if (const int rc = session_plan(ctx, *call, cnt, cnt + NF, s)) return rc;
         for (int k = 0; k < 2; ++k)
-            CK(ctx, lift(sets[k], B, 0, ss->pool[ss->cur ^ 1].rows, session_out_off(*call, k == 1), d_cams));
+            CK(ctx, sets[k].lift(a, *cam, *sc, B, 0, ss->pool[ss->cur ^ 1].rows, s, session_out_off(*call, k == 1), d_cams));
         ctx->launches += 2;
         if (const int rc = session_gather_others(ctx, *call, s)) return rc;
         if (call->retain) {   // plstvo_stereo_session_read: every record of the new frames, compact in call order
             SessionRetained& kr = ss->kept;
             CK(ctx, kr.lay_out((size_t)ooff[0][NF], (size_t)ooff[1][NF], track ? (size_t)call->kept_off_pt[NF] : 0,
                                track ? (size_t)call->kept_off_ls[NF] : 0));
-            cudaEvent_t offsets_up = next_event(ctx);   // sets[k].o_ooff, uploaded on sh above
+            cudaEvent_t offsets_up = next_event(ctx);   // o_ooff, uploaded on sh above
             CK(ctx, cudaEventRecord(offsets_up, sh));
             CK(ctx, cudaStreamWaitEvent(s, offsets_up, 0));
-            for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], NF, 0, kr.rec, a.i32(sets[k].o_ooff), d_cams));
+            for (int k = 0; k < 2; ++k) CK(ctx, sets[k].lift(a, *cam, *sc, NF, 0, kr.rec, s, a.i32(o_ooff[k]), d_cams));
             ctx->launches += 2;
         }
         if (!track) {
@@ -489,13 +429,14 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     if (call) {
         if (const int rc2 = session_gather_named(ctx, *call, ws.prev.rows(PREV_ROLE), s)) return rc2;
     } else {
-        for (int k = 0; k < 2; ++k) CK(ctx, lift(sets[k], B, 0, ws.prev.rows(PREV_ROLE), a.i32(sets[k].o_ooff), d_cams));
+        for (int k = 0; k < 2; ++k)
+            CK(ctx, sets[k].lift(a, *cam, *sc, B, 0, ws.prev.rows(PREV_ROLE), s, a.i32(o_ooff[k]), d_cams));
     }
     // the current-frame role: the set's frames from `first` on (sequence mode: the second frame)
     const int first = sequence ? 1 : 0;
     for (int k = 0; k < 2; ++k) {
-        const Set& st = sets[one_set ? k : 2 + k];
-        CK(ctx, lift(st, B, first, ws.curr.rows(CURR_ROLE), a.i32(sequence ? st.o_ooff2 : st.o_ooff), d_cams));
+        const int j = one_set ? k : 2 + k;
+        CK(ctx, sets[j].lift(a, *cam, *sc, B, first, ws.curr.rows(CURR_ROLE), s, a.i32(sequence ? o_ooff2[j] : o_ooff[j]), d_cams));
     }
     ctx->launches += call ? 2 : 4;
     if (dev && dev->marks) CK(ctx, cudaEventRecord(dev->marks[1], s));
@@ -517,6 +458,16 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
     return 0;
 }
 
+namespace {
+// the point set and the line set of f's frames into fs[0], fs[1] (null for a null f)
+const StereoSet* feature_sets(const PlStereoFeatures* f, StereoSet* fs) {
+    if (!f) return nullptr;
+    fs[0] = StereoSet{false, f->B, f->pl_off, f->pr_off, nullptr, false, f->kp_l, f->kp_r, f->poct_l, f->pdesc_l, f->pdesc_r};
+    fs[1] = StereoSet{true, f->B, f->ll_off, f->lr_off, f->angle_l, false, f->seg_l, f->seg_r, f->loct_l, f->ldesc_l, f->ldesc_r};
+    return fs;
+}
+}  // namespace
+
 extern "C" {
 
 // ticket bookkeeping shared with plstvo_track_batch_async: two slots, plstvo_wait(ticket) blocks until the slot's results are home
@@ -528,7 +479,9 @@ static int stereo_async(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg
     CK(ctx, cudaSetDevice(ctx->device));
     const int slot = acquire_slot(ctx);
     if (slot < 0) return slot;
-    const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, a, b, priors, results, n_stereo, sequence, slot);
+    StereoSet sa[2], sb[2];
+    const int rc = track_stereo_common(ctx, cam, cfg, mc, sc, feature_sets(a, sa), feature_sets(b, sb), priors, results, n_stereo,
+                                       sequence, slot);
     if (rc) return rc;
     CK(ctx, cudaEventRecord(ctx->slot_done[slot], ctx->s_main));
     ctx->slot_busy[slot] = true;
@@ -550,13 +503,16 @@ int plstvo_track_stereo_sequence_async(PlContext* ctx, const PlCamera* cam, cons
 int plstvo_track_stereo_batch(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                               const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
                               const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo) {
-    return track_stereo_common(ctx, cam, cfg, mc, sc, prev, curr, priors, results, n_stereo, false, -1);
+    StereoSet p[2], c[2];
+    return track_stereo_common(ctx, cam, cfg, mc, sc, feature_sets(prev, p), feature_sets(curr, c), priors, results, n_stereo,
+                               false, -1);
 }
 
 int plstvo_track_stereo_sequence(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
                                  const PlStereoConfig* sc, const PlStereoFeatures* frames, const PlPrior* priors,
                                  PlPoseResult* results, int32_t* n_stereo) {
-    return track_stereo_common(ctx, cam, cfg, mc, sc, frames, nullptr, priors, results, n_stereo, true, -1);
+    StereoSet f[2];
+    return track_stereo_common(ctx, cam, cfg, mc, sc, feature_sets(frames, f), nullptr, priors, results, n_stereo, true, -1);
 }
 
 }  // extern "C"

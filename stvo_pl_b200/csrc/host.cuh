@@ -538,25 +538,59 @@ cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPose
 cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
                                     PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s);
 
-// ---- capi_stereo.cu: raw stereo features -> pose, composed by the images path ----
-// Feature data of the four sets that is already in HBM (the images path: ORB's and LBD's outputs, written on s_main / on the
-// stream `lines_ready` was recorded on).  A set with on_device reads xy_l, xy_r, oct, d1, d2 from here instead of uploading
-// the PlStereoFeatures arrays (oct null: all octaves 0); offsets and line angles still come from the host struct.
+// ---- capi_stereo.cu: the stereo step's feature sets, and raw stereo features -> pose, composed by the images path ----
+// One feature set: one kind of feature (points or lines) of nf frames.  Offsets and left line angles are host arrays; xy_l,
+// xy_r (key points or segments), oct and d1, d2 (descriptors) are host arrays, or with on_device HBM (the images path: ORB's
+// and LBD's outputs), where a null oct is octave 0 everywhere.  Stand-alone lifting (lift_only) reads the caller's m12 (host)
+// in place of matchGrid's and has no d2.  check() sets N1, N2; take() lays out the set's slices, which the other members read.
+struct StereoSet {
+    bool lines = false;
+    int nf = 0;
+    const int32_t *l_off = nullptr, *r_off = nullptr;
+    const float* ang = nullptr;
+    bool on_device = false;
+    const float *xy_l = nullptr, *xy_r = nullptr;
+    const int32_t* oct = nullptr;
+    const uint8_t *d1 = nullptr, *d2 = nullptr;
+    bool lift_only = false;
+    const int32_t* m12 = nullptr;
+    size_t N1 = 0, N2 = 0;
+    size_t o_loff = 0, o_roff = 0, o_xyl = 0, o_xyr = 0, o_ang = 0, o_oct = 0, o_d1 = 0, o_d2 = 0, o_m12 = 0, o_cnt = 0,
+           o_gcnt = 0, o_prob = 0;
+
+    // the offsets and the arrays a non-empty side needs
+    int check(PlContext* ctx);
+    // offsets, host-resident inputs (and zero octaves), m12, lifting's counts and, unless lift_only, matchGrid's counts and
+    // problem table
+    void take(Arena& a);
+    // the host arrays on s, then (g given) the set's GridProblem table, filled at probs, for matchGrid's scratch g
+    cudaError_t upload(const Arena& a, cudaStream_t s, const GridScratch* g = nullptr, GridProblem* probs = nullptr) const;
+    // grid cells of the key points / segments, then matchGrid with the stereo window, on s
+    cudaError_t match(const Arena& a, const GridScratch& g, const PlCamera& cam, const PlStereoMatchConfig& mc,
+                      cudaStream_t s) const;
+    // the lifting of frames [first, first + n) into out's entries of the set's kind (all null: counts only), at out_off
+    // (else the left offsets), with the device camera of each frame (cams) or cam
+    cudaError_t lift(const Arena& a, const PlCamera& cam, const PlStereoConfig& sc, int n, int first, const RecPtrs& out,
+                     cudaStream_t s, const int32_t* out_off = nullptr, const PlCamera* cams = nullptr) const;
+    // where the kernels read input p: HBM when it is there, else its slice o
+    template <typename T> const T* in(const Arena& a, const T* p, size_t o) const {
+        return on_device && p ? p : a.at<const T>(o);
+    }
+};
+
+// What a tracking call adds to its feature sets.
 struct StereoDevInputs {
-    struct Set {
-        bool on_device = false;
-        const float *xy_l = nullptr, *xy_r = nullptr; const int32_t* oct = nullptr; const uint8_t *d1 = nullptr, *d2 = nullptr;
-    } set[4];
-    cudaEvent_t lines_ready = nullptr;   // waited on before the first line set's stereo step
+    cudaEvent_t lines_ready = nullptr;   // waited on before the first line set's stereo step (LBD's stream, on the device)
     cudaEvent_t* marks = nullptr;        // [3] timing events: stereo step start, its end, tracking end (all on s_main)
     bool priors_resident = false;        // the workspace's d_priors already holds this call's priors (a session run's steps)
     // set: called on s_main once the solver is enqueued, in place of the results' download (results are then not written)
     std::function<int(const Workspace&)> tracked;
 };
+// prev, curr: [2] the point set and the line set of the previous and the current frames (curr unused with sequence or call)
 int track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlConfig* cfg, const PlStereoMatchConfig* mc,
-                        const PlStereoConfig* sc, const PlStereoFeatures* prev, const PlStereoFeatures* curr,
-                        const PlPrior* priors, PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot,
-                        const StereoDevInputs* dev = nullptr, SessionCall* call = nullptr);
+                        const PlStereoConfig* sc, const StereoSet* prev, const StereoSet* curr, const PlPrior* priors,
+                        PlPoseResult* results, int32_t* n_stereo, bool sequence, int slot, const StereoDevInputs* dev = nullptr,
+                        SessionCall* call = nullptr);
 
 // ---- rectify.cu: rectifyImagesLR on the device, composed by the raw-images path ----
 struct ImgPart {   // consecutive host images of one size
