@@ -766,6 +766,61 @@ int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* s, cons
                                         PlKeyframeState* kf_state /* [n] in / out */, PlPoseResult* results /* [T][n] */,
                                         PlKeyframeResult* kf /* [T][n] */, int32_t* fast_th /* [T + 1][n] or NULL */,
                                         int32_t* n_stereo /* [T][n][4] or NULL */);
+/* ---- the frame loop over uneven streams: a per-step, per-stream schedule (app/imagesStVO.cpp:88-124 per camera) ----
+ * _run and _run_keyframes where a stream may have no frame at a step, start inside the call, or be re-initialised:
+ * schedule [T][n] holds, for stream ids[k] at step t,
+ *   0  no frame: the stream idles, its kept frame, threshold, prior and key-frame state carried unchanged;
+ *   1  insert: insertStereoPair + optimizePose (+ needNewKF / currFrameIsKF with k) + updateFrame, as _run's step;
+ *   2  initialize: StereoFrameHandler::initialize on this frame (src/stereoFrameHandler.cpp:35-52).
+ * frames holds B = the number of non-zero entries, step-major and within a step in ids order (FLD sessions: the key-line
+ * fields in the same order).  frames->fast_th is NULL or [B]: an initialize entry's threshold as _initialize takes it (0:
+ * ocfg->fast_threshold, Config::orbFastTh as HandlerState's initialize starts from), and 0 for every insert entry.
+ * k == NULL: no key-frame test, and kf_state and kf must be NULL; else the test of _run_keyframes, kf_state [n] in / out.
+ * Contract: the call equals, byte for byte, this chain on the same session.  For t = 0 .. T - 1, one
+ * plstvo_stereo_session_initialize on step t's code-2 entries (in ids order, at their thresholds), then one
+ * plstvo_stereo_session_insert on its code-1 entries; a chain call with no entries is not made.  Per stream, the insert
+ * takes the threshold and prior _run / _run_keyframes would carry to it (th_0 = fast_th0 as _run maps it, priors [n] or
+ * NULL at the call's start), and the key-frame state from kf_state; an idle step carries all three unchanged; an
+ * initialize resets them to what HandlerState's initialize leaves: the entry's threshold, priorOf of the fresh frame (Tfw = I,
+ * Tfw_cov = I, DT = I, DT_cov = 0, err_norm = -1) and plstvo_initial_keyframe_state.  priors NULL starts every stream from
+ * that fresh prior too, which optimizePose treats as insert's NULL (err_norm < 0 fails isGoodSolution).
+ * Under it: results [T][n] and kf [T][n] are written for code-1 entries only (other rows untouched); n_stereo [T][n][4]
+ * is insert's row for a code-1 entry and {0, 0, points, lines} for a code-2 entry (idle rows untouched); fast_th [T + 1][n]
+ * row t holds the threshold each stream's frame of step t was detected with, and for an idle stream its carried threshold
+ * (the one its next insert would take); row T the carried thresholds after the call, as in _run; kf_state comes back as the chain's test stands after step T - 1; the
+ * kept frames, what plstvo_stereo_session_read returns (the last step with any entry, as its last chain call retains it:
+ * the insert when the step has both kinds) and with k what plstvo_stereo_session_read_keyframes returns (rows' step is the
+ * step t) are the chain's.  Every entry 1 is the existing run: the outputs equal _run (k NULL) and _run_keyframes (k set).
+ * T = 0, or no non-zero entry, runs nothing: fast_th's rows are all row 0 and what _read returns is left as _run leaves it
+ * (k set: no key frames kept, as _run_keyframes).  A second call continues a first exactly as _run_keyframes states it.
+ * Work: the 2 B present images go up once and are rectified / converted per group (each group's streams' rectifiers) into
+ * one device copy; LSD (or the FLD cut of the caller's lines) and LBD run once over all of them, one line block per image.
+ * Then each step with entries runs its initialize group (ORB at the host thresholds, the stereo step, the session's
+ * commit), then its insert group (ORB at thresholds gathered on the device, the stereo step, tracking and the handler update),
+ * each group as _initialize / _insert would, so a step with both kinds costs two groups' host hops (ORB's key-point counts,
+ * the stereo step's survivor counts, and the initialize group's final synchronise) instead of one.  A step with no entries
+ * costs nothing.  The threshold, prior and key-frame state of each named stream stay in a device slot for the whole call:
+ * session_schedule_gather_kernel reads an insert group's from the slots before its ORB, and session_schedule_update_kernel
+ * writes them back after its test (or resets an initialize group's); idle slots are not touched.  Moves and integer
+ * writes only; the arithmetic stays in session_handler_kernel and session_keyframe_kernel.
+ * Device memory besides the session's pools: _run's, with B present frames for T n, plus the slots (n thresholds, priors
+ * and key-frame states), a [T + 1][n] threshold table and the largest insert group's threshold rows and states.  With a
+ * rectifier each group's images pass the rectifier's staging, then are copied into the call's grey copy (twice with the
+ * colour FLD branch's RGB2GRAY plane).  plstvo_track_stereo_images_stage_times then covers the whole call as for _run: [0]
+ * uploads and preparation, [1] ORB summed over the groups, [2] LSD + LBD, [3] the stereo step summed, [4] tracking and the
+ * state updates summed.
+ * Checks before any work, each leaving the session and context usable: every check of _run (k NULL) or _run_keyframes (k
+ * set), with the image limit counting the present images only (2 B > 65535), plus PLSTVO_E_INVALID for a schedule value
+ * outside {0, 1, 2}, a NULL schedule with T n > 0, kf_state or kf non-NULL with k NULL, a code-1 entry for a stream that
+ * holds no frame at that step (it held one at the call's start or had an earlier code-2 entry in the call), a non-zero
+ * frames->fast_th of a code-1 entry and an initialize threshold outside [0, 255]; PLSTVO_E_SIZE for frames->B != the
+ * number of non-zero entries.  A failure part-way follows _run's rule. */
+int plstvo_stereo_session_run_schedule(PlContext* ctx, PlStereoSession* s, const PlHandlerConfig* h, const PlKeyframeConfig* k,
+                                       int n, const int32_t* ids, int T, const uint8_t* schedule /* [T][n] */,
+                                       const PlStereoImages* frames, const int32_t* fast_th0 /* [n] or NULL */,
+                                       const PlPrior* priors /* [n] or NULL */, PlKeyframeState* kf_state /* [n] or NULL */,
+                                       PlPoseResult* results /* [T][n] */, PlKeyframeResult* kf /* [T][n] or NULL */,
+                                       int32_t* fast_th /* [T + 1][n] or NULL */, int32_t* n_stereo /* [T][n][4] or NULL */);
 /* Copies the key frames the last plstvo_stereo_session_run_keyframes kept into out's non-NULL point and line arrays, in
  * (step, call position) order, key frame j's rows after key frame j - 1's (m12_* / inlier_* are not read), and writes
  * rows [n_kf][4]: step, stream id, stereo points, stereo lines (rows may be NULL to learn n_kf).  Returns n_kf.

@@ -933,6 +933,15 @@ public:
         c_.check(plstvo_stereo_session_run_keyframes(c_.get(), s_, &h, &k, n, ids, T, &frames, fast_th0, priors, kf_state,
                                                      results, kf, fast_th, n_stereo));
     }
+    // plstvo_stereo_session_run_schedule: run() / runKeyframes() over uneven streams; schedule [T][n] (0 idle, 1 insert,
+    // 2 initialize), frames one per non-zero entry step-major; k null runs no key-frame test (kf_state, kf null)
+    void runSchedule(const PlHandlerConfig& h, const PlKeyframeConfig* k, int n, const int32_t* ids, int T,
+                     const uint8_t* schedule, const PlStereoImages& frames, const int32_t* fast_th0, const PlPrior* priors,
+                     PlKeyframeState* kf_state, PlPoseResult* results, PlKeyframeResult* kf = nullptr,
+                     int32_t* fast_th = nullptr, int32_t* n_stereo = nullptr) {
+        c_.check(plstvo_stereo_session_run_schedule(c_.get(), s_, &h, k, n, ids, T, schedule, &frames, fast_th0, priors, kf_state,
+                                                    results, kf, fast_th, n_stereo));
+    }
     // plstvo_stereo_session_use_fld_lines: the reference's FLD line branch, before any stream is initialised.  On, every call
     // takes each frame's key lines in frames' key-line fields (fldKeyLines' rows; step-major for run / runKeyframes) and
     // LSD does not run.
@@ -1336,7 +1345,135 @@ public:
         return kf;
     }
 
+    // Uneven streams in one session call (plstvo_stereo_session_run_schedule): schedule[t][k] is 0 when stream ids[k] has no
+    // frame at step t, 1 for insertStereoPairs, 2 for initialize (at orb_fast_th, as initialize() above); img_l[t] / img_r[t]
+    // hold step t's frames of its non-zero entries in ids order.  Each stream then stands as after the per-frame initialize /
+    // insertStereoPairs + optimizePose (+ needNewKF / currFrameIsKF with kf) + updateFrame calls of its entries, and a
+    // stream with no entry is untouched.  results (optional) receives [T][n] results (rows of non-insert entries zero);
+    // kf non-null runs the key-frame test and receives its [T][n] tests.  keepFeatures' arrays hold the last step's last
+    // group (its inserts, or its initialised frames).
+    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<uint8_t>>& schedule,
+                               const std::vector<std::vector<const uint8_t*>>& img_l,
+                               const std::vector<std::vector<const uint8_t*>>& img_r,
+                               std::vector<PlPoseResult>* results = nullptr, std::vector<PlKeyframeResult>* kf = nullptr) {
+        runSchedule(ids, schedule, img_l, img_r, nullptr, nullptr, results, kf);
+    }
+    // the same on the FLD branch: seg_l[t][j] / seg_r[t][j] are the segments of img_l[t][j] / img_r[t][j]
+    void insertStereoSequences(const std::vector<int32_t>& ids, const std::vector<std::vector<uint8_t>>& schedule,
+                               const std::vector<std::vector<const uint8_t*>>& img_l,
+                               const std::vector<std::vector<const uint8_t*>>& img_r,
+                               const std::vector<std::vector<Segments>>& seg_l, const std::vector<std::vector<Segments>>& seg_r,
+                               std::vector<PlPoseResult>* results = nullptr, std::vector<PlKeyframeResult>* kf = nullptr) {
+        runSchedule(ids, schedule, img_l, img_r, &seg_l, &seg_r, results, kf);
+    }
+
 private:
+    // the scheduled insertStereoSequences: the session call, then each stream's HandlerState as its last entry leaves it
+    void runSchedule(const std::vector<int32_t>& ids, const std::vector<std::vector<uint8_t>>& schedule,
+                     const std::vector<std::vector<const uint8_t*>>& img_l, const std::vector<std::vector<const uint8_t*>>& img_r,
+                     const std::vector<std::vector<Segments>>* fl, const std::vector<std::vector<Segments>>* fr,
+                     std::vector<PlPoseResult>* results, std::vector<PlKeyframeResult>* kf) {
+        const char* who = "StereoStreamsHandler::insertStereoSequences";
+        const size_t n = ids.size(), T = schedule.size();
+        if (img_l.size() != T || img_r.size() != T) throw Error(PLSTVO_E_INVALID, std::string(who) + ": one image list per step");
+        std::vector<int32_t> th0, th_init;
+        std::vector<PlPrior> priors;
+        std::vector<PlKeyframeState> state;
+        std::vector<uint8_t> flat;
+        std::vector<const uint8_t*> l, r;
+        std::vector<Segments> sl, sr;
+        for (int32_t id : ids) {
+            const Stream& s = at(id);
+            th0.push_back(s.orb_fast_th);
+            priors.push_back(priorOf(s.prev_frame));
+            state.push_back(s.kf.state());
+        }
+        for (size_t t = 0; t < T; ++t) {
+            if (schedule[t].size() != n) throw Error(PLSTVO_E_INVALID, std::string(who) + ": one schedule entry per stream and step");
+            size_t m = 0;
+            for (uint8_t c : schedule[t]) {
+                flat.push_back(c);
+                if (c) th_init.push_back(c == 2 ? hcfg_.orb_fast_th : 0);   // :38; an insert's threshold is the device's
+                m += c != 0;
+            }
+            if (img_l[t].size() != m || img_r[t].size() != m)
+                throw Error(PLSTVO_E_INVALID, std::string(who) + ": one image per non-zero entry");
+            l.insert(l.end(), img_l[t].begin(), img_l[t].end());
+            r.insert(r.end(), img_r[t].begin(), img_r[t].end());
+            if (fl && fr) {
+                if ((*fl)[t].size() != m || (*fr)[t].size() != m)
+                    throw Error(PLSTVO_E_INVALID, std::string(who) + ": one segment list per image");
+                sl.insert(sl.end(), (*fl)[t].begin(), (*fl)[t].end());
+                sr.insert(sr.end(), (*fr)[t].begin(), (*fr)[t].end());
+            }
+        }
+        if (fl && fr && (fl->size() != T || fr->size() != T))
+            throw Error(PLSTVO_E_INVALID, std::string(who) + ": one segment list per image");
+        if (T == 0 || n == 0 || l.empty()) return;
+        pack_.pack(cam_.width, cam_.height, channels_, l, r, th_init, who);
+        attachLines(fl ? &sl : nullptr, fr ? &sr : nullptr, who);
+        std::vector<PlPoseResult> res(n * T);
+        std::vector<int32_t> ns(4 * n * T);
+        const PlKeyframeConfig kc = hcfg_.keyframes();
+        if (kf) kf->assign(n * T, PlKeyframeResult{});
+        session_.runSchedule(hcfg_.device(), kf ? &kc : nullptr, (int)n, ids.data(), (int)T, flat.data(), pack_.view, th0.data(),
+                             priors.data(), kf ? state.data() : nullptr, res.data(), kf ? kf->data() : nullptr, nullptr,
+                             ns.data());
+        // the last step with entries: what keepFeatures reads, its insert group or else its initialize group
+        size_t last = T;
+        for (size_t t = T; t-- > 0 && last == T;)
+            for (uint8_t c : schedule[t]) last = c ? t : last;
+        std::vector<int32_t> read_ids, read_ns;
+        bool read_insert = false;
+        for (size_t k = 0; k < n; ++k) read_insert = read_insert || schedule[last][k] == 1;
+        for (size_t k = 0; k < n; ++k) {
+            const uint8_t c = schedule[last][k];
+            if (c != (read_insert ? 1 : 2)) continue;
+            read_ids.push_back(ids[k]);
+            read_ns.insert(read_ns.end(), ns.begin() + 4 * (last * n + k) + (read_insert ? 0 : 2), ns.begin() + 4 * (last * n + k) + 4);
+        }
+        if (keep_) session_.read((int)read_ids.size(), read_ns.data(), read_insert, read_);
+        // each stream's entries replayed in order on its HandlerState, as the per-frame calls leave it: initialize resets the
+        // frame, threshold and key-frame test; an insert publishes its result (optimizePose), applies currFrameIsKF's pose
+        // reset where the device's test fired, and updateFrame moves the frame into prev_frame with the next threshold
+        for (size_t k = 0; k < n; ++k) {
+            Stream& s = streams_[(size_t)ids[k]];
+            size_t last_insert = T;
+            bool insert_last = false;   // no initialize after the last insert
+            for (size_t t = 0; t < T; ++t) {
+                const uint8_t c = schedule[t][k];
+                if (!c) continue;
+                s.has_prev = true;
+                insert_last = c == 1;
+                if (c == 2) {   // as initialize() above
+                    s.initialize(hcfg_, StereoFrame{});
+                    s.curr_frame = StereoFrame{};
+                    continue;
+                }
+                const PlPoseResult& r = res[t * n + k];
+                s.result = r;
+                std::copy(ns.begin() + 4 * (t * n + k), ns.begin() + 4 * (t * n + k) + 4, s.n_stereo.begin());
+                s.curr_frame = StereoFrame{};
+                s.optimizePose(r);
+                if (kf && (*kf)[t * n + k].new_kf) {   // currFrameIsKF on curr_frame (the test's state: below)
+                    s.curr_frame.Tfw = se3::identity4();
+                    identityCov(s.curr_frame.Tfw_cov);
+                }
+                s.updateFrame(hcfg_);
+                last_insert = t;
+            }
+            if (kf && insert_last) {   // the device's test as it stands after the stream's last insert
+                s.kf = KeyframeTest::fromState(state[k]);
+                const PlKeyframeResult& kl = (*kf)[last_insert * n + k];
+                s.kf.entropy_curr = kl.entropy_curr;
+                s.kf.entropy_ratio = kl.entropy_ratio;
+                s.kf.kf_t = kl.t;
+                s.kf.kf_r = kl.r;
+            }
+        }
+        if (keep_) detail::splitRead(read_, read_ns.data(), read_insert ? 4 : 2, named(read_ids), &HandlerState::prev_frame);
+        if (results) *results = std::move(res);
+    }
     // the FLD branch's key lines of the packed frames (fl / fr null: none given)
     void attachLines(const std::vector<Segments>* fl, const std::vector<Segments>* fr, const char* who) {
         if (!fl != !fr) throw Error(PLSTVO_E_INVALID, std::string(who) + ": segments for both sides or neither");

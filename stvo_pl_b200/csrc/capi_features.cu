@@ -923,6 +923,18 @@ struct LineBlocks {
         return 0;
     }
 
+    // The caller's key lines of f's B frames, both sides checked whole, then one block per image in the order the call's
+    // images took on the device: block z is image side[z] (0 left, 1 right) of frame frame[z]
+    int cut_images(PlContext* ctx, const PlStereoImages* f, const std::vector<int>& frame, const std::vector<int>& side) {
+        const LineSrc whole[2] = {LineSrc{f->B, f->ll_off, f->seg_l, f->angle_l, f->npix_l},
+                                  LineSrc{f->B, f->lr_off, f->seg_r, f->angle_r, f->npix_r}};
+        for (const LineSrc& l : whole)
+            if (const int rc = lbd_check_lines(ctx, l)) return rc;
+        off.assign(frame.size(), {});
+        for (size_t z = 0; z < frame.size(); ++z) add_block(z, whole[side[z]], (size_t)frame[z], 1);
+        return 0;
+    }
+
     // LSD's key lines of nblk blocks of nf images: its host continuation on stream s (where its device half ran), with the
     // images calls' key-line checks
     int take_lsd(PlContext* ctx, const PlLsdConfig* lc, const LsdLaunch& lsd, cudaStream_t s, int nblk, int nf) {
@@ -990,6 +1002,32 @@ void stereo_set_inputs(const OrbDetected& orb, int ob, bool pts, const LineBlock
     }
     if (lines.run_lbd) {
         const size_t l0 = (size_t)lines.lbase[(size_t)lb], l1 = (size_t)lines.lbase[(size_t)lb + 1];
+        Ls.xy_l = lines.d_seg + 4 * l0; Ls.xy_r = lines.d_seg + 4 * l1;
+        Ls.d1 = lines.d_ldesc + 32 * l0; Ls.d2 = lines.d_ldesc + 32 * l1;
+    }
+}
+
+// The line set of one group of a scheduled run (nf frames): line blocks of one image each, lb .. lb + nf - 1 the left images
+// and the next nf the right ones.  Their offsets and left angles are joined into l_off, r_off and ang (host), and the rows
+// are one slice of LBD's output, as the blocks are consecutive.
+void schedule_line_inputs(const LineBlocks& lines, int lb, int nf, std::vector<int32_t>& l_off, std::vector<int32_t>& r_off,
+                          std::vector<float>& ang, StereoSet& Ls) {
+    if (lines.lsrc.empty()) return;
+    l_off.assign(1, 0);
+    r_off.assign(1, 0);
+    ang.clear();
+    for (int i = 0; i < nf; ++i) {
+        const LineSrc& l = lines.lsrc[(size_t)lb + i];
+        const LineSrc& r = lines.lsrc[(size_t)(lb + nf + i)];
+        l_off.push_back(l_off.back() + l.off[1]);
+        r_off.push_back(r_off.back() + r.off[1]);
+        ang.insert(ang.end(), l.angle, l.angle + l.off[1]);
+    }
+    Ls.l_off = l_off.data();
+    Ls.r_off = r_off.data();
+    Ls.ang = ang.data();
+    if (lines.run_lbd) {
+        const size_t l0 = (size_t)lines.lbase[(size_t)lb], l1 = (size_t)lines.lbase[(size_t)(lb + nf)];
         Ls.xy_l = lines.d_seg + 4 * l0; Ls.xy_r = lines.d_seg + 4 * l1;
         Ls.d1 = lines.d_ldesc + 32 * l0; Ls.d2 = lines.d_ldesc + 32 * l1;
     }
@@ -1517,6 +1555,26 @@ void plstvo_kitti_handler_config(PlHandlerConfig* h) {
 }
 
 namespace {
+// the handler config's checks of a session run
+int handler_check(PlContext* ctx, const PlHandlerConfig* h) {
+    if (!h) return fail(ctx, PLSTVO_E_INVALID, "null handler config");
+    if (h->fast_min_th < 1 || h->fast_min_th > h->fast_max_th || h->fast_max_th > 255 || h->fast_inc_th < 0 ||
+        h->fast_feat_th < 0 || !std::isfinite(h->fast_err_th))
+        return fail(ctx, PLSTVO_E_INVALID, "handler config out of range");
+    return 0;
+}
+
+// the key-frame arguments' checks of a session run with the test (n streams)
+int keyframe_check(PlContext* ctx, const PlKeyframeConfig* k, int n, const PlKeyframeState* kf_state, const PlKeyframeResult* kf) {
+    if (!k || !kf_state || !kf) return fail(ctx, PLSTVO_E_INVALID, "null key-frame config, state or results");
+    if (std::isnan(k->min_entropy_ratio) || std::isnan(k->max_kf_t_dist) || std::isnan(k->max_kf_r_dist))
+        return fail(ctx, PLSTVO_E_INVALID, "NaN in the key-frame config");
+    for (int i = 0; i < n; ++i)
+        if ((kf_state[i].prev_f_iskf != 0 && kf_state[i].prev_f_iskf != 1) || kf_state[i].N_prevKF_currF < 0)
+            return fail(ctx, PLSTVO_E_INVALID, "key-frame state with prev_f_iskf outside {0, 1} or a negative N_prevKF_currF");
+    return 0;
+}
+
 // plstvo_stereo_session_run after the context lock: the checks, then the state-independent stages once over every image
 // (upload, rectifier, LSD, LBD) and the steps (ORB at the device threshold row, the stereo step, tracking, the handler
 // update), each committed to the session as an insert is.  session_finish synchronises both streams after a failure.  With kc
@@ -1526,10 +1584,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
                 const PlStereoImages* frames, const int32_t* fast_th0, const PlPrior* priors, PlPoseResult* results,
                 int32_t* fast_th, int32_t* n_stereo, const PlKeyframeConfig* kc = nullptr, PlKeyframeState* kf_state = nullptr,
                 PlKeyframeResult* kf = nullptr) {
-    if (!h) return fail(ctx, PLSTVO_E_INVALID, "null handler config");
-    if (h->fast_min_th < 1 || h->fast_min_th > h->fast_max_th || h->fast_max_th > 255 || h->fast_inc_th < 0 ||
-        h->fast_feat_th < 0 || !std::isfinite(h->fast_err_th))
-        return fail(ctx, PLSTVO_E_INVALID, "handler config out of range");
+    if (const int rc = handler_check(ctx, h)) return rc;
     if (T < 0) return fail(ctx, PLSTVO_E_INVALID, "negative T");
     if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
     if ((long long)frames->B != (long long)T * n) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from T * n");
@@ -1748,6 +1803,395 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     }
     return 0;
 }
+
+// One group of a scheduled run: a step's initialize entries or its insert entries, which the chain hands to one session call
+struct SchedGroup {
+    int t = 0;
+    bool track = false;
+    std::vector<int32_t> ids;   // the group's streams, in the order of the call's ids
+    std::vector<int> pos;       // their call positions: their state slots
+    std::vector<int> frame;     // their frames' indices in frames
+    int img0 = 0;               // the group's first image on the device: its left images, then its right ones
+    int e0 = 0, r0 = 0;         // its first entry in the entry table, and (insert) its first row of the insert results
+};
+
+// plstvo_stereo_session_run_schedule after the context lock: the checks, then each step's initialize group and insert group
+// as the chain's two calls.  The present images go up, are prepared and have their key lines found and described once, in
+// group order; each stream's FAST threshold, prior and key-frame state live in a device slot for the whole call, gathered
+// for an insert group's ORB, solver and test by session_schedule_gather_kernel and written back (reset after an initialize)
+// by session_schedule_update_kernel.  *ran: some group ran; *last_track, *last_n: the last group (what retention holds).
+int session_schedule(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, const PlKeyframeConfig* kc, int n,
+                     const int32_t* ids, int T, const uint8_t* schedule, const PlStereoImages* frames, const int32_t* fast_th0,
+                     const PlPrior* priors, PlKeyframeState* kf_state, PlPoseResult* results, PlKeyframeResult* kf,
+                     int32_t* fast_th, int32_t* n_stereo, bool* ran, bool* last_track, int* last_n) {
+    if (const int rc = handler_check(ctx, h)) return rc;
+    if (T < 0) return fail(ctx, PLSTVO_E_INVALID, "negative T");
+    if (n < 0 || !frames) return fail(ctx, PLSTVO_E_INVALID, "null frames or negative n");
+    const long long TN = (long long)T * n;
+    if (TN > 0 && !schedule) return fail(ctx, PLSTVO_E_INVALID, "null schedule");
+    long long B = 0;
+    for (long long i = 0; i < TN; ++i) {
+        if (schedule[i] > 2) return fail(ctx, PLSTVO_E_INVALID, "schedule value outside {0, 1, 2}");
+        B += schedule[i] != 0;
+    }
+    if ((long long)frames->B != B) return fail(ctx, PLSTVO_E_SIZE, "frames->B differs from the schedule's non-zero entries");
+    const bool lns = ss->cfg.has_lines != 0, fld = ss->fld && lns;   // fld: the caller's key lines, in frames' order
+    if (const int rc = check_key_line_fields(ctx, &frames, 1, !ss->fld, ss->fld && !lns, false)) return rc;
+    const PlOrbDetectConfig* oc = &ss->oc;
+    std::vector<int32_t> th0((size_t)n);
+    for (int k = 0; k < n; ++k) {
+        if (fast_th0 && (fast_th0[k] < 0 || fast_th0[k] > 255)) return fail(ctx, PLSTVO_E_INVALID, "fast_th0 outside [0, 255]");
+        th0[(size_t)k] = fast_th0 && fast_th0[k] ? fast_th0[k] : oc->fast_threshold;
+        if (th0[(size_t)k] < 0 || th0[(size_t)k] > 255)
+            return fail(ctx, PLSTVO_E_INVALID, "ocfg->fast_threshold outside [0, 255] where fast_th0 leaves it");
+    }
+    auto all_rows = [&]() {   // no group runs: every threshold row is row 0
+        for (int t = 0; fast_th && t <= T; ++t) std::copy(th0.begin(), th0.end(), fast_th + (size_t)t * n);
+    };
+    if (T == 0) {
+        all_rows();
+        return 0;
+    }
+    if (n > 0 && (!ids || !results)) return fail(ctx, PLSTVO_E_INVALID, "null ids or results");
+    if (2 * B > 65535) return fail(ctx, PLSTVO_E_INVALID, "more than 65535 images in one call");
+    if (const int rc = session_check_ids(ctx, ss, false, n, ids)) return rc;
+    // which stream holds a frame at each entry (held at the call's start, or initialised at an earlier step of it), and the
+    // initialize entries' thresholds
+    std::vector<uint8_t> live((size_t)n);
+    for (int k = 0; k < n; ++k) live[(size_t)k] = ss->live[(size_t)ids[k]];
+    std::vector<int32_t> entry_th((size_t)B, 0), frame_of((size_t)TN, -1);
+    for (long long i = 0, b = 0; i < TN; ++i) {
+        const int code = schedule[i], k = (int)(i % n);
+        if (!code) continue;
+        const int32_t ft = frames->fast_th ? frames->fast_th[b] : 0;
+        if (code == 1 && !live[(size_t)k])
+            return fail(ctx, PLSTVO_E_INVALID, "insert on a stream with no frame at that step: initialize it first, before or in the call");
+        if (code == 1 && ft) return fail(ctx, PLSTVO_E_INVALID, "frames->fast_th of an insert entry must be 0: the run sets its thresholds");
+        if (code == 2) {
+            entry_th[(size_t)b] = ft ? ft : oc->fast_threshold;
+            if (entry_th[(size_t)b] < 0 || entry_th[(size_t)b] > 255)
+                return fail(ctx, PLSTVO_E_INVALID, "an initialize entry's threshold outside [0, 255]");
+            live[(size_t)k] = 1;
+        }
+        frame_of[(size_t)i] = (int32_t)b++;
+    }
+    if (oc->n_features > PLSTVO_MAX_FEATURES)
+        return fail(ctx, PLSTVO_E_INVALID, "ocfg.n_features exceeds PLSTVO_MAX_FEATURES: a step could fail on a feature limit");
+    const PlCamera& cam = ss->cam;
+    const bool pts = ss->cfg.has_points != 0;
+    const int W = cam.width, H = cam.height, n_img = (int)(2 * B);
+    if (const int rc = orb_detect_check(ctx, oc)) return rc;
+    if (pts && B > 0) {
+        PlOrbConfig orb_cfg;
+        OrbDevLevels levels;
+        std::vector<int32_t> tabs;
+        std::vector<size_t> tab_off;
+        if (const int rc = orb_detect_levels(ctx, oc, W, H, orb_cfg, levels, tabs, tab_off)) return rc;
+    }
+    LsdLaunch lsd{};
+    if (B > 0)
+        if (const int rc = images_check(ctx, W, H, pts, lns, &frames, 1, lns && !fld ? &ss->lc : nullptr, n_img, lsd)) return rc;
+    // the groups in chain order, the entry table, and the device order of the images (frame, side)
+    std::vector<SchedGroup> groups;
+    std::vector<SchedEntry> entries;
+    std::vector<int> img_frame, img_side;
+    int n_ins = 0, max_e = 0, max_ins = 0;
+    for (int t = 0; t < T; ++t)
+        for (int code : {2, 1}) {
+            SchedGroup g;
+            g.t = t;
+            g.track = code == 1;
+            for (int k = 0; k < n; ++k)
+                if (schedule[(size_t)t * n + k] == code) {
+                    g.ids.push_back(ids[k]);
+                    g.pos.push_back(k);
+                    g.frame.push_back(frame_of[(size_t)t * n + k]);
+                }
+            const int ne = (int)g.ids.size();
+            if (!ne) continue;
+            g.img0 = (int)img_frame.size();
+            g.e0 = (int)entries.size();
+            g.r0 = n_ins;
+            for (int i = 0; i < ne; ++i) entries.push_back(SchedEntry{g.pos[(size_t)i], entry_th[(size_t)g.frame[(size_t)i]]});
+            for (int side = 0; side < 2; ++side)
+                for (int i = 0; i < ne; ++i) {
+                    img_frame.push_back(g.frame[(size_t)i]);
+                    img_side.push_back(side);
+                }
+            if (g.track) {
+                n_ins += ne;
+                max_ins = std::max(max_ins, ne);
+            }
+            max_e = std::max(max_e, ne);
+            groups.push_back(std::move(g));
+        }
+    LineBlocks lines;   // one block per device image
+    if (fld && B > 0)
+        if (const int rc = lines.cut_images(ctx, frames, img_frame, img_side)) return rc;
+    if (B == 0) {   // every stream idles at every step
+        all_rows();
+        return 0;
+    }
+    *ran = true;
+    CK(ctx, cudaSetDevice(ctx->device));
+    CK(ctx, ctx->img_ev.create());
+    CK(ctx, ctx->img_join.create(cudaEventDisableTiming));
+    ctx->img_timed = false;
+    Events<2> run_ev;      // the call's start, the end of its uploads and preparation
+    Events<3> marks[2];    // stereo step start, its end, tracking end, of even and odd groups
+    CK(ctx, run_ev.create());
+    CK(ctx, marks[0].create());
+    CK(ctx, marks[1].create());
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, cudaEventRecord(run_ev[0], s));
+    const size_t px = (size_t)W * H;
+    const PlRectifier* rect = ss->rect;
+    const bool prepare = rect && (pts || lns);
+    const bool rgb = prepare && ss->fld && lns && rect->channels > 1;   // rectify_call's RGB2GRAY plane, which LBD reads
+    const bool keep = ss->retain;
+    // the grey images in group order; the entry table; the slots (thresholds [n], priors [n], key-frame states [n]); the
+    // slots' thresholds before each step with entries and after the last ([T + 1][n]); an insert group's ORB threshold row
+    // and the handler's next row ([2 max_ins] each); the insert results [n_ins], and with the test the group's states, the
+    // decisions [n_ins] and with retention the key frames' segments [n_ins]
+    Arena a;
+    const size_t o_img = a.take(pts || lns ? (size_t)n_img * px : 0), o_rgb = a.take(rgb ? (size_t)n_img * px : 0),
+                 o_ent = a.take(entries.size() * sizeof(SchedEntry)), o_ths = a.take((size_t)n * 4),
+                 o_pri = a.take((size_t)n * sizeof(PlPrior)), o_snap = a.take((size_t)(T + 1) * n * 4),
+                 o_th = a.take((size_t)2 * max_ins * 4), o_thn = a.take((size_t)2 * max_ins * 4),
+                 o_res = a.take((size_t)n_ins * sizeof(PlPoseResult));
+    size_t o_kfs = 0, o_kfst = 0, o_kfr = 0, o_kfseg = 0;
+    if (kc) {
+        o_kfs = a.take((size_t)n * sizeof(PlKeyframeState));
+        o_kfst = a.take((size_t)max_ins * sizeof(PlKeyframeState));
+        o_kfr = a.take((size_t)n_ins * sizeof(PlKeyframeResult));
+        o_kfseg = a.take(keep ? (size_t)n_ins * sizeof(GatherSeg) : 0);
+    }
+    CK(ctx, a.alloc(ctx->arena_run));
+    // the insert groups' priors are gathered straight into the workspace's, which no group then regrows
+    CK(ctx, ctx->ws.d_priors.ensure((size_t)std::max(max_ins, 1) * sizeof(PlPrior)));
+    PlPrior fresh{};   // priorOf of a freshly initialised frame; priors NULL starts every stream from it
+    for (int i = 0; i < 16; ++i) fresh.Tfw[i] = fresh.DT[i] = (i % 5 == 0) ? 1.0 : 0.0;
+    for (int i = 0; i < 36; ++i) fresh.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+    fresh.err_norm = -1.0;
+    const std::vector<PlPrior> pri0 = priors ? std::vector<PlPrior>(priors, priors + n) : std::vector<PlPrior>((size_t)n, fresh);
+    CK(ctx, a.up(o_ent, entries.data(), entries.size() * sizeof(SchedEntry), s));
+    CK(ctx, a.up(o_ths, th0.data(), (size_t)n * 4, s));
+    CK(ctx, a.up(o_pri, pri0.data(), (size_t)n * sizeof(PlPrior), s));
+    if (kc) CK(ctx, a.up(o_kfs, kf_state, (size_t)n * sizeof(PlKeyframeState), s));
+    const SchedEntry* d_ent = a.at<SchedEntry>(o_ent);
+    int32_t* d_ths = a.at<int32_t>(o_ths);
+    PlPrior* d_pri = a.at<PlPrior>(o_pri);
+    PlKeyframeState* d_kfs = kc ? a.at<PlKeyframeState>(o_kfs) : nullptr;
+    int32_t* d_th = a.at<int32_t>(o_th);
+    int32_t* d_thn = a.at<int32_t>(o_thn);
+    uint8_t* d_img = a.u8(o_img);
+    const uint8_t* d_rgb = rgb ? a.u8(o_rgb) : nullptr;
+    const int ch = rect ? rect->channels : 1;
+    auto host_image = [&](int z) {
+        return (img_side[(size_t)z] ? frames->img_r : frames->img_l) + (size_t)img_frame[(size_t)z] * px * ch;
+    };
+    if (prepare) {   // per group, as its streams' rectifiers take them; the prepared images are copied into group order
+        for (const SchedGroup& g : groups) {
+            const int ne = (int)g.ids.size();
+            std::vector<ImgPart> parts;
+            for (int z = g.img0; z < g.img0 + 2 * ne; ++z) parts.push_back(ImgPart{host_image(z), 1});
+            const SessionCall gc{ss, g.track, false, ne, g.ids.data()};
+            const uint8_t* out = nullptr;
+            const uint8_t* out_rgb = nullptr;
+            if (const int rc = rectify_call(ctx, rect, &gc, ne, 2 * ne, parts, s, &out, &out_rgb)) return rc;
+            CK(ctx, cudaMemcpyAsync(d_img + (size_t)g.img0 * px, out, 2 * ne * px, cudaMemcpyDeviceToDevice, s));
+            if (rgb)
+                CK(ctx, cudaMemcpyAsync(a.u8(o_rgb) + (size_t)g.img0 * px, out_rgb, 2 * ne * px, cudaMemcpyDeviceToDevice, s));
+        }
+    } else if (pts || lns) {   // runs of consecutive host images in one copy each
+        for (int z = 0; z < n_img;) {
+            int e = z + 1;
+            while (e < n_img && host_image(e) == host_image(e - 1) + px) ++e;
+            CK(ctx, a.up(o_img + (size_t)z * px, host_image(z), (size_t)(e - z) * px, s));
+            z = e;
+        }
+    }
+    CK(ctx, cudaEventRecord(run_ev[1], s));
+    // the lines of every image: LSD alone on the main stream (FLD: the caller's), then LBD on the second stream beside the
+    // first group's ORB
+    if (lns && !fld) {
+        if (const int rc = lsd_enqueue(ctx, lsd, d_img, nullptr, {}, s)) return rc;
+        if (const int rc = lines.take_lsd(ctx, &ss->lc, lsd, s, n_img, 1)) return rc;
+    }
+    if (lines.run_lbd) {
+        cudaEvent_t ready = next_event(ctx);
+        CK(ctx, cudaEventRecord(ready, s));
+        if (const int rc = lines.describe(ctx, W, H, d_rgb ? d_rgb : d_img, ready, {})) return rc;
+    }
+    float* ms = ctx->img_ms;
+    std::fill(ms, ms + 5, 0.f);
+    auto add_ms = [&](int k, cudaEvent_t from, cudaEvent_t to) -> int {
+        float v = 0;
+        CK(ctx, cudaEventElapsedTime(&v, from, to));
+        ms[k] += v;
+        return 0;
+    };
+    const double k_entropy = 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0)));   // KeyframeTest::needNewKF's constant
+    std::vector<GatherSeg> kf_segs(kc && keep ? (size_t)n_ins : 0);   // [n_ins], as uploaded
+    const LineBlocks no_lines;
+    std::vector<int32_t> none((size_t)max_e + 1, 0), pl_off, pr_off, l_off, r_off, ns((size_t)4 * max_e);
+    std::vector<float> ang;
+    std::vector<int32_t> th_init;
+    int last_t = -1;
+    for (size_t j = 0; j < groups.size(); ++j) {
+        const SchedGroup& g = groups[j];
+        const int ne = (int)g.ids.size();
+        if (g.t != last_t) {   // the slots' thresholds before the step
+            CK(ctx, cudaMemcpyAsync(a.u8(o_snap) + (size_t)g.t * n * 4, d_ths, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+            last_t = g.t;
+        }
+        SessionCall step = session_begin(ss, g.track, ne, g.ids.data());
+        // the retention arena holds the last group (every insert group's rows for the key frames)
+        step.retain = keep && (j + 1 == groups.size() || (kc && g.track));
+        if (g.track) {
+            CK(ctx, launch_session_schedule_gather(ne, d_ent + g.e0, d_ths, d_pri, d_kfs, d_th, ctx->ws.d_priors.as<PlPrior>(),
+                                                   kc ? a.at<PlKeyframeState>(o_kfst) : nullptr, s));
+            ctx->launches++;
+        } else {   // initialize: each frame at its entry's threshold, from the host as _initialize takes it
+            th_init.assign((size_t)2 * ne, 0);
+            for (int i = 0; i < ne; ++i) th_init[(size_t)i] = th_init[(size_t)(ne + i)] = entries[(size_t)(g.e0 + i)].th;
+        }
+        OrbDetected orb;
+        if (pts) {
+            if (const int rc = orb_detect_enqueue(ctx, oc, 2 * ne, W, H, d_img + (size_t)g.img0 * px, {},
+                                                  g.track ? nullptr : th_init.data(), INT_MAX, nullptr, orb,
+                                                  g.track ? d_th : nullptr))
+                return rc;
+        } else {
+            orb.off.assign((size_t)2 * ne + 1, 0);
+        }
+        StereoSet sets[2];
+        stereo_set_inputs(orb, 0, pts, no_lines, 0, ne, none, pl_off, pr_off, sets);
+        schedule_line_inputs(lines, g.img0, ne, l_off, r_off, ang, sets[1]);
+        StereoDevInputs dev;
+        dev.lines_ready = lines.joined;
+        cudaEvent_t* mk = marks[j % 2].ev;
+        dev.marks = mk;
+        if (g.track) {
+            dev.priors_resident = true;   // gathered above
+            dev.tracked = [&](const Workspace& ws) -> int {
+                PlPrior* wp = ws.d_priors.as<PlPrior>();
+                PlKeyframeState* kfst = kc ? a.at<PlKeyframeState>(o_kfst) : nullptr;
+                CK(ctx, launch_session_handler(*h, ne, ws.d_results.as<PlPoseResult>(), d_th, d_thn, wp,
+                                               a.at<PlPoseResult>(o_res) + g.r0, s));
+                ctx->launches++;
+                if (kc) {
+                    PlKeyframeResult* d_kf = a.at<PlKeyframeResult>(o_kfr) + g.r0;
+                    CK(ctx, launch_session_keyframe(*kc, k_entropy, ne, ws.d_results.as<PlPoseResult>(), kfst, d_kf, wp, s));
+                    ctx->launches++;
+                    if (keep) {   // as session_run: the key frames' rows into the step's own chunk (chunk t: step t)
+                        GatherSeg* seg = kf_segs.data() + g.r0;
+                        int32_t np = 0, nl = 0;
+                        for (int i = 0; i < ne; ++i) {
+                            seg[i] = GatherSeg{np, np, step.new_pt[(size_t)i], nl, nl, step.new_ls[(size_t)i]};
+                            np += seg[i].n_pt;
+                            nl += seg[i].n_ls;
+                        }
+                        const size_t o = o_kfseg + (size_t)g.r0 * sizeof(GatherSeg);
+                        CK(ctx, a.up(o, seg, (size_t)ne * sizeof(GatherSeg), s));
+                        while (ss->kf_steps.size() < (size_t)g.t)   // steps without inserts keep an empty chunk
+                            ss->kf_steps.push_back(std::unique_ptr<SessionRetained>(new SessionRetained()));
+                        ss->kf_steps.push_back(std::unique_ptr<SessionRetained>(new SessionRetained()));
+                        SessionRetained& c = *ss->kf_steps.back();
+                        CK(ctx, c.lay_out((size_t)np, (size_t)nl, 0, 0));
+                        CK(ctx, launch_session_gather(ss->kept.rec, c.rec, false, a.at<GatherSeg>(o), ne, s, d_kf));
+                        ctx->launches++;
+                    }
+                }
+                CK(ctx, launch_session_schedule_update(ne, d_ent + g.e0, false, d_thn, wp, kfst, d_ths, d_pri, d_kfs, s));
+                ctx->launches++;
+                CK(ctx, cudaEventRecord(mk[2], s));
+                // as session_run: later uploads on s_h2d wait for this group's end
+                cudaEvent_t step_done = next_event(ctx);
+                CK(ctx, cudaEventRecord(step_done, s));
+                CK(ctx, cudaStreamWaitEvent(ctx->s_h2d, step_done, 0));
+                return 0;
+            };
+        }
+        const int rc = track_stereo_common(ctx, &cam, &ss->cfg, &ss->mc, &ss->sc, sets, nullptr, nullptr, results,
+                                           n_stereo ? ns.data() : nullptr, false, -1, &dev, &step);
+        if (rc) return rc;
+        if (!g.track) {
+            CK(ctx, launch_session_schedule_update(ne, d_ent + g.e0, true, nullptr, nullptr, nullptr, d_ths, d_pri, d_kfs, s));
+            ctx->launches++;
+        }
+        session_commit(step);
+        for (int i = 0; n_stereo && i < ne; ++i) {   // an initialize entry's row: {0, 0, points, lines}
+            int32_t* row = n_stereo + ((size_t)g.t * n + g.pos[(size_t)i]) * 4;
+            for (int c = 0; c < 4; ++c)
+                row[c] = g.track ? ns[(size_t)4 * i + c] : c < 2 ? 0 : ns[(size_t)2 * i + c - 2];
+        }
+        // the stereo step's count readback synchronised the main stream: this group's ORB and the last group are done
+        if (pts)
+            if (const int rc2 = add_ms(1, ctx->orb_det_ev[0], ctx->orb_det_ev[4])) return rc2;
+        if (j > 0) {
+            const cudaEvent_t* pm = marks[(j - 1) % 2].ev;
+            if (const int rc2 = add_ms(3, pm[0], pm[1])) return rc2;
+            if (const int rc2 = add_ms(4, pm[1], pm[2])) return rc2;
+        }
+    }
+    CK(ctx, cudaMemcpyAsync(a.u8(o_snap) + (size_t)T * n * 4, d_ths, (size_t)n * 4, cudaMemcpyDeviceToDevice, s));
+    std::vector<PlPoseResult> res((size_t)n_ins);
+    std::vector<PlKeyframeResult> kres(kc ? (size_t)n_ins : 0);
+    std::vector<PlKeyframeState> kfs_out(kc ? (size_t)n : 0);
+    std::vector<int32_t> snap((size_t)(T + 1) * n);
+    CK(ctx, a.down(res.data(), o_res, res.size() * sizeof(PlPoseResult), s));
+    if (kc) {
+        CK(ctx, a.down(kres.data(), o_kfr, kres.size() * sizeof(PlKeyframeResult), s));
+        CK(ctx, a.down(kfs_out.data(), o_kfs, (size_t)n * sizeof(PlKeyframeState), s));
+    }
+    CK(ctx, a.down(snap.data(), o_snap, snap.size() * 4, s));
+    CK(ctx, cudaStreamSynchronize(s));
+    CK(ctx, cudaStreamSynchronize(ctx->s_alt));
+    const cudaEvent_t* pm = marks[(groups.size() - 1) % 2].ev;
+    if (const int rc = add_ms(3, pm[0], pm[1])) return rc;
+    if (const int rc = add_ms(4, pm[1], pm[2])) return rc;
+    if (const int rc = add_ms(0, run_ev[0], run_ev[1])) return rc;
+    if (lns && !fld)
+        if (const int rc = add_ms(2, ctx->lsd_ev[0], lines.run_lbd ? ctx->lbd_ev[2] : ctx->lsd_ev[5])) return rc;
+    if (fld && lines.run_lbd)
+        if (const int rc = add_ms(2, ctx->lbd_ev[0], ctx->lbd_ev[2])) return rc;
+    ctx->img_timed = true;
+    // the insert entries' rows; the threshold rows: row t is the slots before the next step with entries (or after the last
+    // step), with each initialize entry's threshold in place
+    std::vector<uint8_t> has_entries((size_t)T, 0);
+    for (const SchedGroup& g : groups) {
+        has_entries[(size_t)g.t] = 1;
+        for (int i = 0; g.track && i < (int)g.ids.size(); ++i) {
+            const size_t at = (size_t)g.t * n + g.pos[(size_t)i], r = (size_t)(g.r0 + i);
+            results[at] = res[r];
+            if (kc) kf[at] = kres[r];
+        }
+    }
+    if (fast_th) {
+        for (int t = T, next = T; t >= 0; --t) {
+            if (t < T && has_entries[(size_t)t]) next = t;
+            std::copy(snap.begin() + (size_t)next * n, snap.begin() + (size_t)(next + 1) * n, fast_th + (size_t)t * n);
+        }
+        for (const SchedGroup& g : groups)
+            for (int i = 0; !g.track && i < (int)g.ids.size(); ++i)
+                fast_th[(size_t)g.t * n + g.pos[(size_t)i]] = entries[(size_t)(g.e0 + i)].th;
+    }
+    if (kc) {
+        std::copy(kfs_out.begin(), kfs_out.end(), kf_state);
+        for (const SchedGroup& g : groups)
+            for (int i = 0; keep && g.track && i < (int)g.ids.size(); ++i) {
+                const size_t r = (size_t)(g.r0 + i);
+                if (!kres[r].new_kf) continue;
+                const GatherSeg& sg = kf_segs[r];
+                ss->kf_rows.insert(ss->kf_rows.end(), {g.t, g.ids[(size_t)i], sg.n_pt, sg.n_ls});
+                ss->kf_off.insert(ss->kf_off.end(), {sg.src_pt, sg.src_ls});
+            }
+    }
+    *last_track = groups.back().track;
+    *last_n = (int)groups.back().ids.size();
+    return 0;
+}
 }  // namespace
 
 int plstvo_stereo_session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, int n, const int32_t* ids, int T,
@@ -1782,14 +2226,30 @@ int plstvo_stereo_session_run_keyframes(PlContext* ctx, PlStereoSession* ss, con
     LOCK(ctx);
     if (const int rc = session_check(ctx, ss)) return rc;
     session_start(ss, true);   // what the last call retained is discarded, also by a run of T = 0
-    if (!k || !kf_state || !kf) return fail(ctx, PLSTVO_E_INVALID, "null key-frame config, state or results");
-    if (std::isnan(k->min_entropy_ratio) || std::isnan(k->max_kf_t_dist) || std::isnan(k->max_kf_r_dist))
-        return fail(ctx, PLSTVO_E_INVALID, "NaN in the key-frame config");
-    for (int i = 0; i < n; ++i)
-        if ((kf_state[i].prev_f_iskf != 0 && kf_state[i].prev_f_iskf != 1) || kf_state[i].N_prevKF_currF < 0)
-            return fail(ctx, PLSTVO_E_INVALID, "key-frame state with prev_f_iskf outside {0, 1} or a negative N_prevKF_currF");
+    if (const int rc = keyframe_check(ctx, k, n, kf_state, kf)) return rc;
     const int rc = session_run(ctx, ss, h, n, ids, T, frames, fast_th0, priors, results, fast_th, n_stereo, k, kf_state, kf);
     if (session_finish(ctx, ss, rc, true, n, T > 0) == 0) ss->kf_valid = ss->retain;
+    return rc;
+}
+
+int plstvo_stereo_session_run_schedule(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, const PlKeyframeConfig* k,
+                                       int n, const int32_t* ids, int T, const uint8_t* schedule, const PlStereoImages* frames,
+                                       const int32_t* fast_th0, const PlPrior* priors, PlKeyframeState* kf_state,
+                                       PlPoseResult* results, PlKeyframeResult* kf, int32_t* fast_th, int32_t* n_stereo) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (const int rc = session_check(ctx, ss)) return rc;
+    session_start(ss, k != nullptr);   // as _run (k NULL) or _run_keyframes leaves what the last call retained
+    if (k) {
+        if (const int rc = keyframe_check(ctx, k, n, kf_state, kf)) return rc;
+    } else if (kf_state || kf) {
+        return fail(ctx, PLSTVO_E_INVALID, "kf_state and kf must be NULL without a key-frame config");
+    }
+    bool ran = false, track = false;
+    int last_n = 0;
+    const int rc = session_schedule(ctx, ss, h, k, n, ids, T, schedule, frames, fast_th0, priors, kf_state, results, kf, fast_th,
+                                    n_stereo, &ran, &track, &last_n);
+    if (session_finish(ctx, ss, rc, track, last_n, ran) == 0 && k) ss->kf_valid = ss->retain;
     return rc;
 }
 

@@ -537,6 +537,21 @@ cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPose
 // update) take Tfw = I, Tfw_cov = I.  k_entropy = 3 (1 + log 2 pi), as the host computes it.
 cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
                                     PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s);
+// plstvo_stereo_session_run_schedule: one entry of a step's initialize or insert group, the call position of its stream
+// (its state slot) and, for an initialize, the threshold its frame is detected with
+struct SchedEntry {
+    int32_t slot, th;
+};
+// The slots' gather before an insert group's ORB, on s for its n entries: thresholds into th [2 n] (both halves), priors [n]
+// (ws's d_priors) and, kfs_slot non-null, the key-frame states into kfs [n]
+cudaError_t launch_session_schedule_gather(int n, const SchedEntry* e, const int32_t* th_slot, const PlPrior* prior_slot,
+                                           const PlKeyframeState* kfs_slot, int32_t* th, PlPrior* priors, PlKeyframeState* kfs,
+                                           cudaStream_t s);
+// The slots' update after a group, on s: an insert group's th_next [2 n] (left half read), priors [n] and kfs [n] (kfs_slot
+// non-null) into its entries' slots, or (init) the slots reset to what initialize leaves
+cudaError_t launch_session_schedule_update(int n, const SchedEntry* e, bool init, const int32_t* th_next, const PlPrior* priors,
+                                           const PlKeyframeState* kfs, int32_t* th_slot, PlPrior* prior_slot,
+                                           PlKeyframeState* kfs_slot, cudaStream_t s);
 
 // ---- capi_stereo.cu: the stereo step's feature sets, and raw stereo features -> pose, composed by the images path ----
 // One feature set: one kind of feature (points or lines) of nf frames.  Offsets and left line angles are host arrays; xy_l,

@@ -79,6 +79,55 @@ __global__ void session_handler_kernel(PlHandlerConfig h, int n, const PlPoseRes
     res_out[k] = r;
 }
 
+// A scheduled run's state gather: entry k of a step's insert group reads its stream's slot, the threshold into both halves
+// of ORB's row th [2 n], the prior into the workspace's priors and the key-frame state (kfs non-null) into the step's table.
+// Moves only: the slots hold exactly what session_handler_kernel and session_keyframe_kernel wrote.
+__global__ void session_schedule_gather_kernel(int n, const SchedEntry* __restrict__ e, const int32_t* __restrict__ th_slot,
+                                               const PlPrior* __restrict__ prior_slot,
+                                               const PlKeyframeState* __restrict__ kfs_slot, int32_t* __restrict__ th,
+                                               PlPrior* __restrict__ priors, PlKeyframeState* __restrict__ kfs) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const int s = e[k].slot;
+    th[k] = th[n + k] = th_slot[s];
+    priors[k] = prior_slot[s];
+    if (kfs) kfs[k] = kfs_slot[s];
+}
+
+// A scheduled run's state update after a step's group: an insert group writes each entry's next threshold (th_next, row
+// layout of session_handler_kernel), prior and key-frame state back into its stream's slot; an initialize group (init)
+// resets the slot to what HandlerState::initialize leaves: the entry's threshold, priorOf of a fresh frame (Tfw = I,
+// Tfw_cov = I, DT = I, DT_cov = 0, err_norm = -1) and plstvo_initial_keyframe_state.  Slots no entry names stay as they are.
+__global__ void session_schedule_update_kernel(int n, const SchedEntry* __restrict__ e, bool init,
+                                               const int32_t* __restrict__ th_next, const PlPrior* __restrict__ priors,
+                                               const PlKeyframeState* __restrict__ kfs, int32_t* __restrict__ th_slot,
+                                               PlPrior* __restrict__ prior_slot, PlKeyframeState* __restrict__ kfs_slot) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n) return;
+    const int s = e[k].slot;
+    if (!init) {
+        th_slot[s] = th_next[k];
+        prior_slot[s] = priors[k];
+        if (kfs_slot) kfs_slot[s] = kfs[k];
+        return;
+    }
+    th_slot[s] = e[k].th;
+    PlPrior& p = prior_slot[s];
+    for (int i = 0; i < 16; ++i) p.Tfw[i] = p.DT[i] = (i % 5 == 0) ? 1.0 : 0.0;
+    for (int i = 0; i < 36; ++i) {
+        p.Tfw_cov[i] = (i % 7 == 0) ? 1.0 : 0.0;
+        p.DT_cov[i] = 0.0;
+    }
+    p.err_norm = -1.0;
+    if (!kfs_slot) return;
+    PlKeyframeState& q = kfs_slot[s];
+    q.prev_f_iskf = 1;
+    q.N_prevKF_currF = 0;
+    q.entropy_first_prevKF = 0.0;
+    for (int i = 0; i < 16; ++i) q.T_prevKF[i] = (i % 5 == 0) ? 1.0 : 0.0;
+    for (int i = 0; i < 36; ++i) q.cov_prevKF_currF[i] = 0.0;
+}
+
 // offsets into SessionCall::meta
 size_t meta_named(const SessionCall& c) { return 2 * (size_t)c.n; }
 size_t meta_others(const SessionCall& c) { return meta_named(c) + (size_t)c.n * (sizeof(GatherSeg) / 4); }
@@ -106,6 +155,23 @@ cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPose
                                    int32_t* th_next, PlPrior* priors, PlPoseResult* res_out, cudaStream_t s) {
     if (n <= 0) return cudaSuccess;
     session_handler_kernel<<<(n + 127) / 128, 128, 0, s>>>(h, n, results, th, th_next, priors, res_out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_session_schedule_gather(int n, const SchedEntry* e, const int32_t* th_slot, const PlPrior* prior_slot,
+                                           const PlKeyframeState* kfs_slot, int32_t* th, PlPrior* priors, PlKeyframeState* kfs,
+                                           cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    session_schedule_gather_kernel<<<(n + 127) / 128, 128, 0, s>>>(n, e, th_slot, prior_slot, kfs_slot, th, priors, kfs);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_session_schedule_update(int n, const SchedEntry* e, bool init, const int32_t* th_next, const PlPrior* priors,
+                                           const PlKeyframeState* kfs, int32_t* th_slot, PlPrior* prior_slot,
+                                           PlKeyframeState* kfs_slot, cudaStream_t s) {
+    if (n <= 0) return cudaSuccess;
+    session_schedule_update_kernel<<<(n + 127) / 128, 128, 0, s>>>(n, e, init, th_next, priors, kfs, th_slot, prior_slot,
+                                                                     kfs_slot);
     return cudaGetLastError();
 }
 

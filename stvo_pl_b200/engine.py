@@ -156,6 +156,9 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_stereo_session_run_keyframes": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), vp, C.c_int, i32p, C.c_int,
                                                           C.POINTER(T.PlStereoImages), i32p, vp, vp, vp, vp, i32p, i32p]),
         "plstvo_stereo_session_read_keyframes": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut), i32p]),
+        "plstvo_stereo_session_run_schedule": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), vp, C.c_int, i32p, C.c_int,
+                                                         C.POINTER(C.c_uint8), C.POINTER(T.PlStereoImages), i32p, vp, vp, vp,
+                                                         vp, i32p, i32p]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)   # AttributeError if the library does not export a declared symbol
@@ -189,7 +192,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams", "plstvo_default_handler_config",
     "plstvo_kitti_handler_config", "plstvo_stereo_session_run", "plstvo_default_keyframe_config",
     "plstvo_initial_keyframe_state", "plstvo_stereo_session_run_keyframes", "plstvo_stereo_session_read_keyframes",
-    "plstvo_fld_key_lines", "plstvo_stereo_session_use_fld_lines"]
+    "plstvo_fld_key_lines", "plstvo_stereo_session_use_fld_lines", "plstvo_stereo_session_run_schedule"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -295,6 +298,16 @@ class StereoSession:
         T.KEYFRAME_STATE_DTYPE record per stream (handler.KeyframeTest.to_state()), updated in place on success.  Returns
         (results [T_, n], kf [T_, n] of T.KEYFRAME_RESULT_DTYPE, fast_th [T_ + 1, n], n_stereo [T_, n, 4])."""
         return self.eng.stereo_session_run_keyframes(self, hcfg, kcfg, ids, T_, frames, kf_state, fast_th0, priors)
+
+    def run_schedule(self, hcfg, ids, schedule, frames: dict, fast_th0=None, priors=None, kcfg=None, kf_state=None):
+        """plstvo_stereo_session_run_schedule: run() / run_keyframes() over uneven streams.  schedule uint8 [T_, len(ids)]: 0
+        the stream idles at that step, 1 insert, 2 initialize; frames holds one frame per non-zero entry, step-major and in ids
+        order within a step (handler.schedule_frames packs them), fast_th optional (initialize entries' thresholds, 0 for
+        inserts).  kcfg None: no key-frame test (kf_state must be None); else kf_state as for run_keyframes, updated in place.
+        Returns (results [T_, n], fast_th [T_ + 1, n], n_stereo [T_, n, 4]), with kcfg (results, kf [T_, n], fast_th,
+        n_stereo); the rows of entries that are not inserts are zero in results and kf, and in n_stereo where the stream
+        idles."""
+        return self.eng.stereo_session_run_schedule(self, hcfg, ids, schedule, frames, fast_th0, priors, kcfg, kf_state)
 
     def read_keyframes(self):
         """plstvo_stereo_session_read_keyframes: (rows [n_kf, 4] of step, stream id, points, lines; pt; ls), pt / ls holding
@@ -1055,6 +1068,52 @@ class Engine:
         del keep
         ss.last = (True, n_stereo[-1].copy()) if T_ > 0 else last
         return results, kf, fast_th, n_stereo
+
+    def stereo_session_run_schedule(self, ss: StereoSession, hcfg, ids, schedule, frames: dict, fast_th0=None, priors=None,
+                                    kcfg=None, kf_state=None):
+        ss.check_frames(frames)
+        h = hcfg if isinstance(hcfg, T.PlHandlerConfig) else T.handler_config(hcfg)
+        ids = np.ascontiguousarray(ids, np.int32)
+        n = len(ids)
+        raw = np.asarray(schedule)
+        if raw.size and (not np.issubdtype(raw.dtype, np.integer) or raw.min() < 0 or raw.max() > 255):
+            raise ValueError("schedule: integers, 0 idle, 1 insert, 2 initialize (the library refuses other values)")
+        sched = np.ascontiguousarray(raw, np.uint8).reshape(-1, n) if n else np.zeros((len(raw), 0), np.uint8)
+        T_ = sched.shape[0]
+        fs, keep = T.stereo_images_as_c(frames)
+        th0 = None if fast_th0 is None else np.ascontiguousarray(fast_th0, np.int32).reshape(-1)
+        pri = None if priors is None else np.ascontiguousarray(priors, T.PRIOR_DTYPE).reshape(-1)
+        if (th0 is not None and len(th0) != n) or (pri is not None and len(pri) != n):
+            raise ValueError("fast_th0 and priors take one entry per stream of ids")
+        k = kf = None
+        if kcfg is not None:
+            k = (np.ascontiguousarray(kcfg, T.KEYFRAME_CONFIG_DTYPE).reshape(-1) if isinstance(kcfg, np.ndarray)
+                 else T.keyframe_config(kcfg))
+            if not (isinstance(kf_state, np.ndarray) and kf_state.dtype == T.KEYFRAME_STATE_DTYPE
+                    and kf_state.flags.c_contiguous and kf_state.size == n):
+                raise ValueError("kf_state: a contiguous T.KEYFRAME_STATE_DTYPE array of one entry per stream, updated in place")
+            kf = np.zeros((T_, n), dtype=T.KEYFRAME_RESULT_DTYPE)
+        elif kf_state is not None:
+            raise ValueError("kf_state without a key-frame config")
+        results = np.zeros((T_, n), dtype=T.POSE_RESULT_DTYPE)
+        fast_th = np.zeros((T_ + 1, n), np.int32)
+        n_stereo = np.zeros((T_, n, 4), np.int32)
+        last, ss.last = ss.last, None
+        self._ck(self.lib.plstvo_stereo_session_run_schedule(
+            self.ctx, ss.handle, C.byref(h), None if k is None else k.ctypes.data, n, _p(ids, T.c_int32_p), T_,
+            sched.ctypes.data_as(C.POINTER(C.c_uint8)), C.byref(fs), _p(th0, T.c_int32_p),
+            None if pri is None else pri.ctypes.data, None if kf_state is None else kf_state.ctypes.data,
+            results.ctypes.data, None if kf is None else kf.ctypes.data, _p(fast_th, T.c_int32_p), _p(n_stereo, T.c_int32_p)))
+        del keep
+        # read() returns the last step with entries as its last chain call (the insert where the step has both kinds)
+        steps = np.nonzero(sched.any(axis=1))[0]
+        if len(steps):
+            row = sched[steps[-1]]
+            ss.last = ((True, n_stereo[steps[-1]][row == 1].copy()) if (row == 1).any()
+                       else (False, n_stereo[steps[-1]][row == 2][:, 2:].copy()))
+        else:
+            ss.last = last
+        return (results, fast_th, n_stereo) if k is None else (results, kf, fast_th, n_stereo)
 
     def track_stereo_images_stage_times(self):
         """Device ms of the last images call: uploads, ORB, LBD (overlaps ORB; after the LSD form, the lines: LSD's first launch

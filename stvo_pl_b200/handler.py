@@ -255,3 +255,106 @@ class StereoFrameHandler:
         self.matched_pt = np.zeros(0, np.int64)
         self.matched_ls = np.zeros(0, np.int64)
         self.prev_frame, self.curr_frame = self.curr_frame, None
+
+
+# ---- scheduled session runs (plstvo_stereo_session_run_schedule): frames packing and the per-stream chain ----
+SCHEDULE_IDLE, SCHEDULE_INSERT, SCHEDULE_INITIALIZE = 0, 1, 2
+_LINE_SIDES = (("ll_off", "seg_l", "angle_l", "npix_l"), ("lr_off", "seg_r", "angle_r", "npix_r"))
+
+
+def take_frames(frames: dict, idx) -> dict:
+    """Frames idx (in that order) of a frames dict: images and fast_th sliced, and each side's key lines (FLD branch:
+    ll_off / seg_l / angle_l / npix_l and the right side's) cut per frame and re-based to one CSR."""
+    idx = np.asarray(idx, np.int64)
+    out = {k: np.asarray(frames[k])[idx] for k in ("img_l", "img_r")}
+    if frames.get("fast_th") is not None:
+        out["fast_th"] = np.asarray(frames["fast_th"], np.int32)[idx]
+    for off_k, seg_k, ang_k, npix_k in _LINE_SIDES:
+        if frames.get(off_k) is None:
+            continue
+        off = np.asarray(frames[off_k], np.int64)
+        rows = np.concatenate([np.arange(off[i], off[i + 1]) for i in idx]) if len(idx) else np.zeros(0, np.int64)
+        out[off_k] = np.concatenate([[0], np.cumsum(off[idx + 1] - off[idx])]).astype(np.int32)
+        out[seg_k] = np.asarray(frames[seg_k], np.float32).reshape(-1, 4)[rows]
+        out[ang_k] = np.asarray(frames[ang_k], np.float32)[rows]
+        out[npix_k] = np.asarray(frames[npix_k], np.int32)[rows]
+    return out
+
+
+def join_frames(parts) -> dict:
+    """The frames dicts parts concatenated in order (take_frames' keys), key lines re-based to one CSR per side."""
+    parts = list(parts)
+    out = {k: np.concatenate([np.asarray(p[k]) for p in parts]) for k in ("img_l", "img_r")}
+    if all(p.get("fast_th") is not None for p in parts) and parts:
+        out["fast_th"] = np.concatenate([np.asarray(p["fast_th"], np.int32) for p in parts])
+    for off_k, seg_k, ang_k, npix_k in _LINE_SIDES:
+        if not parts or parts[0].get(off_k) is None:
+            continue
+        counts = np.concatenate([np.diff(np.asarray(p[off_k], np.int64)) for p in parts])
+        out[off_k] = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+        out[seg_k] = np.concatenate([np.asarray(p[seg_k], np.float32).reshape(-1, 4) for p in parts])
+        out[ang_k] = np.concatenate([np.asarray(p[ang_k], np.float32) for p in parts])
+        out[npix_k] = np.concatenate([np.asarray(p[npix_k], np.int32) for p in parts])
+    return out
+
+
+def schedule_frames(schedule, frame_of) -> dict:
+    """The frames of a schedule [T, n], packed as plstvo_stereo_session_run_schedule takes them: one per non-zero entry,
+    step-major and in call order within a step.  frame_of(t, k) gives entry (t, k)'s frame as a one-frame dict."""
+    sched = np.asarray(schedule)
+    return join_frames(frame_of(t, k) for t in range(sched.shape[0]) for k in range(sched.shape[1]) if sched[t, k])
+
+
+def schedule_groups(schedule):
+    """Per step t, the chain's two calls: (t, initialize positions, insert positions, their frames' indices in the packed
+    frames, in the same order).  Steps with no entries are skipped."""
+    sched = np.asarray(schedule)
+    b, out = 0, []
+    for t in range(sched.shape[0]):
+        where = {}
+        for k in range(sched.shape[1]):
+            if sched[t, k]:
+                where[k] = b
+                b += 1
+        init = [k for k in where if sched[t, k] == SCHEDULE_INITIALIZE]
+        ins = [k for k in where if sched[t, k] == SCHEDULE_INSERT]
+        if where:
+            out.append((t, init, ins, [where[k] for k in init], [where[k] for k in ins]))
+    return out
+
+
+def fresh_prior() -> np.ndarray:
+    """priorOf of a freshly initialised frame (Tfw = I, Tfw_cov = I, DT = I, DT_cov = 0, err_norm = -1): one T.PRIOR_DTYPE."""
+    p = np.zeros(1, T.PRIOR_DTYPE)
+    p["Tfw"], p["Tfw_cov"], p["DT"], p["err_norm"] = np.eye(4), np.eye(6), np.eye(4), -1.0
+    return p
+
+
+class ScheduleStreams:
+    """The per-stream state a scheduled run carries, on the host: the FAST threshold the stream's next frame takes, its prior
+    and, with the key-frame test, its state.  An idle step changes nothing; initialize resets all three to what
+    HandlerState's initialize leaves; an insert takes them and leaves updateFrame's threshold, priorOf the published result
+    and the test's state (currFrameIsKF's Tfw = I, Tfw_cov = I where it fired)."""
+
+    def __init__(self, hcfg: HandlerConfig, th0, priors=None, kf_state=None):
+        self.hcfg = hcfg
+        self.th = np.asarray(th0, np.int32).copy()
+        n = len(self.th)
+        self.prior = np.repeat(fresh_prior(), n) if priors is None else np.array(priors, T.PRIOR_DTYPE).reshape(-1).copy()
+        self.kf = None if kf_state is None else np.array(kf_state, T.KEYFRAME_STATE_DTYPE).reshape(-1).copy()
+
+    def initialize(self, k: int, th: int):
+        self.th[k] = th
+        self.prior[k] = fresh_prior()[0]
+        if self.kf is not None:
+            self.kf[k] = KeyframeTest().to_state()[0]
+
+    def inserted(self, k: int, r, kf_state=None, new_kf: bool = False):
+        """Stream k's insert gave result r (and, with the test, the state after it and whether the frame became a key frame)."""
+        self.th[k] = update_fast_threshold(self.hcfg, int(self.th[k]), r["DT"], float(r["err_norm"]), int(r["n_inliers_pt"]))
+        for f in ("Tfw", "Tfw_cov", "DT", "DT_cov", "err_norm"):
+            self.prior[k][f] = r[f]
+        if self.kf is not None and kf_state is not None:
+            self.kf[k] = kf_state
+        if new_kf:
+            self.prior[k]["Tfw"], self.prior[k]["Tfw_cov"] = np.eye(4), np.eye(6)
