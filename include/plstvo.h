@@ -746,7 +746,11 @@ typedef struct PlKeyframeResult {
  * where kf[t][k].new_kf is 1, and that each step's results go through plstvo.hpp's KeyframeTest::needNewKF, starting from
  * kf_state[k].  Under it results (optimizePose's rows, Tfw before any reset), n_stereo and fast_th are byte for byte the
  * loop's; kf[t][k].new_kf and .N_prevKF_currF are the host test's; the four diagnostics agree with it to the last few ulps
- * (the device's log and acos are CUDA's); and kf_state comes back as the host test stands after step T - 1.
+ * (the device's log and acos are CUDA's); and kf_state comes back as the host test stands after step T - 1.  The decisions
+ * are held to the reference's own needNewKF, not only to the host test: wherever t, r and the entropy ratio lie outside the
+ * rounding band of their thresholds they are the exact ones, and on non-finite poses and covariances (a NaN cosine keeps
+ * r = 0; a zero pivot with inf or NaN below it gives a NaN determinant) they are the reference's.  Inside a band (a few ulps
+ * of fp64's log, acos and summation order) either decision may be taken.
  * A second call continues a first exactly when given fast_th0 = row T, the returned kf_state, and priors built from the last
  * results with that reset applied.
  * The test runs in session_keyframe_kernel, one thread per stream after session_handler_kernel: one launch per step more
@@ -1002,6 +1006,13 @@ int  plstvo_debug_algebra(PlContext* ctx, int n, const double* H, const double* 
 #define PLSTVO_PH_FIN_EIG 146
 #define PLSTVO_PH_OUT 152
 int  plstvo_debug_pose_helpers(PlContext* ctx, int n, const double* in, double* out);
+/* test hook: one launch of the key-frame test a session run with the test runs after each step (needNewKF, then
+ * currFrameIsKF where it fires), on n caller-placed streams.  Of results [n] only Tfw, DT and DT_cov are read; state [n] is
+ * read and written back (the next call continues from it); out [n] receives each stream's PlKeyframeResult; priors [n]
+ * (NULL: none read or returned) is read and written back, and a stream that fires has its Tfw and Tfw_cov set to I there.
+ * k is not checked (NaN thresholds included), so that a test may place any value. */
+int  plstvo_debug_keyframe(PlContext* ctx, const PlKeyframeConfig* k, int n, const PlPoseResult* results,
+                           PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors);
 /* POPC issue-rate micro-benchmark: returns 32-bit popcounts per second on this device */
 int  plstvo_popc_rate(PlContext* ctx, double* popc_per_s);
 

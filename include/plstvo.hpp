@@ -554,8 +554,12 @@ inline Mat4 inverse(const Mat4& T) {                     // inverse_se3: [R^T, -
 }
 inline Vec6 logmap(const Mat4& T) {                      // logmap_se3: x = [V^-1 t ; w]
     double cosine = (T[0] + T[5] + T[10] - 1.0) / 2.0;
-    cosine = std::min(1.0, std::max(-1.0, cosine));
-    const double sine = std::min(1.0, std::sqrt(1.0 - cosine * cosine)), theta = std::acos(cosine);
+    if (cosine > 1.0) cosine = 1.0;                      // the reference's clamps: a NaN cosine stays NaN (theta NaN, w = 0)
+    else if (cosine < -1.0) cosine = -1.0;
+    double sine = std::sqrt(1.0 - cosine * cosine);
+    if (sine > 1.0) sine = 1.0;
+    else if (sine < -1.0) sine = -1.0;
+    const double theta = std::acos(cosine);
     double w[3] = {0, 0, 0}, V[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
     if (theta > 0.000001) {
         const double k = theta / (2.0 * sine);
@@ -640,18 +644,18 @@ inline Mat4 expmap(const Vec6& x) {                      // expmap_se3 (src/auxi
     return Mat4{R[0], R[1], R[2], t[0], R[3], R[4], R[5], t[1], R[6], R[7], R[8], t[2], 0, 0, 0, 1};
 }
 inline Mat6 uncTinv(const Mat4& T, const Mat6& cov) { return sandwich(adjoint(inverse(T)), cov); }   // uncTinv_se3
-inline double det6(Mat6 A) {                             // Matrix6d::determinant (partial-pivot LU)
+inline double det6(Mat6 A) {                             // Matrix6d::determinant (partial-pivot LU, run to the end)
     double det = 1.0;
     for (int c = 0; c < 6; ++c) {
         int piv = c;
         for (int r = c + 1; r < 6; ++r)
             if (std::fabs(A[6 * r + c]) > std::fabs(A[6 * piv + c])) piv = r;
-        if (A[6 * piv + c] == 0.0) return 0.0;
         if (piv != c) {
             for (int j = 0; j < 6; ++j) std::swap(A[6 * c + j], A[6 * piv + j]);
             det = -det;
         }
         det *= A[6 * c + c];
+        if (A[6 * c + c] == 0.0) continue;               // a zero pivot skips its elimination; the product runs on
         for (int r = c + 1; r < 6; ++r) {
             const double f = A[6 * r + c] / A[6 * c + c];
             for (int j = c + 1; j < 6; ++j) A[6 * r + j] -= f * A[6 * c + j];

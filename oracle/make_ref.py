@@ -11,16 +11,17 @@ absent, and its CMake build is off limits).  Its pose path, however, only needs 
   3. writes oracle/_ref/libplstvo_ref.so, whose C entry points mirror the oracle's (oracle/plstvo_oracle.h).
 
 What is and is not the reference's code in that library: every line of optimizeFunctions, optimizeFunctionsRobust,
-gaussNewtonOptimization[Robust], removeOutliers, isGoodSolution, optimizePose, lineSegmentOverlap, projection, the
-SE(3) helpers and the MAD statistics IS the reference's text.  The dense 6x6 decompositions those lines call
-(ColPivHouseholderQR::solve / logAbsDeterminant, Matrix::inverse, SelfAdjointEigenSolver::eigenvalues) are the
-stand-in's, not Eigen's.
+gaussNewtonOptimization[Robust], removeOutliers, isGoodSolution, optimizePose, the key-frame test (needNewKF,
+currFrameIsKF), lineSegmentOverlap, projection, the SE(3) helpers and the MAD statistics IS the reference's text.  The dense
+6x6 decompositions those lines call (ColPivHouseholderQR::solve / logAbsDeterminant, Matrix::inverse, Matrix::determinant,
+SelfAdjointEigenSolver::eigenvalues) are the stand-in's, not Eigen's.
 
 Runs only where /root/reference exists (this container).  The GPU box uses the prebuilt .so that travels with the
 snapshot.  `python oracle/make_ref.py` builds; `--check` only verifies the ranges.
 """
 from __future__ import annotations
 
+import hashlib
 import os
 import re
 import subprocess
@@ -30,6 +31,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 REF = os.environ.get("PLSTVO_REFERENCE", "/root/reference")
 OUT = os.path.join(HERE, "_ref")
 LIB = os.path.join(OUT, "libplstvo_ref.so")
+STAMP = LIB + ".stamp"   # hash of the recipe the library was built from (see build())
 SHIM = os.path.join(HERE, "ref_shim")
 
 # (group, file, first line, last line, regex the first line must match)
@@ -56,6 +58,8 @@ RANGES = [
     ("handler", "src/stereoFrameHandler.cpp", 549, 694, r"^void StereoFrameHandler::optimizeFunctions\("),
     ("handler", "src/stereoFrameHandler.cpp", 696, 962, r"^void StereoFrameHandler::optimizeFunctionsRobust\("),
     ("handler", "src/stereoFrameHandler.cpp", 988, 1067, r"^void StereoFrameHandler::removeOutliers\("),
+    ("handler", "src/stereoFrameHandler.cpp", 1136, 1187, r"^bool StereoFrameHandler::needNewKF\(\)"),
+    ("handler", "src/stereoFrameHandler.cpp", 1189, 1218, r"^void StereoFrameHandler::currFrameIsKF\(\)"),
 ]
 
 
@@ -85,9 +89,29 @@ def available() -> bool:
     return os.path.isdir(os.path.join(REF, "src"))
 
 
+def recipe_hash() -> str:
+    """sha256 of everything the library is built from in this repository: the driver, the stand-ins, the C-ABI header it
+    marshals and this recipe (its RANGES).  A library is current only when its stamp holds this hash: file times say nothing
+    once a tree has been checked out or copied."""
+    h = hashlib.sha256()
+    for p in [os.path.join(SHIM, n) for n in ("ref_driver.cpp", "eigen_standin.h", "stvo_standin.h")] + \
+             [os.path.join(HERE, "..", "include", "plstvo.h"), os.path.abspath(__file__)]:
+        with open(p, "rb") as f:
+            h.update(f.read())
+    return h.hexdigest()
+
+
+def current() -> bool:
+    """The library exists and was built from this repository's recipe."""
+    try:
+        with open(STAMP) as f:
+            return os.path.exists(LIB) and f.read().strip() == recipe_hash()
+    except OSError:
+        return False
+
+
 def build(force: bool = False) -> str:
-    srcs = [os.path.join(SHIM, n) for n in ("ref_driver.cpp", "eigen_standin.h", "stvo_standin.h")] + [os.path.abspath(__file__)]
-    if not force and os.path.exists(LIB) and all(os.path.getmtime(s) <= os.path.getmtime(LIB) for s in srcs):
+    if not force and current():
         return LIB
     if not available():
         if os.path.exists(LIB):
@@ -105,6 +129,8 @@ def build(force: bool = False) -> str:
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("g++ failed: " + " ".join(cmd))
+    with open(STAMP, "w") as f:
+        f.write(recipe_hash() + "\n")
     return LIB
 
 

@@ -1638,12 +1638,12 @@ double orc_det6(const double Ain[36]) {   /* Eigen: PartialPivLU determinant for
         int piv = c;
         for (int r = c + 1; r < 6; ++r)
             if (fabs(A[6 * r + c]) > fabs(A[6 * piv + c])) piv = r;
-        if (A[6 * piv + c] == 0.0) return 0.0;
         if (piv != c) {
             for (int j = 0; j < 6; ++j) { double t = A[6 * c + j]; A[6 * c + j] = A[6 * piv + j]; A[6 * piv + j] = t; }
             det = -det;
         }
         det *= A[6 * c + c];
+        if (A[6 * c + c] == 0.0) continue;   /* a zero pivot skips its elimination; the product runs on (0 * inf = NaN) */
         for (int r = c + 1; r < 6; ++r) {
             const double f = A[6 * r + c] / A[6 * c + c];
             for (int j = c + 1; j < 6; ++j) A[6 * r + j] -= f * A[6 * c + j];

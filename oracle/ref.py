@@ -58,6 +58,12 @@ class Ref:
         L.ref_optimize_pose.restype = C.c_int
         L.ref_optimize_pose.argtypes = [C.POINTER(T.PlCamera), C.POINTER(T.PlConfig), C.POINTER(T.PlMatchedBatch),
                                         C.c_void_p, C.c_void_p, u8p, u8p]
+        # the key-frame entry exists only in a library built by the recipe that added it; a prebuilt library from an older
+        # recipe (where the reference is not at hand to rebuild it) still serves everything above
+        self.has_need_new_kf = hasattr(L, "ref_need_new_kf")
+        if self.has_need_new_kf:
+            L.ref_need_new_kf.restype = C.c_int
+            L.ref_need_new_kf.argtypes = [C.c_void_p, C.c_void_p, dp, dp, dp, C.c_void_p, dp, dp]
 
     @staticmethod
     def _d(a):
@@ -176,6 +182,26 @@ class Ref:
                                         inl_pt.ctypes.data_as(T.c_uint8_p), inl_ls.ctypes.data_as(T.c_uint8_p))
         return rc, res, inl_pt[:-1], inl_ls[:-1]
 
+    def need_new_kf(self, kcfg, state, Tfw, DT, DT_cov):
+        """StereoFrameHandler::needNewKF, then currFrameIsKF where it fires, on one frame from the handler state `state` (one
+        T.KEYFRAME_STATE_DTYPE record, updated in place).  Returns (T.KEYFRAME_RESULT_DTYPE record, the frame's Tfw and
+        Tfw_cov afterwards).  The diagnostics are the function's own printed values (17 digits); entropy_curr is NaN where it
+        fires (the reference does not print it there)."""
+        if not self.has_need_new_kf:
+            raise RuntimeError(f"{make_ref.LIB} was built without ref_need_new_kf; rebuild it with oracle/make_ref.py")
+        k = np.ascontiguousarray(kcfg, T.KEYFRAME_CONFIG_DTYPE).reshape(-1)
+        if not (isinstance(state, np.ndarray) and state.dtype == T.KEYFRAME_STATE_DTYPE and state.flags.c_contiguous
+                and state.size == 1):
+            raise ValueError("state: one contiguous T.KEYFRAME_STATE_DTYPE record, updated in place")
+        o = np.zeros(1, T.KEYFRAME_RESULT_DTYPE)
+        Tfw_out, cov_out = np.zeros(16), np.zeros(36)
+        a, b, c = self._d(Tfw).ravel(), self._d(DT).ravel(), self._d(DT_cov).ravel()
+        rc = self.lib.ref_need_new_kf(k.ctypes.data, state.ctypes.data, self._dp(a), self._dp(b), self._dp(c), o.ctypes.data,
+                                      self._dp(Tfw_out), self._dp(cov_out))
+        if rc:
+            raise RuntimeError("ref_need_new_kf could not read needNewKF's printed line")
+        return o[0], Tfw_out.reshape(4, 4), cov_out.reshape(6, 6)
+
 
 class Recorded:
     """The Ref surface served from stored answers: what the reference's code returned for each call a test made, recorded once
@@ -233,3 +259,4 @@ class Recorded:
             return tuple(vals) if e["tuple"] else vals[0]
 
         return call
+

@@ -5,7 +5,9 @@
 // oracle/make_ref.py from /root/reference by line range, never committed).  Entry points mirror oracle/plstvo_oracle.h
 // (orc_* -> ref_*) so tests/test_oracle_ref.py can feed both the same inputs.
 #include <cstdint>
+#include <cstdlib>
 #include <sstream>
+#include <string>
 
 #include "stvo_standin.h"
 #include "include/plstvo.h"
@@ -296,6 +298,62 @@ int ref_optimize_pose(const PlCamera* cam, const PlConfig* cfg, const PlMatchedB
             for (size_t i = 0; i < q.lns.size(); ++i) inlier_ls[matched->ls_off[p] + i] = q.lns[i].inlier;
     }
     return rc;
+}
+
+// StereoFrameHandler::needNewKF on one frame (Tfw, DT, DT_cov) from the handler state s, then currFrameIsKF where it fires;
+// s comes back as the handler's SLAM variables stand after both.  The function keeps its diagnostics in locals and only
+// prints them, so they are read back from its own cout line, printed at 17 significant digits (round-trip exact): o gets the
+// decision, N_prevKF_currF as needNewKF leaves it, and entropy_ratio, t, r; entropy_curr only where it does not fire (the
+// firing line leaves it out; NaN there).  Tfw_out / Tfw_cov_out (each may be NULL): the frame's Tfw, Tfw_cov afterwards
+// (Tfw_cov enters as zero).
+int ref_need_new_kf(const PlKeyframeConfig* k, PlKeyframeState* s, const double Tfw[16], const double DT[16],
+                    const double DT_cov[36], PlKeyframeResult* o, double Tfw_out[16], double Tfw_cov_out[36]) {
+    Config::minEntropyRatio() = k->min_entropy_ratio;
+    Config::maxKFTDist() = k->max_kf_t_dist;
+    Config::maxKFRDist() = k->max_kf_r_dist;
+    StereoFrame f;
+    f.Tfw = m4(Tfw);
+    f.DT = m4(DT);
+    f.DT_cov = m6(DT_cov);
+    f.Tfw_cov = Matrix6d::Zero();
+    StereoFrameHandler h;
+    h.curr_frame = &f;
+    h.prev_f_iskf = s->prev_f_iskf != 0;
+    h.entropy_first_prevKF = s->entropy_first_prevKF;
+    h.T_prevKF = m4(s->T_prevKF);
+    h.cov_prevKF_currF = m6(s->cov_prevKF_currF);
+    h.N_prevKF_currF = s->N_prevKF_currF;
+    bool kf;
+    std::string line;
+    {
+        Quiet quiet;
+        const std::streamsize prec = std::cout.precision(17);
+        kf = h.needNewKF();
+        std::cout.precision(prec);
+        line = quiet.sink.str();
+    }
+    o->new_kf = kf ? 1 : 0;
+    o->N_prevKF_currF = h.N_prevKF_currF;
+    // "Entropy ratio: ratio\tt r N" or "No new KF needed: ratio\tentropy_curr entropy_first det\tt r N"
+    const size_t colon = line.find(':');
+    if (colon == std::string::npos) return PLSTVO_E_INVALID;
+    std::istringstream in(line.substr(colon + 1));
+    std::vector<double> v;
+    for (std::string tok; in >> tok;) v.push_back(std::strtod(tok.c_str(), nullptr));
+    if (v.size() != (kf ? 4u : 7u)) return PLSTVO_E_INVALID;
+    o->entropy_ratio = v[0];
+    o->entropy_curr = kf ? std::numeric_limits<double>::quiet_NaN() : v[1];
+    o->t = v[kf ? 1 : 4];
+    o->r = v[kf ? 2 : 5];
+    if (kf) h.currFrameIsKF();
+    s->prev_f_iskf = h.prev_f_iskf ? 1 : 0;
+    s->entropy_first_prevKF = h.entropy_first_prevKF;
+    out(h.T_prevKF, s->T_prevKF);
+    out(h.cov_prevKF_currF, s->cov_prevKF_currF);
+    s->N_prevKF_currF = h.N_prevKF_currF;
+    if (Tfw_out) out(f.Tfw, Tfw_out);
+    if (Tfw_cov_out) out(f.Tfw_cov, Tfw_cov_out);
+    return 0;
 }
 
 }  // extern "C"

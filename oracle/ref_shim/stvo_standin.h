@@ -2,7 +2,7 @@
 //
 // TEST INFRASTRUCTURE (oracle/_ref).  OURS: only the members the pose path touches, with the reference's own names and
 // types (include/stereoFeatures.h:30-121, include/stereoFrame.h:85-103, include/stereoFrameHandler.h:53-98,
-// include/pinholeStereoCamera.h:75-88, include/config.h:39-105 of rubengooj/stvo-pl).  The function BODIES are not
+// include/pinholeStereoCamera.h:75-88, include/config.h:39-110 of rubengooj/stvo-pl).  CV_PI is OpenCV's literal.  The function BODIES are not
 // here: oracle/make_ref.py cuts them verbatim out of /root/reference into oracle/_ref/extracted_*.inc.
 #pragma once
 #include <iostream>
@@ -19,6 +19,7 @@ typedef Matrix<double, 6, 1> Vector6d;   // include/auxiliar.h:42-43
 typedef Matrix<double, 6, 6> Matrix6d;
 
 #define EIGEN_MAKE_ALIGNED_OPERATOR_NEW
+#define CV_PI 3.1415926535897932384626433832795   // opencv2/core/cvdef.h
 
 // ---- src/auxiliar.cpp free functions (bodies extracted) ----
 Matrix3d skew(Vector3d v);
@@ -48,10 +49,14 @@ public:
     static double& minError() { return getInstance().min_error; }
     static double& minErrorChange() { return getInstance().min_error_change; }
     static double& inlierK() { return getInstance().inlier_k; }
+    static double& minEntropyRatio() { return getInstance().min_entropy_ratio; }
+    static double& maxKFTDist() { return getInstance().max_kf_t_dist; }
+    static double& maxKFRDist() { return getInstance().max_kf_r_dist; }
     bool has_points = true, has_lines = true, use_motion_model = false;
     double homog_th = 1e-7;
     int min_features = 10, max_iters = 5, max_iters_ref = 10;
     double min_error = 1e-7, min_error_change = 1e-7, inlier_k = 4.0;
+    double min_entropy_ratio = 0.85, max_kf_t_dist = 5.0, max_kf_r_dist = 15.0;
 };
 
 class PinholeStereoCamera {
@@ -103,6 +108,8 @@ public:
     Matrix6d DT_cov;
     Vector6d DT_cov_eig;
     double err_norm;
+    vector<PointFeature*> stereo_pt;
+    vector<LineFeature*> stereo_ls;
 };
 
 class StereoFrameHandler {
@@ -115,6 +122,8 @@ public:
     void levenbergMarquardtOptimization(Matrix4d& DT, Matrix6d& DT_cov, double& err_, int max_iters);   // dead in the reference (mode == 0)
     void optimizeFunctions(Matrix4d DT, Matrix6d& H, Vector6d& g, double& e);
     void optimizeFunctionsRobust(Matrix4d DT, Matrix6d& H, Vector6d& g, double& e);
+    bool needNewKF();
+    void currFrameIsKF();
 
     list<PointFeature*> matched_pt;
     list<LineFeature*> matched_ls;
@@ -122,6 +131,13 @@ public:
     StereoFrame* curr_frame;
     PinholeStereoCamera* cam;
     int n_inliers, n_inliers_pt, n_inliers_ls;
+
+    // slam-specific variables (include/stereoFrameHandler.h:81-86)
+    bool prev_f_iskf;
+    double entropy_first_prevKF;
+    Matrix4d T_prevKF;
+    Matrix6d cov_prevKF_currF;
+    int N_prevKF_currF;
 };
 
 }  // namespace StVO

@@ -1118,6 +1118,30 @@ int plstvo_debug_pose_helpers(PlContext* ctx, int n, const double* in, double* o
     return 0;
 }
 
+int plstvo_debug_keyframe(PlContext* ctx, const PlKeyframeConfig* k, int n, const PlPoseResult* results, PlKeyframeState* state,
+                          PlKeyframeResult* out, PlPrior* priors) {
+    if (!ctx || !k || n < 0 || (n > 0 && (!results || !state || !out))) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (n == 0) return 0;
+    CK(ctx, cudaSetDevice(ctx->device));
+    Arena a;
+    const size_t o_res = a.take((size_t)n * sizeof(PlPoseResult)), o_st = a.take((size_t)n * sizeof(PlKeyframeState)),
+                 o_out = a.take((size_t)n * sizeof(PlKeyframeResult)), o_pri = a.take((size_t)n * sizeof(PlPrior));
+    CK(ctx, a.alloc(ctx->scratch));
+    cudaStream_t s = ctx->s_main;
+    CK(ctx, a.up(o_res, results, (size_t)n * sizeof(PlPoseResult), s));
+    CK(ctx, a.up(o_st, state, (size_t)n * sizeof(PlKeyframeState), s));
+    CK(ctx, a.up(o_pri, priors, (size_t)n * sizeof(PlPrior), s));
+    CK(ctx, launch_session_keyframe(*k, keyframe_k_entropy(), n, a.at<PlPoseResult>(o_res), a.at<PlKeyframeState>(o_st),
+                                    a.at<PlKeyframeResult>(o_out), a.at<PlPrior>(o_pri), s));
+    ctx->launches++;
+    CK(ctx, a.down(state, o_st, (size_t)n * sizeof(PlKeyframeState), s));
+    CK(ctx, a.down(out, o_out, (size_t)n * sizeof(PlKeyframeResult), s));
+    CK(ctx, a.down(priors, o_pri, (size_t)n * sizeof(PlPrior), s));
+    CK(ctx, cudaStreamSynchronize(s));
+    return 0;
+}
+
 int plstvo_popc_rate(PlContext* ctx, double* popc_per_s) {
     if (!ctx || !popc_per_s) return PLSTVO_E_INVALID;
     LOCK(ctx);

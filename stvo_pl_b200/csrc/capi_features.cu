@@ -1660,7 +1660,7 @@ int session_run(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig* h, i
     CK(ctx, a.alloc(ctx->arena_run));
     CK(ctx, a.up(o_th, th0.data(), th0.size() * 4, s));
     if (kc) CK(ctx, a.up(o_kfs, kf_state, (size_t)n * sizeof(PlKeyframeState), s));
-    const double k_entropy = 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0)));   // KeyframeTest::needNewKF's constant
+    const double k_entropy = keyframe_k_entropy();
     std::vector<GatherSeg> kf_segs(kc && keep ? (size_t)T * n : 0);   // [T][n], as uploaded
     const int32_t* d_th = a.i32(o_th);
     const int ch = rect ? rect->channels : 1;
@@ -2031,7 +2031,7 @@ int session_schedule(PlContext* ctx, PlStereoSession* ss, const PlHandlerConfig*
         ms[k] += v;
         return 0;
     };
-    const double k_entropy = 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0)));   // KeyframeTest::needNewKF's constant
+    const double k_entropy = keyframe_k_entropy();
     std::vector<GatherSeg> kf_segs(kc && keep ? (size_t)n_ins : 0);   // [n_ins], as uploaded
     const LineBlocks no_lines;
     std::vector<int32_t> none((size_t)max_e + 1, 0), pl_off, pr_off, l_off, r_off, ns((size_t)4 * max_e);

@@ -4,6 +4,7 @@
 #pragma once
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <functional>
 #include <initializer_list>
@@ -537,6 +538,9 @@ cudaError_t launch_session_handler(const PlHandlerConfig& h, int n, const PlPose
 // update) take Tfw = I, Tfw_cov = I.  k_entropy = 3 (1 + log 2 pi), as the host computes it.
 cudaError_t launch_session_keyframe(const PlKeyframeConfig& cfg, double k_entropy, int n, const PlPoseResult* results,
                                     PlKeyframeState* state, PlKeyframeResult* out, PlPrior* priors, cudaStream_t s);
+// KeyframeTest::needNewKF's constant 3 (1 + log 2 pi) (src/stereoFrameHandler.cpp:1144, :1165), as the host computes it: the
+// one value every launch_session_keyframe caller passes
+inline double keyframe_k_entropy() { return 3.0 * (1.0 + std::log(2.0 * std::acos(-1.0))); }
 // plstvo_stereo_session_run_schedule: one entry of a step's initialize or insert group, the call position of its stream
 // (its state slot) and, for an initialize, the threshold its frame is detected with
 struct SchedEntry {

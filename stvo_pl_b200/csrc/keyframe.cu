@@ -6,7 +6,10 @@
 // with its pivoting, loop order and divisions.  Each a * b + c is spelled __dadd_rn(__dmul_rn(a, b), c) so that nvcc forms
 // no FMA (the host rounds the product and the sum apart).  Division and sqrt are IEEE-rounded on both sides.  The only
 // operations left that can differ from the host are CUDA's log (of the two determinants) and acos (in logmap); the constant
-// 3 (1 + log 2 pi) is computed on the host and passed in.
+// 3 (1 + log 2 pi) is computed on the host and passed in.  Non-finite inputs take the reference's paths: logmap's clamps
+// keep a NaN cosine (r = 0), and det6 runs its LU to the end past a zero pivot (0 * inf = NaN).
+// tests/test_gpu_keyframe_decisions.py holds the kernel, through plstvo_debug_keyframe, to the reference's own needNewKF
+// and to a 60-digit restatement (tests/hp_keyframe.py) at its thresholds.
 #include "host.cuh"
 
 namespace plstvo {
@@ -44,10 +47,11 @@ __device__ void inverse4(const double* T, double* Ti) {
 // se3::logmap: x = [V^-1 t ; w]
 __device__ void logmap(const double* T, double* x) {
     double cosine = sub(add(add(T[0], T[5]), T[10]), 1.0) / 2.0;
-    cosine = (-1.0 < cosine) ? cosine : -1.0;   // std::max(-1.0, c), then std::min(1.0, c): NaN becomes -1 as on the host
-    cosine = (cosine < 1.0) ? cosine : 1.0;
+    if (cosine > 1.0) cosine = 1.0;              // the reference's if / else if: a NaN cosine stays NaN, so theta is NaN,
+    else if (cosine < -1.0) cosine = -1.0;       // the branch below is skipped, w = 0 and V = I
     double sine = sqrt(sub(1.0, mul(cosine, cosine)));
-    sine = (sine < 1.0) ? sine : 1.0;
+    if (sine > 1.0) sine = 1.0;
+    else if (sine < -1.0) sine = -1.0;
     const double theta = acos(cosine);   // CUDA's acos: may differ from the host's in the last ulp
     double w[3] = {0, 0, 0}, V[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
     if (theta > 0.000001) {
@@ -104,14 +108,14 @@ __device__ void sandwich(const double* A, const double* C, double* AC, double* o
             out[6 * i + j] = acc;
         }
 }
-// se3::det6: partial-pivot LU on a copy (A is overwritten)
+// se3::det6: partial-pivot LU on a copy (A is overwritten).  A zero pivot skips its column's elimination and the product
+// runs on over the whole diagonal, as Matrix6d::determinant's LU does: a zero pivot with an inf or NaN further down gives NaN
 __device__ double det6(double* A) {
     double det = 1.0;
     for (int c = 0; c < 6; ++c) {
         int piv = c;
         for (int r = c + 1; r < 6; ++r)
             if (fabs(A[6 * r + c]) > fabs(A[6 * piv + c])) piv = r;
-        if (A[6 * piv + c] == 0.0) return 0.0;
         if (piv != c) {
             for (int j = 0; j < 6; ++j) {
                 const double v = A[6 * c + j];
@@ -121,6 +125,7 @@ __device__ double det6(double* A) {
             det = -det;
         }
         det = mul(det, A[6 * c + c]);
+        if (A[6 * c + c] == 0.0) continue;
         for (int r = c + 1; r < 6; ++r) {
             const double f = A[6 * r + c] / A[6 * c + c];
             for (int j = c + 1; j < 6; ++j) A[6 * r + j] = sub(A[6 * r + j], mul(f, A[6 * c + j]));

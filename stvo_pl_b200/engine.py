@@ -89,6 +89,7 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_popc_rate": (C.c_int, [vp, dp]),
         "plstvo_debug_algebra": (C.c_int, [vp, C.c_int, dp, dp, dp, dp, dp, dp]),
         "plstvo_debug_pose_helpers": (C.c_int, [vp, C.c_int, dp, dp]),
+        "plstvo_debug_keyframe": (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp]),
         "plstvo_debug_select": (C.c_int, [vp, C.c_int, i32p, dp, i32p, dp, C.c_int, dp]),
         "plstvo_debug_tc_partials": (C.c_int, [vp, C.c_int, u8p, i32p, u8p, i32p, C.c_float, u32p, u32p, u32p, u32p]),
         "plstvo_debug_color_planes": (C.c_int, [vp, vp, C.POINTER(vp), C.c_int, u8p, u8p, u8p, u8p]),
@@ -178,7 +179,7 @@ EXPORTED_SYMBOLS = [
     "plstvo_host_alloc", "plstvo_host_free", "plstvo_launch_count", "plstvo_batch_kernel_times", "plstvo_batch_stage_times",
     "plstvo_batch_phase_cycles",
     "plstvo_gn_eval_stream", "plstvo_popc_rate", "plstvo_debug_algebra", "plstvo_debug_pose_helpers",
-    "plstvo_debug_select", "plstvo_debug_tc_partials", "plstvo_debug_color_planes",
+    "plstvo_debug_keyframe", "plstvo_debug_select", "plstvo_debug_tc_partials", "plstvo_debug_color_planes",
     "plstvo_default_orb_config", "plstvo_orb_compute_batch", "plstvo_orb_kernel_times",
     "plstvo_default_orb_detect_config", "plstvo_orb_detect_and_compute_batch", "plstvo_orb_detect_kernel_times",
     "plstvo_lbd_compute_batch", "plstvo_lbd_kernel_times", "plstvo_default_lsd_config", "plstvo_lsd_detect_batch",
@@ -1306,6 +1307,24 @@ class Engine:
             res[name] = v.astype(bool) if name in ("chol_ok", "chol0_ok", "regs_ok", "surely", "good_fast", "good_full",
                                                    "fin_good") else v
         return res
+
+    def debug_keyframe(self, kcfg, results, state, priors=None):
+        """One launch of the session run's key-frame test (test hook) on n placed streams: kcfg one T.KEYFRAME_CONFIG_DTYPE
+        record (not checked), results [n] of T.POSE_RESULT_DTYPE (Tfw, DT and DT_cov read), state [n] of
+        T.KEYFRAME_STATE_DTYPE updated in place, priors None or [n] of T.PRIOR_DTYPE updated in place (a stream that fires
+        takes Tfw = I, Tfw_cov = I).  Returns the [n] T.KEYFRAME_RESULT_DTYPE rows."""
+        k = np.ascontiguousarray(kcfg, T.KEYFRAME_CONFIG_DTYPE).reshape(-1)
+        res = np.ascontiguousarray(results, T.POSE_RESULT_DTYPE).reshape(-1)
+        n = len(res)
+        for name, a, dt in (("state", state, T.KEYFRAME_STATE_DTYPE), ("priors", priors, T.PRIOR_DTYPE)):
+            if a is not None and not (isinstance(a, np.ndarray) and a.dtype == dt and a.flags.c_contiguous and a.size == n):
+                raise ValueError(f"{name}: a contiguous array of {n} {dt} records, updated in place")
+        if state is None:
+            raise ValueError("state: one T.KEYFRAME_STATE_DTYPE record per stream")
+        out = np.zeros(n, T.KEYFRAME_RESULT_DTYPE)
+        self._ck(self.lib.plstvo_debug_keyframe(self.ctx, k.ctypes.data, n, res.ctypes.data, state.ctypes.data, out.ctypes.data,
+                                                None if priors is None else priors.ctypes.data))
+        return out
 
     def synchronize(self):
         self._ck(self.lib.plstvo_synchronize(self.ctx))

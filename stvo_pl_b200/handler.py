@@ -68,8 +68,14 @@ def _adjoint_se3(T):
 def _logmap_se3(T):
     """src/auxiliar.cpp:143-173."""
     R = T[:3, :3]
-    cosine = min(1.0, max(-1.0, (np.trace(R) - 1.0) / 2.0))
-    sine = min(1.0, np.sqrt(1.0 - cosine * cosine))
+    cosine = (np.trace(R) - 1.0) / 2.0
+    if cosine > 1.0:                   # the reference's if / else if: a NaN cosine stays NaN (theta NaN, w = 0, V = I)
+        cosine = 1.0
+    elif cosine < -1.0:
+        cosine = -1.0
+    sine = np.sqrt(1.0 - cosine * cosine)
+    if sine > 1.0:
+        sine = 1.0
     theta = np.arccos(cosine)
     w, V = np.zeros(3), np.eye(3)
     if theta > 1e-6:
@@ -78,6 +84,28 @@ def _logmap_se3(T):
         s = _skew(w) / theta
         V = np.eye(3) + s * (1.0 - cosine) / theta + s @ s * (theta - sine) / theta
     return np.concatenate([np.linalg.solve(V, T[:3, 3]), w])
+
+
+def _det6(A):
+    """Matrix6d::determinant: partial-pivot LU in the order plstvo.hpp's se3::det6 takes.  A zero pivot skips its column's
+    elimination and the product runs on over the whole diagonal (so a zero pivot with an inf or NaN further down is NaN)."""
+    A = np.array(A, np.float64).reshape(6, 6)
+    det = 1.0
+    for c in range(6):
+        piv = c
+        for r in range(c + 1, 6):
+            if abs(A[r, c]) > abs(A[piv, c]):
+                piv = r
+        if piv != c:
+            A[[c, piv]] = A[[piv, c]]
+            det = -det
+        det *= A[c, c]
+        if A[c, c] == 0.0:
+            continue
+        for r in range(c + 1, 6):
+            f = A[r, c] / A[c, c]
+            A[r, c + 1:] -= f * A[c, c + 1:]
+    return float(det)
 
 
 def chain_poses(results, Tfw0=None, cov0=None):
@@ -113,7 +141,7 @@ class KeyframeTest:
         Tfw, DT, DT_cov = np.asarray(Tfw).reshape(4, 4), np.asarray(DT).reshape(4, 4), np.asarray(DT_cov).reshape(6, 6)
         with np.errstate(all="ignore"):
             if self.prev_f_iskf:
-                d = np.linalg.det(DT_cov)
+                d = _det6(DT_cov)
                 self.entropy_first_prevKF = self.K_ENTROPY + 0.5 * np.log(d) if d != 0.0 else -999999999.99
                 self.prev_f_iskf = False
             dX = _logmap_se3(_inverse_se3(Tfw) @ self.T_prevKF)
@@ -122,7 +150,7 @@ class KeyframeTest:
             adj_inv = _adjoint_se3(_inverse_se3(DT))
             adj_kf = _adjoint_se3(self.T_prevKF)
             self.cov_prevKF_currF = self.cov_prevKF_currF + adj_kf @ (adj_inv @ DT_cov @ adj_inv.T) @ adj_kf.T
-            self.entropy_curr = float(self.K_ENTROPY + 0.5 * np.log(np.linalg.det(self.cov_prevKF_currF)))
+            self.entropy_curr = float(self.K_ENTROPY + 0.5 * np.log(_det6(self.cov_prevKF_currF)))
             self.entropy_ratio = float(self.entropy_curr / self.entropy_first_prevKF)
         degenerate = not DT_cov.any() and np.array_equal(DT, np.eye(4))
         if (self.entropy_ratio < c.min_entropy_ratio or not np.isfinite(self.entropy_ratio) or degenerate
