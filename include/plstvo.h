@@ -665,6 +665,30 @@ int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* s, int on);
  * succeeded since retention was turned on, or the last call on the session failed (any failed call discards what was
  * retained, so a read never mixes two calls). */
 int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* s, const PlStereoFrameOut* out);
+/* ---- drawing each new frame: StereoFrame::plotStereoFrame (src/stereoFrame.cpp:618-663), the image app/imagesStVO.cpp:109
+ * hands its scene ----
+ * Plot switch, off at creation.  on != 0 requires retention on (PLSTVO_E_INVALID otherwise) and takes effect from the next
+ * _initialize / _insert: each successful call then also draws, for each new frame in call order, the image the reference's
+ * curr_frame->plotStereoFrame() returns for it: the frame's left image after the session's rectification (its stream's
+ * rectifier on a _create_cams session) in BGR (a grey image replicated, as cvtColor(GRAY2BGR); BGRA with alpha dropped, as
+ * cvtColor(BGRA2BGR)), then cv::circle(img, Point(int(pl.x), int(pl.y)), 3, Scalar(0, 200, 0), 1) for every row of pt_pl
+ * and cv::line(img, Point(int(spl.x), int(spl.y)), Point(int(epl.x), int(epl.y)), Scalar(0, 200, 0), 1) for every row of
+ * ls_spl / ls_epl that plstvo_stereo_session_read returns for the call, both LINE_8, byte for byte with OpenCV 4.13 (clipped
+ * at the border, each line drawn from spl to epl).  It costs one base-image launch and, where the call has a point or a line,
+ * one drawing launch per call, and a session-owned arena of 3 bytes per pixel per new frame (counted by
+ * plstvo_stereo_session_device_bytes), plus 16 bytes per new frame for a colour session's map table and, where no stage of
+ * the call reads the images on the device (a grey session without a rectifier and with has_points 0), 1 byte per pixel per
+ * new frame for their upload.  With plotting on the call's frames must hold both images (PLSTVO_E_INVALID otherwise), even
+ * where has_points and has_lines are 0.  on == 0 frees the arena at once, as does retention off, which also turns plotting
+ * off; with plotting off a call's launches, device memory and results are those of a session never switched on, and with
+ * it on its results, n_stereo and _read rows are the same.  _run, _run_keyframes and _run_schedule draw nothing.  Returns
+ * 0, or PLSTVO_E_INVALID for a null or foreign session or retention off. */
+int plstvo_stereo_session_plot(PlContext* ctx, PlStereoSession* s, int on);
+/* Copies the last call's images, [n][height][width][3] BGR bytes in call order, into out and returns that call's n.
+ * PLSTVO_E_INVALID: ctx, s or out null, a session of another context, plotting off, no _initialize / _insert succeeded
+ * since plotting was turned on, the last call on the session failed, or it was a run (every run, even of T = 0, discards the
+ * last plot, as any failed call does). */
+int plstvo_stereo_session_read_plot(PlContext* ctx, const PlStereoSession* s, uint8_t* out /* [n][height][width][3] */);
 
 /* ---- running the handler's frame loop over many frames per stream in one call (app/imagesStVO.cpp:88-124) ----
  * The Config values of updateFrame's adaptive FAST threshold (include/config.h:50, :67-71; src/config.cpp:52, :72-76).

@@ -952,6 +952,18 @@ public:
     void useFLDLines(bool on) { c_.check(plstvo_stereo_session_use_fld_lines(c_.get(), s_, on ? 1 : 0)); }
     // plstvo_stereo_session_retain: keep each following call's frames and matches for read() (off frees them)
     void retain(bool on) { c_.check(plstvo_stereo_session_retain(c_.get(), s_, on ? 1 : 0)); }
+    // plstvo_stereo_session_plot: draw each following initialize / insert's plotStereoFrame images for readPlot() (retention
+    // must be on; off frees them)
+    void plot(bool on) { c_.check(plstvo_stereo_session_plot(c_.get(), s_, on ? 1 : 0)); }
+    // plstvo_stereo_session_read_plot of the last initialize / insert: n images of [height][width][3] BGR bytes into out,
+    // sized from that call's n; returns n
+    int readPlot(int n, int width, int height, std::vector<uint8_t>& out) const {
+        out.resize((size_t)std::max(n, 1) * width * height * 3);
+        if (c_.check(plstvo_stereo_session_read_plot(c_.get(), s_, out.data())) != n)
+            throw Error(PLSTVO_E_INVALID, "StereoSession::readPlot: n differs from the last call's");
+        out.resize((size_t)n * width * height * 3);
+        return n;
+    }
     // plstvo_stereo_session_read of the last call, into out's vectors sized from that call's n and n_stereo ([n][2] after an
     // initialize, [n][4] after an insert, as the call wrote it); out.m12_* / inlier_* are emptied after an initialize
     struct Frames {
@@ -1183,14 +1195,28 @@ public:
             session_.read(1, ns, false, read_);
             detail::splitRead(read_, ns, 2, {this}, &HandlerState::prev_frame);
         }
+        if (plot_) session_.readPlot(1, cam_.width, cam_.height, plot_img_);
         has_prev_ = true;
     }
     // keep each frame's stereo features and the matches on the host after every call (off by default); effective from the
     // next initialize / insertStereoPair
     void keepFeatures(bool on) {
-        session_.retain(on);
+        session_.retain(on || plot_);   // plotting draws the retained rows
         keep_ = on;
     }
+    // draw each new frame's plotStereoFrame() image on the device after every call (off by default); effective from the next
+    // initialize / insertStereoPair
+    void plotFrames(bool on) {
+        if (on) session_.retain(true);
+        session_.plot(on);
+        if (!on && !keep_) session_.retain(false);
+        plot_ = on;
+        plot_img_.clear();
+    }
+    // StereoFrame::plotStereoFrame() of the frame the last initialize / insertStereoPair produced, as app/imagesStVO.cpp:109
+    // hands it to its scene: [height][width][3] BGR bytes, the rectified left image with the stereo points' circles and the
+    // stereo lines in (0, 200, 0).  Empty with plotFrames off.
+    const std::vector<uint8_t>& plotStereoFrame() const { return plot_img_; }
     void insertStereoPair(const uint8_t* img_l, const uint8_t* img_r, int idx = 0) {   // :54-60
         if (!has_prev_) throw Error(PLSTVO_E_INVALID, "initialize() first");
         images(img_l, img_r);
@@ -1209,6 +1235,7 @@ public:
             session_.read(1, n_stereo.data(), true, read_);
             detail::splitRead(read_, n_stereo.data(), 4, {this}, &HandlerState::curr_frame);
         }
+        if (plot_) session_.readPlot(1, cam_.width, cam_.height, plot_img_);
         tracked(result_);
     }
     void optimizePose() { HandlerState::optimizePose(result_); }
@@ -1233,6 +1260,8 @@ private:
     int32_t th_ = 0;
     bool has_prev_ = false;
     bool keep_ = false;
+    bool plot_ = false;
+    std::vector<uint8_t> plot_img_;
     StereoSession::Frames read_;
 };
 
@@ -1247,6 +1276,7 @@ public:
         std::array<int32_t, 4> n_stereo{};               // stereo points, lines of prev, then of curr, in the stream's last insert
         PlPoseResult result{};
         bool has_prev = false;
+        std::vector<uint8_t> plot;                       // plotFrames: the image of the stream's last initialize / insert
     };
     StereoStreamsHandler(Context& ctx, const PlCamera& cam, const PlConfig& cfg, const PlStereoMatchConfig& mc,
                          const PlStereoConfig& sc, const PlOrbDetectConfig& oc, const PlLsdConfig& lc, int n_streams,
@@ -1379,6 +1409,7 @@ private:
                      std::vector<PlPoseResult>* results, std::vector<PlKeyframeResult>* kf) {
         const char* who = "StereoStreamsHandler::insertStereoSequences";
         const size_t n = ids.size(), T = schedule.size();
+        clearPlots(ids);
         if (img_l.size() != T || img_r.size() != T) throw Error(PLSTVO_E_INVALID, std::string(who) + ": one image list per step");
         std::vector<int32_t> th0, th_init;
         std::vector<PlPrior> priors;
@@ -1504,6 +1535,7 @@ private:
             s.has_prev = true;
         }
         if (keep_) detail::splitRead(read_, ns.data(), 2, named(ids), &HandlerState::prev_frame);
+        splitPlot(ids);
     }
     void insertStereoPairs(const std::vector<int32_t>& ids, const std::vector<const uint8_t*>& img_l,
                            const std::vector<const uint8_t*>& img_r, const std::vector<Segments>* fl,
@@ -1531,6 +1563,20 @@ private:
             s.tracked(s.result);
         }
         if (keep_) detail::splitRead(read_, ns.data(), 4, named(ids), &HandlerState::curr_frame);
+        splitPlot(ids);
+    }
+    // a run draws nothing: the streams it names lose their last image
+    void clearPlots(const std::vector<int32_t>& ids) {
+        for (int32_t id : ids)
+            if (id >= 0 && (size_t)id < streams_.size()) streams_[(size_t)id].plot.clear();
+    }
+    // plotFrames: the last call's images into the named streams' plot, in call order
+    void splitPlot(const std::vector<int32_t>& ids) {
+        if (!plot_) return;
+        const size_t px = (size_t)cam_.width * cam_.height * 3;
+        session_.readPlot((int)ids.size(), cam_.width, cam_.height, plot_read_);
+        for (size_t k = 0; k < ids.size(); ++k)
+            streams_[(size_t)ids[k]].plot.assign(plot_read_.begin() + k * px, plot_read_.begin() + (k + 1) * px);
     }
 
 public:
@@ -1542,9 +1588,21 @@ public:
     // StereoImageHandler::keepFeatures for every stream: initialize fills the named streams' prev_frame arrays,
     // insertStereoPairs their curr_frame arrays and matches_pt / _ls, inlier_pt / _ls
     void keepFeatures(bool on) {
-        session_.retain(on);
+        session_.retain(on || plot_);   // plotting draws the retained rows
         keep_ = on;
     }
+    // StereoImageHandler::plotFrames for every stream: initialize and insertStereoPairs fill the named streams' images; the
+    // insertStereoSequences overloads draw nothing and clear the images of the streams they name
+    void plotFrames(bool on) {
+        if (on) session_.retain(true);
+        session_.plot(on);
+        if (!on && !keep_) session_.retain(false);
+        plot_ = on;
+        for (Stream& s : streams_) s.plot.clear();
+    }
+    // StereoImageHandler::plotStereoFrame() of stream id: the image of the frame its last initialize / insertStereoPairs
+    // produced ([height][width][3] BGR bytes; empty with plotFrames off, or after an insertStereoSequences naming it)
+    const std::vector<uint8_t>& plotStereoFrame(int id) { return at(id).plot; }
     Stream& stream(int id) { return at(id); }
     int streams() const { return (int)streams_.size(); }
     const StereoSession& session() const { return session_; }
@@ -1557,6 +1615,7 @@ private:
              const std::vector<std::vector<Segments>>* fr, std::vector<PlPoseResult>* results,
              std::vector<PlKeyframeResult>* kf, std::vector<KeyFrame>* keyframes) {
         const size_t n = ids.size(), T = img_l.size();
+        clearPlots(ids);
         if (img_r.size() != T) throw Error(PLSTVO_E_INVALID, "StereoStreamsHandler::insertStereoSequences: T differs between sides");
         std::vector<int32_t> th0;
         std::vector<PlPrior> priors;
@@ -1669,6 +1728,8 @@ private:
     detail::StereoImagesBatch pack_;
     bool keep_ = false;
     StereoSession::Frames read_;
+    bool plot_ = false;
+    std::vector<uint8_t> plot_read_;
 };
 
 }  // namespace plstvo

@@ -14,8 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libplstvo_b200.so")
 SOURCES = ["match.cu", "match_tc.cu", "match_grid.cu", "lift.cu", "solve.cu", "gn_stream.cu", "orb.cu", "lbd.cu", "lsd.cu", "rectify.cu", "session.cu", "keyframe.cu", "capi.cu", "capi_stereo.cu",
-           "capi_features.cu"]
-HEADERS = ["common.cuh", "records.h", "host.cuh", "match_finalize.cuh", "match_tc.cuh", "gn_stream.cuh", "orb_pattern.h", os.path.join("..", "..", "include", "plstvo.h")]
+           "capi_features.cu", "plot.cu"]
+HEADERS = ["common.cuh", "records.h", "host.cuh", "match_finalize.cuh", "match_tc.cuh", "gn_stream.cuh", "orb_pattern.h", "remap.cuh", os.path.join("..", "..", "include", "plstvo.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "--use_fast_math=false"]
 

@@ -345,6 +345,7 @@ struct OrbDetected {
     const float *xy = nullptr, *angle = nullptr, *response = nullptr;
     const int32_t* octave = nullptr;
     const uint8_t* desc = nullptr;
+    const uint8_t* images = nullptr;   // the grey device images ORB read (written on s_main)
 };
 
 // Enqueues detection and description of n_img (> 0) images on s_main, for a checked config and per-image FAST thresholds th
@@ -403,6 +404,7 @@ int orb_detect_enqueue(PlContext* ctx, const PlOrbDetectConfig* cfg, int n_img, 
     CK(ctx, a.alloc(ctx->arena_orb));
     cudaStream_t s = ctx->s_main;
     const uint8_t* img = d_img ? d_img : a.u8(o_img);
+    out.images = img;
     if (!d_img) {
         size_t o = o_img;
         for (const ImgPart& ip : parts) {
@@ -1073,14 +1075,15 @@ int images_check(PlContext* ctx, int W, int H, bool pts, bool lns, const PlStere
 // colour conversion of rect, or in a session call with per-stream rectifiers, stream ids[k]'s rectifier for image k of each
 // block.  A colour session on the FLD branch with lines also gets the RGB2GRAY plane LBD reads (*d_lbd; else null).
 int rectify_call(PlContext* ctx, const PlRectifier* rect, const SessionCall* call, int n, int n_img,
-                 const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out, const uint8_t** d_lbd) {
+                 const std::vector<ImgPart>& parts, cudaStream_t s, const uint8_t** d_out, const uint8_t** d_lbd,
+                 const uint8_t** d_raw = nullptr) {
     const PlStereoSession* ss = call ? call->ss : nullptr;
     std::vector<const PlRectifier*> call_rects;   // a session's per-stream rectifiers, call order
     if (ss && !ss->rects.empty())
         for (int k = 0; k < n; ++k) call_rects.push_back(ss->rects[(size_t)call->ids[k]]);
     const bool rgb = ss && ss->fld && ss->cfg.has_lines && rect->channels > 1;
     return rectify_enqueue(ctx, rect, n_img, n, parts, s, d_out, call_rects.empty() ? nullptr : call_rects.data(),
-                           rgb ? d_lbd : nullptr);
+                           rgb ? d_lbd : nullptr, d_raw);
 }
 }  // namespace
 
@@ -1116,8 +1119,10 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     const int nblk = 2 * nfs, n_img = nblk * NF;
     LineBlocks lines;   // key lines per image block: one frame set's left, right images
     LsdLaunch lsd{};
+    const bool plot = call && call->plot;
     if (NF > 0) {
         if (const int rc = images_check(ctx, W, H, pts, lns, fs, nfs, run_lsd ? lc : nullptr, n_img, lsd)) return rc;
+        if (plot && (!prev->img_l || !prev->img_r)) return fail(ctx, PLSTVO_E_INVALID, "null images: the plot draws on them");
         if (lns && !run_lsd)
             if (const int rc = lines.cut(ctx, fs, nfs, 1, NF)) return rc;
     }
@@ -1151,9 +1156,10 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     // raw images: they go up into the rectifier's staging slot, and every stage reads the grey device copy the rectifier
     // writes (the remap's, or for colour images the conversion's)
     const uint8_t* rectified = nullptr;
+    const uint8_t* staged = nullptr;   // the raw images in the rectifier's staging
     cudaEvent_t rectified_ready = nullptr;
-    if (rect && (pts || lns)) {
-        if (const int rc = rectify_call(ctx, rect, call, NF, n_img, iparts, ctx->s_main, &rectified, &d_rgb))
+    if (rect && (pts || lns || plot)) {
+        if (const int rc = rectify_call(ctx, rect, call, NF, n_img, iparts, ctx->s_main, &rectified, &d_rgb, &staged))
             return rc;
         rectified_ready = next_event(ctx);
         CK(ctx, cudaEventRecord(rectified_ready, ctx->s_main));
@@ -1193,6 +1199,12 @@ static int track_images_run(PlContext* ctx, const PlCamera* cam, const PlConfig*
     std::vector<int32_t> pl_off[2], pr_off[2], none((size_t)NF + 1, 0);
     StereoSet sets[2][2];
     for (int j = 0; j < nfs; ++j) stereo_set_inputs(orb, 2 * j, pts, lines, 2 * j, NF, none, pl_off[j], pr_off[j], sets[j]);
+    if (plot) {   // the plot's base images: the left images come first in every device copy above
+        const bool colour = rect && rect->channels > 1;
+        call->plot_raw = colour ? staged : nullptr;
+        call->plot_grey = colour ? nullptr : rectified ? rectified : pts ? orb.images : nullptr;
+        call->plot_host = colour || call->plot_grey ? nullptr : prev->img_l;
+    }
     StereoDevInputs dev;
     dev.lines_ready = lines.joined;
     dev.marks = ctx->img_ev.ev + 1;
@@ -1361,6 +1373,7 @@ void plstvo_stereo_session_destroy(PlStereoSession* ss) {
         ss->pool[1].buf.release();
         ss->d_meta.release();
         ss->kept.buf.release();
+        ss->plot_buf.release();
         ss->d_cams.release();
         ss->kf_steps.clear();
     }
@@ -1372,7 +1385,8 @@ int64_t plstvo_stereo_session_device_bytes(const PlStereoSession* ss) {
     LOCK(ss->ctx);
     size_t kf = 0;
     for (const auto& c : ss->kf_steps) kf += c->buf.cap;
-    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap + ss->d_cams.cap + kf);
+    return (int64_t)(ss->pool[0].buf.cap + ss->pool[1].buf.cap + ss->d_meta.cap + ss->kept.buf.cap + ss->plot_buf.cap +
+                     ss->d_cams.cap + kf);
 }
 
 namespace {
@@ -1394,16 +1408,18 @@ void session_drop_keyframes(PlStereoSession* ss) {
 }
 
 // The start and the end of a call that changes the session: initialize / insert, run and run_keyframes.  The start drops the
-// key frames and, with discard, invalidates what the last call retained.  The end of a failed call (rc) does both and
-// synchronises both streams: the line stages may still run on the second stream, and ORB or a step on the first, and the
-// next call may reuse their arenas.  The end of a successful one marks the retention arena as the call's (track, n): an empty
-// call (n = 0) retains nothing, and a run of T = 0 (ran false) leaves it as it was.
+// key frames and the last plot and, with discard, invalidates what the last call retained.  The end of a failed call (rc)
+// does both and synchronises both streams: the line stages may still run on the second stream, and ORB or a step on the
+// first, and the next call may reuse their arenas.  The end of a successful one marks the retention arena as the call's
+// (track, n): an empty call (n = 0) retains nothing, and a run of T = 0 (ran false) leaves it as it was; with drew (an
+// initialize / insert while plotting is on) the plot arena holds the call's images.
 void session_start(PlStereoSession* ss, bool discard) {
     if (discard) ss->kept.valid = false;
+    ss->plot_valid = false;
     session_drop_keyframes(ss);
 }
 
-int session_finish(PlContext* ctx, PlStereoSession* ss, int rc, bool track, int n, bool ran = true) {
+int session_finish(PlContext* ctx, PlStereoSession* ss, int rc, bool track, int n, bool ran = true, bool drew = false) {
     if (rc) {
         ss->kept.valid = false;
         session_drop_keyframes(ss);
@@ -1415,6 +1431,7 @@ int session_finish(PlContext* ctx, PlStereoSession* ss, int rc, bool track, int 
         ss->kept.track = track;
         ss->kept.n = n;
         ss->kept.valid = n > 0 || ss->kept.lay_out(0, 0, 0, 0) == cudaSuccess;
+        ss->plot_valid = drew && ss->kept.valid;
     }
     return 0;
 }
@@ -1436,11 +1453,43 @@ int plstvo_stereo_session_retain(PlContext* ctx, PlStereoSession* ss, int on) {
     ss->retain = on != 0;
     session_drop_keyframes(ss);
     ss->kept.valid = false;
-    if (!on) {
+    if (!on) {   // plotting draws the retained rows: it goes off with retention
+        ss->plot = ss->plot_valid = false;
         CK(ctx, cudaSetDevice(ctx->device));
         ss->kept.buf.release();   // every call that wrote it blocked until done
+        ss->plot_buf.release();
     }
     return 0;
+}
+
+int plstvo_stereo_session_plot(PlContext* ctx, PlStereoSession* ss, int on) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (const int rc = session_check(ctx, ss)) return rc;
+    if (on && !ss->retain) return fail(ctx, PLSTVO_E_INVALID, "retention is off: plstvo_stereo_session_retain(ctx, s, 1) first");
+    if (on && ss->plot) return 0;   // already on: the last plot stays readable
+    ss->plot = on != 0;
+    ss->plot_valid = false;
+    if (!on) {
+        CK(ctx, cudaSetDevice(ctx->device));
+        ss->plot_buf.release();   // every call that wrote it blocked until done
+    }
+    return 0;
+}
+
+int plstvo_stereo_session_read_plot(PlContext* ctx, const PlStereoSession* ss, uint8_t* out) {
+    if (!ctx) return PLSTVO_E_INVALID;
+    LOCK(ctx);
+    if (const int rc = session_check(ctx, out ? ss : nullptr, "null session or output")) return rc;
+    if (!ss->plot) return fail(ctx, PLSTVO_E_INVALID, "plotting is off: plstvo_stereo_session_plot(ctx, s, 1) first");
+    if (!ss->plot_valid)
+        return fail(ctx, PLSTVO_E_INVALID, "nothing plotted: no initialize / insert succeeded since plotting was turned on, "
+                                           "or the last call failed or was a run");
+    CK(ctx, cudaSetDevice(ctx->device));
+    const size_t bytes = (size_t)ss->kept.n * ss->cam.width * ss->cam.height * 3;
+    if (bytes) CK(ctx, cudaMemcpyAsync(out, ss->plot_buf.p, bytes, cudaMemcpyDeviceToHost, ctx->s_main));
+    CK(ctx, cudaStreamSynchronize(ctx->s_main));
+    return ss->kept.n;
 }
 
 int plstvo_stereo_session_read(PlContext* ctx, const PlStereoSession* ss, const PlStereoFrameOut* out) {
@@ -1503,6 +1552,7 @@ int session_images(PlContext* ctx, PlStereoSession* ss, bool track, int n, const
     if (const int rc = session_check_ids(ctx, ss, track, n, ids)) return rc;
     if (const int rc = check_key_line_fields(ctx, &frames, 1, false, ss->fld && !ss->cfg.has_lines, false)) return rc;
     SessionCall call = session_begin(ss, track, n, ids);
+    call.plot = ss->plot;
     // the FLD branch: the caller's key lines (the images call's checks), LSD and its config unused
     const int rc = track_images_common(ctx, &ss->cam, &ss->cfg, &ss->mc, &ss->sc, &ss->oc, !ss->fld,
                                        !ss->fld && ss->has_lc ? &ss->lc : nullptr, frames, nullptr, priors, results, n_stereo,
@@ -1517,7 +1567,8 @@ int session_call(PlContext* ctx, PlStereoSession* ss, bool track, int n, const i
     LOCK(ctx);
     if (const int rc = session_check(ctx, ss)) return rc;
     session_start(ss, true);
-    return session_finish(ctx, ss, session_images(ctx, ss, track, n, ids, frames, priors, results, n_stereo), track, n);
+    return session_finish(ctx, ss, session_images(ctx, ss, track, n, ids, frames, priors, results, n_stereo), track, n, true,
+                          ss->plot);
 }
 }  // namespace
 

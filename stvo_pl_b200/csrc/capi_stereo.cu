@@ -400,6 +400,10 @@ int plstvo::track_stereo_common(PlContext* ctx, const PlCamera* cam, const PlCon
             CK(ctx, cudaStreamWaitEvent(s, offsets_up, 0));
             for (int k = 0; k < 2; ++k) CK(ctx, sets[k].lift(a, *cam, *sc, NF, 0, kr.rec, s, a.i32(o_ooff[k]), d_cams));
             ctx->launches += 2;
+            if (call->plot)   // plotStereoFrame: drawn from the rows just retained, before the call's images can be reused
+                if (const int rc = session_plot(ctx, *call, cam->width, cam->height, kr.rec, ooff[0], ooff[1], a.i32(o_ooff[0]),
+                                                a.i32(o_ooff[1]), s))
+                    return rc;
         }
         if (!track) {
             if (dev && dev->marks) {

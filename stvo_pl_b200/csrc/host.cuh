@@ -492,6 +492,10 @@ struct PlStereoSession {
     // ---- plstvo_stereo_session_retain / _read ----
     bool retain = false;
     plstvo::SessionRetained kept;                    // the last call's records while retain is on
+    // ---- plstvo_stereo_session_plot / _read_plot: the last initialize / insert's plotStereoFrame images, [kept.n][H][W][3]
+    // (plot_valid: that call succeeded and drew them) ----
+    bool plot = false, plot_valid = false;
+    plstvo::DevBuf plot_buf;
     // ---- plstvo_stereo_session_run_keyframes / _read_keyframes: per step, every named stream's new rows (the key frames'
     // filled), and the key frames' rows [n_kf][4] (step, stream id, points, lines) with their chunk offsets [n_kf][2] ----
     std::vector<std::unique_ptr<plstvo::SessionRetained>> kf_steps;
@@ -514,7 +518,20 @@ struct SessionCall {
     std::vector<int32_t> new_pt, new_ls;             // [n] the new frames' stereo points / lines
     std::vector<int32_t> meta;                       // uploaded: out_off_pt [n], out_off_ls [n], GatherSeg named [n], others
     int n_others = 0;
+    // plstvo_stereo_session_plot (initialize / insert only, with retain): where the new frames' left images are on the device
+    // (the images path fills it before the stereo step)
+    bool plot = false;
+    const uint8_t* plot_grey = nullptr;   // grey sessions: the grey device copy, the n left images first (null: plot_host)
+    const uint8_t* plot_host = nullptr;   // grey sessions where no stage put the images on the device: the caller's left images
+    const uint8_t* plot_raw = nullptr;    // colour sessions: the rectifier's staging, the n left images first
 };
+
+// plot.cu: plotStereoFrame of c's n new frames into the session's plot arena, enqueued on s: the base image (plot_grey /
+// plot_host replicated into B, G, R, or the colour staging remapped with each frame's left maps), then the circles of the
+// points and the lines of rec's rows, frame k's at pt_off[k] .. pt_off[k + 1] (ls_off for the lines; device copies d_pt_off,
+// d_ls_off).  The images are W x H.
+int session_plot(PlContext* ctx, const SessionCall& c, int W, int H, const RecPtrs& rec, const std::vector<int32_t>& pt_off,
+                 const std::vector<int32_t>& ls_off, const int32_t* d_pt_off, const int32_t* d_ls_off, cudaStream_t s);
 
 // Lays out pool[cur ^ 1] for the new frames' counts (new_pt, new_ls [n], call order) and the untouched streams' kept frames,
 // grows it if need be, and uploads the call's offsets and gather segments on s.  PLSTVO_E_TOO_LARGE: more than INT_MAX rows.
@@ -620,9 +637,10 @@ struct ImgPart {   // consecutive host images of one size
 // alternate left, right maps, and for a colour rectifier the conversion to grey after it.  rects (optional, [per_block], of
 // rect's size and channels): image z is prepared by rects[z % per_block] instead, a null entry or one without maps copying
 // (grey) or converting (colour) the image.  d_rgb (optional, colour rectifiers only): the same launch also writes the
-// COLOR_RGB2GRAY conversion of each remapped (or unmapped) image into a second grey slot, *d_rgb.
+// COLOR_RGB2GRAY conversion of each remapped (or unmapped) image into a second grey slot, *d_rgb.  d_raw (optional): where the
+// staged raw images start, in the order of parts.
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
                     cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects = nullptr,
-                    const uint8_t** d_rgb = nullptr);
+                    const uint8_t** d_rgb = nullptr, const uint8_t** d_raw = nullptr);
 
 }  // namespace plstvo

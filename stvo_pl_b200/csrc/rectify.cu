@@ -7,26 +7,11 @@
 #include <cstring>
 
 #include "host.cuh"
+#include "remap.cuh"
 
 using namespace plstvo;
 
 namespace {
-
-// cv::remap's fixed point (INTER_BITS 5, INTER_REMAP_COEF_BITS 15): the weights of the four taps are ((32 - ax)(32 - ay),
-// ax (32 - ay), (32 - ax) ay, ax ay) * 32, OpenCV's INTER_LINEAR table exactly (each bilinear product is a multiple of
-// 1/1024), and the result is (sum + 2^14) >> 15, which is (sum / 32 + 2^9) >> 10.  A tap outside the image reads 0.
-__device__ __forceinline__ uint32_t remap_pixel(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
-    f &= 1023u;   // OpenCV indexes its table with map2 & (INTER_TAB_SIZE2 - 1)
-    const int ax = (int)(f & 31u), ay = (int)(f >> 5);
-    const int x = m.x, y = m.y;
-    const bool x0 = (unsigned)x < (unsigned)W, x1 = (unsigned)(x + 1) < (unsigned)W;
-    const bool y0 = (unsigned)y < (unsigned)H, y1 = (unsigned)(y + 1) < (unsigned)H;
-    const uint8_t* r0 = S + (size_t)y * W + x;
-    const int v00 = (x0 && y0) ? __ldg(r0) : 0, v01 = (x1 && y0) ? __ldg(r0 + 1) : 0;
-    const int v10 = (x0 && y1) ? __ldg(r0 + W) : 0, v11 = (x1 && y1) ? __ldg(r0 + W + 1) : 0;
-    const int sum = v00 * ((32 - ax) * (32 - ay)) + v01 * (ax * (32 - ay)) + v10 * ((32 - ax) * ay) + v11 * (ax * ay);
-    return (uint32_t)((sum + 512) >> 10);
-}
 
 // 4 bytes from 4-byte aligned D on, else byte by byte
 __device__ __forceinline__ void store4(uint8_t* D, uint32_t v) {
@@ -135,41 +120,7 @@ __global__ void __launch_bounds__(256) color_convert_kernel(const uint8_t* __res
     }
 }
 
-// remap_pixel on each of the first three channels of a C-channel image, then the conversion: cv::remap of a multi-channel
-// image interpolates every channel with the same weights as the one-channel remap, and the reference converts the remapped
-// image.  Alpha is not read: a 4-channel tap is one aligned 4-byte load, of which the top byte is dropped.
-template <int C>
-__device__ __forceinline__ void remap_channels(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f, uint32_t ch[3]) {
-    f &= 1023u;
-    const int ax = (int)(f & 31u), ay = (int)(f >> 5);
-    const int x = m.x, y = m.y;
-    const bool x0 = (unsigned)x < (unsigned)W, x1 = (unsigned)(x + 1) < (unsigned)W;
-    const bool y0 = (unsigned)y < (unsigned)H, y1 = (unsigned)(y + 1) < (unsigned)H;
-    const int w00 = (32 - ax) * (32 - ay), w01 = ax * (32 - ay), w10 = (32 - ax) * ay, w11 = ax * ay;
-    const ptrdiff_t row = (ptrdiff_t)W * C;
-    const uint8_t* r0 = S + ((ptrdiff_t)y * W + x) * C;
-    if constexpr (C == 4) {
-        const uint32_t t00 = (x0 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0)) : 0u;
-        const uint32_t t01 = (x1 && y0) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + 4)) : 0u;
-        const uint32_t t10 = (x0 && y1) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + row)) : 0u;
-        const uint32_t t11 = (x1 && y1) ? __ldg(reinterpret_cast<const uint32_t*>(r0 + row + 4)) : 0u;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const int sh = 8 * c;
-            const int sum = (int)((t00 >> sh) & 255u) * w00 + (int)((t01 >> sh) & 255u) * w01 +
-                            (int)((t10 >> sh) & 255u) * w10 + (int)((t11 >> sh) & 255u) * w11;
-            ch[c] = (uint32_t)((sum + 512) >> 10);
-        }
-    } else {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {
-            const int v00 = (x0 && y0) ? __ldg(r0 + c) : 0, v01 = (x1 && y0) ? __ldg(r0 + C + c) : 0;
-            const int v10 = (x0 && y1) ? __ldg(r0 + row + c) : 0, v11 = (x1 && y1) ? __ldg(r0 + row + C + c) : 0;
-            ch[c] = (uint32_t)((v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + 512) >> 10);
-        }
-    }
-}
-
+// remap_channels (remap.cuh), then the conversion: the reference converts the remapped image
 template <int C>
 __device__ __forceinline__ uint32_t remap_grey(const uint8_t* __restrict__ S, int W, int H, short2 m, uint32_t f) {
     uint32_t ch[3];
@@ -337,7 +288,8 @@ cudaError_t launch_color_prepare(int n_img, int per_block, int W, int H, bool ma
 }
 
 int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_block, const std::vector<ImgPart>& parts,
-                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects, const uint8_t** d_rgb) {
+                    cudaStream_t s, const uint8_t** d_out, const PlRectifier* const* rects, const uint8_t** d_rgb,
+                    const uint8_t** d_raw) {
     const int W = rect->width, H = rect->height, Ch = rect->channels;
     const size_t bytes = (size_t)n_img * W * H;
     CK(ctx, cudaSetDevice(ctx->device));
@@ -382,6 +334,7 @@ int rectify_enqueue(PlContext* ctx, const PlRectifier* rect, int n_img, int per_
     ctx->launches += launches;
     *d_out = a.u8(o_out);
     if (d_rgb) *d_rgb = rgb ? a.u8(o_rgb) : nullptr;
+    if (d_raw) *d_raw = a.u8(o_raw);
     return 0;
 }
 

@@ -148,6 +148,8 @@ def load_library(path: str = LIB_PATH) -> C.CDLL:
         "plstvo_stereo_session_retain": (C.c_int, [vp, vp, C.c_int]),
         "plstvo_stereo_session_use_fld_lines": (C.c_int, [vp, vp, C.c_int]),
         "plstvo_stereo_session_read": (C.c_int, [vp, vp, C.POINTER(T.PlStereoFrameOut)]),
+        "plstvo_stereo_session_plot": (C.c_int, [vp, vp, C.c_int]),
+        "plstvo_stereo_session_read_plot": (C.c_int, [vp, vp, C.POINTER(C.c_uint8)]),
         "plstvo_default_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
         "plstvo_kitti_handler_config": (None, [C.POINTER(T.PlHandlerConfig)]),
         "plstvo_stereo_session_run": (C.c_int, [vp, vp, C.POINTER(T.PlHandlerConfig), C.c_int, i32p, C.c_int,
@@ -193,7 +195,8 @@ EXPORTED_SYMBOLS = [
     "plstvo_track_batch_cams", "plstvo_stereo_session_create_cams", "plstvo_default_handler_config",
     "plstvo_kitti_handler_config", "plstvo_stereo_session_run", "plstvo_default_keyframe_config",
     "plstvo_initial_keyframe_state", "plstvo_stereo_session_run_keyframes", "plstvo_stereo_session_read_keyframes",
-    "plstvo_fld_key_lines", "plstvo_stereo_session_use_fld_lines", "plstvo_stereo_session_run_schedule"]
+    "plstvo_fld_key_lines", "plstvo_stereo_session_use_fld_lines", "plstvo_stereo_session_run_schedule",
+    "plstvo_stereo_session_plot", "plstvo_stereo_session_read_plot"]
 
 
 def _p(a: Optional[np.ndarray], typ):
@@ -266,8 +269,9 @@ class StereoSession:
     """A PlStereoSession: n_streams stereo streams, each stream's previous frame kept in HBM as its stereo features
     (Engine.stereo_session_create).  initialize / insert name any subset of the streams; close() or the owning Engine frees it."""
 
-    def __init__(self, eng: "Engine", handle, n_streams: int, rect: Optional[Rectifier] = None):
+    def __init__(self, eng: "Engine", handle, n_streams: int, rect: Optional[Rectifier] = None, size=(0, 0)):
         self.eng, self.handle, self.n_streams, self.rect = eng, handle, n_streams, rect
+        self.width, self.height = size   # the cameras' image size, which sizes read_plot()'s images
         self.last = None   # the last call, if it succeeded: (insert, n_stereo), which sizes read()'s arrays
 
     def check_frames(self, frames: dict):
@@ -334,6 +338,21 @@ class StereoSession:
         """plstvo_stereo_session_retain: from the next initialize / insert on, keep each call's new frames and matches on the
         device for read(); off frees them."""
         self.eng._ck(self.eng.lib.plstvo_stereo_session_retain(self.eng.ctx, self.handle, 1 if on else 0))
+
+    def plot(self, on: bool):
+        """plstvo_stereo_session_plot: from the next initialize / insert on, draw each new frame's plotStereoFrame image on the
+        device for read_plot() (retention must be on); off frees them."""
+        self.eng._ck(self.eng.lib.plstvo_stereo_session_plot(self.eng.ctx, self.handle, 1 if on else 0))
+
+    def read_plot(self) -> np.ndarray:
+        """plstvo_stereo_session_read_plot of the last initialize / insert: uint8[n, H, W, 3], each new frame's left image
+        (rectified, in BGR) with its stereo points' circles and stereo lines drawn in (0, 200, 0), in call order."""
+        n = len(self.last[1]) if self.last is not None else 0
+        out = np.zeros((max(n, 1), self.height, self.width, 3), np.uint8)
+        got = self.eng._ck(self.eng.lib.plstvo_stereo_session_read_plot(self.eng.ctx, self.handle, _p(out, T.c_uint8_p)))
+        if got != n:
+            raise PlstvoError(-1, f"plstvo_stereo_session_read_plot returned {got} frames, the last call had {n}")
+        return out[:n]
 
     def read(self):
         """plstvo_stereo_session_read of the last call: (pt, ls, m12_pt, inlier_pt, m12_ls, inlier_ls).  pt / ls hold the new
@@ -941,7 +960,7 @@ class Engine:
                                                   None if rect is None else rect.handle, n_streams)
         if not h:
             raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
-        ss = StereoSession(self, h, n_streams, rect)
+        ss = StereoSession(self, h, n_streams, rect, (cam.width, cam.height))
         self._sessions.append(ss)
         return ss
 
@@ -965,7 +984,7 @@ class Engine:
                                                        C.byref(ocfg), None if lcfg is None else C.byref(lcfg), rarr, n_streams)
         if not h:
             raise PlstvoError(-1, (self.lib.plstvo_last_error(self.ctx) or b"").decode())
-        ss = StereoSession(self, h, n_streams, first)
+        ss = StereoSession(self, h, n_streams, first, (cams[0].width, cams[0].height))
         self._sessions.append(ss)
         return ss
 
